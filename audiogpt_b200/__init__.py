@@ -1,4 +1,4 @@
-"""audiogpt_b200 -- B200-native (sm_100a) back-end for AudioGPT's generative hot path.
+"""audiogpt_b200 -- H100 (sm_90a) back-end for AudioGPT's generative hot path.
 
 Drop-in classes (same names / signatures / state-dict layouts as the reference):
 
@@ -33,7 +33,7 @@ _INSTALL_MAP = {
 
 
 def install(strict: bool = False):
-    """Make AudioGPT's tool classes pick up the B200 back-end.
+    """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
     ``NeuralSeq/`` and ``text_to_audio/Make_An_Audio/``) and before ``audio-chatgpt.py`` builds its

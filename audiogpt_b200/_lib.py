@@ -92,7 +92,7 @@ def check(rc: int):
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError("audiogpt_b200 needs a CUDA device (B200 / sm_100a); there is no CPU fallback")
+        raise RuntimeError("audiogpt_b200 needs a CUDA device (H100 / sm_90a); there is no CPU fallback")
 
 
 def host_weight_array(tensors):

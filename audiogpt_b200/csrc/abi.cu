@@ -58,7 +58,6 @@ int agpt_attention(const float* q, int q_pitch, const float* k, int k_pitch, con
     attention(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, d, Lq, Lk, (cudaStream_t)stream);
   });
 }
-int agpt_set_tc_version(int v) { return guarded([&] { tc_set_version(v); }); }
 double agpt_fma_peak_tflops(void) {
   double v = -1.0;
   guarded([&] { v = fma_peak_tflops(); });

@@ -1,22 +1,20 @@
-// Multi-head attention on the 5th-generation tensor cores (tcgen05 + TMEM): softmax_j(q_i . k_j * d^-0.5) v_j
-// with heads outermost in the channel dimension ('b n (h d)'), as CrossAttention.forward computes it
-// (ldm/modules/attention.py:170-193).  Both contractions -- S = Q K^T and O = P V -- run as
-// tcgen05.mma.kind::f16 on error-compensated fp16 hi/lo parts (x = hi + lo; hi*hi + lo*hi + hi*lo, fp32
-// accumulation in TMEM: the arithmetic of tcconv5.cu), the softmax is the exact online (running max / running
-// sum) form in fp32 registers.
+// Multi-head attention on the Hopper tensor cores (wgmma): softmax_j(q_i . k_j * d^-0.5) v_j with heads outermost in
+// the channel dimension ('b n (h d)'), as CrossAttention.forward computes it (ldm/modules/attention.py:170-193).
+// Both contractions -- S = Q K^T and O = P V -- run as wgmma on error-compensated fp16 hi/lo parts (x = hi + lo;
+// hi*hi + lo*hi + hi*lo with fp32 accumulation: the arithmetic of tcconv5.cu); the softmax is the exact online
+// (running max / running sum) form in fp32 registers.
 //
-// One CTA = 128 queries of one (sample, head); 4 warps, thread = query row = TMEM lane.  Per block of 64 keys:
+// One CTA = one warpgroup = 64 queries of one (sample, head).  Per block of 64 keys:
 //   all threads   K block  [64 keys][d]  -> fp16 hi/lo, K-major SWIZZLE_128B tile (B operand of S)
 //                 V block  [64 keys][d]  -> TRANSPOSED fp16 hi/lo tile [d rows][64 keys] (B operand of O, K = keys)
-//   one thread    S[128 x 64] = Q K^T            (Q tile converted once per CTA, pre-scaled by d^-0.5 * log2 e)
-//   all threads   tcgen05.ld S -> running max m, p = exp2(s - m), running sum l; P hi/lo -> K-major tile (A operand)
-//   one thread    O_blk[128 x d] = P V           (fresh accumulator)
-//   all threads   tcgen05.ld O_blk -> acc = acc * exp2(m_old - m_new) + O_blk   (fp32 registers)
-// Shared memory: 96 KB for d <= 64 (two CTAs per SM overlap each other's softmax and MMA phases), 152 KB for d = 80.
-// SASS: UTCHMMA (MMA), LDTM (tcgen05.ld), no LDG/STG inside the MMA loop other than the K/V block loads.
+//   wgmma         S[64 x 64] = Q K^T in registers (Q tile converted once per CTA, pre-scaled by d^-0.5 * log2 e)
+//   all threads   running max m, p = exp2(s - m), running sum l over the fragment rows (4 lanes share a row);
+//                 P hi/lo -> K-major tile (A operand of O); O *= exp2(m_old - m_new)
+//   wgmma         O[64 x DP] += P V in registers
 #include <cuda_fp16.h>
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "tc_h16.cuh"
 #include "models.h"
 #include "nn_kernels.h"
 
@@ -24,76 +22,38 @@ namespace agpt {
 namespace {
 
 constexpr int AT_BK = 64;          // keys per block = one 128-byte swizzle span of fp16
-constexpr int AT_ROWS = 128;       // queries per CTA (UMMA_M)
+constexpr int AT_ROWS = 64;        // queries per CTA (wgmma M)
 
-__device__ __forceinline__ uint32_t at_f2h2_sat(float a, float b) {
-  uint32_t r;
-  asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
-  return r;
-}
-__device__ __forceinline__ uint32_t at_split2(float a, float b, uint32_t& lo) {
-  const uint32_t h = at_f2h2_sat(a, b);
-  const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&h));
-  lo = at_f2h2_sat(a - hf.x, b - hf.y);
-  return h;
-}
-__device__ __forceinline__ void at_umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 consecutive fp32 columns of this thread's TMEM lane
-__device__ __forceinline__ void at_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void at_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// D = head dim (multiple of 8, <= 128).  NCH = 64-channel chunks of the head dim; DP = D rounded up to 16 (UMMA N / K granularity)
+// D = head dim (multiple of 8, <= 128).  NCH = 64-channel chunks of the head dim; DP = D rounded up to 16 (the N of
+// the P V wgmma and the K granularity of Q K^T)
 template <int D>
 struct AtCfg {
   static constexpr int NCH = (D + 63) / 64;
   static constexpr int DP = (D + 15) / 16 * 16;
-  static constexpr int VROWS = (DP + 7) / 8 * 8;
   static constexpr uint32_t Q_BYTES = 2u * NCH * AT_ROWS * 128;          // hi + lo
   static constexpr uint32_t K_BYTES = 2u * NCH * AT_BK * 128;
-  static constexpr uint32_t V_BYTES = 2u * VROWS * 128;                  // [DP rows][64 keys] hi + lo
+  static constexpr uint32_t V_BYTES = 2u * DP * 128;                     // [DP rows][64 keys] hi + lo
   static constexpr uint32_t P_BYTES = 2u * AT_ROWS * 128;
   static constexpr uint32_t TOTAL = Q_BYTES + K_BYTES + V_BYTES + P_BYTES;
-  static constexpr uint32_t TMEM_COLS = (AT_BK + DP <= 128) ? 128 : 256;
   static constexpr bool PF = D <= 64;      // software-prefetch the next K / V block into registers (register budget: d <= 64)
   static constexpr int KIT = (AT_BK * NCH * 8 + 127) / 128;   // K items (8 channels of one key) per thread
-  static constexpr int VIT = (VROWS / 4 + 1) / 2;             // V channel quads per thread
+  static constexpr int VIT = (DP / 4 + 1) / 2;                // V channel quads per thread
 };
+
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t a, uint64_t b) {
+  if constexpr (N == 16) wgmma_n16(d, a, b);
+  else if constexpr (N == 32) wgmma_n32(d, a, b);
+  else if constexpr (N == 48) wgmma_n48(d, a, b);
+  else if constexpr (N == 64) wgmma_n64(d, a, b);
+  else wgmma_n80(d, a, b);
+}
 
 template <int D>
 __global__ void __launch_bounds__(128) attention_tc_kernel(
     const float* __restrict__ q, int q_pitch, const float* __restrict__ k, int k_pitch,
     const float* __restrict__ v, int v_pitch, float* __restrict__ o, int o_pitch,
-    int Lq, int Lk, float qscale /* d^-0.5 * log2(e) */, __half* __restrict__ phi, __half* __restrict__ plo) {
+    int Lq, int Lk, float qscale /* d^-0.5 * log2(e) */) {
   using Cf = AtCfg<D>;
   extern __shared__ uint8_t at_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -102,24 +62,16 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
   uint8_t* k_hi = smem + Cf::Q_BYTES;
   uint8_t* k_lo = k_hi + Cf::NCH * AT_BK * 128;
   uint8_t* v_hi = smem + Cf::Q_BYTES + Cf::K_BYTES;
-  uint8_t* v_lo = v_hi + Cf::VROWS * 128;
+  uint8_t* v_lo = v_hi + Cf::DP * 128;
   uint8_t* p_hi = smem + Cf::Q_BYTES + Cf::K_BYTES + Cf::V_BYTES;
   uint8_t* p_lo = p_hi + AT_ROWS * 128;
-  __shared__ uint64_t bar;
-  __shared__ uint32_t tmem_slot;
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * AT_ROWS;
-  if (tid == 0) { mbar_init(&bar, 1); fence_barrier_init(); }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(smem_u32(&tmem_slot)), "r"(Cf::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // ---- Q tile: [128 queries][D] fp32 -> pre-scaled fp16 hi/lo, 8-channel items like the conv transform
+  constexpr int CH8 = Cf::NCH * 8;                    // 16-byte chunks per row over all 64-channel chunks
+  // ---- Q tile: [64 queries][D] fp32 -> pre-scaled fp16 hi/lo, 8-channel items like the conv transform
   {
     const float* qb = q + ((long)n * Lq) * q_pitch + h * D;
-    constexpr int CH8 = Cf::NCH * 8;                    // 16-byte chunks per row over all 64-channel chunks
     for (int it = tid; it < AT_ROWS * CH8; it += 128) {
       const int row = it / CH8, c8 = it - row * CH8;
       const int ch = c8 * 8;
@@ -130,39 +82,29 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
         b = *reinterpret_cast<const float4*>(p + 4);
       }
       uint4 hi, lo;
-      hi.x = at_split2(a.x * qscale, a.y * qscale, lo.x);
-      hi.y = at_split2(a.z * qscale, a.w * qscale, lo.y);
-      hi.z = at_split2(b.x * qscale, b.y * qscale, lo.z);
-      hi.w = at_split2(b.z * qscale, b.w * qscale, lo.w);
+      hi.x = split2(a.x * qscale, a.y * qscale, lo.x);
+      hi.y = split2(a.z * qscale, a.w * qscale, lo.y);
+      hi.z = split2(b.x * qscale, b.y * qscale, lo.z);
+      hi.w = split2(b.z * qscale, b.w * qscale, lo.w);
       const uint32_t off = (uint32_t)(c8 >> 3) * (AT_ROWS * 128) + sw128(row, c8 & 7);
       *reinterpret_cast<uint4*>(q_hi + off) = hi;
       *reinterpret_cast<uint4*>(q_lo + off) = lo;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t lane_base = ((uint32_t)(warp * 32)) << 16;
-  const uint32_t tm_s = tmem, tm_o = tmem + AT_BK;        // S: columns [0, 64), O_blk: [64, 64 + DP)
 
-  // instruction descriptors: D = F32 (bit 4), A = B = F16, both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-  const uint32_t idesc_s = (1u << 4) | ((uint32_t)(AT_BK >> 3) << 17) | ((uint32_t)(AT_ROWS >> 4) << 24);
-  const uint32_t idesc_o = (1u << 4) | ((uint32_t)(Cf::DP >> 3) << 17) | ((uint32_t)(AT_ROWS >> 4) << 24);
-
-  float acc[Cf::DP];
+  // fragment of this thread (wgmma accumulator layout): rows r and r + 8, columns 8i + 2 (lane % 4) + {0, 1}
+  const int r = warp * 16 + (lane >> 2), cq = 2 * (lane & 3);
+  float acc[Cf::DP / 2];
 #pragma unroll
-  for (int c = 0; c < Cf::DP; ++c) acc[c] = 0.f;
-  float m_run = -INFINITY, l_run = 0.f;
+  for (int c = 0; c < Cf::DP / 2; ++c) acc[c] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};    // l_run: this thread's partial sums of its rows
   const float* kb = k + ((long)n * Lk) * k_pitch + h * D;
   const float* vb = v + ((long)n * Lk) * v_pitch + h * D;
   const int nblk = (Lk + AT_BK - 1) / AT_BK;
-  uint32_t phase = 0;
 
   // K items: (key row, 8-channel chunk) -> two float4; V items: (key, channel quad) -> one float4
   float4 kreg[Cf::KIT][2];
   float4 vreg[Cf::VIT];
-  constexpr int CH8 = Cf::NCH * 8;
   auto load_kv = [&](int j0) {
 #pragma unroll
     for (int u = 0; u < Cf::KIT; ++u) {
@@ -195,8 +137,8 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
       const int row = it / CH8, c8 = it - row * CH8;
       const float4 a = kreg[u][0], b = kreg[u][1];
       uint4 hi, lo;
-      hi.x = at_split2(a.x, a.y, lo.x); hi.y = at_split2(a.z, a.w, lo.y);
-      hi.z = at_split2(b.x, b.y, lo.z); hi.w = at_split2(b.z, b.w, lo.w);
+      hi.x = split2(a.x, a.y, lo.x); hi.y = split2(a.z, a.w, lo.y);
+      hi.z = split2(b.x, b.y, lo.z); hi.w = split2(b.z, b.w, lo.w);
       const uint32_t off = (uint32_t)(c8 >> 3) * (AT_BK * 128) + sw128(row, c8 & 7);
       *reinterpret_cast<uint4*>(k_hi + off) = hi;
       *reinterpret_cast<uint4*>(k_lo + off) = lo;
@@ -206,7 +148,7 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
 #pragma unroll
     for (int u = 0; u < Cf::VIT; ++u) {
       const int c4 = half + 2 * u;
-      if (c4 >= Cf::VROWS / 4) continue;
+      if (c4 >= Cf::DP / 4) continue;
       const int ch = c4 * 4;
       const float vals[4] = {vreg[u].x, vreg[u].y, vreg[u].z, vreg[u].w};
 #pragma unroll
@@ -228,126 +170,109 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
     store_kv();
     if (Cf::PF && blk + 1 < nblk) load_kv(j0 + AT_BK);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
     // ---- S = Q K^T
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one()) {
-        uint32_t nz = 0;
+    float s[AT_BK / 2];
 #pragma unroll
-        for (int c = 0; c < Cf::NCH; ++c) {
-          const int kv = (D - c * 64) < 64 ? (D - c * 64) : 64;
-          const int ksteps = (kv + 15) >> 4;
-          const uint64_t dqh = make_desc(smem_u32(q_hi + c * AT_ROWS * 128)), dql = make_desc(smem_u32(q_lo + c * AT_ROWS * 128));
-          const uint64_t dkh = make_desc(smem_u32(k_hi + c * AT_BK * 128)), dkl = make_desc(smem_u32(k_lo + c * AT_BK * 128));
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const uint64_t ko = (uint64_t)(2 * ks);
-            at_umma_f16(tm_s, dqh + ko, dkh + ko, idesc_s, nz);
-            nz = 1u;
-            at_umma_f16(tm_s, dql + ko, dkh + ko, idesc_s, 1u);
-            at_umma_f16(tm_s, dqh + ko, dkl + ko, idesc_s, 1u);
-          }
-        }
-        umma_commit(&bar);
-      }
-      __syncwarp();
-    }
-    mbar_wait(&bar, phase);
-    phase ^= 1u;
-    tc_fence_after();
-    // ---- online softmax on this thread's row (scores are already in log2 units)
-    float s[AT_BK];
-    at_ld32(tm_s + lane_base, s);
-    at_ld32(tm_s + lane_base + 32u, s + 32);
-    float mb = -INFINITY;
+    for (int i = 0; i < AT_BK / 2; ++i) s[i] = 0.f;
+    wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < AT_BK; ++j) {
-      if (j0 + j >= Lk) s[j] = -INFINITY;
-      mb = fmaxf(mb, s[j]);
-    }
-    const float m_new = fmaxf(m_run, mb);
-    const float alpha = (m_run == -INFINITY) ? 0.f : exp2f(m_run - m_new);
-    float lsum = 0.f;
+    for (int c = 0; c < Cf::NCH; ++c) {
+      constexpr int kv_last = D - (Cf::NCH - 1) * 64;
+      const int ksteps = ((c == Cf::NCH - 1 ? kv_last : 64) + 15) >> 4;
+      const uint64_t dqh = make_desc(smem_u32(q_hi + c * AT_ROWS * 128)), dql = make_desc(smem_u32(q_lo + c * AT_ROWS * 128));
+      const uint64_t dkh = make_desc(smem_u32(k_hi + c * AT_BK * 128)), dkl = make_desc(smem_u32(k_lo + c * AT_BK * 128));
 #pragma unroll
-    for (int j = 0; j < AT_BK; ++j) { s[j] = exp2f(s[j] - m_new); lsum += s[j]; }     // exp2(-inf) = 0 for masked keys
-    l_run = l_run * alpha + lsum;
-    m_run = m_new;
-#pragma unroll
-    for (int c8 = 0; c8 < 8; ++c8) {
-      uint4 hi, lo;
-      hi.x = at_split2(s[8 * c8 + 0], s[8 * c8 + 1], lo.x);
-      hi.y = at_split2(s[8 * c8 + 2], s[8 * c8 + 3], lo.y);
-      hi.z = at_split2(s[8 * c8 + 4], s[8 * c8 + 5], lo.z);
-      hi.w = at_split2(s[8 * c8 + 6], s[8 * c8 + 7], lo.w);
-      const uint32_t off = sw128(tid, c8);
-      *reinterpret_cast<uint4*>(p_hi + off) = hi;
-      *reinterpret_cast<uint4*>(p_lo + off) = lo;
-    }
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    // ---- O_blk = P V   (K = 64 keys: 4 k-steps)
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dph = make_desc(smem_u32(p_hi)), dpl = make_desc(smem_u32(p_lo));
-        const uint64_t dvh = make_desc(smem_u32(v_hi)), dvl = make_desc(smem_u32(v_lo));
-#pragma unroll
-        for (int ks = 0; ks < AT_BK / 16; ++ks) {
+      for (int ks = 0; ks < 4; ++ks) {
+        if (ks < ksteps) {
           const uint64_t ko = (uint64_t)(2 * ks);
-          at_umma_f16(tm_o, dph + ko, dvh + ko, idesc_o, ks > 0 ? 1u : 0u);
-          at_umma_f16(tm_o, dpl + ko, dvh + ko, idesc_o, 1u);
-          at_umma_f16(tm_o, dph + ko, dvl + ko, idesc_o, 1u);
+          wgmma_n64(s, dqh + ko, dkh + ko);
+          wgmma_n64(s, dql + ko, dkh + ko);
+          wgmma_n64(s, dqh + ko, dkl + ko);
         }
-        umma_commit(&bar);
       }
-      __syncwarp();
     }
-    mbar_wait(&bar, phase);
-    phase ^= 1u;
-    tc_fence_after();
+    wgmma_commit();
+    wgmma_wait<0>();
+    // ---- online softmax over the two rows of this thread (scores are already in log2 units)
+    float mb[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < AT_BK / 8; ++i)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        if (j0 + 8 * i + cq + (e & 1) >= Lk) s[4 * i + e] = -INFINITY;
+        mb[e >> 1] = fmaxf(mb[e >> 1], s[4 * i + e]);
+      }
+    float alpha[2], m_new[2];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      mb[rr] = fmaxf(mb[rr], __shfl_xor_sync(0xffffffffu, mb[rr], 1));
+      mb[rr] = fmaxf(mb[rr], __shfl_xor_sync(0xffffffffu, mb[rr], 2));
+      m_new[rr] = fmaxf(m_run[rr], mb[rr]);
+      alpha[rr] = (m_run[rr] == -INFINITY) ? 0.f : exp2f(m_run[rr] - m_new[rr]);
+      m_run[rr] = m_new[rr];
+    }
+    float lsum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < AT_BK / 2; ++i) {
+      s[i] = exp2f(s[i] - m_new[(i >> 1) & 1]);      // exp2(-inf) = 0 for masked keys
+      lsum[(i >> 1) & 1] += s[i];
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) l_run[rr] = l_run[rr] * alpha[rr] + lsum[rr];
+    // P hi/lo -> K-major [64 rows][64 keys] tiles
+#pragma unroll
+    for (int i = 0; i < AT_BK / 8; ++i)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        uint32_t lo;
+        const uint32_t hi = split2(s[4 * i + 2 * rr], s[4 * i + 2 * rr + 1], lo);
+        const uint32_t off = sw128(r + 8 * rr, i) + (uint32_t)cq * 2u;
+        *reinterpret_cast<uint32_t*>(p_hi + off) = hi;
+        *reinterpret_cast<uint32_t*>(p_lo + off) = lo;
+      }
+#pragma unroll
+    for (int c = 0; c < Cf::DP / 2; ++c) acc[c] *= alpha[(c >> 1) & 1];
+    fence_proxy_async();
+    __syncthreads();
+    // ---- O += P V   (K = 64 keys: 4 k-steps)
+    wgmma_fence();
     {
-      float ob[16];
+      const uint64_t dph = make_desc(smem_u32(p_hi)), dpl = make_desc(smem_u32(p_lo));
+      const uint64_t dvh = make_desc(smem_u32(v_hi)), dvl = make_desc(smem_u32(v_lo));
 #pragma unroll
-      for (int c0 = 0; c0 < Cf::DP; c0 += 16) {
-        at_ld16(tm_o + lane_base + (uint32_t)c0, ob);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[c0 + i] = fmaf(acc[c0 + i], alpha, ob[i]);
+      for (int ks = 0; ks < AT_BK / 16; ++ks) {
+        const uint64_t ko = (uint64_t)(2 * ks);
+        wgmma_f16<Cf::DP>(acc, dph + ko, dvh + ko);
+        wgmma_f16<Cf::DP>(acc, dpl + ko, dvh + ko);
+        wgmma_f16<Cf::DP>(acc, dph + ko, dvl + ko);
       }
     }
-    tc_fence_before();
-    __syncthreads();      // every thread is done with S / O_blk / the K, V, P tiles of this block
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncthreads();      // every thread is done with the K, V, P tiles of this block
   }
 
-  if (q0 + tid < Lq && phi) {     // operand planes (fp16 hi/lo) instead of the fp32 tensor: the consumer is a plane-fed GEMM
-    const float inv = 1.f / l_run;
-    const long base = ((long)n * Lq + q0 + tid) * o_pitch + h * D;
 #pragma unroll
-    for (int c = 0; c < D; c += 8) {
-      uint4 hi, lo;
-      hi.x = at_split2(acc[c] * inv, acc[c + 1] * inv, lo.x); hi.y = at_split2(acc[c + 2] * inv, acc[c + 3] * inv, lo.y);
-      hi.z = at_split2(acc[c + 4] * inv, acc[c + 5] * inv, lo.z); hi.w = at_split2(acc[c + 6] * inv, acc[c + 7] * inv, lo.w);
-      *reinterpret_cast<uint4*>(phi + base + c) = hi;
-      *reinterpret_cast<uint4*>(plo + base + c) = lo;
+  for (int rr = 0; rr < 2; ++rr) {
+    float l = l_run[rr];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int qi = q0 + r + 8 * rr;
+    if (qi >= Lq) continue;
+    const float inv = 1.f / l;
+    float* op = o + ((long)n * Lq + qi) * o_pitch + h * D;
+#pragma unroll
+    for (int i = 0; i < Cf::DP / 8; ++i) {
+      const int c = 8 * i + cq;
+      if (c < D) *reinterpret_cast<float2*>(op + c) = make_float2(acc[4 * i + 2 * rr] * inv, acc[4 * i + 2 * rr + 1] * inv);
     }
-  } else if (q0 + tid < Lq) {
-    const float inv = 1.f / l_run;
-    float* op = o + ((long)n * Lq + q0 + tid) * o_pitch + h * D;
-#pragma unroll
-    for (int c = 0; c < D; c += 4)
-      *reinterpret_cast<float4*>(op + c) = make_float4(acc[c] * inv, acc[c + 1] * inv, acc[c + 2] * inv, acc[c + 3] * inv);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(Cf::TMEM_COLS) : "memory");
   }
 }
 
 template <int D>
 void launch_at(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, float* o, int o_pitch,
-               int N, int heads, int Lq, int Lk, cudaStream_t st, __half* phi, __half* plo) {
+               int N, int heads, int Lq, int Lk, cudaStream_t st) {
   using Cf = AtCfg<D>;
   const size_t smem = Cf::TOTAL + 1024;
   static bool done[64] = {false};
@@ -359,357 +284,18 @@ void launch_at(const float* q, int q_pitch, const float* k, int k_pitch, const f
   }
   const float qscale = (1.0f / sqrtf((float)D)) * 1.4426950408889634f;     // dim_head ** -0.5 (attention.py:158), in log2 units
   dim3 grid(cdiv(Lq, AT_ROWS), heads, N);
-  attention_tc_kernel<D><<<grid, 128, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, qscale, phi, plo);
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// Plane-fed variant: q, k, v arrive as fp16 hi/lo operand planes (written by the epilogue of the projection GEMMs),
-// so the K / V blocks go from global memory straight into the swizzled operand tiles with cp.async -- no fp32 -> fp16
-// conversions in the key loop (the ncu source view of the fp32-input kernel above charges half of its stall samples
-// to F2FP, the quarter-rate conversion pipe: profiles/r2k_attention_findings.md).  What is left on that pipe is
-// exp2 and the split of P.
-//   * 8 warps: warp w and w + 4 share a TMEM lane quadrant and split the 64 keys of a block (32 columns of S each),
-//     each with its own running max / sum / accumulator (O_blk goes to two TMEM accumulators, one per key half);
-//     the two partial softmaxes merge once, after the last block.  Twice the warps per SM hide the conversion latency.
-//   * V is consumed as it lies in memory, [keys][d]: an MN-major B operand (instruction-descriptor bit 16), the tile
-//     layout is the K tile's.  VT = true keeps the transposed K-major tile of the kernel above as the A/B variant.
-//   * single K and V buffers: K(i+1) is fetched while block i's softmax runs, V(i+1) while block i+1's S runs.
-template <int D>
-struct ApCfg {
-  static constexpr int NCH = (D + 63) / 64;
-  static constexpr int DP = (D + 15) / 16 * 16;
-  static constexpr int C8 = D / 8;                                        // 16-byte chunks per row
-  static constexpr uint32_t Q_BYTES = 2u * NCH * AT_ROWS * 128;
-  static constexpr uint32_t K_BYTES = 2u * NCH * AT_BK * 128;
-  static constexpr uint32_t V_BYTES = K_BYTES;                            // the transposed variant needs 2 * DP * 128 <= this
-  static constexpr uint32_t P_BYTES = 2u * AT_ROWS * 128;
-  static constexpr uint32_t TOTAL = Q_BYTES + K_BYTES + V_BYTES + P_BYTES;
-  static constexpr uint32_t TMEM_COLS = (AT_BK + 2 * DP <= 128) ? 128 : 256;
-  static constexpr int MINB = (D <= 64) ? 2 : 1;
-};
-
-__device__ __forceinline__ void at_cp16(void* dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
-}
-template <int N_>
-__device__ __forceinline__ void at_cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N_) : "memory"); }
-
-// MN-major SWIZZLE_128B descriptor: LBO = stride between 64-element blocks of the MN dimension, SBO = 1024 B (8 k-rows)
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-template <int D, bool VT>
-__global__ void __launch_bounds__(256, ApCfg<D>::MINB) attention_pl_kernel(
-    const __half* __restrict__ qh, const __half* __restrict__ ql, int q_pitch,
-    const __half* __restrict__ kh, const __half* __restrict__ kl, int k_pitch,
-    const __half* __restrict__ vh, const __half* __restrict__ vl, int v_pitch,
-    float* __restrict__ o, int o_pitch, int Lq, int Lk, float qscale /* d^-0.5 * log2(e) */,
-    __half* __restrict__ phi, __half* __restrict__ plo) {
-  using Cf = ApCfg<D>;
-  extern __shared__ uint8_t at_smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* q_hi = smem;
-  uint8_t* q_lo = q_hi + Cf::NCH * AT_ROWS * 128;
-  uint8_t* k_hi = smem + Cf::Q_BYTES;
-  uint8_t* k_lo = k_hi + Cf::NCH * AT_BK * 128;
-  uint8_t* v_hi = smem + Cf::Q_BYTES + Cf::K_BYTES;
-  uint8_t* v_lo = v_hi + (VT ? Cf::DP * 128 : Cf::NCH * AT_BK * 128);
-  uint8_t* p_hi = smem + Cf::Q_BYTES + Cf::K_BYTES + Cf::V_BYTES;
-  uint8_t* p_lo = p_hi + AT_ROWS * 128;
-  __shared__ uint64_t bar_s, bar_o;
-  __shared__ uint32_t tmem_slot;
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int quad = warp & 3, half = warp >> 2, row = quad * 32 + lane;
-  const int n = blockIdx.z, h = blockIdx.y, q0 = blockIdx.x * AT_ROWS;
-  if (tid == 0) { mbar_init(&bar_s, 1); mbar_init(&bar_o, 1); fence_barrier_init(); }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(smem_u32(&tmem_slot)), "r"(Cf::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // the tiles start as zeros: padding channels (d .. 64) are never written again, rows past Lk keep finite data
-  for (uint32_t i = tid; i < Cf::TOTAL / 16; i += 256) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
-  __syncthreads();
-  pdl_wait();          // the zero fill and the TMEM allocation overlap the previous kernel's tail
-
-  const __half* kbh = kh + ((long)n * Lk) * k_pitch + h * D;
-  const __half* kbl = kl + ((long)n * Lk) * k_pitch + h * D;
-  const __half* vbh = vh + ((long)n * Lk) * v_pitch + h * D;
-  const __half* vbl = vl + ((long)n * Lk) * v_pitch + h * D;
-  auto issue_k = [&](int j0) {
-    for (int it = tid; it < AT_BK * Cf::C8; it += 256) {
-      const int r = it / Cf::C8, c8 = it - r * Cf::C8;
-      if (j0 + r >= Lk) continue;
-      const long src = (long)(j0 + r) * k_pitch + c8 * 8;
-      const uint32_t off = (uint32_t)(c8 >> 3) * (AT_BK * 128) + sw128(r, c8 & 7);
-      at_cp16(k_hi + off, kbh + src);
-      at_cp16(k_lo + off, kbl + src);
-    }
-  };
-  auto issue_v = [&](int j0) {
-    if (!VT) {
-      for (int it = tid; it < AT_BK * Cf::C8; it += 256) {
-        const int r = it / Cf::C8, c8 = it - r * Cf::C8;
-        if (j0 + r >= Lk) continue;
-        const long src = (long)(j0 + r) * v_pitch + c8 * 8;
-        const uint32_t off = (uint32_t)(c8 >> 3) * (AT_BK * 128) + sw128(r, c8 & 7);
-        at_cp16(v_hi + off, vbh + src);
-        at_cp16(v_lo + off, vbl + src);
-      }
-    } else {
-      // transposed tile [channel rows][64 keys]: lanes take consecutive keys
-      const int key = tid & 63, part = tid >> 6;
-      const bool kok = j0 + key < Lk;
-      for (int c8 = part; c8 < Cf::C8; c8 += 4) {
-        uint4 a = make_uint4(0u, 0u, 0u, 0u), b = a;
-        if (kok) {
-          a = *reinterpret_cast<const uint4*>(vbh + (long)(j0 + key) * v_pitch + c8 * 8);
-          b = *reinterpret_cast<const uint4*>(vbl + (long)(j0 + key) * v_pitch + c8 * 8);
-        }
-        const __half* ah = reinterpret_cast<const __half*>(&a);
-        const __half* bl = reinterpret_cast<const __half*>(&b);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const uint32_t off = sw128(c8 * 8 + i, key >> 3) + (uint32_t)(key & 7) * 2u;
-          *reinterpret_cast<__half*>(v_hi + off) = ah[i];
-          *reinterpret_cast<__half*>(v_lo + off) = bl[i];
-        }
-      }
-    }
-  };
-
-  // ---- Q tile (unscaled: the scale is applied to S), then the first K and V blocks
-  {
-    const __half* qbh = qh + ((long)n * Lq) * q_pitch + h * D;
-    const __half* qbl = ql + ((long)n * Lq) * q_pitch + h * D;
-    for (int it = tid; it < AT_ROWS * Cf::C8; it += 256) {
-      const int r = it / Cf::C8, c8 = it - r * Cf::C8;
-      if (q0 + r >= Lq) continue;
-      const long src = (long)(q0 + r) * q_pitch + c8 * 8;
-      const uint32_t off = (uint32_t)(c8 >> 3) * (AT_ROWS * 128) + sw128(r, c8 & 7);
-      at_cp16(q_hi + off, qbh + src);
-      at_cp16(q_lo + off, qbl + src);
-    }
-  }
-  issue_k(0);
-  cp_async_commit_();
-  issue_v(0);
-  cp_async_commit_();
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t lane_base = ((uint32_t)(quad * 32)) << 16;
-  const uint32_t tm_s = tmem, tm_o = tmem + AT_BK;        // S: columns [0, 64); O_blk of key half x: [64 + x * DP, ...)
-  const uint32_t idesc_s = (1u << 4) | ((uint32_t)(AT_BK >> 3) << 17) | ((uint32_t)(AT_ROWS >> 4) << 24);
-  const uint32_t idesc_o = (1u << 4) | (VT ? 0u : (1u << 16)) | ((uint32_t)(Cf::DP >> 3) << 17) | ((uint32_t)(AT_ROWS >> 4) << 24);
-
-  float acc[Cf::DP];
-#pragma unroll
-  for (int c = 0; c < Cf::DP; ++c) acc[c] = 0.f;
-  float m_run = -INFINITY, l_run = 0.f;
-  const int nblk = (Lk + AT_BK - 1) / AT_BK;
-  uint32_t ph_s = 0, ph_o = 0;
-
-  for (int blk = 0; blk < nblk; ++blk) {
-    const int j0 = blk * AT_BK;
-    at_cp_wait<1>();                 // everything but the youngest group (V of this block): Q and K(blk) have landed
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one()) {
-        uint32_t nz = 0;
-#pragma unroll
-        for (int c = 0; c < Cf::NCH; ++c) {
-          const int kv = (D - c * 64) < 64 ? (D - c * 64) : 64;
-          const int ksteps = (kv + 15) >> 4;
-          const uint64_t dqh = make_desc(smem_u32(q_hi + c * AT_ROWS * 128)), dql = make_desc(smem_u32(q_lo + c * AT_ROWS * 128));
-          const uint64_t dkh = make_desc(smem_u32(k_hi + c * AT_BK * 128)), dkl = make_desc(smem_u32(k_lo + c * AT_BK * 128));
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const uint64_t ko = (uint64_t)(2 * ks);
-            at_umma_f16(tm_s, dqh + ko, dkh + ko, idesc_s, nz);
-            nz = 1u;
-            at_umma_f16(tm_s, dql + ko, dkh + ko, idesc_s, 1u);
-            at_umma_f16(tm_s, dqh + ko, dkl + ko, idesc_s, 1u);
-          }
-        }
-        umma_commit(&bar_s);
-      }
-      __syncwarp();
-    }
-    mbar_wait(&bar_s, ph_s);
-    ph_s ^= 1u;
-    tc_fence_after();
-    if (blk + 1 < nblk) issue_k(j0 + AT_BK);      // the K tile is free once S is complete
-    cp_async_commit_();
-    // ---- online softmax over this thread's 32 keys of the block
-    float s[32];
-    at_ld32(tm_s + lane_base + (uint32_t)(32 * half), s);
-    float mb = -INFINITY;
-    const int jb = j0 + 32 * half;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      s[j] = (jb + j < Lk) ? s[j] * qscale : -INFINITY;
-      mb = fmaxf(mb, s[j]);
-    }
-    const float m_new = fmaxf(m_run, mb);
-    float alpha = 1.f;
-    if (m_new == -INFINITY) {          // no valid key for this half so far
-#pragma unroll
-      for (int j = 0; j < 32; ++j) s[j] = 0.f;
-    } else {
-      alpha = exp2f(m_run - m_new);    // exp2(-inf) = 0 on the first valid block
-      float lsum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) { s[j] = exp2f(s[j] - m_new); lsum += s[j]; }
-      l_run = l_run * alpha + lsum;
-      m_run = m_new;
-    }
-#pragma unroll
-    for (int c8 = 0; c8 < 4; ++c8) {
-      uint4 hi, lo;
-      hi.x = at_split2(s[8 * c8 + 0], s[8 * c8 + 1], lo.x);
-      hi.y = at_split2(s[8 * c8 + 2], s[8 * c8 + 3], lo.y);
-      hi.z = at_split2(s[8 * c8 + 4], s[8 * c8 + 5], lo.z);
-      hi.w = at_split2(s[8 * c8 + 6], s[8 * c8 + 7], lo.w);
-      const uint32_t off = sw128(row, 4 * half + c8);
-      *reinterpret_cast<uint4*>(p_hi + off) = hi;
-      *reinterpret_cast<uint4*>(p_lo + off) = lo;
-    }
-    at_cp_wait<1>();                 // V(blk) has landed (K(blk + 1) may still be in flight)
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    // ---- O_blk(half x) = P[:, 32x .. 32x + 32) V[32x .. 32x + 32, :]   (two k-steps per key half)
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dph = make_desc(smem_u32(p_hi)), dpl = make_desc(smem_u32(p_lo));
-#pragma unroll
-        for (int kk = 0; kk < AT_BK / 16; ++kk) {
-          const uint32_t td = tm_o + (uint32_t)((kk >> 1) * Cf::DP);
-          const uint32_t accf = (kk & 1) ? 1u : 0u;
-          const uint64_t ka = (uint64_t)(2 * kk);
-          uint64_t dvh, dvl;
-          if (VT) {
-            dvh = make_desc(smem_u32(v_hi)) + ka;
-            dvl = make_desc(smem_u32(v_lo)) + ka;
-          } else {
-            dvh = make_desc_mn(smem_u32(v_hi) + (uint32_t)kk * 16u * 128u, AT_BK * 128);
-            dvl = make_desc_mn(smem_u32(v_lo) + (uint32_t)kk * 16u * 128u, AT_BK * 128);
-          }
-          at_umma_f16(td, dph + ka, dvh, idesc_o, accf);
-          at_umma_f16(td, dpl + ka, dvh, idesc_o, 1u);
-          at_umma_f16(td, dph + ka, dvl, idesc_o, 1u);
-        }
-        umma_commit(&bar_o);
-      }
-      __syncwarp();
-    }
-    mbar_wait(&bar_o, ph_o);
-    ph_o ^= 1u;
-    tc_fence_after();
-    if (blk + 1 < nblk) issue_v(j0 + AT_BK);      // the V tile is free once O_blk is complete
-    cp_async_commit_();
-    {
-      float ob[16];
-#pragma unroll
-      for (int c0 = 0; c0 < Cf::DP; c0 += 16) {
-        at_ld16(tm_o + (uint32_t)(half * Cf::DP) + lane_base + (uint32_t)c0, ob);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[c0 + i] = fmaf(acc[c0 + i], alpha, ob[i]);
-      }
-    }
-    tc_fence_before();
-  }
-  at_cp_wait<0>();
-  __syncthreads();                  // all MMAs are complete (bar_o) and every thread has left the loop: the tiles are free
-
-  // ---- merge the two key halves of a row through shared memory, normalise, store
-  float* mw = reinterpret_cast<float*>(smem);              // [128 rows][D + 2]
-  if (half == 1) {
-    float* w = mw + row * (D + 2);
-    w[0] = m_run; w[1] = l_run;
-#pragma unroll
-    for (int c = 0; c < D; ++c) w[2 + c] = acc[c];
-  }
-  __syncthreads();
-  if (half == 0 && q0 + row < Lq) {
-    const float* w = mw + row * (D + 2);
-    const float m1 = w[0], l1 = w[1];
-    const float m = fmaxf(m_run, m1);
-    const float a0 = exp2f(m_run - m);
-    const float a1 = (m1 == -INFINITY) ? 0.f : exp2f(m1 - m);
-    const float inv = 1.f / (l_run * a0 + l1 * a1);
-    const float s0 = a0 * inv, s1 = a1 * inv;
-#pragma unroll
-    for (int c = 0; c < D; ++c) acc[c] = acc[c] * s0 + w[2 + c] * s1;
-    if (phi) {
-      const long base = ((long)n * Lq + q0 + row) * o_pitch + h * D;
-#pragma unroll
-      for (int c = 0; c < D; c += 8) {
-        uint4 hi, lo;
-        hi.x = at_split2(acc[c], acc[c + 1], lo.x); hi.y = at_split2(acc[c + 2], acc[c + 3], lo.y);
-        hi.z = at_split2(acc[c + 4], acc[c + 5], lo.z); hi.w = at_split2(acc[c + 6], acc[c + 7], lo.w);
-        *reinterpret_cast<uint4*>(phi + base + c) = hi;
-        *reinterpret_cast<uint4*>(plo + base + c) = lo;
-      }
-    } else {
-      float* op = o + ((long)n * Lq + q0 + row) * o_pitch + h * D;
-#pragma unroll
-      for (int c = 0; c < D; c += 4)
-        *reinterpret_cast<float4*>(op + c) = make_float4(acc[c], acc[c + 1], acc[c + 2], acc[c + 3]);
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(Cf::TMEM_COLS) : "memory");
-  }
-}
-
-template <int D, bool VT>
-void launch_ap(const __half* qh, const __half* ql, int q_pitch, const __half* kh, const __half* kl, int k_pitch,
-               const __half* vh, const __half* vl, int v_pitch, float* o, int o_pitch, int N, int heads, int Lq, int Lk,
-               cudaStream_t st, __half* phi, __half* plo) {
-  using Cf = ApCfg<D>;
-  static_assert(2u * Cf::DP * 128u <= Cf::V_BYTES, "transposed V tile does not fit");
-  const size_t smem = Cf::TOTAL + 1024;
-  static bool done[64] = {false};
-  int dev = 0;
-  AGPT_CUDA(cudaGetDevice(&dev));
-  if (!done[dev & 63]) {
-    AGPT_CUDA(cudaFuncSetAttribute(attention_pl_kernel<D, VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    done[dev & 63] = true;
-  }
-  const float qscale = (1.0f / sqrtf((float)D)) * 1.4426950408889634f;
-  dim3 grid(cdiv(Lq, AT_ROWS), heads, N);
-  launch_pdl(attention_pl_kernel<D, VT>, grid, dim3(256), smem, st, qh, ql, q_pitch, kh, kl, k_pitch, vh, vl, v_pitch, o, o_pitch, Lq, Lk,
-             qscale, phi, plo);
+  attention_tc_kernel<D><<<grid, 128, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, qscale);
 }
 
 }  // namespace
 
 // returns false when the head dim / alignment is not supported (caller uses the fp32 kernel)
 bool attention_tc(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st, __half* phi, __half* plo) {
+                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st) {
   if ((q_pitch | k_pitch | v_pitch | o_pitch) % 4 != 0) return false;
   if (((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
         reinterpret_cast<uintptr_t>(o)) & 15) != 0) return false;
-  if (phi && ((o_pitch % 8) != 0 || (d % 8) != 0 || ((reinterpret_cast<uintptr_t>(phi) | reinterpret_cast<uintptr_t>(plo)) & 15) != 0)) return false;
-#define AGPT_ATC(D_) launch_at<D_>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, Lq, Lk, st, phi, plo)
+#define AGPT_ATC(D_) launch_at<D_>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, Lq, Lk, st)
   switch (d) {
     case 8: AGPT_ATC(8); break;
     case 16: AGPT_ATC(16); break;
@@ -720,42 +306,6 @@ bool attention_tc(const float* q, int q_pitch, const float* k, int k_pitch, cons
     default: return false;
   }
 #undef AGPT_ATC
-  count_launch(1);
-  AGPT_CUDA(cudaGetLastError());
-  return true;
-}
-
-
-// q / k / v as fp16 hi/lo planes (pitches in elements); returns false when the shape is not supported
-bool attention_planes(const __half* qh, const __half* ql, int q_pitch, const __half* kh, const __half* kl, int k_pitch,
-                      const __half* vh, const __half* vl, int v_pitch, float* o, int o_pitch, int N, int heads, int d,
-                      int Lq, int Lk, cudaStream_t st, __half* phi, __half* plo) {
-  if ((q_pitch | k_pitch | v_pitch) % 8 != 0 || d % 8 != 0 || Lk < 1) return false;
-  const uintptr_t al = reinterpret_cast<uintptr_t>(qh) | reinterpret_cast<uintptr_t>(ql) | reinterpret_cast<uintptr_t>(kh) |
-                       reinterpret_cast<uintptr_t>(kl) | reinterpret_cast<uintptr_t>(vh) | reinterpret_cast<uintptr_t>(vl);
-  if (al & 15) return false;
-  if (phi) {
-    if ((o_pitch % 8) != 0 || ((reinterpret_cast<uintptr_t>(phi) | reinterpret_cast<uintptr_t>(plo)) & 15) != 0) return false;
-  } else if ((o_pitch % 4) != 0 || (reinterpret_cast<uintptr_t>(o) & 15) != 0) {
-    return false;
-  }
-  static int vt = -1;
-  if (vt < 0) { const char* e = getenv("AGPT_ATTN_VT"); vt = (e && e[0] == '1') ? 1 : 0; }
-#define AGPT_APL(D_)                                                                                                     \
-  do {                                                                                                                   \
-    if (vt) launch_ap<D_, true>(qh, ql, q_pitch, kh, kl, k_pitch, vh, vl, v_pitch, o, o_pitch, N, heads, Lq, Lk, st, phi, plo);  \
-    else launch_ap<D_, false>(qh, ql, q_pitch, kh, kl, k_pitch, vh, vl, v_pitch, o, o_pitch, N, heads, Lq, Lk, st, phi, plo);    \
-  } while (0)
-  switch (d) {
-    case 8: AGPT_APL(8); break;
-    case 16: AGPT_APL(16); break;
-    case 32: AGPT_APL(32); break;
-    case 40: AGPT_APL(40); break;
-    case 64: AGPT_APL(64); break;
-    case 80: AGPT_APL(80); break;
-    default: return false;
-  }
-#undef AGPT_APL
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
   return true;

@@ -1,4 +1,4 @@
-// Common host/device helpers for libagpt_b200 (sm_100a only).
+// Common host/device helpers for libagpt_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -35,12 +35,11 @@ struct Error : public std::runtime_error {
 
 // ---- programmatic dependent launch ---------------------------------------------
 // The denoising steps are chains of 50-240 short dependent kernels.  A kernel launched through launch_pdl() may
-// start (block scheduling, shared-memory carve-up, barrier init, TMEM allocation, tensor-map prefetch) while its
+// start (block scheduling, shared-memory carve-up, barrier init, tensor-map prefetch) while its
 // predecessor in the stream is still draining; it calls pdl_wait() before its first access to global memory, which
 // returns once the predecessor has completed and flushed.  ONLY kernels that call pdl_wait() may go through
-// launch_pdl(); everything else keeps the ordinary stream order.  Measured on the graph-replayed loops (profiles/
-// r2n_pdl_ab.txt): DiffSinger C3 -2.6 %, DDIM-100 +1.4 %, HiFi-GAN unchanged -- the replayed graphs leave little launch
-// gap to hide and the early CTAs compete with the predecessor's last wave.  Opt-in: AGPT_PDL=1.
+// launch_pdl(); everything else keeps the ordinary stream order.  The replayed graphs leave little launch gap
+// to hide and the early CTAs compete with the predecessor's last wave, so it is opt-in: AGPT_PDL=1.
 inline bool pdl_enabled() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("AGPT_PDL"); v = (e && e[0] == '1') ? 1 : 0; }

@@ -1,4 +1,4 @@
-// DiffNet epsilon-predictor + GaussianDiffusion step arithmetic on sm_100a.
+// DiffNet epsilon-predictor + GaussianDiffusion step arithmetic on sm_90a.
 // Reference: NeuralSeq/modules/diff/net.py:58-130 (DiffNet, ResidualBlock, SinusoidalPosEmb),
 //            NeuralSeq/modules/diff/shallow_diffusion_tts.py:134-204 (p_sample / PLMS algebra).
 // Parity: tests/test_diffusion_gpu.py against oracle/diffusion_ref.py and tests/golden/diffusion_*.npz.
@@ -73,51 +73,6 @@ __global__ void p_sample_tab_kernel(float* __restrict__ x, const float* __restri
   }
 }
 
-// ---- operand-plane helpers of the plane-fed DiffNet layers (tcconv7.cu consumes fp16 hi/lo planes) ----
-__device__ __forceinline__ void dn_split(float v, __half& hi, __half& lo) {
-  hi = __float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f));
-  lo = __float2half_rn(v - __half2float(hi));
-}
-// planes of x[b][t][c] + vec[b][c]   (net.py:67: y = x + diffusion_projection(step)); vec_gs = 0: one row for all samples
-__global__ void addvec_planes_kernel(const float* __restrict__ x, const float* __restrict__ vec, int vec_gs, long per_sample, int C,
-                                     __half* __restrict__ phi, __half* __restrict__ plo, long total) {
-  pdl_wait();
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const long b = i / per_sample;
-    const int c = (int)(i % C);
-    dn_split(x[i] + vec[b * vec_gs + c], phi[i], plo[i]);
-  }
-}
-// y [rows][2C] with (gate, filter) pairs interleaved -> planes of sigmoid(gate) * tanh(filter) [rows][C]   (net.py:72-74)
-__global__ void gate_planes_kernel(const float* __restrict__ y, __half* __restrict__ phi, __half* __restrict__ plo, long n2) {
-  pdl_wait();
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += (long)gridDim.x * blockDim.x) {
-    const float4 v = __ldg(reinterpret_cast<const float4*>(y) + i);     // (g0, f0, g1, f1)
-    const float o0 = sigmoidf_(v.x) * tanhf(v.y), o1 = sigmoidf_(v.z) * tanhf(v.w);
-    const __half2 hh = __floats2half2_rn(o0, o1);
-    const float2 hf = __half22float2(hh);
-    reinterpret_cast<__half2*>(phi)[i] = hh;
-    reinterpret_cast<__half2*>(plo)[i] = __floats2half2_rn(o0 - hf.x, o1 - hf.y);
-  }
-}
-// o [rows][2C] = output_projection(z) (bias included): x <- (x + o[:C]) / sqrt(2) in place, skip (+)= o[C:], and the
-// planes of x_new + vec_next (the next layer's diffusion projection) when phi != nullptr   (net.py:76-78, 67)
-__global__ void diffout_planes_kernel(const float* __restrict__ o, float* __restrict__ x, float* __restrict__ skip, int accumulate,
-                                      const float* __restrict__ vec_next, int vec_gs, long per_sample, int C,
-                                      __half* __restrict__ phi, __half* __restrict__ plo, long total) {
-  pdl_wait();
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const long row = i / C;
-    const int c = (int)(i - row * C);
-    const float r2 = 0.70710678118654752440f;
-    const float xn = (x[i] + o[row * 2 * C + c]) * r2;
-    x[i] = xn;
-    const float sk = o[row * 2 * C + C + c];
-    skip[i] = accumulate ? skip[i] + sk : sk;
-    if (phi) { const long b = i / per_sample; dn_split(xn + vec_next[b * vec_gs + c], phi[i], plo[i]); }
-  }
-}
-
 __global__ void axpby5_kernel(const float* __restrict__ x, const float* __restrict__ e0, const float* __restrict__ e1,
                               const float* __restrict__ e2, const float* __restrict__ e3,
                               const float* __restrict__ coef, long n, float* __restrict__ out) {
@@ -165,7 +120,6 @@ struct Diffnet : Handle {
   // state
   int B = 0, T = 0;
   DevBuf condT, condp, xT, xcur, z, skip, hbuf, emb, e1, e2, dproj, eps_tmp;
-  DevBuf ybuf, obuf, plx, plz;    // plane-fed layers: raw GEMM outputs [rows][2C] and the operand planes of x + dproj / z
   // sampling-loop state (one captured step replayed; see gd_sample_loop)
   DevBuf dproj_table, dproj_cur, coef_table, t_dev, step_ctr, loop_eps, loop_x;
   cudaGraphExec_t step_graph = nullptr;
@@ -241,50 +195,6 @@ struct Diffnet : Handle {
       tapconv_launch(P, st);
     }
     const long gs = (long)T * C;
-    static int allow_planes = -1;
-    if (allow_planes < 0) { const char* e = getenv("AGPT_DIFFNET_PLANES"); allow_planes = (e && e[0] == '0') ? 0 : 1; }
-    if (allow_planes && C % 16 == 0 && (2 << (cfg.dilation_cycle_length - 1)) <= 120 && tc_enabled() && tc_get_version() >= 6) {
-      // ---- plane-fed residual layers: both GEMMs of a layer run on tcconv7 (TMA -> tcgen05, TMA epilogue) writing
-      // raw fp32 [rows][2C]; two light passes apply the gate / the residual-skip update and write the operand planes
-      // of the next GEMM.  (The fused-epilogue kernels of round 1 were latency-bound at 6 400 rows: 38 + 30 us per layer.)
-      const long rows = (long)B * T, n = rows * C;
-      ybuf.ensure((size_t)rows * 2 * C); obuf.ensure((size_t)rows * 2 * C);
-      plx.ensure((size_t)n + 16); plz.ensure((size_t)n + 16);
-      __half* xh = reinterpret_cast<__half*>(plx.p); __half* xl = xh + n;
-      __half* zh = reinterpret_cast<__half*>(plz.p); __half* zl = zh + n;
-      const unsigned eg = (unsigned)std::min<long>(cdivl(n, 256), 4736);
-      launch_pdl(addvec_planes_kernel, dim3(eg), dim3(256), 0, st, xcur.p, dprojv, dproj_gs, gs, C, xh, xl, n);
-      count_launch(1);
-      auto gemm = [&](const PackedConv& pc, int dilv, const __half* ih, const __half* il, float* outp_, const float* res_,
-                      long res_gs, int res_pitch) {
-        TapConvParams P = tapconv_params(pc, B, T, 0, dilv);
-        P.in = nullptr; P.in_gstride = gs; P.in_pitch = C;
-        P.out = outp_; P.out_gstride = (long)T * 2 * C; P.out_pitch = 2 * C;
-        P.pro = PRO_NONE; P.epi = res_ ? EPI_RES : EPI_BIAS;
-        P.res = res_; P.res_gstride = res_gs; P.res_pitch = res_pitch;
-        PlaneIO Q;
-        memset(&Q, 0, sizeof(Q));
-        Q.in_hi = ih; Q.in_lo = il; Q.in_gstride = gs; Q.in_pitch = C;
-        Q.store_f32 = 1;
-        const double r = (double)rows;
-        void* rec = profile_begin(P, true, 4.0 * (r * C + r * 2 * C * (res_ ? 2 : 1) + (double)pc.ntaps * C * 2 * C), st);
-        AGPT_CHECK(tcconv7_launch(P, Q, st), "plane-fed kernel rejected a DiffNet layer");
-        profile_end(rec, st);
-        count_launch(1);
-      };
-      for (int l = 0; l < L; ++l) {
-        const int d = 1 << (l % cfg.dilation_cycle_length);
-        // y = dilated_conv(x + dproj) + conditioner_projection(cond)     (net.py:67-71; the conditioner is the TMA-loaded residual)
-        gemm(dil[l], d, xh, xl, ybuf.p, condp.p + (long)l * 2 * C, (long)T * L * 2 * C, L * 2 * C);
-        launch_pdl(gate_planes_kernel, dim3(eg), dim3(256), 0, st, ybuf.p, zh, zl, n / 2);
-        gemm(outp[l], 1, zh, zl, obuf.p, nullptr, 0, 0);
-        const bool last = l + 1 == L;
-        launch_pdl(diffout_planes_kernel, dim3(eg), dim3(256), 0, st, obuf.p, xcur.p, skip.p, l > 0 ? 1 : 0, last ? dprojv : dprojv + (long)(l + 1) * C, dproj_gs, gs, C,
-                   last ? nullptr : xh, last ? nullptr : xl, n);
-        count_launch(2);
-      }
-      AGPT_CUDA(cudaGetLastError());
-    } else
     for (int l = 0; l < L; ++l) {
       const int d = 1 << (l % cfg.dilation_cycle_length);
       {  // y = dilated_conv(x + dproj) + cond_proj ; z = sigmoid(gate)*tanh(filter)   (net.py:67-74)

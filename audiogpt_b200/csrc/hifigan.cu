@@ -1,4 +1,4 @@
-// HiFi-GAN generator on sm_100a: host driver + the small non-contraction kernels.
+// HiFi-GAN generator on sm_90a: host driver + the small non-contraction kernels.
 // Arithmetic follows NeuralSeq/modules/hifigan/hifigan.py:144-169 (reference) and is
 // parity-checked against oracle/hifigan_ref.py in tests/test_hifigan_gpu.py.
 #include "common.cuh"
@@ -123,7 +123,7 @@ struct AaFilter { float f[12]; };
 constexpr int AA_TT = 64;
 __global__ void __launch_bounds__(256) aa_snake_kernel(const float* __restrict__ x, float* __restrict__ y,
                                                         const float* __restrict__ a, const float* __restrict__ inv_b,
-                                                        int L, int C, AaFilter F, __half* __restrict__ phi, __half* __restrict__ plo) {
+                                                        int L, int C, AaFilter F) {
   __shared__ float xs[AA_TT + 12][32];
   __shared__ float ss[2 * AA_TT + 10][32];
   const int tx = threadIdx.x, ty = threadIdx.y;
@@ -163,14 +163,7 @@ __global__ void __launch_bounds__(256) aa_snake_kernel(const float* __restrict__
     float acc = 0.f;
 #pragma unroll
     for (int k = 0; k < 12; ++k) acc = fmaf(F.f[k], ss[2 * r + k][tx], acc);
-    if (phi) {        // operand planes for the plane-fed conv that consumes this activation (no fp32 copy)
-      const __half hh = __float2half_rn(fminf(fmaxf(acc, -65504.f), 65504.f));
-      const long o = ((long)b * L + t) * C + c;
-      phi[o] = hh;
-      plo[o] = __float2half_rn(acc - __half2float(hh));
-    } else {
-      yb[(long)t * C + c] = acc;
-    }
+    yb[(long)t * C + c] = acc;
   }
 }
 
@@ -340,8 +333,6 @@ struct Hifigan : Handle {
   AaFilter aaf;                     // the 12 Kaiser-sinc taps (state-dict buffer)
   int c_last = 0, hop = 1;
   DevBuf melT, buf[6], sbuf;        // sbuf: activated conv input (BigVGAN only)
-  DevBuf pbuf[5];                   // operand planes (fp16 hi | lo = one fp32 tensor's bytes each): cur, X, A, R0, R1
-  bool planes_ok = false;           // every ResBlock conv fits the plane-fed kernel (halo <= 128 rows)
   DevBuf io_mel, io_wav, io_har;  // staging for the host-buffer entry point
   float* pin_mel = nullptr; float* pin_wav = nullptr; size_t pin_mel_n = 0, pin_wav_n = 0;
   cudaStream_t own_stream = nullptr;
@@ -352,125 +343,8 @@ struct Hifigan : Handle {
     if (own_stream) cudaStreamDestroy(own_stream);
   }
 
-  // ---- plane mode (default for HiFi-GAN without NSF excitation): every tensor that feeds a conv exists as fp16 hi/lo
-  // OPERAND PLANES of leaky_relu(x, 0.1), written by the producing conv's epilogue; the convs run on the plane-fed
-  // kernel (tcconv7.cu: TMA -> tcgen05, no transform warps).  Data flow per ResBlock1 pair (hifigan.py:54-61):
-  //   c1: P(x) -> P(A) only (A is never needed in fp32);  c2: P(A) + residual x (fp32) -> x' fp32 + P(x');
-  //   the last pair reduce-adds x'/3 into the MRF accumulator, whose planes are made by one light pass per stage.
-  struct Planes { __half* hi; __half* lo; };
-  Planes planes_of(DevBuf& b, size_t elems) {
-    float* p = b.ensure(elems + 8);
-    __half* h = reinterpret_cast<__half*>(p);
-    return Planes{h, h + elems};
-  }
-  bool conv_planes(const PackedConv& pc, int Bn, long L, int Cin_, int dil, Planes in, float* out_f32, int out_pitch, long out_gs,
-                   Planes* outp, int epi, const float* res_, float scale, int accumulate, cudaStream_t st) {
-    TapConvParams P = tapconv_params(pc, Bn, (int)L, 0, dil);
-    P.in = nullptr; P.in_gstride = L * Cin_; P.in_pitch = Cin_;
-    P.out = out_f32; P.out_gstride = out_gs; P.out_pitch = out_pitch;
-    P.pro = PRO_NONE; P.epi = epi; P.scale = scale; P.accumulate = accumulate;
-    P.res = res_; P.res_gstride = out_gs; P.res_pitch = out_pitch;
-    PlaneIO Q;
-    memset(&Q, 0, sizeof(Q));
-    Q.in_hi = in.hi; Q.in_lo = in.lo; Q.in_gstride = L * Cin_; Q.in_pitch = Cin_;
-    if (outp) { Q.out_hi = outp->hi; Q.out_lo = outp->lo; Q.outp_gstride = out_gs; Q.outp_pitch = out_pitch; }
-    Q.out_pro = PRO_LRELU; Q.out_slope = 0.1f;
-    Q.store_f32 = out_f32 != nullptr ? 1 : 0;
-    const double rows = (double)Bn * (double)L;
-    const double bytes = 4.0 * rows * Cin_ /* hi + lo planes */ + (Q.store_f32 ? 4.0 * rows * pc.Cout : 0.0) +
-                         (outp ? 4.0 * rows * pc.Cout : 0.0) + (res_ ? 4.0 * rows * pc.Cout : 0.0) +
-                         (epi == EPI_ACC && accumulate ? 4.0 * rows * pc.Cout : 0.0) + 4.0 * pc.ntaps * pc.Cin * pc.Cout;
-    void* rec = profile_begin(P, true, bytes, st);
-    if (!tcconv7_launch(P, Q, st)) return false;
-    profile_end(rec, st);
-    count_launch(1);
-    AGPT_CUDA(cudaGetLastError());
-    return true;
-  }
-
-  void forward_planes(const float* mel, int B, int T, float* wav, cudaStream_t st) {
-    const int C0 = cfg.upsample_initial_channel;
-    size_t mx = (size_t)T * C0;
-    {
-      long L = T; int C = C0;
-      for (int i = 0; i < cfg.num_upsamples; ++i) { L *= cfg.upsample_rates[i]; C /= 2; mx = std::max(mx, (size_t)L * C); }
-    }
-    mx *= (size_t)B;
-    for (int i = 0; i < 6; ++i) if (i != 3) buf[i].ensure(mx);     // buf[3] (the fp32 c1 output) is not needed
-    melT.ensure((size_t)B * T * cfg.n_mels);
-    float *cur = buf[0].p, *acc = buf[1].p, *X = buf[2].p, *R0 = buf[4].p, *R1 = buf[5].p;
-    Planes Pcur = planes_of(pbuf[0], mx), PX = planes_of(pbuf[1], mx), PA = planes_of(pbuf[2], mx);
-    Planes PR[2] = {planes_of(pbuf[3], mx), planes_of(pbuf[4], mx)};
-    launch_cf_to_cl(mel, melT.p, B, cfg.n_mels, T, st);
-    {
-      TapConvParams P = tapconv_params(conv_pre, B, T, 0, 1);
-      P.in = melT.p; P.in_gstride = (long)T * cfg.n_mels; P.in_pitch = cfg.n_mels;
-      P.out = cur; P.out_gstride = (long)T * C0; P.out_pitch = C0;
-      P.pro = PRO_NONE; P.epi = EPI_BIAS;
-      tapconv_launch(P, st);
-    }
-    long L = T; int C = C0;
-    const float inv_nk = 1.f / (float)cfg.num_kernels;
-    for (int i = 0; i < cfg.num_upsamples; ++i) {
-      const int u = cfg.upsample_rates[i];
-      const int Co = C / 2;
-      make_planes(cur, Pcur.hi, Pcur.lo, (long)B * L * C, PRO_LRELU, 0.1f, st);
-      // leaky_relu(0.1) -> ConvTranspose1d (polyphase: u * Co output channels per input row); X fp32 + P(X)
-      AGPT_CHECK(conv_planes(ups[i], B, L, C, 1, Pcur, X, u * Co, L * u * Co, &PX, EPI_BIAS, nullptr, 1.f, 0, st),
-                 "plane-fed kernel rejected an upsample layer");
-      L *= u; C = Co;
-      const long gs = L * C;
-      for (int j = 0; j < cfg.num_kernels; ++j) {
-        const ResBlockW& rb = rbs[i * cfg.num_kernels + j];
-        const float* x = X;
-        Planes px = PX;
-        const int nd = (int)rb.dil.size();
-        for (int n = 0; n < nd; ++n) {
-          const bool last = (n == nd - 1);
-          float* dst = last ? acc : ((n & 1) ? R1 : R0);
-          Planes pin = px;
-          if (cfg.resblock_type == 1) {
-            AGPT_CHECK(conv_planes(rb.c1[n], B, L, C, rb.dil[n], px, nullptr, C, gs, &PA, EPI_BIAS, nullptr, 1.f, 0, st),
-                       "plane-fed kernel rejected a ResBlock conv");
-            pin = PA;
-          }
-          const PackedConv& pc = (cfg.resblock_type == 1) ? rb.c2[n] : rb.c1[n];
-          const int d2 = (cfg.resblock_type == 1) ? 1 : rb.dil[n];
-          bool ok;
-          if (last) ok = conv_planes(pc, B, L, C, d2, pin, dst, C, gs, nullptr, EPI_ACC, x, inv_nk, j > 0 ? 1 : 0, st);
-          else ok = conv_planes(pc, B, L, C, d2, pin, dst, C, gs, &PR[n & 1], EPI_RES, x, 1.f, 0, st);
-          AGPT_CHECK(ok, "plane-fed kernel rejected a ResBlock conv");
-          x = dst; px = PR[n & 1];
-        }
-      }
-      std::swap(cur, acc);
-    }
-    {
-      const int threads = 256;
-      dim3 grid(cdiv((int)L, threads), B);
-      const size_t smem = (size_t)cfg.c_out * 7 * C * sizeof(float);
-      if (C == 32 && smem <= 8 * 1024)
-        conv_post32_kernel<<<grid, CP_ROWS, smem, st>>>(cur, post_w.p, post_b.p, wav, (int)L, cfg.c_out, 0.01f);
-      else
-        conv_post_kernel<<<grid, threads, smem, st>>>(cur, post_w.p, post_b.p, wav, (int)L, C, cfg.c_out, 0.01f);
-      count_launch(1);
-      AGPT_CUDA(cudaGetLastError());
-    }
-  }
-
   void forward(const float* mel, const float* har, int B, int T, float* wav, cudaStream_t st) {
     AGPT_CHECK(B >= 1 && T >= 1, "empty batch");
-    {
-      // Measured on B200 (profiles/r2c_planes_microbench.txt, r2c_bench_planes.json): the plane-fed kernel wins on the
-      // latency-bound small GEMMs of the UNet but LOSES on this generator's big epilogue-bound layers (8 x 800 frames:
-      // 21.8 ms vs 18.5 ms) -- the extra plane stores cost more than the transform warps did.  Opt-in: AGPT_PLANES=1.
-      static int allow_planes = -1;
-      if (allow_planes < 0) { const char* e = getenv("AGPT_PLANES"); allow_planes = (e && e[0] == '1') ? 1 : 0; }
-      if (allow_planes && planes_ok && !har && cfg.activation == 0 && tc_enabled() && tc_get_version() >= 6) {
-        forward_planes(mel, B, T, wav, st);
-        return;
-      }
-    }
     const int C0 = cfg.upsample_initial_channel;
     // buffer sizing: max over stages of L_i * C_i
     size_t mx = (size_t)T * C0;
@@ -487,24 +361,10 @@ struct Hifigan : Handle {
     float* S = sbuf.p;
     auto snake = [&](const float* src, float* dst, long Lr, int Cr, const SnakeW& w) {
       dim3 block(32, 8), grid(cdiv((int)Lr, AA_TT), cdiv(Cr, 32), B);
-      aa_snake_kernel<<<grid, block, 0, st>>>(src, dst, w.a.p, w.inv_b.p, (int)Lr, Cr, aaf, nullptr, nullptr);
+      aa_snake_kernel<<<grid, block, 0, st>>>(src, dst, w.a.p, w.inv_b.p, (int)Lr, Cr, aaf);
       count_launch(1);
       AGPT_CUDA(cudaGetLastError());
     };
-    // BigVGAN in plane mode: the anti-aliased snake writes fp16 hi/lo operand planes and the conv that follows runs on
-    // the plane-fed kernel (fp32 result, no emitted planes: the next consumer is again a snake reading fp32)
-    static int allow_planes_b = -1;
-    if (allow_planes_b < 0) { const char* e = getenv("AGPT_PLANES"); allow_planes_b = (e && e[0] == '1') ? 1 : 0; }
-    const bool bplanes = big && allow_planes_b && planes_ok && !har && tc_enabled() && tc_get_version() >= 6;
-    Planes PS{nullptr, nullptr};
-    if (bplanes) PS = planes_of(pbuf[0], mx);
-    auto snake_planes = [&](const float* src, long Lr, int Cr, const SnakeW& w) {
-      dim3 block(32, 8), grid(cdiv((int)Lr, AA_TT), cdiv(Cr, 32), B);
-      aa_snake_kernel<<<grid, block, 0, st>>>(src, nullptr, w.a.p, w.inv_b.p, (int)Lr, Cr, aaf, PS.hi, PS.lo);
-      count_launch(1);
-      AGPT_CUDA(cudaGetLastError());
-    };
-
     launch_cf_to_cl(mel, melT.p, B, cfg.n_mels, T, st);
     {
       TapConvParams P = tapconv_params(conv_pre, B, T, 0, 1);
@@ -518,11 +378,7 @@ struct Hifigan : Handle {
     for (int i = 0; i < cfg.num_upsamples; ++i) {
       const int u = cfg.upsample_rates[i];
       const int Co = C / 2;
-      if (bplanes) {
-        make_planes(cur, PS.hi, PS.lo, (long)B * L * C, PRO_NONE, 0.f, st);
-        AGPT_CHECK(conv_planes(ups[i], B, L, C, 1, PS, X, u * Co, L * u * Co, nullptr, EPI_BIAS, nullptr, 1.f, 0, st),
-                   "plane-fed kernel rejected an upsample layer");
-      } else {  // leaky_relu(0.1) -> ConvTranspose1d   (hifigan.py:153-154)
+      {  // leaky_relu(0.1) -> ConvTranspose1d   (hifigan.py:153-154)
         TapConvParams P = tapconv_params(ups[i], B, (int)L, 0, 1);
         P.in = cur; P.in_gstride = L * C; P.in_pitch = C;
         P.out = X; P.out_gstride = L * u * Co; P.out_pitch = u * Co;
@@ -547,23 +403,6 @@ struct Hifigan : Handle {
           const bool last = (n == nd - 1);
           float* dst = last ? acc : ((n & 1) ? R1 : R0);
           const float* conv_in = x;
-          if (bplanes) {
-            if (cfg.resblock_type == 1) {
-              snake_planes(x, L, C, rb.act[2 * n]);          // xt = a1(x)   (AMPBlock1.forward, models.py:75-76)
-              AGPT_CHECK(conv_planes(rb.c1[n], B, L, C, rb.dil[n], PS, A, C, gs, nullptr, EPI_BIAS, nullptr, 1.f, 0, st),
-                         "plane-fed kernel rejected an AMPBlock conv");
-              conv_in = A;
-            }
-            snake_planes(conv_in, L, C, rb.act[cfg.resblock_type == 1 ? 2 * n + 1 : n]);
-            const PackedConv& pc2 = (cfg.resblock_type == 1) ? rb.c2[n] : rb.c1[n];
-            const int d2 = (cfg.resblock_type == 1) ? 1 : rb.dil[n];
-            bool ok2;
-            if (last) ok2 = conv_planes(pc2, B, L, C, d2, PS, dst, C, gs, nullptr, EPI_ACC, x, inv_nk, j > 0 ? 1 : 0, st);
-            else ok2 = conv_planes(pc2, B, L, C, d2, PS, dst, C, gs, nullptr, EPI_RES, x, 1.f, 0, st);
-            AGPT_CHECK(ok2, "plane-fed kernel rejected an AMPBlock conv");
-            x = dst;
-            continue;
-          }
           if (cfg.resblock_type == 1) {
             if (big) snake(x, S, L, C, rb.act[2 * n]);      // xt = a1(x)   (AMPBlock1.forward, models.py:75-76)
             const int gq = (rb.g1[n] && L % rb.g1[n] == 0) ? rb.g1[n] : 1;      // time-grouped view [L/g][g*C] of the same memory
@@ -686,21 +525,6 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
       }
     }
   }
-  {  // plane mode needs every ResBlock conv's halo inside one tensor-map box (128 + (k-1)*dil <= 256 rows),
-     // 16-byte aligned fp16 rows (channels % 8) and channel counts the TMA epilogue's 32-column boxes cover
-    bool ok = true;
-    int Cc = C0;
-    for (int i = 0; i < nu; ++i) {
-      Cc /= 2;
-      if (Cc % 32 != 0) ok = false;
-      for (int j = 0; j < nk; ++j) {
-        const ResBlockW& rb = h->rbs[i * nk + j];
-        for (int d : rb.dil) if ((rb.ks - 1) * d > 120) ok = false;
-      }
-    }
-    if (C0 % 32 != 0) ok = false;
-    h->planes_ok = ok;
-  }
   if (cfg->activation != 0) load_snake(h->act_post, C);
   {  // conv_post [c_out][C][7] -> [c_out][7][C]
     const float* w = next(); const float* b = next();
@@ -737,9 +561,8 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
 }
 
 // Optional (AGPT_HIFI_L2_MB=<per-tensor MB>): run the generator over sub-batches whose per-stage tensors
-// fit the 126 MB L2 together.  Utterances are independent, so this changes nothing numerically.
-// Measured on B200 (B=8, T=800): 57-60 ms with sub-batching vs 51.4 ms without -- the smaller grids cost
-// more than the L2 hits save -- so it is OFF by default.
+// fit the 50 MB L2 together.  Utterances are independent, so this changes nothing numerically.
+// OFF by default: the smaller grids of a sub-batch fill fewer SMs (not measured on H100).
 static void hifigan_forward_l2(Hifigan* h, const float* mel, const float* har, int B, int T, float* wav, cudaStream_t st) {
   static long target = -1;
   if (target < 0) {

@@ -1,5 +1,5 @@
 // Micro-benchmark / tuning entry: one tapconv layer of a given shape on random data, timed with
-// CUDA events; optionally returns the per-CTA phase timestamps of the tcgen05 kernel.
+// CUDA events; optionally returns the per-CTA phase timestamps of the tensor-core kernel.
 #include <random>
 #include "tapconv.cuh"
 #include "models.h"
@@ -52,25 +52,7 @@ void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, i
     P.tc_flags_user = 2;
   }
   cudaStream_t st = nullptr;
-  // version 8: the plane-fed kernel (tcconv7.cu) -- planes of lrelu(x) in, fp32 result + planes of lrelu(result) out
-  const bool planes_mode = use_tc && tc_get_version() == 8;
-  DevBuf pin, pout;
-  PlaneIO PQ;
-  memset(&PQ, 0, sizeof(PQ));
-  if (planes_mode) {
-    AGPT_CHECK(!is2d, "the plane-fed kernel handles 1-D layers");
-    pin.ensure(nin + 8); pout.ensure(nout + 8);      // two fp16 planes = one fp32 tensor's bytes
-    __half* ih = reinterpret_cast<__half*>(pin.p); __half* il = ih + nin;
-    __half* oh = reinterpret_cast<__half*>(pout.p); __half* ol = oh + nout;
-    make_planes(x.p, ih, il, (long)nin, PRO_LRELU, 0.1f, st);
-    PQ.in_hi = ih; PQ.in_lo = il; PQ.in_gstride = (long)L * Cin; PQ.in_pitch = Cin;
-    PQ.out_hi = oh; PQ.out_lo = ol; PQ.outp_gstride = (long)L * Cout; PQ.outp_pitch = Cout;
-    PQ.out_pro = PRO_LRELU; PQ.out_slope = 0.1f; PQ.store_f32 = 1;
-  }
-  auto launch = [&]() {
-    if (planes_mode) { AGPT_CHECK(tcconv7_launch(P, PQ, st), "the plane-fed kernel rejected this layer"); count_launch(1); }
-    else tapconv_launch(P, st);
-  };
+  auto launch = [&]() { tapconv_launch(P, st); };
   for (int i = 0; i < 2; ++i) launch();
   cudaEvent_t e0, e1;
   AGPT_CUDA(cudaEventCreate(&e0)); AGPT_CUDA(cudaEventCreate(&e1));
@@ -83,8 +65,6 @@ void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, i
   out[0] = ms / reps;
   out[1] = 2.0 * G * (double)L * Cin * Cout * taps / (out[0] * 1e-3) / 1e12;
   out[2] = -1.0;
-  const int tcv = tc_get_version();
-  const bool raw_dbg = (tcv == 3 && taps >= 5) || tcv == 4 || tcv == 6 || tcv == 7;
   if (dbg_avg && use_tc) {
     std::vector<long long> h((size_t)nctas * 8);
     AGPT_CUDA(cudaMemcpy(h.data(), dbgbuf.p, h.size() * 8, cudaMemcpyDeviceToHost));
@@ -93,11 +73,6 @@ void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, i
     for (long c = 0; c < nctas; ++c) {
       const long long* d = &h[c * 8];
       if (d[0] == 0) continue;
-      if (raw_dbg) {                      // v3: the kernel already stores durations
-        for (int i = 0; i < 8; ++i) acc[i] += (double)d[i];
-        ++n;
-        continue;
-      }
       if (d[5] == 0) continue;
       acc[0] += (double)(d[1] - d[0]);   // setup
       acc[1] += (double)(d[2] - d[1]);   // until first activation tile is ready
@@ -132,19 +107,6 @@ void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, i
       const double rms = std::sqrt(sr / (double)nout);
       rel2[0] = finite ? (rms > 0 ? mx / rms : mx) : 1e30;
       rel2[1] = finite ? (rms > 0 ? std::sqrt(se / (double)nout) / rms : std::sqrt(se / (double)nout)) : 1e30;
-      if (planes_mode) {   // the emitted planes must hold lrelu(fp32 result): hi + lo == prologue(out) to 2^-21 relative
-        std::vector<__half> ph(nout), pl(nout);
-        AGPT_CUDA(cudaMemcpy(ph.data(), PQ.out_hi, nout * 2, cudaMemcpyDeviceToHost));
-        AGPT_CUDA(cudaMemcpy(pl.data(), PQ.out_lo, nout * 2, cudaMemcpyDeviceToHost));
-        double pm = 0;
-        for (size_t i = 0; i < nout; ++i) {
-          const float ref = a[i] > 0.f ? a[i] : 0.1f * a[i];
-          const double got = (double)__half2float(ph[i]) + (double)__half2float(pl[i]);
-          // hi + lo reproduces the value to 2^-21 relative, with the absolute floor 2^-24 of an fp16-subnormal lo part
-          pm = std::max(pm, std::fabs(got - (double)ref) / (std::fabs((double)ref) * 4.8e-7 + 6.0e-8));
-        }
-        if (pm > 1.0) rel2[0] = std::max(rel2[0], pm);          // a plane outside that bound fails the caller's gate
-      }
     }
   }
   tc_set_enabled(tc_prev ? 1 : 0);

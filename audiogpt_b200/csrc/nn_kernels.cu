@@ -11,7 +11,7 @@
 
 namespace agpt {
 
-// fp16 hi/lo operand-plane split of one value (tcconv7.cu consumes these planes through tensor maps)
+// fp16 hi/lo operand-plane split of one value (optional fp16 hi/lo output of the normalisation kernels)
 __device__ __forceinline__ void plane_split(float v, __half& hi, __half& lo) {
   hi = __float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f));
   lo = __float2half_rn(v - __half2float(hi));
@@ -258,40 +258,14 @@ __global__ void __launch_bounds__(128) attention_kernel(
 static int g_attn_tc = -1;
 void attention_set_tc(int on) { g_attn_tc = on; }
 bool attention_tc_enabled() {
-  if (g_attn_tc < 0) { const char* e = getenv("AGPT_ATTN_TC"); g_attn_tc = (e && e[0] == '0') ? 0 : ((e && e[0] == '2') ? 2 : 1); }
+  if (g_attn_tc < 0) { const char* e = getenv("AGPT_ATTN_TC"); g_attn_tc = (e && e[0] == '0') ? 0 : 1; }
   return g_attn_tc >= 1;
 }
 
 void attention(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st, __half* phi, __half* plo) {
-  if (g_attn_tc < 0) { const char* e = getenv("AGPT_ATTN_TC"); g_attn_tc = (e && e[0] == '0') ? 0 : ((e && e[0] == '2') ? 2 : 1); }
-  if (g_attn_tc == 2) {
-    // plane-fed kernel on fp32 inputs (test / A-B route; the UNet hands it the planes its projection GEMMs emit):
-    // split the three operands into fp16 hi/lo planes of the same pitch first
-    static DevBuf tmp[3];
-    const float* src[3] = {q, k, v};
-    const long cnt[3] = {(long)N * Lq * q_pitch, (long)N * Lk * k_pitch, (long)N * Lk * v_pitch};
-    __half* hi[3]; __half* lo[3];
-    bool ok = true;
-    for (int i = 0; i < 3; ++i) {
-      const long c8 = (cnt[i] + 7) & ~7L;
-      tmp[i].ensure((size_t)c8 + 16);            // 2 planes of c8 halves = c8 floats
-      hi[i] = reinterpret_cast<__half*>(tmp[i].p);
-      lo[i] = hi[i] + c8;
-      ok = ok && (reinterpret_cast<uintptr_t>(src[i]) & 15) == 0;
-    }
-    if (ok) {
-      // the last row may be shorter than its pitch (q / k / v views into one qkv tensor): stay inside the allocation
-      const long used[3] = {cnt[0] - q_pitch + heads * d, cnt[1] - k_pitch + heads * d, cnt[2] - v_pitch + heads * d};
-      for (int i = 0; i < 3; ++i) make_planes(src[i], hi[i], lo[i], used[i], PRO_NONE, 0.f, st);
-      if (attention_planes(hi[0], lo[0], q_pitch, hi[1], lo[1], k_pitch, hi[2], lo[2], v_pitch, o, o_pitch, N, heads, d,
-                           Lq, Lk, st, phi, plo))
-        return;
-    }
-  }
-  // tensor-core path (QK^T and PV on tcgen05, attention_tc.cu); the fp32 kernel below is the A/B reference
-  if (g_attn_tc >= 1 && attention_tc(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, d, Lq, Lk, st, phi, plo)) return;
-  AGPT_CHECK(!phi, "operand-plane output needs the tcgen05 attention kernel (o must be given for the fp32 kernel)");
+               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st) {
+  // tensor-core path (QK^T and PV on wgmma, attention_tc.cu); the fp32 kernel below is the A/B reference
+  if (attention_tc_enabled() && attention_tc(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, d, Lq, Lk, st)) return;
   const float scale = 1.0f / sqrtf((float)d);   // dim_head ** -0.5  (attention.py:158)
   dim3 grid(cdiv(Lq, 64), heads, N);
 #define AGPT_ATT(DH_) attention_kernel<DH_><<<grid, 128, 0, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, scale)
@@ -382,25 +356,6 @@ void softmax_rows(float* x, int pitch, long rows, int cols, float scale, cudaStr
   AGPT_CUDA(cudaGetLastError());
 }
 
-// ------------------------------------------------------------------ GEGLU gate (attention.py:37-48) on operand planes
-// in [rows][2*Cg] with (a, gate) channel pairs interleaved (pack_conv_pairs) -> planes of a * gelu_erf(gate) [rows][Cg]
-__global__ void geglu_planes_kernel(const float* __restrict__ in, __half* __restrict__ phi, __half* __restrict__ plo, long n_pairs2) {
-  pdl_wait();
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n_pairs2; i += (long)gridDim.x * blockDim.x) {
-    const float4 v = __ldg(reinterpret_cast<const float4*>(in) + i);     // (a0, g0, a1, g1)
-    const float o0 = v.x * gelu_erf(v.y), o1 = v.z * gelu_erf(v.w);
-    const __half2 hh = __floats2half2_rn(fminf(fmaxf(o0, -65504.f), 65504.f), fminf(fmaxf(o1, -65504.f), 65504.f));
-    const float2 hf = __half22float2(hh);
-    reinterpret_cast<__half2*>(phi)[i] = hh;
-    reinterpret_cast<__half2*>(plo)[i] = __floats2half2_rn(o0 - hf.x, o1 - hf.y);
-  }
-}
-void geglu_planes(const float* in, __half* phi, __half* plo, long rows, int Cg, cudaStream_t st) {
-  const long n = rows * Cg / 2;
-  launch_pdl(geglu_planes_kernel, dim3((unsigned)std::min<long>(cdivl(n, 256), 8192)), dim3(256), 0, st, in, phi, plo, n);
-  count_launch(1);
-  AGPT_CUDA(cudaGetLastError());
-}
 
 // ------------------------------------------------------------------ timestep embedding (cos || sin)
 struct TParam { int t[256]; };

@@ -14,22 +14,15 @@ size_t groupnorm_scratch_doubles(int N, int C);
 void layernorm(const float* x, float* y, const float* gamma, const float* beta, long rows, int C, float eps,
                cudaStream_t st, __half* phi = nullptr, __half* plo = nullptr);
 void attention(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st,
-               __half* phi = nullptr, __half* plo = nullptr);
+               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st);
 void transpose_pad(const float* in, int in_pitch, int rows, int cols, float* out, int rows_pad, cudaStream_t st);
 void copy_pad_rows(const float* in, int in_pitch, int rows, int cols, float* out, int rows_pad, cudaStream_t st);
 void softmax_rows(float* x, int pitch, long rows, int cols, float scale, cudaStream_t st);
-// tcgen05 version (attention_tc.cu); false = unsupported head dim / alignment
+// tensor-core version (attention_tc.cu); false = unsupported head dim / alignment
 bool attention_tc(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st,
-                  __half* phi = nullptr, __half* plo = nullptr);
-// plane-fed tcgen05 attention: q / k / v are fp16 hi/lo operand planes (pitches in elements)
-bool attention_planes(const __half* qh, const __half* ql, int q_pitch, const __half* kh, const __half* kl, int k_pitch,
-                      const __half* vh, const __half* vl, int v_pitch, float* o, int o_pitch, int N, int heads, int d,
-                      int Lq, int Lk, cudaStream_t st, __half* phi = nullptr, __half* plo = nullptr);
-void geglu_planes(const float* in, __half* phi, __half* plo, long rows, int Cg, cudaStream_t st);
+                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st);
 void attention_set_tc(int on);
-bool attention_tc_enabled();   // 1 (default) tcgen05, 2 tcgen05 through operand planes (fp32 inputs converted first), 0 fp32 kernel, -1 environment (AGPT_ATTN_TC)
+bool attention_tc_enabled();   // 1 (default) wgmma kernel, 0 fp32 kernel, -1 environment (AGPT_ATTN_TC)
 void timestep_embedding(float* out, const int* t_host, int N, int dim, cudaStream_t st);
 void concat_channels(const float* a, int Ca, const float* b, int Cb, float* out, long rows, cudaStream_t st);
 void upsample_nearest2(const float* in, float* out, int N, int H, int W, int C, cudaStream_t st);

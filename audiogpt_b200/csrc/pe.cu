@@ -1,9 +1,9 @@
-// PitchExtractor on sm_100a: mel [B][T][80] -> (pitch_pred [B][T][2], f0_denorm_pred [B][T]) -- the network that
+// PitchExtractor on sm_90a: mel [B][T][80] -> (pitch_pred [B][T][2], f0_denorm_pred [B][T]) -- the network that
 // recovers F0 from a generated mel-spectrogram for the NSF vocoder on the text-to-singing path.
 // Reference: NeuralSeq/modules/fastspeech/pe.py:119-148 (PitchExtractor), :7-42 (Prenet), :44-116 (ConvBlock /
 // ConvStacks), modules/fastspeech/tts_modules.py:217-260 (PitchPredictor), modules/commons/common_layers.py:87-142
 // (SinusoidalPositionalEmbedding), utils/__init__.py:145-157 (make_positions), utils/pitch_utils.py:63-76 (denorm_f0).
-// The mel is already channels-last; every Conv1d / Linear is a tap-GEMM on the tcgen05 kernels, BatchNorm1d (eval) is
+// The mel is already channels-last; every Conv1d / Linear is a tap-GEMM on the tensor-core kernel, BatchNorm1d (eval) is
 // a per-channel affine fused with the non-padding mask, GroupNorm + ReLU + residual is one gn_fused launch.
 // Parity: tests/test_pe_gpu.py against tests/golden/pe_{small,base}.npz (made by the reference module) and oracle/pe_ref.py.
 #include "common.cuh"

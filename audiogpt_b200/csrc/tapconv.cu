@@ -20,7 +20,7 @@ void profile_enable(int on) {
   }
 }
 
-// Sums over the records since profile_enable(1): per variant (FMA BN = 128, 64, 32; 3 = tcgen05)
+// Sums over the records since profile_enable(1): per variant (FMA BN = 128, 64, 32; 3 = wgmma)
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches) {
   for (int v = 0; v < 4; ++v) { ms[v] = 0; flops[v] = 0; bytes[v] = 0; launches[v] = 0; }
   AGPT_CUDA(cudaDeviceSynchronize());
@@ -258,8 +258,8 @@ void profile_end(void* r, cudaStream_t st) {
   if (r) AGPT_CUDA(cudaEventRecord(static_cast<ProfRec*>(r)->e1, st));
 }
 
-// Dispatch: tcgen05 version when the layer has a tensor-core weight image and the operands are
-// 16-byte addressable, else the fp32-FMA version.  Both are sm_100a CUDA; there is no other path.
+// Dispatch: tensor-core version when the layer has a tensor-core weight image and the operands are
+// 16-byte addressable, else the fp32-FMA version.  Both are sm_90a CUDA; there is no other path.
 void tapconv_launch(TapConvParams P, cudaStream_t st) {
   AGPT_CHECK(P.ntaps >= 1 && P.ntaps <= kMaxTaps, "ntaps");
   AGPT_CHECK(P.cin_pad % TC_KC == 0 && P.cout_pad % 4 == 0, "padding");

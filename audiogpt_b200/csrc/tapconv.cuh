@@ -97,16 +97,6 @@ __host__ __device__ inline int tc_row_out(const TapConvParams& P, int gz, int q,
   return j < P.Wreal ? h * P.Wreal + j : -1;
 }
 
-// Operand planes of the plane-fed kernel (tcconv7.cu): fp16 hi/lo parts of prologue(x), [G][L][C] each.
-struct PlaneIO {
-  const __half* in_hi; const __half* in_lo; long in_gstride; int in_pitch;       // operand planes of the input
-  __half* out_hi; __half* out_lo; long outp_gstride; int outp_pitch;             // planes to emit (nullptr: none)
-  int out_pro; float out_slope;                                                  // consumer prologue applied before the split
-  int store_f32;                                                                 // also store the fp32 result (residual / accumulator use)
-};
-bool tcconv7_launch(TapConvParams P, const PlaneIO& Q, cudaStream_t st);
-int tc_env_flags();      // AGPT_TC_DBGFLAGS experiment switches (bit 2 = 4: no stacked weight parts)
-void make_planes(const float* x, __half* hi, __half* lo, long n, int pro, float slope, cudaStream_t st);
 
 // ---------------------------------------------------------------- host side
 struct PackedConv {
@@ -130,17 +120,14 @@ inline int tc_pick_bn(int cout) {
 struct PackedConv;
 // Fill geometry-dependent fields (offsets, halo, smem rows) and launch (tapconv.cu).
 void tapconv_launch(TapConvParams P, cudaStream_t st);
-void tcconv_launch(TapConvParams P, cudaStream_t st);          // tcgen05 dispatcher (tcconv.cu)
+void tcconv_launch(TapConvParams P, cudaStream_t st);          // tensor-core dispatcher (tcconv.cu)
 bool tcconv5_launch(TapConvParams P, cudaStream_t st);
-bool tcconv6_launch(TapConvParams P, cudaStream_t st, bool force);
 struct HTile { int bn; const float* w; long ntiles; };
-HTile pick_h_tile(const TapConvParams& P, int sms, bool with96 = true, bool with256 = true);   // tile width for the fp16 kernels (tcconv5.cu): tcconv6 has no 96, tcconv7 no 256
+HTile pick_h_tile(const TapConvParams& P, int sms);   // tile width of the fp16 tensor-core kernel (tcconv5.cu)
 void pack_h_weights(struct PackedConv& pc, const std::vector<float>& h);
 bool tcconv_supported(const TapConvParams& P);
 void pack_tc_weights(struct PackedConv& pc, const std::vector<float>& h);
 void tc_set_enabled(int on);
-void tc_set_version(int v);
-int tc_get_version();
 bool tc_enabled();
 void profile_enable(int on);
 void* profile_begin(const TapConvParams& P, bool tc, double bytes_override, cudaStream_t st);
@@ -209,8 +196,8 @@ inline void pack_conv(PackedConv& pc, const float* w, const float* b, int Cout, 
 // Conv1d (dilation 1, "same" padding) on g CONSECUTIVE TIME STEPS AT ONCE: the [L][C] tensor is read as [L/g][g*C]
 // (the same memory), so a k-tap conv over C channels becomes a conv over g*C channels with block-Toeplitz weights
 //   W'[s][(i, ci)][(j, co)] = w[co][ci][g*s + i - j + c],   c = (k-1)/2,  s = floor((j + t - c) / g)
-// over super-taps s.  Narrow layers (C = 32 / 64) are bound by the NUMBER of tcgen05.mma instructions -- each one
-// re-reads its 128-row A slice whatever N is (profiles/r1e_findings.md) -- and this raises N per instruction from C to
+// over super-taps s.  Narrow layers (C = 32 / 64) are bound by the NUMBER of MMA instructions -- each one
+// re-reads its A slice from shared memory whatever N is -- and this raises N per instruction from C to
 // g*C = 128: k = 11, C = 32, g = 4 needs 5 super-taps x 8 k-steps per 512 time steps instead of 11 x 2 per 128
 // (2.2x fewer MMAs); the zero blocks of W' cost 1.45x the algorithmic MACs, which the tensor pipe has to spare.
 inline void pack_conv_grouped(PackedConv& pc, const float* w, const float* b, int C, int K, int g) {

@@ -1,7 +1,7 @@
-// Shared fused epilogue of the tapconv kernels (fp32 FMA version and tcgen05 versions):
+// Shared fused epilogue of the tapconv kernels (fp32 FMA version and tensor-core version):
 // one call handles 4 consecutive output channels of one output row.  Split in two phases so
 // that a kernel can issue the global READS of several items (residual, old accumulator) before
-// consuming any of them (memory-level parallelism in the tcgen05 epilogue).
+// consuming any of them (memory-level parallelism in the tensor-core epilogue).
 #pragma once
 #include "tapconv.cuh"
 

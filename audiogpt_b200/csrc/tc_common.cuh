@@ -1,13 +1,12 @@
-// PTX wrappers shared by the tcgen05 kernels (mbarrier, bulk/async copies, tcgen05 MMA/commit/fences,
-// UMMA shared-memory descriptors).  Encodings follow cute/arch/mma_sm100_desc.hpp (CUTLASS, vendored
-// headers in the image) and the PTX ISA; SASS shows UTCHMMA / UBLKCP / LDTM for these.
+// PTX wrappers shared by the tensor-core kernels (mbarrier, bulk/async copies, wgmma fences and shared-memory
+// matrix descriptors).  Encodings follow the PTX ISA; SASS shows HGMMA / UBLKCP for these.
 #pragma once
 #include "common.cuh"
 
 namespace agpt {
 namespace {
 
-constexpr int TC_ROWS = 128;      // UMMA_M
+constexpr int TC_ROWS = 128;      // output rows per tile: two warpgroups of wgmma M = 64
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -35,8 +34,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -78,19 +75,23 @@ __device__ __forceinline__ float4 ldg_stream(const float* p) {
   return v;
 }
 
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, sm_100):
+// warpgroup MMA (wgmma) ordering: fence before the first wgmma that reads / writes accumulator registers touched by
+// other instructions; commit closes a group of issued wgmmas; wait<N> blocks until at most N groups are pending
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (PTX ISA "matrix descriptor", sm_90):
 //   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (=1024B: 8 rows x 128B)
-//   [46,48) version=1 | [49,52) base_offset=0 | [61,64) layout=2 (SWIZZLE_128B)
+//   [49,52) base_offset=0 | [62,64) layout=1 (SWIZZLE_128B).  The swizzle is a function of the shared-memory address,
+//   so a start address shifted by whole 128-byte rows (a conv tap) or by 32 bytes (a k-step) addresses the same tile.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
 

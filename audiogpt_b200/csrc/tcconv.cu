@@ -1,18 +1,10 @@
-// Dispatcher of the tcgen05 tap-GEMM generations (the kernels live in tcconv5.cu / tcconv6.cu):
+// Dispatcher of the fp16 hi/lo tensor-core tap-GEMM (the kernel lives in tcconv5.cu):
 //
 //   out[g, p, co] = epi( bias[co] + sum_tap sum_ci pro(in[g, p + off_tap, ci]) * W[tap][ci][co] )
 //
 // Same TapConvParams contract (and the same fused prologue / epilogue table) as the fp32-FMA kernel in tapconv.cu;
-// the inner product runs as tcgen05.mma.kind::f16 on error-compensated fp16 hi/lo operand parts with the
-// accumulator tile [128 rows x BN cols] in tensor memory (header of tcconv5.cu).
-//
-//   tcconv6_kernel  persistent CTAs, dedicated transform / MMA / weight / epilogue warps, TMA epilogue: used
-//                   whenever a launch has more tiles than SMs (AGPT_TC_V=7: always)
-//   tcconv5_kernel  one tile per CTA, 8 worker warps (transform, then LSU epilogue): single-wave launches, 2-D
-//                   convs, gate / GEGLU / diff-out epilogues (AGPT_TC_V=5: always)
-//
-// Round 1's 3xTF32 generations (tcconv / tcconv2 / tcconv3) were measured baselines (profiles/r1b_*, r1c_*) and are
-// gone from the tree; `git show 33583de:audiogpt_b200/csrc/tcconv2.cu` has them.
+// the inner product runs as wgmma on error-compensated fp16 hi/lo operand parts with fp32 accumulation in registers
+// (header of tcconv5.cu): one [128 x BN] tile per CTA.
 #include "tapconv.cuh"
 #include "models.h"
 
@@ -23,14 +15,12 @@ void pack_tc_weights(PackedConv& pc, const std::vector<float>& h) {
   pack_h_weights(pc, h);   // fp16 hi/lo operand images (tcconv5.cu)
 }
 
-static int g_tc_version = -1;  // -1: AGPT_TC_V or the default
-void tc_set_version(int v) { g_tc_version = v; }
 static int g_tc_enabled = -1;   // -1: read AGPT_TENSOR_CORES from the environment on first use
 void tc_set_enabled(int on) { g_tc_enabled = on != 0 ? 1 : 0; }
 bool tc_enabled() {
   if (g_tc_enabled < 0) {
     const char* e = getenv("AGPT_TENSOR_CORES");
-    g_tc_enabled = (e && e[0] == '0') ? 0 : 1;   // default ON (validated on B200: tests/test_*_gpu.py)
+    g_tc_enabled = (e && e[0] == '0') ? 0 : 1;   // default ON (tests/test_*_gpu.py)
   }
   return g_tc_enabled == 1;
 }
@@ -42,34 +32,10 @@ bool tcconv_supported(const TapConvParams& P) {
   return true;
 }
 
-static int g_tc_flags_env = 0;
-int tc_get_version() {
-  int& ver = g_tc_version;
-  if (ver < 0) {
-    const char* e = getenv("AGPT_TC_V");
-    ver = e ? atoi(e) : 6;   // 6 (default): v6 where a CTA gets more than one tile, else v5; 5: v5 only; 7: v6 forced
-    if (ver < 5 || ver > 8) ver = 6;     // 8: dev / test selector of the plane-fed kernel in agpt_bench_tapconv (else = 6)
-  }
-  static bool env_done = false;
-  if (!env_done) {
-    env_done = true;
-    const char* d = getenv("AGPT_TC_DBGFLAGS");     // experiment switches (bits 2..)
-    if (d) g_tc_flags_env = atoi(d) & ~3;
-  }
-  return ver;
-}
-
-int tc_env_flags() {
-  tc_get_version();
-  return g_tc_flags_env;
-}
-
 void tcconv_launch(TapConvParams P, cudaStream_t st) {
-  const int ver = tc_get_version();
-  P.tc_flags = g_tc_flags_env | P.tc_flags_user;
-  if ((ver == 6 || ver == 7) && tcconv6_launch(P, st, ver == 7)) return;
+  P.tc_flags = P.tc_flags_user;
   if (tcconv5_launch(P, st)) return;
-  throw Error("tcconv: layer does not fit the shared-memory budget of the tcgen05 kernels (image too wide for the halo tile?)");
+  throw Error("tcconv: layer does not fit the shared-memory budget of the tensor-core kernel (image too wide for the halo tile?)");
 }
 
 }  // namespace agpt

@@ -1,12 +1,7 @@
-// tcconv v5: the v2 tap-GEMM with FP16 hi/lo operands (kind::f16) instead of TF32 hi/lo.
+// tcconv v5: the tap-GEMM on the Hopper tensor cores (wgmma) with error-compensated FP16 hi/lo operands.
 //
-// x = hi + lo with hi = fp16(x), lo = fp16(x - hi): both parts carry an 11-bit significand, exactly
-// like the TF32 split of v2, so the three products x_hi*w_hi + x_lo*w_hi + x_hi*w_lo accumulated
-// in fp32 (TMEM) have the same 2^-22 relative truncation error -- but an fp16 element is 2 bytes,
-// so one 128-byte swizzle row holds 64 channels and one tcgen05.mma (K = 16) does twice the
-// MACs of a tf32 one (K = 8) for the same shared-memory operand bytes.  The main loop of v2 is
-// bound by shared-memory operand bandwidth (profiles/r1b_conv_microbench.txt), so halving the number
-// of MMA instructions per channel halves its time.
+// x = hi + lo with hi = fp16(x), lo = fp16(x - hi): both parts carry an 11-bit significand, so the three
+// products x_hi*w_hi + x_lo*w_hi + x_hi*w_lo accumulated in fp32 have a 2^-22 relative truncation error.
 //
 // Range: fp16 is finite up to 65504.  WEIGHTS are pre-scaled per layer by a power of two so that
 // max|w| lands in [2^13, 2^14) (both parts stay normal numbers; the exact inverse scale is applied
@@ -14,9 +9,10 @@
 // the networks on this path stay orders of magnitude below); below 2^-14 the lo part becomes a
 // subnormal, i.e. the absolute representation error of an activation is max(2^-22 |x|, 2^-25).
 //
-// Everything else is v2: K-major SWIZZLE_128B tiles, a conv tap = a row-shifted descriptor start
-// address, 8 worker warps (transform, then epilogue), warp 4 = MMA issuer, warp 5 = weight producer
-// (cp.async.bulk), mbarrier full/empty rings.
+// One CTA = one [128 rows x BN] output tile.  K-major SWIZZLE_128B operand tiles, a conv tap = a row-shifted
+// descriptor start address.  Two worker warpgroups convert fp32 activations into the fp16 hi/lo tiles, then each
+// issues wgmma for its 64 rows with the accumulator in registers (one wgmma group in flight while the next chunk is
+// converted), then runs the fused epilogue; warp 8 streams the weights (cp.async.bulk, mbarrier full/empty ring).
 #include "tapconv.cuh"
 #include "tapconv_epi.cuh"
 #include "tc_common.cuh"
@@ -31,7 +27,7 @@ constexpr int MAX_NA = 4, MAX_NW = 8;
 constexpr int kMaxDyn = 227 * 1024 - 256;   // the kernel also has a small static __shared__ block
 
 struct Tc5Smem {
-  uint32_t a_hi[MAX_NA], a_lo[MAX_NA], w[MAX_NW], raw[2], rowinfo, rowp, bars, tmem_slot, total;
+  uint32_t a_hi[MAX_NA], a_lo[MAX_NA], w[MAX_NW], raw[2], rowinfo, rowp, bars, total;
 };
 __host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int RRA, int NA, int NW, int NR) {
   uint32_t o = 0;
@@ -42,25 +38,34 @@ __host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int RRA, int NA, 
   s.rowinfo = o; o += RRA * 4;
   s.rowp = o; o += TC_ROWS * 4;
   o = (o + 15) & ~15u;
-  s.bars = o; o += 32 * 8;
-  s.tmem_slot = o; o += 16;
+  s.bars = o; o += 2 * MAX_NW * 8;
   s.total = o;
 }
 
-constexpr int V5_THREADS = 320;   // 8 worker warps (0-3, 6-9) + warp 4 (MMA issuer) + warp 5 (weight producer)
+constexpr int V5_THREADS = 288;   // 8 worker warps = 2 warpgroups (transform, wgmma, epilogue) + warp 8 (weight producer)
+constexpr int NWK = 256;          // worker threads
 
-// TMEM allocations are powers of two >= 32 columns
-__host__ __device__ constexpr int tmem_cols(int bn) { return bn <= 32 ? 32 : (bn <= 64 ? 64 : (bn <= 128 ? 128 : 256)); }
-// Stacked weight parts (tiles up to 128 columns): the hi and lo blocks of a weight stage are contiguous rows of one
-// K-major tile, so ONE MMA of width 2 BN computes [A_hi W_hi | A_hi W_lo] into two column ranges of the accumulator
-// and a second of width BN adds A_lo W_hi to the first -- 2 instructions and 20 KB of operand reads per k-step
-// instead of 3 and 24 KB (the MMAs of these kernels are bound by the shared-memory operand fetch: measured
-// ~ (4 KB + 32 B x N) / 100 B per clock and MMA, profiles/r2j_*).  The epilogue adds the two ranges.
-__host__ __device__ constexpr bool tc5_stackable(int bn) { return bn <= 128; }
-__host__ __device__ constexpr int tc5_tmem(int bn) { return tc5_stackable(bn) ? tmem_cols(2 * bn) : tmem_cols(bn); }
+// wgmma width of a BN-column tile: 128 where it divides BN, else 64, else 32 (BN = 96)
+__host__ __device__ constexpr int tc5_nb(int bn) { return bn % 128 == 0 ? 128 : (bn % 64 == 0 ? 64 : 32); }
 
-template <int BN, int NWK>
-__global__ void __launch_bounds__(NWK == 256 ? V5_THREADS : 192, 1) tcconv5_kernel(const __grid_constant__ TapConvParams P) {
+template <int NB>
+__device__ __forceinline__ void wgmma_nb(float* d, uint64_t a, uint64_t b) {
+  if constexpr (NB == 128) wgmma_n128(d, a, b);
+  else if constexpr (NB == 64) wgmma_n64(d, a, b);
+  else wgmma_n32(d, a, b);
+}
+
+// compiler-only fence on the accumulator registers (no instruction): keeps other code from being moved across the
+// asynchronous wgmma that reads and writes them
+template <int N>
+__device__ __forceinline__ void fence_acc(float* a) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(a[i])::"memory");
+}
+
+template <int BN>
+__global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_constant__ TapConvParams P) {
+  constexpr int NB = tc5_nb(BN), NJ = BN / NB;
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
   const int RRA = P.R, NA = P.tc_na, NW = P.tc_nw, NR = P.tc_nr;
@@ -68,40 +73,29 @@ __global__ void __launch_bounds__(NWK == 256 ? V5_THREADS : 192, 1) tcconv5_kern
   if (threadIdx.x == 0) tc5_layout(S, BN, RRA, NA, NW, NR);
   __syncthreads();
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S.bars);
-  uint64_t* a_full = bars + 0;            // [MAX_NA]
-  uint64_t* a_empty = bars + MAX_NA;      // [MAX_NA]
-  uint64_t* w_full = bars + 2 * MAX_NA;   // [MAX_NW]
-  uint64_t* w_empty = w_full + MAX_NW;    // [MAX_NW]
-  uint64_t* acc_full = w_empty + MAX_NW;
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + S.tmem_slot);
+  uint64_t* w_full = bars;                // [MAX_NW]
+  uint64_t* w_empty = bars + MAX_NW;      // [MAX_NW]
   int* rowinfo = reinterpret_cast<int*>(smem + S.rowinfo);
   int* rowp = reinterpret_cast<int*>(smem + S.rowp);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const bool is_worker = warp < 4 || warp >= 6;
-  const int xt = warp < 4 ? tid : tid - 64;      // worker thread index 0..NWK-1
-  const int quad = warp & 3;                      // TMEM lane quadrant this warp may access
-  const int sub = warp < 4 ? 0 : 1;               // which of the two worker warps of that quadrant
+  // warpgroup index broadcast from lane 0: ptxas then sees the role branches as warpgroup-uniform, which keeps the
+  // wgmmas of the worker warpgroups asynchronous instead of serialized
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // workers: output rows 64 wg .. 64 wg + 63 of the tile
+  const bool is_worker = wg < 2;
+  const int xt = tid;                             // worker thread index 0..NWK-1
   const int gz = blockIdx.z, g = tc_sample(P, gz), co0 = blockIdx.y * BN, q0 = blockIdx.x * TC_ROWS;
   const int Wv = tc_wv(P);
   const int Lv = tc_lv(P);
   const int nchunks = P.tc_chunks_h, ntaps = P.ntaps, total = nchunks * ntaps;
   const int lo = P.lo_al;
   const bool dbg_on = (P.tc_flags & 2) && P.dbg;
-  const bool stk = tc5_stackable(BN) && !(P.tc_flags & 4);
   long long* dbg = dbg_on ? P.dbg + 8 * ((long)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
   if (dbg_on && tid == 0) dbg[0] = clock64();
 
   if (tid == 0) {
-    for (int i = 0; i < NA; ++i) { mbar_init(&a_full[i], NWK); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 1); }
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NWK / 32); }
     fence_barrier_init();
-  }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(smem_u32((const void*)tmem_slot)), "r"((uint32_t)tc5_tmem(BN)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   if (is_worker) {
     for (int i = xt; i < RRA; i += NWK) {
@@ -110,10 +104,7 @@ __global__ void __launch_bounds__(NWK == 256 ? V5_THREADS : 192, 1) tcconv5_kern
     }
     if (xt < TC_ROWS) rowp[xt] = tc_row_out(P, gz, q0 + xt, Wv, Lv);   // output row -> real position (or -1)
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();          // everything above overlaps the previous kernel's tail
   if (dbg_on && tid == 0) dbg[1] = clock64();
 
@@ -157,17 +148,27 @@ __global__ void __launch_bounds__(NWK == 256 ? V5_THREADS : 192, 1) tcconv5_kern
         }
       }
     }
+    // this warpgroup's accumulator: rows 64 wg .. 64 wg + 63, BN columns in NJ blocks of NB (wgmma fragment layout)
+    float acc[NJ][NB / 2];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+      for (int i = 0; i < NB / 2; ++i) acc[j][i] = 0.f;
     const int items = RRA * 8;
+    int it = 0, prev = -1;     // prev: weight stage of the newest wgmma group, released once that group has completed
     for (int c = 0; c < nchunks; ++c) {
-      const int buf = c % NA, n = c / NA;
+      const int buf = c % NA;
       const int rb = (NR == 2) ? (c & 1) : 0;
       const int kv = min(H_KCH, P.Cin - c * H_KCH);
       const int nq = ((kv + 15) >> 4) << 1;                 // 16-byte fp16 chunks (8 channels) the k-steps touch
+      const int ksteps = (kv + 15) >> 4;
       // raw(c) landed?  (with NR == 2 one younger group -- raw(c+1) -- may still be in flight)
       if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
       else cp_async_wait_all_();
+      // past this barrier raw(c) is visible to every worker, and the wgmmas that last read a_*[buf] (chunk c - NA) have
+      // completed in both warpgroups: each warpgroup keeps at most one wgmma group in flight, and none across a chunk
+      // boundary when NA == 1
       named_bar_sync(1, NWK);
-      if (n >= 1) mbar_wait(&a_empty[buf], (uint32_t)((n - 1) & 1));
       uint8_t* ahi = smem + S.a_hi[buf];
       uint8_t* alo = smem + S.a_lo[buf];
       const uint8_t* rawb = smem + S.raw[rb];
@@ -190,24 +191,52 @@ __global__ void __launch_bounds__(NWK == 256 ? V5_THREADS : 192, 1) tcconv5_kern
         *reinterpret_cast<uint4*>(ahi + o) = h;
         *reinterpret_cast<uint4*>(alo + o) = l;
       }
-      fence_proxy_async();
-      mbar_arrive(&a_full[buf]);
-      // refill the raw buffer just consumed
+      fence_proxy_async();               // generic-proxy stores -> visible to wgmma operand reads
+      named_bar_sync(1, NWK);            // a_*[buf] complete; everyone finished reading raw[rb]
       const int cn = c + NR;
-      if (cn < nchunks) {
-        named_bar_sync(1, NWK);          // everyone finished reading raw[rb]
-        issue_raw(cn, rb);
+      if (cn < nchunks) issue_raw(cn, rb);
+      // =========================== worker warps: wgmma over the taps of chunk c ===========================
+      // products x_hi w_hi + x_lo w_hi + x_hi w_lo into one fp32 accumulator; a tap is a start address shifted by rows
+      const uint32_t ahi0 = smem_u32(ahi) + (uint32_t)(wg * 64 - lo) * 128u, alo0 = smem_u32(alo) + (uint32_t)(wg * 64 - lo) * 128u;
+      for (int t = 0; t < ntaps; ++t, ++it) {
+        const int s = it % NW;
+        mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
+        const uint32_t shift = (uint32_t)P.tap_off[t] * 128u;
+        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
+        const uint32_t ws = smem_u32(smem + S.w[s]);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        wgmma_fence();
+        for (int k = 0; k < ksteps; ++k) {
+          const uint64_t ko = (uint64_t)((k * 32) >> 4);
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) {
+            const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
+            wgmma_nb<NB>(acc[j], dah + ko, dwh);
+            wgmma_nb<NB>(acc[j], dal + ko, dwh);
+            wgmma_nb<NB>(acc[j], dah + ko, dwl);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        prev = s;
+      }
+      if (NA == 1) {
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&w_empty[prev]);
+        prev = -1;
       }
     }
     // =========================== worker warps: epilogue ===========================
-    // TMEM -> registers (x inverse weight scale) -> swizzled staging block [128 rows][32 cols] in shared
-    // memory (the operand buffers are free now) -> coalesced (row, 16-byte chunk) items through the
-    // fused epilogue.  Each TMEM lane quadrant has two worker warps; they alternate over the
-    // 32-column blocks.  The global READS of a block (residual / old accumulator) are issued one
-    // block ahead -- for block 0 before the accumulator is complete.
+    // registers (x inverse weight scale) -> swizzled staging block [128 rows][32 cols] in shared memory (the operand
+    // buffers are free now) -> coalesced (row, 16-byte chunk) items through the fused epilogue.  The global READS of a
+    // block (residual / old accumulator) are issued one block ahead -- for block 0 before the accumulator is complete.
     EpiPre pre[8];
     int pp[8];
-    constexpr int nitem = (TC_ROWS * 8) / NWK;   // 4 or 8 items per worker and block
+    constexpr int nitem = (TC_ROWS * 8) / NWK;   // 4 items per worker and block
     const float dsc = P.tc_descale;
     auto load_block = [&](int cb) {
 #pragma unroll
@@ -218,47 +247,25 @@ __global__ void __launch_bounds__(NWK == 256 ? V5_THREADS : 192, 1) tcconv5_kern
       }
     };
     load_block(0);
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
+    if (dbg_on && tid == 0) { dbg[2] = dbg[1]; dbg[3] = clock64(); dbg[6] = 0; dbg[7] = 0; }   // the workers issue the wgmmas: no waits of a separate issuer
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+    named_bar_sync(1, NWK);                      // both warpgroups' wgmmas are done reading the operand buffers
     if (dbg_on && tid == 0) dbg[4] = clock64();
     uint8_t* stg0 = smem + S.a_hi[0];            // 2 x 16 KB inside the first operand buffers (>= 32 KB)
-    const int myrow = quad * 32 + lane;
-#pragma unroll 1
-    for (int cb = 0, blk = 0; cb < BN; cb += 32, ++blk) {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int blk = 0; blk < BN / 32; ++blk) {
+      const int cb = blk * 32;
       uint8_t* stg = stg0 + (blk & 1) * (TC_ROWS * 128);
-      if (NWK == 128 || sub == (blk & 1)) {
-        uint32_t rg[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)cb;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(rg[0]), "=r"(rg[1]), "=r"(rg[2]), "=r"(rg[3]), "=r"(rg[4]), "=r"(rg[5]), "=r"(rg[6]), "=r"(rg[7]),
-              "=r"(rg[8]), "=r"(rg[9]), "=r"(rg[10]), "=r"(rg[11]), "=r"(rg[12]), "=r"(rg[13]), "=r"(rg[14]), "=r"(rg[15]),
-              "=r"(rg[16]), "=r"(rg[17]), "=r"(rg[18]), "=r"(rg[19]), "=r"(rg[20]), "=r"(rg[21]), "=r"(rg[22]), "=r"(rg[23]),
-              "=r"(rg[24]), "=r"(rg[25]), "=r"(rg[26]), "=r"(rg[27]), "=r"(rg[28]), "=r"(rg[29]), "=r"(rg[30]), "=r"(rg[31])
-            : "r"(taddr) : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (stk) {       // + the A_hi W_lo range
-          uint32_t r2[32];
-          asm volatile(
-              "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-              "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-              "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-              : "=r"(r2[0]), "=r"(r2[1]), "=r"(r2[2]), "=r"(r2[3]), "=r"(r2[4]), "=r"(r2[5]), "=r"(r2[6]), "=r"(r2[7]),
-                "=r"(r2[8]), "=r"(r2[9]), "=r"(r2[10]), "=r"(r2[11]), "=r"(r2[12]), "=r"(r2[13]), "=r"(r2[14]), "=r"(r2[15]),
-                "=r"(r2[16]), "=r"(r2[17]), "=r"(r2[18]), "=r"(r2[19]), "=r"(r2[20]), "=r"(r2[21]), "=r"(r2[22]), "=r"(r2[23]),
-                "=r"(r2[24]), "=r"(r2[25]), "=r"(r2[26]), "=r"(r2[27]), "=r"(r2[28]), "=r"(r2[29]), "=r"(r2[30]), "=r"(r2[31])
-              : "r"(taddr + (uint32_t)BN) : "memory");
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      const float* a = &acc[cb / NB][4 * ((cb % NB) / 8)];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) rg[i] = __float_as_uint(__uint_as_float(rg[i]) + __uint_as_float(r2[i]));
-        }
-#pragma unroll
-        for (int qd = 0; qd < 8; ++qd)
-          *reinterpret_cast<float4*>(stg + sw128(myrow, qd)) =
-              make_float4(__uint_as_float(rg[4 * qd]) * dsc, __uint_as_float(rg[4 * qd + 1]) * dsc,
-                          __uint_as_float(rg[4 * qd + 2]) * dsc, __uint_as_float(rg[4 * qd + 3]) * dsc);
+      for (int i8 = 0; i8 < 4; ++i8) {
+        const int col = 8 * i8 + c0;
+        *reinterpret_cast<float2*>(stg + sw128(r0, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
+        *reinterpret_cast<float2*>(stg + sw128(r0 + 8, col >> 2) + (col & 3) * 4) =
+            make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
       }
       named_bar_sync(1, NWK);
       const int jc = xt & 7;                       // all items of this thread share the 4-channel group
@@ -275,76 +282,16 @@ __global__ void __launch_bounds__(NWK == 256 ? V5_THREADS : 192, 1) tcconv5_kern
       // barrier, so no extra barrier is needed here
     }
     if (dbg_on && tid == 0) dbg[5] = clock64();
-  } else if (warp == 4) {
-    // =========================== MMA issuer ===========================
-    // the whole warp runs the loop (converged waits); one ELECTED lane issues, so that ptxas keeps the
-    // descriptors in uniform registers instead of a per-MMA divergence "waterfall"
-    {
-      // kind::f16: D = F32 (bit 4), A = B = F16 (format 0), both K-major, N >> 3 at [17,23), M >> 4 at [24,29)
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_ROWS >> 4) << 24);
-      const uint32_t idesc2 = (1u << 4) | ((uint32_t)((2 * BN > 256 ? BN : 2 * BN) >> 3) << 17) | ((uint32_t)(TC_ROWS >> 4) << 24);
-      long long dbg_wa = 0, dbg_ww = 0;
-      int it = 0;
-      for (int c = 0; c < nchunks; ++c) {
-        const int buf = c % NA;
-        const int kv = min(H_KCH, P.Cin - c * H_KCH);
-        const int ksteps = (kv + 15) >> 4;
-        long long tw0 = dbg_on ? clock64() : 0;
-        mbar_wait(&a_full[buf], (uint32_t)((c / NA) & 1));
-        tc_fence_after();
-        if (dbg_on) { const long long t1 = clock64(); if (c == 0 && lane == 0) dbg[2] = t1; dbg_wa += t1 - tw0; }
-        const uint32_t ahi0 = smem_u32(smem + S.a_hi[buf]), alo0 = smem_u32(smem + S.a_lo[buf]);
-        for (int t = 0; t < ntaps; ++t, ++it) {
-          const int s = it % NW;
-          tw0 = dbg_on ? clock64() : 0;
-          mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
-          tc_fence_after();
-          if (dbg_on) dbg_ww += clock64() - tw0;
-          const uint32_t shift = (uint32_t)(P.tap_off[t] - lo) * 128u;
-          const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
-          const uint64_t dwh = make_desc(smem_u32(smem + S.w[s]));
-          const uint64_t dwl = make_desc(smem_u32(smem + S.w[s] + BN * 128));
-          if (elect_one()) {
-            for (int k = 0; k < ksteps; ++k) {
-              const uint64_t ko = (uint64_t)((k * 32) >> 4);
-              if (stk) {
-                umma_f16(tmem_base, dah + ko, dwh + ko, idesc2, (it > 0 || k > 0) ? 1u : 0u);   // [hi x hi | hi x lo]
-                umma_f16(tmem_base, dal + ko, dwh + ko, idesc, 1u);                              // += lo x hi
-              } else {
-                umma_f16(tmem_base, dah + ko, dwh + ko, idesc, (it > 0 || k > 0) ? 1u : 0u);
-                umma_f16(tmem_base, dal + ko, dwh + ko, idesc, 1u);
-                umma_f16(tmem_base, dah + ko, dwl + ko, idesc, 1u);
-              }
-            }
-            umma_commit(&w_empty[s]);
-            if (t == ntaps - 1) {
-              umma_commit(&a_empty[buf]);
-              if (c == nchunks - 1) umma_commit(acc_full);
-            }
-          }
-          __syncwarp();
-        }
-      }
-      if (dbg_on && lane == 0) { dbg[3] = clock64(); dbg[6] = dbg_wa; dbg[7] = dbg_ww; }
+  } else if (lane == 0) {
+    // =========================== weight producer (warp 8) ===========================
+    const uint32_t bytes = 2u * BN * 128u;
+    const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(P.w_h) + (size_t)blockIdx.y * (size_t)total * bytes;
+    for (int it = 0; it < total; ++it) {
+      const int s = it % NW, n = it / NW;
+      if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
+      mbar_arrive_expect_tx(&w_full[s], bytes);
+      bulk_g2s(smem + S.w[s], wsrc + (size_t)it * bytes, bytes, &w_full[s]);
     }
-  } else if (warp == 5) {
-    // =========================== weight producer ===========================
-    if (lane == 0) {
-      const uint32_t bytes = 2u * BN * 128u;
-      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(P.w_h) + (size_t)blockIdx.y * (size_t)total * bytes;
-      for (int it = 0; it < total; ++it) {
-        const int s = it % NW, n = it / NW;
-        if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
-        mbar_arrive_expect_tx(&w_full[s], bytes);
-        bulk_g2s(smem + S.w[s], wsrc + (size_t)it * bytes, bytes, &w_full[s]);
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tc5_tmem(BN)) : "memory");
   }
 }
 
@@ -392,7 +339,6 @@ void pack_h_weights(PackedConv& pc, const std::vector<float>& h) {
   pc.h_descale = 1.f / wscale;
   pc.h_chunks = cdiv(pc.Cin, H_KCH);
   build_h_image(pc, h, pc.tc_bn, wscale, pc.w_h);
-  if (pc.Cout % 256 == 0) build_h_image(pc, h, 256, wscale, pc.w_h256);
   if (pc.tc_bn == 128) build_h_image(pc, h, 64, wscale, pc.w_h64);   // narrower tiles for launches that would not fill the SMs
   if (pc.tc_bn == 128 && pc.Cout > 128) build_h_image(pc, h, 96, wscale, pc.w_h96);
 }
@@ -422,9 +368,6 @@ static bool tcconv5_try(TapConvParams P, int BN, cudaStream_t st) {
   int NW = (int)std::min<long>(MAX_NW, (avail - NA * abytes - NR * rbytes) / wbytes);
   NW = std::max(2, std::min(NW, std::max(2, iters)));
   P.tc_na = NA; P.tc_nw = NW; P.tc_nr = NR;
-  // tiny tiles (BN=32, <= 3 taps, one chunk) are launch/teardown bound: 4 worker warps are enough
-  P.tc_nwk = (BN <= 32 && iters <= 4) ? 128 : 256;
-  const int nthreads = P.tc_nwk == 128 ? 192 : V5_THREADS;
   Tc5Smem S;
   tc5_layout(S, BN, RRA, NA, NW, NR);
   const size_t smem = (size_t)S.total + 1024;
@@ -435,34 +378,28 @@ static bool tcconv5_try(TapConvParams P, int BN, cudaStream_t st) {
   AGPT_CUDA(cudaGetDevice(&dev));
   static bool attr_done_dev[64] = {false};
   if (!attr_done_dev[dev & 63]) {
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<256, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<128, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<96, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32, 128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
     attr_done_dev[dev & 63] = true;
   }
-  if (BN == 256) launch_pdl(tcconv5_kernel<256, 256>, grid, dim3(nthreads), smem, st, P);
-  else if (BN == 128) launch_pdl(tcconv5_kernel<128, 256>, grid, dim3(nthreads), smem, st, P);
-  else if (BN == 96) launch_pdl(tcconv5_kernel<96, 256>, grid, dim3(nthreads), smem, st, P);
-  else if (BN == 64) launch_pdl(tcconv5_kernel<64, 256>, grid, dim3(nthreads), smem, st, P);
-  else if (P.tc_nwk == 128) launch_pdl(tcconv5_kernel<32, 128>, grid, dim3(nthreads), smem, st, P);
-  else launch_pdl(tcconv5_kernel<32, 256>, grid, dim3(nthreads), smem, st, P);
+  if (BN == 128) launch_pdl(tcconv5_kernel<128>, grid, dim3(V5_THREADS), smem, st, P);
+  else if (BN == 96) launch_pdl(tcconv5_kernel<96>, grid, dim3(V5_THREADS), smem, st, P);
+  else if (BN == 64) launch_pdl(tcconv5_kernel<64>, grid, dim3(V5_THREADS), smem, st, P);
+  else launch_pdl(tcconv5_kernel<32>, grid, dim3(V5_THREADS), smem, st, P);
   return true;
 }
 
-// Tile width: the candidate (256 / native 128|64|32 / 96 and 64 for native-128 layers) with the smallest
-// waves x per-tile cost, where waves = ceil(tiles / SMs).  Per-tile cost relative to BN = 128 from the
-// micro-benchmarks (profiles/r1e_*): wider tiles amortise the activation operand, narrower ones fill the SMs.
-HTile pick_h_tile(const TapConvParams& P, int sms, bool with96, bool with256) {
-  static int allow256 = -1;
-  if (allow256 < 0) { const char* e = getenv("AGPT_TC_BN256"); allow256 = (e && e[0] == '0') ? 0 : 1; }
+// Tile width: the candidate (native 128|64|32, or 96 and 64 for native-128 layers) with the smallest waves x per-tile
+// cost, where waves = ceil(tiles / SMs): wider tiles amortise the activation operand, narrower ones fill the SMs.  No
+// 256-wide tile: its accumulator (128 registers per thread of a warpgroup) spills next to the transform's registers.
+HTile pick_h_tile(const TapConvParams& P, int sms) {
   const int Lv = tc_lv(P);
   const long rt = (long)cdiv(Lv, TC_ROWS) * tc_groups(P);
   static int allow96 = -1;
   if (allow96 < 0) { const char* e = getenv("AGPT_TC_BN96"); allow96 = (e && e[0] == '0') ? 0 : 1; }
-  auto cost = [](int bn) { return bn == 256 ? 1.7 : (bn == 128 ? 1.0 : (bn == 96 ? 0.82 : (bn == 64 ? 0.62 : 0.45))); };
+  auto cost = [](int bn) { return bn == 128 ? 1.0 : (bn == 96 ? 0.82 : (bn == 64 ? 0.62 : 0.45)); };
   HTile best{P.tc_bn, P.w_h, rt * cdiv(P.Cout, P.tc_bn)};
   double bs = (double)cdiv(best.ntiles, (long)sms) * cost(P.tc_bn);
   auto consider = [&](int bn, const float* w) {
@@ -471,9 +408,8 @@ HTile pick_h_tile(const TapConvParams& P, int sms, bool with96, bool with256) {
     const double sc = (double)cdiv(nt, (long)sms) * cost(bn);
     if (sc < bs - 1e-9) { bs = sc; best = HTile{bn, w, nt}; }
   };
-  if (allow256 && with256) consider(256, P.w_h256);
   if (P.tc_bn == 128) consider(64, P.w_h64);
-  if (P.tc_bn == 128 && allow96 && with96) consider(96, P.w_h96);   // e.g. 640 channels on 16 row tiles: 112 tiles in one wave
+  if (P.tc_bn == 128 && allow96) consider(96, P.w_h96);   // e.g. 640 channels on 16 row tiles: 112 tiles in one wave
   return best;
 }
 

@@ -1,4 +1,4 @@
-// Make-An-Audio UNet (ResBlock + SpatialTransformer) and the DDIM loop on sm_100a.
+// Make-An-Audio UNet (ResBlock + SpatialTransformer) and the DDIM loop on sm_90a.
 // Reference: ldm/modules/diffusionmodules/openaimodel.py:443-744 (ctor + forward),
 //            :255-275 (ResBlock._forward), :91-160 (Up/Downsample);
 //            ldm/modules/attention.py:37-64,152-261; ldm/models/diffusion/ddim.py:117-225.
@@ -55,8 +55,7 @@ struct Unet : Handle {
 
   // per-call state
   int ctxN = 0, ctxS = 0;
-  DevBuf ctx_kv, ctx_kv_pl;     // hoisted cross-attention K / V of the context: fp32 and fp16 hi/lo planes
-  __half* ctx_hi = nullptr; __half* ctx_lo = nullptr;
+  DevBuf ctx_kv;                // hoisted cross-attention K / V of the context
   DevBuf arena;
   size_t arena_off = 0, arena_cap = 0;
   DevBuf ddim_eps, ddim_x, ddim_p0;
@@ -89,14 +88,6 @@ struct Unet : Handle {
     P.out = ctx_kv.p; P.out_gstride = 0; P.out_pitch = kv_total;
     P.epi = EPI_BIAS;
     tapconv_launch(P, s);
-    ctx_hi = ctx_lo = nullptr;
-    if (kv_total % 8 == 0) {     // operand planes for the plane-fed attention kernel
-      const size_t n = (size_t)N * S * kv_total, n8 = (n + 7) & ~(size_t)7;
-      ctx_kv_pl.ensure(n8 + 16);
-      ctx_hi = reinterpret_cast<__half*>(ctx_kv_pl.p);
-      ctx_lo = ctx_hi + n8;
-      make_planes(ctx_kv.p, ctx_hi, ctx_lo, (long)n, PRO_NONE, 0.f, s);
-    }
   }
 
   // ---- building blocks --------------------------------------------------------------
@@ -139,125 +130,7 @@ struct Unet : Handle {
     return out;
   }
 
-  // ---- operand planes inside the transformer blocks: LayerNorm / GroupNorm / attention / the GEGLU epilogue write
-  // their outputs as fp16 hi/lo planes and the 1-tap GEMMs that consume them run on the plane-fed kernel
-  // (tcconv7.cu: TMA -> tcgen05, deep operand ring, TMA epilogue) instead of tcconv5's load-convert chain, which
-  // was latency-bound on these small-M GEMMs (35-55 TFLOP/s on the 1 560-row level, profiles/r2a_layers_unet.txt).
-  struct Planes { __half* hi; __half* lo; };
-  Planes alloc_planes(size_t elems) {
-    __half* h = reinterpret_cast<__half*>(alloc(elems + 16));
-    return Planes{h, h + ((elems + 7) & ~(size_t)7)};
-  }
-  static bool planes_enabled() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("AGPT_UNET_PLANES"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v == 1 && tc_enabled() && tc_get_version() >= 6 && attention_tc_enabled();   // the plane path's attention writes planes: tcgen05 kernels only
-  }
-  // out [rows][Cout] = planes [rows][Cin] x W (+ bias, + residual); optionally also planes of the result
-  bool linear_planes(const PackedConv& pc, Planes in, int in_pitch, float* out, int out_pitch, long rows, int epi,
-                     const float* res_, int res_pitch, Planes* outp, cudaStream_t s) {
-    TapConvParams P = tapconv_params(pc, 1, (int)rows, 0, 1);
-    P.in = nullptr; P.in_pitch = in_pitch;
-    P.out = out; P.out_pitch = out_pitch; P.out_gstride = rows * out_pitch;
-    P.epi = epi; P.pro = PRO_NONE;
-    P.res = res_; P.res_pitch = res_pitch; P.res_gstride = rows * res_pitch;
-    PlaneIO Q;
-    memset(&Q, 0, sizeof(Q));
-    Q.in_hi = in.hi; Q.in_lo = in.lo; Q.in_pitch = in_pitch; Q.in_gstride = rows * in_pitch;
-    if (outp) { Q.out_hi = outp->hi; Q.out_lo = outp->lo; Q.outp_pitch = out_pitch; Q.outp_gstride = rows * out_pitch; }
-    Q.out_pro = PRO_NONE; Q.store_f32 = out ? 1 : 0;
-    const double r = (double)rows;
-    void* rec = profile_begin(P, true, 4.0 * (r * pc.Cin + r * pc.Cout * ((out ? 1 : 0) + (outp ? 1 : 0) + (res_ ? 1 : 0)) + (double)pc.Cin * pc.Cout), s);
-    if (!tcconv7_launch(P, Q, s)) return false;
-    profile_end(rec, s);
-    count_launch(1);
-    AGPT_CUDA(cudaGetLastError());
-    return true;
-  }
-
-  float* run_st_planes(const StW& t, const float* x, int N, int H, int W, cudaStream_t s) {
-    const int HW = H * W;
-    const long rows = (long)N * HW;
-    const int C = t.inner;
-    Planes pa = alloc_planes(rows * std::max(C, t.ch));       // LayerNorm / GroupNorm output
-    Planes pt = alloc_planes(rows * C);                       // attention output
-    Planes pf = alloc_planes(rows * 4 * C);                   // GEGLU output
-    Planes ph = alloc_planes(rows * C);                       // planes of the block output (proj_out's operand)
-    groupnorm(x, nullptr, t.gn_g.p, t.gn_b.p, N, HW, t.ch, 32, 1e-6f, false, nullptr, s, pa.hi, pa.lo);
-    float* h = alloc(rows * C);
-    AGPT_CHECK(linear_planes(t.proj_in, pa, t.ch, h, C, rows, EPI_BIAS, nullptr, 0, nullptr, s), "plane-fed GEMM rejected proj_in");
-    float* a = alloc(rows * C);
-    float* qkv = alloc(rows * 3 * C);
-    float* ff8 = alloc(rows * 8 * C);
-    static int attn_pl = -1;
-    if (attn_pl < 0) { const char* e = getenv("AGPT_ATTN_PL"); attn_pl = (e && e[0] == '0') ? 0 : 1; }
-    const bool apl = attn_pl && attention_tc_enabled() && ctx_hi && t.dhead % 8 == 0 && C % 8 == 0 &&
-                     (t.dhead == 8 || t.dhead == 16 || t.dhead == 32 || t.dhead == 40 || t.dhead == 64 || t.dhead == 80);
-    Planes pq = apl ? alloc_planes(rows * 3 * C) : Planes{nullptr, nullptr};     // q | k | v planes of the projection GEMMs
-    for (size_t bi = 0; bi < t.blocks.size(); ++bi) {
-      const XfBlockW& b = t.blocks[bi];
-      const bool last = bi + 1 == t.blocks.size();
-      layernorm(h, nullptr, b.ln1_g.p, b.ln1_b.p, rows, C, 1e-5f, s, pa.hi, pa.lo);
-      if (apl) {     // q, k, v leave the projection GEMM as operand planes; the attention kernel copies them into its tiles
-        AGPT_CHECK(linear_planes(b.qkv1, pa, C, nullptr, 3 * C, rows, EPI_BIAS, nullptr, 0, &pq, s), "plane-fed GEMM rejected qkv");
-        AGPT_CHECK(attention_planes(pq.hi, pq.lo, 3 * C, pq.hi + C, pq.lo + C, 3 * C, pq.hi + 2 * C, pq.lo + 2 * C, 3 * C, nullptr, C,
-                                    N, t.heads, t.dhead, HW, HW, s, pt.hi, pt.lo), "plane-fed attention rejected the self-attention");
-      } else {
-        AGPT_CHECK(linear_planes(b.qkv1, pa, C, qkv, 3 * C, rows, EPI_BIAS, nullptr, 0, nullptr, s), "plane-fed GEMM rejected qkv");
-        attention(qkv, 3 * C, qkv + C, 3 * C, qkv + 2 * C, 3 * C, nullptr, C, N, t.heads, t.dhead, HW, HW, s, pt.hi, pt.lo);
-      }
-      float* h2 = alloc(rows * C);
-      AGPT_CHECK(linear_planes(b.out1, pt, C, h2, C, rows, EPI_RES, h, C, nullptr, s), "plane-fed GEMM rejected attn1.to_out");
-      AGPT_CHECK(ctxN == N, "context batch (agpt_unet_set_context) differs from the UNet batch");
-      layernorm(h2, nullptr, b.ln2_g.p, b.ln2_b.p, rows, C, 1e-5f, s, pa.hi, pa.lo);
-      if (apl) {
-        AGPT_CHECK(linear_planes(b.q2, pa, C, nullptr, C, rows, EPI_BIAS, nullptr, 0, &pq, s), "plane-fed GEMM rejected attn2.to_q");
-        AGPT_CHECK(attention_planes(pq.hi, pq.lo, C, ctx_hi + b.kv_off, ctx_lo + b.kv_off, kv_total, ctx_hi + b.kv_off + C,
-                                    ctx_lo + b.kv_off + C, kv_total, nullptr, C, N, t.heads, t.dhead, HW, ctxS, s, pt.hi, pt.lo),
-                   "plane-fed attention rejected the cross-attention");
-      } else {
-        AGPT_CHECK(linear_planes(b.q2, pa, C, qkv, C, rows, EPI_BIAS, nullptr, 0, nullptr, s), "plane-fed GEMM rejected attn2.to_q");
-        attention(qkv, C, ctx_kv.p + b.kv_off, kv_total, ctx_kv.p + b.kv_off + C, kv_total, nullptr, C, N, t.heads, t.dhead,
-                  HW, ctxS, s, pt.hi, pt.lo);
-      }
-      float* h3 = alloc(rows * C);
-      AGPT_CHECK(linear_planes(b.out2, pt, C, h3, C, rows, EPI_RES, h2, C, nullptr, s), "plane-fed GEMM rejected attn2.to_out");
-      // GEGLU feed-forward (attention.py:37-64): ff1 on the plane-fed kernel writes the (a, gate) pairs in fp32, one
-      // light pass turns them into the planes of a * gelu(gate) that ff2 consumes (AGPT_GEGLU_TC5=1: round-1 path,
-      // the gate fused in the one-tile-per-CTA kernel's epilogue)
-      static int geglu_tc5 = -1;
-      if (geglu_tc5 < 0) { const char* e = getenv("AGPT_GEGLU_TC5"); geglu_tc5 = (e && e[0] == '1') ? 1 : 0; }
-      if (!geglu_tc5) {
-        layernorm(h3, nullptr, b.ln3_g.p, b.ln3_b.p, rows, C, 1e-5f, s, pa.hi, pa.lo);
-        AGPT_CHECK(linear_planes(b.ff1, pa, C, ff8, 8 * C, rows, EPI_BIAS, nullptr, 0, nullptr, s), "plane-fed GEMM rejected ff.net.0.proj");
-        geglu_planes(ff8, pf.hi, pf.lo, rows, 4 * C, s);
-      } else {
-        layernorm(h3, a, b.ln3_g.p, b.ln3_b.p, rows, C, 1e-5f, s);
-        TapConvParams P = tapconv_params(b.ff1, 1, (int)rows, 0, 1);
-        P.in = a; P.in_pitch = C;
-        P.out = nullptr; P.out_pitch = 4 * C;
-        P.epi = EPI_GEGLU;
-        P.pl_hi = pf.hi; P.pl_lo = pf.lo; P.pl_pitch = 4 * C;
-        tapconv_launch(P, s);
-      }
-      float* h4 = alloc(rows * C);
-      AGPT_CHECK(linear_planes(b.ff2, pf, 4 * C, h4, C, rows, EPI_RES, h3, C, last ? &ph : nullptr, s), "plane-fed GEMM rejected ff.net.2");
-      h = h4;
-    }
-    float* out = alloc(rows * t.ch);
-    AGPT_CHECK(linear_planes(t.proj_out, ph, C, out, t.ch, rows, EPI_RES, x, t.ch, nullptr, s), "plane-fed GEMM rejected proj_out");
-    return out;
-  }
-
-  bool st_planes_ok(const StW& t) const {
-    // fp16 rows must be 16-byte aligned for the tensor maps; the tcgen05 attention must cover the head dim
-    const int d = t.dhead;
-    return planes_enabled() && t.inner % 8 == 0 && t.ch % 8 == 0 && (d == 8 || d == 16 || d == 32 || d == 40 || d == 64 || d == 80) &&
-           attention_tc_enabled();
-  }
-
   float* run_st(const StW& t, const float* x, int N, int H, int W, cudaStream_t s) {
-    if (st_planes_ok(t)) return run_st_planes(t, x, N, H, W, s);
     const int HW = H * W;
     const long rows = (long)N * HW;
     const int C = t.inner;

@@ -1,9 +1,9 @@
-// AutoencoderKL.decode (Make-An-Audio first stage) on sm_100a: latent [B,4,10,78] -> mel image [B,1,80,624].
+// AutoencoderKL.decode (Make-An-Audio first stage) on sm_90a: latent [B,4,10,78] -> mel image [B,1,80,624].
 // Reference: ldm/models/autoencoder.py:351-354 (decode = post_quant_conv -> decoder),
 //            ldm/modules/diffusionmodules/model.py:462-568 (Decoder), :121-143 (ResnetBlock, temb None),
 //            :150-203 (AttnBlock: single head of width C, scale C^-0.5), :43-49 (Upsample: nearest x2 then conv),
 //            :33-39 (swish, GroupNorm(32, eps 1e-6)).
-// Activations are channels-last rows [B][H*W][C]; every 3x3 / 1x1 conv is a tap-GEMM on the tcgen05 kernels
+// Activations are channels-last rows [B][H*W][C]; every 3x3 / 1x1 conv is a tap-GEMM on the tensor-core kernel
 // (wide maps -- 156, 312, 624 columns -- in STRIP mode, TapConvParams::strips: the halo of a 128-row tile would
 // otherwise span two 625-wide image rows); GroupNorm(+swish) is the fused single-kernel GroupNorm of nn_kernels.cu;
 // the seven AttnBlocks (780 tokens x 512 ch, 3 120 tokens x 256 ch) run as Q K^T / row softmax / P V with the

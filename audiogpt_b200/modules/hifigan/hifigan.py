@@ -11,7 +11,7 @@ weight-norm removal (``*.weight_g`` / ``*.weight_v``  vs  ``*.weight``), so
     model = HifiGanGenerator(config); model.load_state_dict(state, strict=True)
     model.remove_weight_norm(); model = model.eval().to(device)
 
-The arithmetic runs in libagpt_b200.so (hand-written sm_100a kernels); the
+The arithmetic runs in libagpt_b200.so (hand-written sm_90a kernels); the
 module only stores parameters.  There is no CPU path: ``forward`` on a CPU
 tensor raises.
 """
@@ -215,7 +215,7 @@ class HifiGanGenerator(nn.Module, _lib.HandleOwner):
         """x: [B, 80, T] fp32 CUDA -> [B, c_out, T*hop]   (hifigan.py:144-169)"""
         if not x.is_cuda:
             raise RuntimeError("audiogpt_b200.HifiGanGenerator runs on CUDA only (no CPU fallback); "
-                               "move the model and input to a B200 device")
+                               "move the model and input to a CUDA device (H100)")
         x = x.contiguous().float()
         B, M, T = x.shape
         self._ensure_engine(x.device)

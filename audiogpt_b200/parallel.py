@@ -7,7 +7,7 @@ The only collectives are the two the north star names, both outside the kernels:
 * one broadcast of the packed weights at start-up (``broadcast_state_dict``), and
 * one all-gather of the finished fp32 waveforms per batch (``all_gather_rows``).
 
-One process per GPU (``torch.distributed``; NCCL over NVLink on the B200 box, gloo in the
+One process per GPU (``torch.distributed``; NCCL over NVLink on a multi-GPU machine, gloo in the
 CPU tests).  The reference has no inference-time multi-GPU at all: its tool classes are
 pinned to fixed devices by hand (audio-chatgpt.py:1051-1073).
 """
@@ -228,7 +228,7 @@ def run_mixed(jobs: Sequence[Tuple[str, int]], run_job, *, sync=None, run_group=
 
     Returns, on every rank: ``assignment`` (per-rank job indices), ``busy_s`` (per-rank busy seconds),
     ``makespan_s`` (max over ranks), ``jobs_per_s`` and ``busy_fraction`` (busy / makespan per rank).
-    ``sync`` is called before each clock read (pass ``torch.cuda.synchronize`` on a GPU box).
+    ``sync`` is called before each clock read (pass ``torch.cuda.synchronize`` on a GPU).
     ``run_group(kind, indices)`` (optional) lets a rank serve its OWN jobs of one kind in micro-batches of at most
     ``group_size[kind]`` (default 1) -- e.g. four text-to-audio clips as one CFG batch of 8; the assignment itself
     is unchanged."""

@@ -12,7 +12,7 @@ after weight-norm removal (including the ``*.filter`` buffers of every ``Activat
 
 BigVGAN is the HiFi-GAN generator with every leaky-relu replaced by an anti-aliased periodic
 activation; the engine is the same C-ABI object (``agpt_hifigan_*`` with ``cfg.activation != 0``): the
-convolutions run on the tcgen05 tap-GEMM kernels, the activations in ``aa_snake_kernel``
+convolutions run on the wgmma tap-GEMM kernel, the activations in ``aa_snake_kernel``
 (csrc/hifigan.cu).  CUDA only -- no CPU path.
 """
 from __future__ import annotations

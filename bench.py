@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the AudioGPT generative hot path on B200 (contract: see the task brief).
+"""Benchmark of the AudioGPT generative hot path on one or more H100s.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload hifigan|ddim]
 
@@ -17,11 +17,11 @@ BASELINE.json's metric has two halves; one JSON line carries both:
   value     : device-resident inputs, CUDA-event timed, barrier + synchronize on both sides, max over ranks
   e2e       : the same metric through the public host-buffer call (pinned H2D of the inputs, D2H of the result
               inside the timed region): agpt_hifigan_vocode_host / DDIMSampler.sample on host tensors
-  roofline  : the tcgen05 tap-GEMM against the measured bf16/fp16 tensor peak (MEASURED_PEAKS.json).  `frac` is
+  roofline  : the wgmma tap-GEMM against the measured bf16/fp16 tensor peak (MEASURED_PEAKS.json).  `frac` is
               on ALGORITHMIC FLOPs (SURVEY.md 8d: 0.614 GFLOP per mel frame, 18.66 TFLOP per clip); `frac_issued`
               counts the three fp16 products the error-compensated arithmetic issues per MAC.
   cpu_baseline / --impl reference : the CPU oracle (oracle/*.py: the reference's forward restated on torch's own
-              fp32 CPU kernels -- the reference is pure Python and does not travel to the GPU box) on the host cores
+              fp32 CPU kernels; the reference itself is pure Python) on the host cores
   extra     : DiffSinger C3 chain (16 utt x 400 frames x 100 p_sample steps), BigVGAN base, each one full run
 
 With N > 1 (torchrun, one rank per GPU) every rank works on its own batch (weak scaling, no data-path
@@ -48,7 +48,7 @@ import torch  # noqa: E402
 B_PER_GPU, T_FRAMES, HOP, SR = 8, 800, 256, 22050
 METRIC, UNIT = "mel_frames_per_s_vocoded", "frames/s"
 WORKLOAD = "HiFi-GAN V1 22.05kHz vocoder, batch 8 x 800 mel frames per GPU (FastSpeech2->HiFi-GAN, BASELINE configs[1])"
-ARITH = "3xfp16-split: x = hi + lo fp16 parts, products hi*hi + lo*hi + hi*lo on tcgen05 kind::f16, fp32 accumulate in TMEM"
+ARITH = "3xfp16-split: x = hi + lo fp16 parts, products hi*hi + lo*hi + hi*lo on wgmma (f16 inputs), fp32 accumulate in registers"
 
 DDIM_B, DDIM_S, DDIM_SCALE, DDIM_SHAPE = 4, 100, 1.5, (4, 10, 78)
 DDIM_METRIC, DDIM_UNIT = "clips_per_s_ddim100_cfg", "clips/s"
@@ -62,7 +62,7 @@ def base_config(n_gpus):
             "global_batch": B_PER_GPU * n_gpus, "hop": HOP, "sample_rate": SR,
             "weights": "seeded random (specs.synth_hifigan(HIFIGAN_V1, 1234))", "arith": ARITH,
             "parallelism": f"batch-sharded x{n_gpus}, no data-path collective",
-            "l2_policy": "activation working set per step ~2.5 GB >> 126 MB L2 (no explicit flush needed)"}
+            "l2_policy": "activation working set per step ~2.5 GB >> 50 MB L2 (no explicit flush needed)"}
 
 
 def ddim_config(n_gpus):
@@ -70,7 +70,7 @@ def ddim_config(n_gpus):
             "cfg_scale": DDIM_SCALE, "latent": list(DDIM_SHAPE), "context": [77, 1024],
             "weights": "seeded random (specs.synth_unet(UNET_TXT2AUDIO, 4040))", "arith": ARITH,
             "parallelism": f"clips sharded x{n_gpus}, no data-path collective",
-            "l2_policy": "weights 641 MB fp32 (1.28 GB as fp16 hi/lo images) re-read every forward >> 126 MB L2"}
+            "l2_policy": "weights 641 MB fp32 (1.28 GB as fp16 hi/lo images) re-read every forward >> 50 MB L2"}
 
 
 def load_peaks():
@@ -139,8 +139,7 @@ _ALLOC_NOTE = ""
 
 def _cpu_allocator_tuning():
     """The CPU forward allocates and frees 50-MB intermediates; with glibc's defaults every one of them is mmap'ed,
-    page-faulted and unmapped again, which on a 128-CPU box costs the 16-thread CPU path 5x (measured: 473 -> 2 500
-    frames/s, profiles/r2s_reference_arm.txt).  Keep freed memory in the heap instead (what MALLOC_MMAP_MAX_=0
+    page-faulted and unmapped again, which the multi-threaded CPU path pays for in kernel time.  Keep freed memory in the heap instead (what MALLOC_MMAP_MAX_=0
     MALLOC_TRIM_THRESHOLD_=... would do from the environment): the CPU arms get their best."""
     global _ALLOC_NOTE
     if _ALLOC_NOTE:
@@ -249,15 +248,15 @@ def run_reference_arm(args):
                      "cpu_baseline": {"value": ddim_rate, "unit": DDIM_UNIT, "cores": ddim_cores, "kind": "port",
                                       "sample": f"B=1: 3 of the {DDIM_S} DDIM steps (CFG pair per step); clips/s = 1/(s_per_step x {DDIM_S})"},
                      "s_per_ddim_step": ddim_sps},
-            "note": "CPU oracle port of HifiGanGenerator.forward / DDIMSampler+UNetModel (the reference is pure PyTorch and "
-                    "/root/reference does not travel to the GPU box, so kind = port); ms_per_step and frames_per_step "
+            "note": "CPU oracle port of HifiGanGenerator.forward / DDIMSampler+UNetModel (the reference is pure PyTorch, "
+                    "so kind = port); ms_per_step and frames_per_step "
                     "describe the bounded sample actually run; RTF = value*hop/sample_rate"}
     line["x_realtime"] = rate * HOP / SR
     print(json.dumps(line))
 
 
 # ------------------------------------------------------------------------------------ GPU arm: DDIM (C4)
-def measure_ddim(dev, rank, n_gpus, chains, peaks, want_cpu, keep=None):
+def measure_ddim(dev, rank, n_gpus, chains, peaks, want_cpu, keep=None, dump=None):
     """All ranks: DDIM-100 + CFG for DDIM_B clips per rank.  Returns the 'ddim' object (rank 0) or None.
     ``keep`` (a dict) receives the sampler so that the mixed-dispatch measurement can reuse the 160 M-param engine."""
     import ctypes as C
@@ -302,6 +301,9 @@ def measure_ddim(dev, rank, n_gpus, chains, peaks, want_cpu, keep=None):
     barrier()
     ms = e0.elapsed_time(e1)
     launches = _lib.launch_count() - l0
+    if dump and rank == 0:      # the latents [4, 4, 10, 78] the caller of the timed chain receives from its last chain
+        os.makedirs(dump, exist_ok=True)
+        np.save(os.path.join(dump, "latent.npy"), z.float().cpu().numpy())
     # e2e: host tensors in, host latent out, through DDIMSampler.sample
     t0 = time.perf_counter()
     for _ in range(chains):
@@ -326,12 +328,7 @@ def measure_ddim(dev, rank, n_gpus, chains, peaks, want_cpu, keep=None):
     clips = B * n_gpus
     value = clips / (ms_chain * 1e-3)
     ach = DDIM_TFLOP_PER_CLIP * B / (ms_chain * 1e-3)             # per GPU, algorithmic
-    peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1590.0)))
-    ddim_traffic = None
-    try:      # DRAM bytes of one 4-clip chain (100 steps) from the committed ncu launch list of the DDIM steps
-        ddim_traffic = json.load(open(os.path.join(ROOT, "profiles", "ddim_traffic.json"))).get("dram_bytes_per_chain")
-    except Exception:
-        pass
+    peak = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))
     out = {"metric": DDIM_METRIC, "value": value, "unit": DDIM_UNIT, "n_gpus": n_gpus, "steps": chains, "warmup": 1,
            "ms_per_step": ms_chain, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
            "data": "synthetic", "config": ddim_config(n_gpus),
@@ -340,14 +337,13 @@ def measure_ddim(dev, rank, n_gpus, chains, peaks, want_cpu, keep=None):
                    "h2d_bytes_per_step": int(xT_h.nbytes + c_h.nbytes + uc_h.nbytes), "d2h_bytes_per_step": int(z_h.nbytes),
                    "api": "DDIMSampler.sample(S=100, ...) on pinned host tensors -> .cpu() latent"},
            "gpu_launches": int(launches), "launches_per_ddim_step": lps,
-           "roofline": {"kernel": "whole DDIM chain: tcconv5/6 tap-GEMMs + GroupNorm / LayerNorm / attention / update kernels",
+           "roofline": {"kernel": "whole DDIM chain: tcconv5 tap-GEMMs + GroupNorm / LayerNorm / attention / update kernels",
                         "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
                         "frac_issued": 3.0 * ach / peak, "algorithmic_tflop_per_clip": DDIM_TFLOP_PER_CLIP,
                         "peak_source": ("MEASURED_PEAKS.json bf16_tflops_sustained (a kernel timed inside a long step)"
-                                        if peaks else "fallback 1.59 PFLOP/s dense bf16/fp16"),
+                                        if peaks else "fallback: H100 SXM data sheet, 989 TFLOP/s dense fp16 at 700 W"),
                         "note": "achieved = 18.66 algorithmic TFLOP per clip x clips per GPU / chain time (all kernels of the "
-                                "chain, not only the GEMMs); traffic = DRAM bytes of one chain (profiles/ddim_traffic.json)",
-                        "traffic": ddim_traffic}}
+                                "chain, not only the GEMMs)"}}
     if want_cpu:
         r, sps, cores = cpu_ddim_rate(3)
         out["cpu_baseline"] = {"value": r, "unit": DDIM_UNIT, "cores": cores, "kind": "port",
@@ -432,7 +428,7 @@ def run_ours(args):
         sampler = ClockSampler(local)
         if rank == 0:
             sampler.start()
-        d = measure_ddim(dev, rank, n_gpus, max(1, args.steps), peaks, want_cpu=(n_gpus == 1))
+        d = measure_ddim(dev, rank, n_gpus, max(1, args.steps), peaks, want_cpu=(n_gpus == 1), dump=args.dump_outputs)
         if rank == 0:
             d["clocks"] = sampler.stop()
             print(json.dumps(d))
@@ -451,8 +447,8 @@ def run_ours(args):
     mel = mel_host.to(dev)
     frames_step = B_PER_GPU * T_FRAMES * n_gpus
     # finished waveforms -> every rank: asynchronous NCCL all-gather on NCCL's stream under the next step (default), or
-    # AGPT_GATHER=p2p: copy engines over NVLink (parallel.P2PGather).  Measured on one 4-GPU box (profiles/r2w_*): no gather
-    # 18.94 ms per step, NCCL 19.07, copy engines 19.86 -- N - 1 serial peer copies per rank stop paying past N = 2
+    # AGPT_GATHER=p2p: copy engines over NVLink (parallel.P2PGather).  N - 1 serial peer copies per rank; the
+    # copy-engine gather has not been measured against NCCL on H100
     gather, gather_kind = None, None
     if n_gpus > 1:
         gsel = os.environ.get("AGPT_GATHER", "nccl")
@@ -493,7 +489,7 @@ def run_ours(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        step_device()
+        wav_last = step_device()
     if gather is not None:
         gather.drain()               # the compute stream waits for every outstanding gather: inside the timed region
     e1.record()
@@ -509,6 +505,10 @@ def run_ours(args):
     clocks = sampler.stop() if rank == 0 else None
     ms_per_step = ms / args.steps
     value = frames_step / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        # the waveforms [B, 1, T x hop] the caller of the timed step receives in its last step (6.6 MB in float32)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "wav.npy"), wav_last.float().cpu().numpy())
 
     # ---- e2e: host buffers through the C-ABI (H2D + forward + D2H + sync inside the call)
     mel_np = mel_host.numpy()
@@ -539,13 +539,8 @@ def run_ours(args):
         _lib.check(L.agpt_profile_enable(0))
         tot_ms = sum(msv)
         ach_tf = sum(flv) / (tot_ms * 1e-3) / 1e12
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "tapconv_traffic.json"))).get("dram_bytes_per_launch")
-        except Exception:
-            pass
-        variants = ["fma_BN128", "fma_BN64", "fma_BN32", "tcgen05_3xFP16"]
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        variants = ["fma_BN128", "fma_BN64", "fma_BN32", "wgmma_3xFP16"]
         tc_on = lnv[3] > 0
         per_variant = {variants[i]: {"launches": int(lnv[i]), "ms": msv[i],
                                      "tflops": (flv[i] / (msv[i] * 1e-3) / 1e12) if msv[i] > 0 else None,
@@ -553,25 +548,25 @@ def run_ours(args):
                        for i in range(4) if lnv[i] > 0}
         hbm = {"bound": "hbm", "achieved": sum(byv) / (tot_ms * 1e-3) / 1e9, "peak": hbm_peak, "unit": "GB/s",
                "frac": sum(byv) / (tot_ms * 1e-3) / 1e9 / hbm_peak,
-               "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6.65 TB/s",
+               "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback: H100 SXM data sheet, 3.35 TB/s",
                "note": "per-launch algorithmic bytes (in+out+residual+weights of every conv launch); the path is compute-bound "
                        "(AI ~ 10^3 FLOP/B, SURVEY.md 8d) so this fraction is small by construction"}
         if tc_on:
-            f16_peak = float(peaks.get("bf16_tflops", 1590.0))
+            f16_peak = float(peaks.get("bf16_tflops", 989.0))
             roofline = {
-                "kernel": "tcconv6_kernel<BN,NI> / tcconv5_kernel<BN,NWK> (tcgen05 tap-GEMM, 3 x fp16 hi/lo products; "
+                "kernel": "tcconv5_kernel<BN> (wgmma tap-GEMM, 3 x fp16 hi/lo products; "
                           "all contractions of the generator)",
                 "bound": "tensor", "achieved": ach_tf, "peak": f16_peak, "unit": "TFLOP/s",
                 "frac": ach_tf / f16_peak, "frac_issued": 3.0 * ach_tf / f16_peak,
                 "achieved_issued_tflops": 3.0 * ach_tf,
-                "peak_source": ("MEASURED_PEAKS.json bf16_tflops (burst: kernels timed one by one); kind::f16 issues at the bf16 rate"
-                                if peaks else "fallback 1.59 PFLOP/s dense bf16/fp16"),
+                "peak_source": ("MEASURED_PEAKS.json bf16_tflops (burst: kernels timed one by one); fp16 wgmma issues at the bf16 rate"
+                                if peaks else "fallback: H100 SXM data sheet, 989 TFLOP/s dense fp16 at 700 W"),
                 "note": "achieved / frac are on ALGORITHMIC FLOPs (SURVEY.md 8d: 0.614 GFLOP per mel frame, zero-padded polyphase "
                         "taps not counted); the tensor pipe issues 3 fp16 products per fp32-grade MAC (frac_issued)",
                 "fp32_fma_peak_tflops_measured": fma_peak,
                 "algorithmic_vs_fp32_fma_peak": ach_tf / fma_peak if fma_peak > 0 else None,
                 "share_of_step": tot_ms / ms_per_step if n_gpus == 1 else None,
-                "per_variant": per_variant, "hbm": hbm, "traffic": traffic,
+                "per_variant": per_variant, "hbm": hbm,
             }
         else:
             roofline = {
@@ -580,7 +575,7 @@ def run_ours(args):
                 "frac": ach_tf / fma_peak if fma_peak > 0 else None,
                 "peak_source": "fp32 FFMA saturation probe run in this process (agpt_fma_peak_tflops)",
                 "share_of_step": tot_ms / ms_per_step if n_gpus == 1 else None,
-                "per_variant": per_variant, "hbm": hbm, "traffic": traffic,
+                "per_variant": per_variant, "hbm": hbm,
             }
     # ---- the other half of the metric: DDIM-100 clips/s on the C4 shard (all ranks), then the mixed dispatch (C5)
     ddim, mixed, keep = None, None, {}
@@ -732,10 +727,13 @@ def main():
     ap.add_argument("--no-ddim", action="store_true", help="skip the DDIM C4 measurement")
     ap.add_argument("--no-mixed", action="store_true", help="skip the mixed-dispatch (BASELINE configs[4]) measurement")
     ap.add_argument("--no-extra", action="store_true", help="skip the secondary DiffSinger / BigVGAN measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (seeded inputs: identical from run to "
+                         "run) as float32: DIR/wav.npy (hifigan workload) or DIR/latent.npy (ddim workload)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
-    if args.workload == "ddim" and args.impl == "ours":
-        args.steps = min(args.steps, 5)
+    if args.dump_outputs and args.impl != "ours":
+        raise SystemExit("--dump-outputs applies to the timed GPU path (--impl ours)")
     if args.impl == "reference":
         run_reference_arm(args)
     else:

@@ -1,4 +1,4 @@
-/* libagpt_b200 -- C ABI of the B200-native AudioGPT generative back-end.
+/* libagpt_b200 -- C ABI of the H100 (sm_90a) AudioGPT generative back-end.
  *
  * The reference (AIGC-Audio/AudioGPT) is pure Python: it has no FFI layer, its
  * "plugin boundary" is the Python class surface listed in SURVEY.md 8(b).  The
@@ -31,38 +31,33 @@ int agpt_version(void);
 long long agpt_launch_count(void);
 void agpt_destroy(agpt_handle h);
 /* Measurement helpers (bench.py): per-launch CUDA-event timing of the tapconv kernel,
- * summed per variant v = {0,1,2: fp32-FMA tiles BN=128/64/32; 3: tcgen05 version}; an fp32-FMA
+ * summed per variant v = {0,1,2: fp32-FMA tiles BN=128/64/32; 3: wgmma tensor-core version}; an fp32-FMA
  * saturation probe returning the measured TFLOP/s of the current device.       */
 int agpt_profile_enable(int on);
 int agpt_profile_collect(double ms[4], double flops[4], double bytes[4], long long launches[4]);
 /* dev tooling: one text line per recorded launch ("variant G L Cin Cout ntaps span epi Wreal ms flops"); returns bytes written or -1 */
 long agpt_profile_dump(char* out, long cap);
 double agpt_fma_peak_tflops(void);
-/* 1 (default): contractions run on the tcgen05 tensor cores with error-compensated fp16 parts
- * ("3xfp16": x = hi + lo, products hi*hi + lo*hi + hi*lo, fp32 accumulation in TMEM; weights pre-scaled
+/* 1 (default): contractions run on the tensor cores (wgmma) with error-compensated fp16 parts
+ * ("3xfp16": x = hi + lo, products hi*hi + lo*hi + hi*lo, fp32 accumulation; weights pre-scaled
  * by a power of two per layer); 0: the fp32-FMA kernels only.  Environment: AGPT_TENSOR_CORES.        */
 int agpt_set_tensor_cores(int on);
-/* tcgen05 kernel schedule: 6 (default) = persistent kernel (tcconv6) where a CTA gets more than one tile,
- * one-tile-per-CTA kernel (tcconv5) otherwise; 5 = tcconv5 only; 7 = tcconv6 forced; -1 = environment
- * (AGPT_TC_V) / default.                                                                               */
-int agpt_set_tc_version(int v);
 /* Multi-head attention softmax_j(q_i . k_j * d^-0.5) v_j, heads outermost in the channel dim ('b n (h d)'),
  * CrossAttention.forward (ldm/modules/attention.py:170-193): q [N][Lq][q_pitch], k / v [N][Lk][pitch] device rows with
- * head h at channels [h*d, (h+1)*d); o [N][Lq][o_pitch].  Default: QK^T and PV on the tcgen05 tensor cores
- * (error-compensated fp16 parts, fp32 accumulation, exact online softmax; d in {8,16,32,40,64,80});
- * agpt_set_attention_tc(0) / AGPT_ATTN_TC=0 selects the fp32-FMA kernel, (2) / =2 routes the call through the
- * plane-fed kernel the UNet uses internally (q / k / v split into fp16 hi/lo planes first; test / A-B route).      */
+ * head h at channels [h*d, (h+1)*d); o [N][Lq][o_pitch].  Default: QK^T and PV on the tensor cores (wgmma,
+ * error-compensated fp16 parts, fp32 accumulation, exact online softmax; d in {8,16,32,40,64,80});
+ * agpt_set_attention_tc(0) / AGPT_ATTN_TC=0 selects the fp32-FMA kernel, -1 = environment / default.            */
 int agpt_attention(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, float* o,
                    int o_pitch, int N, int heads, int d, int Lq, int Lk, void* stream);
 int agpt_set_attention_tc(int on);
 /* Micro-benchmark of one tapconv layer (random data): out3 = {ms per launch, algorithmic TFLOP/s,
- * max |tcgen05 - fp32 FMA| when check != 0}; dbg8 (tcgen05 only) = average per-CTA phase cycles
+ * max |tensor-core - fp32 FMA| when check != 0}; dbg8 (tensor-core kernel only) = average per-CTA phase cycles
  * {setup, first activation tile, MMA issue loop, drain, epilogue, total, wait-on-activations,
  * wait-on-weights}.  Wreal > 0 selects a 3x3 conv on an (L/Wreal) x Wreal image.              */
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc,
                        int reps, int check, double* out3, double* dbg8_or_null);
 /* Numerics probe of one layer: activations ~ N(0,1) * x_scale, weights with a weight-norm-like gain spread
- * (output channel gains log-uniform over a factor w_spread); runs the selected tcgen05 kernel and the fp32-FMA
+ * (output channel gains log-uniform over a factor w_spread); runs the tensor-core kernel and the fp32-FMA
  * kernel on the same data.  rel2 = {max |diff| / rms(ref), rms(diff) / rms(ref)} (1e30 if anything is not finite). */
 int agpt_check_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, double x_scale,
                        double w_spread, double* rel2);

@@ -1,4 +1,4 @@
-"""CPU emulation of the tensor-core arithmetic of csrc/tcconv5.cu / tcconv6.cu ("3 x fp16 parts"):
+"""CPU emulation of the tensor-core arithmetic of csrc/tcconv5.cu / attention_tc.cu ("3 x fp16 parts"):
 documents the error bound the GPU parity tests rely on, without a GPU.
 
 x = x_hi + x_lo (x_hi = fp16(x) with saturation, x_lo = fp16(x - x_hi)); weights the same after a per-layer

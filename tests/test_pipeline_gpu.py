@@ -1,5 +1,5 @@
 """End-to-end and cross-cutting GPU tests: diffusion -> mel -> HiFi-GAN -> waveform pipeline against the
-CPU oracle, the vocoder wrapper (numpy in / numpy out), and the three generations of the tcgen05
+CPU oracle, the vocoder wrapper (numpy in / numpy out), and the tensor-core
 tap-GEMM kernel against the fp32-FMA kernel on the layer shapes of the BASELINE configs."""
 import ctypes as C
 
@@ -81,42 +81,18 @@ SHAPES = [  # G, L, Cin, Cout, K, dil, Wreal
 ]
 
 
-@pytest.mark.parametrize("ver", [5, 6, 7])
-def test_tcgen05_schedules_match_fma(ver):
-    """agpt_check_tapconv runs the layer with the selected tcgen05 schedule (5 = one tile per CTA, 6 = default mix,
-    7 = persistent kernel forced, which also exercises CTAs that own 0 or 1 tiles) and with the fp32-FMA kernel on
-    the same random data.  Stated tolerance, RELATIVE to the output rms: rms diff <= 2e-5, max |diff| <= 2e-4 over
-    up to 1.5 M outputs (measured on B200: rms 5e-7 .. 1e-5 growing with the contraction length K = taps x C_in up to
+def test_tensor_core_tapconv_matches_fma():
+    """agpt_check_tapconv runs the layer on the wgmma tap-GEMM (tcconv5: one tile per CTA, tile width picked to fill
+    the SMs) and on the fp32-FMA kernel with the same random data.  Stated tolerance, RELATIVE to the output rms: rms diff <= 2e-5, max |diff| <= 2e-4 over
+    up to 1.5 M outputs (rms 5e-7 .. 1e-5 growing with the contraction length K = taps x C_in up to
     2 816, max 6e-6 .. 6e-5; the 3 x fp16-part arithmetic truncates at 2^-22 per product and drops lo x lo)."""
     L = _lib.lib()
     torch.zeros(1).cuda()
-    _lib.check(L.agpt_set_tc_version(ver))
-    try:
-        for G, Ln, Cin, Cout, K, dil, Wr in SHAPES:
-            for epi_res in (0, 1):
-                rel = (C.c_double * 2)()
-                _lib.check(L.agpt_check_tapconv(G, Ln, Cin, Cout, K, dil, Wr, epi_res, C.c_double(1.0), C.c_double(1.0), rel))
-                assert rel[0] < 2e-4 and rel[1] < 2e-5, (ver, G, Ln, Cin, Cout, K, dil, Wr, epi_res, rel[0], rel[1])
-    finally:
-        _lib.check(L.agpt_set_tc_version(-1))
-
-
-def test_plane_fed_kernel_matches_fma():
-    """Schedule selector 8 runs the layer on the plane-fed kernel (tcconv7: TMA-fed fp16 hi/lo operand planes in, fp32 result
-    + planes of the result out) against the fp32-FMA kernel; 1-D layers only.  The 1 560-row shapes take the 64- and
-    96-wide tiles the launcher picks when 128-wide tiles would leave SMs idle (last column tile partial at 96)."""
-    L = _lib.lib()
-    torch.zeros(1).cuda()
-    _lib.check(L.agpt_set_tc_version(8))
-    try:
-        for G, Ln, Cin, Cout, K, dil, Wr in [(2, 3000, 256, 256, 11, 5, 0), (16, 400, 256, 512, 3, 2, 0), (1, 1560, 640, 640, 1, 1, 0),
-                                             (1, 1560, 640, 1920, 1, 1, 0), (1, 6240, 320, 320, 1, 1, 0), (2, 500, 96, 40, 5, 2, 0)]:
-            for epi_res in (0, 1):
-                rel = (C.c_double * 2)()
-                _lib.check(L.agpt_check_tapconv(G, Ln, Cin, Cout, K, dil, Wr, epi_res, C.c_double(1.0), C.c_double(1.0), rel))
-                assert rel[0] < 2e-4 and rel[1] < 2e-5, (G, Ln, Cin, Cout, K, dil, epi_res, rel[0], rel[1])
-    finally:
-        _lib.check(L.agpt_set_tc_version(-1))
+    for G, Ln, Cin, Cout, K, dil, Wr in SHAPES:
+        for epi_res in (0, 1):
+            rel = (C.c_double * 2)()
+            _lib.check(L.agpt_check_tapconv(G, Ln, Cin, Cout, K, dil, Wr, epi_res, C.c_double(1.0), C.c_double(1.0), rel))
+            assert rel[0] < 2e-4 and rel[1] < 2e-5, (G, Ln, Cin, Cout, K, dil, Wr, epi_res, rel[0], rel[1])
 
 
 @pytest.mark.parametrize("x_scale,w_spread,tol_max,tol_rms", [
