@@ -11,6 +11,8 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.ldm.models.autoencoder.AutoencoderKL          (decode side; not installed over the reference class)
     audiogpt_b200.modules.fastspeech.pe.PitchExtractor
     audiogpt_b200.vocoder.bigvgan.models.BigVGAN / VocoderBigVGAN
+    audiogpt_b200.modules.fastspeech.fs2.FastSpeech2                (installed with install(front_end=True))
+    audiogpt_b200.modules.diffsinger_midi.fs2.FastSpeech2MIDI       (installed with install(front_end=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -30,9 +32,14 @@ _INSTALL_MAP = {
     "vocoder.bigvgan.models": ("audiogpt_b200.vocoder.bigvgan.models", ["BigVGAN", "VocoderBigVGAN"]),
     "modules.fastspeech.pe": ("audiogpt_b200.modules.fastspeech.pe", ["PitchExtractor"]),
 }
+# the acoustic front-end, grafted only on request (install(front_end=True))
+_FRONT_END_MAP = {
+    "modules.fastspeech.fs2": ("audiogpt_b200.modules.fastspeech.fs2", ["FastSpeech2"]),
+    "modules.diffsinger_midi.fs2": ("audiogpt_b200.modules.diffsinger_midi.fs2", ["FastSpeech2MIDI"]),
+}
 
 
-def install(strict: bool = False):
+def install(strict: bool = False, front_end: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -42,11 +49,14 @@ def install(strict: bool = False):
     HifiGanGenerator``, ``instantiate_from_config({'target':
     'ldm.modules.diffusionmodules.openaimodel.UNetModel', ...})`` and ``DDIMSampler(model)`` all
     resolve to the drop-ins.  Modules that are not importable are registered in ``sys.modules``
-    as aliases of ours when ``strict`` is False.  Returns the list of patched names."""
+    as aliases of ours when ``strict`` is False.  ``front_end=True`` also replaces FastSpeech2 and
+    FastSpeech2MIDI, so GaussianDiffusion's front-end (and any other user of those classes) runs on the engine.
+    Returns the list of patched names."""
     import importlib
     import sys
     patched = []
-    for ref_name, (our_name, attrs) in _INSTALL_MAP.items():
+    todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}))
+    for ref_name, (our_name, attrs) in todo.items():
         ours = importlib.import_module(our_name)
         try:
             ref = importlib.import_module(ref_name)

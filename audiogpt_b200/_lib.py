@@ -60,6 +60,13 @@ class PeCfg(C.Structure):
                 ("predictor_hidden", C.c_int), ("predictor_layers", C.c_int), ("predictor_kernel", C.c_int)]
 
 
+class Fs2Cfg(C.Structure):
+    _fields_ = [(n, C.c_int) for n in (
+        "hidden_size", "num_heads", "enc_layers", "dec_layers", "enc_ffn_kernel", "dec_ffn_kernel", "n_tokens", "out_dims",
+        "predictor_hidden", "dur_predictor_layers", "dur_predictor_kernel", "predictor_layers", "predictor_kernel",
+        "use_pos_embed", "rel_pos", "pitch_type", "use_energy_embed", "use_midi")]
+
+
 _lock = threading.Lock()
 _lib = None
 

@@ -243,6 +243,39 @@ int agpt_pe_forward(agpt_handle h, const float* mel, int B, int T, float* pitch_
   });
 }
 
+int agpt_attention_masked(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
+                          const uint8_t* key_padding_mask, float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(q && k && v && o && key_padding_mask && N >= 1 && heads >= 1 && Lq >= 1 && Lk >= 1, "bad argument");
+    attention(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, d, Lq, Lk, (cudaStream_t)stream, key_padding_mask);
+  });
+}
+
+int agpt_fs2_create(const agpt_fs2_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(fs2_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_fs2_encode(agpt_handle h, const int* txt_tokens, int B, int T_txt, const int* pitch_midi, const float* midi_dur,
+                    const int* is_slur, int predict_dur, float* dur, int* dur_choice, int* mel_len_host, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(txt_tokens && dur && (!predict_dur || mel_len_host), "null argument");
+    fs2_encode(as(h, kMagicFs2, "fastspeech2"), txt_tokens, B, T_txt, pitch_midi, midi_dur, is_slur, predict_dur, dur, dur_choice,
+               mel_len_host, (cudaStream_t)stream);
+  });
+}
+
+int agpt_fs2_decode(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out, const float* f0, const float* uv, const float* energy,
+                    int use_uv, int pitch_norm, float f0_mean, float f0_std, float* pitch_pred, float* f0_denorm, int* pitch_coarse,
+                    float* energy_pred, float* decoder_inp, float* mel_out, void* stream) {
+  return guarded([&] {
+    fs2_decode(as(h, kMagicFs2, "fastspeech2"), T_mel, mel2ph, mel2ph_out, f0, uv, energy, use_uv, pitch_norm, f0_mean, f0_std, pitch_pred,
+               f0_denorm, pitch_coarse, energy_pred, decoder_inp, mel_out, (cudaStream_t)stream);
+  });
+}
+
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                        int check, double* out3, double* dbg8_or_null) {
   return guarded([&] { bench_tapconv(G, L, Cin, Cout, K, dil, Wreal, epi_res, use_tc, reps, check, out3, dbg8_or_null); });

@@ -24,7 +24,7 @@ namespace {
 constexpr int AT_BK = 64;          // keys per block = one 128-byte swizzle span of fp16
 constexpr int AT_ROWS = 64;        // queries per CTA (wgmma M)
 
-// D = head dim (multiple of 8, <= 128).  NCH = 64-channel chunks of the head dim; DP = D rounded up to 16 (the N of
+// D = head dim (multiple of 8, <= 128; 128 is FastSpeech2's hidden 256 over 2 heads).  NCH = 64-channel chunks of the head dim; DP = D rounded up to 16 (the N of
 // the P V wgmma and the K granularity of Q K^T)
 template <int D>
 struct AtCfg {
@@ -46,14 +46,17 @@ __device__ __forceinline__ void wgmma_f16(float* d, uint64_t a, uint64_t b) {
   else if constexpr (N == 32) wgmma_n32(d, a, b);
   else if constexpr (N == 48) wgmma_n48(d, a, b);
   else if constexpr (N == 64) wgmma_n64(d, a, b);
-  else wgmma_n80(d, a, b);
+  else if constexpr (N == 80) wgmma_n80(d, a, b);
+  else wgmma_n128(d, a, b);
 }
 
-template <int D>
+// MASK: kpm [N][Lk] bytes, 1 = padding key (fairseq's key_padding_mask); a query whose keys are all padding gets zeros.
+// The parameter is last and unread without MASK, so the unmasked instantiations are the kernels they were before it.
+template <int D, bool MASK>
 __global__ void __launch_bounds__(128) attention_tc_kernel(
     const float* __restrict__ q, int q_pitch, const float* __restrict__ k, int k_pitch,
     const float* __restrict__ v, int v_pitch, float* __restrict__ o, int o_pitch,
-    int Lq, int Lk, float qscale /* d^-0.5 * log2(e) */) {
+    int Lq, int Lk, float qscale /* d^-0.5 * log2(e) */, const uint8_t* __restrict__ kpm) {
   using Cf = AtCfg<D>;
   extern __shared__ uint8_t at_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -200,7 +203,11 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
     for (int i = 0; i < AT_BK / 8; ++i)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        if (j0 + 8 * i + cq + (e & 1) >= Lk) s[4 * i + e] = -INFINITY;
+        const int key = j0 + 8 * i + cq + (e & 1);
+        if (key >= Lk) s[4 * i + e] = -INFINITY;
+        if constexpr (MASK) {
+          if (key < Lk && kpm[(long)n * Lk + key]) s[4 * i + e] = -INFINITY;
+        }
         mb[e >> 1] = fmaxf(mb[e >> 1], s[4 * i + e]);
       }
     float alpha[2], m_new[2];
@@ -211,6 +218,9 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
       m_new[rr] = fmaxf(m_run[rr], mb[rr]);
       alpha[rr] = (m_run[rr] == -INFINITY) ? 0.f : exp2f(m_run[rr] - m_new[rr]);
       m_run[rr] = m_new[rr];
+      if constexpr (MASK) {
+        if (m_new[rr] == -INFINITY) m_new[rr] = 0.f;     // every key so far is padding: p = exp2(-inf) = 0, not NaN
+      }
     }
     float lsum[2] = {0.f, 0.f};
 #pragma unroll
@@ -260,7 +270,8 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const int qi = q0 + r + 8 * rr;
     if (qi >= Lq) continue;
-    const float inv = 1.f / l;
+    float inv = 1.f / l;
+    if constexpr (MASK) inv = l > 0.f ? inv : 0.f;      // all keys padding: zeros
     float* op = o + ((long)n * Lq + qi) * o_pitch + h * D;
 #pragma unroll
     for (int i = 0; i < Cf::DP / 8; ++i) {
@@ -270,32 +281,34 @@ __global__ void __launch_bounds__(128) attention_tc_kernel(
   }
 }
 
-template <int D>
+template <int D, bool MASK>
 void launch_at(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, float* o, int o_pitch,
-               int N, int heads, int Lq, int Lk, cudaStream_t st) {
+               int N, int heads, int Lq, int Lk, const uint8_t* kpm, cudaStream_t st) {
   using Cf = AtCfg<D>;
   const size_t smem = Cf::TOTAL + 1024;
   static bool done[64] = {false};
   int dev = 0;
   AGPT_CUDA(cudaGetDevice(&dev));
   if (!done[dev & 63]) {
-    AGPT_CUDA(cudaFuncSetAttribute(attention_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    AGPT_CUDA(cudaFuncSetAttribute(attention_tc_kernel<D, MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     done[dev & 63] = true;
   }
   const float qscale = (1.0f / sqrtf((float)D)) * 1.4426950408889634f;     // dim_head ** -0.5 (attention.py:158), in log2 units
   dim3 grid(cdiv(Lq, AT_ROWS), heads, N);
-  attention_tc_kernel<D><<<grid, 128, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, qscale);
+  attention_tc_kernel<D, MASK><<<grid, 128, smem, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, qscale, kpm);
 }
 
 }  // namespace
 
 // returns false when the head dim / alignment is not supported (caller uses the fp32 kernel)
 bool attention_tc(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st) {
+                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st, const uint8_t* kpm) {
   if ((q_pitch | k_pitch | v_pitch | o_pitch) % 4 != 0) return false;
   if (((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
         reinterpret_cast<uintptr_t>(o)) & 15) != 0) return false;
-#define AGPT_ATC(D_) launch_at<D_>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, Lq, Lk, st)
+#define AGPT_ATC(D_)                                                                                   \
+  (kpm ? launch_at<D_, true>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, Lq, Lk, kpm, st) \
+       : launch_at<D_, false>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, Lq, Lk, nullptr, st))
   switch (d) {
     case 8: AGPT_ATC(8); break;
     case 16: AGPT_ATC(16); break;
@@ -303,6 +316,7 @@ bool attention_tc(const float* q, int q_pitch, const float* k, int k_pitch, cons
     case 40: AGPT_ATC(40); break;
     case 64: AGPT_ATC(64); break;
     case 80: AGPT_ATC(80); break;
+    case 128: AGPT_ATC(128); break;
     default: return false;
   }
 #undef AGPT_ATC

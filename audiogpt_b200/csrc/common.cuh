@@ -125,6 +125,7 @@ constexpr uint32_t kMagicDiffnet = 0x44494646;  // 'DIFF'
 constexpr uint32_t kMagicUnet = 0x554e4554;     // 'UNET'
 constexpr uint32_t kMagicVae = 0x56414544;      // 'VAED'
 constexpr uint32_t kMagicPe = 0x50495443;       // 'PITC'
+constexpr uint32_t kMagicFs2 = 0x46533220;      // 'FS2 '
 
 // ---- small device functions --------------------------------------------------
 __device__ __forceinline__ float lrelu(float x, float a) { return x > 0.f ? x : a * x; }

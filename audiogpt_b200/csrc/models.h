@@ -45,6 +45,13 @@ Handle* pe_create(const agpt_pe_cfg* cfg, const float* const* W, int nW, int dev
 void pe_forward(Handle* h, const float* mel, int B, int T, float* pitch_pred, float* f0, int use_uv, int norm_mode,
                 float f0_mean, float f0_std, cudaStream_t st);
 
+Handle* fs2_create(const agpt_fs2_cfg* cfg, const float* const* W, int nW, int device);
+void fs2_encode(Handle* h, const int* tok, int B, int T, const int* pmidi, const float* mdur, const int* slur, int predict, float* dur,
+                int* dur_choice, int* mel_len_host, cudaStream_t st);
+void fs2_decode(Handle* h, int Tm, const int* mel2ph_in, int* mel2ph_out, const float* f0, const float* uv, const float* energy, int use_uv,
+                int norm, float f0_mean, float f0_std, float* pitch_pred, float* f0d, int* coarse, float* e_pred, float* dec_inp, float* mel,
+                cudaStream_t st);
+
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                    int check, double* out, double* dbg_avg, double x_scale = 1.0, double w_spread = 1.0, double* rel2 = nullptr);
 

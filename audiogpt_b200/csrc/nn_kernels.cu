@@ -174,11 +174,13 @@ void layernorm(const float* x, float* y, const float* gamma, const float* beta, 
 // softmax_j(q_i . k_j * scale) v_j, heads outermost in the channel dim ('b n (h d)').
 // Two lanes share one query row (each holds half of the head dim); K/V tiles of 32 keys
 // are staged in shared memory and read as warp-wide broadcasts.
-template <int DH>
+// MASK: kpm [N][Lk] bytes, 1 = padding key; a query whose keys are all padding gets zeros (last parameter, unread
+// without MASK)
+template <int DH, bool MASK>
 __global__ void __launch_bounds__(128) attention_kernel(
     const float* __restrict__ q, int q_pitch, const float* __restrict__ k, int k_pitch,
     const float* __restrict__ v, int v_pitch, float* __restrict__ o, int o_pitch,
-    int Lq, int Lk, float scale) {
+    int Lq, int Lk, float scale, const uint8_t* __restrict__ kpm) {
   constexpr int D = 2 * DH, KT = 32;
   __shared__ __align__(16) float Ks[KT][D];
   __shared__ __align__(16) float Vs[KT][D];
@@ -225,11 +227,17 @@ __global__ void __launch_bounds__(128) attention_kernel(
       }
       d += __shfl_xor_sync(0xffffffffu, d, 1);
       if (j0 + j >= Lk) d = -INFINITY;
+      if constexpr (MASK) {
+        if (j0 + j < Lk && kpm[(long)n * Lk + j0 + j]) d = -INFINITY;
+      }
       s[j] = d;
       tmax = fmaxf(tmax, d);
     }
-    const float mn = fmaxf(m, tmax);
+    float mn = fmaxf(m, tmax);
     const float corr = (m == -INFINITY) ? 0.f : expf(m - mn);
+    if constexpr (MASK) {
+      if (mn == -INFINITY) { m = mn; continue; }     // every key so far is padding: nothing to accumulate
+    }
     l *= corr;
 #pragma unroll
     for (int c = 0; c < DH; ++c) acc[c] *= corr;
@@ -247,7 +255,8 @@ __global__ void __launch_bounds__(128) attention_kernel(
     m = mn;
   }
   if (valid) {
-    const float inv = 1.f / l;
+    float inv = 1.f / l;
+    if constexpr (MASK) inv = l > 0.f ? inv : 0.f;     // all keys padding: zeros
     float* op = o + ((long)n * Lq + qi) * o_pitch + h * D + half * DH;
 #pragma unroll
     for (int c = 0; c < DH; c += 4)
@@ -263,12 +272,14 @@ bool attention_tc_enabled() {
 }
 
 void attention(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st) {
+               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st, const uint8_t* kpm) {
   // tensor-core path (QK^T and PV on wgmma, attention_tc.cu); the fp32 kernel below is the A/B reference
-  if (attention_tc_enabled() && attention_tc(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, d, Lq, Lk, st)) return;
+  if (attention_tc_enabled() && attention_tc(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, N, heads, d, Lq, Lk, st, kpm)) return;
   const float scale = 1.0f / sqrtf((float)d);   // dim_head ** -0.5  (attention.py:158)
   dim3 grid(cdiv(Lq, 64), heads, N);
-#define AGPT_ATT(DH_) attention_kernel<DH_><<<grid, 128, 0, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, scale)
+#define AGPT_ATT(DH_)                                                                                                     \
+  (kpm ? attention_kernel<DH_, true><<<grid, 128, 0, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, scale, kpm) \
+       : attention_kernel<DH_, false><<<grid, 128, 0, st>>>(q, q_pitch, k, k_pitch, v, v_pitch, o, o_pitch, Lq, Lk, scale, nullptr))
   switch (d) {
     case 8: AGPT_ATT(4); break;
     case 16: AGPT_ATT(8); break;
@@ -276,7 +287,8 @@ void attention(const float* q, int q_pitch, const float* k, int k_pitch, const f
     case 40: AGPT_ATT(20); break;
     case 64: AGPT_ATT(32); break;
     case 80: AGPT_ATT(40); break;
-    default: throw Error("attention: unsupported head dim " + std::to_string(d) + " (supported: 8,16,32,40,64,80)");
+    case 128: AGPT_ATT(64); break;
+    default: throw Error("attention: unsupported head dim " + std::to_string(d) + " (supported: 8,16,32,40,64,80,128)");
   }
 #undef AGPT_ATT
   count_launch(1);

@@ -13,14 +13,15 @@ size_t groupnorm_scratch_doubles(int N, int C);
 // phi / plo given: the result is written as fp16 hi/lo operand planes [rows][C] INSTEAD of the fp32 tensor y
 void layernorm(const float* x, float* y, const float* gamma, const float* beta, long rows, int C, float eps,
                cudaStream_t st, __half* phi = nullptr, __half* plo = nullptr);
+// kpm: optional key-padding mask [N][Lk] bytes (1 = padding key); a query whose keys are all padding gets zeros
 void attention(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st);
+               float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st, const uint8_t* kpm = nullptr);
 void transpose_pad(const float* in, int in_pitch, int rows, int cols, float* out, int rows_pad, cudaStream_t st);
 void copy_pad_rows(const float* in, int in_pitch, int rows, int cols, float* out, int rows_pad, cudaStream_t st);
 void softmax_rows(float* x, int pitch, long rows, int cols, float scale, cudaStream_t st);
 // tensor-core version (attention_tc.cu); false = unsupported head dim / alignment
 bool attention_tc(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
-                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st);
+                  float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk, cudaStream_t st, const uint8_t* kpm = nullptr);
 void attention_set_tc(int on);
 bool attention_tc_enabled();   // 1 (default) wgmma kernel, 0 fp32 kernel, -1 environment (AGPT_ATTN_TC)
 void timestep_embedding(float* out, const int* t_host, int N, int dim, cudaStream_t st);

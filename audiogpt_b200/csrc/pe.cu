@@ -10,6 +10,7 @@
 #include "tapconv.cuh"
 #include "nn_kernels.h"
 #include "models.h"
+#include "fs_layers.cuh"
 
 namespace agpt {
 
@@ -23,40 +24,6 @@ __global__ void pe_mask_kernel(const float* __restrict__ mel, float* __restrict_
 #pragma unroll
   for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) mask[r] = s == 0.f ? 0.f : 1.f;
-}
-// x[r][c] = (x[r][c] * a[c] + b[c]) * mask[r]   (BatchNorm1d in eval mode, then the non-padding mask; a / b may be null)
-__global__ void pe_affine_mask_kernel(float* __restrict__ x, const float* __restrict__ a, const float* __restrict__ b,
-                                      const float* __restrict__ mask, long total, int C) {
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const long r = i / C;
-    const int c = (int)(i - r * C);
-    float v = x[i];
-    if (a) v = v * a[c] + b[c];
-    x[i] = v * mask[r];
-  }
-}
-// positions = cumsum(x[..., 0] != 0) * (x[..., 0] != 0)  (padding_idx 0), then x += alpha * [sin(pos f_i) | cos(pos f_i)]
-__global__ void pe_positions_kernel(const float* __restrict__ x, int* __restrict__ pos, int T, int C) {
-  if (threadIdx.x != 0) return;                       // one sequential scan per utterance (T <= a few thousand frames)
-  const int b = blockIdx.x;
-  int run = 0;
-  for (int t = 0; t < T; ++t) {
-    const bool nz = x[((long)b * T + t) * C] != 0.f;
-    run += nz ? 1 : 0;
-    pos[(long)b * T + t] = nz ? run : 0;
-  }
-}
-__global__ void pe_posemb_add_kernel(float* __restrict__ x, const int* __restrict__ pos, float alpha, long total, int C, float neg_emb) {
-  const int half = C / 2;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const long r = i / C;
-    const int c = (int)(i - r * C);
-    const int p = pos[r];
-    if (p == 0 || c >= 2 * half) continue;              // the padding row of the table is zero; odd dims pad with a zero column
-    const int k = c < half ? c : c - half;
-    const float a = (float)p * expf((float)k * neg_emb);
-    x[i] += alpha * (c < half ? sinf(a) : cosf(a));
-  }
 }
 // pred4 [rows][4] (channels 0, 1 used) -> pitch_pred [rows][2], f0 [rows] = denorm_f0(pred[..., 0], pred[..., 1] > 0, padding)
 __global__ void pe_denorm_kernel(const float* __restrict__ pred4, const float* __restrict__ mask, float* __restrict__ pitch_pred,
@@ -75,20 +42,12 @@ __global__ void pe_denorm_kernel(const float* __restrict__ pred4, const float* _
 
 struct PeNet : Handle {
   agpt_pe_cfg cfg;
-  PackedConv pre_conv[3], pre_out, enc_in, enc_out, lin;
+  PackedConv pre_conv[3], pre_out, enc_in, enc_out;
   DevBuf bn_a[3], bn_b[3];
-  std::vector<PackedConv> enc_conv, pp_conv;
-  std::vector<DevBuf> enc_g, enc_b, pp_g, pp_b;
-  float alpha = 1.f;
-  DevBuf mask, buf[3], pos, pred4;
-
-  void conv(const PackedConv& pc, const float* in, int cin, float* out, int cout_pitch, int B, int T, int epi, cudaStream_t st) {
-    TapConvParams P = tapconv_params(pc, B, T, 0, 1);
-    P.in = in; P.in_gstride = (long)T * cin; P.in_pitch = cin;
-    P.out = out; P.out_gstride = (long)T * cout_pitch; P.out_pitch = cout_pitch;
-    P.epi = epi;
-    tapconv_launch(P, st);
-  }
+  std::vector<PackedConv> enc_conv;
+  std::vector<DevBuf> enc_g, enc_b;
+  PitchPredictorNet pp;
+  DevBuf mask, buf[4], pred4;
 
   void forward(const float* mel, int B, int T, float* pitch_pred, float* f0, int use_uv, int norm_mode, float f0_mean, float f0_std,
                cudaStream_t st) {
@@ -96,50 +55,36 @@ struct PeNet : Handle {
     const int H = cfg.hidden_size, P_ = cfg.predictor_hidden, M = cfg.n_mel_bins;
     const long rows = (long)B * T;
     const int Cmax = std::max(H, P_);
-    mask.ensure(rows); pos.ensure(rows); pred4.ensure(rows * 4);
+    mask.ensure(rows); pred4.ensure(rows * 4);
     for (auto& b : buf) b.ensure((size_t)rows * Cmax);
     float *x = buf[0].p, *y = buf[1].p, *z = buf[2].p;
-    const unsigned eg = (unsigned)std::min<long>(cdivl(rows * Cmax, 256), 2368);
     pe_mask_kernel<<<(unsigned)cdivl(rows, 8), 256, 0, st>>>(mel, mask.p, rows, M);
     count_launch(1);
     // ---- Prenet (pe.py:23-42): 3 x [Conv1d k5 -> ReLU -> BatchNorm1d(eval) -> x mask], out_proj, x mask
     const float* in = mel;
     int cin = M;
     for (int l = 0; l < 3; ++l) {
-      conv(pre_conv[l], in, cin, x, H, B, T, EPI_RELU, st);
-      pe_affine_mask_kernel<<<eg, 256, 0, st>>>(x, bn_a[l].p, bn_b[l].p, mask.p, rows * H, H);
-      count_launch(1);
+      fs_conv(pre_conv[l], in, cin, x, H, B, T, EPI_RELU, st);
+      fs_affine_mask(x, bn_a[l].p, bn_b[l].p, mask.p, rows, H, st);
       std::swap(x, y);
       in = y; cin = H;
     }
-    conv(pre_out, in, H, x, H, 1, (int)rows, EPI_BIAS, st);
-    pe_affine_mask_kernel<<<eg, 256, 0, st>>>(x, nullptr, nullptr, mask.p, rows * H, H);
-    count_launch(1);
+    fs_conv(pre_out, in, H, x, H, 1, (int)rows, EPI_BIAS, st);
+    fs_affine_mask(x, nullptr, nullptr, mask.p, rows, H, st);
     // ---- ConvStacks (pe.py:98-116): in_proj, n x [x + ReLU(GroupNorm(C/16 groups)(ConvNorm k5 (x)))], out_proj
     if (!enc_conv.empty()) {
-      conv(enc_in, x, H, y, H, 1, (int)rows, EPI_BIAS, st);
+      fs_conv(enc_in, x, H, y, H, 1, (int)rows, EPI_BIAS, st);
       std::swap(x, y);
       for (size_t l = 0; l < enc_conv.size(); ++l) {
-        conv(enc_conv[l], x, H, y, H, B, T, EPI_BIAS, st);
+        fs_conv(enc_conv[l], x, H, y, H, B, T, EPI_BIAS, st);
         groupnorm_ex(y, z, enc_g[l].p, enc_b[l].p, B, T, H, H / 16, 1e-5f, 2, x, st);
         std::swap(x, z);
       }
-      conv(enc_out, x, H, y, H, 1, (int)rows, EPI_BIAS, st);
+      fs_conv(enc_out, x, H, y, H, 1, (int)rows, EPI_BIAS, st);
       std::swap(x, y);
     }
     // ---- PitchPredictor (tts_modules.py:247-260)
-    pe_positions_kernel<<<B, 32, 0, st>>>(x, reinterpret_cast<int*>(pos.p), T, H);
-    const float neg_emb = (float)(-(std::log(10000.0) / (double)(H / 2 - 1)));
-    pe_posemb_add_kernel<<<eg, 256, 0, st>>>(x, reinterpret_cast<const int*>(pos.p), alpha, rows * H, H, neg_emb);
-    count_launch(2);
-    cin = H;
-    for (size_t l = 0; l < pp_conv.size(); ++l) {
-      conv(pp_conv[l], x, cin, y, P_, B, T, EPI_RELU, st);
-      layernorm(y, z, pp_g[l].p, pp_b[l].p, rows, P_, 1e-5f, st);
-      std::swap(x, z);
-      cin = P_;
-    }
-    conv(lin, x, P_, pred4.p, 4, 1, (int)rows, EPI_BIAS, st);
+    pp.forward(x, H, B, T, y, z, buf[3].p, pred4.p, st);
     pe_denorm_kernel<<<(unsigned)std::min<long>(cdivl(rows, 256), 1184), 256, 0, st>>>(pred4.p, mask.p, pitch_pred, f0, rows, use_uv,
                                                                                    norm_mode, f0_mean, f0_std);
     count_launch(1);
@@ -181,22 +126,7 @@ Handle* pe_create(const agpt_pe_cfg* cfg, const float* const* W, int nW, int dev
     { auto w = next(); auto b = next(); pack_conv(h->enc_in, w, b, H, H, 1, false); }
     { auto w = next(); auto b = next(); pack_conv(h->enc_out, w, b, H, H, 1, false); }
   }
-  h->alpha = next()[0];
-  h->pp_conv.resize(cfg->predictor_layers); h->pp_g.resize(cfg->predictor_layers); h->pp_b.resize(cfg->predictor_layers);
-  cin = H;
-  for (int l = 0; l < cfg->predictor_layers; ++l) {
-    { auto w = next(); auto b = next(); pack_conv(h->pp_conv[l], w, b, P, cin, k, false); }
-    { auto g = next(); auto b = next(); up_(h->pp_g[l], g, P); up_(h->pp_b[l], b, P); }
-    cin = P;
-  }
-  {  // Linear(P -> 2), padded to 4 output channels so that rows stay float4-addressable
-    auto w = next(); auto b = next();
-    std::vector<float> wp((size_t)4 * P, 0.f), bp(4, 0.f);
-    memcpy(wp.data(), w, sizeof(float) * 2 * P);
-    bp[0] = b[0]; bp[1] = b[1];
-    pack_conv(h->lin, wp.data(), bp.data(), 4, P, 1, false);
-  }
-  next();                              // pitch_predictor.embed_positions._float_tensor (a device marker buffer)
+  h->pp.load(next, H, P, k, cfg->predictor_layers, 2);
   AGPT_CHECK(idx == nW, "weight array count does not match the config");
   return h;
 }

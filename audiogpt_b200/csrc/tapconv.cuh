@@ -41,6 +41,7 @@ enum Epi : int {
   EPI_TANH = 9,     // tanh(v + bias)
   EPI_MISH = 10,    // mish(v + bias) = x * tanh(softplus(x))   (NeuralSeq/modules/diff/diffusion.py:68-70)
   EPI_SILU = 11,    // silu(v + bias)
+  EPI_GELU_SCALED = 12,   // gelu_erf(scale * (v + bias))   (TransformerFFNLayer: conv * k^-0.5, then F.gelu)
 };
 
 struct TapConvParams {

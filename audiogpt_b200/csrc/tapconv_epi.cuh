@@ -102,6 +102,9 @@ __device__ __forceinline__ void epi_store_cv(const TapConvParams& P, int g, int 
     case EPI_SILU:
       v.x = siluf_(v.x); v.y = siluf_(v.y); v.z = siluf_(v.z); v.w = siluf_(v.w);
       break;
+    case EPI_GELU_SCALED:
+      v.x = gelu_erf(v.x * P.scale); v.y = gelu_erf(v.y * P.scale); v.z = gelu_erf(v.z * P.scale); v.w = gelu_erf(v.w * P.scale);
+      break;
     case EPI_ADDVEC: break;   // the vector is part of cv
     case EPI_GATE:
     case EPI_GEGLU: {

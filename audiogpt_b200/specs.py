@@ -597,3 +597,148 @@ def synth_diffnet(cfg, seed: int = 2024):
 
 def synth_unet(cfg, seed: int = 4040):
     return synth_state_dict(unet_param_shapes(cfg), seed)
+
+
+# ---------------------------------------------------------------------------------------------- FastSpeech2 / FastSpeech2MIDI
+# hidden 64, 2 heads (head dim 32), every optional branch of the frame path on: pitch 'frame' + energy
+FS2_SMALL = dict(hidden_size=64, num_heads=2, enc_layers=2, dec_layers=2, enc_ffn_kernel=9, dec_ffn_kernel=9, n_tokens=40,
+                 out_dims=80, predictor_hidden=64, dur_predictor_layers=2, dur_predictor_kernel=3, predictor_layers=2,
+                 predictor_kernel=5, use_pos_embed=1, rel_pos=0, pitch_type="frame", use_energy_embed=1, use_midi=0)
+# egs/egs_bases/tts/fs2.yaml (BASELINE config C2): hidden 256, 2 heads, 4 + 4 FFT layers, pitch 'frame' (standard norm, uv)
+FS2_C2 = dict(FS2_SMALL, hidden_size=256, enc_layers=4, dec_layers=4, n_tokens=80, predictor_hidden=256, use_energy_embed=0)
+# configs/tts/fs2.yaml: pitch 'ph' with log norm
+FS2_PH = dict(FS2_C2, pitch_type="ph")
+# egs/egs_bases/svs/midi/e2e/opencpop/ds1000.yaml (AudioGPT's text-to-singing tool): MIDI encoder, rel_pos, no pitch embedding,
+# 5-layer duration / pitch predictors
+FS2_DS1000 = dict(FS2_C2, rel_pos=1, pitch_type=None, dur_predictor_layers=5, predictor_layers=5, use_midi=1)
+
+
+def _fft_shapes(s, p, H, L, k):
+    for i in range(L):
+        q = f"{p}.layers.{i}.op"
+        s[f"{q}.layer_norm1.weight"] = (H,); s[f"{q}.layer_norm1.bias"] = (H,)
+        s[f"{q}.self_attn.in_proj_weight"] = (3 * H, H)
+        s[f"{q}.self_attn.out_proj.weight"] = (H, H)
+        s[f"{q}.layer_norm2.weight"] = (H,); s[f"{q}.layer_norm2.bias"] = (H,)
+        s[f"{q}.ffn.ffn_1.weight"] = (4 * H, H, k); s[f"{q}.ffn.ffn_1.bias"] = (4 * H,)
+        s[f"{q}.ffn.ffn_2.weight"] = (H, 4 * H); s[f"{q}.ffn.ffn_2.bias"] = (H,)
+    s[f"{p}.layer_norm.weight"] = (H,); s[f"{p}.layer_norm.bias"] = (H,)
+
+
+def _predictor_shapes(s, p, H, P, k, layers, odim):
+    s[f"{p}.pos_embed_alpha"] = (1,)
+    cin = H
+    for l in range(layers):
+        s[f"{p}.conv.{l}.1.weight"] = (P, cin, k); s[f"{p}.conv.{l}.1.bias"] = (P,)
+        s[f"{p}.conv.{l}.3.weight"] = (P,); s[f"{p}.conv.{l}.3.bias"] = (P,)
+        cin = P
+    s[f"{p}.linear.weight"] = (odim, P); s[f"{p}.linear.bias"] = (odim,)
+    s[f"{p}.embed_positions._float_tensor"] = (1,)
+
+
+def fs2_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of NeuralSeq/modules/fastspeech/fs2.py:22-72 FastSpeech2 (FastspeechEncoder /
+    FastspeechDecoder of EncSALayers, DurationPredictor, Pitch / EnergyPredictor) and, with use_midi, of
+    modules/diffsinger_midi/fs2.py:46-53 FastSpeech2MIDI.  The shared token embedding appears under both of its names.
+    The order is the one agpt_fs2_create consumes (strict load_state_dict does not depend on it)."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    H, P = int(cfg["hidden_size"]), int(cfg["predictor_hidden"])
+    s["encoder_embed_tokens.weight"] = (int(cfg["n_tokens"]), H)
+    s["encoder.embed_tokens.weight"] = (int(cfg["n_tokens"]), H)
+    if not cfg["rel_pos"]:
+        s["encoder.embed_positions._float_tensor"] = (1,)
+    _fft_shapes(s, "encoder", H, int(cfg["enc_layers"]), int(cfg["enc_ffn_kernel"]))
+    s["decoder.pos_embed_alpha"] = (1,)
+    s["decoder.embed_positions._float_tensor"] = (1,)
+    _fft_shapes(s, "decoder", H, int(cfg["dec_layers"]), int(cfg["dec_ffn_kernel"]))
+    s["mel_out.weight"] = (int(cfg["out_dims"]), H); s["mel_out.bias"] = (int(cfg["out_dims"]),)
+    cin = H
+    for l in range(int(cfg["dur_predictor_layers"])):
+        s[f"dur_predictor.conv.{l}.1.weight"] = (P, cin, int(cfg["dur_predictor_kernel"]))
+        s[f"dur_predictor.conv.{l}.1.bias"] = (P,)
+        s[f"dur_predictor.conv.{l}.3.weight"] = (P,); s[f"dur_predictor.conv.{l}.3.bias"] = (P,)
+        cin = P
+    s["dur_predictor.linear.weight"] = (1, P); s["dur_predictor.linear.bias"] = (1,)
+    k, nl = int(cfg["predictor_kernel"]), int(cfg["predictor_layers"])
+    if cfg["pitch_type"]:
+        s["pitch_embed.weight"] = (300, H)
+        _predictor_shapes(s, "pitch_predictor", H, P, k, nl, 2 if cfg["pitch_type"] == "frame" else 1)
+    if cfg["use_energy_embed"]:
+        s["energy_embed.weight"] = (256, H)
+        _predictor_shapes(s, "energy_predictor", H, P, k, nl, 1)
+    if cfg["use_midi"]:
+        s["midi_embed.weight"] = (300, H)
+        s["midi_dur_layer.weight"] = (H, 1); s["midi_dur_layer.bias"] = (H,)
+        s["is_slur_embed.weight"] = (2, H)
+    return s
+
+
+def synth_fs2(cfg, seed: int = 808):
+    """Seeded FastSpeech2 weights with realistic operating points: the duration Linear gives exp(xs) - 1 of about 4-8
+    frames per token (else mel2ph is empty), the energy Linear a positive energy (the reference indexes its embedding
+    with it), the 'ph' pitch Linear log2 F0 around 7.5 (about 180 Hz).  Padding rows of the token embedding are zero, as
+    Embedding(padding_idx=0) initialises them, and both names of the shared embedding hold the same tensor."""
+    shapes = fs2_param_shapes(cfg)
+    sd = synth_state_dict(shapes, seed, convtranspose_prefixes=())
+    emb = sd["encoder_embed_tokens.weight"].clone()
+    emb[0] = 0
+    sd["encoder_embed_tokens.weight"] = emb
+    sd["encoder.embed_tokens.weight"] = emb
+    for k in sd:
+        if k.endswith("pos_embed_alpha"):
+            sd[k] = torch.tensor([0.7])
+        elif k.endswith("_float_tensor"):
+            sd[k] = torch.zeros(1)
+    sd["dur_predictor.linear.weight"] = sd["dur_predictor.linear.weight"] * 0.3
+    sd["dur_predictor.linear.bias"] = torch.tensor([1.9])
+    if cfg["use_energy_embed"]:
+        sd["energy_predictor.linear.weight"] = sd["energy_predictor.linear.weight"] * 0.3
+        sd["energy_predictor.linear.bias"] = torch.tensor([2.0])
+    if cfg["pitch_type"] == "ph":
+        sd["pitch_predictor.linear.weight"] = sd["pitch_predictor.linear.weight"] * 0.3
+        sd["pitch_predictor.linear.bias"] = torch.tensor([7.5])
+    return sd
+
+
+def fs2_hparams(cfg):
+    """The hparams a reference FastSpeech2 / FastSpeech2MIDI of this engine config is built from (the shipped configs'
+    values for everything the config does not vary)."""
+    return dict(hidden_size=cfg["hidden_size"], num_heads=cfg["num_heads"], enc_layers=cfg["enc_layers"],
+                dec_layers=cfg["dec_layers"], enc_ffn_kernel_size=cfg["enc_ffn_kernel"], dec_ffn_kernel_size=cfg["dec_ffn_kernel"],
+                audio_num_mel_bins=cfg["out_dims"], predictor_hidden=cfg["predictor_hidden"],
+                dur_predictor_layers=cfg["dur_predictor_layers"], dur_predictor_kernel=cfg["dur_predictor_kernel"],
+                predictor_layers=cfg["predictor_layers"], predictor_kernel=cfg["predictor_kernel"],
+                use_pos_embed=bool(cfg["use_pos_embed"]), rel_pos=bool(cfg["rel_pos"]), encoder_type="fft", decoder_type="fft",
+                ffn_act="gelu", ffn_padding="SAME", dur_loss="mse", use_spk_id=False, use_spk_embed=False, use_split_spk_id=False,
+                num_spk=1, dropout=0.1, predictor_dropout=0.5, predictor_grad=0.1, use_pitch_embed=cfg["pitch_type"] is not None,
+                pitch_type=cfg["pitch_type"] or "frame", use_uv=True, pitch_norm="log" if cfg["pitch_type"] == "ph" else "standard",
+                f0_mean=220.0, f0_std=60.0, use_energy_embed=bool(cfg["use_energy_embed"]), pitch_ar=False,
+                use_midi=bool(cfg["use_midi"]))
+
+
+class TokenDictionary:
+    """The two methods FastSpeech2.__init__ reads from its phone encoder: len() and pad() (= 0)."""
+
+    def __init__(self, n):
+        self.n = int(n)
+
+    def __len__(self):
+        return self.n
+
+    def pad(self):
+        return 0
+
+
+def synth_fs2_inputs(cfg, B, T, seed):
+    """Ragged token batch with a padded tail: lengths T, T - 3, T // 2 (cycled), ids in [1, n_tokens); MIDI inputs
+    (pitch_midi 40..79, midi_dur 0.1..1.0 s, is_slur) zero on padding.  CPU tensors."""
+    g = torch.Generator().manual_seed(int(seed))
+    lens = [(T, T - 3, T // 2)[i % 3] for i in range(B)]
+    valid = torch.arange(T)[None, :] < torch.tensor(lens)[:, None]
+    tok = torch.randint(1, int(cfg["n_tokens"]), (B, T), generator=g) * valid
+    out = dict(txt_tokens=tok)
+    if cfg["use_midi"]:
+        out["pitch_midi"] = torch.randint(40, 80, (B, T), generator=g) * valid
+        out["midi_dur"] = (0.1 + 0.9 * torch.rand((B, T), generator=g)) * valid
+        out["is_slur"] = torch.randint(0, 2, (B, T), generator=g) * valid
+    return out

@@ -50,6 +50,12 @@ int agpt_set_tensor_cores(int on);
 int agpt_attention(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, float* o,
                    int o_pitch, int N, int heads, int d, int Lq, int Lk, void* stream);
 int agpt_set_attention_tc(int on);
+/* Same with a key-padding mask (fairseq MultiheadAttention's key_padding_mask, modules/commons/common_layers.py:235-364):
+ * key_padding_mask [N][Lk] bytes, 1 = padding key (need not be a suffix).  d in {8,16,32,40,64,80,128}.  A query whose
+ * keys are all padding gets zeros (the reference gets NaN there).                                                 */
+int agpt_attention_masked(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
+                          const uint8_t* key_padding_mask, float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk,
+                          void* stream);
 /* Micro-benchmark of one tapconv layer (random data): out3 = {ms per launch, algorithmic TFLOP/s,
  * max |tensor-core - fp32 FMA| when check != 0}; dbg8 (tensor-core kernel only) = average per-CTA phase cycles
  * {setup, first activation tile, MMA issue loop, drain, epilogue, total, wait-on-activations,
@@ -250,6 +256,44 @@ int agpt_pe_create(const agpt_pe_cfg* cfg, const float* const* host_weights, int
  * all-zero mel frames (padding) give F0 = 0.                                                                      */
 int agpt_pe_forward(agpt_handle h, const float* mel, int B, int T, float* pitch_pred, float* f0_denorm, int use_uv,
                     int pitch_norm, float f0_mean, float f0_std, void* stream);
+
+/* ------------------------------------------------------------------ FastSpeech2 / FastSpeech2MIDI
+ * Replaces FastSpeech2.forward (NeuralSeq/modules/fastspeech/fs2.py:79-226) and FastSpeech2MIDI.forward
+ * (modules/diffsinger_midi/fs2.py:55-118) for encoder_type = decoder_type = 'fft', ffn_act 'gelu', ffn_padding 'SAME',
+ * dur_loss 'mse', no speaker conditioning: the acoustic front-end of the TTS and text-to-singing paths.           */
+typedef struct {
+  int hidden_size, num_heads;
+  int enc_layers, dec_layers;
+  int enc_ffn_kernel, dec_ffn_kernel;
+  int n_tokens;                /* len(dictionary) */
+  int out_dims;                /* audio_num_mel_bins */
+  int predictor_hidden;        /* resolved: hparams['predictor_hidden'] or hidden_size */
+  int dur_predictor_layers, dur_predictor_kernel;
+  int predictor_layers, predictor_kernel;
+  int use_pos_embed;           /* encoder positions (the decoder always has them) */
+  int rel_pos;                 /* 0: fairseq sinusoidal table; 1: espnet RelPositionalEncoding (x * sqrt(H) + pe) */
+  int pitch_type;              /* 0: use_pitch_embed off; 1: 'frame'; 2: 'ph' */
+  int use_energy_embed;
+  int use_midi;                /* FastSpeech2MIDI: midi_embed / midi_dur_layer / is_slur_embed in the encoder input */
+} agpt_fs2_cfg;
+/* host_weights: fp32 HOST arrays in the key order of audiogpt_b200.specs.fs2_param_shapes(cfg) (both names of the shared
+ * token embedding and the _float_tensor marker buffers are passed; the duplicates and markers are ignored).       */
+int agpt_fs2_create(const agpt_fs2_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* Token side: txt_tokens [B][T_txt] int32 (0 = padding); pitch_midi / is_slur int32 and midi_dur fp32 [B][T_txt] (MIDI
+ * model; midi_dur / is_slur may be NULL).  dur [B][T_txt] = the duration predictor's log-domain output.  predict_dur != 0:
+ * dur_choice [B][T_txt] int32 (may be NULL) = clamp(round(exp(dur) - 1), 0), and mel_len_host [B] (HOST) = frames per
+ * utterance -- the call synchronises the stream for this one device -> host copy.  The encoder output stays in the
+ * handle for agpt_fs2_decode.                                                                                       */
+int agpt_fs2_encode(agpt_handle h, const int* txt_tokens, int B, int T_txt, const int* pitch_midi, const float* midi_dur,
+                    const int* is_slur, int predict_dur, float* dur, int* dur_choice, int* mel_len_host, void* stream);
+/* Frame side, T_mel frames: mel2ph [B][T_mel] int32 (teacher-forced) or NULL = expand the durations predicted by the last
+ * encode into mel2ph_out.  f0 / uv / energy: teacher-forced values or NULL (f0 is [B][T_txt] for pitch_type 'ph').
+ * pitch_norm 1 'standard', 2 'log'.  Outputs (device): pitch_pred ([B][T_mel][2] 'frame', [B][T_txt][1] 'ph'), f0_denorm
+ * and pitch_coarse (int32) on the same grid; energy_pred [B][T_mel]; decoder_inp [B][T_mel][H]; mel_out
+ * [B][T_mel][out_dims] or NULL to skip the decoder.                                                                */
+int agpt_fs2_decode(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out, const float* f0, const float* uv,
+                    const float* energy, int use_uv, int pitch_norm, float f0_mean, float f0_std, float* pitch_pred,
+                    float* f0_denorm, int* pitch_coarse, float* energy_pred, float* decoder_inp, float* mel_out, void* stream);
 
 #ifdef __cplusplus
 }
