@@ -9,6 +9,8 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.ldm.modules.diffusionmodules.openaimodel.UNetModel
     audiogpt_b200.ldm.models.diffusion.ddim.DDIMSampler
     audiogpt_b200.ldm.models.autoencoder.AutoencoderKL          (decode side; not installed over the reference class)
+    audiogpt_b200.ldm.models.autoencoder.AutoencoderKLWithEncoder   (whole first stage; installed as AutoencoderKL
+                                                                     with install(first_stage=True))
     audiogpt_b200.modules.fastspeech.pe.PitchExtractor
     audiogpt_b200.vocoder.bigvgan.models.BigVGAN / VocoderBigVGAN
     audiogpt_b200.modules.fastspeech.fs2.FastSpeech2                (installed with install(front_end=True))
@@ -19,7 +21,8 @@ There is no CPU fallback.
 """
 __version__ = "0.1.0"
 
-# reference module name -> (our module, attributes to graft onto the reference module)
+# reference module name -> (our module, attributes to graft onto the reference module: a list of names, or a
+# {reference name: our name} mapping)
 _INSTALL_MAP = {
     "modules.hifigan.hifigan": ("audiogpt_b200.modules.hifigan.hifigan", ["HifiGanGenerator"]),
     "vocoders.hifigan": ("audiogpt_b200.vocoders.hifigan", ["HifiGAN", "load_model"]),
@@ -37,9 +40,13 @@ _FRONT_END_MAP = {
     "modules.fastspeech.fs2": ("audiogpt_b200.modules.fastspeech.fs2", ["FastSpeech2"]),
     "modules.diffsinger_midi.fs2": ("audiogpt_b200.modules.diffsinger_midi.fs2", ["FastSpeech2MIDI"]),
 }
+# the whole first stage of the Make-An-Audio tools, grafted only on request (install(first_stage=True))
+_FIRST_STAGE_MAP = {
+    "ldm.models.autoencoder": ("audiogpt_b200.ldm.models.autoencoder", {"AutoencoderKL": "AutoencoderKLWithEncoder"}),
+}
 
 
-def install(strict: bool = False, front_end: bool = False):
+def install(strict: bool = False, front_end: bool = False, first_stage: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -51,29 +58,51 @@ def install(strict: bool = False, front_end: bool = False):
     resolve to the drop-ins.  Modules that are not importable are registered in ``sys.modules``
     as aliases of ours when ``strict`` is False.  ``front_end=True`` also replaces FastSpeech2 and
     FastSpeech2MIDI, so GaussianDiffusion's front-end (and any other user of those classes) runs on the engine.
+    ``first_stage=True`` also replaces ``ldm.models.autoencoder.AutoencoderKL`` by AutoencoderKLWithEncoder, so
+    every Make-An-Audio tool encodes and decodes its first stage on the engine, and records the reference's
+    DiagonalGaussianDistribution as the class its encode() returns.
     Returns the list of patched names."""
     import importlib
     import sys
+    import types
     patched = []
-    todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}))
+    todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}), **(_FIRST_STAGE_MAP if first_stage else {}))
     for ref_name, (our_name, attrs) in todo.items():
         ours = importlib.import_module(our_name)
+        names = attrs if isinstance(attrs, dict) else {a: a for a in attrs}
         try:
             ref = importlib.import_module(ref_name)
         except Exception:
             if strict:
                 raise
-            sys.modules.setdefault(ref_name, ours)
+            alias = ours
+            if any(a != b for a, b in names.items()):
+                # a renamed graft: the alias is a copy of our module with the reference's names bound to our classes
+                alias = types.ModuleType(ref_name, ours.__doc__)
+                alias.__dict__.update({k: v for k, v in vars(ours).items() if not k.startswith("__")})
+                for a, b in names.items():
+                    setattr(alias, a, getattr(ours, b))
+            sys.modules.setdefault(ref_name, alias)
             patched.append(ref_name + " (aliased)")
             continue
-        for a in attrs:
+        for a, b in names.items():
             theirs = getattr(ref, a, None)
-            mine = getattr(ours, a)
+            mine = getattr(ours, b)
             # configs the drop-in does not cover (e.g. the inpainting AttentionBlock UNet) keep the reference class
             if hasattr(mine, "_reference_cls") and isinstance(theirs, type) and theirs is not mine:
                 mine._reference_cls = theirs
             setattr(ref, a, mine)
         patched.append(ref_name)
+    if first_stage:
+        # get_first_stage_encoding checks isinstance(posterior, DiagonalGaussianDistribution) against the reference's
+        # own class (ddpm_audio.py:157-164): encode() must build that class when it exists
+        try:
+            dist = importlib.import_module("ldm.modules.distributions.distributions")
+            from .ldm.models.autoencoder import AutoencoderKLWithEncoder
+            AutoencoderKLWithEncoder._posterior_cls = dist.DiagonalGaussianDistribution
+        except Exception:
+            if strict:
+                raise
     # the vocoder registry of the reference keeps its own dict: register ours there too
     try:
         bv = importlib.import_module("vocoders.base_vocoder")

@@ -88,6 +88,9 @@ def lib() -> C.CDLL:
         L.agpt_launch_count.restype = C.c_longlong
         L.agpt_destroy.argtypes = [C.c_void_p]
         L.agpt_destroy.restype = None
+        L.agpt_vae_encoder_create.argtypes = [C.POINTER(VaeCfg), C.c_int, C.POINTER(C.POINTER(C.c_float)), C.c_int, C.c_int,
+                                              C.POINTER(C.c_void_p)]
+        L.agpt_vae_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         _lib = L
         return L
 

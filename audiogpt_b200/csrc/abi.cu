@@ -227,6 +227,20 @@ int agpt_vae_decode(agpt_handle h, const float* z, int B, int H, int W, float* o
   });
 }
 
+int agpt_vae_encoder_create(const agpt_vae_cfg* cfg, int in_channels, const float* const* host_weights, int n_weights,
+                            int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(vae_encoder_create(cfg, in_channels, host_weights, n_weights, device));
+  });
+}
+
+int agpt_vae_encode(agpt_handle h, const float* x, int B, int H, int W, float* moments, void* stream) {
+  return guarded([&] {
+    vae_encode(as(h, kMagicVaeEnc, "vae encoder"), x, B, H, W, moments, (cudaStream_t)stream);
+  });
+}
+
 int agpt_pe_create(const agpt_pe_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
   return guarded([&] {
     AGPT_CHECK(cfg && host_weights && out, "null argument");

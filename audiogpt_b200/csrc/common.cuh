@@ -124,6 +124,7 @@ constexpr uint32_t kMagicHifigan = 0x48494649;  // 'HIFI'
 constexpr uint32_t kMagicDiffnet = 0x44494646;  // 'DIFF'
 constexpr uint32_t kMagicUnet = 0x554e4554;     // 'UNET'
 constexpr uint32_t kMagicVae = 0x56414544;      // 'VAED'
+constexpr uint32_t kMagicVaeEnc = 0x56414545;   // 'VAEE'
 constexpr uint32_t kMagicPe = 0x50495443;       // 'PITC'
 constexpr uint32_t kMagicFs2 = 0x46533220;      // 'FS2 '
 

@@ -40,6 +40,8 @@ long unet_launches_per_step(Handle* h);
 
 Handle* vae_create(const agpt_vae_cfg* cfg, const float* const* W, int nW, int device);
 void vae_decode(Handle* h, const float* z, int B, int H, int W, float* out, cudaStream_t st);
+Handle* vae_encoder_create(const agpt_vae_cfg* cfg, int in_channels, const float* const* W, int nW, int device);
+void vae_encode(Handle* h, const float* x, int B, int H, int W, float* moments, cudaStream_t st);
 
 Handle* pe_create(const agpt_pe_cfg* cfg, const float* const* W, int nW, int device);
 void pe_forward(Handle* h, const float* mel, int B, int T, float* pitch_pred, float* f0, int use_uv, int norm_mode,

@@ -478,9 +478,11 @@ void upsample_nearest2(const float* in, float* out, int N, int H, int W, int C, 
   AGPT_CUDA(cudaGetLastError());
 }
 
-// im2col for Conv2d(k3, stride 2, pad 1): col[n][ho][wo][tap*C + c] = x[n][2ho+kh-1][2wo+kw-1][c]
+// im2col for a 3x3 stride-2 Conv2d: col[n][ho][wo][tap*C + c] = x[n][2ho+kh-pad][2wo+kw-pad][c], zero outside x.
+// pad 1: the UNet's Conv2d(k3, stride 2, padding 1); pad 0: the VAE encoder's Downsample, F.pad(x, (0,1,0,1)) then a
+// conv without padding -- the one zero row / column past the end is the same out-of-range read
 __global__ void im2col_s2_kernel(const float* __restrict__ in, float* __restrict__ col, int N, int H, int W, int C,
-                                 int Ho, int Wo) {
+                                 int Ho, int Wo, int pad) {
   pdl_wait();
   const long total = (long)N * Ho * Wo * 9 * (C / 4);
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -490,15 +492,16 @@ __global__ void im2col_s2_kernel(const float* __restrict__ in, float* __restrict
     const int wo = (int)(r % Wo); r /= Wo;
     const int ho = (int)(r % Ho);
     const int n = (int)(r / Ho);
-    const int hi = 2 * ho + tap / 3 - 1, wi = 2 * wo + tap % 3 - 1;
+    const int hi = 2 * ho + tap / 3 - pad, wi = 2 * wo + tap % 3 - pad;
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (hi >= 0 && hi < H && wi >= 0 && wi < W) v = *reinterpret_cast<const float4*>(in + (((long)n * H + hi) * W + wi) * C + c);
     *reinterpret_cast<float4*>(col + ((((long)n * Ho + ho) * Wo + wo) * 9 + tap) * C + c) = v;
   }
 }
-void im2col_stride2(const float* in, float* col, int N, int H, int W, int C, int Ho, int Wo, cudaStream_t st) {
+void im2col_stride2(const float* in, float* col, int N, int H, int W, int C, int Ho, int Wo, int pad, cudaStream_t st) {
   const long total = (long)N * Ho * Wo * 9 * (C / 4);
-  launch_pdl(im2col_s2_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, in, col, N, H, W, C, Ho, Wo);
+  launch_pdl(im2col_s2_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, in, col, N, H, W, C, Ho, Wo,
+             pad);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }

@@ -192,7 +192,7 @@ struct Unet : Handle {
         case L_DOWN: {
           const int Ho = (a.H - 1) / 2 + 1, Wo = (a.W - 1) / 2 + 1;
           float* col = alloc((size_t)N * Ho * Wo * 9 * a.C);
-          im2col_stride2(a.p, col, N, a.H, a.W, a.C, Ho, Wo, s);
+          im2col_stride2(a.p, col, N, a.H, a.W, a.C, Ho, Wo, 1, s);
           float* o = alloc((size_t)N * Ho * Wo * a.C);
           linear(down_convs[l.idx], col, 9 * a.C, o, a.C, (long)N * Ho * Wo, EPI_BIAS, nullptr, 0, s);
           a = {o, a.C, Ho, Wo};

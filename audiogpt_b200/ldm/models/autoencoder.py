@@ -1,13 +1,19 @@
-"""Drop-in for ``ldm.models.autoencoder.AutoencoderKL`` -- the DECODE side (SURVEY.md 8f row 1).
+"""Drop-ins for ``ldm.models.autoencoder.AutoencoderKL`` (SURVEY.md 8f row 1).
 
-Reference: /root/reference/text_to_audio/Make_An_Audio/ldm/models/autoencoder.py:304-354
-(``decode(z) = decoder(post_quant_conv(z))``) with ``Decoder`` from
-ldm/modules/diffusionmodules/model.py:462-568.  Same constructor keywords as the reference's
-``first_stage_config`` (``ddconfig``, ``lossconfig``, ``embed_dim``, ``ckpt_path``, ``ignore_keys``,
-``image_key``, ``colorize_nlabels``, ``monitor``), same ``decode(z)`` signature, same state-dict keys for
-what it owns (``post_quant_conv.*``, ``decoder.*``); checkpoints load with ``strict=False`` exactly like
-``init_from_ckpt`` does (``encoder.*``, ``quant_conv.*``, ``loss.*`` entries are ignored: the encoder only
-runs for inpainting / training and is outside the accelerated path).
+Reference: /root/reference/text_to_audio/Make_An_Audio/ldm/models/autoencoder.py:304-362
+(``encode(x) = DiagonalGaussianDistribution(quant_conv(encoder(x)))``, ``decode(z) = decoder(post_quant_conv(z))``)
+with ``Encoder`` / ``Decoder`` from ldm/modules/diffusionmodules/model.py:368-568.  Both classes take the
+constructor keywords of the reference's ``first_stage_config`` (``ddconfig``, ``lossconfig``, ``embed_dim``,
+``ckpt_path``, ``ignore_keys``, ``image_key``, ``colorize_nlabels``, ``monitor``); checkpoints load with
+``strict=False`` exactly like ``init_from_ckpt`` does.
+
+* ``AutoencoderKL`` -- the DECODE side: owns ``post_quant_conv.*`` and ``decoder.*`` (``encoder.*``,
+  ``quant_conv.*``, ``loss.*`` checkpoint entries are ignored).  What the text-to-audio and image-to-audio tools
+  need; ``bench.py`` times it.
+* ``AutoencoderKLWithEncoder`` -- the whole first stage: also owns ``encoder.*`` and ``quant_conv.*`` (its keys are
+  the reference class's), adds ``encode(x)`` and ``forward(input, sample_posterior)``.  ``install(first_stage=True)``
+  grafts it as the reference's ``AutoencoderKL``.  The decoder and the encoder are separate engines, each built
+  lazily from its own parameters: a tool that only decodes never uploads the encoder.
 
 Arithmetic: libagpt_b200.so (csrc/vae.cu).  CUDA only, inference only.
 """
@@ -19,6 +25,7 @@ import torch
 from torch import nn
 
 from ... import _lib, paramtree, specs
+from ..modules.distributions.distributions import DiagonalGaussianDistribution
 
 
 class AutoencoderKL(nn.Module, _lib.HandleOwner):
@@ -67,7 +74,7 @@ class AutoencoderKL(nn.Module, _lib.HandleOwner):
         return c
 
     def _ensure_engine(self, device):
-        sig = (paramtree.params_signature(self), device.index)
+        sig = (paramtree.params_signature(self, self._shapes), device.index)
         if self._h.value and sig == self._engine_sig:
             return
         self._destroy()
@@ -95,11 +102,69 @@ class AutoencoderKL(nn.Module, _lib.HandleOwner):
         return out
 
     def encode(self, x):
-        raise NotImplementedError("audiogpt_b200.AutoencoderKL accelerates decode() only (the encoder is used by "
-                                  "inpainting / training, outside the SURVEY.md 8 hot path)")
+        raise NotImplementedError("audiogpt_b200.AutoencoderKL accelerates decode() only; "
+                                  "audiogpt_b200.ldm.models.autoencoder.AutoencoderKLWithEncoder also runs encode()")
 
     def forward(self, input, sample_posterior=True):
         raise NotImplementedError("training forward is out of scope; call decode(z)")
 
     def get_last_layer(self):
         return paramtree.get_param(self, "decoder.conv_out.weight")
+
+
+class AutoencoderKLWithEncoder(AutoencoderKL):
+    """The whole first stage: decode() as AutoencoderKL, plus encode() and forward() on the encoder engine."""
+
+    # install(first_stage=True) records the reference's DiagonalGaussianDistribution here, so that encode() returns
+    # what LatentDiffusion.get_first_stage_encoding (ddpm_audio.py:157-164) accepts; None = the drop-in class
+    _posterior_cls = None
+
+    def __init__(self, ddconfig, lossconfig=None, embed_dim=4, ckpt_path=None, ignore_keys=(), image_key="image",
+                 colorize_nlabels=None, monitor=None):
+        super().__init__(ddconfig, lossconfig=lossconfig, embed_dim=embed_dim, ckpt_path=None, ignore_keys=ignore_keys,
+                         image_key=image_key, colorize_nlabels=colorize_nlabels, monitor=monitor)
+        self._enc_shapes = specs.vae_encoder_param_shapes(self.cfg)
+        paramtree.build(self, self._enc_shapes)
+        self._enc = _lib.HandleOwner()
+        self._enc_sig = None
+        if ckpt_path is not None:
+            self.init_from_ckpt(ckpt_path, ignore_keys=ignore_keys)
+
+    def _ensure_encoder(self, device):
+        sig = (paramtree.params_signature(self, self._enc_shapes), device.index)
+        if self._enc._h.value and sig == self._enc_sig:
+            return
+        self._enc._destroy()
+        _lib.require_cuda()
+        arr, keep = _lib.host_weight_array([paramtree.get_param(self, k).data for k in self._enc_shapes])
+        cfg = self._cfg_struct()
+        h = C.c_void_p()
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        _lib.check(_lib.lib().agpt_vae_encoder_create(C.byref(cfg), self.cfg["in_channels"], arr, len(keep), idx,
+                                                      C.byref(h)))
+        self._enc._h = h
+        self._enc_sig = sig
+
+    @torch.no_grad()
+    def encode(self, x):
+        """x [B, in_channels, H, W] -> posterior over z [B, embed_dim, H // 2^(levels-1), W // 2^(levels-1)]
+        (autoencoder.py:345-349).  H and W must be at least 2^(levels-1)."""
+        if not x.is_cuda:
+            raise RuntimeError("audiogpt_b200.AutoencoderKLWithEncoder runs on CUDA only (no CPU fallback)")
+        if x.dim() != 4 or x.shape[1] != self.cfg["in_channels"]:
+            raise ValueError(f"expected x of shape [B, {self.cfg['in_channels']}, H, W], got {tuple(x.shape)}")
+        self._ensure_encoder(x.device)
+        x = x.contiguous().float()
+        B, _, H, W = x.shape
+        f = 2 ** (len(self.cfg["ch_mult"]) - 1)
+        moments = torch.empty((B, 2 * self.embed_dim, H // f, W // f), device=x.device, dtype=torch.float32)
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.lib().agpt_vae_encode(self._enc._h, _lib.fptr(x), B, H, W, _lib.fptr(moments),
+                                                  _lib.cur_stream(x.device)))
+        return (self._posterior_cls or DiagonalGaussianDistribution)(moments)
+
+    def forward(self, input, sample_posterior=True):
+        """(decode(z), posterior) with z drawn from the posterior or its mode (autoencoder.py:355-362)"""
+        posterior = self.encode(input)
+        z = posterior.sample() if sample_posterior else posterior.mode()
+        return self.decode(z), posterior

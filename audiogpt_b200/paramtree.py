@@ -58,6 +58,7 @@ def build(root: nn.Module, shapes: Dict[str, Sequence[int]], init=None):
         add_param(root, key, t)
 
 
-def params_signature(module: nn.Module):
-    """Cheap change detector: (data_ptr, version) of every parameter."""
-    return tuple((p.data_ptr(), p._version, p.device.type) for p in module.parameters())
+def params_signature(module: nn.Module, keys: Sequence[str] = None):
+    """Cheap change detector: (data_ptr, version) of every parameter, or of the parameters named in ``keys``."""
+    ps = module.parameters() if keys is None else (get_param(module, k) for k in keys)
+    return tuple((p.data_ptr(), p._version, p.device.type) for p in ps)

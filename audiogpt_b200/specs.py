@@ -487,6 +487,23 @@ def vae_decoder_plan(cfg):
     return block_in, levels
 
 
+def _vae_res_shapes(s, p, cin, cout):
+    """ResnetBlock without time embedding (model.py:82-119)"""
+    s[f"{p}.norm1.weight"] = (cin,); s[f"{p}.norm1.bias"] = (cin,)
+    s[f"{p}.conv1.weight"] = (cout, cin, 3, 3); s[f"{p}.conv1.bias"] = (cout,)
+    s[f"{p}.norm2.weight"] = (cout,); s[f"{p}.norm2.bias"] = (cout,)
+    s[f"{p}.conv2.weight"] = (cout, cout, 3, 3); s[f"{p}.conv2.bias"] = (cout,)
+    if cin != cout:
+        s[f"{p}.nin_shortcut.weight"] = (cout, cin, 1, 1); s[f"{p}.nin_shortcut.bias"] = (cout,)
+
+
+def _vae_attn_shapes(s, p, c):
+    """AttnBlock (model.py:150-175)"""
+    s[f"{p}.norm.weight"] = (c,); s[f"{p}.norm.bias"] = (c,)
+    for n in ("q", "k", "v", "proj_out"):
+        s[f"{p}.{n}.weight"] = (c, c, 1, 1); s[f"{p}.{n}.bias"] = (c,)
+
+
 def vae_decoder_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
     """post_quant_conv (ldm/models/autoencoder.py:307) + decoder.* (model.py:462-536) of AutoencoderKL."""
     s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
@@ -495,30 +512,17 @@ def vae_decoder_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
     s["post_quant_conv.bias"] = (zc,)
     block_in, levels = vae_decoder_plan(cfg)
 
-    def res(p, cin, cout):
-        s[f"{p}.norm1.weight"] = (cin,); s[f"{p}.norm1.bias"] = (cin,)
-        s[f"{p}.conv1.weight"] = (cout, cin, 3, 3); s[f"{p}.conv1.bias"] = (cout,)
-        s[f"{p}.norm2.weight"] = (cout,); s[f"{p}.norm2.bias"] = (cout,)
-        s[f"{p}.conv2.weight"] = (cout, cout, 3, 3); s[f"{p}.conv2.bias"] = (cout,)
-        if cin != cout:
-            s[f"{p}.nin_shortcut.weight"] = (cout, cin, 1, 1); s[f"{p}.nin_shortcut.bias"] = (cout,)
-
-    def attn(p, c):
-        s[f"{p}.norm.weight"] = (c,); s[f"{p}.norm.bias"] = (c,)
-        for n in ("q", "k", "v", "proj_out"):
-            s[f"{p}.{n}.weight"] = (c, c, 1, 1); s[f"{p}.{n}.bias"] = (c,)
-
     s["decoder.conv_in.weight"] = (block_in, zc, 3, 3)
     s["decoder.conv_in.bias"] = (block_in,)
-    res("decoder.mid.block_1", block_in, block_in)
-    attn("decoder.mid.attn_1", block_in)
-    res("decoder.mid.block_2", block_in, block_in)
+    _vae_res_shapes(s, "decoder.mid.block_1", block_in, block_in)
+    _vae_attn_shapes(s, "decoder.mid.attn_1", block_in)
+    _vae_res_shapes(s, "decoder.mid.block_2", block_in, block_in)
     last = block_in
     for i_level, blocks, up in levels:
         for j, (cin, cout, has_attn) in enumerate(blocks):
-            res(f"decoder.up.{i_level}.block.{j}", cin, cout)
+            _vae_res_shapes(s, f"decoder.up.{i_level}.block.{j}", cin, cout)
             if has_attn:
-                attn(f"decoder.up.{i_level}.attn.{j}", cout)
+                _vae_attn_shapes(s, f"decoder.up.{i_level}.attn.{j}", cout)
             last = cout
         if up:
             s[f"decoder.up.{i_level}.upsample.conv.weight"] = (last, last, 3, 3)
@@ -531,6 +535,73 @@ def vae_decoder_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
 
 def synth_vae_decoder(cfg, seed: int = 5150):
     return synth_state_dict(vae_decoder_param_shapes(cfg), seed, convtranspose_prefixes=())
+
+
+def vae_encoder_plan(cfg):
+    """Block list of ldm Encoder.__init__ (model.py:368-437): returns
+    (block_in at the bottom, [(level, [(cin, cout, has_attn), ...], has_downsample), ...] in execution order).
+    Every level has num_res_blocks blocks (in_ch_mult = (1,) + ch_mult); all but the last end in a Downsample."""
+    ch, mult = int(cfg["ch"]), list(cfg["ch_mult"])
+    curr_res = int(cfg["resolution"])
+    levels = []
+    bi = ch
+    for i_level in range(len(mult)):
+        bo = ch * mult[i_level]
+        blocks = []
+        for _ in range(int(cfg["num_res_blocks"])):
+            blocks.append((bi, bo, curr_res in cfg["attn_resolutions"]))
+            bi = bo
+        down = i_level != len(mult) - 1
+        levels.append((i_level, blocks, down))
+        if down:
+            curr_res //= 2
+    return bi, levels
+
+
+def vae_encoder_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """encoder.* (model.py:368-437) + quant_conv (ldm/models/autoencoder.py:322) of AutoencoderKL, in the order the
+    engine consumes them (each level's blocks interleaved with their attention blocks)."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    ch, zc, ed = int(cfg["ch"]), int(cfg["z_channels"]), int(cfg["embed_dim"])
+    s["encoder.conv_in.weight"] = (ch, int(cfg.get("in_channels", 1)), 3, 3)
+    s["encoder.conv_in.bias"] = (ch,)
+    block_in, levels = vae_encoder_plan(cfg)
+    for i_level, blocks, down in levels:
+        for j, (cin, cout, has_attn) in enumerate(blocks):
+            _vae_res_shapes(s, f"encoder.down.{i_level}.block.{j}", cin, cout)
+            if has_attn:
+                _vae_attn_shapes(s, f"encoder.down.{i_level}.attn.{j}", cout)
+        if down:
+            c = blocks[-1][1]
+            s[f"encoder.down.{i_level}.downsample.conv.weight"] = (c, c, 3, 3)
+            s[f"encoder.down.{i_level}.downsample.conv.bias"] = (c,)
+    _vae_res_shapes(s, "encoder.mid.block_1", block_in, block_in)
+    _vae_attn_shapes(s, "encoder.mid.attn_1", block_in)
+    _vae_res_shapes(s, "encoder.mid.block_2", block_in, block_in)
+    s["encoder.norm_out.weight"] = (block_in,); s["encoder.norm_out.bias"] = (block_in,)
+    s["encoder.conv_out.weight"] = (2 * zc, block_in, 3, 3)
+    s["encoder.conv_out.bias"] = (2 * zc,)
+    s["quant_conv.weight"] = (2 * ed, 2 * zc, 1, 1)
+    s["quant_conv.bias"] = (2 * ed,)
+    return s
+
+
+def synth_vae_encoder(cfg, seed: int = 5151):
+    return synth_state_dict(vae_encoder_param_shapes(cfg), seed, convtranspose_prefixes=())
+
+
+def synth_masked_mel(B: int, H: int, W: int, seed: int) -> torch.Tensor:
+    """Seeded mel-like image [B, 1, H, W] in [-1, 1] with a band of frames masked to -1, prepared the way the Inpaint
+    tool prepares its encoder input (audio-chatgpt.py:437-444: masked_mel = (1 - mask) * mel in [0, 1], then * 2 - 1).
+    Row b masks frames [W * (0.3 + 0.1 b), + W / 6) (modulo W)."""
+    g = torch.Generator(device="cpu")
+    g.manual_seed(int(seed))
+    mel = torch.sigmoid(1.5 * torch.randn((B, 1, H, W), generator=g, dtype=torch.float32))
+    mask = torch.zeros((B, 1, H, W), dtype=torch.float32)
+    for b in range(B):
+        lo = int(W * (0.3 + 0.1 * b)) % W
+        mask[b, :, :, lo:lo + max(1, W // 6)] = 1.0
+    return ((1.0 - mask) * mel) * 2.0 - 1.0
 
 
 # ---------------------------------------------------------------------------------------------- PitchExtractor

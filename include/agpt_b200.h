@@ -236,6 +236,20 @@ int agpt_vae_create(const agpt_vae_cfg* cfg, const float* const* host_weights, i
 /* z [B, embed_dim, H, W] (device) -> out [B, out_ch, H * 2^(levels-1), W * 2^(levels-1)] (device) */
 int agpt_vae_decode(agpt_handle h, const float* z, int B, int H, int W, float* out, void* stream);
 
+/* ------------------------------------------------------------------ AutoencoderKL.encode (first stage, encoder side)
+ * Replaces the arithmetic of AutoencoderKL.encode = quant_conv(Encoder.forward(x)) (autoencoder.py:345-349,
+ * model.py:368-459; Downsample :60-79): the masked-mel encoding of the Inpaint tool (audio-chatgpt.py:507) and the
+ * first half of AutoencoderKL.forward.  The posterior (DiagonalGaussianDistribution) is built by the caller.
+ * cfg: the same agpt_vae_cfg as the decoder (num_res_blocks blocks per level, attn_at_level as there);
+ * in_channels: ddconfig in_channels (1 for mel images).
+ * host_weights: fp32 HOST arrays in the key order of audiogpt_b200.specs.vae_encoder_param_shapes(cfg) (encoder.*,
+ * then quant_conv.*).                                                                                             */
+int agpt_vae_encoder_create(const agpt_vae_cfg* cfg, int in_channels, const float* const* host_weights, int n_weights,
+                            int device, agpt_handle* out);
+/* x [B, in_channels, H, W] (device) -> moments [B, 2 * embed_dim, H >> (levels-1), W >> (levels-1)] (device):
+ * mean then logvar (before the clamp).  H and W below 2^(levels-1) are rejected.                                  */
+int agpt_vae_encode(agpt_handle h, const float* x, int B, int H, int W, float* moments, void* stream);
+
 /* ------------------------------------------------------------------ PitchExtractor
  * Replaces PitchExtractor.forward (NeuralSeq/modules/fastspeech/pe.py:119-148: Prenet :7-42, ConvStacks :82-116,
  * PitchPredictor modules/fastspeech/tts_modules.py:217-260, denorm_f0 utils/pitch_utils.py:63-76): F0 from a generated
