@@ -67,12 +67,60 @@ class Fs2Cfg(C.Structure):
         "use_pos_embed", "rel_pos", "pitch_type", "use_energy_embed", "use_midi")]
 
 
+# (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
+# takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
+_I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
+_W = C.POINTER(C.POINTER(C.c_float))     # const float* const* host_weights
+_OUT = C.POINTER(C.c_void_p)             # agpt_handle* out
+PROTOTYPES = {
+    "agpt_last_error": (C.c_char_p, []),
+    "agpt_version": (_I, []),
+    "agpt_launch_count": (C.c_longlong, []),
+    "agpt_destroy": (None, [_P]),
+    "agpt_profile_enable": (_I, [_I]),
+    "agpt_profile_collect": (_I, [_P, _P, _P, _P]),
+    "agpt_profile_dump": (_L, [_P, _L]),
+    "agpt_fma_peak_tflops": (_D, []),
+    "agpt_set_tensor_cores": (_I, [_I]),
+    "agpt_attention": (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "agpt_set_attention_tc": (_I, [_I]),
+    "agpt_attention_masked": (_I, [_P, _I, _P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "agpt_bench_tapconv": (_I, [_I] * 11 + [_P, _P]),
+    "agpt_check_tapconv": (_I, [_I] * 8 + [_D, _D, _P]),
+    "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
+    "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),
+    "agpt_hifigan_vocode_host": (_I, [_P, _P, _P, _I, _I, _P]),
+    "agpt_nsf_source": (_I, [_P, _I, _I, _I, _F, _P, _F, _P, _P, _F, _F, _F, _P, _P]),
+    "agpt_diffnet_create": (_I, [C.POINTER(DiffnetCfg), _W, _I, _I, _OUT]),
+    "agpt_diffnet_set_cond": (_I, [_P, _P, _I, _I, _P]),
+    "agpt_diffnet_eps": (_I, [_P, _P, _P, _P, _P]),
+    "agpt_gd_p_sample": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _L, _P, _P]),
+    "agpt_gd_sample_loop": (_I, [_P, _P, _I, _I, _P, _P, _L, _I, _P]),
+    "agpt_diffnet_launches_per_step": (_L, [_P]),
+    "agpt_axpby5": (_I, [_P, _P, _P, _P, _P, _P, _I, _L, _P, _P]),
+    "agpt_unet_create": (_I, [C.POINTER(UnetCfg), _W, _I, _I, _OUT]),
+    "agpt_unet_set_context": (_I, [_P, _P, _I, _I, _P]),
+    "agpt_unet_forward": (_I, [_P, _P, _P, _I, _I, _I, _P, _P]),
+    "agpt_ddim_update": (_I, [_P, _P, _I, _F, _F, _F, _F, _F, _P, _F, _I, _L, _P, _P, _P]),
+    "agpt_unet_ddim_sample": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P]),
+    "agpt_unet_launches_per_step": (_L, [_P]),
+    "agpt_vae_create": (_I, [C.POINTER(VaeCfg), _W, _I, _I, _OUT]),
+    "agpt_vae_decode": (_I, [_P, _P, _I, _I, _I, _P, _P]),
+    "agpt_vae_encoder_create": (_I, [C.POINTER(VaeCfg), _I, _W, _I, _I, _OUT]),
+    "agpt_vae_encode": (_I, [_P, _P, _I, _I, _I, _P, _P]),
+    "agpt_pe_create": (_I, [C.POINTER(PeCfg), _W, _I, _I, _OUT]),
+    "agpt_pe_forward": (_I, [_P, _P, _I, _I, _P, _P, _I, _I, _F, _F, _P]),
+    "agpt_fs2_create": (_I, [C.POINTER(Fs2Cfg), _W, _I, _I, _OUT]),
+    "agpt_fs2_encode": (_I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _P, _P]),
+    "agpt_fs2_decode": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _F, _F, _P, _P, _P, _P, _P, _P, _P]),
+}
+
 _lock = threading.Lock()
 _lib = None
 
 
 def lib() -> C.CDLL:
-    """Load the library once.  Raises if it has not been built (no fallback)."""
+    """Load the library once and declare every prototype.  Raises if it has not been built (no fallback)."""
     global _lib
     if _lib is not None:
         return _lib
@@ -84,13 +132,9 @@ def lib() -> C.CDLL:
                 f"{LIB_PATH} not found: build it with `python -m audiogpt_b200.build` "
                 "(audiogpt_b200 has no CPU/PyTorch fallback)")
         L = C.CDLL(LIB_PATH)
-        L.agpt_last_error.restype = C.c_char_p
-        L.agpt_launch_count.restype = C.c_longlong
-        L.agpt_destroy.argtypes = [C.c_void_p]
-        L.agpt_destroy.restype = None
-        L.agpt_vae_encoder_create.argtypes = [C.POINTER(VaeCfg), C.c_int, C.POINTER(C.POINTER(C.c_float)), C.c_int, C.c_int,
-                                              C.POINTER(C.c_void_p)]
-        L.agpt_vae_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        for name, (restype, argtypes) in PROTOTYPES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         _lib = L
         return L
 
@@ -126,23 +170,55 @@ def launch_count() -> int:
     return int(lib().agpt_launch_count())
 
 
-class HandleOwner:
-    """Owns an agpt_handle; destroyed with the Python object."""
+def call(name: str, device, *args):
+    """agpt_<name>(*args, stream) on ``device``'s current stream; raises on a non-zero return."""
+    with torch.cuda.device(device):
+        check(getattr(lib(), "agpt_" + name)(*args, cur_stream(device)))
 
-    def __init__(self):
-        self._h = C.c_void_p(None)
 
-    def _destroy(self):
-        h = getattr(self, "_h", None)
-        if h is not None and h.value:
+class Engine:
+    """One agpt_handle built by ``create`` (an agpt_*_create entry point) from a module's weights; destroyed with the
+    Python object."""
+
+    def __init__(self, create: str):
+        self.create = create
+        self.h = C.c_void_p()
+        self.sig = None
+
+    def destroy(self):
+        if self.h.value:
             try:
-                lib().agpt_destroy(h)
+                lib().agpt_destroy(self.h)
             except Exception:   # interpreter shutdown: module globals may already be gone
                 pass
-            try:
-                h.value = None
-            except Exception:
-                pass
+            self.h.value = None
+        self.sig = None
 
     def __del__(self):
-        self._destroy()
+        self.destroy()
+
+    def ensure(self, device: torch.device, sources, build) -> bool:
+        """Build the handle on ``device`` unless it was built there from ``sources`` as they are now: the same
+        (data_ptr, _version, device.type) of every tensor.  ``build()`` returns (the create call's leading arguments,
+        the weight tensors in the C ABI's order).  Returns True when it (re)built the handle."""
+        require_cuda()
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        sig = (tuple((t.data_ptr(), t._version, t.device.type) for t in sources), idx)
+        if self.h.value and sig == self.sig:
+            return False
+        self.destroy()
+        args, weights = build()
+        arr, keep = host_weight_array(weights)
+        h = C.c_void_p()
+        check(getattr(lib(), self.create)(*args, arr, len(keep), idx, C.byref(h)))
+        self.h, self.sig = h, sig
+        return True
+
+    def call(self, name: str, device, *args):
+        """agpt_<name>(handle, *args, stream) on ``device``'s current stream."""
+        call(name, device, self.h, *args)
+
+
+# ``_h = _lib.engine_handle`` in a class body: the handle of the instance's ``_engine`` (bench.py and the samplers
+# pass it to the entry points that take a model handle)
+engine_handle = property(lambda self: self._engine.h)

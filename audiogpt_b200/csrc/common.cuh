@@ -8,6 +8,7 @@
 #include <vector>
 #include <stdexcept>
 #include <cstdlib>
+#include <memory>
 #include <utility>
 
 namespace agpt {
@@ -93,10 +94,19 @@ struct DevBuf {
     }
     return p;
   }
-  void upload(const std::vector<float>& h) {
-    ensure(h.size());
-    AGPT_CUDA(cudaMemcpy(p, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice));
+  void upload(const float* h, size_t count) {
+    ensure(count);
+    AGPT_CUDA(cudaMemcpy(p, h, count * sizeof(float), cudaMemcpyHostToDevice));
   }
+  void upload(const std::vector<float>& h) { upload(h.data(), h.size()); }
+};
+
+// The host weight arrays of a *_create call, consumed in the order of the model's parameter table.
+struct WeightCursor {
+  const float* const* W;
+  int n, idx = 0;
+  const float* next() { AGPT_CHECK(idx < n, "too few weight arrays"); return W[idx++]; }
+  void done() const { AGPT_CHECK(idx == n, "weight array count does not match the config"); }
 };
 
 // RAII device scope for the C-ABI entry points: the reference deployment pins tools to different GPUs in ONE

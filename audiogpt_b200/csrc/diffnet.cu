@@ -234,35 +234,34 @@ struct Diffnet : Handle {
 
 Handle* diffnet_create(const agpt_diffnet_cfg* cfg, const float* const* W, int nW, int device) {
   DeviceGuard dg_(device);
-  auto* h = new Diffnet();
-  h->magic = kMagicDiffnet; h->device = device; h->cfg = *cfg;
   const int C = cfg->residual_channels, H = cfg->hidden_size, M = cfg->in_dims, L = cfg->residual_layers;
   AGPT_CHECK(C % 8 == 0 && C >= 8 && L >= 1 && cfg->dilation_cycle_length >= 1, "bad DiffNet config");
-  AGPT_CHECK(nW == 6 + 8 * L + 4, "weight array count does not match the config");
-  int idx = 0;
-  auto next = [&]() { return W[idx++]; };
-  { auto w = next(); auto b = next(); pack_conv(h->in_proj, w, b, C, M, 1, false); }
-  { auto w = next(); auto b = next(); pack_conv(h->mlp0, w, b, 4 * C, C, 1, false); }
-  { auto w = next(); auto b = next(); pack_conv(h->mlp2, w, b, C, 4 * C, 1, false); }
+  std::unique_ptr<Diffnet> h(new Diffnet());
+  h->magic = kMagicDiffnet; h->device = device; h->cfg = *cfg;
+  WeightCursor wc{W, nW};
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(h->in_proj, w, b, C, M, 1, false); }
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(h->mlp0, w, b, 4 * C, C, 1, false); }
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(h->mlp2, w, b, C, 4 * C, 1, false); }
   h->dil.resize(L); h->outp.resize(L);
   std::vector<float> dpw((size_t)L * C * C), dpb((size_t)L * C), cw((size_t)L * 2 * C * H), cb((size_t)L * 2 * C);
   for (int l = 0; l < L; ++l) {
-    { auto w = next(); auto b = next(); pack_conv_pairs(h->dil[l], w, b, 2 * C, C, 3); }
-    { auto w = next(); auto b = next();
+    { auto w = wc.next(); auto b = wc.next(); pack_conv_pairs(h->dil[l], w, b, 2 * C, C, 3); }
+    { auto w = wc.next(); auto b = wc.next();
       memcpy(&dpw[(size_t)l * C * C], w, sizeof(float) * C * C); memcpy(&dpb[(size_t)l * C], b, sizeof(float) * C); }
-    { auto w = next(); auto b = next();   // conditioner: interleave (gate,filter) like the dilated conv
+    { auto w = wc.next(); auto b = wc.next();   // conditioner: interleave (gate,filter) like the dilated conv
       for (int co = 0; co < 2 * C; ++co) {
         const int dst = 2 * (co % C) + co / C;
         memcpy(&cw[((size_t)l * 2 * C + dst) * H], w + (size_t)co * H, sizeof(float) * H);
         cb[(size_t)l * 2 * C + dst] = b[co];
       } }
-    { auto w = next(); auto b = next(); pack_conv(h->outp[l], w, b, 2 * C, C, 1, false); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(h->outp[l], w, b, 2 * C, C, 1, false); }
   }
   pack_conv(h->dproj_all, dpw.data(), dpb.data(), L * C, C, 1, false);
   pack_conv(h->cond_all, cw.data(), cb.data(), L * 2 * C, H, 1, false);
-  { auto w = next(); auto b = next(); pack_conv(h->skip_proj, w, b, C, C, 1, false, 1.f / std::sqrt((float)L)); }
-  { auto w = next(); auto b = next(); pack_conv(h->out_proj, w, b, M, C, 1, false); }
-  return h;
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(h->skip_proj, w, b, C, C, 1, false, 1.f / std::sqrt((float)L)); }
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(h->out_proj, w, b, M, C, 1, false); }
+  wc.done();
+  return h.release();
 }
 
 void diffnet_set_cond(Handle* hh, const float* cond, int B, int T, cudaStream_t st) {

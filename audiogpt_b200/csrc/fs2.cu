@@ -367,20 +367,18 @@ struct Fs2Net : Handle {
 };
 
 namespace {
-void up_(DevBuf& d, const float* p, size_t n) { d.upload(std::vector<float>(p, p + n)); }
-
-void load_stack(FftStack& S, const std::function<const float*()>& next, int H, int L, int k) {
+void load_stack(FftStack& S, WeightCursor& wc, int H, int L, int k) {
   S.layers.resize(L);
   for (auto& l : S.layers) {
     l.k = k;
-    { auto g = next(); auto b = next(); up_(l.ln1g, g, H); up_(l.ln1b, b, H); }
-    pack_conv(l.qkv, next(), nullptr, 3 * H, H, 1, false);        // in_proj_weight [3H][H], no bias
-    pack_conv(l.out, next(), nullptr, H, H, 1, false);            // out_proj.weight, no bias
-    { auto g = next(); auto b = next(); up_(l.ln2g, g, H); up_(l.ln2b, b, H); }
-    { auto w = next(); auto b = next(); pack_conv(l.ffn1, w, b, 4 * H, H, k, false); }
-    { auto w = next(); auto b = next(); pack_conv(l.ffn2, w, b, H, 4 * H, 1, false); }
+    { auto g = wc.next(); auto b = wc.next(); l.ln1g.upload(g, H); l.ln1b.upload(b, H); }
+    pack_conv(l.qkv, wc.next(), nullptr, 3 * H, H, 1, false);        // in_proj_weight [3H][H], no bias
+    pack_conv(l.out, wc.next(), nullptr, H, H, 1, false);            // out_proj.weight, no bias
+    { auto g = wc.next(); auto b = wc.next(); l.ln2g.upload(g, H); l.ln2b.upload(b, H); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(l.ffn1, w, b, 4 * H, H, k, false); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(l.ffn2, w, b, H, 4 * H, 1, false); }
   }
-  { auto g = next(); auto b = next(); up_(S.lng, g, H); up_(S.lnb, b, H); }
+  { auto g = wc.next(); auto b = wc.next(); S.lng.upload(g, H); S.lnb.upload(b, H); }
 }
 }  // namespace
 
@@ -392,54 +390,53 @@ Handle* fs2_create(const agpt_fs2_cfg* cfg, const float* const* W, int nW, int d
                  cfg->enc_ffn_kernel <= kMaxTaps && cfg->dec_ffn_kernel <= kMaxTaps && cfg->dur_predictor_kernel % 2 == 1 &&
                  cfg->dur_predictor_kernel <= kMaxTaps && cfg->pitch_type >= 0 && cfg->pitch_type <= 2,
              "bad FastSpeech2 config");
-  auto* h = new Fs2Net();
+  std::unique_ptr<Fs2Net> h(new Fs2Net());
   h->magic = kMagicFs2; h->device = device; h->cfg = *cfg;
-  int idx = 0;
-  std::function<const float*()> next = [&]() -> const float* { AGPT_CHECK(idx < nW, "too few weight arrays"); return W[idx++]; };
-  up_(h->E, next(), (size_t)cfg->n_tokens * H);                   // encoder_embed_tokens.weight
-  next();                                                         // encoder.embed_tokens.weight (the same tensor)
-  if (!cfg->rel_pos) next();                                      // encoder.embed_positions._float_tensor
-  load_stack(h->enc, next, H, cfg->enc_layers, cfg->enc_ffn_kernel);
-  h->dec_alpha = next()[0];                                       // decoder.pos_embed_alpha
-  next();                                                         // decoder.embed_positions._float_tensor
-  load_stack(h->dec, next, H, cfg->dec_layers, cfg->dec_ffn_kernel);
-  { auto w = next(); auto b = next(); pack_conv(h->mel_out, w, b, cfg->out_dims, H, 1, false); }
+  WeightCursor wc{W, nW};
+  h->E.upload(wc.next(), (size_t)cfg->n_tokens * H);                // encoder_embed_tokens.weight
+  wc.next();                                                      // encoder.embed_tokens.weight (the same tensor)
+  if (!cfg->rel_pos) wc.next();                                   // encoder.embed_positions._float_tensor
+  load_stack(h->enc, wc, H, cfg->enc_layers, cfg->enc_ffn_kernel);
+  h->dec_alpha = wc.next()[0];                                    // decoder.pos_embed_alpha
+  wc.next();                                                      // decoder.embed_positions._float_tensor
+  load_stack(h->dec, wc, H, cfg->dec_layers, cfg->dec_ffn_kernel);
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(h->mel_out, w, b, cfg->out_dims, H, 1, false); }
   h->dp_conv.resize(cfg->dur_predictor_layers); h->dp_g.resize(cfg->dur_predictor_layers); h->dp_b.resize(cfg->dur_predictor_layers);
   int cin = H;
   for (int l = 0; l < cfg->dur_predictor_layers; ++l) {
-    { auto w = next(); auto b = next(); pack_conv(h->dp_conv[l], w, b, P, cin, cfg->dur_predictor_kernel, false); }
-    { auto g = next(); auto b = next(); up_(h->dp_g[l], g, P); up_(h->dp_b[l], b, P); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(h->dp_conv[l], w, b, P, cin, cfg->dur_predictor_kernel, false); }
+    { auto g = wc.next(); auto b = wc.next(); h->dp_g[l].upload(g, P); h->dp_b[l].upload(b, P); }
     cin = P;
   }
   {  // Linear(P -> 1) padded to 4 output channels
-    auto w = next(); auto b = next();
+    auto w = wc.next(); auto b = wc.next();
     std::vector<float> wp((size_t)4 * P, 0.f), bp(4, 0.f);
     memcpy(wp.data(), w, sizeof(float) * P);
     bp[0] = b[0];
     pack_conv(h->dp_lin, wp.data(), bp.data(), 4, P, 1, false);
   }
   if (cfg->pitch_type) {
-    up_(h->pitchE, next(), (size_t)300 * H);
-    h->pitch_pp.load(next, H, P, cfg->predictor_kernel, cfg->predictor_layers, cfg->pitch_type == 1 ? 2 : 1);
+    h->pitchE.upload(wc.next(), (size_t)300 * H);
+    h->pitch_pp.load(wc, H, P, cfg->predictor_kernel, cfg->predictor_layers, cfg->pitch_type == 1 ? 2 : 1);
   }
   if (cfg->use_energy_embed) {
-    up_(h->energyE, next(), (size_t)256 * H);
-    h->energy_pp.load(next, H, P, cfg->predictor_kernel, cfg->predictor_layers, 1);
+    h->energyE.upload(wc.next(), (size_t)256 * H);
+    h->energy_pp.load(wc, H, P, cfg->predictor_kernel, cfg->predictor_layers, 1);
   }
   if (cfg->use_midi) {
-    up_(h->midiE, next(), (size_t)300 * H);
-    up_(h->mdw, next(), H);
-    up_(h->mdb, next(), H);
-    up_(h->slurE, next(), (size_t)2 * H);
+    h->midiE.upload(wc.next(), (size_t)300 * H);
+    h->mdw.upload(wc.next(), H);
+    h->mdb.upload(wc.next(), H);
+    h->slurE.upload(wc.next(), (size_t)2 * H);
   }
-  AGPT_CHECK(idx == nW, "weight array count does not match the config");
+  wc.done();
   if (cfg->rel_pos) {   // espnet div_term: exp(arange(0, H, 2) * -(ln 10000 / H)) in fp32
     std::vector<float> d(H / 2);
     const float c = (float)(-(std::log(10000.0) / (double)H));
     for (int i = 0; i < H / 2; ++i) d[i] = (float)std::exp((double)((float)(2 * i) * c));
     h->rel_div.upload(d);
   }
-  return h;
+  return h.release();
 }
 
 void fs2_encode(Handle* hh, const int* tok, int B, int T, const int* pmidi, const float* mdur, const int* slur, int predict, float* dur,

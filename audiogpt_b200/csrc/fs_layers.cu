@@ -73,27 +73,25 @@ void fs_posemb_add(const float* in, float* out, const int* pos, float alpha, lon
   count_launch(1);
 }
 
-static void up_(DevBuf& d, const float* p, int n) { d.upload(std::vector<float>(p, p + n)); }
-
-void PitchPredictorNet::load(const std::function<const float*()>& next, int H, int P_, int k, int layers, int odim) {
+void PitchPredictorNet::load(WeightCursor& wc, int H, int P_, int k, int layers, int odim) {
   AGPT_CHECK(odim >= 1 && odim <= 4 && k % 2 == 1 && k <= kMaxTaps, "bad pitch predictor config");
   P = P_;
-  alpha = next()[0];
+  alpha = wc.next()[0];
   conv.resize(layers); g.resize(layers); b.resize(layers);
   int cin = H;
   for (int l = 0; l < layers; ++l) {
-    { auto w = next(); auto bb = next(); pack_conv(conv[l], w, bb, P, cin, k, false); }
-    { auto gg = next(); auto bb = next(); up_(g[l], gg, P); up_(b[l], bb, P); }
+    { auto w = wc.next(); auto bb = wc.next(); pack_conv(conv[l], w, bb, P, cin, k, false); }
+    { auto gg = wc.next(); auto bb = wc.next(); g[l].upload(gg, P); b[l].upload(bb, P); }
     cin = P;
   }
   {  // Linear(P -> odim), padded to 4 output channels so that rows stay float4-addressable
-    auto w = next(); auto bb = next();
+    auto w = wc.next(); auto bb = wc.next();
     std::vector<float> wp((size_t)4 * P, 0.f), bp(4, 0.f);
     memcpy(wp.data(), w, sizeof(float) * odim * P);
     for (int i = 0; i < odim; ++i) bp[i] = bb[i];
     pack_conv(lin, wp.data(), bp.data(), 4, P, 1, false);
   }
-  next();                              // embed_positions._float_tensor (a device marker buffer)
+  wc.next();                           // embed_positions._float_tensor (a device marker buffer)
 }
 
 void PitchPredictorNet::forward(const float* x, int H, int B, int T, float* s0, float* s1, float* s2, float* pred4, cudaStream_t st) {

@@ -1,7 +1,6 @@
 // Layers shared by the FastSpeech-family drivers (pe.cu: PitchExtractor, fs2.cu: FastSpeech2 / FastSpeech2MIDI).
 // Activations are channels-last rows [B][T][C].
 #pragma once
-#include <functional>
 #include <vector>
 #include "common.cuh"
 #include "tapconv.cuh"
@@ -30,7 +29,7 @@ struct PitchPredictorNet {
   DevBuf pos;
   // consumes, in state-dict order: pos_embed_alpha, conv.{l}.1.weight / .bias, conv.{l}.3.weight / .bias, linear.weight /
   // .bias, embed_positions._float_tensor
-  void load(const std::function<const float*()>& next, int H, int P_, int k, int layers, int odim);
+  void load(WeightCursor& wc, int H, int P_, int k, int layers, int odim);
   // x [B][T][H] (read only) -> pred4 [B][T][4] (channels >= odim are zero); s0 / s1 / s2: scratch of B*T*max(H, P) floats
   void forward(const float* x, int H, int B, int T, float* s0, float* s1, float* s2, float* pred4, cudaStream_t st);
 };

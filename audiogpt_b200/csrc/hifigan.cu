@@ -453,28 +453,31 @@ struct Hifigan : Handle {
 
 Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int nW, int device) {
   DeviceGuard dg_(device);
-  auto* h = new Hifigan();
-  h->magic = kMagicHifigan; h->device = device; h->cfg = *cfg;
   const int nu = cfg->num_upsamples, nk = cfg->num_kernels;
   AGPT_CHECK(nu >= 1 && nu <= AGPT_MAX_UPS && nk >= 1 && nk <= AGPT_MAX_RBK, "bad config");
-  int idx = 0;
-  auto next = [&]() -> const float* { AGPT_CHECK(idx < nW, "too few weight arrays"); return W[idx++]; };
   const int C0 = cfg->upsample_initial_channel;
-  { const float* w = next(); const float* b = next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
+  for (int i = 0, C = C0; i < nu; ++i, C /= 2)
+    AGPT_CHECK(C % 2 == 0 && (C / 2) % 4 == 0, "channel counts must stay multiples of 4");
+  for (int j = 0; j < nk; ++j)
+    AGPT_CHECK(cfg->resblock_kernel_sizes[j] % 2 == 1 && cfg->resblock_kernel_sizes[j] <= kMaxTaps,
+               "resblock kernel size must be odd and <= 11");
+  std::unique_ptr<Hifigan> h(new Hifigan());
+  h->magic = kMagicHifigan; h->device = device; h->cfg = *cfg;
+  WeightCursor wc{W, nW};
+  { const float* w = wc.next(); const float* b = wc.next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
   h->ups.resize(nu);
   int C = C0; h->hop = 1;
   for (int i = 0; i < nu; ++i) {
-    const float* w = next(); const float* b = next();
+    const float* w = wc.next(); const float* b = wc.next();
     const int u = cfg->upsample_rates[i], k = cfg->upsample_kernel_sizes[i];
-    AGPT_CHECK(C % 2 == 0 && (C / 2) % 4 == 0, "channel counts must stay multiples of 4");
     pack_convtranspose(h->ups[i], w, b, C, C / 2, k, u, (k - u) / 2);
     C /= 2; h->hop *= u;
   }
   h->c_last = C;
   // BigVGAN (cfg.activation 1 = Snake, 2 = SnakeBeta): alpha [, beta] vectors follow each block's convs
   auto load_snake = [&](SnakeW& sw, int ch) {
-    const float* al = next();
-    const float* be = (cfg->activation == 2) ? next() : al;
+    const float* al = wc.next();
+    const float* be = (cfg->activation == 2) ? wc.next() : al;
     std::vector<float> a(ch), ib(ch);
     for (int c = 0; c < ch; ++c) {
       const float av = cfg->snake_logscale ? std::exp(al[c]) : al[c];
@@ -491,7 +494,6 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
     for (int j = 0; j < nk; ++j) {
       ResBlockW& rb = h->rbs[i * nk + j];
       rb.ks = cfg->resblock_kernel_sizes[j];
-      AGPT_CHECK(rb.ks % 2 == 1 && rb.ks <= kMaxTaps, "resblock kernel size must be odd and <= 11");
       const int nd = cfg->resblock_num_dilations[j];
       rb.dil.assign(cfg->resblock_dilations[j], cfg->resblock_dilations[j] + nd);
       // narrow stages: dilation-1 convs with k >= 7 also get a time-grouped image (N = 128 per MMA instead of C)
@@ -505,7 +507,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
       };
       rb.c1.resize(nd); rb.c1g.resize(nd); rb.g1.assign(nd, 0);
       for (int n = 0; n < nd; ++n) {
-        const float* w = next(); const float* b = next();
+        const float* w = wc.next(); const float* b = wc.next();
         pack_conv(rb.c1[n], w, b, C, C, rb.ks, false);
         rb.g1[n] = group_of(rb.dil[n]);
         if (rb.g1[n]) pack_conv_grouped(rb.c1g[n], w, b, C, rb.ks, rb.g1[n]);
@@ -513,7 +515,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
       if (cfg->resblock_type == 1) {
         rb.c2.resize(nd); rb.c2g.resize(nd); rb.g2.assign(nd, 0);
         for (int n = 0; n < nd; ++n) {
-          const float* w = next(); const float* b = next();
+          const float* w = wc.next(); const float* b = wc.next();
           pack_conv(rb.c2[n], w, b, C, C, rb.ks, false);
           rb.g2[n] = group_of(1);
           if (rb.g2[n]) pack_conv_grouped(rb.c2g[n], w, b, C, rb.ks, rb.g2[n]);
@@ -527,20 +529,20 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   }
   if (cfg->activation != 0) load_snake(h->act_post, C);
   {  // conv_post [c_out][C][7] -> [c_out][7][C]
-    const float* w = next(); const float* b = next();
+    const float* w = wc.next(); const float* b = wc.next();
     std::vector<float> pw((size_t)cfg->c_out * 7 * C);
     for (int oc = 0; oc < cfg->c_out; ++oc)
       for (int c = 0; c < C; ++c)
         for (int k = 0; k < 7; ++k) pw[((size_t)oc * 7 + k) * C + c] = w[((size_t)oc * C + c) * 7 + k];
     h->post_w.upload(pw);
-    h->post_b.upload(std::vector<float>(b, b + cfg->c_out));
+    h->post_b.upload(b, cfg->c_out);
   }
   if (cfg->activation != 0) {   // the Kaiser-sinc taps (identical upsample / downsample buffers of every Activation1d)
-    const float* f = next();
+    const float* f = wc.next();
     for (int k = 0; k < 12; ++k) h->aaf.f[k] = f[k];
   }
   if (cfg->use_nsf) {
-    next(); next();  // m_source.l_linear.{weight,bias}: the source module stays on the host side (RNG)
+    wc.next(); wc.next();  // m_source.l_linear.{weight,bias}: the source module stays on the host side (RNG)
     h->noise.resize(nu);
     int Cc = C0;
     for (int i = 0; i < nu; ++i) {
@@ -551,13 +553,13 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
         int stv = 1; for (int q = i + 1; q < nu; ++q) stv *= cfg->upsample_rates[q];
         nc.st = stv; nc.K = 2 * stv; nc.pad = stv / 2;
       } else { nc.st = 1; nc.K = 1; nc.pad = 0; }
-      const float* w = next(); const float* b = next();
-      nc.w.upload(std::vector<float>(w, w + (size_t)Cc * nc.K));
-      nc.b.upload(std::vector<float>(b, b + Cc));
+      const float* w = wc.next(); const float* b = wc.next();
+      nc.w.upload(w, (size_t)Cc * nc.K);
+      nc.b.upload(b, Cc);
     }
   }
-  AGPT_CHECK(idx == nW, "weight array count does not match the config");
-  return h;
+  wc.done();
+  return h.release();
 }
 
 // Optional (AGPT_HIFI_L2_MB=<per-tensor MB>): run the generator over sub-batches whose per-stage tensors

@@ -92,22 +92,19 @@ struct PeNet : Handle {
   }
 };
 
-static void up_(DevBuf& d, const float* p, int n) { d.upload(std::vector<float>(p, p + n)); }
-
 Handle* pe_create(const agpt_pe_cfg* cfg, const float* const* W, int nW, int device) {
   DeviceGuard dg_(device);
-  auto* h = new PeNet();
-  h->magic = kMagicPe; h->device = device; h->cfg = *cfg;
   const int H = cfg->hidden_size, M = cfg->n_mel_bins, P = cfg->predictor_hidden, k = cfg->predictor_kernel;
   AGPT_CHECK(H % 16 == 0 && P % 4 == 0 && M % 4 == 0 && k % 2 == 1 && k <= kMaxTaps, "bad PitchExtractor config");
-  int idx = 0;
-  auto next = [&]() -> const float* { AGPT_CHECK(idx < nW, "too few weight arrays"); return W[idx++]; };
+  std::unique_ptr<PeNet> h(new PeNet());
+  h->magic = kMagicPe; h->device = device; h->cfg = *cfg;
+  WeightCursor wc{W, nW};
   int cin = M;
   for (int l = 0; l < 3; ++l) {
-    auto w = next(); auto b = next();
+    auto w = wc.next(); auto b = wc.next();
     pack_conv(h->pre_conv[l], w, b, H, cin, 5, false);
-    auto g = next(); auto be = next(); auto mu = next(); auto var = next();
-    next();                            // num_batches_tracked
+    auto g = wc.next(); auto be = wc.next(); auto mu = wc.next(); auto var = wc.next();
+    wc.next();                            // num_batches_tracked
     std::vector<float> a(H), bb(H);
     for (int c = 0; c < H; ++c) {      // BatchNorm1d eval: (x - mean) / sqrt(var + eps) * gamma + beta, eps = 1e-5
       a[c] = g[c] / std::sqrt(var[c] + 1e-5f);
@@ -116,19 +113,19 @@ Handle* pe_create(const agpt_pe_cfg* cfg, const float* const* W, int nW, int dev
     h->bn_a[l].upload(a); h->bn_b[l].upload(bb);
     cin = H;
   }
-  { auto w = next(); auto b = next(); pack_conv(h->pre_out, w, b, H, H, 1, false); }
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(h->pre_out, w, b, H, H, 1, false); }
   h->enc_conv.resize(cfg->conv_layers); h->enc_g.resize(cfg->conv_layers); h->enc_b.resize(cfg->conv_layers);
   for (int l = 0; l < cfg->conv_layers; ++l) {
-    { auto w = next(); auto b = next(); pack_conv(h->enc_conv[l], w, b, H, H, 5, false); }
-    { auto g = next(); auto b = next(); up_(h->enc_g[l], g, H); up_(h->enc_b[l], b, H); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(h->enc_conv[l], w, b, H, H, 5, false); }
+    { auto g = wc.next(); auto b = wc.next(); h->enc_g[l].upload(g, H); h->enc_b[l].upload(b, H); }
   }
   if (cfg->conv_layers > 0) {
-    { auto w = next(); auto b = next(); pack_conv(h->enc_in, w, b, H, H, 1, false); }
-    { auto w = next(); auto b = next(); pack_conv(h->enc_out, w, b, H, H, 1, false); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(h->enc_in, w, b, H, H, 1, false); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(h->enc_out, w, b, H, H, 1, false); }
   }
-  h->pp.load(next, H, P, k, cfg->predictor_layers, 2);
-  AGPT_CHECK(idx == nW, "weight array count does not match the config");
-  return h;
+  h->pp.load(wc, H, P, k, cfg->predictor_layers, 2);
+  wc.done();
+  return h.release();
 }
 
 void pe_forward(Handle* hh, const float* mel, int B, int T, float* pitch_pred, float* f0, int use_uv, int norm_mode,

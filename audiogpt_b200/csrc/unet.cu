@@ -302,21 +302,18 @@ struct Unet : Handle {
   }
 };
 
-static void upload_vec(DevBuf& d, const float* p, int n) { d.upload(std::vector<float>(p, p + n)); }
-
 Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int device) {
   DeviceGuard dg_(device);
-  auto* u = new Unet();
-  u->magic = kMagicUnet; u->device = device; u->cfg = *cfg;
   const int mc = cfg->model_channels, temb = 4 * mc, ctx = cfg->context_dim, depth = cfg->transformer_depth;
-  u->mc = mc; u->temb = temb; u->ctx_dim = ctx;
   AGPT_CHECK(mc % 32 == 0, "model_channels must be a multiple of 32 (GroupNorm32)");
   AGPT_CHECK(cfg->num_levels >= 1 && cfg->num_levels <= AGPT_MAX_LEVELS, "levels");
-  int idx = 0;
-  auto next = [&]() -> const float* { AGPT_CHECK(idx < nW, "too few weight arrays"); return W[idx++]; };
+  std::unique_ptr<Unet> u(new Unet());
+  u->magic = kMagicUnet; u->device = device; u->cfg = *cfg;
+  u->mc = mc; u->temb = temb; u->ctx_dim = ctx;
+  WeightCursor wc{W, nW};
 
-  { auto w = next(); auto b = next(); pack_conv(u->time0, w, b, temb, mc, 1, false); }
-  { auto w = next(); auto b = next(); pack_conv(u->time2, w, b, temb, temb, 1, false); }
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(u->time0, w, b, temb, mc, 1, false); }
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(u->time2, w, b, temb, temb, 1, false); }
 
   std::vector<float> embw, embb, kvw;   // batched projections, filled while walking the blocks
   int emb_off = 0, kv_off = 0;
@@ -331,14 +328,14 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
     ResW& r = u->res.back();
     r.cin = cin; r.cout = cout;
     AGPT_CHECK(cin % 32 == 0 && cout % 32 == 0, "ResBlock channels must be multiples of 32");
-    { auto g = next(); auto b = next(); upload_vec(r.gn1_g, g, cin); upload_vec(r.gn1_b, b, cin); }
-    { auto w = next(); auto b = next(); pack_conv(r.conv1, w, b, cout, cin, 9, true); }
-    { auto w = next(); auto b = next();
+    { auto g = wc.next(); auto b = wc.next(); r.gn1_g.upload(g, cin); r.gn1_b.upload(b, cin); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(r.conv1, w, b, cout, cin, 9, true); }
+    { auto w = wc.next(); auto b = wc.next();
       embw.insert(embw.end(), w, w + (size_t)cout * temb); embb.insert(embb.end(), b, b + cout);
       r.emb_off = emb_off; emb_off += cout; }
-    { auto g = next(); auto b = next(); upload_vec(r.gn2_g, g, cout); upload_vec(r.gn2_b, b, cout); }
-    { auto w = next(); auto b = next(); pack_conv(r.conv2, w, b, cout, cout, 9, true); }
-    if (cin != cout) { auto w = next(); auto b = next(); pack_conv(r.skip, w, b, cout, cin, 1, false); r.has_skip = true; }
+    { auto g = wc.next(); auto b = wc.next(); r.gn2_g.upload(g, cout); r.gn2_b.upload(b, cout); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(r.conv2, w, b, cout, cout, 9, true); }
+    if (cin != cout) { auto w = wc.next(); auto b = wc.next(); pack_conv(r.skip, w, b, cout, cin, 1, false); r.has_skip = true; }
     return (int)u->res.size() - 1;
   };
 
@@ -347,42 +344,42 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
     StW& t = u->st.back();
     t.ch = ch; heads_for(ch, t.heads, t.dhead); t.inner = t.heads * t.dhead;
     const int C = t.inner;
-    { auto g = next(); auto b = next(); upload_vec(t.gn_g, g, ch); upload_vec(t.gn_b, b, ch); }
-    { auto w = next(); auto b = next(); pack_conv(t.proj_in, w, b, C, ch, 1, false); }
+    { auto g = wc.next(); auto b = wc.next(); t.gn_g.upload(g, ch); t.gn_b.upload(b, ch); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(t.proj_in, w, b, C, ch, 1, false); }
     t.blocks.resize(depth);
     for (int d = 0; d < depth; ++d) {
       XfBlockW& b = t.blocks[d];
       {  // attn1: to_q, to_k, to_v (no bias) -> one [3C][C] GEMM ; to_out.0 (bias)
-        auto wq = next(); auto wk = next(); auto wv = next();
+        auto wq = wc.next(); auto wk = wc.next(); auto wv = wc.next();
         std::vector<float> cat((size_t)3 * C * C);
         memcpy(&cat[0], wq, sizeof(float) * C * C);
         memcpy(&cat[(size_t)C * C], wk, sizeof(float) * C * C);
         memcpy(&cat[(size_t)2 * C * C], wv, sizeof(float) * C * C);
         pack_conv(b.qkv1, cat.data(), nullptr, 3 * C, C, 1, false);
-        auto wo = next(); auto bo = next(); pack_conv(b.out1, wo, bo, C, C, 1, false);
+        auto wo = wc.next(); auto bo = wc.next(); pack_conv(b.out1, wo, bo, C, C, 1, false);
       }
       {  // attn2: to_q on x; to_k/to_v on the context -> hoisted, batched over all blocks
-        auto wq = next(); auto wk = next(); auto wv = next();
+        auto wq = wc.next(); auto wk = wc.next(); auto wv = wc.next();
         pack_conv(b.q2, wq, nullptr, C, C, 1, false);
         kvw.insert(kvw.end(), wk, wk + (size_t)C * ctx);
         kvw.insert(kvw.end(), wv, wv + (size_t)C * ctx);
         b.kv_off = kv_off; kv_off += 2 * C;
-        auto wo = next(); auto bo = next(); pack_conv(b.out2, wo, bo, C, C, 1, false);
+        auto wo = wc.next(); auto bo = wc.next(); pack_conv(b.out2, wo, bo, C, C, 1, false);
       }
-      { auto w = next(); auto bb = next(); pack_conv_pairs(b.ff1, w, bb, 8 * C, C, 1); }
-      { auto w = next(); auto bb = next(); pack_conv(b.ff2, w, bb, C, 4 * C, 1, false); }
-      { auto g = next(); auto bb = next(); upload_vec(b.ln1_g, g, C); upload_vec(b.ln1_b, bb, C); }
-      { auto g = next(); auto bb = next(); upload_vec(b.ln2_g, g, C); upload_vec(b.ln2_b, bb, C); }
-      { auto g = next(); auto bb = next(); upload_vec(b.ln3_g, g, C); upload_vec(b.ln3_b, bb, C); }
+      { auto w = wc.next(); auto bb = wc.next(); pack_conv_pairs(b.ff1, w, bb, 8 * C, C, 1); }
+      { auto w = wc.next(); auto bb = wc.next(); pack_conv(b.ff2, w, bb, C, 4 * C, 1, false); }
+      { auto g = wc.next(); auto bb = wc.next(); b.ln1_g.upload(g, C); b.ln1_b.upload(bb, C); }
+      { auto g = wc.next(); auto bb = wc.next(); b.ln2_g.upload(g, C); b.ln2_b.upload(bb, C); }
+      { auto g = wc.next(); auto bb = wc.next(); b.ln3_g.upload(g, C); b.ln3_b.upload(bb, C); }
     }
-    { auto w = next(); auto b = next(); pack_conv(t.proj_out, w, b, ch, C, 1, false); }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(t.proj_out, w, b, ch, C, 1, false); }
     return (int)u->st.size() - 1;
   };
 
   // ---- walk the constructor rules (openaimodel.py:516-693) ----
   u->cin_pad = round_up(cfg->in_channels, 4);
   {
-    auto w = next(); auto b = next();
+    auto w = wc.next(); auto b = wc.next();
     // input conv: pad Cin to a multiple of 4 so that activation rows stay float4-aligned
     std::vector<float> wp((size_t)mc * u->cin_pad * 9, 0.f);
     for (int co = 0; co < mc; ++co)
@@ -405,7 +402,7 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
       chans.push_back(ch);
     }
     if (level != cfg->num_levels - 1) {
-      auto w = next(); auto b = next();
+      auto w = wc.next(); auto b = wc.next();
       // stride-2 conv as im2col + GEMM: weight [Cout][Cin][3][3] -> [Cout][(kh*3+kw)*Cin + ci]
       std::vector<float> wp((size_t)ch * 9 * ch);
       for (int co = 0; co < ch; ++co)
@@ -433,7 +430,7 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
       ch = mc * m;
       if (cfg->attn_at_level[level]) blk.layers.push_back({L_ST, make_st(ch), 0});
       if (level && i == cfg->num_res_blocks) {
-        auto w = next(); auto b = next();
+        auto w = wc.next(); auto b = wc.next();
         u->up_convs.emplace_back();
         pack_conv(u->up_convs.back(), w, b, ch, ch, 9, true);
         blk.layers.push_back({L_UP, (int)u->up_convs.size() - 1, ch});
@@ -442,8 +439,8 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
     }
   }
   u->final_ch = ch;
-  { auto g = next(); auto b = next(); upload_vec(u->out_gn_g, g, ch); upload_vec(u->out_gn_b, b, ch); }
-  { auto w = next(); auto b = next(); pack_conv(u->conv_out, w, b, cfg->out_channels, ch, 9, true);
+  { auto g = wc.next(); auto b = wc.next(); u->out_gn_g.upload(g, ch); u->out_gn_b.upload(b, ch); }
+  { auto w = wc.next(); auto b = wc.next(); pack_conv(u->conv_out, w, b, cfg->out_channels, ch, 9, true);
     if (cfg->out_channels == 4 && cfg->in_channels == 4) {
       std::vector<float> w9((size_t)9 * ch * 4), b4(4);
       for (int co = 0; co < 4; ++co) {
@@ -453,12 +450,12 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
       }
       u->out_w9c4.upload(w9); u->out_b4.upload(b4);
     } }
-  AGPT_CHECK(idx == nW, "weight array count does not match the config");
+  wc.done();
 
   u->emb_total = emb_off; u->kv_total = kv_off;
   pack_conv(u->emb_all, embw.data(), embb.data(), emb_off, temb, 1, false);
   pack_conv(u->ctx_kv_all, kvw.data(), nullptr, kv_off, ctx, 1, false);
-  return u;
+  return u.release();
 }
 
 void unet_set_context(Handle* hh, const float* ctx, int N, int S, cudaStream_t st) {

@@ -16,7 +16,6 @@
 // Parity: tests/test_vae_gpu.py and tests/test_vae_encoder_gpu.py against tests/golden/vae_{small,txt2audio}.npz
 // and vae_enc_{small,txt2audio}.npz (made by the reference modules) and the CPU oracles oracle/vae_ref.py and
 // oracle/vae_enc_ref.py.
-#include <memory>
 #include "common.cuh"
 #include "tapconv.cuh"
 #include "nn_kernels.h"
@@ -41,16 +40,6 @@ struct VLevel {
   bool up = false;            // decoder: ends in an Upsample (upconv)
   bool down = false;          // encoder: ends in a Downsample (downconv, im2col form [C][9*C])
   PackedConv upconv, downconv;
-};
-
-static void upload_vec_(DevBuf& d, const float* p, int n) { d.upload(std::vector<float>(p, p + n)); }
-
-// host weight arrays consumed in table order
-struct WeightCursor {
-  const float* const* W;
-  int n, idx = 0;
-  const float* next() { AGPT_CHECK(idx < n, "too few weight arrays"); return W[idx++]; }
-  void done() const { AGPT_CHECK(idx == n, "weight array count does not match the config"); }
 };
 
 // What the decoder and the encoder have in common: the layer drivers, the attention scratch and the rotating
@@ -155,9 +144,9 @@ struct VaeBase : Handle {
   void load_res(VResW& r, WeightCursor& wc, int cin, int cout) {
     r.cin = cin; r.cout = cout;
     AGPT_CHECK(cin % 32 == 0 && cout % 32 == 0, "ResnetBlock channels must be multiples of 32");
-    { auto g = wc.next(); auto b = wc.next(); upload_vec_(r.g1, g, cin); upload_vec_(r.b1, b, cin); }
+    { auto g = wc.next(); auto b = wc.next(); r.g1.upload(g, cin); r.b1.upload(b, cin); }
     { auto w = wc.next(); auto b = wc.next(); pack_conv(r.conv1, w, b, cout, cin, 9, true); }
-    { auto g = wc.next(); auto b = wc.next(); upload_vec_(r.g2, g, cout); upload_vec_(r.b2, b, cout); }
+    { auto g = wc.next(); auto b = wc.next(); r.g2.upload(g, cout); r.b2.upload(b, cout); }
     { auto w = wc.next(); auto b = wc.next(); pack_conv(r.conv2, w, b, cout, cout, 9, true); }
     if (cin != cout) { auto w = wc.next(); auto b = wc.next(); pack_conv(r.nin, w, b, cout, cin, 1, false); r.has_nin = true; }
   }
@@ -165,7 +154,7 @@ struct VaeBase : Handle {
     attns.emplace_back();
     VAttnW& a = attns.back();
     a.c = c;
-    { auto g = wc.next(); auto b = wc.next(); upload_vec_(a.g, g, c); upload_vec_(a.b, b, c); }
+    { auto g = wc.next(); auto b = wc.next(); a.g.upload(g, c); a.b.upload(b, c); }
     auto wq = wc.next(); auto bq = wc.next(); auto wk = wc.next(); auto bk = wc.next(); auto wv = wc.next(); auto bv = wc.next();
     std::vector<float> cat((size_t)3 * c * c), cb((size_t)3 * c);
     memcpy(&cat[0], wq, sizeof(float) * c * c); memcpy(&cat[(size_t)c * c], wk, sizeof(float) * c * c);
@@ -238,10 +227,10 @@ struct Vae : VaeBase {
 
 Handle* vae_create(const agpt_vae_cfg* cfg, const float* const* W, int nW, int device) {
   DeviceGuard dg_(device);
-  auto* v = new Vae();
-  v->magic = kMagicVae; v->device = device; v->cfg = *cfg;
   const int nl = cfg->num_levels;
   AGPT_CHECK(nl >= 1 && nl <= AGPT_MAX_LEVELS && cfg->ch % 32 == 0, "bad VAE config (ch must be a multiple of 32: GroupNorm(32))");
+  std::unique_ptr<Vae> v(new Vae());
+  v->magic = kMagicVae; v->device = device; v->cfg = *cfg;
   WeightCursor wc{W, nW};
   const int zc = cfg->z_channels, ed = cfg->embed_dim;
   v->cin_pad = round_up(std::max(zc, ed), 4);
@@ -282,10 +271,10 @@ Handle* vae_create(const agpt_vae_cfg* cfg, const float* const* W, int nW, int d
     if (l.up) { auto w = wc.next(); auto b = wc.next(); pack_conv(l.upconv, w, b, bo, bo, 9, true); }
   }
   v->last_ch = bi;
-  { auto g = wc.next(); auto b = wc.next(); upload_vec_(v->gno, g, bi); upload_vec_(v->bno, b, bi); }
+  { auto g = wc.next(); auto b = wc.next(); v->gno.upload(g, bi); v->bno.upload(b, bi); }
   { auto w = wc.next(); auto b = wc.next(); pack_conv(v->conv_out, w, b, cfg->out_ch, bi, 9, true); }
   wc.done();
-  return v;
+  return v.release();
 }
 
 void vae_decode(Handle* hh, const float* z, int B, int H, int W, float* out, cudaStream_t st) {
@@ -407,7 +396,7 @@ Handle* vae_encoder_create(const agpt_vae_cfg* cfg, int in_channels, const float
   v->mid_attn = v->load_attn(wc, bi);
   v->load_res(v->mid2, wc, bi, bi);
   v->last_ch = bi;
-  { auto g = wc.next(); auto b = wc.next(); upload_vec_(v->gno, g, bi); upload_vec_(v->bno, b, bi); }
+  { auto g = wc.next(); auto b = wc.next(); v->gno.upload(g, bi); v->bno.upload(b, bi); }
   {  // conv_out [2z][C][3][3] followed by quant_conv [2e][2z][1][1]: one 3x3 conv [2e][C][3][3], composed in fp64
     const int z2 = 2 * cfg->z_channels, e2 = 2 * cfg->embed_dim;
     auto w = wc.next(); auto b = wc.next(); auto qw = wc.next(); auto qb = wc.next();

@@ -28,11 +28,12 @@ from ... import _lib, paramtree, specs
 from ..modules.distributions.distributions import DiagonalGaussianDistribution
 
 
-class AutoencoderKL(nn.Module, _lib.HandleOwner):
+class AutoencoderKL(nn.Module):
+    _h = _lib.engine_handle
+
     def __init__(self, ddconfig, lossconfig=None, embed_dim=4, ckpt_path=None, ignore_keys=(), image_key="image",
                  colorize_nlabels=None, monitor=None):
-        nn.Module.__init__(self)
-        _lib.HandleOwner.__init__(self)
+        super().__init__()
         dd = dict(ddconfig)
         assert dd.get("double_z", True), "AutoencoderKL needs double_z (autoencoder.py:320)"
         if dd.get("attn_type", "vanilla") != "vanilla" or dd.get("use_linear_attn", False):
@@ -47,7 +48,7 @@ class AutoencoderKL(nn.Module, _lib.HandleOwner):
                         attn_resolutions=[int(v) for v in dd["attn_resolutions"]], dropout=0.0, double_z=True)
         self._shapes = specs.vae_decoder_param_shapes(self.cfg)
         paramtree.build(self, self._shapes)
-        self._engine_sig = None
+        self._engine = _lib.Engine("agpt_vae_create")
         if monitor is not None:
             self.monitor = monitor
         if ckpt_path is not None:
@@ -73,32 +74,22 @@ class AutoencoderKL(nn.Module, _lib.HandleOwner):
             c.attn_at_level[i] = 1 if (cfg["resolution"] // 2 ** i) in cfg["attn_resolutions"] else 0
         return c
 
-    def _ensure_engine(self, device):
-        sig = (paramtree.params_signature(self, self._shapes), device.index)
-        if self._h.value and sig == self._engine_sig:
-            return
-        self._destroy()
-        _lib.require_cuda()
-        arr, keep = _lib.host_weight_array([paramtree.get_param(self, k).data for k in self._shapes])
-        cfg = self._cfg_struct()
-        h = C.c_void_p()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        _lib.check(_lib.lib().agpt_vae_create(C.byref(cfg), arr, len(keep), idx, C.byref(h)))
-        self._h = h
-        self._engine_sig = sig
+    def _build(self, engine, shapes, device, *args):
+        """Build ``engine`` from the parameters named in ``shapes``; ``args``: the create call's arguments after the cfg."""
+        ws = [paramtree.get_tensor(self, k) for k in shapes]
+        engine.ensure(device, ws, lambda: ((C.byref(self._cfg_struct()),) + args, ws))
 
     @torch.no_grad()
     def decode(self, z):
         """z [B, embed_dim, H, W] -> [B, out_ch, H * 2^(levels-1), W * 2^(levels-1)]  (autoencoder.py:351-354)"""
         if not z.is_cuda:
             raise RuntimeError("audiogpt_b200.AutoencoderKL runs on CUDA only (no CPU fallback)")
-        self._ensure_engine(z.device)
+        self._build(self._engine, self._shapes, z.device)
         z = z.contiguous().float()
         B, _, H, W = z.shape
         f = 2 ** (len(self.cfg["ch_mult"]) - 1)
         out = torch.empty((B, self.cfg["out_ch"], H * f, W * f), device=z.device, dtype=torch.float32)
-        with torch.cuda.device(z.device):
-            _lib.check(_lib.lib().agpt_vae_decode(self._h, _lib.fptr(z), B, H, W, _lib.fptr(out), _lib.cur_stream(z.device)))
+        self._engine.call("vae_decode", z.device, _lib.fptr(z), B, H, W, _lib.fptr(out))
         return out
 
     def encode(self, x):
@@ -125,25 +116,9 @@ class AutoencoderKLWithEncoder(AutoencoderKL):
                          image_key=image_key, colorize_nlabels=colorize_nlabels, monitor=monitor)
         self._enc_shapes = specs.vae_encoder_param_shapes(self.cfg)
         paramtree.build(self, self._enc_shapes)
-        self._enc = _lib.HandleOwner()
-        self._enc_sig = None
+        self._enc_engine = _lib.Engine("agpt_vae_encoder_create")
         if ckpt_path is not None:
             self.init_from_ckpt(ckpt_path, ignore_keys=ignore_keys)
-
-    def _ensure_encoder(self, device):
-        sig = (paramtree.params_signature(self, self._enc_shapes), device.index)
-        if self._enc._h.value and sig == self._enc_sig:
-            return
-        self._enc._destroy()
-        _lib.require_cuda()
-        arr, keep = _lib.host_weight_array([paramtree.get_param(self, k).data for k in self._enc_shapes])
-        cfg = self._cfg_struct()
-        h = C.c_void_p()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        _lib.check(_lib.lib().agpt_vae_encoder_create(C.byref(cfg), self.cfg["in_channels"], arr, len(keep), idx,
-                                                      C.byref(h)))
-        self._enc._h = h
-        self._enc_sig = sig
 
     @torch.no_grad()
     def encode(self, x):
@@ -153,14 +128,12 @@ class AutoencoderKLWithEncoder(AutoencoderKL):
             raise RuntimeError("audiogpt_b200.AutoencoderKLWithEncoder runs on CUDA only (no CPU fallback)")
         if x.dim() != 4 or x.shape[1] != self.cfg["in_channels"]:
             raise ValueError(f"expected x of shape [B, {self.cfg['in_channels']}, H, W], got {tuple(x.shape)}")
-        self._ensure_encoder(x.device)
+        self._build(self._enc_engine, self._enc_shapes, x.device, self.cfg["in_channels"])
         x = x.contiguous().float()
         B, _, H, W = x.shape
         f = 2 ** (len(self.cfg["ch_mult"]) - 1)
         moments = torch.empty((B, 2 * self.embed_dim, H // f, W // f), device=x.device, dtype=torch.float32)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().agpt_vae_encode(self._enc._h, _lib.fptr(x), B, H, W, _lib.fptr(moments),
-                                                  _lib.cur_stream(x.device)))
+        self._enc_engine.call("vae_encode", x.device, _lib.fptr(x), B, H, W, _lib.fptr(moments))
         return (self._posterior_cls or DiagonalGaussianDistribution)(moments)
 
     def forward(self, input, sample_posterior=True):

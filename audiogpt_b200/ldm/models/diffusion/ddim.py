@@ -212,12 +212,9 @@ class DDIMSampler(object):
         ci = (C.c_int * S)(*[int(s) for s in order])
         fa = lambda t: (C.c_float * S)(*[float(t[j]) for j in idx])
         out, p0 = torch.empty_like(x), torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().agpt_unet_ddim_sample(
-                unet._h, _lib.fptr(x), B, H, W, S, ci, fa(self._h_alphas), fa(self._h_alphas_prev),
-                fa(self._h_sigmas), fa(self._h_sqrt_one_minus_alphas),
-                C.c_float(float(scale) if guided else 1.0), _lib.fptr(out), _lib.fptr(p0),
-                _lib.cur_stream(x.device)))
+        _lib.call("unet_ddim_sample", x.device, unet._h, _lib.fptr(x), B, H, W, S, ci, fa(self._h_alphas),
+                  fa(self._h_alphas_prev), fa(self._h_sigmas), fa(self._h_sqrt_one_minus_alphas),
+                  float(scale) if guided else 1.0, _lib.fptr(out), _lib.fptr(p0))
         return out, p0
 
     @torch.no_grad()
@@ -262,12 +259,9 @@ class DDIMSampler(object):
             noise = torch.nn.functional.dropout(noise, p=noise_dropout)
         x = x.contiguous().float(); e2 = e2.contiguous().float()
         x_prev, pred_x0 = torch.empty_like(x), torch.empty_like(x)
-        with torch.cuda.device(device):
-            _lib.check(_lib.lib().agpt_ddim_update(
-                _lib.fptr(x), _lib.fptr(e2), 1 if single else 0, C.c_float(float(unconditional_guidance_scale)),
-                C.c_float(a_t), C.c_float(a_prev), C.c_float(sg), C.c_float(sq),
-                _lib.fptr(noise) if noise is not None else None, C.c_float(float(temperature)), b,
-                C.c_long(x[0].numel()), _lib.fptr(x_prev), _lib.fptr(pred_x0), _lib.cur_stream(device)))
+        _lib.call("ddim_update", device, _lib.fptr(x), _lib.fptr(e2), 1 if single else 0, float(unconditional_guidance_scale),
+                  a_t, a_prev, sg, sq, _lib.fptr(noise) if noise is not None else None, float(temperature), b,
+                  x[0].numel(), _lib.fptr(x_prev), _lib.fptr(pred_x0))
         if quantize_denoised:
             raise NotImplementedError("quantize_denoised needs a VQ first stage (not on the AudioGPT path)")
         return x_prev, pred_x0

@@ -41,7 +41,7 @@ def _unsupported(kw):
     return bad
 
 
-class UNetModel(nn.Module, _lib.HandleOwner):
+class UNetModel(nn.Module):
     # Set by audiogpt_b200.install(): the reference's own UNetModel class.  AudioGPT also builds UNets this back-end
     # does not cover (the inpainting model's AttentionBlock UNet, openaimodel.py:278-410); since install() replaces the
     # class object inside the reference module, constructing one of THOSE configs returns an instance of the
@@ -49,6 +49,7 @@ class UNetModel(nn.Module, _lib.HandleOwner):
     # This is a routing of unsupported model VARIANTS, not a fallback of the accelerated path: a supported config
     # never leaves the CUDA engine, and without install() (no reference class known) unsupported configs raise.
     _reference_cls = None
+    _h = _lib.engine_handle
 
     def __new__(cls, *args, **kwargs):
         if cls is UNetModel and cls._reference_cls is not None and not args and _unsupported(kwargs):
@@ -62,7 +63,6 @@ class UNetModel(nn.Module, _lib.HandleOwner):
                  use_new_attention_order=False, use_spatial_transformer=False, transformer_depth=1,
                  context_dim=None, n_embed=None, legacy=True):
         nn.Module.__init__(self)
-        _lib.HandleOwner.__init__(self)
         unsupported = _unsupported(dict(dims=dims, conv_resample=conv_resample, num_classes=num_classes, use_fp16=use_fp16,
                                         use_scale_shift_norm=use_scale_shift_norm, resblock_updown=resblock_updown,
                                         use_spatial_transformer=use_spatial_transformer, n_embed=n_embed,
@@ -85,7 +85,7 @@ class UNetModel(nn.Module, _lib.HandleOwner):
                         context_dim=self.context_dim, legacy=legacy)
         self._shapes = specs.unet_param_shapes(self.cfg)
         paramtree.build(self, self._shapes)
-        self._engine_sig = None
+        self._engine = _lib.Engine("agpt_unet_create")
         self._ctx_key = None
 
     # ------------------------------------------------------------------ engine
@@ -100,34 +100,19 @@ class UNetModel(nn.Module, _lib.HandleOwner):
         c.transformer_depth, c.context_dim = self.transformer_depth, self.context_dim
         return c
 
-    def _ensure_engine(self, device):
-        sig = (paramtree.params_signature(self), device.index)
-        if self._h.value and sig == self._engine_sig:
-            return
-        self._destroy()
-        _lib.require_cuda()
-        arr, keep = _lib.host_weight_array([paramtree.get_param(self, k).data for k in self._shapes])
-        cfg = self._cfg_struct()
-        h = C.c_void_p()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        _lib.check(_lib.lib().agpt_unet_create(C.byref(cfg), arr, len(keep), idx, C.byref(h)))
-        self._h = h
-        self._engine_sig = sig
-        self._ctx_key = None
-
     def set_context(self, context: torch.Tensor):
         """context [N, S, context_dim]: hoists to_k/to_v(context) of all cross-attentions; cached per tensor."""
         if not context.is_cuda:
             raise RuntimeError("audiogpt_b200.UNetModel runs on CUDA only (no CPU fallback)")
-        self._ensure_engine(context.device)
+        ws = [paramtree.get_tensor(self, k) for k in self._shapes]
+        if self._engine.ensure(context.device, ws, lambda: ((C.byref(self._cfg_struct()),), ws)):
+            self._ctx_key = None
         key = (context.data_ptr(), context._version, tuple(context.shape))
         if key == self._ctx_key:
             return
         c = context.contiguous().float()
         assert c.dim() == 3 and c.shape[2] == self.context_dim, "context must be [N, S, context_dim]"
-        with torch.cuda.device(c.device):
-            _lib.check(_lib.lib().agpt_unet_set_context(self._h, _lib.fptr(c), c.shape[0], c.shape[1],
-                                                         _lib.cur_stream(c.device)))
+        self._engine.call("unet_set_context", c.device, _lib.fptr(c), c.shape[0], c.shape[1])
         self._ctx_key = key
         # keep BOTH tensors alive while the key is live: `c` is what the engine read, `context` is what the key
         # was computed from (when they differ -- fp16 / non-contiguous input -- a freed `context` could hand its
@@ -145,9 +130,7 @@ class UNetModel(nn.Module, _lib.HandleOwner):
         t = timesteps.tolist() if torch.is_tensor(timesteps) else [int(v) for v in timesteps]
         tt = (C.c_int * N)(*[int(v) for v in t])
         out = torch.empty((N, self.out_channels, H, W), device=x.device, dtype=torch.float32)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().agpt_unet_forward(self._h, _lib.fptr(x), tt, N, H, W, _lib.fptr(out),
-                                                     _lib.cur_stream(x.device)))
+        self._engine.call("unet_forward", x.device, _lib.fptr(x), tt, N, H, W, _lib.fptr(out))
         return out
 
     def convert_to_fp16(self):  # API parity; the engine computes in fp32

@@ -23,10 +23,11 @@ from ... import _lib, paramtree, specs
 from ...utils import hparams as _hp
 
 
-class DiffNet(nn.Module, _lib.HandleOwner):
+class DiffNet(nn.Module):
+    _h = _lib.engine_handle
+
     def __init__(self, in_dims=80, **overrides):
-        nn.Module.__init__(self)
-        _lib.HandleOwner.__init__(self)
+        super().__init__()
         hp = dict(_hp.resolve())
         hp.update(overrides)
         self.cfg = dict(in_dims=in_dims, hidden_size=hp["hidden_size"],
@@ -35,36 +36,21 @@ class DiffNet(nn.Module, _lib.HandleOwner):
                         dilation_cycle_length=hp["dilation_cycle_length"])
         self._shapes = specs.diffnet_param_shapes(self.cfg)
         paramtree.build(self, self._shapes)
-        self._engine_sig = None
-        self._cond_key = None
-
-    def _ensure_engine(self, device):
-        sig = (paramtree.params_signature(self), device.index)
-        if self._h.value and sig == self._engine_sig:
-            return
-        self._destroy()
-        _lib.require_cuda()
-        cfg = _lib.DiffnetCfg(**self.cfg)
-        arr, keep = _lib.host_weight_array([paramtree.get_param(self, k).data for k in self._shapes])
-        h = C.c_void_p()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        _lib.check(_lib.lib().agpt_diffnet_create(C.byref(cfg), arr, len(keep), idx, C.byref(h)))
-        self._h = h
-        self._engine_sig = sig
+        self._engine = _lib.Engine("agpt_diffnet_create")
         self._cond_key = None
 
     def set_cond(self, cond: torch.Tensor):
         """cond [B, hidden, T]; cached until a different tensor (or an in-place change) arrives."""
         if not cond.is_cuda:
             raise RuntimeError("audiogpt_b200.DiffNet runs on CUDA only (no CPU fallback)")
-        self._ensure_engine(cond.device)
+        ws = [paramtree.get_tensor(self, k) for k in self._shapes]
+        if self._engine.ensure(cond.device, ws, lambda: ((C.byref(_lib.DiffnetCfg(**self.cfg)),), ws)):
+            self._cond_key = None
         key = (cond.data_ptr(), cond._version, tuple(cond.shape))
         if key == self._cond_key:
             return
         c = cond.contiguous().float()
-        with torch.cuda.device(cond.device):
-            _lib.check(_lib.lib().agpt_diffnet_set_cond(self._h, _lib.fptr(c), c.shape[0], c.shape[2],
-                                                         _lib.cur_stream(cond.device)))
+        self._engine.call("diffnet_set_cond", cond.device, _lib.fptr(c), c.shape[0], c.shape[2])
         self._cond_key = key
         # hold the keyed tensor: while it is alive the caching allocator cannot hand its block to the next
         # utterance's decoder_inp (same B/T/H, version 0), which would make the key match a different cond
@@ -81,6 +67,5 @@ class DiffNet(nn.Module, _lib.HandleOwner):
         assert len(t) == B
         tt = (C.c_int * B)(*[int(v) for v in t])
         out = torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().agpt_diffnet_eps(self._h, _lib.fptr(x), tt, _lib.fptr(out), _lib.cur_stream(x.device)))
+        self._engine.call("diffnet_eps", x.device, _lib.fptr(x), tt, _lib.fptr(out))
         return out

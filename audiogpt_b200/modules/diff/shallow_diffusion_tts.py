@@ -164,22 +164,15 @@ class GaussianDiffusion(nn.Module):
         out = torch.empty_like(x)
         tt = (C.c_int * b)(*tl)
         n = x[0].numel()
-        L = _lib.lib()
-        with torch.cuda.device(x.device):
-            st = _lib.cur_stream(x.device)
-            if self._fast():
-                self.denoise_fn.set_cond(cond)
-                _lib.check(L.agpt_gd_p_sample(self.denoise_fn._h, _lib.fptr(x), None, tt,
-                                              coef.ctypes.data_as(C.c_void_p),
-                                              _lib.fptr(noise) if noise is not None else None,
-                                              1 if clip_denoised else 0, b, C.c_long(n), _lib.fptr(out), st))
-            else:
-                eps = self.denoise_fn(x, torch.tensor(tl, device=x.device, dtype=torch.long), cond=cond)
-                eps = eps.contiguous().float()
-                _lib.check(L.agpt_gd_p_sample(None, _lib.fptr(x), _lib.fptr(eps), tt,
-                                              coef.ctypes.data_as(C.c_void_p),
-                                              _lib.fptr(noise) if noise is not None else None,
-                                              1 if clip_denoised else 0, b, C.c_long(n), _lib.fptr(out), st))
+        if self._fast():
+            self.denoise_fn.set_cond(cond)
+            h, eps = self.denoise_fn._h, None
+        else:
+            eps = self.denoise_fn(x, torch.tensor(tl, device=x.device, dtype=torch.long), cond=cond)
+            h, eps = None, eps.contiguous().float()
+        _lib.call("gd_p_sample", x.device, h, _lib.fptr(x), _lib.fptr(eps) if eps is not None else None, tt,
+                  coef.ctypes.data_as(C.c_void_p), _lib.fptr(noise) if noise is not None else None,
+                  1 if clip_denoised else 0, b, n, _lib.fptr(out))
         return out
 
     def _eps(self, x, tl, cond):
@@ -193,9 +186,7 @@ class GaussianDiffusion(nn.Module):
         coef[:, :len(rows[0])] = np.asarray(rows, dtype=np.float32)
         ptrs = [_lib.fptr(e) for e in es] + [None] * (4 - len(es))
         out = torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().agpt_axpby5(_lib.fptr(x), *ptrs, coef.ctypes.data_as(C.c_void_p), b,
-                                              C.c_long(x[0].numel()), _lib.fptr(out), _lib.cur_stream(x.device)))
+        _lib.call("axpby5", x.device, _lib.fptr(x), *ptrs, coef.ctypes.data_as(C.c_void_p), b, x[0].numel(), _lib.fptr(out))
         return out
 
     def _plms_scalars(self, tv, interval):
@@ -284,7 +275,6 @@ class GaussianDiffusion(nn.Module):
         self.denoise_fn.set_cond(cond)
         per_step = b * n * 4
         chunk = max(1, min(t0, self.NOISE_CHUNK_BYTES // max(per_step, 1)))
-        L = _lib.lib()
         t_hi = t0
         while t_hi > 0:
             t_lo = max(0, t_hi - chunk)
@@ -301,10 +291,8 @@ class GaussianDiffusion(nn.Module):
                 tv = t_hi - 1 - k
                 coef[k] = (tb["A"][tv], tb["B"][tv], tb["c1"][tv], tb["c2"][tv],
                            float(tb["sigma"][tv]) if tv != 0 else 0.0)
-            with torch.cuda.device(x.device):
-                _lib.check(L.agpt_gd_sample_loop(self.denoise_fn._h, _lib.fptr(x), t_hi, t_lo,
-                                                 coef.ctypes.data_as(C.c_void_p), _lib.fptr(bank),
-                                                 C.c_long(b * n), 1, _lib.cur_stream(x.device)))
+            _lib.call("gd_sample_loop", x.device, self.denoise_fn._h, _lib.fptr(x), t_hi, t_lo,
+                      coef.ctypes.data_as(C.c_void_p), _lib.fptr(bank), b * n, 1)
             t_hi = t_lo
         return x
 

@@ -59,12 +59,12 @@ def fs2_config(hp, n_tokens, out_dims, use_midi):
                 use_energy_embed=int(bool(hp.get("use_energy_embed", False))), use_midi=int(use_midi))
 
 
-class FastSpeech2(nn.Module, _lib.HandleOwner):
+class FastSpeech2(nn.Module):
     _use_midi = False
+    _h = _lib.engine_handle
 
     def __init__(self, dictionary, out_dims=None):
-        nn.Module.__init__(self)
-        _lib.HandleOwner.__init__(self)
+        super().__init__()
         hp = _hp.resolve()
         self.dictionary = dictionary
         self.padding_idx = dictionary.pad()
@@ -80,36 +80,12 @@ class FastSpeech2(nn.Module, _lib.HandleOwner):
             if key == "encoder.embed_tokens.weight":
                 continue
             if key.endswith("_float_tensor"):
-                parts = key.split(".")
-                paramtree._descend(self, parts[:-1]).register_buffer(parts[-1], torch.zeros(shape))
+                paramtree.add_buffer(self, key, torch.zeros(shape))
             else:
                 paramtree.add_param(self, key, torch.zeros(shape))
         # FastspeechEncoder holds the same Embedding object as encoder_embed_tokens (fs2.py:30,36)
-        paramtree._descend(self, ["encoder", "embed_tokens"]).register_parameter(
-            "weight", paramtree.get_param(self, "encoder_embed_tokens.weight"))
-        self._engine_sig = None
-
-    def _tensor(self, key):
-        parts = key.split(".")
-        node = self
-        for p in parts[:-1]:
-            node = node._modules[p]
-        t = node._parameters.get(parts[-1])
-        return t if t is not None else node._buffers[parts[-1]]
-
-    def _ensure_engine(self, device):
-        sig = (tuple((self._tensor(k).data_ptr(), self._tensor(k)._version) for k in self._shapes), device.index)
-        if self._h.value and sig == self._engine_sig:
-            return
-        self._destroy()
-        _lib.require_cuda()
-        arr, keep = _lib.host_weight_array([self._tensor(k).data.float() for k in self._shapes])
-        cfg = _lib.Fs2Cfg(**dict(self.cfg, pitch_type=_PITCH_TYPES[self.cfg["pitch_type"]]))
-        h = C.c_void_p()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        _lib.check(_lib.lib().agpt_fs2_create(C.byref(cfg), arr, len(keep), idx, C.byref(h)))
-        self._h = h
-        self._engine_sig = sig
+        paramtree.add_param(self, "encoder.embed_tokens.weight", paramtree.get_param(self, "encoder_embed_tokens.weight"))
+        self._engine = _lib.Engine("agpt_fs2_create")
 
     @torch.no_grad()
     def forward(self, txt_tokens, mel2ph=None, spk_embed=None, ref_mels=None, f0=None, uv=None, energy=None,
@@ -126,8 +102,9 @@ class FastSpeech2(nn.Module, _lib.HandleOwner):
             raise RuntimeError("audiogpt_b200.FastSpeech2 runs on CUDA only (no CPU fallback)")
         hp = _hp.resolve()
         dev = txt_tokens.device
-        self._ensure_engine(dev)
-        L = _lib.lib()
+        ws = [paramtree.get_tensor(self, k) for k in self._shapes]
+        self._engine.ensure(dev, ws, lambda: (
+            (C.byref(_lib.Fs2Cfg(**dict(self.cfg, pitch_type=_PITCH_TYPES[self.cfg["pitch_type"]]))),), ws))
         i32 = dict(device=dev, dtype=torch.int32)
         f32 = dict(device=dev, dtype=torch.float32)
         tok = txt_tokens.to(**i32).contiguous()
@@ -140,39 +117,35 @@ class FastSpeech2(nn.Module, _lib.HandleOwner):
         ptr = lambda t: None if t is None else _lib.fptr(t)   # noqa: E731
         ret = {}
         pitch_type = self.cfg["pitch_type"]
-        with torch.cuda.device(dev):
-            st = _lib.cur_stream(dev)
-            dur = torch.empty((B, Tt), **f32)
-            if mel2ph is None:
-                dch = torch.empty((B, Tt), **i32)
-                mel_len = (C.c_int * B)()
-                _lib.check(L.agpt_fs2_encode(self._h, ptr(tok), B, Tt, *map(ptr, midi), 1, ptr(dur), ptr(dch), mel_len, st))
-                Tm = max(mel_len)
-                ret["dur"] = dur[:, :, None]
-                ret["dur_choice"] = dch.long()
-                m2p_in, m2p_out = None, torch.empty((B, Tm), **i32)
-            else:
-                _lib.check(L.agpt_fs2_encode(self._h, ptr(tok), B, Tt, *map(ptr, midi), 0, ptr(dur), None, None, st))
-                ret["dur"] = dur
-                Tm = mel2ph.shape[1]
-                m2p_in, m2p_out = mel2ph.to(**i32).contiguous(), None
-            grid = Tt if pitch_type == "ph" else Tm
-            pitch_pred = f0d = coarse = energy_pred = mel_out = None
-            if pitch_type is not None:
-                pitch_pred = torch.empty((B, grid, 2 if pitch_type == "frame" else 1), **f32)
-                f0d = torch.empty((B, grid), **f32)
-                coarse = torch.empty((B, grid), **i32)
-            if self.cfg["use_energy_embed"]:
-                energy_pred = torch.empty((B, Tm), **f32)
-            decoder_inp = torch.empty((B, Tm, self.hidden_size), **f32)
-            if not skip_decoder:
-                mel_out = torch.empty((B, Tm, self.out_dims), **f32)
-            tf = [None if t is None else t.to(**f32).contiguous() for t in (f0, uv, energy)]
-            _lib.check(L.agpt_fs2_decode(
-                self._h, Tm, ptr(m2p_in), ptr(m2p_out), *map(ptr, tf), int(bool(hp.get("use_uv"))),
-                _NORMS.get(hp.get("pitch_norm"), 0), C.c_float(float(hp.get("f0_mean", 0.0))),
-                C.c_float(float(hp.get("f0_std", 1.0))), ptr(pitch_pred), ptr(f0d), ptr(coarse), ptr(energy_pred),
-                ptr(decoder_inp), ptr(mel_out), st))
+        dur = torch.empty((B, Tt), **f32)
+        if mel2ph is None:
+            dch = torch.empty((B, Tt), **i32)
+            mel_len = (C.c_int * B)()
+            self._engine.call("fs2_encode", dev, ptr(tok), B, Tt, *map(ptr, midi), 1, ptr(dur), ptr(dch), mel_len)
+            Tm = max(mel_len)
+            ret["dur"] = dur[:, :, None]
+            ret["dur_choice"] = dch.long()
+            m2p_in, m2p_out = None, torch.empty((B, Tm), **i32)
+        else:
+            self._engine.call("fs2_encode", dev, ptr(tok), B, Tt, *map(ptr, midi), 0, ptr(dur), None, None)
+            ret["dur"] = dur
+            Tm = mel2ph.shape[1]
+            m2p_in, m2p_out = mel2ph.to(**i32).contiguous(), None
+        grid = Tt if pitch_type == "ph" else Tm
+        pitch_pred = f0d = coarse = energy_pred = mel_out = None
+        if pitch_type is not None:
+            pitch_pred = torch.empty((B, grid, 2 if pitch_type == "frame" else 1), **f32)
+            f0d = torch.empty((B, grid), **f32)
+            coarse = torch.empty((B, grid), **i32)
+        if self.cfg["use_energy_embed"]:
+            energy_pred = torch.empty((B, Tm), **f32)
+        decoder_inp = torch.empty((B, Tm, self.hidden_size), **f32)
+        if not skip_decoder:
+            mel_out = torch.empty((B, Tm, self.out_dims), **f32)
+        tf = [None if t is None else t.to(**f32).contiguous() for t in (f0, uv, energy)]
+        self._engine.call("fs2_decode", dev, Tm, ptr(m2p_in), ptr(m2p_out), *map(ptr, tf), int(bool(hp.get("use_uv"))),
+                          _NORMS.get(hp.get("pitch_norm"), 0), float(hp.get("f0_mean", 0.0)), float(hp.get("f0_std", 1.0)),
+                          ptr(pitch_pred), ptr(f0d), ptr(coarse), ptr(energy_pred), ptr(decoder_inp), ptr(mel_out))
         ret["mel2ph"] = mel2ph if mel2ph is not None else m2p_out.long()
         if pitch_type is not None:
             ret["pitch_pred"] = pitch_pred

@@ -20,10 +20,11 @@ from ...utils import hparams as _hp
 _BUFFER_SUFFIXES = ("running_mean", "running_var", "num_batches_tracked", "_float_tensor")
 
 
-class PitchExtractor(nn.Module, _lib.HandleOwner):
+class PitchExtractor(nn.Module):
+    _h = _lib.engine_handle
+
     def __init__(self, n_mel_bins=80, conv_layers=2):
-        nn.Module.__init__(self)
-        _lib.HandleOwner.__init__(self)
+        super().__init__()
         hp = _hp.resolve()
         self.hidden_size = int(hp["hidden_size"])
         ph = int(hp.get("predictor_hidden", -1))
@@ -37,37 +38,13 @@ class PitchExtractor(nn.Module, _lib.HandleOwner):
         self._shapes = specs.pe_param_shapes(self.cfg)
         for key, shape in self._shapes.items():
             if key.endswith(_BUFFER_SUFFIXES):      # registered as buffers, like the reference's BatchNorm1d / positional table
-                parts = key.split(".")
-                node = paramtree._descend(self, parts[:-1])
                 val = torch.zeros(shape, dtype=torch.long if key.endswith("num_batches_tracked") else torch.float32)
                 if key.endswith("running_var"):
                     val = torch.ones(shape)
-                node.register_buffer(parts[-1], val)
+                paramtree.add_buffer(self, key, val)
             else:
                 paramtree.add_param(self, key, torch.zeros(shape))
-        self._engine_sig = None
-
-    def _tensor(self, key):
-        parts = key.split(".")
-        node = self
-        for p in parts[:-1]:
-            node = node._modules[p]
-        t = node._parameters.get(parts[-1])
-        return t if t is not None else node._buffers[parts[-1]]
-
-    def _ensure_engine(self, device):
-        sig = (tuple((self._tensor(k).data_ptr(), self._tensor(k)._version) for k in self._shapes), device.index)
-        if self._h.value and sig == self._engine_sig:
-            return
-        self._destroy()
-        _lib.require_cuda()
-        arr, keep = _lib.host_weight_array([self._tensor(k).data.float() for k in self._shapes])
-        cfg = _lib.PeCfg(**self.cfg)
-        h = C.c_void_p()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        _lib.check(_lib.lib().agpt_pe_create(C.byref(cfg), arr, len(keep), idx, C.byref(h)))
-        self._h = h
-        self._engine_sig = sig
+        self._engine = _lib.Engine("agpt_pe_create")
 
     @torch.no_grad()
     def forward(self, mel_input=None):
@@ -75,15 +52,14 @@ class PitchExtractor(nn.Module, _lib.HandleOwner):
         if not mel_input.is_cuda:
             raise RuntimeError("audiogpt_b200.PitchExtractor runs on CUDA only (no CPU fallback)")
         hp = _hp.resolve()
-        self._ensure_engine(mel_input.device)
+        ws = [paramtree.get_tensor(self, k) for k in self._shapes]
+        self._engine.ensure(mel_input.device, ws, lambda: ((C.byref(_lib.PeCfg(**self.cfg)),), ws))
         mel = mel_input.contiguous().float()
         B, T, _ = mel.shape
         pred = torch.empty((B, T, 2), device=mel.device, dtype=torch.float32)
         f0 = torch.empty((B, T), device=mel.device, dtype=torch.float32)
         use_uv = 1 if (hp.get("pitch_type") == "frame" and hp.get("use_uv")) else 0
         norm = {"standard": 1, "log": 2}.get(hp.get("pitch_norm"), 0)
-        with torch.cuda.device(mel.device):
-            _lib.check(_lib.lib().agpt_pe_forward(self._h, _lib.fptr(mel), B, T, _lib.fptr(pred), _lib.fptr(f0), use_uv, norm,
-                                                  C.c_float(float(hp.get("f0_mean", 0.0))), C.c_float(float(hp.get("f0_std", 1.0))),
-                                                  _lib.cur_stream(mel.device)))
+        self._engine.call("pe_forward", mel.device, _lib.fptr(mel), B, T, _lib.fptr(pred), _lib.fptr(f0), use_uv, norm,
+                          float(hp.get("f0_mean", 0.0)), float(hp.get("f0_std", 1.0)))
         return {"pitch_pred": pred, "f0_denorm_pred": f0}

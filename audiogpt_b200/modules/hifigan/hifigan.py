@@ -91,30 +91,36 @@ class SourceModuleHnNSF(nn.Module):
         har = torch.empty((B, L), device=f0.device, dtype=torch.float32)
         ri = rand_ini.contiguous().float()
         nz = noise.contiguous().float()
-        with torch.cuda.device(f0.device):
-            _lib.check(_lib.lib().agpt_nsf_source(
-                _lib.fptr(f0c), B, L, dim, C.c_float(float(self.sampling_rate)), w.ctypes.data_as(C.c_void_p),
-                C.c_float(b), _lib.fptr(ri), _lib.fptr(nz), C.c_float(float(self.sine_amp)),
-                C.c_float(float(self.noise_std)), C.c_float(float(self.voiced_threshold)), _lib.fptr(har),
-                _lib.cur_stream(f0.device)))
+        _lib.call("nsf_source", f0.device, _lib.fptr(f0c), B, L, dim, float(self.sampling_rate), w.ctypes.data_as(C.c_void_p),
+                  b, _lib.fptr(ri), _lib.fptr(nz), float(self.sine_amp), float(self.noise_std), float(self.voiced_threshold),
+                  _lib.fptr(har))
         uv = (f0 > self.voiced_threshold).to(f0.dtype)
         return har[:, :, None], noise_src, uv
 
 
-class HifiGanGenerator(nn.Module, _lib.HandleOwner):
+class HifiGanGenerator(nn.Module):
+    _h = _lib.engine_handle
+
     def __init__(self, h, c_out=1):
-        nn.Module.__init__(self)
-        _lib.HandleOwner.__init__(self)
+        super().__init__()
         self.h = h
-        self.c_out = c_out
-        self.num_kernels = len(h["resblock_kernel_sizes"])
-        self.num_upsamples = len(h["upsample_rates"])
-        self.hop = int(np.prod(h["upsample_rates"]))
-        self._use_nsf = bool(h.get("use_pitch_embed", False))
-        self._shapes = specs.hifigan_param_shapes(h, c_out)
+        self._init_generator(dict(h, activation=0, snake_logscale=0), c_out, specs.hifigan_param_shapes(h, c_out),
+                             bool(h.get("use_pitch_embed", False)))
+        if self._use_nsf:
+            self.harmonic_num = 8
+            self.m_source = SourceModuleHnNSF(sampling_rate=h["audio_sample_rate"], harmonic_num=self.harmonic_num)
+
+    def _init_generator(self, hd, c_out, shapes, use_nsf):
+        """What HiFi-GAN and BigVGAN share.  ``hd``: the config with HiFi-GAN's keys plus ``activation`` (0 leaky-relu,
+        1 snake, 2 snakebeta) and ``snake_logscale`` (0 / 1); ``shapes``: the folded state-dict table."""
+        self._hd, self.c_out, self._shapes, self._use_nsf = hd, c_out, shapes, use_nsf
+        self.num_kernels = len(hd["resblock_kernel_sizes"])
+        self.num_upsamples = len(hd["upsample_rates"])
+        self.hop = int(np.prod(hd["upsample_rates"]))
         self._weight_norm = True
+        self._engine = _lib.Engine("agpt_hifigan_create")
         g = torch.Generator().manual_seed(0)
-        for key, shape in self._shapes.items():
+        for key, shape in shapes.items():
             if key.startswith("m_source."):
                 continue
             if _wn_key(key):
@@ -123,11 +129,10 @@ class HifiGanGenerator(nn.Module, _lib.HandleOwner):
                 paramtree.add_param(self, key + "_g", n.clone())
                 paramtree.add_param(self, key + "_v", v)
             else:
-                paramtree.add_param(self, key, torch.zeros(shape))
-        if self._use_nsf:
-            self.harmonic_num = 8
-            self.m_source = SourceModuleHnNSF(sampling_rate=h["audio_sample_rate"], harmonic_num=self.harmonic_num)
-        self._engine_sig = None
+                paramtree.add_param(self, key, self._initial_value(key, shape))
+
+    def _initial_value(self, key, shape):
+        return torch.zeros(shape)
 
     # ------------------------------------------------------------------ weight-norm
     def remove_weight_norm(self):
@@ -143,7 +148,6 @@ class HifiGanGenerator(nn.Module, _lib.HandleOwner):
             paramtree.del_param(self, key + "_v")
             paramtree.add_param(self, key, w)
         self._weight_norm = False
-        self._engine_sig = None
 
     def load_state_dict(self, state_dict, strict=True, **kw):
         has_wn = any(k.endswith(".weight_g") for k in state_dict)
@@ -158,16 +162,13 @@ class HifiGanGenerator(nn.Module, _lib.HandleOwner):
                 elif not k.endswith(".weight_v"):
                     sd[k] = v
             state_dict = sd
-        self._engine_sig = None
         return super().load_state_dict(state_dict, strict=strict, **kw)
 
     def folded_weights(self):
         """fp32 tensors in specs.hifigan_param_shapes order, weight-norm folded."""
         out = []
         for key in self._shapes:
-            if key.startswith("m_source."):
-                out.append(paramtree.get_param(self, key).data)
-            elif self._weight_norm and _wn_key(key):
+            if self._weight_norm and _wn_key(key):
                 out.append(fold_weight_norm(paramtree.get_param(self, key + "_g").data,
                                             paramtree.get_param(self, key + "_v").data))
             else:
@@ -176,38 +177,29 @@ class HifiGanGenerator(nn.Module, _lib.HandleOwner):
 
     # ------------------------------------------------------------------ engine
     def _cfg(self):
-        h = self.h
+        hd = self._hd
         c = _lib.HifiganCfg()
         # the reference hard-codes Conv1d(80, ...) for conv_pre (hifigan.py:118); take it from the parameter table
         c.n_mels, c.c_out = int(self._shapes["conv_pre.weight"][1]), self.c_out
-        c.upsample_initial_channel = int(h["upsample_initial_channel"])
+        c.upsample_initial_channel = int(hd["upsample_initial_channel"])
         c.num_upsamples = self.num_upsamples
-        for i, (u, k) in enumerate(zip(h["upsample_rates"], h["upsample_kernel_sizes"])):
+        for i, (u, k) in enumerate(zip(hd["upsample_rates"], hd["upsample_kernel_sizes"])):
             c.upsample_rates[i], c.upsample_kernel_sizes[i] = int(u), int(k)
-        c.resblock_type = 1 if str(h["resblock"]) == "1" else 2
+        c.resblock_type = 1 if str(hd["resblock"]) == "1" else 2
         c.num_kernels = self.num_kernels
-        for j, (ks, dil) in enumerate(zip(h["resblock_kernel_sizes"], h["resblock_dilation_sizes"])):
+        for j, (ks, dil) in enumerate(zip(hd["resblock_kernel_sizes"], hd["resblock_dilation_sizes"])):
             c.resblock_kernel_sizes[j] = int(ks)
             c.resblock_num_dilations[j] = len(dil)
             for n, d in enumerate(dil):
                 c.resblock_dilations[j][n] = int(d)
-        c.use_nsf = 1 if self._use_nsf else 0
+        c.use_nsf = int(self._use_nsf)
+        c.activation, c.snake_logscale = hd["activation"], hd["snake_logscale"]
         return c
 
-    def _ensure_engine(self, device: torch.device):
-        sig = (paramtree.params_signature(self), device.index)
-        if self._h.value and sig == self._engine_sig:
-            return
-        self._destroy()
-        _lib.require_cuda()
-        L = _lib.lib()
-        arr, keep = _lib.host_weight_array(self.folded_weights())
-        cfg = self._cfg()
-        h = C.c_void_p()
-        idx = device.index if device.index is not None else torch.cuda.current_device()
-        _lib.check(L.agpt_hifigan_create(C.byref(cfg), arr, len(keep), idx, C.byref(h)))
-        self._h = h
-        self._engine_sig = sig
+    def _build_engine(self, device):
+        # the weight-norm layout changes the keys, so the engine is signed by the whole state dict
+        self._engine.ensure(device, self.state_dict(keep_vars=True).values(),
+                            lambda: ((C.byref(self._cfg()),), self.folded_weights()))
 
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
@@ -218,7 +210,7 @@ class HifiGanGenerator(nn.Module, _lib.HandleOwner):
                                "move the model and input to a CUDA device (H100)")
         x = x.contiguous().float()
         B, M, T = x.shape
-        self._ensure_engine(x.device)
+        self._build_engine(x.device)
         har = None
         if f0 is not None:
             if not self._use_nsf:
@@ -227,17 +219,15 @@ class HifiGanGenerator(nn.Module, _lib.HandleOwner):
             har, _, _ = self.m_source(f0u)
             har = har.transpose(1, 2).contiguous()
         wav = torch.empty((B, self.c_out, T * self.hop), device=x.device, dtype=torch.float32)
-        with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().agpt_hifigan_forward(
-                self._h, _lib.fptr(x), _lib.fptr(har) if har is not None else None,
-                B, T, _lib.fptr(wav), _lib.cur_stream(x.device)))
+        self._engine.call("hifigan_forward", x.device, _lib.fptr(x), _lib.fptr(har) if har is not None else None,
+                          B, T, _lib.fptr(wav))
         return wav
 
     @torch.no_grad()
     def vocode_host(self, mel: np.ndarray, har: np.ndarray = None, device=None) -> np.ndarray:
         """Host-buffer entry (numpy [B,80,T] -> numpy [B,c_out,T*hop]); H2D/D2H inside the call."""
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        self._ensure_engine(dev)
+        self._build_engine(dev)
         mel = np.ascontiguousarray(mel, dtype=np.float32)
         B, M, T = mel.shape
         wav = np.empty((B, self.c_out, T * self.hop), dtype=np.float32)

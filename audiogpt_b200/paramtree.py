@@ -33,9 +33,10 @@ def _descend(root: nn.Module, parts):
 
 
 def add_param(root: nn.Module, key: str, value: torch.Tensor):
+    """Hang ``value`` at ``key``; an nn.Parameter is registered as is (a parameter shared under two keys)."""
     parts = key.split(".")
     node = _descend(root, parts[:-1])
-    node.register_parameter(parts[-1], nn.Parameter(value, requires_grad=False))
+    node.register_parameter(parts[-1], value if isinstance(value, nn.Parameter) else nn.Parameter(value, requires_grad=False))
 
 
 def del_param(root: nn.Module, key: str):
@@ -44,21 +45,32 @@ def del_param(root: nn.Module, key: str):
     del node._parameters[parts[-1]]
 
 
-def get_param(root: nn.Module, key: str) -> torch.Tensor:
+def add_buffer(root: nn.Module, key: str, value: torch.Tensor):
+    parts = key.split(".")
+    _descend(root, parts[:-1]).register_buffer(parts[-1], value)
+
+
+def _leaf(root: nn.Module, key: str):
     parts = key.split(".")
     node = root
     for p in parts[:-1]:
         node = node._modules[p]
-    return node._parameters[parts[-1]]
+    return node, parts[-1]
+
+
+def get_param(root: nn.Module, key: str) -> torch.Tensor:
+    node, name = _leaf(root, key)
+    return node._parameters[name]
+
+
+def get_tensor(root: nn.Module, key: str) -> torch.Tensor:
+    """The parameter or, failing that, the buffer at ``key``."""
+    node, name = _leaf(root, key)
+    t = node._parameters.get(name)
+    return t if t is not None else node._buffers[name]
 
 
 def build(root: nn.Module, shapes: Dict[str, Sequence[int]], init=None):
     for key, shape in shapes.items():
         t = torch.zeros(tuple(shape), dtype=torch.float32) if init is None else init(key, tuple(shape))
         add_param(root, key, t)
-
-
-def params_signature(module: nn.Module, keys: Sequence[str] = None):
-    """Cheap change detector: (data_ptr, version) of every parameter, or of the parameters named in ``keys``."""
-    ps = module.parameters() if keys is None else (get_param(module, k) for k in keys)
-    return tuple((p.data_ptr(), p._version, p.device.type) for p in ps)

@@ -23,8 +23,8 @@ import numpy as np
 import torch
 from torch import nn
 
-from ... import _lib, paramtree, specs
-from ...modules.hifigan.hifigan import HifiGanGenerator, fold_weight_norm, _wn_key
+from ... import specs
+from ...modules.hifigan.hifigan import HifiGanGenerator
 
 LRELU_SLOPE = 0.1
 
@@ -47,7 +47,6 @@ def _as_dict(h):
 class BigVGAN(HifiGanGenerator):
     def __init__(self, h):
         nn.Module.__init__(self)
-        _lib.HandleOwner.__init__(self)
         self.h = h
         hd = _as_dict(h)
         hd.setdefault("num_mels", 80)
@@ -58,66 +57,23 @@ class BigVGAN(HifiGanGenerator):
         hd["resblock_dilation_sizes"] = [[int(d) for d in dl] for dl in hd["resblock_dilation_sizes"]]
         if str(hd["activation"]) not in ("snake", "snakebeta"):
             raise NotImplementedError("activation incorrectly specified. check the config file and look for 'activation'.")
-        self._hd = hd
-        self.c_out = 1
-        self.num_kernels = len(hd["resblock_kernel_sizes"])
-        self.num_upsamples = len(hd["upsample_rates"])
-        self.hop = int(np.prod(hd["upsample_rates"]))
-        self._use_nsf = False
-        self._shapes = specs.bigvgan_param_shapes(hd)
-        self._weight_norm = True
-        g = torch.Generator().manual_seed(0)
-        filt = specs.kaiser_sinc_filter12()
-        for key, shape in self._shapes.items():
-            if key.endswith(".filter"):
-                paramtree.add_param(self, key, filt.clone())
-            elif _wn_key(key):
-                v = torch.randn(shape, generator=g) * 0.01
-                n = v.reshape(shape[0], -1).norm(dim=1).reshape(-1, *([1] * (len(shape) - 1)))
-                paramtree.add_param(self, key + "_g", n.clone())
-                paramtree.add_param(self, key + "_v", v)
-            elif key.endswith((".act.alpha", ".act.beta")):
-                init = torch.zeros(shape) if hd["snake_logscale"] else torch.ones(shape)
-                paramtree.add_param(self, key, init)
-            else:
-                paramtree.add_param(self, key, torch.zeros(shape))
-        self._engine_sig = None
+        shapes = specs.bigvgan_param_shapes(hd)
+        hd.update(activation=2 if str(hd["activation"]) == "snakebeta" else 1, snake_logscale=int(bool(hd["snake_logscale"])))
+        self._init_generator(hd, 1, shapes, False)
+
+    def _initial_value(self, key, shape):
+        if key.endswith(".filter"):
+            return specs.kaiser_sinc_filter12()
+        if key.endswith((".act.alpha", ".act.beta")):
+            return torch.zeros(shape) if self._hd["snake_logscale"] else torch.ones(shape)
+        return torch.zeros(shape)
 
     def folded_weights(self):
         """C-ABI order (include/agpt_b200.h, agpt_hifigan_cfg): state-dict order without the filter buffers,
         then the 12 filter taps once."""
-        out, filt = [], None
-        for key in self._shapes:
-            if key.endswith(".filter"):
-                filt = paramtree.get_param(self, key).data.reshape(-1)
-                continue
-            if self._weight_norm and _wn_key(key):
-                out.append(fold_weight_norm(paramtree.get_param(self, key + "_g").data,
-                                            paramtree.get_param(self, key + "_v").data))
-            else:
-                out.append(paramtree.get_param(self, key).data)
-        out.append(filt)
-        return out
-
-    def _cfg(self):
-        hd = self._hd
-        c = _lib.HifiganCfg()
-        c.n_mels, c.c_out = int(hd["num_mels"]), 1
-        c.upsample_initial_channel = int(hd["upsample_initial_channel"])
-        c.num_upsamples = self.num_upsamples
-        for i, (u, k) in enumerate(zip(hd["upsample_rates"], hd["upsample_kernel_sizes"])):
-            c.upsample_rates[i], c.upsample_kernel_sizes[i] = int(u), int(k)
-        c.resblock_type = 1 if str(hd["resblock"]) == "1" else 2
-        c.num_kernels = self.num_kernels
-        for j, (ks, dil) in enumerate(zip(hd["resblock_kernel_sizes"], hd["resblock_dilation_sizes"])):
-            c.resblock_kernel_sizes[j] = int(ks)
-            c.resblock_num_dilations[j] = len(dil)
-            for n, d in enumerate(dil):
-                c.resblock_dilations[j][n] = int(d)
-        c.use_nsf = 0
-        c.activation = 2 if str(hd["activation"]) == "snakebeta" else 1
-        c.snake_logscale = 1 if hd["snake_logscale"] else 0
-        return c
+        ws = dict(zip(self._shapes, super().folded_weights()))
+        filt = [ws.pop(k) for k in list(ws) if k.endswith(".filter")][-1]
+        return list(ws.values()) + [filt.reshape(-1)]
 
     @torch.no_grad()
     def forward(self, x):

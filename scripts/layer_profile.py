@@ -5,7 +5,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from audiogpt_b200 import _lib, specs
 L = _lib.lib()
-L.agpt_profile_dump.restype = C.c_long
 which = sys.argv[1] if len(sys.argv) > 1 else "hifigan"
 B = int(sys.argv[2]) if len(sys.argv) > 2 else 8
 if which == "hifigan":

@@ -42,7 +42,6 @@ def attention_share(m, x):
     """per-launch tap-GEMM records of one encode: the AttnBlock GEMMs are the 1-tap launches that produce q|k|v
     (Cout = 3 Cin), the scores (Cout = tokens), P V (Cin = tokens) and proj_out (residual epilogue, Cin = Cout)"""
     L = _lib.lib()
-    L.agpt_profile_dump.restype = C.c_long
     torch.cuda.synchronize()
     _lib.check(L.agpt_profile_enable(1))
     try:

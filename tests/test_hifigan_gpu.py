@@ -68,13 +68,12 @@ def test_resblock2():
 
 def test_nsf_noise_convs():
     """har_source captured from the reference run -> noise_convs path (hifigan.py:155-157)."""
-    import ctypes as C
     from audiogpt_b200 import _lib
     g = load_golden("hifigan_small_nsf")
     h = dict(specs.HIFIGAN_SMALL, use_pitch_embed=True, audio_sample_rate=24000)
     m = build(h, 5678)
     mel, har = T(g["mel"]).cuda(), T(g["har_source"]).cuda().contiguous()
-    m._ensure_engine(mel.device)
+    m._build_engine(mel.device)
     wav = torch.empty((2, 1, 20 * 256), device="cuda")
     _lib.check(_lib.lib().agpt_hifigan_forward(m._h, _lib.fptr(mel), _lib.fptr(har), 2, 20, _lib.fptr(wav),
                                                _lib.cur_stream()))

@@ -16,18 +16,82 @@ from audiogpt_b200 import parallel, specs
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
+def _header_api():
+    """(prototypes, structs, defines) parsed from include/agpt_b200.h: {name: (return type, [parameter types])} with
+    comments, parameter names and `const` stripped and arrays written as pointers, {agpt_*_cfg: [(field, [array
+    lengths])]}, {macro: int}."""
+    hdr = re.sub(r"/\*.*?\*/", " ", open(os.path.join(ROOT, "include", "agpt_b200.h")).read(), flags=re.S)
+    defines = {k: int(v) for k, v in re.findall(r"#define\s+(\w+)\s+(\d+)", hdr)}
+
+    def ctype(decl, named=True):
+        t = re.sub(r"\[[^]]*\]", "", decl).replace("const", " ")
+        if named:
+            t = re.sub(r"\w+\s*$", "", t)
+        t = re.sub(r"\s*\*\s*", "*", " ".join(t.split())).strip()
+        return t + "*" * ("[" in decl)
+
+    protos = {}
+    for ret, name, params in re.findall(r"^([A-Za-z_][\w\s\*]*?)\s*\b(agpt_\w+)\s*\(([^)]*)\)\s*;", hdr, re.M | re.S):
+        params = [] if params.strip() == "void" else [ctype(p) for p in params.split(",")]
+        protos[name] = (ctype(ret, named=False), params)
+    structs = {}
+    for body, name in re.findall(r"typedef struct \{(.*?)\}\s*(agpt_\w+_cfg)\s*;", hdr, re.S):
+        fields = []
+        for decl in filter(str.strip, body.split(";")):
+            assert decl.strip().startswith("int "), decl
+            for f in decl.strip()[len("int"):].split(","):
+                dims = [defines[d] for d in re.findall(r"\[(\w+)\]", f)]
+                fields.append((f.split("[")[0].strip(), dims))
+        structs[name] = fields
+    return protos, structs, defines
+
+
 def test_library_exports_every_declared_symbol():
+    """Every declared entry point is exported, and _lib declares its prototype and mirrors its cfg structs exactly."""
+    from audiogpt_b200 import _lib
     from audiogpt_b200.build import build
     lib_path = build()
-    hdr = open(os.path.join(ROOT, "include", "agpt_b200.h")).read()
-    names = sorted(set(re.findall(r"\b(agpt_[a-z0-9_]+)\s*\(", hdr)))
-    assert len(names) >= 18
+    protos, structs, defines = _header_api()
+    assert len(protos) >= 40 and len(structs) == 6
     L = ctypes.CDLL(lib_path)
-    for n in names:
+    for n in protos:
         assert hasattr(L, n), f"{n} declared in include/agpt_b200.h but not exported"
-    L.agpt_last_error.restype = ctypes.c_char_p
-    assert L.agpt_version() >= 100
-    assert isinstance(L.agpt_last_error(), bytes)
+    # the ctypes mirror of every agpt_*_cfg: field names, order, int type and array lengths
+    cfg_cls = {f"agpt_{c[:-3].lower()}_cfg": getattr(_lib, c) for c in dir(_lib) if c.endswith("Cfg")}
+    assert set(cfg_cls) == set(structs)
+    for name, fields in structs.items():
+        got = []
+        for fname, ft in cfg_cls[name]._fields_:
+            dims = []
+            while hasattr(ft, "_length_"):
+                dims.append(ft._length_)
+                ft = ft._type_
+            assert ft is ctypes.c_int, (name, fname)
+            got.append((fname, dims))
+        assert got == fields, name
+    assert {k: getattr(_lib, k) for k in defines if k.startswith("AGPT_MAX_")} == \
+        {k: v for k, v in defines.items() if k.startswith("AGPT_MAX_")}
+    # the declared prototypes: C type -> ctypes type
+    scalar = {"int": ctypes.c_int, "long": ctypes.c_long, "long long": ctypes.c_longlong, "float": ctypes.c_float,
+              "double": ctypes.c_double, "agpt_handle": ctypes.c_void_p, "agpt_handle*": ctypes.POINTER(ctypes.c_void_p),
+              "float**": ctypes.POINTER(ctypes.POINTER(ctypes.c_float))}
+    scalar.update({f"{s}*": ctypes.POINTER(cfg_cls[s]) for s in structs})
+
+    def expect(t):
+        if t in scalar:
+            return scalar[t]
+        assert t.endswith("*") and not t.endswith("**"), f"no ctypes rule for the C type {t!r}"
+        return ctypes.c_void_p
+
+    assert set(_lib.PROTOTYPES) == set(protos)
+    Lp = _lib.lib()
+    for n, (ret, params) in protos.items():
+        want_ret = None if ret == "void" else ctypes.c_char_p if ret == "char*" else expect(ret)
+        want = (want_ret, [expect(p) for p in params])
+        assert _lib.PROTOTYPES[n] == want, n
+        assert (getattr(Lp, n).restype, getattr(Lp, n).argtypes) == want, n
+    assert Lp.agpt_version() >= 100
+    assert isinstance(Lp.agpt_last_error(), bytes)
 
 
 def test_invalid_handle_is_an_error_not_a_crash():

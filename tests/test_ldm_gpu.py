@@ -187,7 +187,6 @@ def test_eta_noise_path_vs_oracle():
     x = specs.synth_tensor((2, 4, 6, 10), seed=1)
     e2 = specs.synth_tensor((4, 4, 6, 10), seed=2)
     nz = specs.synth_tensor((2, 4, 6, 10), seed=3)
-    import ctypes as C
     from audiogpt_b200 import _lib
     a_t, a_prev, sg = 0.37, 0.52, 0.11
     sq = float(np.sqrt(np.float32(1 - np.float32(a_t))))
@@ -195,9 +194,8 @@ def test_eta_noise_path_vs_oracle():
     ref, ref0 = lr.ddim_step(x, eu + 1.5 * (ec - eu), a_t, a_prev, sg, sq, nz, 0.9)
     xc, ec2, nc = x.cuda(), e2.cuda(), nz.cuda()
     xp, p0 = torch.empty_like(xc), torch.empty_like(xc)
-    _lib.check(_lib.lib().agpt_ddim_update(_lib.fptr(xc), _lib.fptr(ec2), 0, C.c_float(1.5), C.c_float(a_t),
-                                            C.c_float(a_prev), C.c_float(sg), C.c_float(sq), _lib.fptr(nc),
-                                            C.c_float(0.9), 2, C.c_long(x[0].numel()), _lib.fptr(xp), _lib.fptr(p0),
+    _lib.check(_lib.lib().agpt_ddim_update(_lib.fptr(xc), _lib.fptr(ec2), 0, 1.5, a_t, a_prev, sg, sq, _lib.fptr(nc),
+                                            0.9, 2, x[0].numel(), _lib.fptr(xp), _lib.fptr(p0),
                                             _lib.cur_stream()))
     assert rel_rmse(xp.cpu(), ref) < 1e-6 and rel_rmse(p0.cpu(), ref0) < 1e-6
 

@@ -91,7 +91,7 @@ def test_tensor_core_tapconv_matches_fma():
     for G, Ln, Cin, Cout, K, dil, Wr in SHAPES:
         for epi_res in (0, 1):
             rel = (C.c_double * 2)()
-            _lib.check(L.agpt_check_tapconv(G, Ln, Cin, Cout, K, dil, Wr, epi_res, C.c_double(1.0), C.c_double(1.0), rel))
+            _lib.check(L.agpt_check_tapconv(G, Ln, Cin, Cout, K, dil, Wr, epi_res, 1.0, 1.0, rel))
             assert rel[0] < 2e-4 and rel[1] < 2e-5, (G, Ln, Cin, Cout, K, dil, Wr, epi_res, rel[0], rel[1])
 
 
@@ -112,7 +112,7 @@ def test_tcgen05_adversarial_ranges(x_scale, w_spread, tol_max, tol_rms):
     worst = (0.0, 0.0)
     for G, Ln, Cin, Cout, K, dil, Wr in [(2, 9000, 32, 32, 7, 1, 0), (2, 3000, 256, 256, 11, 5, 0), (2, 780, 320, 320, 3, 1, 78)]:
         rel = (C.c_double * 2)()
-        _lib.check(L.agpt_check_tapconv(G, Ln, Cin, Cout, K, dil, Wr, 1, C.c_double(x_scale), C.c_double(w_spread), rel))
+        _lib.check(L.agpt_check_tapconv(G, Ln, Cin, Cout, K, dil, Wr, 1, x_scale, w_spread, rel))
         worst = (max(worst[0], rel[0]), max(worst[1], rel[1]))
         assert rel[0] < tol_max and rel[1] < tol_rms, (x_scale, w_spread, G, Ln, Cin, Cout, K, rel[0], rel[1])
     print(f"x_scale {x_scale:g} w_spread {w_spread:g}: max/rms {worst[0]:.2e}  rms/rms {worst[1]:.2e}")

@@ -116,11 +116,11 @@ def test_engines_are_built_from_their_own_parameters():
     m, _ = build(cfg)
     y = m.decode(specs.synth_tensor((1, 4, 10, 78), seed=3).cuda())
     assert y.shape == (1, 1, 80, 624)
-    assert m._h.value and not m._enc._h.value
+    assert m._h.value and not m._enc_engine.h.value
     dec_h = m._h.value
     x = mel(1).cuda()
     a = m.encode(x).parameters
-    enc_h = m._enc._h.value
+    enc_h = m._enc_engine.h.value
     assert enc_h and m._h.value == dec_h
     with torch.no_grad():
         m.quant_conv.bias.add_(1.0)
