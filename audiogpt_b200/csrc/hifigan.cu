@@ -336,6 +336,7 @@ struct Hifigan : Handle {
   DevBuf io_mel, io_wav, io_har;  // staging for the host-buffer entry point
   float* pin_mel = nullptr; float* pin_wav = nullptr; size_t pin_mel_n = 0, pin_wav_n = 0;
   cudaStream_t own_stream = nullptr;
+  bool fuse_resblock = true;        // AGPT_FUSE_RESBLOCK=0: every ResBlock1 conv as its own launch
 
   ~Hifigan() override {
     if (pin_mel) cudaFreeHost(pin_mel);
@@ -395,6 +396,15 @@ struct Hifigan : Handle {
         AGPT_CUDA(cudaGetLastError());
       }
       const long gs = L * C;
+      auto gview = [&](int g) { return (g && L % g == 0) ? g : 1; };   // time-grouped view [L/g][g*C] of the same memory
+      // one conv of a ResBlock over the view gq (1: plain rows [L][C]); the caller sets the epilogue
+      auto conv = [&](const PackedConv& plain, const PackedConv& grouped, int gq, int dil, const float* in, float* out) {
+        TapConvParams P = gq > 1 ? tapconv_params(grouped, B, (int)(L / gq), 0, 1) : tapconv_params(plain, B, (int)L, 0, dil);
+        P.in = in; P.in_gstride = gs; P.in_pitch = gq * C;
+        P.out = out; P.out_gstride = gs; P.out_pitch = gq * C;
+        P.pro = big ? PRO_NONE : PRO_LRELU; P.slope = 0.1f;
+        return P;
+      };
       for (int j = 0; j < cfg.num_kernels; ++j) {
         const ResBlockW& rb = rbs[i * cfg.num_kernels + j];
         const float* x = X;
@@ -402,32 +412,37 @@ struct Hifigan : Handle {
         for (int n = 0; n < nd; ++n) {
           const bool last = (n == nd - 1);
           float* dst = last ? acc : ((n & 1) ? R1 : R0);
+          auto residual_epi = [&](TapConvParams& P) {   // x + conv(...), on the last pair into the MRF accumulator
+            P.res = x; P.res_gstride = gs; P.res_pitch = P.in_pitch;
+            if (last) { P.epi = EPI_ACC; P.scale = inv_nk; P.accumulate = (j > 0); }
+            else P.epi = EPI_RES;
+          };
+          const bool t1 = cfg.resblock_type == 1;
+          if (t1 && !big && fuse_resblock) {
+            // both convs in one launch (tcpair_launch; not taken for C > 128 or without tensor cores).  c2 takes c1's
+            // view, so a grouped c2 after a dilated c1 runs ungrouped: on H100 that pair is still faster fused.
+            const int gq = gview(rb.g1[n]) == gview(rb.g2[n]) ? gview(rb.g1[n]) : 1;
+            TapConvParams P1 = conv(rb.c1[n], rb.c1g[n], gq, rb.dil[n], x, A);
+            P1.epi = EPI_BIAS;
+            TapConvParams P2 = conv(rb.c2[n], rb.c2g[n], gq, 1, A, dst);
+            residual_epi(P2);
+            if (tcpair_launch(P1, P2, st)) { x = dst; continue; }
+          }
           const float* conv_in = x;
-          if (cfg.resblock_type == 1) {
+          if (t1) {
             if (big) snake(x, S, L, C, rb.act[2 * n]);      // xt = a1(x)   (AMPBlock1.forward, models.py:75-76)
-            const int gq = (rb.g1[n] && L % rb.g1[n] == 0) ? rb.g1[n] : 1;      // time-grouped view [L/g][g*C] of the same memory
-            TapConvParams P = gq > 1 ? tapconv_params(rb.c1g[n], B, (int)(L / gq), 0, 1) : tapconv_params(rb.c1[n], B, (int)L, 0, rb.dil[n]);
-            P.in = big ? S : x; P.in_gstride = gs; P.in_pitch = gq * C;
-            P.out = A; P.out_gstride = gs; P.out_pitch = gq * C;
-            P.pro = big ? PRO_NONE : PRO_LRELU; P.slope = 0.1f; P.epi = EPI_BIAS;
+            TapConvParams P = conv(rb.c1[n], rb.c1g[n], gview(rb.g1[n]), rb.dil[n], big ? S : x, A);
+            P.epi = EPI_BIAS;
             tapconv_launch(P, st);
             conv_in = A;
           }
           if (big) {                                        // a2(xt) resp. AMPBlock2's a(x)
-            snake(conv_in, S, L, C, rb.act[cfg.resblock_type == 1 ? 2 * n + 1 : n]);
+            snake(conv_in, S, L, C, rb.act[t1 ? 2 * n + 1 : n]);
             conv_in = S;
           }
-          const bool t1 = cfg.resblock_type == 1;
-          const int gq0 = t1 ? rb.g2[n] : rb.g1[n];
-          const int gq = (gq0 && L % gq0 == 0) ? gq0 : 1;
-          const PackedConv& pc = gq > 1 ? (t1 ? rb.c2g[n] : rb.c1g[n]) : (t1 ? rb.c2[n] : rb.c1[n]);
-          TapConvParams P = gq > 1 ? tapconv_params(pc, B, (int)(L / gq), 0, 1) : tapconv_params(pc, B, (int)L, 0, t1 ? 1 : rb.dil[n]);
-          P.in = conv_in; P.in_gstride = gs; P.in_pitch = gq * C;
-          P.out = dst; P.out_gstride = gs; P.out_pitch = gq * C;
-          P.pro = big ? PRO_NONE : PRO_LRELU; P.slope = 0.1f;
-          P.res = x; P.res_gstride = gs; P.res_pitch = gq * C;
-          if (last) { P.epi = EPI_ACC; P.scale = inv_nk; P.accumulate = (j > 0); }
-          else P.epi = EPI_RES;
+          TapConvParams P = t1 ? conv(rb.c2[n], rb.c2g[n], gview(rb.g2[n]), 1, conv_in, dst)
+                               : conv(rb.c1[n], rb.c1g[n], gview(rb.g1[n]), rb.dil[n], conv_in, dst);
+          residual_epi(P);
           tapconv_launch(P, st);
           x = dst;
         }
@@ -463,6 +478,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
                "resblock kernel size must be odd and <= 11");
   std::unique_ptr<Hifigan> h(new Hifigan());
   h->magic = kMagicHifigan; h->device = device; h->cfg = *cfg;
+  { const char* e = getenv("AGPT_FUSE_RESBLOCK"); h->fuse_resblock = !(e && e[0] == '0'); }
   WeightCursor wc{W, nW};
   { const float* w = wc.next(); const float* b = wc.next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
   h->ups.resize(nu);

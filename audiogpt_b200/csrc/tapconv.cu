@@ -8,6 +8,7 @@ namespace agpt {
 // ---- optional per-launch CUDA-event profiling (bench.py's roofline leg) ----
 struct ProfRec { cudaEvent_t e0, e1; int variant; double flops, bytes; int G, L, Cin, Cout, ntaps, span, epi, Wreal; };
 static bool g_prof = false;
+constexpr int PROF_PAIR = 16;   // record epi code of a fused ResBlock pair: 16 + the epilogue of its second conv
 static std::vector<ProfRec> g_recs;
 
 bool profile_enabled() { return g_prof; }
@@ -31,7 +32,8 @@ void profile_collect(double* ms, double* flops, double* bytes, long long* launch
   }
 }
 
-// One text line per recorded launch: "variant G L Cin Cout ntaps span epi Wreal ms flops" (dev tooling).
+// One text line per recorded launch: "variant G L Cin Cout ntaps span epi Wreal ms flops" (dev tooling).  A fused
+// ResBlock pair is one line with epi = PROF_PAIR + c2's epi and the taps / spans of both convs summed.
 long profile_dump(char* out, long cap) {
   AGPT_CUDA(cudaDeviceSynchronize());
   long n = 0;
@@ -252,6 +254,22 @@ void* profile_begin(const TapConvParams& P, bool tc, double bytes_override, cuda
   AGPT_CUDA(cudaEventCreate(&rec->e0));
   AGPT_CUDA(cudaEventCreate(&rec->e1));
   AGPT_CUDA(cudaEventRecord(rec->e0, st));
+  return rec;
+}
+// A fused pair (tcpair_launch): the algorithmic FLOPs of both convs (not the recomputed halo rows); bytes of x in,
+// the residual, the output (+ the old accumulator) and both weight sets -- the intermediate never reaches HBM.
+void* profile_begin_pair(const TapConvParams& c1, const TapConvParams& c2, cudaStream_t st) {
+  if (!g_prof) return nullptr;
+  const double rows = (double)c1.G * c1.L;
+  const double bytes = 4.0 * (rows * c1.Cin + 2.0 * rows * c2.Cout + (c2.epi == EPI_ACC && c2.accumulate ? rows * c2.Cout : 0.0) +
+                              (double)c1.ntaps * c1.Cin * c1.Cout + (double)c2.ntaps * c2.Cin * c2.Cout);
+  ProfRec* rec = static_cast<ProfRec*>(profile_begin(c2, true, bytes, st));
+  rec->flops += 2.0 * rows * c1.Cin * c1.Cout * c1.ntaps * (c1.flops_scale > 0.f ? c1.flops_scale : 1.f);
+  int lo = c1.tap_off[0], hi = c1.tap_off[0];
+  for (int t = 1; t < c1.ntaps; ++t) { lo = std::min(lo, c1.tap_off[t]); hi = std::max(hi, c1.tap_off[t]); }
+  rec->ntaps += c1.ntaps;
+  rec->span += hi - lo;
+  rec->epi += PROF_PAIR;
   return rec;
 }
 void profile_end(void* r, cudaStream_t st) {

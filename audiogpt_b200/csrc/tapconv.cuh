@@ -123,6 +123,7 @@ struct PackedConv;
 void tapconv_launch(TapConvParams P, cudaStream_t st);
 void tcconv_launch(TapConvParams P, cudaStream_t st);          // tensor-core dispatcher (tcconv.cu)
 bool tcconv5_launch(TapConvParams P, cudaStream_t st);
+bool tcpair_launch(TapConvParams c1, TapConvParams c2, cudaStream_t st);   // fused ResBlock1 pair (tcconv5.cu)
 struct HTile { int bn; const float* w; long ntiles; };
 HTile pick_h_tile(const TapConvParams& P, int sms);   // tile width of the fp16 tensor-core kernel (tcconv5.cu)
 void pack_h_weights(struct PackedConv& pc, const std::vector<float>& h);
@@ -132,6 +133,7 @@ void tc_set_enabled(int on);
 bool tc_enabled();
 void profile_enable(int on);
 void* profile_begin(const TapConvParams& P, bool tc, double bytes_override, cudaStream_t st);
+void* profile_begin_pair(const TapConvParams& c1, const TapConvParams& c2, cudaStream_t st);
 void profile_end(void* rec, cudaStream_t st);
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches);
 long profile_dump(char* out, long cap);

@@ -295,6 +295,268 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
   }
 }
 
+// One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))), in one CTA per tile (tcpair_launch): the tcconv5 pipeline
+// runs c1 over the 128 intermediate rows qa .. qa + 127 (qa = q0 + lowest tap of c2), c1's accumulator becomes c2's
+// operand tile in shared memory, and the tcconv5 pipeline runs c2 over it; a tile keeps the 128 - span(c2) outputs
+// that read only those rows.  P1 / P2: the two convs' launch parameters (leaky-ReLU prologue, 1-D rows, one co-tile,
+// BN >= C); P2's epilogue (EPI_RES / EPI_ACC) writes the output.  The weight producer streams c1's stages, then c2's,
+// through one mbarrier ring.
+template <int BN>
+__global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_constant__ TapConvParams P1,
+                                                               const __grid_constant__ TapConvParams P2) {
+  constexpr int NB = tc5_nb(BN), NJ = BN / NB;
+  extern __shared__ uint8_t smem_raw_[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
+  const int RRA = P1.R, NA = P1.tc_na, NW = P1.tc_nw, NR = P1.tc_nr;
+  __shared__ Tc5Smem S;
+  if (threadIdx.x == 0) tc5_layout(S, BN, RRA, NA, NW, NR);
+  __syncthreads();
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
+  uint64_t* w_empty = w_full + MAX_NW;
+  int* rowinfo = reinterpret_cast<int*>(smem + S.rowinfo);
+  int* rowp = reinterpret_cast<int*>(smem + S.rowp);
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup-uniform role branches (see tcconv5_kernel)
+  const bool is_worker = wg < 2;
+  const int xt = tid;
+  int span2 = 0;
+  for (int t = 0; t < P2.ntaps; ++t) span2 = max(span2, P2.tap_off[t] - P2.lo_al);
+  const int g = blockIdx.z, Lv = P1.L, q0 = blockIdx.x * (TC_ROWS - span2), qa = q0 + P2.lo_al;
+  const int nchunks = P1.tc_chunks_h, total = nchunks * P1.ntaps;
+  const int lo = P1.lo_al;
+
+  if (tid == 0) {
+    for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NWK / 32); }
+    fence_barrier_init();
+  }
+  if (is_worker) {
+    for (int i = xt; i < RRA; i += NWK) {
+      const int r = qa + lo + i;
+      rowinfo[i] = (r >= 0 && r < Lv) ? r * P1.in_pitch : -1;
+    }
+    if (xt < TC_ROWS) rowp[xt] = (xt < TC_ROWS - span2 && q0 + xt < Lv) ? q0 + xt : -1;
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (is_worker) {
+    const float* __restrict__ ing = P1.in + g * P1.in_gstride;
+    auto issue_raw = [&](int c, int rb) {   // as tcconv5_kernel
+      uint8_t* dst = smem + S.raw[rb];
+      const int kv = min(H_KCH, P1.Cin - c * H_KCH);
+      const int nu = ((kv + 15) >> 4) << 2;
+      for (int idx = xt; idx < RRA * 16; idx += NWK) {
+        const int row = idx >> 4, u = idx & 15;
+        if (u >= nu) continue;
+        const int ch = c * H_KCH + 4 * u;
+        const int a = rowinfo[row];
+        const bool ok = (a >= 0) && (ch < P1.Cin);
+        cp_async16_zfill(dst + row * 256 + (((u >> 1) + ((u & 1) << 3)) << 4), ok ? (ing + a + ch) : P1.in, ok ? 16u : 0u);
+      }
+      cp_async_commit_();
+    };
+    issue_raw(0, 0);
+    if (NR == 2 && nchunks > 1) issue_raw(1, 1);
+    {  // the epilogue's residual / old accumulator rows into L2 while the main loop runs
+      const int lines = (BN * 4) / 128 > 0 ? (BN * 4) / 128 : 1;
+      for (int idx = xt; idx < TC_ROWS * lines; idx += NWK) {
+        const int p = rowp[idx / lines];
+        const int co = (idx % lines) * 32;
+        if (p >= 0 && co < P2.Cout) {
+          asm volatile("prefetch.global.L2 [%0];" ::"l"(P2.res + g * P2.res_gstride + (long)p * P2.res_pitch + co));
+          if (P2.epi == EPI_ACC && P2.accumulate)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(P2.out + g * P2.out_gstride + (long)p * P2.out_pitch + co));
+        }
+      }
+    }
+    float acc[NJ][NB / 2];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+      for (int i = 0; i < NB / 2; ++i) acc[j][i] = 0.f;
+    int it = 0, prev = -1;     // prev: weight stage of the newest wgmma group, released once that group has completed
+    // wgmma over the taps of one conv and one 64-channel chunk of its operand tile (ahi0 / alo0: this warpgroup's rows)
+    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {
+      for (int t = 0; t < Q.ntaps; ++t, ++it) {
+        const int s = it % NW;
+        mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
+        const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
+        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
+        const uint32_t ws = smem_u32(smem + S.w[s]);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        wgmma_fence();
+        for (int k = 0; k < ksteps; ++k) {
+          const uint64_t ko = (uint64_t)((k * 32) >> 4);
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) {
+            const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
+            wgmma_nb<NB>(acc[j], dah + ko, dwh);
+            wgmma_nb<NB>(acc[j], dal + ko, dwh);
+            wgmma_nb<NB>(acc[j], dah + ko, dwl);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        prev = s;
+      }
+    };
+    // =========================== c1: transform + wgmma, chunk by chunk (as tcconv5_kernel) ===========================
+    for (int c = 0; c < nchunks; ++c) {
+      const int buf = c % NA;
+      const int rb = (NR == 2) ? (c & 1) : 0;
+      const int kv = min(H_KCH, P1.Cin - c * H_KCH);
+      const int nq = ((kv + 15) >> 4) << 1;
+      if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
+      else cp_async_wait_all_();
+      named_bar_sync(1, NWK);
+      uint8_t* ahi = smem + S.a_hi[buf];
+      uint8_t* alo = smem + S.a_lo[buf];
+      const uint8_t* rawb = smem + S.raw[rb];
+#pragma unroll 2
+      for (int idx = xt; idx < RRA * 8; idx += NWK) {
+        const int row = idx >> 3, q = idx & 7;
+        if (q >= nq) continue;
+        const float4 x0 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 256 + q * 16), true, nullptr);
+        const float4 x1 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 256 + 128 + q * 16), true, nullptr);
+        uint4 h, l;
+        h.x = split2(x0.x, x0.y, l.x);
+        h.y = split2(x0.z, x0.w, l.y);
+        h.z = split2(x1.x, x1.y, l.z);
+        h.w = split2(x1.z, x1.w, l.w);
+        const uint32_t o = sw128(row, q);
+        *reinterpret_cast<uint4*>(ahi + o) = h;
+        *reinterpret_cast<uint4*>(alo + o) = l;
+      }
+      fence_proxy_async();
+      named_bar_sync(1, NWK);
+      if (c + NR < nchunks) issue_raw(c + NR, rb);
+      mma_taps(P1, smem_u32(ahi) + (uint32_t)(wg * 64 - lo) * 128u, smem_u32(alo) + (uint32_t)(wg * 64 - lo) * 128u,
+               (kv + 15) >> 4);
+      if (NA == 1) {
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&w_empty[prev]);
+        prev = -1;
+      }
+    }
+    // =========================== c1's epilogue -> c2's operand tile ===========================
+    // The arithmetic of c1's EPI_BIAS store followed by c2's PRO_LRELU transform (acc * descale + bias, leaky ReLU,
+    // hi/lo split), so c2 multiplies the operands a separate launch would.  The tile [RR2 rows][C channels] (K-major
+    // SWIZZLE_128B, per 64-channel chunk a hi and a lo block) replaces c1's operand buffers: rows outside the sample are
+    // c2's zero padding, channels >= C are zero, rows >= 128 feed only the discarded outputs and are zero.
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+    if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+    prev = -1;
+    named_bar_sync(1, NWK);                    // both warpgroups' c1 wgmmas are done reading the operand buffers
+    const int RR2 = P2.R, nch2 = P2.tc_chunks_h, C2 = P2.Cin;
+    uint8_t* a2 = smem + S.a_hi[0];
+    const uint32_t lo_part = (uint32_t)nch2 * RR2 * 128;   // the hi blocks, then the lo blocks
+    const float dsc1 = P1.tc_descale;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+      for (int i = 0; i < NB / 8; ++i) {
+        const int col = j * NB + 8 * i + c0;   // accumulator fragment layout: see wgmma_n16
+        const bool cok = col < C2;
+        float2 b = make_float2(0.f, 0.f);
+        if (cok && P1.bias) b = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
+        uint8_t* hi = a2 + (uint32_t)(col >> 6) * RR2 * 128;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + 8 * h;
+          float v0 = 0.f, v1 = 0.f;
+          if (cok && qa + r >= 0 && qa + r < Lv) {
+            v0 = lrelu(__fadd_rn(__fmul_rn(acc[j][4 * i + 2 * h], dsc1), b.x), P2.slope);
+            v1 = lrelu(__fadd_rn(__fmul_rn(acc[j][4 * i + 2 * h + 1], dsc1), b.y), P2.slope);
+          }
+          uint32_t l;
+          const uint32_t hw = split2(v0, v1, l);
+          const uint32_t o = sw128(r, (col & 63) >> 3) + (col & 7) * 2;
+          *reinterpret_cast<uint32_t*>(hi + o) = hw;
+          *reinterpret_cast<uint32_t*>(hi + lo_part + o) = l;
+        }
+      }
+    const int zitems = (RR2 - TC_ROWS) * 8;    // 16-byte units of rows 128 .. RR2 - 1 per block
+    for (int idx = xt; idx < zitems * 2 * nch2; idx += NWK) {
+      const int blk = idx / zitems, u = idx - blk * zitems;
+      *reinterpret_cast<uint4*>(a2 + (uint32_t)blk * RR2 * 128 + TC_ROWS * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+    }
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+      for (int i = 0; i < NB / 2; ++i) acc[j][i] = 0.f;
+    fence_proxy_async();
+    named_bar_sync(1, NWK);
+    // =========================== c2: wgmma over the resident tile ===========================
+    for (int c = 0; c < nch2; ++c) {
+      const uint32_t ahi0 = smem_u32(a2) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * 64 - P2.lo_al) * 128u;
+      mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, C2 - c * H_KCH) + 15) >> 4);
+    }
+    // =========================== c2's epilogue (as tcconv5_kernel) ===========================
+    EpiPre pre[8];
+    int pp[8];
+    constexpr int nitem = (TC_ROWS * 8) / NWK;
+    const float dsc = P2.tc_descale;
+    auto load_block = [&](int cb) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int idx = xt + i * NWK;
+        pp[i] = (i < nitem) ? rowp[idx >> 3] : -1;
+        if (pp[i] >= 0) epi_load(P2, g, pp[i], cb + 4 * (idx & 7), pre[i]);
+      }
+    };
+    load_block(0);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+    named_bar_sync(1, NWK);
+    uint8_t* stg0 = smem + S.a_hi[0];
+#pragma unroll
+    for (int blk = 0; blk < BN / 32; ++blk) {
+      const int cb = blk * 32;
+      uint8_t* stg = stg0 + (blk & 1) * (TC_ROWS * 128);
+      const float* a = &acc[cb / NB][4 * ((cb % NB) / 8)];
+#pragma unroll
+      for (int i8 = 0; i8 < 4; ++i8) {
+        const int col = 8 * i8 + c0;
+        *reinterpret_cast<float2*>(stg + sw128(r0, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
+        *reinterpret_cast<float2*>(stg + sw128(r0 + 8, col >> 2) + (col & 3) * 4) =
+            make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+      }
+      named_bar_sync(1, NWK);
+      const int jc = xt & 7;
+      const float4 cv = epi_colvec(P2, g, cb + 4 * jc);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int idx = xt + i * NWK;
+        const int row = (idx >> 3) & (TC_ROWS - 1);
+        if (pp[i] >= 0)
+          epi_store_cv(P2, g, pp[i], cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
+      }
+      if (cb + 32 < BN) load_block(cb + 32);
+    }
+  } else if (lane == 0) {
+    // =========================== weight producer (warp 8): c1's stages, then c2's ===========================
+    const uint32_t bytes = 2u * BN * 128u;
+    const int total2 = P2.tc_chunks_h * P2.ntaps;
+    for (int it = 0; it < total + total2; ++it) {
+      const int s = it % NW, n = it / NW;
+      if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
+      mbar_arrive_expect_tx(&w_full[s], bytes);
+      const uint8_t* src = it < total ? reinterpret_cast<const uint8_t*>(P1.w_h) + (size_t)it * bytes
+                                      : reinterpret_cast<const uint8_t*>(P2.w_h) + (size_t)(it - total) * bytes;
+      bulk_g2s(smem + S.w[s], src, bytes, &w_full[s]);
+    }
+  }
+}
+
 // fp16 hi/lo weight image: [co-tile][chunk64][tap][hi | lo][BN rows x 128 B, SWIZZLE_128B], pre-scaled
 void build_h_image(const PackedConv& pc, const std::vector<float>& h, int BN, float wscale, DevBuf& dst) {
   const int nct = cdiv(pc.Cout, BN), nch = cdiv(pc.Cin, H_KCH), nt = pc.ntaps;
@@ -343,19 +605,24 @@ void pack_h_weights(PackedConv& pc, const std::vector<float>& h) {
   if (pc.tc_bn == 128 && pc.Cout > 128) build_h_image(pc, h, 96, wscale, pc.w_h96);
 }
 
-// Try one tile width; returns false when it does not fit the shared-memory budget.
-static bool tcconv5_try(TapConvParams P, int BN, cudaStream_t st) {
+// lo_al = the lowest tap offset, R = operand-tile rows (128 + tap span, rounded to the 8-row swizzle atom); returns the span
+static int tc5_rows(TapConvParams& P) {
   int lo = P.tap_off[0], hi = P.tap_off[0];
   for (int t = 1; t < P.ntaps; ++t) { lo = std::min(lo, P.tap_off[t]); hi = std::max(hi, P.tap_off[t]); }
   P.lo_al = lo;
-  const int RRA = round_up(TC_ROWS + (hi - lo), 8);
-  P.R = RRA;
+  P.R = round_up(TC_ROWS + (hi - lo), 8);
+  return hi - lo;
+}
+
+// Shared-memory plan of a BN-wide tile (operand, raw-staging and weight-ring buffers) for P after tc5_rows; false when
+// it does not fit.  a_min: bytes the operand buffers must span at least; iters: weight stages the kernel streams.
+static bool tc5_plan(TapConvParams& P, int BN, long a_min, int iters, size_t& smem) {
+  const int RRA = P.R;
   P.tc_bn = BN;
   const long avail = (long)kMaxDyn - 1024 /*align*/ - (RRA * 4 + TC_ROWS * 4 + 512) /*row tables + barriers*/;
   const long abytes = 2L * RRA * 128, wbytes = 2L * BN * 128;
   const long rbytes = (long)RRA * 256;
   const int nch = P.tc_chunks_h;
-  const int iters = nch * P.ntaps;
   int NA = (P.ntaps == 1) ? 3 : 2;
   NA = std::max(1, std::min(NA, nch));
   if ((long)NA * abytes < 32768) NA = (int)cdiv(32768L, abytes);   // the epilogue stages 2 x 16 KB through the operand buffers
@@ -364,26 +631,43 @@ static bool tcconv5_try(TapConvParams P, int BN, cudaStream_t st) {
   if (!fits(NA, NR, 2) && NA == 3) NA = 2;
   if (!fits(NA, NR, 2) && NR == 2) NR = 1;
   if (!fits(NA, NR, 2) && NA == 2 && abytes >= 32768) NA = 1;
-  if (!fits(NA, NR, 2)) return false;
+  if (NA * abytes < a_min) {
+    NA = (int)cdiv(a_min, abytes);
+    if (!fits(NA, NR, 2) && NR == 2) NR = 1;
+  }
+  if (NA > MAX_NA || !fits(NA, NR, 2)) return false;
   int NW = (int)std::min<long>(MAX_NW, (avail - NA * abytes - NR * rbytes) / wbytes);
   NW = std::max(2, std::min(NW, std::max(2, iters)));
   P.tc_na = NA; P.tc_nw = NW; P.tc_nr = NR;
   Tc5Smem S;
   tc5_layout(S, BN, RRA, NA, NW, NR);
-  const size_t smem = (size_t)S.total + 1024;
-  if (smem > (size_t)kMaxDyn) return false;
-  const int Lv = tc_lv(P);
-  dim3 grid(cdiv(Lv, TC_ROWS), cdiv(P.Cout, BN), tc_groups(P));
+  smem = (size_t)S.total + 1024;
+  return smem <= (size_t)kMaxDyn;
+}
+
+static void tc5_set_smem_limits() {
   int dev = 0;
   AGPT_CUDA(cudaGetDevice(&dev));
   static bool attr_done_dev[64] = {false};
-  if (!attr_done_dev[dev & 63]) {
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    attr_done_dev[dev & 63] = true;
-  }
+  if (attr_done_dev[dev & 63]) return;
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  attr_done_dev[dev & 63] = true;
+}
+
+// Try one tile width; returns false when it does not fit the shared-memory budget.
+static bool tcconv5_try(TapConvParams P, int BN, cudaStream_t st) {
+  tc5_rows(P);
+  size_t smem = 0;
+  if (!tc5_plan(P, BN, 0, P.tc_chunks_h * P.ntaps, smem)) return false;
+  const int Lv = tc_lv(P);
+  dim3 grid(cdiv(Lv, TC_ROWS), cdiv(P.Cout, BN), tc_groups(P));
+  tc5_set_smem_limits();
   if (BN == 128) launch_pdl(tcconv5_kernel<128>, grid, dim3(V5_THREADS), smem, st, P);
   else if (BN == 96) launch_pdl(tcconv5_kernel<96>, grid, dim3(V5_THREADS), smem, st, P);
   else if (BN == 64) launch_pdl(tcconv5_kernel<64>, grid, dim3(V5_THREADS), smem, st, P);
@@ -411,6 +695,34 @@ HTile pick_h_tile(const TapConvParams& P, int sms) {
   if (P.tc_bn == 128) consider(64, P.w_h64);
   if (P.tc_bn == 128 && allow96) consider(96, P.w_h96);   // e.g. 640 channels on 16 row tiles: 112 tiles in one wave
   return best;
+}
+
+// One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))) (c2's epilogue EPI_RES / EPI_ACC), as one launch of
+// tcpair_kernel: c1's output tile stays in shared memory as c2's operand tile, so the intermediate tensor never
+// reaches HBM.  A tile yields 128 - span(c2) output rows (c1 is recomputed on the halo rows of neighbouring tiles).
+// Returns false -- nothing launched -- when the pair needs more than one co-tile or does not fit shared memory.
+bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
+  if (!tcconv_supported(P1) || !P2.w_h) return false;
+  const int BN = P1.tc_bn;
+  if (P2.tc_bn != BN || P1.Cout > BN || P2.Cin != P1.Cout || P2.Cout > BN || P1.Wreal || P2.Wreal || P1.strips ||
+      P1.G != P2.G || P1.L != P2.L || P1.pro != PRO_LRELU || P2.pro != PRO_LRELU || (P2.epi != EPI_RES && P2.epi != EPI_ACC))
+    return false;
+  tc5_rows(P1);
+  const int span2 = tc5_rows(P2);
+  P2.tc_bn = BN;
+  size_t smem = 0;
+  const long a2bytes = 2L * P2.tc_chunks_h * P2.R * 128;   // c2's hi / lo operand tile, in c1's operand buffers
+  if (!tc5_plan(P1, BN, a2bytes, P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps, smem)) return false;
+  dim3 grid(cdiv(tc_lv(P1), TC_ROWS - span2), 1, tc_groups(P1));
+  tc5_set_smem_limits();
+  void* rec = profile_begin_pair(P1, P2, st);
+  if (BN == 128) launch_pdl(tcpair_kernel<128>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+  else if (BN == 64) launch_pdl(tcpair_kernel<64>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+  else launch_pdl(tcpair_kernel<32>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+  profile_end(rec, st);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+  return true;
 }
 
 // returns false when the layer has no fp16 image or does not fit the shared-memory budget
