@@ -337,6 +337,7 @@ struct Hifigan : Handle {
   float* pin_mel = nullptr; float* pin_wav = nullptr; size_t pin_mel_n = 0, pin_wav_n = 0;
   cudaStream_t own_stream = nullptr;
   bool fuse_resblock = true;        // AGPT_FUSE_RESBLOCK=0: every ResBlock1 conv as its own launch
+  bool tall_tiles = true;           // AGPT_TALL_TILES=0: 128-row tiles only (TapConvParams::tc_tall)
 
   ~Hifigan() override {
     if (pin_mel) cudaFreeHost(pin_mel);
@@ -372,6 +373,7 @@ struct Hifigan : Handle {
       P.in = melT.p; P.in_gstride = (long)T * cfg.n_mels; P.in_pitch = cfg.n_mels;
       P.out = cur; P.out_gstride = (long)T * C0; P.out_pitch = C0;
       P.pro = PRO_NONE; P.epi = EPI_BIAS;
+      P.tc_tall = tall_tiles;
       tapconv_launch(P, st);
     }
     long L = T; int C = C0;
@@ -384,6 +386,7 @@ struct Hifigan : Handle {
         P.in = cur; P.in_gstride = L * C; P.in_pitch = C;
         P.out = X; P.out_gstride = L * u * Co; P.out_pitch = u * Co;
         P.pro = big ? PRO_NONE : PRO_LRELU; P.slope = 0.1f; P.epi = EPI_BIAS;   // BigVGAN upsamples x directly (models.py:184-186)
+        P.tc_tall = tall_tiles;
         tapconv_launch(P, st);
       }
       L *= u; C = Co;
@@ -403,6 +406,7 @@ struct Hifigan : Handle {
         P.in = in; P.in_gstride = gs; P.in_pitch = gq * C;
         P.out = out; P.out_gstride = gs; P.out_pitch = gq * C;
         P.pro = big ? PRO_NONE : PRO_LRELU; P.slope = 0.1f;
+        P.tc_tall = tall_tiles;
         return P;
       };
       for (int j = 0; j < cfg.num_kernels; ++j) {
@@ -479,6 +483,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   std::unique_ptr<Hifigan> h(new Hifigan());
   h->magic = kMagicHifigan; h->device = device; h->cfg = *cfg;
   { const char* e = getenv("AGPT_FUSE_RESBLOCK"); h->fuse_resblock = !(e && e[0] == '0'); }
+  { const char* e = getenv("AGPT_TALL_TILES"); h->tall_tiles = !(e && e[0] == '0'); }
   WeightCursor wc{W, nW};
   { const float* w = wc.next(); const float* b = wc.next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
   h->ups.resize(nu);

@@ -10,6 +10,7 @@ struct ProfRec { cudaEvent_t e0, e1; int variant; double flops, bytes; int G, L,
 static bool g_prof = false;
 constexpr int PROF_PAIR = 16;   // record epi code of a fused ResBlock pair: 16 + the epilogue of its second conv
 static std::vector<ProfRec> g_recs;
+static long long g_tall = 0;    // recorded launches that ran 256-row tiles (the dump line has no field for it)
 
 bool profile_enabled() { return g_prof; }
 
@@ -18,8 +19,12 @@ void profile_enable(int on) {
   if (!on) {
     for (auto& r : g_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
     g_recs.clear();
+    g_tall = 0;
   }
 }
+
+void profile_count_tall() { if (g_prof) ++g_tall; }
+long long profile_tall_launches() { return g_tall; }
 
 // Sums over the records since profile_enable(1): per variant (FMA BN = 128, 64, 32; 3 = wgmma)
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches) {

@@ -69,6 +69,9 @@ struct TapConvParams {
   // optional operand-plane copy of the GATE / GEGLU epilogue's output (fp16 hi/lo [L][pl_pitch], G == 1): the
   // consumer (UNet ff2, a 4C-deep 1-tap GEMM) is then plane-fed; with out == nullptr the fp32 tensor is not written
   __half* pl_hi; __half* pl_lo; int pl_pitch;
+  // 1: the tensor-core kernels may run 256-row tiles (tc5_tall in tcconv5.cu decides per launch); set by the HiFi-GAN
+  // driver.  Kept last: the kernels read the fields above at fixed parameter-bank offsets, which stay as they were.
+  int tc_tall;
 };
 
 __host__ __device__ inline int tc_wv(const TapConvParams& P) { return P.Wreal > 0 ? (P.strips > 0 ? P.strip_w + 2 : P.Wreal + 1) : 0; }
@@ -124,8 +127,8 @@ void tapconv_launch(TapConvParams P, cudaStream_t st);
 void tcconv_launch(TapConvParams P, cudaStream_t st);          // tensor-core dispatcher (tcconv.cu)
 bool tcconv5_launch(TapConvParams P, cudaStream_t st);
 bool tcpair_launch(TapConvParams c1, TapConvParams c2, cudaStream_t st);   // fused ResBlock1 pair (tcconv5.cu)
-struct HTile { int bn; const float* w; long ntiles; };
-HTile pick_h_tile(const TapConvParams& P, int sms);   // tile width of the fp16 tensor-core kernel (tcconv5.cu)
+struct HTile { int bn; const float* w; long ntiles; int mt; };
+HTile pick_h_tile(const TapConvParams& P, int sms);   // tile width and height of the fp16 tensor-core kernel (tcconv5.cu)
 void pack_h_weights(struct PackedConv& pc, const std::vector<float>& h);
 bool tcconv_supported(const TapConvParams& P);
 void pack_tc_weights(struct PackedConv& pc, const std::vector<float>& h);
@@ -135,6 +138,8 @@ void profile_enable(int on);
 void* profile_begin(const TapConvParams& P, bool tc, double bytes_override, cudaStream_t st);
 void* profile_begin_pair(const TapConvParams& c1, const TapConvParams& c2, cudaStream_t st);
 void profile_end(void* rec, cudaStream_t st);
+void profile_count_tall();            // a tensor-core launch with 256-row tiles (counted while profiling)
+long long profile_tall_launches();
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches);
 long profile_dump(char* out, long cap);
 double fma_peak_tflops();

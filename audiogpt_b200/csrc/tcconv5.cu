@@ -9,10 +9,11 @@
 // the networks on this path stay orders of magnitude below); below 2^-14 the lo part becomes a
 // subnormal, i.e. the absolute representation error of an activation is max(2^-22 |x|, 2^-25).
 //
-// One CTA = one [128 rows x BN] output tile.  K-major SWIZZLE_128B operand tiles, a conv tap = a row-shifted
-// descriptor start address.  Two worker warpgroups convert fp32 activations into the fp16 hi/lo tiles, then each
-// issues wgmma for its 64 rows with the accumulator in registers (one wgmma group in flight while the next chunk is
-// converted), then runs the fused epilogue; warp 8 streams the weights (cp.async.bulk, mbarrier full/empty ring).
+// One CTA = one [MT rows x BN] output tile (MT = 128, or 256 for narrow tiles).  K-major SWIZZLE_128B operand tiles,
+// a conv tap = a row-shifted descriptor start address.  Two worker warpgroups convert fp32 activations into the fp16
+// hi/lo tiles, then each issues wgmma for its MT / 2 rows (MT / 128 blocks of 64) with the accumulators in registers
+// (one wgmma group in flight while the next chunk is converted), then runs the fused epilogue; warp 8 streams the
+// weights (cp.async.bulk, mbarrier full/empty ring).
 #include "tapconv.cuh"
 #include "tapconv_epi.cuh"
 #include "tc_common.cuh"
@@ -29,14 +30,14 @@ constexpr int kMaxDyn = 227 * 1024 - 256;   // the kernel also has a small stati
 struct Tc5Smem {
   uint32_t a_hi[MAX_NA], a_lo[MAX_NA], w[MAX_NW], raw[2], rowinfo, rowp, bars, total;
 };
-__host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int RRA, int NA, int NW, int NR) {
+__host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int MT, int RRA, int NA, int NW, int NR) {
   uint32_t o = 0;
   for (int i = 0; i < MAX_NA; ++i) { s.a_hi[i] = o; if (i < NA) o += RRA * 128; }
   for (int i = 0; i < MAX_NA; ++i) { s.a_lo[i] = o; if (i < NA) o += RRA * 128; }
   for (int i = 0; i < MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += 2 * BN * 128; }
   for (int i = 0; i < 2; ++i) { s.raw[i] = o; if (i < NR) o += RRA * 256; }
   s.rowinfo = o; o += RRA * 4;
-  s.rowp = o; o += TC_ROWS * 4;
+  s.rowp = o; o += MT * 4;
   o = (o + 15) & ~15u;
   s.bars = o; o += 2 * MAX_NW * 8;
   s.total = o;
@@ -63,14 +64,23 @@ __device__ __forceinline__ void fence_acc(float* a) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(a[i])::"memory");
 }
 
-template <int BN>
+// tile row of epilogue item i of worker xt, (xt + i NWK) / 8, as base + immediate: the tall tiles read the row table
+// with it, so ptxas recomputes each item's row-table address instead of keeping one 64-bit address per item alive from
+// one column block to the next (which spills at 168 registers).  The 128-row tiles keep the form they were tuned with.
+__device__ __forceinline__ int item_row(int xt, int i) { return (xt >> 3) + i * (NWK / 8); }
+
+constexpr int TC_TALL = 256;                 // rows of a tall tile (BN <= 64 only: the doubled accumulator still fits)
+constexpr uint64_t BLK_DESC = (64 * 128) >> 4;   // descriptor start-address step from one 64-row block to the next
+
+template <int BN, int MT>
 __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_constant__ TapConvParams P) {
-  constexpr int NB = tc5_nb(BN), NJ = BN / NB;
+  constexpr int NB = tc5_nb(BN), NJ = BN / NB, MB = MT / 128;   // MB: 64-row blocks per worker warpgroup
+  static_assert(MT == TC_ROWS || (MT == TC_TALL && BN <= 64), "tall tiles are for narrow BN");
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
   const int RRA = P.R, NA = P.tc_na, NW = P.tc_nw, NR = P.tc_nr;
   __shared__ Tc5Smem S;
-  if (threadIdx.x == 0) tc5_layout(S, BN, RRA, NA, NW, NR);
+  if (threadIdx.x == 0) tc5_layout(S, BN, MT, RRA, NA, NW, NR);
   __syncthreads();
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S.bars);
   uint64_t* w_full = bars;                // [MAX_NW]
@@ -81,10 +91,10 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // warpgroup index broadcast from lane 0: ptxas then sees the role branches as warpgroup-uniform, which keeps the
   // wgmmas of the worker warpgroups asynchronous instead of serialized
-  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // workers: output rows 64 wg .. 64 wg + 63 of the tile
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // workers: output rows MT/2 wg .. MT/2 (wg + 1) - 1 of the tile
   const bool is_worker = wg < 2;
   const int xt = tid;                             // worker thread index 0..NWK-1
-  const int gz = blockIdx.z, g = tc_sample(P, gz), co0 = blockIdx.y * BN, q0 = blockIdx.x * TC_ROWS;
+  const int gz = blockIdx.z, g = tc_sample(P, gz), co0 = blockIdx.y * BN, q0 = blockIdx.x * MT;
   const int Wv = tc_wv(P);
   const int Lv = tc_lv(P);
   const int nchunks = P.tc_chunks_h, ntaps = P.ntaps, total = nchunks * ntaps;
@@ -102,7 +112,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
       const int r = tc_row_in(P, gz, q0 + lo + i, Wv, Lv);
       rowinfo[i] = r >= 0 ? r * P.in_pitch : -1;
     }
-    if (xt < TC_ROWS) rowp[xt] = tc_row_out(P, gz, q0 + xt, Wv, Lv);   // output row -> real position (or -1)
+    if (xt < MT) rowp[xt] = tc_row_out(P, gz, q0 + xt, Wv, Lv);   // output row -> real position (or -1)
   }
   __syncthreads();
   pdl_wait();          // everything above overlaps the previous kernel's tail
@@ -139,7 +149,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
       if (P.epi == EPI_ACC && P.accumulate) { pf1 = P.out; gs1 = P.out_gstride; pitch1 = P.out_pitch; }
       if (P.epi == EPI_DIFFOUT) { pf0 = P.out; gs0 = P.out_gstride; pitch0 = P.out_pitch; }
       const int lines = (BN * 4) / 128 > 0 ? (BN * 4) / 128 : 1;     // 128-byte lines per output row
-      for (int idx = xt; idx < TC_ROWS * lines; idx += NWK) {
+      for (int idx = xt; idx < MT * lines; idx += NWK) {
         const int p = rowp[idx / lines];
         const int co = co0 + (idx % lines) * 32;
         if (p >= 0 && co < P.Cout) {
@@ -148,12 +158,15 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
         }
       }
     }
-    // this warpgroup's accumulator: rows 64 wg .. 64 wg + 63, BN columns in NJ blocks of NB (wgmma fragment layout)
-    float acc[NJ][NB / 2];
+    // this warpgroup's accumulator: row block b = rows MT/2 wg + 64 b .. + 63, BN columns in NJ blocks of NB (wgmma
+    // fragment layout)
+    float acc[MB][NJ][NB / 2];
 #pragma unroll
-    for (int j = 0; j < NJ; ++j)
+    for (int b = 0; b < MB; ++b)
 #pragma unroll
-      for (int i = 0; i < NB / 2; ++i) acc[j][i] = 0.f;
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int i = 0; i < NB / 2; ++i) acc[b][j][i] = 0.f;
     const int items = RRA * 8;
     int it = 0, prev = -1;     // prev: weight stage of the newest wgmma group, released once that group has completed
     for (int c = 0; c < nchunks; ++c) {
@@ -196,8 +209,10 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
       const int cn = c + NR;
       if (cn < nchunks) issue_raw(cn, rb);
       // =========================== worker warps: wgmma over the taps of chunk c ===========================
-      // products x_hi w_hi + x_lo w_hi + x_hi w_lo into one fp32 accumulator; a tap is a start address shifted by rows
-      const uint32_t ahi0 = smem_u32(ahi) + (uint32_t)(wg * 64 - lo) * 128u, alo0 = smem_u32(alo) + (uint32_t)(wg * 64 - lo) * 128u;
+      // products x_hi w_hi + x_lo w_hi + x_hi w_lo into one fp32 accumulator; a tap is a start address shifted by rows,
+      // a row block one shifted by 64 rows more: every block reuses the weight stage, which is released (one group
+      // later) when the group holding all blocks' wgmmas has completed
+      const uint32_t ahi0 = smem_u32(ahi) + (uint32_t)(wg * (MT / 2) - lo) * 128u, alo0 = smem_u32(alo) + (uint32_t)(wg * (MT / 2) - lo) * 128u;
       for (int t = 0; t < ntaps; ++t, ++it) {
         const int s = it % NW;
         mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
@@ -205,22 +220,29 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
         const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
         const uint32_t ws = smem_u32(smem + S.w[s]);
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        for (int b = 0; b < MB; ++b)
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
         wgmma_fence();
         for (int k = 0; k < ksteps; ++k) {
           const uint64_t ko = (uint64_t)((k * 32) >> 4);
 #pragma unroll
-          for (int j = 0; j < NJ; ++j) {
-            const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
-            wgmma_nb<NB>(acc[j], dah + ko, dwh);
-            wgmma_nb<NB>(acc[j], dal + ko, dwh);
-            wgmma_nb<NB>(acc[j], dah + ko, dwl);
-          }
+          for (int b = 0; b < MB; ++b)
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+              const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
+              const uint64_t ab = ko + b * BLK_DESC;
+              wgmma_nb<NB>(acc[b][j], dah + ab, dwh);
+              wgmma_nb<NB>(acc[b][j], dal + ab, dwh);
+              wgmma_nb<NB>(acc[b][j], dah + ab, dwl);
+            }
         }
         wgmma_commit();
         wgmma_wait<1>();
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        for (int b = 0; b < MB; ++b)
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
         if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
         prev = s;
       }
@@ -231,51 +253,65 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
       }
     }
     // =========================== worker warps: epilogue ===========================
-    // registers (x inverse weight scale) -> swizzled staging block [128 rows][32 cols] in shared memory (the operand
-    // buffers are free now) -> coalesced (row, 16-byte chunk) items through the fused epilogue.  The global READS of a
-    // block (residual / old accumulator) are issued one block ahead -- for block 0 before the accumulator is complete.
+    // registers (x inverse weight scale) -> swizzled staging block [MT rows][32 cols] in shared memory (the operand
+    // buffers are free now) -> coalesced (row, 16-byte chunk) items through the fused epilogue.  The global READS of
+    // items 0..3 (rows 0..127) of a block (residual / old accumulator) are issued one block ahead -- for block 0 before
+    // the accumulator is complete.  A tall tile holds the reads of 4 items too, next to an accumulator as large as a
+    // 128-wide one: it reads block 0 once that block is staged, and item i + 4 (rows 128..255) once item i is stored.
     EpiPre pre[8];
     int pp[8];
-    constexpr int nitem = (TC_ROWS * 8) / NWK;   // 4 items per worker and block
+    constexpr int nitem = (MT * 8) / NWK;   // 4 items per worker and block (8 on a tall tile)
     const float dsc = P.tc_descale;
     auto load_block = [&](int cb) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int idx = xt + i * NWK;
-        pp[i] = (i < nitem) ? rowp[idx >> 3] : -1;
+        pp[i] = (i < 4 && i < nitem) ? rowp[MT == TC_ROWS ? idx >> 3 : item_row(xt, i)] : -1;
         if (pp[i] >= 0) epi_load(P, g, pp[i], co0 + cb + 4 * (idx & 7), pre[i]);
       }
     };
-    load_block(0);
+    if (MT == TC_ROWS) load_block(0);
     if (dbg_on && tid == 0) { dbg[2] = dbg[1]; dbg[3] = clock64(); dbg[6] = 0; dbg[7] = 0; }   // the workers issue the wgmmas: no waits of a separate issuer
     wgmma_wait<0>();
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+    for (int b = 0; b < MB; ++b)
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
     named_bar_sync(1, NWK);                      // both warpgroups' wgmmas are done reading the operand buffers
     if (dbg_on && tid == 0) dbg[4] = clock64();
-    uint8_t* stg0 = smem + S.a_hi[0];            // 2 x 16 KB inside the first operand buffers (>= 32 KB)
-    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    uint8_t* stg0 = smem + S.a_hi[0];            // 2 x MT x 128 B inside the first operand buffers (tc5_plan)
+    const int r0 = wg * (MT / 2) + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
     for (int blk = 0; blk < BN / 32; ++blk) {
       const int cb = blk * 32;
-      uint8_t* stg = stg0 + (blk & 1) * (TC_ROWS * 128);
-      const float* a = &acc[cb / NB][4 * ((cb % NB) / 8)];
+      uint8_t* stg = stg0 + (blk & 1) * (MT * 128);
 #pragma unroll
-      for (int i8 = 0; i8 < 4; ++i8) {
-        const int col = 8 * i8 + c0;
-        *reinterpret_cast<float2*>(stg + sw128(r0, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
-        *reinterpret_cast<float2*>(stg + sw128(r0 + 8, col >> 2) + (col & 3) * 4) =
-            make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+      for (int b = 0; b < MB; ++b) {
+        const float* a = &acc[b][cb / NB][4 * ((cb % NB) / 8)];
+        const int r = r0 + 64 * b;
+#pragma unroll
+        for (int i8 = 0; i8 < 4; ++i8) {
+          const int col = 8 * i8 + c0;
+          *reinterpret_cast<float2*>(stg + sw128(r, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
+          *reinterpret_cast<float2*>(stg + sw128(r + 8, col >> 2) + (col & 3) * 4) =
+              make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+        }
       }
+      if (MT == TC_TALL && blk == 0) load_block(0);
       named_bar_sync(1, NWK);
       const int jc = xt & 7;                       // all items of this thread share the 4-channel group
       const float4 cv = epi_colvec(P, g, co0 + cb + 4 * jc);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int idx = xt + i * NWK;
-        const int row = (idx >> 3) & (TC_ROWS - 1);   // pp[i] < 0 for i >= nitem
+        const int row = (idx >> 3) & (MT - 1);   // pp[i] < 0 for i >= nitem (items 4..7 of a tall tile: read below)
         if (pp[i] >= 0)
           epi_store_cv(P, g, pp[i], co0 + cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
+        if (i + 4 < nitem) {
+          const int idx4 = idx + 4 * NWK;
+          pp[i + 4] = rowp[item_row(xt, i + 4)];
+          if (pp[i + 4] >= 0) epi_load(P, g, pp[i + 4], co0 + cb + 4 * (idx4 & 7), pre[i + 4]);
+        }
       }
       if (cb + 32 < BN) load_block(cb + 32);
       // staging halves alternate; a half is rewritten two blocks later, after the next named
@@ -296,20 +332,21 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
 }
 
 // One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))), in one CTA per tile (tcpair_launch): the tcconv5 pipeline
-// runs c1 over the 128 intermediate rows qa .. qa + 127 (qa = q0 + lowest tap of c2), c1's accumulator becomes c2's
-// operand tile in shared memory, and the tcconv5 pipeline runs c2 over it; a tile keeps the 128 - span(c2) outputs
+// runs c1 over the MT intermediate rows qa .. qa + MT - 1 (qa = q0 + lowest tap of c2), c1's accumulator becomes c2's
+// operand tile in shared memory, and the tcconv5 pipeline runs c2 over it; a tile keeps the MT - span(c2) outputs
 // that read only those rows.  P1 / P2: the two convs' launch parameters (leaky-ReLU prologue, 1-D rows, one co-tile,
 // BN >= C); P2's epilogue (EPI_RES / EPI_ACC) writes the output.  The weight producer streams c1's stages, then c2's,
 // through one mbarrier ring.
-template <int BN>
+template <int BN, int MT>
 __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_constant__ TapConvParams P1,
                                                                const __grid_constant__ TapConvParams P2) {
-  constexpr int NB = tc5_nb(BN), NJ = BN / NB;
+  constexpr int NB = tc5_nb(BN), NJ = BN / NB, MB = MT / 128;
+  static_assert(MT == TC_ROWS || (MT == TC_TALL && BN <= 64), "tall tiles are for narrow BN");
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
   const int RRA = P1.R, NA = P1.tc_na, NW = P1.tc_nw, NR = P1.tc_nr;
   __shared__ Tc5Smem S;
-  if (threadIdx.x == 0) tc5_layout(S, BN, RRA, NA, NW, NR);
+  if (threadIdx.x == 0) tc5_layout(S, BN, MT, RRA, NA, NW, NR);
   __syncthreads();
   uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
   uint64_t* w_empty = w_full + MAX_NW;
@@ -322,7 +359,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
   const int xt = tid;
   int span2 = 0;
   for (int t = 0; t < P2.ntaps; ++t) span2 = max(span2, P2.tap_off[t] - P2.lo_al);
-  const int g = blockIdx.z, Lv = P1.L, q0 = blockIdx.x * (TC_ROWS - span2), qa = q0 + P2.lo_al;
+  const int g = blockIdx.z, Lv = P1.L, q0 = blockIdx.x * (MT - span2), qa = q0 + P2.lo_al;
   const int nchunks = P1.tc_chunks_h, total = nchunks * P1.ntaps;
   const int lo = P1.lo_al;
 
@@ -335,7 +372,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
       const int r = qa + lo + i;
       rowinfo[i] = (r >= 0 && r < Lv) ? r * P1.in_pitch : -1;
     }
-    if (xt < TC_ROWS) rowp[xt] = (xt < TC_ROWS - span2 && q0 + xt < Lv) ? q0 + xt : -1;
+    if (xt < MT) rowp[xt] = (xt < MT - span2 && q0 + xt < Lv) ? q0 + xt : -1;
   }
   __syncthreads();
   pdl_wait();
@@ -360,7 +397,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
     if (NR == 2 && nchunks > 1) issue_raw(1, 1);
     {  // the epilogue's residual / old accumulator rows into L2 while the main loop runs
       const int lines = (BN * 4) / 128 > 0 ? (BN * 4) / 128 : 1;
-      for (int idx = xt; idx < TC_ROWS * lines; idx += NWK) {
+      for (int idx = xt; idx < MT * lines; idx += NWK) {
         const int p = rowp[idx / lines];
         const int co = (idx % lines) * 32;
         if (p >= 0 && co < P2.Cout) {
@@ -370,11 +407,13 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
         }
       }
     }
-    float acc[NJ][NB / 2];
+    float acc[MB][NJ][NB / 2];   // row block b: rows MT/2 wg + 64 b .. + 63 of the tile
 #pragma unroll
-    for (int j = 0; j < NJ; ++j)
+    for (int b = 0; b < MB; ++b)
 #pragma unroll
-      for (int i = 0; i < NB / 2; ++i) acc[j][i] = 0.f;
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int i = 0; i < NB / 2; ++i) acc[b][j][i] = 0.f;
     int it = 0, prev = -1;     // prev: weight stage of the newest wgmma group, released once that group has completed
     // wgmma over the taps of one conv and one 64-channel chunk of its operand tile (ahi0 / alo0: this warpgroup's rows)
     auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {
@@ -385,22 +424,29 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
         const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
         const uint32_t ws = smem_u32(smem + S.w[s]);
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        for (int b = 0; b < MB; ++b)
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
         wgmma_fence();
         for (int k = 0; k < ksteps; ++k) {
           const uint64_t ko = (uint64_t)((k * 32) >> 4);
 #pragma unroll
-          for (int j = 0; j < NJ; ++j) {
-            const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
-            wgmma_nb<NB>(acc[j], dah + ko, dwh);
-            wgmma_nb<NB>(acc[j], dal + ko, dwh);
-            wgmma_nb<NB>(acc[j], dah + ko, dwl);
-          }
+          for (int b = 0; b < MB; ++b)
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+              const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
+              const uint64_t ab = ko + b * BLK_DESC;
+              wgmma_nb<NB>(acc[b][j], dah + ab, dwh);
+              wgmma_nb<NB>(acc[b][j], dal + ab, dwh);
+              wgmma_nb<NB>(acc[b][j], dah + ab, dwl);
+            }
         }
         wgmma_commit();
         wgmma_wait<1>();
 #pragma unroll
-        for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+        for (int b = 0; b < MB; ++b)
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
         if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
         prev = s;
       }
@@ -435,7 +481,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
       fence_proxy_async();
       named_bar_sync(1, NWK);
       if (c + NR < nchunks) issue_raw(c + NR, rb);
-      mma_taps(P1, smem_u32(ahi) + (uint32_t)(wg * 64 - lo) * 128u, smem_u32(alo) + (uint32_t)(wg * 64 - lo) * 128u,
+      mma_taps(P1, smem_u32(ahi) + (uint32_t)(wg * (MT / 2) - lo) * 128u, smem_u32(alo) + (uint32_t)(wg * (MT / 2) - lo) * 128u,
                (kv + 15) >> 4);
       if (NA == 1) {
         wgmma_wait<0>();
@@ -447,10 +493,12 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
     // The arithmetic of c1's EPI_BIAS store followed by c2's PRO_LRELU transform (acc * descale + bias, leaky ReLU,
     // hi/lo split), so c2 multiplies the operands a separate launch would.  The tile [RR2 rows][C channels] (K-major
     // SWIZZLE_128B, per 64-channel chunk a hi and a lo block) replaces c1's operand buffers: rows outside the sample are
-    // c2's zero padding, channels >= C are zero, rows >= 128 feed only the discarded outputs and are zero.
+    // c2's zero padding, channels >= C are zero, rows >= MT feed only the discarded outputs and are zero.
     wgmma_wait<0>();
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+    for (int b = 0; b < MB; ++b)
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
     if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
     prev = -1;
     named_bar_sync(1, NWK);                    // both warpgroups' c1 wgmmas are done reading the operand buffers
@@ -458,87 +506,103 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
     uint8_t* a2 = smem + S.a_hi[0];
     const uint32_t lo_part = (uint32_t)nch2 * RR2 * 128;   // the hi blocks, then the lo blocks
     const float dsc1 = P1.tc_descale;
-    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    const int r0 = wg * (MT / 2) + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
     for (int j = 0; j < NJ; ++j)
 #pragma unroll
       for (int i = 0; i < NB / 8; ++i) {
         const int col = j * NB + 8 * i + c0;   // accumulator fragment layout: see wgmma_n16
         const bool cok = col < C2;
-        float2 b = make_float2(0.f, 0.f);
-        if (cok && P1.bias) b = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
+        float2 bv = make_float2(0.f, 0.f);
+        if (cok && P1.bias) bv = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
         uint8_t* hi = a2 + (uint32_t)(col >> 6) * RR2 * 128;
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = r0 + 8 * h;
-          float v0 = 0.f, v1 = 0.f;
-          if (cok && qa + r >= 0 && qa + r < Lv) {
-            v0 = lrelu(__fadd_rn(__fmul_rn(acc[j][4 * i + 2 * h], dsc1), b.x), P2.slope);
-            v1 = lrelu(__fadd_rn(__fmul_rn(acc[j][4 * i + 2 * h + 1], dsc1), b.y), P2.slope);
+        for (int b = 0; b < MB; ++b)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 64 * b + 8 * h;
+            float v0 = 0.f, v1 = 0.f;
+            if (cok && qa + r >= 0 && qa + r < Lv) {
+              v0 = lrelu(__fadd_rn(__fmul_rn(acc[b][j][4 * i + 2 * h], dsc1), bv.x), P2.slope);
+              v1 = lrelu(__fadd_rn(__fmul_rn(acc[b][j][4 * i + 2 * h + 1], dsc1), bv.y), P2.slope);
+            }
+            uint32_t l;
+            const uint32_t hw = split2(v0, v1, l);
+            const uint32_t o = sw128(r, (col & 63) >> 3) + (col & 7) * 2;
+            *reinterpret_cast<uint32_t*>(hi + o) = hw;
+            *reinterpret_cast<uint32_t*>(hi + lo_part + o) = l;
           }
-          uint32_t l;
-          const uint32_t hw = split2(v0, v1, l);
-          const uint32_t o = sw128(r, (col & 63) >> 3) + (col & 7) * 2;
-          *reinterpret_cast<uint32_t*>(hi + o) = hw;
-          *reinterpret_cast<uint32_t*>(hi + lo_part + o) = l;
-        }
       }
-    const int zitems = (RR2 - TC_ROWS) * 8;    // 16-byte units of rows 128 .. RR2 - 1 per block
+    const int zitems = (RR2 - MT) * 8;         // 16-byte units of rows MT .. RR2 - 1 per block
     for (int idx = xt; idx < zitems * 2 * nch2; idx += NWK) {
       const int blk = idx / zitems, u = idx - blk * zitems;
-      *reinterpret_cast<uint4*>(a2 + (uint32_t)blk * RR2 * 128 + TC_ROWS * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+      *reinterpret_cast<uint4*>(a2 + (uint32_t)blk * RR2 * 128 + MT * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
     }
 #pragma unroll
-    for (int j = 0; j < NJ; ++j)
+    for (int b = 0; b < MB; ++b)
 #pragma unroll
-      for (int i = 0; i < NB / 2; ++i) acc[j][i] = 0.f;
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int i = 0; i < NB / 2; ++i) acc[b][j][i] = 0.f;
     fence_proxy_async();
     named_bar_sync(1, NWK);
     // =========================== c2: wgmma over the resident tile ===========================
     for (int c = 0; c < nch2; ++c) {
-      const uint32_t ahi0 = smem_u32(a2) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * 64 - P2.lo_al) * 128u;
+      const uint32_t ahi0 = smem_u32(a2) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * (MT / 2) - P2.lo_al) * 128u;
       mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, C2 - c * H_KCH) + 15) >> 4);
     }
     // =========================== c2's epilogue (as tcconv5_kernel) ===========================
     EpiPre pre[8];
     int pp[8];
-    constexpr int nitem = (TC_ROWS * 8) / NWK;
+    constexpr int nitem = (MT * 8) / NWK;
     const float dsc = P2.tc_descale;
-    auto load_block = [&](int cb) {
+    auto load_block = [&](int cb) {   // as tcconv5_kernel: items 0..3 one block ahead, a tall tile's 4..7 during the stores
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int idx = xt + i * NWK;
-        pp[i] = (i < nitem) ? rowp[idx >> 3] : -1;
+        pp[i] = (i < 4 && i < nitem) ? rowp[MT == TC_ROWS ? idx >> 3 : item_row(xt, i)] : -1;
         if (pp[i] >= 0) epi_load(P2, g, pp[i], cb + 4 * (idx & 7), pre[i]);
       }
     };
-    load_block(0);
+    if (MT == TC_ROWS) load_block(0);
     wgmma_wait<0>();
 #pragma unroll
-    for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[j]);
+    for (int b = 0; b < MB; ++b)
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
     named_bar_sync(1, NWK);
     uint8_t* stg0 = smem + S.a_hi[0];
 #pragma unroll
     for (int blk = 0; blk < BN / 32; ++blk) {
       const int cb = blk * 32;
-      uint8_t* stg = stg0 + (blk & 1) * (TC_ROWS * 128);
-      const float* a = &acc[cb / NB][4 * ((cb % NB) / 8)];
+      uint8_t* stg = stg0 + (blk & 1) * (MT * 128);
 #pragma unroll
-      for (int i8 = 0; i8 < 4; ++i8) {
-        const int col = 8 * i8 + c0;
-        *reinterpret_cast<float2*>(stg + sw128(r0, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
-        *reinterpret_cast<float2*>(stg + sw128(r0 + 8, col >> 2) + (col & 3) * 4) =
-            make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+      for (int b = 0; b < MB; ++b) {
+        const float* a = &acc[b][cb / NB][4 * ((cb % NB) / 8)];
+        const int r = r0 + 64 * b;
+#pragma unroll
+        for (int i8 = 0; i8 < 4; ++i8) {
+          const int col = 8 * i8 + c0;
+          *reinterpret_cast<float2*>(stg + sw128(r, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
+          *reinterpret_cast<float2*>(stg + sw128(r + 8, col >> 2) + (col & 3) * 4) =
+              make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+        }
       }
+      if (MT == TC_TALL && blk == 0) load_block(0);
       named_bar_sync(1, NWK);
       const int jc = xt & 7;
       const float4 cv = epi_colvec(P2, g, cb + 4 * jc);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int idx = xt + i * NWK;
-        const int row = (idx >> 3) & (TC_ROWS - 1);
+        const int row = (idx >> 3) & (MT - 1);
         if (pp[i] >= 0)
           epi_store_cv(P2, g, pp[i], cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
+        if (i + 4 < nitem) {
+          const int idx4 = idx + 4 * NWK;
+          pp[i + 4] = rowp[item_row(xt, i + 4)];
+          if (pp[i + 4] >= 0) epi_load(P2, g, pp[i + 4], cb + 4 * (idx4 & 7), pre[i + 4]);
+        }
       }
       if (cb + 32 < BN) load_block(cb + 32);
     }
@@ -605,32 +669,33 @@ void pack_h_weights(PackedConv& pc, const std::vector<float>& h) {
   if (pc.tc_bn == 128 && pc.Cout > 128) build_h_image(pc, h, 96, wscale, pc.w_h96);
 }
 
-// lo_al = the lowest tap offset, R = operand-tile rows (128 + tap span, rounded to the 8-row swizzle atom); returns the span
-static int tc5_rows(TapConvParams& P) {
+// lo_al = the lowest tap offset, R = operand-tile rows (MT + tap span, rounded to the 8-row swizzle atom); returns the span
+static int tc5_rows(TapConvParams& P, int MT) {
   int lo = P.tap_off[0], hi = P.tap_off[0];
   for (int t = 1; t < P.ntaps; ++t) { lo = std::min(lo, P.tap_off[t]); hi = std::max(hi, P.tap_off[t]); }
   P.lo_al = lo;
-  P.R = round_up(TC_ROWS + (hi - lo), 8);
+  P.R = round_up(MT + (hi - lo), 8);
   return hi - lo;
 }
 
-// Shared-memory plan of a BN-wide tile (operand, raw-staging and weight-ring buffers) for P after tc5_rows; false when
+// Shared-memory plan of a BN x MT tile (operand, raw-staging and weight-ring buffers) for P after tc5_rows; false when
 // it does not fit.  a_min: bytes the operand buffers must span at least; iters: weight stages the kernel streams.
-static bool tc5_plan(TapConvParams& P, int BN, long a_min, int iters, size_t& smem) {
+static bool tc5_plan(TapConvParams& P, int BN, int MT, long a_min, int iters, size_t& smem) {
   const int RRA = P.R;
   P.tc_bn = BN;
-  const long avail = (long)kMaxDyn - 1024 /*align*/ - (RRA * 4 + TC_ROWS * 4 + 512) /*row tables + barriers*/;
+  const long avail = (long)kMaxDyn - 1024 /*align*/ - (RRA * 4 + MT * 4 + 512) /*row tables + barriers*/;
   const long abytes = 2L * RRA * 128, wbytes = 2L * BN * 128;
   const long rbytes = (long)RRA * 256;
+  const long stg = 2L * MT * 128;   // the epilogue stages 2 x [MT][32] fp32 through the operand buffers
   const int nch = P.tc_chunks_h;
   int NA = (P.ntaps == 1) ? 3 : 2;
   NA = std::max(1, std::min(NA, nch));
-  if ((long)NA * abytes < 32768) NA = (int)cdiv(32768L, abytes);   // the epilogue stages 2 x 16 KB through the operand buffers
+  if ((long)NA * abytes < stg) NA = (int)cdiv(stg, abytes);
   int NR = (nch > 1) ? 2 : 1;
   auto fits = [&](int na, int nr, int nw) { return na * abytes + nr * rbytes + nw * wbytes <= avail; };
   if (!fits(NA, NR, 2) && NA == 3) NA = 2;
   if (!fits(NA, NR, 2) && NR == 2) NR = 1;
-  if (!fits(NA, NR, 2) && NA == 2 && abytes >= 32768) NA = 1;
+  if (!fits(NA, NR, 2) && NA == 2 && abytes >= stg) NA = 1;
   if (NA * abytes < a_min) {
     NA = (int)cdiv(a_min, abytes);
     if (!fits(NA, NR, 2) && NR == 2) NR = 1;
@@ -640,7 +705,7 @@ static bool tc5_plan(TapConvParams& P, int BN, long a_min, int iters, size_t& sm
   NW = std::max(2, std::min(NW, std::max(2, iters)));
   P.tc_na = NA; P.tc_nw = NW; P.tc_nr = NR;
   Tc5Smem S;
-  tc5_layout(S, BN, RRA, NA, NW, NR);
+  tc5_layout(S, BN, MT, RRA, NA, NW, NR);
   smem = (size_t)S.total + 1024;
   return smem <= (size_t)kMaxDyn;
 }
@@ -650,56 +715,109 @@ static void tc5_set_smem_limits() {
   AGPT_CUDA(cudaGetDevice(&dev));
   static bool attr_done_dev[64] = {false};
   if (attr_done_dev[dev & 63]) return;
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<96>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<96, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
   attr_done_dev[dev & 63] = true;
 }
 
-// Try one tile width; returns false when it does not fit the shared-memory budget.
-static bool tcconv5_try(TapConvParams P, int BN, cudaStream_t st) {
-  tc5_rows(P);
+static int tc5_sms() {
+  int dev = 0;
+  AGPT_CUDA(cudaGetDevice(&dev));
+  static int sms_dev[64] = {0};
+  if (!sms_dev[dev & 63]) AGPT_CUDA(cudaDeviceGetAttribute(&sms_dev[dev & 63], cudaDevAttrMultiProcessorCount, dev));
+  return sms_dev[dev & 63];
+}
+
+// 256-row tiles: the handle allows them (TapConvParams::tc_tall), the tile is narrow (a BN = 128 accumulator doubled
+// would spill), the conv runs over plain 1-D rows, and the grid of tall tiles still fills every SM four times over.
+// A tall tile pays the fixed per-tile latency (operand load, first weight stage, epilogue) once for twice the rows and
+// reuses every weight stage across twice the rows.
+static bool tc5_tall(const TapConvParams& P, int bn, long tall_tiles, int sms) {
+  return P.tc_tall && bn <= 64 && !P.Wreal && !P.strips && tall_tiles >= 4L * sms;
+}
+
+// Try one tile shape; returns false when it does not fit the shared-memory budget.
+static bool tcconv5_try(TapConvParams P, int BN, int MT, cudaStream_t st) {
+  tc5_rows(P, MT);
   size_t smem = 0;
-  if (!tc5_plan(P, BN, 0, P.tc_chunks_h * P.ntaps, smem)) return false;
+  if (!tc5_plan(P, BN, MT, 0, P.tc_chunks_h * P.ntaps, smem)) return false;
   const int Lv = tc_lv(P);
-  dim3 grid(cdiv(Lv, TC_ROWS), cdiv(P.Cout, BN), tc_groups(P));
+  dim3 grid(cdiv(Lv, MT), cdiv(P.Cout, BN), tc_groups(P));
   tc5_set_smem_limits();
-  if (BN == 128) launch_pdl(tcconv5_kernel<128>, grid, dim3(V5_THREADS), smem, st, P);
-  else if (BN == 96) launch_pdl(tcconv5_kernel<96>, grid, dim3(V5_THREADS), smem, st, P);
-  else if (BN == 64) launch_pdl(tcconv5_kernel<64>, grid, dim3(V5_THREADS), smem, st, P);
-  else launch_pdl(tcconv5_kernel<32>, grid, dim3(V5_THREADS), smem, st, P);
+  if (MT == TC_TALL) {
+    if (BN == 64) launch_pdl(tcconv5_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P);
+    else launch_pdl(tcconv5_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P);
+    profile_count_tall();
+  } else if (BN == 128) launch_pdl(tcconv5_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
+  else if (BN == 96) launch_pdl(tcconv5_kernel<96, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
+  else if (BN == 64) launch_pdl(tcconv5_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
+  else launch_pdl(tcconv5_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
   return true;
 }
 
 // Tile width: the candidate (native 128|64|32, or 96 and 64 for native-128 layers) with the smallest waves x per-tile
 // cost, where waves = ceil(tiles / SMs): wider tiles amortise the activation operand, narrower ones fill the SMs.  No
 // 256-wide tile: its accumulator (128 registers per thread of a warpgroup) spills next to the transform's registers.
+// Tile height: 256 rows where tc5_tall allows it, else 128.
 HTile pick_h_tile(const TapConvParams& P, int sms) {
   const int Lv = tc_lv(P);
   const long rt = (long)cdiv(Lv, TC_ROWS) * tc_groups(P);
   static int allow96 = -1;
   if (allow96 < 0) { const char* e = getenv("AGPT_TC_BN96"); allow96 = (e && e[0] == '0') ? 0 : 1; }
   auto cost = [](int bn) { return bn == 128 ? 1.0 : (bn == 96 ? 0.82 : (bn == 64 ? 0.62 : 0.45)); };
-  HTile best{P.tc_bn, P.w_h, rt * cdiv(P.Cout, P.tc_bn)};
+  HTile best{P.tc_bn, P.w_h, rt * cdiv(P.Cout, P.tc_bn), TC_ROWS};
   double bs = (double)cdiv(best.ntiles, (long)sms) * cost(P.tc_bn);
   auto consider = [&](int bn, const float* w) {
     if (!w) return;
     const long nt = rt * cdiv(P.Cout, bn);
     const double sc = (double)cdiv(nt, (long)sms) * cost(bn);
-    if (sc < bs - 1e-9) { bs = sc; best = HTile{bn, w, nt}; }
+    if (sc < bs - 1e-9) { bs = sc; best = HTile{bn, w, nt, TC_ROWS}; }
   };
   if (P.tc_bn == 128) consider(64, P.w_h64);
   if (P.tc_bn == 128 && allow96) consider(96, P.w_h96);   // e.g. 640 channels on 16 row tiles: 112 tiles in one wave
+  const long tall = (long)cdiv(Lv, TC_TALL) * tc_groups(P) * cdiv(P.Cout, best.bn);
+  if (tc5_tall(P, best.bn, tall, sms)) { best.mt = TC_TALL; best.ntiles = tall; }
   return best;
+}
+
+// One launch of tcpair_kernel<BN, MT>; false -- nothing launched -- when it does not fit shared memory.
+static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, cudaStream_t st) {
+  const int BN = P1.tc_bn;
+  tc5_rows(P1, MT);
+  const int span2 = tc5_rows(P2, MT);
+  P2.tc_bn = BN;
+  size_t smem = 0;
+  const long a2bytes = 2L * P2.tc_chunks_h * P2.R * 128;   // c2's hi / lo operand tile, in c1's operand buffers
+  if (!tc5_plan(P1, BN, MT, a2bytes, P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps, smem)) return false;
+  dim3 grid(cdiv(tc_lv(P1), MT - span2), 1, tc_groups(P1));
+  tc5_set_smem_limits();
+  void* rec = profile_begin_pair(P1, P2, st);
+  if (MT == TC_TALL) {
+    if (BN == 64) launch_pdl(tcpair_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+    else launch_pdl(tcpair_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+    profile_count_tall();
+  } else if (BN == 128) launch_pdl(tcpair_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+  else if (BN == 64) launch_pdl(tcpair_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+  else launch_pdl(tcpair_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+  profile_end(rec, st);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+  return true;
 }
 
 // One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))) (c2's epilogue EPI_RES / EPI_ACC), as one launch of
 // tcpair_kernel: c1's output tile stays in shared memory as c2's operand tile, so the intermediate tensor never
-// reaches HBM.  A tile yields 128 - span(c2) output rows (c1 is recomputed on the halo rows of neighbouring tiles).
+// reaches HBM.  A tile yields MT - span(c2) output rows (c1 is recomputed on the halo rows of neighbouring tiles);
+// MT = 256 where tc5_tall allows it, else 128.
 // Returns false -- nothing launched -- when the pair needs more than one co-tile or does not fit shared memory.
 bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (!tcconv_supported(P1) || !P2.w_h) return false;
@@ -707,38 +825,22 @@ bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (P2.tc_bn != BN || P1.Cout > BN || P2.Cin != P1.Cout || P2.Cout > BN || P1.Wreal || P2.Wreal || P1.strips ||
       P1.G != P2.G || P1.L != P2.L || P1.pro != PRO_LRELU || P2.pro != PRO_LRELU || (P2.epi != EPI_RES && P2.epi != EPI_ACC))
     return false;
-  tc5_rows(P1);
-  const int span2 = tc5_rows(P2);
-  P2.tc_bn = BN;
-  size_t smem = 0;
-  const long a2bytes = 2L * P2.tc_chunks_h * P2.R * 128;   // c2's hi / lo operand tile, in c1's operand buffers
-  if (!tc5_plan(P1, BN, a2bytes, P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps, smem)) return false;
-  dim3 grid(cdiv(tc_lv(P1), TC_ROWS - span2), 1, tc_groups(P1));
-  tc5_set_smem_limits();
-  void* rec = profile_begin_pair(P1, P2, st);
-  if (BN == 128) launch_pdl(tcpair_kernel<128>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-  else if (BN == 64) launch_pdl(tcpair_kernel<64>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-  else launch_pdl(tcpair_kernel<32>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-  profile_end(rec, st);
-  count_launch(1);
-  AGPT_CUDA(cudaGetLastError());
-  return true;
+  const int span2 = tc5_rows(P2, TC_TALL);
+  if (tc5_tall(P1, BN, (long)cdiv(tc_lv(P1), TC_TALL - span2) * tc_groups(P1), tc5_sms()) && tcpair_try(P1, P2, TC_TALL, st))
+    return true;
+  return tcpair_try(P1, P2, TC_ROWS, st);
 }
 
 // returns false when the layer has no fp16 image or does not fit the shared-memory budget
 bool tcconv5_launch(TapConvParams P, cudaStream_t st) {
   if (!P.w_h) return false;
-  int dev = 0;
-  AGPT_CUDA(cudaGetDevice(&dev));
-  static int sms_dev[64] = {0};
-  if (!sms_dev[dev & 63]) AGPT_CUDA(cudaDeviceGetAttribute(&sms_dev[dev & 63], cudaDevAttrMultiProcessorCount, dev));
-  const HTile c = pick_h_tile(P, sms_dev[dev & 63]);
-  if (c.bn != P.tc_bn) {
+  const HTile c = pick_h_tile(P, tc5_sms());
+  if (c.bn != P.tc_bn || c.mt != TC_ROWS) {
     TapConvParams Q = P;
     Q.w_h = c.w;
-    if (tcconv5_try(Q, c.bn, st)) return true;
+    if (tcconv5_try(Q, c.bn, c.mt, st)) return true;
   }
-  return tcconv5_try(P, P.tc_bn, st);
+  return tcconv5_try(P, P.tc_bn, TC_ROWS, st);
 }
 
 }  // namespace agpt
