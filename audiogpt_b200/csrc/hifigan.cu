@@ -333,11 +333,13 @@ struct Hifigan : Handle {
   AaFilter aaf;                     // the 12 Kaiser-sinc taps (state-dict buffer)
   int c_last = 0, hop = 1;
   DevBuf melT, buf[6], sbuf;        // sbuf: activated conv input (BigVGAN only)
+  DevBuf plane[6];                  // plane[k]: operand plane of buf[k] (fp16 hi, then lo), HiFi-GAN plane feed only
   DevBuf io_mel, io_wav, io_har;  // staging for the host-buffer entry point
   float* pin_mel = nullptr; float* pin_wav = nullptr; size_t pin_mel_n = 0, pin_wav_n = 0;
   cudaStream_t own_stream = nullptr;
   bool fuse_resblock = true;        // AGPT_FUSE_RESBLOCK=0: every ResBlock1 conv as its own launch
   bool tall_tiles = true;           // AGPT_TALL_TILES=0: 128-row tiles only (TapConvParams::tc_tall)
+  bool plane_feed = true;           // AGPT_PLANE_FEED=0: every tap-GEMM converts its fp32 input itself
 
   ~Hifigan() override {
     if (pin_mel) cudaFreeHost(pin_mel);
@@ -361,6 +363,42 @@ struct Hifigan : Handle {
     const bool big = cfg.activation != 0;          // BigVGAN: anti-aliased snake instead of leaky-relu
     if (big) sbuf.ensure(mx);
     float* S = sbuf.p;
+    // Operand planes (TapConvParams::pi_hi / po_hi): a leaky-ReLU(0.1) tap-GEMM reads its input as a pre-split fp16
+    // hi / lo plane, written once by the epilogue that produced the tensor (or by plane_split where no tap-GEMM did),
+    // instead of converting the fp32 tensor in every tile.  Only tensors of more than 128 channels get a plane: their
+    // consumers (the unfused convs of the first stage, the upsamplers) run several 128-wide co-tiles, each of which
+    // would convert the same rows again, so the plane saves more than the 4 bytes per element its write costs.  The
+    // consumers of narrower tensors (the fused pairs, ups of C <= 128) run one co-tile; there, writing the plane in
+    // the producer's epilogue costs more than the conversion it saves (measured on H100, DESIGN.md section 4).
+    const bool planes = plane_feed && !big && tc_enabled();
+    auto has_plane = [&](int ch) { return planes && ch > 128 && ch % 8 == 0; };
+    size_t mxp = 0;   // elements of the largest tensor with a plane
+    {
+      long Lp = T; int Cp = C0;
+      for (int i = 0; i <= cfg.num_upsamples; ++i) {
+        if (has_plane(Cp)) mxp = std::max(mxp, (size_t)B * Lp * Cp);
+        if (i < cfg.num_upsamples) { Lp *= cfg.upsample_rates[i]; Cp /= 2; }
+      }
+    }
+    if (mxp) for (auto& p : plane) p.ensure(mxp);   // mxp floats = 2 mxp halves: hi [mxp], lo [mxp]
+    auto plane_hi = [&](const float* t) -> __half* {
+      for (int k = 0; k < 6; ++k)
+        if (buf[k].p == t) return reinterpret_cast<__half*>(plane[k].p);
+      throw Error("hifigan: no operand plane for this tensor");
+    };
+    // ch: channels of the tensor (the plane view of a time-grouped launch has the same plane)
+    auto feed = [&](TapConvParams& P, int ch) {                // P reads its input's plane
+      if (!has_plane(ch)) return;
+      P.pi_hi = plane_hi(P.in); P.pi_lo = P.pi_hi + mxp;
+    };
+    auto emit = [&](TapConvParams& P, int ch, bool keep_fp32) {   // P's epilogue writes its output's plane too (or only)
+      if (!has_plane(ch)) return;
+      P.po_hi = plane_hi(P.out); P.po_lo = P.po_hi + mxp; P.po_slope = 0.1f;
+      if (!keep_fp32) P.out = nullptr;
+    };
+    auto split = [&](const float* t, long rows, int ch) {
+      if (has_plane(ch)) plane_split(t, plane_hi(t), plane_hi(t) + mxp, rows * ch, 0.1f, st);
+    };
     auto snake = [&](const float* src, float* dst, long Lr, int Cr, const SnakeW& w) {
       dim3 block(32, 8), grid(cdiv((int)Lr, AA_TT), cdiv(Cr, 32), B);
       aa_snake_kernel<<<grid, block, 0, st>>>(src, dst, w.a.p, w.inv_b.p, (int)Lr, Cr, aaf);
@@ -376,6 +414,7 @@ struct Hifigan : Handle {
       P.tc_tall = tall_tiles;
       tapconv_launch(P, st);
     }
+    split(cur, (long)B * T, C0);   // conv_pre reads the mel, not a plane: its output's plane comes from a split pass
     long L = T; int C = C0;
     const float inv_nk = 1.f / (float)cfg.num_kernels;
     for (int i = 0; i < cfg.num_upsamples; ++i) {
@@ -387,6 +426,8 @@ struct Hifigan : Handle {
         P.out = X; P.out_gstride = L * u * Co; P.out_pitch = u * Co;
         P.pro = big ? PRO_NONE : PRO_LRELU; P.slope = 0.1f; P.epi = EPI_BIAS;   // BigVGAN upsamples x directly (models.py:184-186)
         P.tc_tall = tall_tiles;
+        feed(P, C);
+        if (!har) emit(P, Co, true);   // X is also every first pair's residual
         tapconv_launch(P, st);
       }
       L *= u; C = Co;
@@ -397,6 +438,7 @@ struct Hifigan : Handle {
         nsf_add_kernel<<<grid, block, 0, st>>>(X, har, nc.w.p, nc.b.p, (int)L, C, T * hop, nc.K, nc.st, nc.pad);
         count_launch(1);
         AGPT_CUDA(cudaGetLastError());
+        split(X, (long)B * L, C);   // the plane of X after the excitation add
       }
       const long gs = L * C;
       auto gview = [&](int g) { return (g && L % g == 0) ? g : 1; };   // time-grouped view [L/g][g*C] of the same memory
@@ -416,6 +458,8 @@ struct Hifigan : Handle {
         for (int n = 0; n < nd; ++n) {
           const bool last = (n == nd - 1);
           float* dst = last ? acc : ((n & 1) ? R1 : R0);
+          // dst feeds the next pair, or (the completed MRF sum) the next upsampler; conv_post reads the fp32 sum
+          const bool dst_plane = !last || (j == cfg.num_kernels - 1 && i + 1 < cfg.num_upsamples);
           auto residual_epi = [&](TapConvParams& P) {   // x + conv(...), on the last pair into the MRF accumulator
             P.res = x; P.res_gstride = gs; P.res_pitch = P.in_pitch;
             if (last) { P.epi = EPI_ACC; P.scale = inv_nk; P.accumulate = (j > 0); }
@@ -428,8 +472,10 @@ struct Hifigan : Handle {
             const int gq = gview(rb.g1[n]) == gview(rb.g2[n]) ? gview(rb.g1[n]) : 1;
             TapConvParams P1 = conv(rb.c1[n], rb.c1g[n], gq, rb.dil[n], x, A);
             P1.epi = EPI_BIAS;
+            feed(P1, C);
             TapConvParams P2 = conv(rb.c2[n], rb.c2g[n], gq, 1, A, dst);
             residual_epi(P2);
+            if (dst_plane) emit(P2, C, true);
             if (tcpair_launch(P1, P2, st)) { x = dst; continue; }
           }
           const float* conv_in = x;
@@ -437,6 +483,8 @@ struct Hifigan : Handle {
             if (big) snake(x, S, L, C, rb.act[2 * n]);      // xt = a1(x)   (AMPBlock1.forward, models.py:75-76)
             TapConvParams P = conv(rb.c1[n], rb.c1g[n], gview(rb.g1[n]), rb.dil[n], big ? S : x, A);
             P.epi = EPI_BIAS;
+            feed(P, C);
+            emit(P, C, false);   // A is read only by c2, as a plane
             tapconv_launch(P, st);
             conv_in = A;
           }
@@ -447,6 +495,8 @@ struct Hifigan : Handle {
           TapConvParams P = t1 ? conv(rb.c2[n], rb.c2g[n], gview(rb.g2[n]), 1, conv_in, dst)
                                : conv(rb.c1[n], rb.c1g[n], gview(rb.g1[n]), rb.dil[n], conv_in, dst);
           residual_epi(P);
+          feed(P, C);
+          if (dst_plane) emit(P, C, true);
           tapconv_launch(P, st);
           x = dst;
         }
@@ -484,6 +534,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   h->magic = kMagicHifigan; h->device = device; h->cfg = *cfg;
   { const char* e = getenv("AGPT_FUSE_RESBLOCK"); h->fuse_resblock = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_TALL_TILES"); h->tall_tiles = !(e && e[0] == '0'); }
+  { const char* e = getenv("AGPT_PLANE_FEED"); h->plane_feed = !(e && e[0] == '0'); }
   WeightCursor wc{W, nW};
   { const float* w = wc.next(); const float* b = wc.next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
   h->ups.resize(nu);

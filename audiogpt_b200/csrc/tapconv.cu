@@ -11,6 +11,7 @@ static bool g_prof = false;
 constexpr int PROF_PAIR = 16;   // record epi code of a fused ResBlock pair: 16 + the epilogue of its second conv
 static std::vector<ProfRec> g_recs;
 static long long g_tall = 0;    // recorded launches that ran 256-row tiles (the dump line has no field for it)
+static long long g_plane = 0;   // recorded launches that were plane-fed (likewise)
 
 bool profile_enabled() { return g_prof; }
 
@@ -20,11 +21,14 @@ void profile_enable(int on) {
     for (auto& r : g_recs) { cudaEventDestroy(r.e0); cudaEventDestroy(r.e1); }
     g_recs.clear();
     g_tall = 0;
+    g_plane = 0;
   }
 }
 
 void profile_count_tall() { if (g_prof) ++g_tall; }
 long long profile_tall_launches() { return g_tall; }
+void profile_count_plane() { if (g_prof) ++g_plane; }
+long long profile_plane_launches() { return g_plane; }
 
 // Sums over the records since profile_enable(1): per variant (FMA BN = 128, 64, 32; 3 = wgmma)
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches) {
@@ -248,8 +252,11 @@ void* profile_begin(const TapConvParams& P, bool tc, double bytes_override, cuda
   const double rows = (double)P.G * P.L;
   rec->flops = 2.0 * rows * P.Cin * P.Cout * P.ntaps * (P.flops_scale > 0.f ? P.flops_scale : 1.f);
   const int out_c = (P.epi == EPI_GATE || P.epi == EPI_GEGLU) ? P.Cout / 2 : P.Cout;
+  // an input plane (fp16 hi + lo) moves 4 bytes per element like the fp32 tensor; an output plane adds 4 more, and
+  // a plane-only output (out == nullptr) writes no fp32 tensor
+  const double out_b = (P.out || !P.po_hi ? 1.0 : 0.0) + (P.po_hi ? 1.0 : 0.0);
   rec->bytes = bytes_override > 0 ? bytes_override
-                                  : 4.0 * (rows * P.Cin + rows * out_c + (P.res ? rows * P.Cout : 0.0) +
+                                  : 4.0 * (rows * P.Cin + out_b * rows * out_c + (P.res ? rows * P.Cout : 0.0) +
                                            (P.epi == EPI_ACC && P.accumulate ? rows * P.Cout : 0.0) +
                                            (double)P.ntaps * P.Cin * P.Cout);
   rec->G = P.G; rec->L = P.L; rec->Cin = P.Cin; rec->Cout = P.Cout; rec->ntaps = P.ntaps; rec->epi = P.epi; rec->Wreal = P.Wreal;
@@ -266,7 +273,8 @@ void* profile_begin(const TapConvParams& P, bool tc, double bytes_override, cuda
 void* profile_begin_pair(const TapConvParams& c1, const TapConvParams& c2, cudaStream_t st) {
   if (!g_prof) return nullptr;
   const double rows = (double)c1.G * c1.L;
-  const double bytes = 4.0 * (rows * c1.Cin + 2.0 * rows * c2.Cout + (c2.epi == EPI_ACC && c2.accumulate ? rows * c2.Cout : 0.0) +
+  const double bytes = 4.0 * (rows * c1.Cin + (2.0 + (c2.po_hi ? 1.0 : 0.0)) * rows * c2.Cout +
+                              (c2.epi == EPI_ACC && c2.accumulate ? rows * c2.Cout : 0.0) +
                               (double)c1.ntaps * c1.Cin * c1.Cout + (double)c2.ntaps * c2.Cin * c2.Cout);
   ProfRec* rec = static_cast<ProfRec*>(profile_begin(c2, true, bytes, st));
   rec->flops += 2.0 * rows * c1.Cin * c1.Cout * c1.ntaps * (c1.flops_scale > 0.f ? c1.flops_scale : 1.f);
@@ -288,6 +296,7 @@ void tapconv_launch(TapConvParams P, cudaStream_t st) {
   AGPT_CHECK(P.cin_pad % TC_KC == 0 && P.cout_pad % 4 == 0, "padding");
   AGPT_CHECK(P.epi == EPI_STORE_CF || P.out_pitch % (P.epi == EPI_GATE || P.epi == EPI_GEGLU ? 2 : 4) == 0, "pitch");
   const bool tc = tcconv_supported(P);
+  AGPT_CHECK(tc || (!P.pi_hi && !P.po_hi), "operand planes need the tensor-core tap-GEMM");
   void* rec = profile_begin(P, tc, 0.0, st);
   if (tc) tcconv_launch(P, st);
   else fma_launch(P, st);

@@ -72,6 +72,14 @@ struct TapConvParams {
   // 1: the tensor-core kernels may run 256-row tiles (tc5_tall in tcconv5.cu decides per launch); set by the HiFi-GAN
   // driver.  Kept last: the kernels read the fields above at fixed parameter-bank offsets, which stay as they were.
   int tc_tall;
+  // Operand planes of the leaky-ReLU tap-GEMMs (HiFi-GAN driver; tensor-core kernels only, appended as tc_tall was).
+  // A plane is two fp16 tensors laid out like the fp32 one (same pitch and sample stride, in elements):
+  //   hi = fp16(lrelu(x, slope)),  lo = fp16(lrelu(x, slope) - hi)
+  // bit for bit the operands the kernels' own fp32 transform makes.  pi_*: the input is read from this plane (TMA)
+  // instead of `in`.  po_*: the epilogue also writes the plane of the value it stores (po_slope: the consumer's
+  // slope); with out == nullptr only the plane is written.
+  const __half* pi_hi; const __half* pi_lo;
+  __half* po_hi; __half* po_lo; float po_slope;
 };
 
 __host__ __device__ inline int tc_wv(const TapConvParams& P) { return P.Wreal > 0 ? (P.strips > 0 ? P.strip_w + 2 : P.Wreal + 1) : 0; }
@@ -140,6 +148,10 @@ void* profile_begin_pair(const TapConvParams& c1, const TapConvParams& c2, cudaS
 void profile_end(void* rec, cudaStream_t st);
 void profile_count_tall();            // a tensor-core launch with 256-row tiles (counted while profiling)
 long long profile_tall_launches();
+void profile_count_plane();           // a plane-fed tensor-core launch (counted while profiling)
+long long profile_plane_launches();
+// fp32 [n] -> operand plane hi / lo of lrelu(x, slope) (TapConvParams::pi_hi), n a multiple of 4 (tcconv5.cu)
+void plane_split(const float* x, __half* hi, __half* lo, long n, float slope, cudaStream_t st);
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches);
 long profile_dump(char* out, long cap);
 double fma_peak_tflops();

@@ -4,6 +4,7 @@
 // consuming any of them (memory-level parallelism in the tensor-core epilogue).
 #pragma once
 #include "tapconv.cuh"
+#include "tc_h16.cuh"
 
 namespace agpt {
 
@@ -73,6 +74,19 @@ __device__ __forceinline__ float4 epi_colvec(const TapConvParams& P, int g, int 
   return c;
 }
 
+// operand plane of the 4 stored values (TapConvParams::po_hi): exactly pro_apply5 (leaky ReLU) + split2 of the
+// transform a PRO_LRELU consumer would run on them
+__device__ __forceinline__ void epi_store_plane(const TapConvParams& P, long off, float4 v) {
+  v.x = lrelu(v.x, P.po_slope); v.y = lrelu(v.y, P.po_slope); v.z = lrelu(v.z, P.po_slope); v.w = lrelu(v.w, P.po_slope);
+  uint2 h, l;
+  h.x = split2(v.x, v.y, l.x);
+  h.y = split2(v.z, v.w, l.y);
+  *reinterpret_cast<uint2*>(P.po_hi + off) = h;
+  *reinterpret_cast<uint2*>(P.po_lo + off) = l;
+}
+
+// PL: the plane-fed tensor-core kernels, which may write the output as an operand plane too (or only)
+template <bool PL = false>
 __device__ __forceinline__ void epi_store_cv(const TapConvParams& P, int g, int p, int co, float4 v, const EpiPre& pre,
                                              const float4 cv) {
   if (co >= P.Cout) return;
@@ -149,7 +163,13 @@ __device__ __forceinline__ void epi_store_cv(const TapConvParams& P, int g, int 
     }
     default: break;
   }
-  *reinterpret_cast<float4*>(P.out + g * P.out_gstride + (long)p * P.out_pitch + co) = v;
+  if constexpr (PL) {
+    const long off = g * P.out_gstride + (long)p * P.out_pitch + co;
+    if (P.out) *reinterpret_cast<float4*>(P.out + off) = v;
+    if (P.po_hi) epi_store_plane(P, off, v);
+  } else {
+    *reinterpret_cast<float4*>(P.out + g * P.out_gstride + (long)p * P.out_pitch + co) = v;
+  }
 }
 
 __device__ __forceinline__ void epi_store(const TapConvParams& P, int g, int p, int co, float4 v, const EpiPre& pre) {

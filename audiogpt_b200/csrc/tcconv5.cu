@@ -13,11 +13,13 @@
 // a conv tap = a row-shifted descriptor start address.  Two worker warpgroups convert fp32 activations into the fp16
 // hi/lo tiles, then each issues wgmma for its MT / 2 rows (MT / 128 blocks of 64) with the accumulators in registers
 // (one wgmma group in flight while the next chunk is converted), then runs the fused epilogue; warp 8 streams the
-// weights (cp.async.bulk, mbarrier full/empty ring).
+// weights (cp.async.bulk, mbarrier full/empty ring).  The plane-fed variants (tcconv5_pl_kernel, tcpair_pl_kernel)
+// take the input as pre-split fp16 hi/lo planes: warp 8 also loads them by TMA, and the workers skip the transform.
 #include "tapconv.cuh"
 #include "tapconv_epi.cuh"
 #include "tc_common.cuh"
 #include "tc_h16.cuh"
+#include "tc_tma.cuh"
 #include "models.h"
 
 namespace agpt {
@@ -30,7 +32,9 @@ constexpr int kMaxDyn = 227 * 1024 - 256;   // the kernel also has a small stati
 struct Tc5Smem {
   uint32_t a_hi[MAX_NA], a_lo[MAX_NA], w[MAX_NW], raw[2], rowinfo, rowp, bars, total;
 };
-__host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int MT, int RRA, int NA, int NW, int NR) {
+// pl: a plane-fed tile (the operand buffers' RRA is pl_rows of the tile's rows), which also has the operand buffers'
+// full / empty barriers
+__host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int MT, int RRA, int NA, int NW, int NR, bool pl = false) {
   uint32_t o = 0;
   for (int i = 0; i < MAX_NA; ++i) { s.a_hi[i] = o; if (i < NA) o += RRA * 128; }
   for (int i = 0; i < MAX_NA; ++i) { s.a_lo[i] = o; if (i < NA) o += RRA * 128; }
@@ -40,8 +44,15 @@ __host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int MT, int RRA, 
   s.rowp = o; o += MT * 4;
   o = (o + 15) & ~15u;
   s.bars = o; o += 2 * MAX_NW * 8;
+  if (pl) o += 2 * MAX_NA * 8;
   s.total = o;
 }
+
+// A plane-fed operand chunk arrives as TMA boxes of at most 256 rows (the box limit) and whole 8-row swizzle atoms:
+// pl_box_rows(R) rows each, pl_rows(R) >= R in all; the operand buffers of a plane-fed tile hold pl_rows(R) rows.
+__host__ __device__ inline int pl_boxes(int R) { return (R + 255) / 256; }
+__host__ __device__ inline int pl_box_rows(int R) { const int n = pl_boxes(R); return ((R + n - 1) / n + 7) / 8 * 8; }
+__host__ __device__ inline int pl_rows(int R) { return pl_boxes(R) * pl_box_rows(R); }
 
 constexpr int V5_THREADS = 288;   // 8 worker warps = 2 warpgroups (transform, wgmma, epilogue) + warp 8 (weight producer)
 constexpr int NWK = 256;          // worker threads
@@ -72,19 +83,41 @@ __device__ __forceinline__ int item_row(int xt, int i) { return (xt >> 3) + i * 
 constexpr int TC_TALL = 256;                 // rows of a tall tile (BN <= 64 only: the doubled accumulator still fits)
 constexpr uint64_t BLK_DESC = (64 * 128) >> 4;   // descriptor start-address step from one 64-row block to the next
 
-template <int BN, int MT>
-__global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_constant__ TapConvParams P) {
+// Plane-fed operand chunk c (channels 64 c ..) of rows r0 .. r0 + R - 1 of sample g into operand buffer c % NA, hi
+// and lo planes, completing on a_full; the buffer's previous chunk must have been released on a_empty first.  Rows
+// outside the sample and channels past C load as zeros, which is the conv's zero padding: split(lrelu(0)) = 0.
+__device__ __forceinline__ void pl_load_chunk(uint8_t* smem, const Tc5Smem& S, const CUtensorMap* tmh, const CUtensorMap* tml,
+                                              uint64_t* a_full, uint64_t* a_empty, int NA, int c, int r0, int g, int R) {
+  const int buf = c % NA, nb = pl_boxes(R), br = pl_box_rows(R);
+  if (c >= NA) mbar_wait(&a_empty[buf], (uint32_t)((c / NA - 1) & 1));
+  mbar_arrive_expect_tx(&a_full[buf], 2u * nb * br * 128u);
+  for (int b = 0; b < nb; ++b) {
+    tma_load_3d(smem + S.a_hi[buf] + b * br * 128, tmh, c * H_KCH, r0 + b * br, g, &a_full[buf]);
+    tma_load_3d(smem + S.a_lo[buf] + b * br * 128, tml, c * H_KCH, r0 + b * br, g, &a_full[buf]);
+  }
+}
+
+// PL: plane-fed (TapConvParams::pi_hi): the weight producer also loads each 64-channel chunk of the operand planes
+// straight into the operand buffers with TMA (tmh / tml), so the workers only issue wgmma and run the epilogue; the
+// epilogue may write the output's plane too.  Else the workers convert the fp32 input.
+template <int BN, int MT, bool PL>
+__device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUtensorMap* tmh, const CUtensorMap* tml) {
   constexpr int NB = tc5_nb(BN), NJ = BN / NB, MB = MT / 128;   // MB: 64-row blocks per worker warpgroup
   static_assert(MT == TC_ROWS || (MT == TC_TALL && BN <= 64), "tall tiles are for narrow BN");
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
-  const int RRA = P.R, NA = P.tc_na, NW = P.tc_nw, NR = P.tc_nr;
+  const int RRA = P.R, NA = P.tc_na, NW = P.tc_nw, NR = PL ? 0 : P.tc_nr;
   __shared__ Tc5Smem S;
-  if (threadIdx.x == 0) tc5_layout(S, BN, MT, RRA, NA, NW, NR);
+  if (threadIdx.x == 0) {
+    if constexpr (PL) tc5_layout(S, BN, MT, pl_rows(RRA), NA, NW, 0, true);
+    else tc5_layout(S, BN, MT, RRA, NA, NW, NR);
+  }
   __syncthreads();
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S.bars);
   uint64_t* w_full = bars;                // [MAX_NW]
   uint64_t* w_empty = bars + MAX_NW;      // [MAX_NW]
+  uint64_t* a_full = bars + 2 * MAX_NW;   // [MAX_NA] plane-fed only: operand chunk landed / operand buffer free
+  uint64_t* a_empty = a_full + MAX_NA;
   int* rowinfo = reinterpret_cast<int*>(smem + S.rowinfo);
   int* rowp = reinterpret_cast<int*>(smem + S.rowp);
 
@@ -105,13 +138,16 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
 
   if (tid == 0) {
     for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NWK / 32); }
+    if constexpr (PL)
+      for (int i = 0; i < NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], NWK / 32); }
     fence_barrier_init();
   }
   if (is_worker) {
-    for (int i = xt; i < RRA; i += NWK) {
-      const int r = tc_row_in(P, gz, q0 + lo + i, Wv, Lv);
-      rowinfo[i] = r >= 0 ? r * P.in_pitch : -1;
-    }
+    if constexpr (!PL)
+      for (int i = xt; i < RRA; i += NWK) {
+        const int r = tc_row_in(P, gz, q0 + lo + i, Wv, Lv);
+        rowinfo[i] = r >= 0 ? r * P.in_pitch : -1;
+      }
     if (xt < MT) rowp[xt] = tc_row_out(P, gz, q0 + xt, Wv, Lv);   // output row -> real position (or -1)
   }
   __syncthreads();
@@ -138,8 +174,10 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
       }
       cp_async_commit_();
     };
-    issue_raw(0, 0);
-    if (NR == 2 && nchunks > 1) issue_raw(1, 1);
+    if constexpr (!PL) {
+      issue_raw(0, 0);
+      if (NR == 2 && nchunks > 1) issue_raw(1, 1);
+    }
     {  // pull the epilogue's global operands (residual / old accumulator) into L2 while the main loop runs
       const float* pf0 = nullptr; long gs0 = 0; int pitch0 = 0;
       const float* pf1 = nullptr; long gs1 = 0; int pitch1 = 0;
@@ -175,15 +213,20 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
       const int kv = min(H_KCH, P.Cin - c * H_KCH);
       const int nq = ((kv + 15) >> 4) << 1;                 // 16-byte fp16 chunks (8 channels) the k-steps touch
       const int ksteps = (kv + 15) >> 4;
-      // raw(c) landed?  (with NR == 2 one younger group -- raw(c+1) -- may still be in flight)
-      if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
-      else cp_async_wait_all_();
-      // past this barrier raw(c) is visible to every worker, and the wgmmas that last read a_*[buf] (chunk c - NA) have
-      // completed in both warpgroups: each warpgroup keeps at most one wgmma group in flight, and none across a chunk
-      // boundary when NA == 1
-      named_bar_sync(1, NWK);
+      if constexpr (PL) {
+        mbar_wait(&a_full[buf], (uint32_t)((c / NA) & 1));   // the producer's TMA of chunk c landed
+      } else {
+        // raw(c) landed?  (with NR == 2 one younger group -- raw(c+1) -- may still be in flight)
+        if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
+        else cp_async_wait_all_();
+        // past this barrier raw(c) is visible to every worker, and the wgmmas that last read a_*[buf] (chunk c - NA)
+        // have completed in both warpgroups: each warpgroup keeps at most one wgmma group in flight, and none across a
+        // chunk boundary when NA == 1
+        named_bar_sync(1, NWK);
+      }
       uint8_t* ahi = smem + S.a_hi[buf];
       uint8_t* alo = smem + S.a_lo[buf];
+      if constexpr (!PL) {
       const uint8_t* rawb = smem + S.raw[rb];
 #pragma unroll 2
       for (int idx = xt; idx < items; idx += NWK) {
@@ -208,6 +251,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
       named_bar_sync(1, NWK);            // a_*[buf] complete; everyone finished reading raw[rb]
       const int cn = c + NR;
       if (cn < nchunks) issue_raw(cn, rb);
+      }
       // =========================== worker warps: wgmma over the taps of chunk c ===========================
       // products x_hi w_hi + x_lo w_hi + x_hi w_lo into one fp32 accumulator; a tap is a start address shifted by rows,
       // a row block one shifted by 64 rows more: every block reuses the weight stage, which is released (one group
@@ -244,11 +288,14 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
 #pragma unroll
           for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
         if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        // plane-fed: chunk c - 1's wgmmas have all completed now, so its operand buffer may be refilled
+        if (PL && NA > 1 && t == 0 && c > 0 && lane == 0) mbar_arrive(&a_empty[(c - 1) % NA]);
         prev = s;
       }
       if (NA == 1) {
         wgmma_wait<0>();
         if (lane == 0) mbar_arrive(&w_empty[prev]);
+        if (PL && lane == 0) mbar_arrive(&a_empty[0]);
         prev = -1;
       }
     }
@@ -306,7 +353,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
         const int idx = xt + i * NWK;
         const int row = (idx >> 3) & (MT - 1);   // pp[i] < 0 for i >= nitem (items 4..7 of a tall tile: read below)
         if (pp[i] >= 0)
-          epi_store_cv(P, g, pp[i], co0 + cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
+          epi_store_cv<PL>(P, g, pp[i], co0 + cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
         if (i + 4 < nitem) {
           const int idx4 = idx + 4 * NWK;
           pp[i + 4] = rowp[item_row(xt, i + 4)];
@@ -323,6 +370,8 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
     const uint32_t bytes = 2u * BN * 128u;
     const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(P.w_h) + (size_t)blockIdx.y * (size_t)total * bytes;
     for (int it = 0; it < total; ++it) {
+      if constexpr (PL)   // a chunk's operand tile ahead of its first weight stage
+        if (it % ntaps == 0) pl_load_chunk(smem, S, tmh, tml, a_full, a_empty, NA, it / ntaps, q0 + lo, gz, RRA);
       const int s = it % NW, n = it / NW;
       if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
       mbar_arrive_expect_tx(&w_full[s], bytes);
@@ -331,25 +380,43 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_con
   }
 }
 
+template <int BN, int MT>
+__global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_kernel(const __grid_constant__ TapConvParams P) {
+  tcconv5_body<BN, MT, false>(P, nullptr, nullptr);
+}
+// plane-fed: tmh / tml map the input planes P.pi_hi / P.pi_lo (pl_tensor_maps)
+template <int BN, int MT>
+__global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_pl_kernel(const __grid_constant__ TapConvParams P,
+                                                                  const __grid_constant__ CUtensorMap tmh,
+                                                                  const __grid_constant__ CUtensorMap tml) {
+  tcconv5_body<BN, MT, true>(P, &tmh, &tml);
+}
+
 // One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))), in one CTA per tile (tcpair_launch): the tcconv5 pipeline
 // runs c1 over the MT intermediate rows qa .. qa + MT - 1 (qa = q0 + lowest tap of c2), c1's accumulator becomes c2's
 // operand tile in shared memory, and the tcconv5 pipeline runs c2 over it; a tile keeps the MT - span(c2) outputs
 // that read only those rows.  P1 / P2: the two convs' launch parameters (leaky-ReLU prologue, 1-D rows, one co-tile,
 // BN >= C); P2's epilogue (EPI_RES / EPI_ACC) writes the output.  The weight producer streams c1's stages, then c2's,
 // through one mbarrier ring.
-template <int BN, int MT>
-__global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_constant__ TapConvParams P1,
-                                                               const __grid_constant__ TapConvParams P2) {
+// PL: c1's input is plane-fed (as tcconv5_body), and c2's epilogue may write the output's plane.
+template <int BN, int MT, bool PL>
+__device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapConvParams& P2, const CUtensorMap* tmh,
+                                            const CUtensorMap* tml) {
   constexpr int NB = tc5_nb(BN), NJ = BN / NB, MB = MT / 128;
   static_assert(MT == TC_ROWS || (MT == TC_TALL && BN <= 64), "tall tiles are for narrow BN");
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
-  const int RRA = P1.R, NA = P1.tc_na, NW = P1.tc_nw, NR = P1.tc_nr;
+  const int RRA = P1.R, NA = P1.tc_na, NW = P1.tc_nw, NR = PL ? 0 : P1.tc_nr;
   __shared__ Tc5Smem S;
-  if (threadIdx.x == 0) tc5_layout(S, BN, MT, RRA, NA, NW, NR);
+  if (threadIdx.x == 0) {
+    if constexpr (PL) tc5_layout(S, BN, MT, pl_rows(RRA), NA, NW, 0, true);
+    else tc5_layout(S, BN, MT, RRA, NA, NW, NR);
+  }
   __syncthreads();
   uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
   uint64_t* w_empty = w_full + MAX_NW;
+  uint64_t* a_full = w_full + 2 * MAX_NW;   // [MAX_NA] plane-fed only
+  uint64_t* a_empty = a_full + MAX_NA;
   int* rowinfo = reinterpret_cast<int*>(smem + S.rowinfo);
   int* rowp = reinterpret_cast<int*>(smem + S.rowp);
 
@@ -365,13 +432,16 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
 
   if (tid == 0) {
     for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NWK / 32); }
+    if constexpr (PL)
+      for (int i = 0; i < NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], NWK / 32); }
     fence_barrier_init();
   }
   if (is_worker) {
-    for (int i = xt; i < RRA; i += NWK) {
-      const int r = qa + lo + i;
-      rowinfo[i] = (r >= 0 && r < Lv) ? r * P1.in_pitch : -1;
-    }
+    if constexpr (!PL)
+      for (int i = xt; i < RRA; i += NWK) {
+        const int r = qa + lo + i;
+        rowinfo[i] = (r >= 0 && r < Lv) ? r * P1.in_pitch : -1;
+      }
     if (xt < MT) rowp[xt] = (xt < MT - span2 && q0 + xt < Lv) ? q0 + xt : -1;
   }
   __syncthreads();
@@ -393,8 +463,10 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
       }
       cp_async_commit_();
     };
-    issue_raw(0, 0);
-    if (NR == 2 && nchunks > 1) issue_raw(1, 1);
+    if constexpr (!PL) {
+      issue_raw(0, 0);
+      if (NR == 2 && nchunks > 1) issue_raw(1, 1);
+    }
     {  // the epilogue's residual / old accumulator rows into L2 while the main loop runs
       const int lines = (BN * 4) / 128 > 0 ? (BN * 4) / 128 : 1;
       for (int idx = xt; idx < MT * lines; idx += NWK) {
@@ -415,8 +487,9 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
 #pragma unroll
         for (int i = 0; i < NB / 2; ++i) acc[b][j][i] = 0.f;
     int it = 0, prev = -1;     // prev: weight stage of the newest wgmma group, released once that group has completed
-    // wgmma over the taps of one conv and one 64-channel chunk of its operand tile (ahi0 / alo0: this warpgroup's rows)
-    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {
+    // wgmma over the taps of one conv and one 64-channel chunk of its operand tile (ahi0 / alo0: this warpgroup's rows);
+    // rel >= 0 (plane-fed c1): release that operand buffer once the first tap's group is issued (all older completed)
+    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps, int rel) {
       for (int t = 0; t < Q.ntaps; ++t, ++it) {
         const int s = it % NW;
         mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
@@ -448,6 +521,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
 #pragma unroll
           for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
         if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        if (PL && t == 0 && rel >= 0 && lane == 0) mbar_arrive(&a_empty[rel]);
         prev = s;
       }
     };
@@ -457,11 +531,16 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
       const int rb = (NR == 2) ? (c & 1) : 0;
       const int kv = min(H_KCH, P1.Cin - c * H_KCH);
       const int nq = ((kv + 15) >> 4) << 1;
-      if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
-      else cp_async_wait_all_();
-      named_bar_sync(1, NWK);
+      if constexpr (PL) {
+        mbar_wait(&a_full[buf], (uint32_t)((c / NA) & 1));
+      } else {
+        if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
+        else cp_async_wait_all_();
+        named_bar_sync(1, NWK);
+      }
       uint8_t* ahi = smem + S.a_hi[buf];
       uint8_t* alo = smem + S.a_lo[buf];
+      if constexpr (!PL) {
       const uint8_t* rawb = smem + S.raw[rb];
 #pragma unroll 2
       for (int idx = xt; idx < RRA * 8; idx += NWK) {
@@ -481,11 +560,13 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
       fence_proxy_async();
       named_bar_sync(1, NWK);
       if (c + NR < nchunks) issue_raw(c + NR, rb);
+      }
       mma_taps(P1, smem_u32(ahi) + (uint32_t)(wg * (MT / 2) - lo) * 128u, smem_u32(alo) + (uint32_t)(wg * (MT / 2) - lo) * 128u,
-               (kv + 15) >> 4);
+               (kv + 15) >> 4, (PL && NA > 1 && c > 0) ? (c - 1) % NA : -1);
       if (NA == 1) {
         wgmma_wait<0>();
         if (lane == 0) mbar_arrive(&w_empty[prev]);
+        if (PL && lane == 0) mbar_arrive(&a_empty[0]);
         prev = -1;
       }
     }
@@ -549,7 +630,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
     // =========================== c2: wgmma over the resident tile ===========================
     for (int c = 0; c < nch2; ++c) {
       const uint32_t ahi0 = smem_u32(a2) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * (MT / 2) - P2.lo_al) * 128u;
-      mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, C2 - c * H_KCH) + 15) >> 4);
+      mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, C2 - c * H_KCH) + 15) >> 4, -1);
     }
     // =========================== c2's epilogue (as tcconv5_kernel) ===========================
     EpiPre pre[8];
@@ -597,7 +678,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
         const int idx = xt + i * NWK;
         const int row = (idx >> 3) & (MT - 1);
         if (pp[i] >= 0)
-          epi_store_cv(P2, g, pp[i], cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
+          epi_store_cv<PL>(P2, g, pp[i], cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
         if (i + 4 < nitem) {
           const int idx4 = idx + 4 * NWK;
           pp[i + 4] = rowp[item_row(xt, i + 4)];
@@ -611,6 +692,8 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
     const uint32_t bytes = 2u * BN * 128u;
     const int total2 = P2.tc_chunks_h * P2.ntaps;
     for (int it = 0; it < total + total2; ++it) {
+      if constexpr (PL)   // c1's operand chunks ahead of their first weight stage
+        if (it < total && it % P1.ntaps == 0) pl_load_chunk(smem, S, tmh, tml, a_full, a_empty, NA, it / P1.ntaps, qa + lo, g, RRA);
       const int s = it % NW, n = it / NW;
       if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
       mbar_arrive_expect_tx(&w_full[s], bytes);
@@ -619,6 +702,19 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
       bulk_g2s(smem + S.w[s], src, bytes, &w_full[s]);
     }
   }
+}
+
+template <int BN, int MT>
+__global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_constant__ TapConvParams P1,
+                                                               const __grid_constant__ TapConvParams P2) {
+  tcpair_body<BN, MT, false>(P1, P2, nullptr, nullptr);
+}
+template <int BN, int MT>
+__global__ void __launch_bounds__(V5_THREADS, 1) tcpair_pl_kernel(const __grid_constant__ TapConvParams P1,
+                                                                 const __grid_constant__ TapConvParams P2,
+                                                                 const __grid_constant__ CUtensorMap tmh,
+                                                                 const __grid_constant__ CUtensorMap tml) {
+  tcpair_body<BN, MT, true>(P1, P2, &tmh, &tml);
 }
 
 // fp16 hi/lo weight image: [co-tile][chunk64][tap][hi | lo][BN rows x 128 B, SWIZZLE_128B], pre-scaled
@@ -651,7 +747,32 @@ void build_h_image(const PackedConv& pc, const std::vector<float>& h, int BN, fl
   dst.upload(packed);
 }
 
+// fp32 tensor -> operand plane (TapConvParams::pi_hi), for inputs of plane-fed launches that no tap-GEMM epilogue
+// wrote: the same lrelu + split2 as the fp32 transform and epi_store_plane, 4 elements per thread
+__global__ void plane_split_kernel(const float4* __restrict__ x, uint2* __restrict__ hi, uint2* __restrict__ lo, long n4,
+                                  float slope) {
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += (long)gridDim.x * blockDim.x) {
+    float4 v = x[i];
+    v.x = lrelu(v.x, slope); v.y = lrelu(v.y, slope); v.z = lrelu(v.z, slope); v.w = lrelu(v.w, slope);
+    uint2 h, l;
+    h.x = split2(v.x, v.y, l.x);
+    h.y = split2(v.z, v.w, l.y);
+    hi[i] = h;
+    lo[i] = l;
+  }
+}
+
 }  // namespace
+
+void plane_split(const float* x, __half* hi, __half* lo, long n, float slope, cudaStream_t st) {
+  AGPT_CHECK(n % 4 == 0, "plane_split: element count must be a multiple of 4");
+  const long n4 = n / 4;
+  const int blocks = (int)std::min<long>(cdivl(n4, 256), 132L * 16);
+  plane_split_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const float4*>(x), reinterpret_cast<uint2*>(hi),
+                                             reinterpret_cast<uint2*>(lo), n4, slope);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+}
 
 void pack_h_weights(PackedConv& pc, const std::vector<float>& h) {
   float mx = 0.f;
@@ -680,18 +801,23 @@ static int tc5_rows(TapConvParams& P, int MT) {
 
 // Shared-memory plan of a BN x MT tile (operand, raw-staging and weight-ring buffers) for P after tc5_rows; false when
 // it does not fit.  a_min: bytes the operand buffers must span at least; iters: weight stages the kernel streams.
+// A plane-fed tile (P.pi_hi) has no raw staging; its operand buffers hold pl_rows(R) rows, and it keeps up to every
+// chunk of the operand resident (TMA loads run ahead of the wgmmas), as long as a 4-stage weight ring still fits.
 static bool tc5_plan(TapConvParams& P, int BN, int MT, long a_min, int iters, size_t& smem) {
   const int RRA = P.R;
+  const bool pl = P.pi_hi != nullptr;
   P.tc_bn = BN;
   const long avail = (long)kMaxDyn - 1024 /*align*/ - (RRA * 4 + MT * 4 + 512) /*row tables + barriers*/;
-  const long abytes = 2L * RRA * 128, wbytes = 2L * BN * 128;
+  const long abytes = 2L * (pl ? pl_rows(RRA) : RRA) * 128, wbytes = 2L * BN * 128;
   const long rbytes = (long)RRA * 256;
   const long stg = 2L * MT * 128;   // the epilogue stages 2 x [MT][32] fp32 through the operand buffers
   const int nch = P.tc_chunks_h;
-  int NA = (P.ntaps == 1) ? 3 : 2;
+  int NA = pl ? MAX_NA : ((P.ntaps == 1) ? 3 : 2);
   NA = std::max(1, std::min(NA, nch));
   if ((long)NA * abytes < stg) NA = (int)cdiv(stg, abytes);
-  int NR = (nch > 1) ? 2 : 1;
+  int NR = pl ? 0 : ((nch > 1) ? 2 : 1);
+  auto fits4 = [&](int na) { return na * abytes + 4 * wbytes <= avail; };
+  while (pl && NA > 2 && !fits4(NA) && (NA - 1) * abytes >= stg) --NA;
   auto fits = [&](int na, int nr, int nw) { return na * abytes + nr * rbytes + nw * wbytes <= avail; };
   if (!fits(NA, NR, 2) && NA == 3) NA = 2;
   if (!fits(NA, NR, 2) && NR == 2) NR = 1;
@@ -705,7 +831,7 @@ static bool tc5_plan(TapConvParams& P, int BN, int MT, long a_min, int iters, si
   NW = std::max(2, std::min(NW, std::max(2, iters)));
   P.tc_na = NA; P.tc_nw = NW; P.tc_nr = NR;
   Tc5Smem S;
-  tc5_layout(S, BN, MT, RRA, NA, NW, NR);
+  tc5_layout(S, BN, MT, pl ? pl_rows(RRA) : RRA, NA, NW, NR, pl);
   smem = (size_t)S.total + 1024;
   return smem <= (size_t)kMaxDyn;
 }
@@ -726,6 +852,17 @@ static void tc5_set_smem_limits() {
   AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
   AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
   AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<96, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
   attr_done_dev[dev & 63] = true;
 }
 
@@ -745,6 +882,18 @@ static bool tc5_tall(const TapConvParams& P, int bn, long tall_tiles, int sms) {
   return P.tc_tall && bn <= 64 && !P.Wreal && !P.strips && tall_tiles >= 4L * sms;
 }
 
+// Tensor maps of P's input planes (P.pi_hi / pi_lo) for boxes of 64 channels x pl_box_rows(P.R) rows (after tc5_rows)
+struct PlMaps { CUtensorMap hi, lo; };
+static PlMaps pl_tensor_maps(const TapConvParams& P) {
+  AGPT_CHECK(!P.Wreal && !P.strips, "plane-fed tap-GEMMs run over plain 1-D rows");
+  PlMaps m;
+  const int br = pl_box_rows(P.R);
+  AGPT_CHECK(tma_encode_rows_h(&m.hi, P.pi_hi, P.Cin, P.L, P.G, P.in_pitch, P.in_gstride, br) &&
+                 tma_encode_rows_h(&m.lo, P.pi_lo, P.Cin, P.L, P.G, P.in_pitch, P.in_gstride, br),
+             "cannot encode the operand-plane tensor maps");
+  return m;
+}
+
 // Try one tile shape; returns false when it does not fit the shared-memory budget.
 static bool tcconv5_try(TapConvParams P, int BN, int MT, cudaStream_t st) {
   tc5_rows(P, MT);
@@ -753,6 +902,19 @@ static bool tcconv5_try(TapConvParams P, int BN, int MT, cudaStream_t st) {
   const int Lv = tc_lv(P);
   dim3 grid(cdiv(Lv, MT), cdiv(P.Cout, BN), tc_groups(P));
   tc5_set_smem_limits();
+  if (P.pi_hi) {
+    const PlMaps m = pl_tensor_maps(P);
+    if (MT == TC_TALL) {
+      if (BN == 64) launch_pdl(tcconv5_pl_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
+      else launch_pdl(tcconv5_pl_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
+      profile_count_tall();
+    } else if (BN == 128) launch_pdl(tcconv5_pl_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
+    else if (BN == 96) launch_pdl(tcconv5_pl_kernel<96, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
+    else if (BN == 64) launch_pdl(tcconv5_pl_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
+    else launch_pdl(tcconv5_pl_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
+    profile_count_plane();
+    return true;
+  }
   if (MT == TC_TALL) {
     if (BN == 64) launch_pdl(tcconv5_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P);
     else launch_pdl(tcconv5_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P);
@@ -801,7 +963,17 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, cudaStream_t 
   dim3 grid(cdiv(tc_lv(P1), MT - span2), 1, tc_groups(P1));
   tc5_set_smem_limits();
   void* rec = profile_begin_pair(P1, P2, st);
-  if (MT == TC_TALL) {
+  if (P1.pi_hi) {
+    const PlMaps m = pl_tensor_maps(P1);
+    if (MT == TC_TALL) {
+      if (BN == 64) launch_pdl(tcpair_pl_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
+      else launch_pdl(tcpair_pl_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
+      profile_count_tall();
+    } else if (BN == 128) launch_pdl(tcpair_pl_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
+    else if (BN == 64) launch_pdl(tcpair_pl_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
+    else launch_pdl(tcpair_pl_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
+    profile_count_plane();
+  } else if (MT == TC_TALL) {
     if (BN == 64) launch_pdl(tcpair_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2);
     else launch_pdl(tcpair_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2);
     profile_count_tall();

@@ -37,6 +37,8 @@ int agpt_profile_enable(int on);
 int agpt_profile_collect(double ms[4], double flops[4], double bytes[4], long long launches[4]);
 /* recorded wgmma launches that ran 256-row tiles (narrow HiFi-GAN / BigVGAN convs) since profiling was enabled */
 long long agpt_profile_tall_launches(void);
+/* recorded wgmma launches whose input was a pre-split fp16 operand plane (HiFi-GAN) since profiling was enabled */
+long long agpt_profile_plane_launches(void);
 /* dev tooling: one text line per recorded launch ("variant G L Cin Cout ntaps span epi Wreal ms flops"); returns bytes written or -1 */
 long agpt_profile_dump(char* out, long cap);
 double agpt_fma_peak_tflops(void);
