@@ -46,7 +46,7 @@ _FIRST_STAGE_MAP = {
 }
 
 
-def install(strict: bool = False, front_end: bool = False, first_stage: bool = False):
+def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -61,6 +61,9 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     ``first_stage=True`` also replaces ``ldm.models.autoencoder.AutoencoderKL`` by AutoencoderKLWithEncoder, so
     every Make-An-Audio tool encodes and decodes its first stage on the engine, and records the reference's
     DiagonalGaussianDistribution as the class its encode() returns.
+    ``inpaint=True`` also makes ``UNetModel(...)`` build AttentionUNetModel for the AttentionBlock configs it covers
+    (the Inpaint tool's denoiser) instead of the reference's class, so with ``first_stage=True`` the whole Inpaint
+    chain runs on the engine.
     Returns the list of patched names."""
     import importlib
     import sys
@@ -93,6 +96,10 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
                 mine._reference_cls = theirs
             setattr(ref, a, mine)
         patched.append(ref_name)
+    if inpaint:
+        from .ldm.modules.diffusionmodules.openaimodel import AttentionUNetModel, UNetModel
+        UNetModel._attention_cls = AttentionUNetModel
+        patched.append("ldm.modules.diffusionmodules.openaimodel (AttentionBlock UNets)")
     if first_stage:
         # get_first_stage_encoding checks isinstance(posterior, DiagonalGaussianDistribution) against the reference's
         # own class (ddpm_audio.py:157-164): encode() must build that class when it exists

@@ -46,7 +46,8 @@ class UnetCfg(C.Structure):
                 ("channel_mult", C.c_int * AGPT_MAX_LEVELS),
                 ("attn_at_level", C.c_int * AGPT_MAX_LEVELS),
                 ("num_heads", C.c_int), ("num_head_channels", C.c_int),
-                ("transformer_depth", C.c_int), ("context_dim", C.c_int)]
+                ("transformer_depth", C.c_int), ("context_dim", C.c_int),
+                ("use_spatial_transformer", C.c_int), ("resblock_updown", C.c_int), ("attention_order", C.c_int)]
 
 
 class VaeCfg(C.Structure):
@@ -102,6 +103,7 @@ PROTOTYPES = {
     "agpt_axpby5": (_I, [_P, _P, _P, _P, _P, _P, _I, _L, _P, _P]),
     "agpt_unet_create": (_I, [C.POINTER(UnetCfg), _W, _I, _I, _OUT]),
     "agpt_unet_set_context": (_I, [_P, _P, _I, _I, _P]),
+    "agpt_unet_set_concat": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "agpt_unet_forward": (_I, [_P, _P, _P, _I, _I, _I, _P, _P]),
     "agpt_ddim_update": (_I, [_P, _P, _I, _F, _F, _F, _F, _F, _P, _F, _I, _L, _P, _P, _P]),
     "agpt_unet_ddim_sample": (_I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _P, _P, _P]),

@@ -181,6 +181,13 @@ int agpt_unet_set_context(agpt_handle h, const float* context, int N, int S, voi
   });
 }
 
+int agpt_unet_set_concat(agpt_handle h, const float* c, int N, int C, int H, int W, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(c, "null conditioning");
+    unet_set_concat(as(h, kMagicUnet, "unet"), c, N, C, H, W, (cudaStream_t)stream);
+  });
+}
+
 int agpt_unet_forward(agpt_handle h, const float* x, const int* t_host, int N, int H, int W, float* eps, void* stream) {
   return guarded([&] {
     AGPT_CHECK(x && t_host && eps, "null argument");

@@ -32,6 +32,7 @@ void axpby5(const float* x, const float* e0, const float* e1, const float* e2, c
 
 Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int device);
 void unet_set_context(Handle* h, const float* ctx, int N, int S, cudaStream_t st);
+void unet_set_concat(Handle* h, const float* c, int N, int C, int H, int W, cudaStream_t st);
 void unet_forward(Handle* h, const float* x, const int* t_host, int N, int H, int W, float* eps, cudaStream_t st);
 void unet_ddim_sample(Handle* h, const float* x_T, int B, int H, int W, int S, const int* t_steps,
                       const float* a_t, const float* a_prev, const float* sigma, const float* sqrt_om,

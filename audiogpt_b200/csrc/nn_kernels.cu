@@ -478,6 +478,34 @@ void upsample_nearest2(const float* in, float* out, int N, int H, int W, int C, 
   AGPT_CUDA(cudaGetLastError());
 }
 
+// 2x2 average pool with stride 2 and floor (the ResBlock down path's AvgPool2d(2, 2), openaimodel.py:134-160):
+// out[n][ho][wo][C] = (x[2ho][2wo] + x[2ho][2wo+1] + x[2ho+1][2wo] + x[2ho+1][2wo+1]) / 4, summed in that order
+__global__ void avgpool2_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int H, int W, int C) {
+  pdl_wait();
+  const int Ho = H / 2, Wo = W / 2;
+  const long total = (long)N * Ho * Wo * (C / 4);
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % (C / 4)) * 4;
+    long r = i / (C / 4);
+    const int wo = (int)(r % Wo); r /= Wo;
+    const int ho = (int)(r % Ho);
+    const int n = (int)(r / Ho);
+    const float* p = in + (((long)n * H + 2 * ho) * W + 2 * wo) * C + c;
+    const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + C);
+    const float4 d = *reinterpret_cast<const float4*>(p + (long)W * C), e = *reinterpret_cast<const float4*>(p + (long)W * C + C);
+    *reinterpret_cast<float4*>(out + (((long)n * Ho + ho) * Wo + wo) * C + c) =
+        make_float4((a.x + b.x + d.x + e.x) / 4.f, (a.y + b.y + d.y + e.y) / 4.f, (a.z + b.z + d.z + e.z) / 4.f,
+                    (a.w + b.w + d.w + e.w) / 4.f);
+  }
+}
+void avgpool2(const float* in, float* out, int N, int H, int W, int C, cudaStream_t st) {
+  AGPT_CHECK(C % 4 == 0 && H >= 2 && W >= 2, "avgpool2: channels must be a multiple of 4 and the map at least 2x2");
+  const long total = (long)N * (H / 2) * (W / 2) * (C / 4);
+  launch_pdl(avgpool2_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, in, out, N, H, W, C);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+}
+
 // im2col for a 3x3 stride-2 Conv2d: col[n][ho][wo][tap*C + c] = x[n][2ho+kh-pad][2wo+kw-pad][c], zero outside x.
 // pad 1: the UNet's Conv2d(k3, stride 2, padding 1); pad 0: the VAE encoder's Downsample, F.pad(x, (0,1,0,1)) then a
 // conv without padding -- the one zero row / column past the end is the same out-of-range read

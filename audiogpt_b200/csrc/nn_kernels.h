@@ -27,6 +27,8 @@ bool attention_tc_enabled();   // 1 (default) wgmma kernel, 0 fp32 kernel, -1 en
 void timestep_embedding(float* out, const int* t_host, int N, int dim, cudaStream_t st);
 void concat_channels(const float* a, int Ca, const float* b, int Cb, float* out, long rows, cudaStream_t st);
 void upsample_nearest2(const float* in, float* out, int N, int H, int W, int C, cudaStream_t st);
+// 2x2 average pool, stride 2, floor: out [N][H/2][W/2][C]  (AvgPool2d(2, 2))
+void avgpool2(const float* in, float* out, int N, int H, int W, int C, cudaStream_t st);
 // pad: rows / columns of zeros before the image (1: Conv2d padding=1; 0: the encoder's Downsample, pad after only)
 void im2col_stride2(const float* in, float* col, int N, int H, int W, int C, int Ho, int Wo, int pad, cudaStream_t st);
 void cf_to_cl_pad(const float* in, float* out, int N, int C, int Cpad, int HW, cudaStream_t st, int Nsrc = 0);

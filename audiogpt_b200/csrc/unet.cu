@@ -1,6 +1,7 @@
-// Make-An-Audio UNet (ResBlock + SpatialTransformer) and the DDIM loop on sm_90a.
+// Make-An-Audio UNet (ResBlock + SpatialTransformer or AttentionBlock) and the DDIM loop on sm_90a.
 // Reference: ldm/modules/diffusionmodules/openaimodel.py:443-744 (ctor + forward),
-//            :255-275 (ResBlock._forward), :91-160 (Up/Downsample);
+//            :255-275 (ResBlock._forward, with the up/down variants), :91-160 (Up/Downsample),
+//            :278-406 (AttentionBlock, QKVAttentionLegacy / QKVAttention);
 //            ldm/modules/attention.py:37-64,152-261; ldm/models/diffusion/ddim.py:117-225.
 // Activations are channels-last token rows [N][H*W][C]; every contraction is a tapconv.
 // Parity: tests/test_ldm_gpu.py against oracle/ldm_ref.py and tests/golden/ldm_*.npz.
@@ -17,6 +18,14 @@ struct ResW {
   PackedConv conv1, conv2, skip;
   bool has_skip = false;
   int emb_off = 0;  // channel offset inside the batched emb projection
+  int updown = 0;   // resblock_updown: 1 down (2x2 average pool), 2 up (nearest x2), applied to h after GN+SiLU and to x
+};
+
+// AttentionBlock: GN (no SiLU) -> qkv 1x1 -> self-attention over H*W tokens -> proj_out 1x1 + x
+struct AttnW {
+  int ch = 0, heads = 0, dhead = 0;
+  DevBuf gn_g, gn_b;
+  PackedConv qkv, proj_out;   // qkv rows in [Q | K | V] order, heads outermost inside each
 };
 
 struct XfBlockW {
@@ -32,10 +41,10 @@ struct StW {
   std::vector<XfBlockW> blocks;
 };
 
-enum LayerKind { L_CONV_IN, L_RES, L_ST, L_DOWN, L_UP };
+enum LayerKind { L_CONV_IN, L_RES, L_ST, L_ATTN, L_DOWN, L_UP };
 struct Layer {
   LayerKind kind;
-  int idx;   // index into res / st / misc conv vectors
+  int idx;   // index into res / st / attn / misc conv vectors
   int ch;    // channels (down/up)
 };
 struct Block { std::vector<Layer> layers; };
@@ -49,6 +58,7 @@ struct Unet : Handle {
   DevBuf out_w9c4, out_b4;      // the `out` conv as [9][C][4] fp32 for the fused conv_out + CFG + DDIM-update kernel
   std::vector<ResW> res;
   std::vector<StW> st;
+  std::vector<AttnW> attn;
   std::vector<Block> in_blocks, out_blocks;
   Block mid;
   int emb_total = 0, kv_total = 0, cin_pad = 0;
@@ -56,6 +66,8 @@ struct Unet : Handle {
   // per-call state
   int ctxN = 0, ctxS = 0;
   DevBuf ctx_kv;                // hoisted cross-attention K / V of the context
+  int catN = 0, catH = 0, catW = 0;
+  DevBuf cat_cl;                // concat conditioning [N][H*W][cin_pad - out_channels], zero-padded channels
   DevBuf arena;
   size_t arena_off = 0, arena_cap = 0;
   DevBuf ddim_eps, ddim_x, ddim_p0;
@@ -64,7 +76,11 @@ struct Unet : Handle {
   int emb_gstride = 0;            // row stride of the per-sample ResBlock embedding vectors (0: all samples share one row)
   cudaGraphExec_t step_graph = nullptr;
   cudaStream_t cap_stream = nullptr;
-  struct GraphKey { int N = 0, H = 0, W = 0, single = 0; const void *arena = nullptr, *ctx = nullptr, *x = nullptr; int ctxS = 0; } gkey;
+  struct GraphKey {
+    int N = 0, H = 0, W = 0, single = 0;
+    const void *arena = nullptr, *ctx = nullptr, *x = nullptr, *cat = nullptr;
+    int ctxS = 0;
+  } gkey;
   long launches_per_step = 0;
 
   ~Unet() override {
@@ -90,6 +106,17 @@ struct Unet : Handle {
     tapconv_launch(P, s);
   }
 
+  // the step-invariant conditioning channels of the concat loop, in the kernel layout once per sampling call
+  void set_concat(const float* c, int N, int C, int H, int W, cudaStream_t s) {
+    const int oc = cfg.out_channels;
+    AGPT_CHECK(C == cfg.in_channels - oc && C >= 1, "concat conditioning must have in_channels - out_channels channels");
+    AGPT_CHECK(oc % 4 == 0, "concat conditioning needs out_channels to be a multiple of 4");
+    AGPT_CHECK(N >= 1 && H >= 1 && W >= 1, "empty concat conditioning");
+    cat_cl.ensure((size_t)N * H * W * (cin_pad - oc));
+    cf_to_cl_pad(c, cat_cl.p, N, C, cin_pad - oc, H * W, s);
+    catN = N; catH = H; catW = W;
+  }
+
   // ---- building blocks --------------------------------------------------------------
   void conv3x3(const PackedConv& pc, const float* in, float* out, int N, int H, int W, int epi,
                const float* res_, const float* evec, int evec_stride, cudaStream_t s) {
@@ -111,10 +138,20 @@ struct Unet : Handle {
     tapconv_launch(P, s);
   }
 
-  float* run_res(const ResW& r, const float* x, const float* emb_out, int N, int H, int W, cudaStream_t s) {
+  // H / W are updated to the output resolution of an up / down ResBlock
+  float* run_res(const ResW& r, const float* x, const float* emb_out, int N, int& H, int& W, cudaStream_t s) {
+    float* h1 = alloc((size_t)N * H * W * r.cin);
+    groupnorm(x, h1, r.gn1_g.p, r.gn1_b.p, N, H * W, r.cin, 32, 1e-5f, true, nullptr, s);
+    if (r.updown) {   // openaimodel.py:256-261: h_upd(in_rest(x)), x_upd(x), then in_conv at the new resolution
+      const bool down = r.updown == 1;
+      const int Ho = down ? H / 2 : 2 * H, Wo = down ? W / 2 : 2 * W;
+      float* hr = alloc((size_t)N * Ho * Wo * r.cin);
+      float* xr = alloc((size_t)N * Ho * Wo * r.cin);
+      if (down) { avgpool2(h1, hr, N, H, W, r.cin, s); avgpool2(x, xr, N, H, W, r.cin, s); }
+      else { upsample_nearest2(h1, hr, N, H, W, r.cin, s); upsample_nearest2(x, xr, N, H, W, r.cin, s); }
+      h1 = hr; x = xr; H = Ho; W = Wo;
+    }
     const int HW = H * W;
-    float* h1 = alloc((size_t)N * HW * r.cin);
-    groupnorm(x, h1, r.gn1_g.p, r.gn1_b.p, N, HW, r.cin, 32, 1e-5f, true, nullptr, s);
     float* h2 = alloc((size_t)N * HW * r.cout);
     conv3x3(r.conv1, h1, h2, N, H, W, EPI_ADDVEC, nullptr, emb_out + r.emb_off, emb_gstride, s);
     float* h3 = alloc((size_t)N * HW * r.cout);
@@ -169,6 +206,21 @@ struct Unet : Handle {
     return out;
   }
 
+  // AttentionBlock._forward (openaimodel.py:318-324); the d^-1/4 scale of q and of k is applied once as d^-1/2
+  float* run_attn(const AttnW& a, const float* x, int N, int H, int W, cudaStream_t s) {
+    const int HW = H * W, C = a.ch;
+    const long rows = (long)N * HW;
+    float* xn = alloc(rows * C);
+    groupnorm(x, xn, a.gn_g.p, a.gn_b.p, N, HW, C, 32, 1e-5f, false, nullptr, s);
+    float* qkv = alloc(rows * 3 * C);
+    linear(a.qkv, xn, C, qkv, 3 * C, rows, EPI_BIAS, nullptr, 0, s);
+    float* att = alloc(rows * C);
+    attention(qkv, 3 * C, qkv + C, 3 * C, qkv + 2 * C, 3 * C, att, C, N, a.heads, a.dhead, HW, HW, s);
+    float* out = alloc(rows * C);
+    linear(a.proj_out, att, C, out, C, rows, EPI_RES, x, C, s);
+    return out;
+  }
+
   struct Act { float* p; int C, H, W; };
 
   Act run_block(const Block& blk, Act a, const float* emb_out, int N, cudaStream_t s) {
@@ -183,11 +235,16 @@ struct Unet : Handle {
         case L_RES: {
           const ResW& r = res[l.idx];
           AGPT_CHECK(a.C == r.cin, "ResBlock input channels");
-          a = {run_res(r, a.p, emb_out, N, a.H, a.W, s), r.cout, a.H, a.W};
+          int H = a.H, W = a.W;
+          float* o = run_res(r, a.p, emb_out, N, H, W, s);
+          a = {o, r.cout, H, W};
           break;
         }
         case L_ST:
           a = {run_st(st[l.idx], a.p, N, a.H, a.W, s), a.C, a.H, a.W};
+          break;
+        case L_ATTN:
+          a = {run_attn(attn[l.idx], a.p, N, a.H, a.W, s), a.C, a.H, a.W};
           break;
         case L_DOWN: {
           const int Ho = (a.H - 1) / 2 + 1, Wo = (a.W - 1) / 2 + 1;
@@ -242,9 +299,18 @@ struct Unet : Handle {
   // everything after the embedding: x [Nsrc][C][H][W] (sample n reads n % Nsrc) -> eps [N][Cout][H][W]
   // eps == nullptr selects the FUSED tail of the sampling loop: out-conv + guidance + DDIM update in one kernel
   // (conv_out_ddim: x_io = ddim_x updated in place, coefficients from coef_table[*step_ctr])
-  void forward_core(const float* x, int Nsrc, const float* emb_out, int N, int H, int W, float* eps, cudaStream_t s) {
+  // cat != nullptr: x holds only the out_channels latent; the conditioning channels come from cat [N][H*W][..]
+  void forward_core(const float* x, int Nsrc, const float* emb_out, int N, int H, int W, float* eps, cudaStream_t s,
+                    const float* cat = nullptr) {
     float* x_cl = alloc((size_t)N * H * W * cin_pad);
-    cf_to_cl_pad(x, x_cl, N, cfg.in_channels, cin_pad, H * W, s, Nsrc);
+    if (cat) {
+      const int oc = cfg.out_channels;
+      float* lat = alloc((size_t)N * H * W * oc);
+      cf_to_cl_pad(x, lat, N, oc, oc, H * W, s, Nsrc);
+      concat_channels(lat, oc, cat, cin_pad - oc, x_cl, (long)N * H * W, s);
+    } else {
+      cf_to_cl_pad(x, x_cl, N, cfg.in_channels, cin_pad, H * W, s, Nsrc);
+    }
     Act a{x_cl, cin_pad, H, W};
     std::vector<Act> hs;
     for (const Block& b : in_blocks) { a = run_block(b, a, emb_out, N, s); hs.push_back(a); }
@@ -285,7 +351,7 @@ struct Unet : Handle {
 
   // One DDIM step of the on-device loop: everything step-dependent comes from device tables indexed by step_ctr,
   // so the launch sequence is identical for every step (capturable once, replayed S - 1 times).
-  void ddim_step(int B, int N, int H, int W, long n, cudaStream_t s) {
+  void ddim_step(int B, int N, int H, int W, long n, const float* cat, cudaStream_t s) {
     arena_off = 0;
     int* ctr = reinterpret_cast<int*>(step_ctr.p);
     select_row(emb_table.p, ctr, emb_cur.p, emb_total, s);
@@ -293,9 +359,9 @@ struct Unet : Handle {
     static int fuse_tail = -1;
     if (fuse_tail < 0) { const char* e = getenv("AGPT_FUSE_DDIM"); fuse_tail = (e && e[0] == '0') ? 0 : 1; }
     if (fuse_tail && out_w9c4.p) {
-      forward_core(ddim_x.p, B, emb_cur.p, N, H, W, nullptr, s);      // ... -> GN -> [out conv + CFG + x_prev update]
+      forward_core(ddim_x.p, B, emb_cur.p, N, H, W, nullptr, s, cat);      // ... -> GN -> [out conv + CFG + x_prev update]
     } else {
-      forward_core(ddim_x.p, B, emb_cur.p, N, H, W, ddim_eps.p, s);
+      forward_core(ddim_x.p, B, emb_cur.p, N, H, W, ddim_eps.p, s, cat);
       ddim_update_tab(ddim_x.p, ddim_eps.p, N == B ? 1 : 0, coef_table.p, ctr, B, n, ddim_x.p, ddim_p0.p, s);
     }
     step_inc(ctr, s);
@@ -323,10 +389,10 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
     else { nh = ch / cfg->num_head_channels; dh = cfg->num_head_channels; }
   };
 
-  auto make_res = [&](int cin, int cout) -> int {
+  auto make_res = [&](int cin, int cout, int updown = 0) -> int {
     u->res.emplace_back();
     ResW& r = u->res.back();
-    r.cin = cin; r.cout = cout;
+    r.cin = cin; r.cout = cout; r.updown = updown;
     AGPT_CHECK(cin % 32 == 0 && cout % 32 == 0, "ResBlock channels must be multiples of 32");
     { auto g = wc.next(); auto b = wc.next(); r.gn1_g.upload(g, cin); r.gn1_b.upload(b, cin); }
     { auto w = wc.next(); auto b = wc.next(); pack_conv(r.conv1, w, b, cout, cin, 9, true); }
@@ -376,6 +442,38 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
     return (int)u->st.size() - 1;
   };
 
+  auto make_attn = [&](int ch) -> int {
+    u->attn.emplace_back();
+    AttnW& a = u->attn.back();
+    a.ch = ch; heads_for(ch, a.heads, a.dhead);
+    AGPT_CHECK(a.heads >= 1 && a.heads * a.dhead == ch, "AttentionBlock channels must split evenly into heads");
+    { auto g = wc.next(); auto b = wc.next(); a.gn_g.upload(g, ch); a.gn_b.upload(b, ch); }
+    {
+      auto w = wc.next(); auto b = wc.next();   // qkv: Conv1d [3C][C][1] + bias
+      if (cfg->attention_order == 1) {
+        pack_conv(a.qkv, w, b, 3 * ch, ch, 1, false);   // QKVAttention: already [Q | K | V]
+      } else {
+        // QKVAttentionLegacy: rows per head h are [q_h ; k_h ; v_h] (d each) -> row j*C + h*d + i of [Q | K | V]
+        const int d = a.dhead;
+        std::vector<float> wp((size_t)3 * ch * ch), bp((size_t)3 * ch);
+        for (int h = 0; h < a.heads; ++h)
+          for (int j = 0; j < 3; ++j)
+            for (int i = 0; i < d; ++i) {
+              const size_t src = (size_t)h * 3 * d + j * d + i, dst = (size_t)j * ch + h * d + i;
+              memcpy(&wp[dst * ch], &w[src * ch], sizeof(float) * ch);
+              bp[dst] = b[src];
+            }
+        pack_conv(a.qkv, wp.data(), bp.data(), 3 * ch, ch, 1, false);
+      }
+    }
+    { auto w = wc.next(); auto b = wc.next(); pack_conv(a.proj_out, w, b, ch, ch, 1, false); }
+    return (int)u->attn.size() - 1;
+  };
+  auto attn_layer = [&](int ch) -> Layer {
+    return cfg->use_spatial_transformer ? Layer{L_ST, make_st(ch), 0} : Layer{L_ATTN, make_attn(ch), 0};
+  };
+  AGPT_CHECK(cfg->attention_order == 0 || cfg->attention_order == 1, "attention_order must be 0 (legacy) or 1");
+
   // ---- walk the constructor rules (openaimodel.py:516-693) ----
   u->cin_pad = round_up(cfg->in_channels, 4);
   {
@@ -397,11 +495,15 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
       Block blk;
       blk.layers.push_back({L_RES, make_res(ch, m * mc), 0});
       ch = m * mc;
-      if (cfg->attn_at_level[level]) blk.layers.push_back({L_ST, make_st(ch), 0});
+      if (cfg->attn_at_level[level]) blk.layers.push_back(attn_layer(ch));
       u->in_blocks.push_back(blk);
       chans.push_back(ch);
     }
-    if (level != cfg->num_levels - 1) {
+    if (level != cfg->num_levels - 1 && cfg->resblock_updown) {
+      Block blk; blk.layers.push_back({L_RES, make_res(ch, ch, 1), 0});
+      u->in_blocks.push_back(blk);
+      chans.push_back(ch);
+    } else if (level != cfg->num_levels - 1) {
       auto w = wc.next(); auto b = wc.next();
       // stride-2 conv as im2col + GEMM: weight [Cout][Cin][3][3] -> [Cout][(kh*3+kw)*Cin + ci]
       std::vector<float> wp((size_t)ch * 9 * ch);
@@ -417,9 +519,9 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
   }
   {
     const int r1 = make_res(ch, ch);
-    const int s1 = make_st(ch);
+    const Layer a1 = attn_layer(ch);
     const int r2 = make_res(ch, ch);
-    u->mid.layers = {{L_RES, r1, 0}, {L_ST, s1, 0}, {L_RES, r2, 0}};
+    u->mid.layers = {{L_RES, r1, 0}, a1, {L_RES, r2, 0}};
   }
   for (int level = cfg->num_levels - 1; level >= 0; --level) {
     const int m = cfg->channel_mult[level];
@@ -428,8 +530,10 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
       Block blk;
       blk.layers.push_back({L_RES, make_res(ch + ich, mc * m), 0});
       ch = mc * m;
-      if (cfg->attn_at_level[level]) blk.layers.push_back({L_ST, make_st(ch), 0});
-      if (level && i == cfg->num_res_blocks) {
+      if (cfg->attn_at_level[level]) blk.layers.push_back(attn_layer(ch));
+      if (level && i == cfg->num_res_blocks && cfg->resblock_updown) {
+        blk.layers.push_back({L_RES, make_res(ch, ch, 2), 0});
+      } else if (level && i == cfg->num_res_blocks) {
         auto w = wc.next(); auto b = wc.next();
         u->up_convs.emplace_back();
         pack_conv(u->up_convs.back(), w, b, ch, ch, 9, true);
@@ -441,7 +545,7 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
   u->final_ch = ch;
   { auto g = wc.next(); auto b = wc.next(); u->out_gn_g.upload(g, ch); u->out_gn_b.upload(b, ch); }
   { auto w = wc.next(); auto b = wc.next(); pack_conv(u->conv_out, w, b, cfg->out_channels, ch, 9, true);
-    if (cfg->out_channels == 4 && cfg->in_channels == 4) {
+    if (cfg->out_channels == 4) {   // the sampling loop's latent has 4 channels (any concat conditioning aside)
       std::vector<float> w9((size_t)9 * ch * 4), b4(4);
       for (int co = 0; co < 4; ++co) {
         b4[co] = b[co];
@@ -454,7 +558,7 @@ Handle* unet_create(const agpt_unet_cfg* cfg, const float* const* W, int nW, int
 
   u->emb_total = emb_off; u->kv_total = kv_off;
   pack_conv(u->emb_all, embw.data(), embb.data(), emb_off, temb, 1, false);
-  pack_conv(u->ctx_kv_all, kvw.data(), nullptr, kv_off, ctx, 1, false);
+  if (kv_off) pack_conv(u->ctx_kv_all, kvw.data(), nullptr, kv_off, ctx, 1, false);   // no cross-attention: no context
   return u.release();
 }
 
@@ -463,6 +567,12 @@ void unet_set_context(Handle* hh, const float* ctx, int N, int S, cudaStream_t s
   DeviceGuard dg_(u->device);
   AGPT_CHECK(N >= 1 && S >= 1, "empty context");
   u->set_context(ctx, N, S, st);
+}
+
+void unet_set_concat(Handle* hh, const float* c, int N, int C, int H, int W, cudaStream_t st) {
+  auto* u = static_cast<Unet*>(hh);
+  DeviceGuard dg_(u->device);
+  u->set_concat(c, N, C, H, W, st);
 }
 
 void unet_forward(Handle* hh, const float* x, const int* t_host, int N, int H, int W, float* eps, cudaStream_t st) {
@@ -482,9 +592,19 @@ void unet_ddim_sample(Handle* hh, const float* x_T, int B, int H, int W, int S, 
   DeviceGuard dg_(u->device);
   const bool cfg_on = cfg_scale != 1.0f;
   const int N = cfg_on ? 2 * B : B;
-  AGPT_CHECK(u->ctxN == N, "agpt_unet_set_context must hold [uncond;cond] (2B rows) for guided sampling, B rows otherwise");
+  if (u->kv_total)
+    AGPT_CHECK(u->ctxN == N, "agpt_unet_set_context must hold [uncond;cond] (2B rows) for guided sampling, B rows otherwise");
+  const bool concat = u->cfg.in_channels > u->cfg.out_channels;
+  if (concat) {
+    AGPT_CHECK(!cfg_on, "the on-device loop with concat conditioning samples without guidance (cfg_scale 1)");
+    AGPT_CHECK(u->catN == B && u->catH == H && u->catW == W,
+               "agpt_unet_set_concat must hold the conditioning of this call (B rows, the latent's H and W)");
+  } else {
+    AGPT_CHECK(u->cfg.in_channels == u->cfg.out_channels, "the on-device loop needs in_channels >= out_channels");
+  }
   for (int i = 0; i < S; ++i) AGPT_CHECK(sigma[i] == 0.f, "the on-device loop is the eta = 0 sampler (noise is drawn by the step-wise path)");
-  const long n = (long)u->cfg.in_channels * H * W;
+  const long n = (long)u->cfg.out_channels * H * W;     // the loop state is the latent
+  const float* cat = concat ? u->cat_cl.p : nullptr;
   u->prepare(N, H, W);
   u->ddim_eps.ensure((size_t)N * n);
   u->ddim_x.ensure((size_t)B * n);
@@ -516,14 +636,16 @@ void unet_ddim_sample(Handle* hh, const float* x_T, int B, int H, int W, int S, 
   static int allow_graph = -1;
   if (allow_graph < 0) { const char* e = getenv("AGPT_GRAPH"); allow_graph = (e && e[0] == '0') ? 0 : 1; }
   const long l0 = launch_count_now();
-  u->ddim_step(B, N, H, W, n, st);                                   // step 0, eager
+  u->ddim_step(B, N, H, W, n, cat, st);                              // step 0, eager
   u->launches_per_step = launch_count_now() - l0;
   int done = 1;
   if (allow_graph && S > 1 && !profile_enabled()) {
     Unet::GraphKey k;
     k.N = N; k.H = H; k.W = W; k.single = cfg_on ? 0 : 1; k.arena = u->arena.p; k.ctx = u->ctx_kv.p; k.x = u->ddim_x.p; k.ctxS = u->ctxS;
+    k.cat = cat;
     const bool same = u->step_graph && k.N == u->gkey.N && k.H == u->gkey.H && k.W == u->gkey.W && k.single == u->gkey.single &&
-                      k.arena == u->gkey.arena && k.ctx == u->gkey.ctx && k.x == u->gkey.x && k.ctxS == u->gkey.ctxS;
+                      k.arena == u->gkey.arena && k.ctx == u->gkey.ctx && k.x == u->gkey.x && k.ctxS == u->gkey.ctxS &&
+                      k.cat == u->gkey.cat;
     if (!same) {
       if (u->step_graph) { cudaGraphExecDestroy(u->step_graph); u->step_graph = nullptr; }
       cudaGraph_t g = nullptr;
@@ -532,7 +654,7 @@ void unet_ddim_sample(Handle* hh, const float* x_T, int B, int H, int W, int S, 
       if (!u->cap_stream) AGPT_CUDA(cudaStreamCreateWithFlags(&u->cap_stream, cudaStreamNonBlocking));
       AGPT_CUDA(cudaStreamBeginCapture(u->cap_stream, cudaStreamCaptureModeThreadLocal));
       try {
-        u->ddim_step(B, N, H, W, n, u->cap_stream);
+        u->ddim_step(B, N, H, W, n, cat, u->cap_stream);
       } catch (...) {
         cudaStreamEndCapture(u->cap_stream, &g);
         if (g) cudaGraphDestroy(g);
@@ -548,7 +670,7 @@ void unet_ddim_sample(Handle* hh, const float* x_T, int B, int H, int W, int S, 
     for (; done < S; ++done) AGPT_CUDA(cudaGraphLaunch(u->step_graph, st));
     count_launch(u->launches_per_step * (S - 1));
   }
-  for (; done < S; ++done) u->ddim_step(B, N, H, W, n, st);
+  for (; done < S; ++done) u->ddim_step(B, N, H, W, n, cat, st);
   AGPT_CUDA(cudaMemcpyAsync(x_out, u->ddim_x.p, (size_t)B * n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (pred_x0_out)
     AGPT_CUDA(cudaMemcpyAsync(pred_x0_out, u->ddim_p0.p, (size_t)B * n * sizeof(float), cudaMemcpyDeviceToDevice, st));

@@ -15,7 +15,10 @@ alphas_cumprod, alphas_cumprod_prev, device, apply_model, q_sample for mask mode
   DiffusionWrapper and no per-step Python hook is requested (callbacks, mask,
   score_corrector, quantize, dropout), ``sample`` runs the whole loop inside the library
   (agpt_unet_ddim_sample): K/V of the context are projected once, timesteps never leave
-  the host, no device->host sync per step.
+  the host, no device->host sync per step.  The same holds for AttentionUNetModel (the
+  inpainting UNet) behind a 'concat' DiffusionWrapper with a tensor conditioning and no
+  guidance: the conditioning channels are handed to the engine once per call
+  (agpt_unet_set_concat).  Guided or dict conditionings take the step-wise path.
 """
 from __future__ import annotations
 
@@ -63,13 +66,24 @@ def noise_like(shape, device, repeat=False):
 
 
 def _agpt_unet_of(model):
-    """Our UNetModel if `model` routes apply_model(x,t,c) -> diffusion_model(x,t,context=c)."""
-    from ...modules.diffusionmodules.openaimodel import UNetModel
+    """Our UNetModel if `model` routes apply_model(x,t,c) -> diffusion_model(x,t,context=c), or our AttentionUNetModel
+    if it routes apply_model(x,t,c) -> diffusion_model(cat([x] + c_concat, 1), t) ('concat')."""
+    from ...modules.diffusionmodules.openaimodel import AttentionUNetModel, UNetModel
     wrapper = getattr(model, "model", None)
     unet = getattr(wrapper, "diffusion_model", None)
-    if isinstance(unet, UNetModel) and getattr(wrapper, "conditioning_key", "crossattn") == "crossattn":
+    key = getattr(wrapper, "conditioning_key", "crossattn")
+    if isinstance(unet, AttentionUNetModel):
+        return unet if key == "concat" and unet.in_channels > unet.out_channels else None
+    if isinstance(unet, UNetModel) and key == "crossattn":
         return unet
     return None
+
+
+def _concat_tensor(cond):
+    """The conditioning tensor of a 'concat' call: a tensor, or a one-element list holding one (else None)."""
+    if isinstance(cond, list) and len(cond) == 1:
+        cond = cond[0]
+    return cond if torch.is_tensor(cond) else None
 
 
 class DDIMSampler(object):
@@ -146,11 +160,17 @@ class DDIMSampler(object):
             return None
         if float(self._h_sigmas.abs().max()) != 0.0:        # eta > 0 draws noise per step in torch
             return None
+        unet = _agpt_unet_of(self.model)
+        if unet is not None and unet.in_channels > unet.out_channels:
+            # concat conditioning: fused without guidance only (guided concat sampling takes the step-wise path)
+            c = _concat_tensor(cond)
+            guided = unconditional_conditioning is not None and scale != 1.
+            return unet if c is not None and c.is_cuda and not guided else None
         if not torch.is_tensor(cond) or not cond.is_cuda:
             return None
         if unconditional_conditioning is not None and not torch.is_tensor(unconditional_conditioning):
             return None
-        return _agpt_unet_of(self.model)
+        return unet
 
     @torch.no_grad()
     def ddim_sampling(self, cond, shape, x_T=None, ddim_use_original_steps=False, callback=None, timesteps=None,
@@ -204,8 +224,10 @@ class DDIMSampler(object):
         x = x_T.contiguous().float()
         B, _, H, W = x.shape
         guided = uncond is not None and scale != 1.
-        ctx = torch.cat([uncond, cond]).contiguous() if guided else cond
-        unet.set_context(ctx)
+        if unet.in_channels > unet.out_channels:
+            unet.set_concat(_concat_tensor(cond))
+        else:
+            unet.set_context(torch.cat([uncond, cond]).contiguous() if guided else cond)
         order = np.flip(self.ddim_timesteps)
         S = len(order)
         idx = [S - i - 1 for i in range(S)]
@@ -300,16 +322,19 @@ class LatentDiffusionShim(torch.nn.Module):
     benchmark and tests; inside AudioGPT the real LatentDiffusion object plays this role."""
 
     class _Wrapper(torch.nn.Module):
-        """DiffusionWrapper.forward (ddpm.py:1400-1409) for the conditioning keys a cross-attention UNet can take:
-        'crossattn' (text-to-audio) and 'hybrid' (channel-concatenated conditioning + cross-attention)."""
+        """DiffusionWrapper.forward (ddpm.py:1400-1409) for the conditioning keys: 'crossattn' (text-to-audio),
+        'hybrid' (channel-concatenated conditioning + cross-attention) and 'concat' (channel-concatenated conditioning
+        only: the inpainting UNet)."""
 
         def __init__(self, unet, conditioning_key="crossattn"):
             super().__init__()
-            assert conditioning_key in ("crossattn", "hybrid")
+            assert conditioning_key in ("crossattn", "hybrid", "concat")
             self.diffusion_model = unet
             self.conditioning_key = conditioning_key
 
         def forward(self, x, t, c_concat=None, c_crossattn=None):
+            if self.conditioning_key == "concat":
+                return self.diffusion_model(torch.cat([x] + c_concat, dim=1), t)
             cc = torch.cat(c_crossattn, 1)
             if self.conditioning_key == "hybrid":
                 x = torch.cat([x] + c_concat, dim=1)
@@ -332,8 +357,9 @@ class LatentDiffusionShim(torch.nn.Module):
         return self.betas.device
 
     def apply_model(self, x_noisy, t, cond):
-        if not isinstance(cond, dict):
-            cond = {"c_crossattn": cond if isinstance(cond, list) else [cond]}
+        if not isinstance(cond, dict):      # the key choice of ddpm_audio.py:561-570
+            key = "c_concat" if self.model.conditioning_key == "concat" else "c_crossattn"
+            cond = {key: cond if isinstance(cond, list) else [cond]}
         return self.model(x_noisy, t, **cond)
 
     def q_sample(self, x_start, t, noise=None):

@@ -87,6 +87,15 @@ UNET_SMALL = dict(
     num_heads=4, num_head_channels=-1, use_spatial_transformer=True,
     transformer_depth=1, context_dim=48, legacy=False,
 )
+# Make-An-Audio Inpaint (configs/inpaint/txt2audio_args.yaml:30-45): AttentionBlock UNet, resblock_updown, legacy
+# per-head qkv order, 'concat' conditioning of 5 channels (masked-mel latent + mask) onto the 4-channel latent
+UNET_INPAINT = dict(
+    in_channels=9, out_channels=4, model_channels=320,
+    attention_resolutions=[1, 2], num_res_blocks=2, channel_mult=[1, 2],
+    num_heads=8, resblock_updown=True,
+)
+# same structure, 5x narrower (head dims 16 / 32)
+UNET_INPAINT_SMALL = dict(UNET_INPAINT, model_channels=64, num_heads=4)
 
 # lj_ds_beta6.yaml:5-24 (DiffSpeech mel normalisation range)
 SPEC_MIN = [-4.7574, -4.6783, -4.6431, -4.5832, -4.5390, -4.6771, -4.8089, -4.7672,
@@ -278,9 +287,9 @@ def diffnet_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
 def unet_plan(cfg) -> dict:
     """Walk the constructor logic of openaimodel.py:516-693 and return the block
     list as plain data: each block is a list of layers
-    ('conv_in', cin, cout) | ('res', cin, cout) | ('st', ch, heads, dhead) |
-    ('down', ch) | ('up', ch).  Only the options the shipped configs use are
-    supported (dims=2, conv_resample, no resblock_updown, no class labels,
+    ('conv_in', cin, cout) | ('res', cin, cout) | ('st', ch, heads, dhead, depth) |
+    ('attn', ch, heads, dhead) | ('down', ch) | ('up', ch) | ('resdown', ch) | ('resup', ch).
+    Only the options the shipped configs use are supported (dims=2, conv_resample, no class labels,
     use_scale_shift_norm=False)."""
     mc = cfg["model_channels"]
     mult = list(cfg["channel_mult"])
@@ -288,14 +297,30 @@ def unet_plan(cfg) -> dict:
     attn_res = set(cfg["attention_resolutions"])
     num_heads = cfg.get("num_heads", -1)
     nhc = cfg.get("num_head_channels", -1)
-    if not cfg.get("use_spatial_transformer", False):
-        raise NotImplementedError("only use_spatial_transformer=True UNets are supported")
+    nh_up = cfg.get("num_heads_upsample", -1)
+    nh_up = num_heads if nh_up == -1 else nh_up
+    legacy = cfg.get("legacy", True)
+    st = cfg.get("use_spatial_transformer", False)
+    updown = cfg.get("resblock_updown", False)
     depth = cfg.get("transformer_depth", 1)
 
     def heads_for(ch):
         if nhc == -1:
             return num_heads, ch // num_heads
         return ch // nhc, nhc
+
+    def attn(ch, upsample):
+        if st:
+            nh, dh = heads_for(ch)
+            return ("st", ch, nh, dh, depth)
+        # AttentionBlock(num_heads=..., num_head_channels=dim_head) as the constructor builds it (openaimodel.py:543-561,
+        # 590-597, 643-662): with legacy and num_head_channels == -1 it receives -1 and uses num_heads (num_heads_upsample
+        # in the output blocks); otherwise dim_head is a channel count and the head count is ch // dim_head
+        if nhc == -1 and legacy:
+            nh = nh_up if upsample else num_heads
+        else:
+            nh = ch // heads_for(ch)[1]
+        return ("attn", ch, nh, ch // nh)
 
     inp: List[list] = [[("conv_in", cfg["in_channels"], mc)]]
     chans = [mc]
@@ -305,16 +330,14 @@ def unet_plan(cfg) -> dict:
             layers = [("res", ch, m * mc)]
             ch = m * mc
             if ds in attn_res:
-                nh, dh = heads_for(ch)
-                layers.append(("st", ch, nh, dh, depth))
+                layers.append(attn(ch, False))
             inp.append(layers)
             chans.append(ch)
         if level != len(mult) - 1:
-            inp.append([("down", ch)])
+            inp.append([("resdown" if updown else "down", ch)])
             chans.append(ch)
             ds *= 2
-    nh, dh = heads_for(ch)
-    mid = [("res", ch, ch), ("st", ch, nh, dh, depth), ("res", ch, ch)]
+    mid = [("res", ch, ch), attn(ch, False), ("res", ch, ch)]
     out: List[list] = []
     for level, m in list(enumerate(mult))[::-1]:
         for i in range(nres + 1):
@@ -322,15 +345,14 @@ def unet_plan(cfg) -> dict:
             layers = [("res", ch + ich, mc * m)]
             ch = mc * m
             if ds in attn_res:
-                nh, dh = heads_for(ch)
-                layers.append(("st", ch, nh, dh, depth))
+                layers.append(attn(ch, True))
             if level and i == nres:
-                layers.append(("up", ch))
+                layers.append(("resup" if updown else "up", ch))
                 ds //= 2
             out.append(layers)
     return dict(input_blocks=inp, middle_block=mid, output_blocks=out,
                 model_channels=mc, time_embed_dim=4 * mc, final_ch=ch,
-                context_dim=cfg["context_dim"], out_channels=cfg["out_channels"],
+                context_dim=cfg.get("context_dim"), out_channels=cfg["out_channels"],
                 in_channels=cfg["in_channels"])
 
 
@@ -392,8 +414,17 @@ def unet_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
                 s[f"{p}.bias"] = (l[2],)
             elif l[0] == "res":
                 _res_shapes(s, p, l[1], l[2], temb)
+            elif l[0] in ("resdown", "resup"):
+                _res_shapes(s, p, l[1], l[1], temb)
             elif l[0] == "st":
                 _st_shapes(s, p, l[1], l[2], l[3], l[4], ctx)
+            elif l[0] == "attn":       # AttentionBlock (openaimodel.py:303-312): Conv1d 1x1 qkv / proj_out
+                s[f"{p}.norm.weight"] = (l[1],)
+                s[f"{p}.norm.bias"] = (l[1],)
+                s[f"{p}.qkv.weight"] = (3 * l[1], l[1], 1)
+                s[f"{p}.qkv.bias"] = (3 * l[1],)
+                s[f"{p}.proj_out.weight"] = (l[1], l[1], 1)
+                s[f"{p}.proj_out.bias"] = (l[1],)
             elif l[0] == "down":
                 s[f"{p}.op.weight"] = (l[1], l[1], 3, 3)
                 s[f"{p}.op.bias"] = (l[1],)

@@ -186,6 +186,12 @@ typedef struct {
   int num_head_channels;
   int transformer_depth;
   int context_dim;
+  int use_spatial_transformer;          /* 1: SpatialTransformer blocks (cross-attention on a context);
+                                           0: AttentionBlock (self-attention only, no context) */
+  int resblock_updown;                  /* 1: down/up-sampling ResBlocks (avg-pool / nearest) instead of
+                                           the strided / upsampling convs */
+  int attention_order;                  /* AttentionBlock qkv channel order: 0 legacy per-head [q_h;k_h;v_h]
+                                           (QKVAttentionLegacy), 1 [Q|K|V] (use_new_attention_order) */
 } agpt_unet_cfg;
 
 int agpt_unet_create(const agpt_unet_cfg* cfg, const float* const* host_weights,
@@ -193,6 +199,11 @@ int agpt_unet_create(const agpt_unet_cfg* cfg, const float* const* host_weights,
 /* Hoist the step-invariant to_k/to_v(context) of every cross-attention
  * (attention.py:174-176) for context [N,S,context_dim] (device).             */
 int agpt_unet_set_context(agpt_handle h, const float* context, int N, int S, void* stream);
+/* Concat conditioning of agpt_unet_ddim_sample for a UNet with in_channels > out_channels
+ * (DiffusionWrapper 'concat', ddpm.py:1404-1406): c [N, in_channels - out_channels, H, W] (device) is
+ * appended to the latent's channels at every step.  It is read once here and put into the kernel
+ * layout once; the loop state stays the out_channels latent.                                       */
+int agpt_unet_set_concat(agpt_handle h, const float* c, int N, int C, int H, int W, void* stream);
 /* eps [N,Cout,H,W] = UNet(x [N,Cin,H,W], t [N] host ints, context set above) */
 int agpt_unet_forward(agpt_handle h, const float* x, const int* t_host, int N, int H, int W,
                       float* eps, void* stream);
@@ -206,7 +217,9 @@ int agpt_ddim_update(const float* x, const float* eps2, int eps2_is_single, floa
                      const float* noise, float temperature, int B, long n_per_sample,
                      float* x_prev, float* pred_x0_or_null, void* stream);
 /* Whole DDIM loop on device (ddim.py:117-166, eta = 0) with CFG; context = [uncond ; cond]
- * set through agpt_unet_set_context (2B rows) or B rows when cfg_scale == 1.
+ * set through agpt_unet_set_context (2B rows) or B rows when cfg_scale == 1.  A UNet with
+ * in_channels > out_channels samples x_T [B, out_channels, H, W] with the conditioning of
+ * agpt_unet_set_concat (B rows, same H and W, cfg_scale 1).
  * tables: host arrays of length S in *sampling order* (index S-1 first).  The time-embedding
  * MLP and the ResBlock embedding projections run once for all S timesteps; step 0 runs as plain
  * launches, then ONE captured step (CUDA graph, device-side step counter and coefficient tables)
