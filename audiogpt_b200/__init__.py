@@ -15,6 +15,7 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.vocoder.bigvgan.models.BigVGAN / VocoderBigVGAN
     audiogpt_b200.modules.fastspeech.fs2.FastSpeech2                (installed with install(front_end=True))
     audiogpt_b200.modules.diffsinger_midi.fs2.FastSpeech2MIDI       (installed with install(front_end=True))
+    audiogpt_b200.ldm.modules.encoders.modules.FrozenCLAPEmbedder   (installed with install(text_encoder=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -44,9 +45,14 @@ _FRONT_END_MAP = {
 _FIRST_STAGE_MAP = {
     "ldm.models.autoencoder": ("audiogpt_b200.ldm.models.autoencoder", {"AutoencoderKL": "AutoencoderKLWithEncoder"}),
 }
+# the CLAP text encoder of the Make-An-Audio tools, grafted only on request (install(text_encoder=True))
+_TEXT_ENCODER_MAP = {
+    "ldm.modules.encoders.modules": ("audiogpt_b200.ldm.modules.encoders.modules", ["FrozenCLAPEmbedder"]),
+}
 
 
-def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False):
+def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
+            text_encoder: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -64,12 +70,15 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     ``inpaint=True`` also makes ``UNetModel(...)`` build AttentionUNetModel for the AttentionBlock configs it covers
     (the Inpaint tool's denoiser) instead of the reference's class, so with ``first_stage=True`` the whole Inpaint
     chain runs on the engine.
+    ``text_encoder=True`` also replaces ``ldm.modules.encoders.modules.FrozenCLAPEmbedder``, so the text-to-audio tool's
+    conditioning (get_learned_conditioning) runs on the engine too, from token ids to waveform.
     Returns the list of patched names."""
     import importlib
     import sys
     import types
     patched = []
-    todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}), **(_FIRST_STAGE_MAP if first_stage else {}))
+    todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}), **(_FIRST_STAGE_MAP if first_stage else {}),
+                **(_TEXT_ENCODER_MAP if text_encoder else {}))
     for ref_name, (our_name, attrs) in todo.items():
         ours = importlib.import_module(our_name)
         names = attrs if isinstance(attrs, dict) else {a: a for a in attrs}

@@ -68,6 +68,14 @@ class Fs2Cfg(C.Structure):
         "use_pos_embed", "rel_pos", "pitch_type", "use_energy_embed", "use_midi")]
 
 
+class ClapConfig(C.Structure):
+    """agpt_clap_cfg: the one config struct with float fields (a tagged struct in the header; the create entry point
+    takes it as a plain pointer)."""
+    _fields_ = [(n, C.c_int) for n in (
+        "vocab_size", "max_position_embeddings", "type_vocab_size", "hidden_size", "num_layers", "num_heads",
+        "intermediate_size", "d_proj")] + [("layer_norm_eps", C.c_float), ("proj_layer_norm_eps", C.c_float)]
+
+
 # (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
 # takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
 _I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
@@ -117,6 +125,8 @@ PROTOTYPES = {
     "agpt_fs2_create": (_I, [C.POINTER(Fs2Cfg), _W, _I, _I, _OUT]),
     "agpt_fs2_encode": (_I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _P, _P]),
     "agpt_fs2_decode": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _F, _F, _P, _P, _P, _P, _P, _P, _P]),
+    "agpt_clap_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_clap_encode": (_I, [_P, _P, _I, _I, _P, _P]),
 }
 
 _lock = threading.Lock()

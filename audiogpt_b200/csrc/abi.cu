@@ -299,6 +299,20 @@ int agpt_fs2_decode(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out
   });
 }
 
+int agpt_clap_create(const agpt_clap_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(clap_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_clap_encode(agpt_handle h, const int* input_ids, int N, int L, float* z, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(input_ids && z, "null argument");
+    clap_encode(as(h, kMagicClap, "clap"), input_ids, N, L, z, (cudaStream_t)stream);
+  });
+}
+
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                        int check, double* out3, double* dbg8_or_null) {
   return guarded([&] { bench_tapconv(G, L, Cin, Cout, K, dil, Wreal, epi_res, use_tc, reps, check, out3, dbg8_or_null); });

@@ -55,6 +55,9 @@ void fs2_decode(Handle* h, int Tm, const int* mel2ph_in, int* mel2ph_out, const 
                 int norm, float f0_mean, float f0_std, float* pitch_pred, float* f0d, int* coarse, float* e_pred, float* dec_inp, float* mel,
                 cudaStream_t st);
 
+Handle* clap_create(const agpt_clap_cfg* cfg, const float* const* W, int nW, int device);
+void clap_encode(Handle* h, const int* ids, int N, int L, float* z, cudaStream_t st);
+
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                    int check, double* out, double* dbg_avg, double x_scale = 1.0, double w_spread = 1.0, double* rel2 = nullptr);
 

@@ -844,3 +844,51 @@ def synth_fs2_inputs(cfg, B, T, seed):
         out["midi_dur"] = (0.1 + 0.9 * torch.rand((B, T), generator=g)) * valid
         out["is_slur"] = torch.randint(0, 2, (B, T), generator=g) * valid
     return out
+
+
+# ---------------------------------------------------------------------------------------------- CLAP text encoder
+# FrozenCLAPEmbedder (text_to_audio/Make_An_Audio/ldm/modules/encoders/modules.py:173-212): bert-base-uncased (the
+# BertConfig() defaults) and CLAP's Projection 768 -> 1024 (CLAP/config.yml d_proj), tokens padded to max_length 77
+CLAP_BASE = dict(vocab_size=30522, max_position_embeddings=512, type_vocab_size=2, hidden_size=768, num_layers=12,
+                 num_heads=12, intermediate_size=3072, d_proj=1024, layer_norm_eps=1e-12, proj_layer_norm_eps=1e-5,
+                 max_length=77)
+# same structure, head dim 16; d_proj 48 is UNET_SMALL's context_dim, so it conditions the small UNet
+CLAP_SMALL = dict(CLAP_BASE, vocab_size=1000, max_position_embeddings=80, hidden_size=64, num_layers=2, num_heads=4,
+                  intermediate_size=256, d_proj=48)
+# the fields of agpt_clap_cfg (max_length belongs to the tokenizer)
+CLAP_ENGINE_KEYS = ("vocab_size", "max_position_embeddings", "type_vocab_size", "hidden_size", "num_layers", "num_heads",
+                    "intermediate_size", "d_proj", "layer_norm_eps", "proj_layer_norm_eps")
+
+
+def clap_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of FrozenCLAPEmbedder: caption_encoder.base (HF BertModel: embeddings, encoder
+    layers, pooler) and caption_encoder.projection (CLAP/clap.py:8-14 Projection), in state-dict order, which is the
+    order agpt_clap_create consumes."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    H, I, D = int(cfg["hidden_size"]), int(cfg["intermediate_size"]), int(cfg["d_proj"])
+    b = "caption_encoder.base."
+    s[b + "embeddings.word_embeddings.weight"] = (int(cfg["vocab_size"]), H)
+    s[b + "embeddings.position_embeddings.weight"] = (int(cfg["max_position_embeddings"]), H)
+    s[b + "embeddings.token_type_embeddings.weight"] = (int(cfg["type_vocab_size"]), H)
+    s[b + "embeddings.LayerNorm.weight"] = (H,); s[b + "embeddings.LayerNorm.bias"] = (H,)
+    for i in range(int(cfg["num_layers"])):
+        p = f"{b}encoder.layer.{i}."
+        for n in ("query", "key", "value"):
+            s[f"{p}attention.self.{n}.weight"] = (H, H); s[f"{p}attention.self.{n}.bias"] = (H,)
+        s[p + "attention.output.dense.weight"] = (H, H); s[p + "attention.output.dense.bias"] = (H,)
+        s[p + "attention.output.LayerNorm.weight"] = (H,); s[p + "attention.output.LayerNorm.bias"] = (H,)
+        s[p + "intermediate.dense.weight"] = (I, H); s[p + "intermediate.dense.bias"] = (I,)
+        s[p + "output.dense.weight"] = (H, I); s[p + "output.dense.bias"] = (H,)
+        s[p + "output.LayerNorm.weight"] = (H,); s[p + "output.LayerNorm.bias"] = (H,)
+    s[b + "pooler.dense.weight"] = (H, H); s[b + "pooler.dense.bias"] = (H,)
+    q = "caption_encoder.projection."
+    s[q + "linear1.weight"] = (D, H)
+    s[q + "linear2.weight"] = (D, D)
+    s[q + "layer_norm.weight"] = (D,); s[q + "layer_norm.bias"] = (D,)
+    return s
+
+
+def synth_clap(cfg, seed: int = 7070):
+    """Seeded FrozenCLAPEmbedder weights (synth_state_dict: embedding rows and Linears N(0, 1 / fan_in), LayerNorm
+    scales 1 + 0.1 N, biases 0.05 N)."""
+    return synth_state_dict(clap_param_shapes(cfg), seed, convtranspose_prefixes=())

@@ -326,6 +326,33 @@ int agpt_fs2_decode(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out
                     const float* energy, int use_uv, int pitch_norm, float f0_mean, float f0_std, float* pitch_pred,
                     float* f0_denorm, int* pitch_coarse, float* energy_pred, float* decoder_inp, float* mel_out, void* stream);
 
+/* ------------------------------------------------------------------ CLAP text encoder
+ * Replaces FrozenCLAPEmbedder.encode after tokenization (text_to_audio/Make_An_Audio/ldm/modules/encoders/modules.py:
+ * 205-212): BERT (HF BertModel called with input_ids only, so every position attends to every position, padding
+ * included; token type 0) then CLAP's Projection (ldm/modules/encoders/CLAP/clap.py:8-20, dropout off):
+ * z = LayerNorm(e1 + linear2(gelu(e1))), e1 = linear1(last_hidden_state).  The conditioning of every Make-An-Audio
+ * text-to-audio call (get_learned_conditioning).  Unlike the other configs this one carries floats, so it is a
+ * tagged struct.                                                                                                 */
+typedef struct agpt_clap_cfg {
+  int vocab_size;              /* BertConfig.vocab_size (30522) */
+  int max_position_embeddings; /* 512: the longest sequence */
+  int type_vocab_size;         /* 2 (only type 0 is read) */
+  int hidden_size;             /* 768 */
+  int num_layers;              /* 12 */
+  int num_heads;               /* 12 */
+  int intermediate_size;       /* 3072 */
+  int d_proj;                  /* 1024: the UNet's context_dim */
+  float layer_norm_eps;        /* BERT's LayerNorms (1e-12) */
+  float proj_layer_norm_eps;   /* Projection.layer_norm (1e-5) */
+} agpt_clap_cfg;
+/* host_weights: fp32 HOST arrays in the key order of audiogpt_b200.specs.clap_param_shapes(cfg) (the reference's
+ * state-dict keys under caption_encoder.base.* and caption_encoder.projection.*); the pooler, which encode never
+ * uses, is passed and ignored.                                                                                      */
+int agpt_clap_create(const agpt_clap_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* input_ids [N][L] int32 (device) -> z [N][L][d_proj] (device).  L <= max_position_embeddings; ids outside
+ * [0, vocab_size) are clamped to it (callers are expected to reject them first).                                  */
+int agpt_clap_encode(agpt_handle h, const int* input_ids, int N, int L, float* z, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
