@@ -76,6 +76,24 @@ class ClapConfig(C.Structure):
         "intermediate_size", "d_proj")] + [("layer_norm_eps", C.c_float), ("proj_layer_norm_eps", C.c_float)]
 
 
+class TapconvProbeArgs(C.Structure):
+    """agpt_tapconv_probe_args (a tagged struct in the header: it carries pointers and floats)."""
+    _fields_ = [(n, C.c_int) for n in ("kind", "Cin", "Cout", "K", "dil", "Wreal", "strip_w", "u", "pad", "g")] + [
+        ("w", C.c_void_p), ("b", C.c_void_p), ("G", C.c_int), ("L", C.c_int),
+        ("inp", C.c_void_p), ("in_gstride", C.c_long), ("in_pitch", C.c_int),
+        ("out", C.c_void_p), ("out_gstride", C.c_long), ("out_pitch", C.c_int),
+        ("res", C.c_void_p), ("res_gstride", C.c_long), ("res_pitch", C.c_int),
+        ("out2", C.c_void_p), ("out2_gstride", C.c_long), ("out2_pitch", C.c_int),
+        ("pro", C.c_int), ("slope", C.c_float), ("pvec", C.c_void_p), ("pvec_gstride", C.c_int),
+        ("epi", C.c_int), ("scale", C.c_float), ("accumulate", C.c_int), ("csplit", C.c_int),
+        ("evec", C.c_void_p), ("evec_gstride", C.c_int),
+        ("tc_tall", C.c_int), ("plane_in", C.c_int),
+        ("po_hi", C.c_void_p), ("po_lo", C.c_void_p), ("po_slope", C.c_float),
+        ("pl_hi", C.c_void_p), ("pl_lo", C.c_void_p), ("pl_pitch", C.c_int),
+        ("fma", C.c_int), ("pair", C.c_int),
+        ("w2", C.c_void_p), ("b2", C.c_void_p), ("K2", C.c_int), ("dil2", C.c_int)]
+
+
 # (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
 # takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
 _I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
@@ -96,8 +114,8 @@ PROTOTYPES = {
     "agpt_attention": (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P]),
     "agpt_set_attention_tc": (_I, [_I]),
     "agpt_attention_masked": (_I, [_P, _I, _P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
-    "agpt_bench_tapconv": (_I, [_I] * 11 + [_P, _P]),
-    "agpt_check_tapconv": (_I, [_I] * 8 + [_D, _D, _P]),
+    "agpt_bench_tapconv": (_I, [_I] * 10 + [_P, _P]),
+    "agpt_tapconv_probe": (_I, [_P, _P, _P]),
     "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
     "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "agpt_hifigan_vocode_host": (_I, [_P, _P, _P, _I, _I, _P]),

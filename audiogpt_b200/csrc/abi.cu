@@ -314,16 +314,17 @@ int agpt_clap_encode(agpt_handle h, const int* input_ids, int N, int L, float* z
 }
 
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
-                       int check, double* out3, double* dbg8_or_null) {
-  return guarded([&] { bench_tapconv(G, L, Cin, Cout, K, dil, Wreal, epi_res, use_tc, reps, check, out3, dbg8_or_null); });
+                       double* out2, double* dbg8_or_null) {
+  return guarded([&] {
+    AGPT_CHECK(out2, "null argument");
+    bench_tapconv(G, L, Cin, Cout, K, dil, Wreal, epi_res, use_tc, reps, out2, dbg8_or_null);
+  });
 }
 
-int agpt_check_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, double x_scale,
-                       double w_spread, double* rel2) {
+int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream) {
   return guarded([&] {
-    AGPT_CHECK(rel2, "null argument");
-    double out3[3];
-    bench_tapconv(G, L, Cin, Cout, K, dil, Wreal, epi_res, 1, 1, 1, out3, nullptr, x_scale, w_spread, rel2);
+    AGPT_CHECK(args && ran, "null argument");
+    tapconv_probe(*args, ran, (cudaStream_t)stream);
   });
 }
 

@@ -530,6 +530,12 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   for (int j = 0; j < nk; ++j)
     AGPT_CHECK(cfg->resblock_kernel_sizes[j] % 2 == 1 && cfg->resblock_kernel_sizes[j] <= kMaxTaps,
                "resblock kernel size must be odd and <= 11");
+  // ConvTranspose1d(k, u, padding=(k-u)//2) yields L*u + (k-u) % 2 samples: the engine's polyphase upsampler and its
+  // T * hop output are exactly L*u, so an odd k - u would silently drop the reference's last sample of every stage
+  for (int i = 0; i < nu; ++i)
+    AGPT_CHECK(cfg->upsample_rates[i] >= 1 && cfg->upsample_kernel_sizes[i] >= cfg->upsample_rates[i] &&
+                   (cfg->upsample_kernel_sizes[i] - cfg->upsample_rates[i]) % 2 == 0,
+               "upsample kernel size k and rate u need k >= u and an even k - u (else the stage does not output L*u samples)");
   std::unique_ptr<Hifigan> h(new Hifigan());
   h->magic = kMagicHifigan; h->device = device; h->cfg = *cfg;
   { const char* e = getenv("AGPT_FUSE_RESBLOCK"); h->fuse_resblock = !(e && e[0] == '0'); }

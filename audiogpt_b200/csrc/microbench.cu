@@ -1,37 +1,31 @@
 // Micro-benchmark / tuning entry: one tapconv layer of a given shape on random data, timed with
 // CUDA events; optionally returns the per-CTA phase timestamps of the tensor-core kernel.
+// Conformance entry: one production launch of the primitive on caller-owned tensors (tapconv_probe).
 #include <random>
 #include "tapconv.cuh"
 #include "models.h"
 
 namespace agpt {
 
-// out[0] = ms per launch, out[1] = TFLOP/s (algorithmic), out[2] = max |tc - fma| (when check != 0)
+// out[0] = ms per launch, out[1] = TFLOP/s (algorithmic)
 // dbg_avg[8]: averaged phase deltas in cycles (setup, first-A, mainloop, tail, epilogue, total, waitA, waitW)
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
-                   int check, double* out, double* dbg_avg, double x_scale, double w_spread, double* rel2) {
+                   double* out, double* dbg_avg) {
   std::mt19937 rng(1234);
   std::normal_distribution<float> nd(0.f, 1.f);
   const bool is2d = Wreal > 0;
   const int taps = is2d ? 9 : K;
   std::vector<float> w((size_t)Cout * Cin * taps), b(Cout);
   for (auto& v : w) v = nd(rng) / std::sqrt((float)Cin * taps);
-  if (w_spread > 1.0) {   // weight-norm-like gain spread: output channel co scaled by w_spread^u, u log-uniform in [-1/2, 1/2]
-    std::uniform_real_distribution<float> ud(-0.5f, 0.5f);
-    for (int co = 0; co < Cout; ++co) {
-      const float gsc = std::pow((float)w_spread, ud(rng));
-      for (size_t i = 0; i < (size_t)Cin * taps; ++i) w[(size_t)co * Cin * taps + i] *= gsc;
-    }
-  }
   for (auto& v : b) v = 0.05f * nd(rng);
   PackedConv pc;
   pack_conv(pc, w.data(), b.data(), Cout, Cin, taps, is2d);
   const size_t nin = (size_t)G * L * Cin, nout = (size_t)G * L * Cout;
   std::vector<float> hx(nin);
-  for (auto& v : hx) v = nd(rng) * (float)x_scale;
-  DevBuf x, y, y2, r;
+  for (auto& v : hx) v = nd(rng);
+  DevBuf x, y, r;
   x.upload(hx);
-  y.ensure(nout); y2.ensure(nout); r.ensure(nout);
+  y.ensure(nout); r.ensure(nout);
   AGPT_CUDA(cudaMemset(r.p, 0, nout * 4));
   TapConvParams P = tapconv_params(pc, G, L, Wreal, dil);
   P.in = x.p; P.in_gstride = (long)L * Cin; P.in_pitch = Cin;
@@ -64,7 +58,6 @@ void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, i
   AGPT_CUDA(cudaEventElapsedTime(&ms, e0, e1));
   out[0] = ms / reps;
   out[1] = 2.0 * G * (double)L * Cin * Cout * taps / (out[0] * 1e-3) / 1e12;
-  out[2] = -1.0;
   if (dbg_avg && use_tc) {
     std::vector<long long> h((size_t)nctas * 8);
     AGPT_CUDA(cudaMemcpy(h.data(), dbgbuf.p, h.size() * 8, cudaMemcpyDeviceToHost));
@@ -86,31 +79,83 @@ void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, i
     }
     for (int i = 0; i < 8; ++i) dbg_avg[i] = n ? acc[i] / n : 0.0;
   }
-  if (check) {
-    tc_set_enabled(0);
-    TapConvParams Q = P;
-    Q.out = y2.p; Q.dbg = nullptr; Q.tc_flags_user = 0;
-    tapconv_launch(Q, st);
-    AGPT_CUDA(cudaDeviceSynchronize());
-    std::vector<float> a(nout), c(nout);
-    AGPT_CUDA(cudaMemcpy(a.data(), y.p, nout * 4, cudaMemcpyDeviceToHost));
-    AGPT_CUDA(cudaMemcpy(c.data(), y2.p, nout * 4, cudaMemcpyDeviceToHost));
-    double mx = 0, se = 0, sr = 0;
-    bool finite = true;
-    for (size_t i = 0; i < nout; ++i) {
-      const double d = (double)a[i] - (double)c[i];
-      if (!std::isfinite(a[i])) finite = false;
-      mx = std::max(mx, std::fabs(d)); se += d * d; sr += (double)c[i] * c[i];
-    }
-    out[2] = mx;
-    if (rel2) {   // {max |diff| / rms(reference), rms(diff) / rms(reference)}; reference = the fp32-FMA kernel
-      const double rms = std::sqrt(sr / (double)nout);
-      rel2[0] = finite ? (rms > 0 ? mx / rms : mx) : 1e30;
-      rel2[1] = finite ? (rms > 0 ? std::sqrt(se / (double)nout) / rms : std::sqrt(se / (double)nout)) : 1e30;
-    }
-  }
   tc_set_enabled(tc_prev ? 1 : 0);
   cudaEventDestroy(e0); cudaEventDestroy(e1);
+}
+
+// One launch of the production tap-GEMM path on caller-owned tensors (agpt_tapconv_probe, include/agpt_b200.h).
+void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st) {
+  AGPT_CHECK(a.w && a.G >= 1 && a.L >= 1 && a.Cin >= 1 && a.Cout >= 1, "tapconv probe: bad arguments");
+  AGPT_CHECK(!a.plane_in || (a.pro == PRO_LRELU && !a.fma), "tapconv probe: plane input needs PRO_LRELU on the tensor cores");
+  AGPT_CHECK(!a.pair || (a.kind == 0 && a.w2 && a.res && a.Cin == a.Cout && !a.fma),
+             "tapconv probe: a pair is two Conv1d C -> C with a residual, on the tensor cores");
+  const int dil = a.dil > 0 ? a.dil : 1;
+  int gk = 1;   // time steps per row of the grouped view (kind 3)
+  PackedConv pc, pc2;
+  switch (a.kind) {
+    case 0: pack_conv(pc, a.w, a.b, a.Cout, a.Cin, a.K, false); break;
+    case 1: AGPT_CHECK(a.Wreal > 0 && a.L % a.Wreal == 0, "tapconv probe: 3x3 conv needs L = H * Wreal");
+            pack_conv(pc, a.w, a.b, a.Cout, a.Cin, 9, true); break;
+    case 2: pack_convtranspose(pc, a.w, a.b, a.Cin, a.Cout, a.K, a.u, a.pad); break;
+    case 3: AGPT_CHECK(a.g >= 2 && a.Cin == a.Cout && a.L % a.g == 0 && dil == 1 && a.in_pitch == a.Cin &&
+                           (a.out_pitch == a.Cout || !a.out) && (!a.res || a.res_pitch == a.Cout),
+                       "tapconv probe: grouped conv needs C -> C, L % g == 0, dilation 1 and unpadded rows");
+            pack_conv_grouped(pc, a.w, a.b, a.Cin, a.K, a.g);
+            gk = a.g; break;
+    case 4: AGPT_CHECK(a.Cout % 2 == 0, "tapconv probe: a pair conv has an even Cout");
+            pack_conv_pairs(pc, a.w, a.b, a.Cout, a.Cin, a.K); break;
+    default: throw Error("tapconv probe: unknown kind");
+  }
+  TapConvParams P = tapconv_params(pc, a.G, a.L / gk, a.kind == 1 ? a.Wreal : 0, dil);
+  if (a.kind == 1 && a.strip_w > 0) tapconv_set_strips(P, a.strip_w);
+  P.in = a.in; P.in_gstride = a.in_gstride; P.in_pitch = a.in_pitch * gk;
+  P.out = a.out; P.out_gstride = a.out_gstride; P.out_pitch = a.out_pitch * gk;
+  P.res = a.res; P.res_gstride = a.res_gstride; P.res_pitch = a.res_pitch * gk;
+  P.out2 = a.out2; P.out2_gstride = a.out2_gstride; P.out2_pitch = a.out2_pitch * gk;
+  P.pro = a.pro; P.slope = a.slope; P.pvec = a.pvec; P.pvec_gstride = a.pvec_gstride;
+  P.epi = a.epi; P.scale = a.scale; P.accumulate = a.accumulate; P.csplit = a.csplit;
+  P.evec = a.evec; P.evec_gstride = a.evec_gstride;
+  P.tc_tall = a.tc_tall;
+  P.po_hi = static_cast<__half*>(a.po_hi); P.po_lo = static_cast<__half*>(a.po_lo); P.po_slope = a.po_slope;
+  P.pl_hi = static_cast<__half*>(a.pl_hi); P.pl_lo = static_cast<__half*>(a.pl_lo); P.pl_pitch = a.pl_pitch;
+  DevBuf planes;
+  if (a.plane_in) {   // the input's operand planes, laid out like the fp32 tensor (plane_split covers G sample strides)
+    const long n = (long)a.G * a.in_gstride;
+    planes.ensure((size_t)n);   // n floats = 2 n halves: hi [n], lo [n]
+    __half* hi = reinterpret_cast<__half*>(planes.p);
+    plane_split(a.in, hi, hi + n, n, a.slope, st);
+    P.pi_hi = hi; P.pi_lo = hi + n;
+  }
+  for (int i = 0; i < 4; ++i) ran[i] = -1;
+  tapconv_note_launch(-1, -1, -1, -1);
+  const bool tc_prev = tc_enabled();
+  if (a.fma) tc_set_enabled(0);
+  try {
+    if (a.pair) {
+      pack_conv(pc2, a.w2, a.b2, a.Cout, a.Cout, a.K2, false);
+      TapConvParams P1 = P;                       // c1: leaky ReLU, bias; its output stays in shared memory
+      P1.out = nullptr; P1.res = nullptr; P1.out2 = nullptr; P1.epi = EPI_BIAS; P1.scale = 1.f; P1.accumulate = 0;
+      P1.po_hi = P1.po_lo = nullptr; P1.pl_hi = P1.pl_lo = nullptr;
+      TapConvParams P2 = tapconv_params(pc2, a.G, a.L, 0, a.dil2 > 0 ? a.dil2 : 1);
+      P2.in = nullptr; P2.in_pitch = a.Cout;      // c2 reads c1's tile, never global memory
+      P2.out = P.out; P2.out_gstride = P.out_gstride; P2.out_pitch = P.out_pitch;
+      P2.res = P.res; P2.res_gstride = P.res_gstride; P2.res_pitch = P.res_pitch;
+      P2.pro = PRO_LRELU; P2.slope = a.slope;
+      P2.epi = P.epi; P2.scale = P.scale; P2.accumulate = P.accumulate;
+      P2.tc_tall = a.tc_tall;
+      P2.po_hi = P.po_hi; P2.po_lo = P.po_lo; P2.po_slope = P.po_slope;
+      AGPT_CHECK(tcpair_launch(P1, P2, st), "tapconv probe: the fused pair launch was not taken");
+    } else {
+      tapconv_launch(P, st);
+    }
+    AGPT_CUDA(cudaStreamSynchronize(st));   // the packed weights and planes are freed on return
+  } catch (...) {
+    tc_set_enabled(tc_prev ? 1 : 0);
+    cudaStreamSynchronize(st);
+    throw;
+  }
+  tc_set_enabled(tc_prev ? 1 : 0);
+  tapconv_last_launch(ran);
 }
 
 }  // namespace agpt

@@ -59,6 +59,7 @@ Handle* clap_create(const agpt_clap_cfg* cfg, const float* const* W, int nW, int
 void clap_encode(Handle* h, const int* ids, int N, int L, float* z, cudaStream_t st);
 
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
-                   int check, double* out, double* dbg_avg, double x_scale = 1.0, double w_spread = 1.0, double* rel2 = nullptr);
+                   double* out, double* dbg_avg);
+void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);
 
 }  // namespace agpt

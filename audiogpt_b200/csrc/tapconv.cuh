@@ -150,6 +150,10 @@ void profile_count_tall();            // a tensor-core launch with 256-row tiles
 long long profile_tall_launches();
 void profile_count_plane();           // a plane-fed tensor-core launch (counted while profiling)
 long long profile_plane_launches();
+// The variant of the most recent tap-GEMM launch on this host thread, {1 tensor-core | 0 fp32-FMA, tile width, tile
+// height, 1 plane-fed}, recorded where a kernel is actually launched (agpt_tapconv_probe reports it); -1s before any.
+void tapconv_note_launch(int tc, int bn, int mt, int plane);
+void tapconv_last_launch(int ran[4]);
 // fp32 [n] -> operand plane hi / lo of lrelu(x, slope) (TapConvParams::pi_hi), n a multiple of 4 (tcconv5.cu)
 void plane_split(const float* x, __half* hi, __half* lo, long n, float slope, cudaStream_t st);
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches);

@@ -902,6 +902,7 @@ static bool tcconv5_try(TapConvParams P, int BN, int MT, cudaStream_t st) {
   const int Lv = tc_lv(P);
   dim3 grid(cdiv(Lv, MT), cdiv(P.Cout, BN), tc_groups(P));
   tc5_set_smem_limits();
+  tapconv_note_launch(1, BN, MT, P.pi_hi ? 1 : 0);
   if (P.pi_hi) {
     const PlMaps m = pl_tensor_maps(P);
     if (MT == TC_TALL) {
@@ -963,6 +964,7 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, cudaStream_t 
   dim3 grid(cdiv(tc_lv(P1), MT - span2), 1, tc_groups(P1));
   tc5_set_smem_limits();
   void* rec = profile_begin_pair(P1, P2, st);
+  tapconv_note_launch(1, BN, MT, P1.pi_hi ? 1 : 0);
   if (P1.pi_hi) {
     const PlMaps m = pl_tensor_maps(P1);
     if (MT == TC_TALL) {

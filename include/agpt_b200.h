@@ -60,17 +60,49 @@ int agpt_set_attention_tc(int on);
 int agpt_attention_masked(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
                           const uint8_t* key_padding_mask, float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk,
                           void* stream);
-/* Micro-benchmark of one tapconv layer (random data): out3 = {ms per launch, algorithmic TFLOP/s,
- * max |tensor-core - fp32 FMA| when check != 0}; dbg8 (tensor-core kernel only) = average per-CTA phase cycles
- * {setup, first activation tile, MMA issue loop, drain, epilogue, total, wait-on-activations,
- * wait-on-weights}.  Wreal > 0 selects a 3x3 conv on an (L/Wreal) x Wreal image.              */
+/* Micro-benchmark of one tapconv layer (random data): out2 = {ms per launch, algorithmic TFLOP/s}; dbg8
+ * (tensor-core kernel only) = average per-CTA phase cycles {setup, first activation tile, MMA issue loop, drain,
+ * epilogue, total, wait-on-activations, wait-on-weights}.  Wreal > 0 selects a 3x3 conv on an (L/Wreal) x Wreal
+ * image.                                                                                                       */
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc,
-                       int reps, int check, double* out3, double* dbg8_or_null);
-/* Numerics probe of one layer: activations ~ N(0,1) * x_scale, weights with a weight-norm-like gain spread
- * (output channel gains log-uniform over a factor w_spread); runs the tensor-core kernel and the fp32-FMA
- * kernel on the same data.  rel2 = {max |diff| / rms(ref), rms(diff) / rms(ref)} (1e30 if anything is not finite). */
-int agpt_check_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, double x_scale,
-                       double w_spread, double* rel2);
+                       int reps, double* out2, double* dbg8_or_null);
+
+/* Conformance entry of the tap-GEMM primitive (tests/test_tapconv_gpu.py): ONE launch of the production path --
+ * the production weight packer, tapconv_launch (or the fused pair launch) -- on caller-owned device tensors.
+ * Weights and bias are fp32 HOST arrays in the torch layouts; everything else passes through to the launch
+ * parameters as given (pitches and sample strides in elements).                                               */
+typedef struct agpt_tapconv_probe_args {
+  int kind;        /* 0 Conv1d w [Cout][Cin][K] (dilation dil), "same" padding
+                      1 Conv2d w [Cout][Cin][3][3] on (L / Wreal) x Wreal images, padding 1; strip_w > 0: strip mode
+                      2 ConvTranspose1d w [Cin][Cout][K], stride u, padding pad: the output [L][u*Cout] is [L*u][Cout]
+                      3 Conv1d (dilation 1) over g time steps at once: the [L][C] tensors are viewed as [L/g][g*C]
+                        (pitches must equal C), Cin == Cout == C
+                      4 Conv1d with (first half, second half) output channels interleaved, for EPI_GATE / EPI_GEGLU:
+                        the epilogue's res operand is in the interleaved order                                    */
+  int Cin, Cout, K, dil, Wreal, strip_w, u, pad, g;
+  const float* w;  /* host */
+  const float* b;  /* host, NULL = no bias */
+  int G, L;
+  const float* in; long in_gstride; int in_pitch;
+  float* out; long out_gstride; int out_pitch;          /* out may be NULL when a plane output is set */
+  const float* res; long res_gstride; int res_pitch;
+  float* out2; long out2_gstride; int out2_pitch;
+  int pro; float slope; const float* pvec; int pvec_gstride;
+  int epi; float scale; int accumulate; int csplit; const float* evec; int evec_gstride;
+  int tc_tall;
+  int plane_in;    /* split `in` into fp16 hi / lo operand planes (probe-owned) and feed the launch from them;
+                      PRO_LRELU only (the split applies the slope), tensor cores only                           */
+  void* po_hi; void* po_lo; float po_slope;            /* output operand plane (fp16), NULL = none */
+  void* pl_hi; void* pl_lo; int pl_pitch;              /* EPI_GATE / EPI_GEGLU output plane (fp16), NULL = none */
+  int fma;         /* 1: force the fp32-FMA kernel (the tensor-core setting is restored afterwards) */
+  int pair;        /* 1: fused ResBlock pair out = epi(c2(lrelu(c1(lrelu(in))))) in one launch: c1 = (w, b, K, dil),
+                      Cin == Cout; c2 = (w2, b2, K2, dil2) Conv1d [Cout][Cout][K2]; the epilogue fields are c2's.
+                      An error when the pair launch is not taken.                                                */
+  const float* w2; const float* b2; int K2, dil2;
+} agpt_tapconv_probe_args;
+/* ran = what actually launched: {1 tensor-core | 0 fp32-FMA, tile width BN, tile height MT, 1 plane-fed}.
+ * Synchronises `stream` before returning.                                                                   */
+int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream);
 
 /* ------------------------------------------------------------------ HiFi-GAN
  * Replaces HifiGanGenerator.__init__/forward/remove_weight_norm

@@ -177,3 +177,17 @@ def test_cpu_tensor_raises():
     m = HifiGanGenerator(specs.HIFIGAN_SMALL)
     with pytest.raises(RuntimeError):
         m(torch.zeros(1, 80, 4))
+
+
+def test_odd_upsample_kernel_minus_rate_is_rejected():
+    """ConvTranspose1d(k, u, padding=(k-u)//2) gives L*u + 1 samples when k - u is odd; the engine's polyphase stage
+    computes exactly L*u, so such a config must fail at create instead of returning a waveform that is not the
+    reference's"""
+    from oracle import hifigan_ref as hr
+    h = dict(specs.HIFIGAN_SMALL, upsample_kernel_sizes=[16, 16, 4, 5])
+    mel = specs.synth_tensor((1, 80, 6), seed=3)
+    ref = hr.hifigan_forward(specs.synth_hifigan(h, 1234), h, mel)
+    assert ref.shape[-1] != 6 * 256                      # what the engine would silently disagree with
+    m = build(h, 1234)
+    with pytest.raises(RuntimeError, match="even k - u"):
+        m(mel.cuda())

@@ -377,3 +377,22 @@ def test_bench_reference_arm_contract():
     r1 = subprocess.run([sys.executable, os.path.join(root, "bench.py"), "--impl", "reference", "--steps", "1", "--warmup", "1"],
                         capture_output=True, text=True, timeout=120, env=env, cwd=root)
     assert r1.returncode == 0 and r1.stdout.strip() == ""
+
+
+def test_tapconv_probe_args_mirror_the_header():
+    """_lib.TapconvProbeArgs has the fields of agpt_tapconv_probe_args in the header's order and C types (a mismatch
+    would hand the probe shifted launch parameters)."""
+    from audiogpt_b200 import _lib
+    hdr = re.sub(r"/\*.*?\*/", " ", open(os.path.join(ROOT, "include", "agpt_b200.h")).read(), flags=re.S)
+    body = re.search(r"typedef struct agpt_tapconv_probe_args \{(.*?)\}\s*agpt_tapconv_probe_args;", hdr, re.S).group(1)
+    want = []
+    for decl in filter(str.strip, body.split(";")):
+        decl = decl.replace("const", " ").strip()
+        ptr = "*" in decl
+        t = decl.split()[0]
+        for name in decl.split(None, 1)[1].replace("*", " ").split(","):
+            ct = ctypes.c_void_p if ptr else {"int": ctypes.c_int, "long": ctypes.c_long, "float": ctypes.c_float}[t]
+            want.append((name.strip(), ct))
+    got = [(n, t) for n, t in _lib.TapconvProbeArgs._fields_]
+    assert [t for _, t in got] == [t for _, t in want]
+    assert [n for n, _ in got] == [("inp" if n == "in" else n) for n, _ in want]   # `in` is a Python keyword
