@@ -16,6 +16,7 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.modules.fastspeech.fs2.FastSpeech2                (installed with install(front_end=True))
     audiogpt_b200.modules.diffsinger_midi.fs2.FastSpeech2MIDI       (installed with install(front_end=True))
     audiogpt_b200.ldm.modules.encoders.modules.FrozenCLAPEmbedder   (installed with install(text_encoder=True))
+    audiogpt_b200.wav_evaluation.models.CLAPWrapper.CLAPWrapper     (installed with install(scorer=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -49,10 +50,15 @@ _FIRST_STAGE_MAP = {
 _TEXT_ENCODER_MAP = {
     "ldm.modules.encoders.modules": ("audiogpt_b200.ldm.modules.encoders.modules", ["FrozenCLAPEmbedder"]),
 }
+# the CLAP candidate scorer of the text-to-audio tool, grafted only on request (install(scorer=True)); the reference
+# module does not import on torch 2.x, so outside strict mode this is the sys.modules alias
+_SCORER_MAP = {
+    "wav_evaluation.models.CLAPWrapper": ("audiogpt_b200.wav_evaluation.models.CLAPWrapper", ["CLAPWrapper"]),
+}
 
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
-            text_encoder: bool = False):
+            text_encoder: bool = False, scorer: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -72,13 +78,15 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     chain runs on the engine.
     ``text_encoder=True`` also replaces ``ldm.modules.encoders.modules.FrozenCLAPEmbedder``, so the text-to-audio tool's
     conditioning (get_learned_conditioning) runs on the engine too, from token ids to waveform.
+    ``scorer=True`` also replaces ``wav_evaluation.models.CLAPWrapper.CLAPWrapper``, so the import inside
+    T2A.select_best_audio resolves to the drop-in and the candidate scoring runs on the engine.
     Returns the list of patched names."""
     import importlib
     import sys
     import types
     patched = []
     todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}), **(_FIRST_STAGE_MAP if first_stage else {}),
-                **(_TEXT_ENCODER_MAP if text_encoder else {}))
+                **(_TEXT_ENCODER_MAP if text_encoder else {}), **(_SCORER_MAP if scorer else {}))
     for ref_name, (our_name, attrs) in todo.items():
         ours = importlib.import_module(our_name)
         names = attrs if isinstance(attrs, dict) else {a: a for a in attrs}

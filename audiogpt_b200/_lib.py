@@ -76,6 +76,11 @@ class ClapConfig(C.Structure):
         "intermediate_size", "d_proj")] + [("layer_norm_eps", C.c_float), ("proj_layer_norm_eps", C.c_float)]
 
 
+class Cnn14Config(C.Structure):
+    """agpt_cnn14_cfg (a tagged struct in the header, like agpt_clap_cfg; the create entry point takes a plain pointer)."""
+    _fields_ = [(n, C.c_int) for n in ("window_size", "hop_size", "mel_bins", "out_emb", "d_proj")]
+
+
 class TapconvProbeArgs(C.Structure):
     """agpt_tapconv_probe_args (a tagged struct in the header: it carries pointers and floats)."""
     _fields_ = [(n, C.c_int) for n in ("kind", "Cin", "Cout", "K", "dil", "Wreal", "strip_w", "u", "pad", "g")] + [
@@ -145,6 +150,11 @@ PROTOTYPES = {
     "agpt_fs2_decode": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _F, _F, _P, _P, _P, _P, _P, _P, _P]),
     "agpt_clap_create": (_I, [_P, _W, _I, _I, _OUT]),
     "agpt_clap_encode": (_I, [_P, _P, _I, _I, _P, _P]),
+    "agpt_clap_encode_cls": (_I, [_P, _P, _P, _P, _I, _I, _P, _P]),
+    "agpt_clap_similarity": (_I, [_P, _I, _P, _I, _I, _F, _P, _P]),
+    "agpt_cnn14_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_cnn14_set_resample": (_I, [_P, _I, _I, _I, _P, _I]),
+    "agpt_cnn14_embed": (_I, [_P, _P, _L, _I, _P, _P, _P]),
 }
 
 _lock = threading.Lock()

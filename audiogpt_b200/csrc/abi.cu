@@ -313,6 +313,42 @@ int agpt_clap_encode(agpt_handle h, const int* input_ids, int N, int L, float* z
   });
 }
 
+int agpt_clap_encode_cls(agpt_handle h, const int* input_ids, const int* token_type_ids, const int* attention_mask, int N,
+                         int L, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(input_ids && token_type_ids && attention_mask && out, "null argument");
+    clap_encode_cls(as(h, kMagicClap, "clap"), input_ids, token_type_ids, attention_mask, N, L, out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_clap_similarity(const float* a, int Na, const float* t, int Nt, int D, float scale, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(a && t && out, "null argument");
+    clap_similarity(a, Na, t, Nt, D, scale, out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_cnn14_create(const agpt_cnn14_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(cnn14_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_cnn14_set_resample(agpt_handle h, int orig_freq, int new_freq, int width, const float* table_host, int clip_samples) {
+  return guarded([&] {
+    cnn14_set_resample(as(h, kMagicCnn14, "cnn14"), orig_freq, new_freq, width, table_host, clip_samples);
+  });
+}
+
+int agpt_cnn14_embed(agpt_handle h, const float* wav, long n_samples, int B, const int* start_or_tile_host, float* out_emb,
+                     void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(wav && start_or_tile_host && out_emb, "null argument");
+    cnn14_embed(as(h, kMagicCnn14, "cnn14"), wav, n_samples, B, start_or_tile_host, out_emb, (cudaStream_t)stream);
+  });
+}
+
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                        double* out2, double* dbg8_or_null) {
   return guarded([&] {

@@ -138,6 +138,7 @@ constexpr uint32_t kMagicVaeEnc = 0x56414545;   // 'VAEE'
 constexpr uint32_t kMagicPe = 0x50495443;       // 'PITC'
 constexpr uint32_t kMagicFs2 = 0x46533220;      // 'FS2 '
 constexpr uint32_t kMagicClap = 0x434c4150;     // 'CLAP'
+constexpr uint32_t kMagicCnn14 = 0x434e4e45;    // 'CNNE'
 
 // ---- small device functions --------------------------------------------------
 __device__ __forceinline__ float lrelu(float x, float a) { return x > 0.f ? x : a * x; }

@@ -57,6 +57,12 @@ void fs2_decode(Handle* h, int Tm, const int* mel2ph_in, int* mel2ph_out, const 
 
 Handle* clap_create(const agpt_clap_cfg* cfg, const float* const* W, int nW, int device);
 void clap_encode(Handle* h, const int* ids, int N, int L, float* z, cudaStream_t st);
+void clap_encode_cls(Handle* h, const int* ids, const int* type_ids, const int* mask, int N, int L, float* out, cudaStream_t st);
+void clap_similarity(const float* a, int Na, const float* t, int Nt, int D, float scale, float* out, cudaStream_t st);
+
+Handle* cnn14_create(const agpt_cnn14_cfg* cfg, const float* const* W, int nW, int device);
+void cnn14_set_resample(Handle* h, int orig, int nw, int width, const float* table, int clip);
+void cnn14_embed(Handle* h, const float* wav, long n_samples, int B, const int* start_host, float* out, cudaStream_t st);
 
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                    double* out, double* dbg_avg);

@@ -20,6 +20,7 @@ import math
 from collections import OrderedDict
 from typing import Dict, List, Sequence, Tuple
 
+import numpy as np
 import torch
 
 # --------------------------------------------------------------------------
@@ -892,3 +893,169 @@ def synth_clap(cfg, seed: int = 7070):
     """Seeded FrozenCLAPEmbedder weights (synth_state_dict: embedding rows and Linears N(0, 1 / fan_in), LayerNorm
     scales 1 + 0.1 N, biases 0.05 N)."""
     return synth_state_dict(clap_param_shapes(cfg), seed, convtranspose_prefixes=())
+
+
+# ---------------------------------------------------------------------------------------------- CLAP candidate scorer
+# wav_evaluation/models/CLAPWrapper.py: the CLAP model T2A.select_best_audio scores its candidates with
+# (useful_ckpts/CLAP/config.yml).  bert = the text tower's BertConfig (bert-base-uncased: BertConfig() defaults);
+# Projection LayerNorms use nn.LayerNorm's default eps.
+CLAP_SCORER = dict(text_model="bert-base-uncased", text_len=100, transformer_embed_dim=768,
+                   freeze_text_encoder_weights=True, audioenc_name="Cnn14", out_emb=2048, sampling_rate=44100,
+                   duration=9, fmin=50, fmax=14000, n_fft=1028, hop_size=320, mel_bins=64, window_size=1024,
+                   d_proj=1024, temperature=0.003, num_classes=527, batch_size=1024, demo=False,
+                   bert=dict(CLAP_BASE, proj_layer_norm_eps=1e-5))
+# the same audio tower with a CLAP_SMALL-sized BERT (positions for text_len 100 and one longer prompt)
+CLAP_SCORER_SMALL = dict(CLAP_SCORER, transformer_embed_dim=64,
+                         bert=dict(CLAP_SMALL, max_position_embeddings=128, d_proj=1024))
+CNN14_CHANNELS = (64, 128, 256, 512, 1024, 2048)   # conv_block1..6 (audio.py:132-137)
+BN_EPS = 1e-5                                       # nn.BatchNorm2d default
+
+
+def clap_scorer_bert_cfg(cfg):
+    """The agpt_clap_cfg of the scorer's text tower (its Projection is transformer_embed_dim -> d_proj)."""
+    b = dict(cfg["bert"], d_proj=int(cfg["d_proj"]))
+    assert b["hidden_size"] == cfg["transformer_embed_dim"], "transformer_embed_dim must equal the BERT width"
+    return {k: b[k] for k in CLAP_ENGINE_KEYS}
+
+
+def _projection_shapes(s, p, d_in, d_out):
+    s[p + "linear1.weight"] = (d_out, d_in)
+    s[p + "linear2.weight"] = (d_out, d_out)
+    s[p + "layer_norm.weight"] = (d_out,); s[p + "layer_norm.bias"] = (d_out,)
+
+
+def _bn_shapes(s, p, c):
+    for n in ("weight", "bias", "running_mean", "running_var"):
+        s[f"{p}.{n}"] = (c,)
+    s[p + ".num_batches_tracked"] = ()
+
+
+def clap_scorer_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of wav_evaluation.models.clap.CLAP (the checkpoint's "model" dict) in state-dict
+    order: logit_scale, audio_encoder (Cnn14 with torchlibrosa's Spectrogram / LogmelFilterBank, then Projection),
+    caption_encoder (HF BertModel without the position_ids buffer, then Projection).  A 2022 checkpoint also holds
+    caption_encoder.base.embeddings.position_ids, which current transformers no longer registers."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    s["logit_scale"] = ()
+    a = "audio_encoder.base."
+    nb = int(cfg["window_size"]) // 2 + 1
+    s[a + "spectrogram_extractor.stft.conv_real.weight"] = (nb, 1, int(cfg["window_size"]))
+    s[a + "spectrogram_extractor.stft.conv_imag.weight"] = (nb, 1, int(cfg["window_size"]))
+    s[a + "logmel_extractor.melW"] = (nb, int(cfg["mel_bins"]))
+    _bn_shapes(s, a + "bn0", int(cfg["mel_bins"]))
+    cin = 1
+    for i, c in enumerate(CNN14_CHANNELS):
+        p = f"{a}conv_block{i + 1}."
+        s[p + "conv1.weight"] = (c, cin, 3, 3)
+        s[p + "conv2.weight"] = (c, c, 3, 3)
+        _bn_shapes(s, p + "bn1", c)
+        _bn_shapes(s, p + "bn2", c)
+        cin = c
+    E = int(cfg["out_emb"])
+    s[a + "fc1.weight"] = (E, cin); s[a + "fc1.bias"] = (E,)
+    s[a + "fc_audioset.weight"] = (int(cfg["num_classes"]), E); s[a + "fc_audioset.bias"] = (int(cfg["num_classes"]),)
+    _projection_shapes(s, "audio_encoder.projection.", E, int(cfg["d_proj"]))
+    for k, v in clap_param_shapes(clap_scorer_bert_cfg(cfg)).items():
+        s[k] = v
+    return s
+
+
+def cnn14_engine_keys(cfg):
+    """The audio-tower keys agpt_cnn14_create consumes, in its order: the clap_scorer_param_shapes order without
+    fc_audioset (the scorer never uses clipwise_output) and num_batches_tracked."""
+    return [k for k in clap_scorer_param_shapes(cfg) if k.startswith("audio_encoder.")
+            and ".fc_audioset." not in k and not k.endswith("num_batches_tracked")]
+
+
+def sinc_resample_kernel(orig_freq: int, new_freq: int, lowpass_filter_width: int = 6, rolloff: float = 0.99):
+    """torchaudio.transforms.Resample(orig_freq, new_freq)'s polyphase filter at its defaults (sinc_interp_hann),
+    restated from torchaudio.functional.functional._get_sinc_resample_kernel: returns (kernel [new][2 width + orig]
+    fp32, width, orig, new), the rates reduced by their gcd.  Output sample k * new + p is
+    sum_j kernel[p][j] * x[k * orig + j - width] (zero outside the clip); there are ceil(new * L / orig) of them."""
+    g = math.gcd(int(orig_freq), int(new_freq))
+    orig, new = int(orig_freq) // g, int(new_freq) // g
+    base = min(orig, new) * rolloff
+    width = math.ceil(lowpass_filter_width * orig / base)
+    idx = torch.arange(-width, width + orig, dtype=torch.float64)[None, None] / orig
+    t = torch.arange(0, -new, -1)[:, None, None] / new + idx
+    t *= base
+    t = t.clamp_(-lowpass_filter_width, lowpass_filter_width)
+    window = torch.cos(t * math.pi / lowpass_filter_width / 2) ** 2
+    t *= math.pi
+    kernels = torch.where(t == 0, torch.tensor(1.0).to(t), t.sin() / t)
+    kernels *= window * (base / orig)
+    return kernels.to(torch.float32)[:, 0], width, orig, new
+
+
+def stft_dft_weights(n_fft: int):
+    """torchlibrosa STFT's conv_real / conv_imag weights [n_fft/2 + 1][1][n_fft]: the DFT rows exp(-2 pi i k n / N)
+    times the periodic Hann window (librosa get_window('hann', fftbins=True))."""
+    n = np.arange(n_fft)
+    win = 0.5 - 0.5 * np.cos(2 * np.pi * n / n_fft)
+    k = np.arange(n_fft // 2 + 1)
+    ph = 2 * np.pi * ((k[:, None] * n[None, :]) % n_fft) / n_fft
+    real = np.cos(ph) * win[None, :]
+    imag = -np.sin(ph) * win[None, :]
+    return (torch.from_numpy(real.astype(np.float32))[:, None, :], torch.from_numpy(imag.astype(np.float32))[:, None, :])
+
+
+def slaney_mel(sr: float, n_fft: int, n_mels: int, fmin: float, fmax: float) -> np.ndarray:
+    """librosa.filters.mel(sr=sr, n_fft=n_fft, n_mels=n_mels, fmin=fmin, fmax=fmax) (Slaney scale and area
+    normalisation, its defaults) restated in numpy: [n_mels][n_fft/2 + 1] fp32."""
+    f_sp, min_log_hz, min_log_mel, logstep = 200.0 / 3, 1000.0, 15.0, math.log(6.4) / 27.0
+
+    def hz_to_mel(f):
+        f = np.asanyarray(f, dtype=np.float64)
+        return np.where(f >= min_log_hz, min_log_mel + np.log(np.maximum(f, 1e-10) / min_log_hz) / logstep, f / f_sp)
+
+    def mel_to_hz(m):
+        return np.where(m >= min_log_mel, min_log_hz * np.exp(logstep * (m - min_log_mel)), f_sp * m)
+
+    fftfreqs = np.fft.rfftfreq(n=n_fft, d=1.0 / sr)
+    mel_f = mel_to_hz(np.linspace(hz_to_mel(fmin), hz_to_mel(fmax), n_mels + 2))
+    fdiff = np.diff(mel_f)
+    ramps = np.subtract.outer(mel_f, fftfreqs)
+    w = np.zeros((n_mels, len(fftfreqs)))
+    for i in range(n_mels):
+        w[i] = np.maximum(0, np.minimum(-ramps[i] / fdiff[i], ramps[i + 2] / fdiff[i + 1]))
+    w *= (2.0 / (mel_f[2:n_mels + 2] - mel_f[:n_mels]))[:, None]
+    return w.astype(np.float32)
+
+
+def synth_clap_scorer(cfg, seed: int = 9090):
+    """Seeded CLAP scorer weights in the checkpoint's layout (synth_state_dict draws, then): the real periodic-Hann DFT
+    rows and Slaney mel matrix of the config; convs and fc1 at He gain; BatchNorm running statistics with positive
+    variance (bn0's centred on the log-mel range of a speech-level clip), so log-mels and activations keep O(1)
+    magnitudes through the 12 convs; logit_scale = log(1 / 0.07) as CLAP initialises it."""
+    shapes = clap_scorer_param_shapes(cfg)
+    sd = synth_state_dict(shapes, seed, convtranspose_prefixes=(),
+                          gains={"audio_encoder.base.conv_block": math.sqrt(2.0), "audio_encoder.base.fc1": math.sqrt(2.0)})
+    a = "audio_encoder.base."
+    sd[a + "spectrogram_extractor.stft.conv_real.weight"], sd[a + "spectrogram_extractor.stft.conv_imag.weight"] = \
+        stft_dft_weights(int(cfg["window_size"]))
+    sd[a + "logmel_extractor.melW"] = torch.from_numpy(np.ascontiguousarray(slaney_mel(
+        cfg["sampling_rate"], cfg["window_size"], cfg["mel_bins"], cfg["fmin"], cfg["fmax"]).T))
+    g = torch.Generator().manual_seed(int(seed) + 1)
+    for k, shape in shapes.items():
+        if k.endswith("num_batches_tracked"):
+            sd[k] = torch.tensor(0, dtype=torch.long)
+        elif k.endswith("running_mean"):
+            sd[k] = (-5.0 + 3.0 * torch.randn(shape, generator=g)) if k.startswith(a + "bn0") else 0.1 * torch.randn(shape, generator=g)
+        elif k.endswith("running_var"):
+            sd[k] = (100.0 if k.startswith(a + "bn0") else 1.0) * (0.5 + torch.rand(shape, generator=g))
+    sd["logit_scale"] = torch.tensor(math.log(1 / 0.07), dtype=torch.float32)
+    return sd
+
+
+def synth_scorer_clips(lens=(159744, 40000, 159744), sr: int = 16000, seed: int = 31):
+    """Seeded mono test clips for the scorer (float32 numpy, one per length): a few sines with a slow amplitude
+    envelope plus noise, different in every clip.  The default lengths are T2A's candidates (80 x 624 mel frames at
+    hop 256: cropped) and a short clip (tiled)."""
+    rs = np.random.RandomState(int(seed))
+    clips = []
+    for i, n in enumerate(lens):
+        t = np.arange(int(n)) / sr
+        x = sum(0.2 / (j + 1) * np.sin(2 * np.pi * rs.uniform(80, 4000) * t + rs.uniform(0, 6)) for j in range(4 + 2 * i))
+        x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.5, 3) * t)) + 0.02 * (i + 1) * rs.randn(int(n))
+        clips.append(x.astype(np.float32))
+    return clips

@@ -385,6 +385,46 @@ int agpt_clap_create(const agpt_clap_cfg* cfg, const float* const* host_weights,
  * [0, vocab_size) are clamped to it (callers are expected to reject them first).                                  */
 int agpt_clap_encode(agpt_handle h, const int* input_ids, int N, int L, float* z, void* stream);
 
+/* ------------------------------------------------------------------ CLAP candidate scorer
+ * Replaces the arithmetic of wav_evaluation.models.CLAPWrapper (text_to_audio/Make_An_Audio/wav_evaluation/models/
+ * CLAPWrapper.py:119-215, clap.py, audio.py:107-179): get_text_embeddings / get_audio_embeddings / compute_similarity,
+ * with which T2A.select_best_audio (audio-chatgpt.py:185-199) picks the best of its candidate clips.
+ *
+ * Text tower: an agpt_clap_create handle built from the scorer checkpoint's caption_encoder.* weights.  BERT is
+ * called with token_type_ids and attention_mask (padding keys masked out); only the [CLS] row goes through the
+ * Projection.  input_ids / token_type_ids / attention_mask [N][L] int32 (device); ids and type ids outside the tables
+ * are clamped (callers are expected to reject them first).  out [N][d_proj] (device): the embedding divided by its
+ * norm twice, as the reference does.  The plain agpt_clap_encode path is unchanged.                              */
+int agpt_clap_encode_cls(agpt_handle h, const int* input_ids, const int* token_type_ids, const int* attention_mask, int N,
+                         int L, float* out, void* stream);
+/* out [Na][Nt] = scale * a t^T (a [Na][D], t [Nt][D], device; fp32 FMA dots): compute_similarity's (t @ a.T).T, scale
+ * = logit_scale.exp() or 1 (use_logit_scale=False).                                                               */
+int agpt_clap_similarity(const float* a, int Na, const float* t, int Nt, int D, float scale, float* out, void* stream);
+
+/* Audio tower: Cnn14 (torchlibrosa Spectrogram n_fft = win = window_size, hop_size, periodic Hann, center + reflect,
+ * power 2; LogmelFilterBank ref 1, amin 1e-10, no top_db; bn0; six ConvBlocks 1 -> 64 -> ... -> 2048 with 2x2 average
+ * pools after blocks 1-5; mean over mel, max + mean over time; relu(fc1)) and the audio Projection, eval mode.
+ * A tagged struct, as agpt_clap_cfg.                                                                            */
+typedef struct agpt_cnn14_cfg {
+  int window_size;   /* 1024 */
+  int hop_size;      /* 320 */
+  int mel_bins;      /* 64 (Cnn14's bn0 is BatchNorm2d(64)) */
+  int out_emb;       /* 2048: fc1's width */
+  int d_proj;        /* 1024 */
+} agpt_cnn14_cfg;
+/* host_weights: fp32 HOST arrays in the key order of audiogpt_b200.specs.cnn14_engine_keys(cfg): the checkpoint's
+ * audio_encoder.* keys without fc_audioset.* and num_batches_tracked.  BatchNorms are folded (eps 1e-5).          */
+int agpt_cnn14_create(const agpt_cnn14_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* The resampler and clip length of the following agpt_cnn14_embed calls: torchaudio.transforms.Resample's polyphase
+ * filter table_host [new_freq][2 width + orig_freq] (HOST, rates reduced by their gcd; 1 / 1 / 0 with the table {1}
+ * is no resampling) and clip_samples = duration * the INPUT rate (resample_and_duration's target length).          */
+int agpt_cnn14_set_resample(agpt_handle h, int orig_freq, int new_freq, int width, const float* table_host, int clip_samples);
+/* wav [B][n_samples] (device, at the input rate) -> out_emb [B][d_proj] (device): resampled (R = ceil(new * n /
+ * orig) samples), fitted to clip_samples -- start_or_tile_host[b] (HOST) is the crop start in [0, R - clip) when R >
+ * clip, and -1 (tile: repeat, then cut) otherwise -- then Cnn14, Projection and the two L2 normalisations.        */
+int agpt_cnn14_embed(agpt_handle h, const float* wav, long n_samples, int B, const int* start_or_tile_host, float* out_emb,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif
