@@ -340,6 +340,7 @@ struct Hifigan : Handle {
   bool fuse_resblock = true;        // AGPT_FUSE_RESBLOCK=0: every ResBlock1 conv as its own launch
   bool tall_tiles = true;           // AGPT_TALL_TILES=0: 128-row tiles only (TapConvParams::tc_tall)
   bool plane_feed = true;           // AGPT_PLANE_FEED=0: every tap-GEMM converts its fp32 input itself
+  bool pair_dual = true;            // AGPT_PAIR_DUAL=0: no fused pair runs two CTAs per SM (TapConvParams::tc_dual)
 
   ~Hifigan() override {
     if (pin_mel) cudaFreeHost(pin_mel);
@@ -472,6 +473,7 @@ struct Hifigan : Handle {
             const int gq = gview(rb.g1[n]) == gview(rb.g2[n]) ? gview(rb.g1[n]) : 1;
             TapConvParams P1 = conv(rb.c1[n], rb.c1g[n], gq, rb.dil[n], x, A);
             P1.epi = EPI_BIAS;
+            P1.tc_dual = pair_dual;
             feed(P1, C);
             TapConvParams P2 = conv(rb.c2[n], rb.c2g[n], gq, 1, A, dst);
             residual_epi(P2);
@@ -541,6 +543,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   { const char* e = getenv("AGPT_FUSE_RESBLOCK"); h->fuse_resblock = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_TALL_TILES"); h->tall_tiles = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_PLANE_FEED"); h->plane_feed = !(e && e[0] == '0'); }
+  { const char* e = getenv("AGPT_PAIR_DUAL"); h->pair_dual = !(e && e[0] == '0'); }
   WeightCursor wc{W, nW};
   { const float* w = wc.next(); const float* b = wc.next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
   h->ups.resize(nu);

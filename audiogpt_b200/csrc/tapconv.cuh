@@ -80,6 +80,9 @@ struct TapConvParams {
   // slope); with out == nullptr only the plane is written.
   const __half* pi_hi; const __half* pi_lo;
   __half* po_hi; __half* po_lo; float po_slope;
+  // 1: a fused ResBlock pair (tcpair_launch) may run as two 128-row CTAs per SM (tcpair2_kernel); set by the HiFi-GAN
+  // driver unless AGPT_PAIR_DUAL=0.
+  int tc_dual;
 };
 
 __host__ __device__ inline int tc_wv(const TapConvParams& P) { return P.Wreal > 0 ? (P.strips > 0 ? P.strip_w + 2 : P.Wreal + 1) : 0; }
@@ -148,6 +151,8 @@ void* profile_begin_pair(const TapConvParams& c1, const TapConvParams& c2, cudaS
 void profile_end(void* rec, cudaStream_t st);
 void profile_count_tall();            // a tensor-core launch with 256-row tiles (counted while profiling)
 long long profile_tall_launches();
+void profile_count_dual();            // a fused-pair launch with two CTAs per SM (counted while profiling)
+long long profile_dual_launches();
 void profile_count_plane();           // a plane-fed tensor-core launch (counted while profiling)
 long long profile_plane_launches();
 // The variant of the most recent tap-GEMM launch on this host thread, {1 tensor-core | 0 fp32-FMA, tile width, tile

@@ -28,18 +28,22 @@ namespace {
 
 constexpr int MAX_NA = 4, MAX_NW = 8;
 constexpr int kMaxDyn = 227 * 1024 - 256;   // the kernel also has a small static __shared__ block
+// per CTA of tcpair2_kernel: two CTAs, each with its static block and the 1 KB the hardware reserves per CTA, share
+// the SM's 228 KB
+constexpr int kDualDyn = 113 * 1024 - 256;
 
 struct Tc5Smem {
   uint32_t a_hi[MAX_NA], a_lo[MAX_NA], w[MAX_NW], raw[2], rowinfo, rowp, bars, total;
 };
 // pl: a plane-fed tile (the operand buffers' RRA is pl_rows of the tile's rows), which also has the operand buffers'
-// full / empty barriers
-__host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int MT, int RRA, int NA, int NW, int NR, bool pl = false) {
+// full / empty barriers.  raw_pitch: bytes per row of a raw staging buffer (64 fp32 channels; 32 in tcpair2_kernel).
+__host__ __device__ inline void tc5_layout(Tc5Smem& s, int BN, int MT, int RRA, int NA, int NW, int NR, bool pl = false,
+                                           int raw_pitch = 256) {
   uint32_t o = 0;
   for (int i = 0; i < MAX_NA; ++i) { s.a_hi[i] = o; if (i < NA) o += RRA * 128; }
   for (int i = 0; i < MAX_NA; ++i) { s.a_lo[i] = o; if (i < NA) o += RRA * 128; }
   for (int i = 0; i < MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += 2 * BN * 128; }
-  for (int i = 0; i < 2; ++i) { s.raw[i] = o; if (i < NR) o += RRA * 256; }
+  for (int i = 0; i < 2; ++i) { s.raw[i] = o; if (i < NR) o += RRA * raw_pitch; }
   s.rowinfo = o; o += RRA * 4;
   s.rowp = o; o += MT * 4;
   o = (o + 15) & ~15u;
@@ -399,18 +403,21 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_pl_kernel(const __grid_
 // BN >= C); P2's epilogue (EPI_RES / EPI_ACC) writes the output.  The weight producer streams c1's stages, then c2's,
 // through one mbarrier ring.
 // PL: c1's input is plane-fed (as tcconv5_body), and c2's epilogue may write the output's plane.
-template <int BN, int MT, bool PL>
+// HALF: c1's input (Cin <= 64: one chunk) is staged in 32-channel halves of 128-byte rows, P1.tc_nr of them in flight
+// (tcpair2_kernel: two CTAs per SM, where 256-byte staging rows would not fit).
+template <int BN, int MT, bool PL, bool HALF = false>
 __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapConvParams& P2, const CUtensorMap* tmh,
                                             const CUtensorMap* tml) {
   constexpr int NB = tc5_nb(BN), NJ = BN / NB, MB = MT / 128;
   static_assert(MT == TC_ROWS || (MT == TC_TALL && BN <= 64), "tall tiles are for narrow BN");
+  static_assert(!HALF || (MT == TC_ROWS && BN <= 64 && !PL), "half staging is for the 128-row transform path");
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
   const int RRA = P1.R, NA = P1.tc_na, NW = P1.tc_nw, NR = PL ? 0 : P1.tc_nr;
   __shared__ Tc5Smem S;
   if (threadIdx.x == 0) {
     if constexpr (PL) tc5_layout(S, BN, MT, pl_rows(RRA), NA, NW, 0, true);
-    else tc5_layout(S, BN, MT, RRA, NA, NW, NR);
+    else tc5_layout(S, BN, MT, RRA, NA, NW, NR, false, HALF ? 128 : 256);
   }
   __syncthreads();
   uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
@@ -463,7 +470,27 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
       }
       cp_async_commit_();
     };
-    if constexpr (!PL) {
+    // HALF: 32-channel half h of the input rows into raw[rb], 128 bytes per row.  16-byte unit u (4 channels) of row r
+    // sits at slot ((u >> 1) + 4 (u & 1)) ^ 4 ((r >> 2) & 1): the two units of an 8-channel item, and the rows r and
+    // r + 4 that one quarter-warp of the transform reads, fall into different banks
+    auto issue_half = [&](int h, int rb) {
+      uint8_t* dst = smem + S.raw[rb];
+      const int nu = (((P1.Cin + 15) >> 4) << 2) - 8 * h;   // units of this half the MMA k-steps touch
+      for (int idx = xt; idx < RRA * 8; idx += NWK) {
+        const int row = idx >> 3, u = idx & 7;
+        if (u >= nu) continue;
+        const int ch = h * 32 + 4 * u;
+        const int a = rowinfo[row];
+        const bool ok = (a >= 0) && (ch < P1.Cin);
+        const int slot = ((u >> 1) + ((u & 1) << 2)) ^ (((row >> 2) & 1) << 2);
+        cp_async16_zfill(dst + row * 128 + (slot << 4), ok ? (ing + a + ch) : P1.in, ok ? 16u : 0u);
+      }
+      cp_async_commit_();
+    };
+    if constexpr (HALF) {
+      issue_half(0, 0);
+      if (NR == 2) issue_half(1, 1);
+    } else if constexpr (!PL) {
       issue_raw(0, 0);
       if (NR == 2 && nchunks > 1) issue_raw(1, 1);
     }
@@ -533,14 +560,46 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
       const int nq = ((kv + 15) >> 4) << 1;
       if constexpr (PL) {
         mbar_wait(&a_full[buf], (uint32_t)((c / NA) & 1));
-      } else {
+      } else if constexpr (!HALF) {
         if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
         else cp_async_wait_all_();
         named_bar_sync(1, NWK);
       }
       uint8_t* ahi = smem + S.a_hi[buf];
       uint8_t* alo = smem + S.a_lo[buf];
-      if constexpr (!PL) {
+      if constexpr (HALF) {
+      // the chunk's halves: both in flight (NR == 2), or staged one after the other in raw[0]
+      const int nh = (kv + 31) >> 5;
+      for (int h = 0; h < nh; ++h) {
+        if (NR == 2 && h + 1 < nh) asm volatile("cp.async.wait_group 1;" ::: "memory");
+        else cp_async_wait_all_();
+        named_bar_sync(1, NWK);
+        const uint8_t* rawb = smem + S.raw[NR == 2 ? h : 0];
+#pragma unroll 2
+        for (int idx = xt; idx < RRA * 4; idx += NWK) {
+          // a quarter-warp converts items q = 0..3 of rows r and r + 4: its swizzled operand stores hit 8 distinct slots
+          const int row = ((idx >> 5) << 3) + ((idx >> 3) & 3) + (((idx >> 2) & 1) << 2), q = idx & 3, qg = 4 * h + q;
+          if (qg >= nq) continue;
+          const int sw = ((row >> 2) & 1) << 6;
+          const float4 x0 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 128 + ((q * 16) ^ sw)), true, nullptr);
+          const float4 x1 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 128 + ((64 + q * 16) ^ sw)), true, nullptr);
+          uint4 hv, lv;
+          hv.x = split2(x0.x, x0.y, lv.x);
+          hv.y = split2(x0.z, x0.w, lv.y);
+          hv.z = split2(x1.x, x1.y, lv.z);
+          hv.w = split2(x1.z, x1.w, lv.w);
+          const uint32_t o = sw128(row, qg);
+          *reinterpret_cast<uint4*>(ahi + o) = hv;
+          *reinterpret_cast<uint4*>(alo + o) = lv;
+        }
+        if (NR == 1 && h + 1 < nh) {
+          named_bar_sync(1, NWK);          // everyone finished reading raw[0]
+          issue_half(h + 1, 0);
+        }
+      }
+      fence_proxy_async();
+      named_bar_sync(1, NWK);
+      } else if constexpr (!PL) {
       const uint8_t* rawb = smem + S.raw[rb];
 #pragma unroll 2
       for (int idx = xt; idx < RRA * 8; idx += NWK) {
@@ -636,16 +695,19 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
     EpiPre pre[8];
     int pp[8];
     constexpr int nitem = (MT * 8) / NWK;
+    // items whose global reads are issued one block ahead; item i + LA is read once item i is stored.  HALF keeps 1 to
+    // stay within the registers of two CTAs per SM.
+    constexpr int LA = HALF ? 1 : 4;
     const float dsc = P2.tc_descale;
-    auto load_block = [&](int cb) {   // as tcconv5_kernel: items 0..3 one block ahead, a tall tile's 4..7 during the stores
+    auto load_block = [&](int cb) {   // as tcconv5_kernel: items 0..LA-1 one block ahead, the rest during the stores
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int idx = xt + i * NWK;
-        pp[i] = (i < 4 && i < nitem) ? rowp[MT == TC_ROWS ? idx >> 3 : item_row(xt, i)] : -1;
+        pp[i] = (i < LA && i < nitem) ? rowp[MT == TC_ROWS && !HALF ? idx >> 3 : item_row(xt, i)] : -1;
         if (pp[i] >= 0) epi_load(P2, g, pp[i], cb + 4 * (idx & 7), pre[i]);
       }
     };
-    if (MT == TC_ROWS) load_block(0);
+    if (MT == TC_ROWS && !HALF) load_block(0);
     wgmma_wait<0>();
 #pragma unroll
     for (int b = 0; b < MB; ++b)
@@ -669,7 +731,7 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
               make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
         }
       }
-      if (MT == TC_TALL && blk == 0) load_block(0);
+      if ((MT == TC_TALL || HALF) && blk == 0) load_block(0);   // not next to the whole accumulator
       named_bar_sync(1, NWK);
       const int jc = xt & 7;
       const float4 cv = epi_colvec(P2, g, cb + 4 * jc);
@@ -679,10 +741,10 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
         const int row = (idx >> 3) & (MT - 1);
         if (pp[i] >= 0)
           epi_store_cv<PL>(P2, g, pp[i], cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
-        if (i + 4 < nitem) {
-          const int idx4 = idx + 4 * NWK;
-          pp[i + 4] = rowp[item_row(xt, i + 4)];
-          if (pp[i + 4] >= 0) epi_load(P2, g, pp[i + 4], cb + 4 * (idx4 & 7), pre[i + 4]);
+        if (i + LA < nitem) {
+          const int idxa = idx + LA * NWK;
+          pp[i + LA] = rowp[item_row(xt, i + LA)];
+          if (pp[i + LA] >= 0) epi_load(P2, g, pp[i + LA], cb + 4 * (idxa & 7), pre[i + LA]);
         }
       }
       if (cb + 32 < BN) load_block(cb + 32);
@@ -708,6 +770,14 @@ template <int BN, int MT>
 __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_constant__ TapConvParams P1,
                                                                const __grid_constant__ TapConvParams P2) {
   tcpair_body<BN, MT, false>(P1, P2, nullptr, nullptr);
+}
+// The same 128-row pair tile with two CTAs per SM (tcpair_plan_dual): one tile's input load, transform, c1 -> c2
+// hand-off and epilogue run beside the other tile's wgmmas.  Needs <= 112 registers per thread and <= kDualDyn bytes
+// of shared memory.
+template <int BN>
+__global__ void __launch_bounds__(V5_THREADS, 2) tcpair2_kernel(const __grid_constant__ TapConvParams P1,
+                                                                const __grid_constant__ TapConvParams P2) {
+  tcpair_body<BN, TC_ROWS, false, true>(P1, P2, nullptr, nullptr);
 }
 template <int BN, int MT>
 __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_pl_kernel(const __grid_constant__ TapConvParams P1,
@@ -836,6 +906,29 @@ static bool tc5_plan(TapConvParams& P, int BN, int MT, long a_min, int iters, si
   return smem <= (size_t)kMaxDyn;
 }
 
+// Shared-memory plan of tcpair2_kernel for P (c1 of a pair, after tc5_rows) within kDualDyn: operand buffers of at
+// least a_min bytes (c2's resident tile) and the epilogue's staging, the raw input in 32-channel halves of 128-byte rows
+// (both in flight where they fit, else one after the other), and as many weight stages as the rest holds, at least 2.
+// False when it does not fit or c1 has more than one 64-channel chunk.
+static bool tcpair_plan_dual(TapConvParams& P, int BN, long a_min, int iters, size_t& smem) {
+  if (P.tc_chunks_h != 1) return false;
+  const long abytes = 2L * P.R * 128, wbytes = 2L * BN * 128;
+  const int NA = (int)cdiv(std::max(a_min, 2L * TC_ROWS * 128), abytes);
+  if (NA > MAX_NA) return false;
+  for (int NR = cdiv(P.Cin, 32); NR >= 1; --NR) {
+    Tc5Smem S;
+    tc5_layout(S, BN, TC_ROWS, P.R, NA, 2, NR, false, 128);
+    const long spare = (long)kDualDyn - 1024 - S.total;
+    if (spare < 0) continue;
+    const int NW = (int)std::min<long>(std::min<long>(MAX_NW, std::max(2, iters)), 2 + spare / wbytes);
+    tc5_layout(S, BN, TC_ROWS, P.R, NA, NW, NR, false, 128);
+    P.tc_bn = BN; P.tc_na = NA; P.tc_nw = NW; P.tc_nr = NR;
+    smem = (size_t)S.total + 1024;
+    return smem <= (size_t)kDualDyn;
+  }
+  return false;
+}
+
 static void tc5_set_smem_limits() {
   int dev = 0;
   AGPT_CUDA(cudaGetDevice(&dev));
@@ -863,6 +956,10 @@ static void tc5_set_smem_limits() {
   AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
   AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
   AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDualDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDualDyn));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<64>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
   attr_done_dev[dev & 63] = true;
 }
 
@@ -952,20 +1049,32 @@ HTile pick_h_tile(const TapConvParams& P, int sms) {
   return best;
 }
 
-// One launch of tcpair_kernel<BN, MT>; false -- nothing launched -- when it does not fit shared memory.
-static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, cudaStream_t st) {
+// One launch of tcpair_kernel<BN, MT>, or with dual of tcpair2_kernel<BN> (MT = 128); false -- nothing launched -- when
+// it does not fit shared memory, or (dual) the SM does not take two CTAs of it.
+static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, bool dual, cudaStream_t st) {
   const int BN = P1.tc_bn;
   tc5_rows(P1, MT);
   const int span2 = tc5_rows(P2, MT);
   P2.tc_bn = BN;
   size_t smem = 0;
   const long a2bytes = 2L * P2.tc_chunks_h * P2.R * 128;   // c2's hi / lo operand tile, in c1's operand buffers
-  if (!tc5_plan(P1, BN, MT, a2bytes, P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps, smem)) return false;
+  const int iters = P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps;
+  if (dual ? !tcpair_plan_dual(P1, BN, a2bytes, iters, smem) : !tc5_plan(P1, BN, MT, a2bytes, iters, smem)) return false;
   dim3 grid(cdiv(tc_lv(P1), MT - span2), 1, tc_groups(P1));
   tc5_set_smem_limits();
+  if (dual) {
+    int per_sm = 0;
+    AGPT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
+        &per_sm, BN == 64 ? tcpair2_kernel<64> : tcpair2_kernel<32>, V5_THREADS, smem));
+    if (per_sm != 2) return false;
+  }
   void* rec = profile_begin_pair(P1, P2, st);
   tapconv_note_launch(1, BN, MT, P1.pi_hi ? 1 : 0);
-  if (P1.pi_hi) {
+  if (dual) {
+    if (BN == 64) launch_pdl(tcpair2_kernel<64>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+    else launch_pdl(tcpair2_kernel<32>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+    profile_count_dual();
+  } else if (P1.pi_hi) {
     const PlMaps m = pl_tensor_maps(P1);
     if (MT == TC_TALL) {
       if (BN == 64) launch_pdl(tcpair_pl_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
@@ -988,10 +1097,17 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, cudaStream_t 
   return true;
 }
 
+// Two 128-row CTAs per SM (tcpair2_kernel) instead of one 256- or 128-row CTA: the handle allows it
+// (TapConvParams::tc_dual), the pair is narrow (BN <= 64: one 64-channel chunk) and converts its fp32 input.
+static bool tcpair_dual(const TapConvParams& P1) {
+  return P1.tc_dual && P1.tc_bn <= 64 && !P1.pi_hi;
+}
+
 // One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))) (c2's epilogue EPI_RES / EPI_ACC), as one launch of
 // tcpair_kernel: c1's output tile stays in shared memory as c2's operand tile, so the intermediate tensor never
 // reaches HBM.  A tile yields MT - span(c2) output rows (c1 is recomputed on the halo rows of neighbouring tiles);
-// MT = 256 where tc5_tall allows it, else 128.
+// two 128-row CTAs per SM where tcpair_dual allows it and the plan fits, else MT = 256 where tc5_tall allows it, else
+// 128.
 // Returns false -- nothing launched -- when the pair needs more than one co-tile or does not fit shared memory.
 bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (!tcconv_supported(P1) || !P2.w_h) return false;
@@ -999,10 +1115,12 @@ bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (P2.tc_bn != BN || P1.Cout > BN || P2.Cin != P1.Cout || P2.Cout > BN || P1.Wreal || P2.Wreal || P1.strips ||
       P1.G != P2.G || P1.L != P2.L || P1.pro != PRO_LRELU || P2.pro != PRO_LRELU || (P2.epi != EPI_RES && P2.epi != EPI_ACC))
     return false;
+  if (tcpair_dual(P1) && tcpair_try(P1, P2, TC_ROWS, true, st)) return true;
   const int span2 = tc5_rows(P2, TC_TALL);
-  if (tc5_tall(P1, BN, (long)cdiv(tc_lv(P1), TC_TALL - span2) * tc_groups(P1), tc5_sms()) && tcpair_try(P1, P2, TC_TALL, st))
+  if (tc5_tall(P1, BN, (long)cdiv(tc_lv(P1), TC_TALL - span2) * tc_groups(P1), tc5_sms()) &&
+      tcpair_try(P1, P2, TC_TALL, false, st))
     return true;
-  return tcpair_try(P1, P2, TC_ROWS, st);
+  return tcpair_try(P1, P2, TC_ROWS, false, st);
 }
 
 // returns false when the layer has no fp16 image or does not fit the shared-memory budget
