@@ -13,6 +13,7 @@ static std::vector<ProfRec> g_recs;
 static long long g_tall = 0;    // recorded launches that ran 256-row tiles (the dump line has no field for it)
 static long long g_plane = 0;   // recorded launches that were plane-fed (likewise)
 static long long g_dual = 0;    // recorded launches of the two-CTAs-per-SM pair kernel (likewise)
+static long long g_pipe = 0;    // recorded launches of the two-tiles-per-CTA pair kernel (likewise)
 
 bool profile_enabled() { return g_prof; }
 
@@ -24,6 +25,7 @@ void profile_enable(int on) {
     g_tall = 0;
     g_plane = 0;
     g_dual = 0;
+    g_pipe = 0;
   }
 }
 
@@ -37,6 +39,8 @@ void profile_count_plane() { if (g_prof) ++g_plane; }
 long long profile_plane_launches() { return g_plane; }
 void profile_count_dual() { if (g_prof) ++g_dual; }
 long long profile_dual_launches() { return g_dual; }
+void profile_count_pipe() { if (g_prof) ++g_pipe; }
+long long profile_pipe_launches() { return g_pipe; }
 
 // Sums over the records since profile_enable(1): per variant (FMA BN = 128, 64, 32; 3 = wgmma)
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches) {

@@ -83,6 +83,9 @@ struct TapConvParams {
   // 1: a fused ResBlock pair (tcpair_launch) may run as two 128-row CTAs per SM (tcpair2_kernel); set by the HiFi-GAN
   // driver unless AGPT_PAIR_DUAL=0.
   int tc_dual;
+  // 1: a C = 128 fused pair may run on tcpair_pipe_kernel (two tiles in flight per CTA); set by the HiFi-GAN driver
+  // unless AGPT_PAIR_PIPE=0.
+  int tc_pipe;
 };
 
 __host__ __device__ inline int tc_wv(const TapConvParams& P) { return P.Wreal > 0 ? (P.strips > 0 ? P.strip_w + 2 : P.Wreal + 1) : 0; }
@@ -153,6 +156,8 @@ void profile_count_tall();            // a tensor-core launch with 256-row tiles
 long long profile_tall_launches();
 void profile_count_dual();            // a fused-pair launch with two CTAs per SM (counted while profiling)
 long long profile_dual_launches();
+void profile_count_pipe();            // a fused-pair launch of tcpair_pipe_kernel (counted while profiling)
+long long profile_pipe_launches();
 void profile_count_plane();           // a plane-fed tensor-core launch (counted while profiling)
 long long profile_plane_launches();
 // The variant of the most recent tap-GEMM launch on this host thread, {1 tensor-core | 0 fp32-FMA, tile width, tile

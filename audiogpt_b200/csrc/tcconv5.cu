@@ -787,6 +787,261 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_pl_kernel(const __grid_c
   tcpair_body<BN, MT, true>(P1, P2, &tmh, &tml);
 }
 
+// ---- C = 128 fused pairs with two tiles in flight per CTA (tcpair_pipe_kernel) ----
+// tcpair_kernel<128, 128> runs load -> transform -> c1 -> hand-off -> c2 -> epilogue in order, and its 168 registers
+// and 70+ KB operand tiles rule out a second CTA per SM.  This kernel splits the roles instead: warpgroups 0-1 only
+// issue c1's wgmmas, hand c1's accumulator over to c2's operand tile, issue c2's and dump c2's accumulator (x descale)
+// as fp32; warpgroup 2 converts the NEXT tile's input and runs the PREVIOUS tile's epilogue from its dump; warp 12
+// streams the weights through one ring across c1, c2 and the tiles.  Each CTA walks a strided sequence of the pair's
+// tiles with two operand sets used ping-pong; a set's life is input(t) -> c1 operand -> c2 operand -> fp32 dump(t) ->
+// epilogue(t) -> input(t + 2).  Every output row sums the same wgmma products in the same order, and its epilogue
+// runs the same float operations, as in tcpair_kernel<128, 128>: the results are bit-identical.
+// 4 warpgroups: 2 wgmma, 1 data, 1 whose warp 12 streams the weights.  Launched at 128 registers per thread, the
+// warpgroups then rebalance them (setmaxnreg): 2 x 168 (accumulator + hand-off) + 152 (input transform, epilogue) + 24.
+constexpr int PIPE_THREADS = 512;
+constexpr int PIPE_MMA = 256, PIPE_DATA = 128;
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
+// operand set s: [hi chunk 0][hi chunk 1][lo chunk 0][lo chunk 1] of R1 rows x 128 B (c1's input), then c2's tile in
+// the same form with R2 <= R1 rows, then the dump: 4 column blocks of [128 rows][32 fp32] (64 KB <= 512 R1 B)
+struct PipeSmem { uint32_t set[2], w[MAX_NW], bars, total; };
+__host__ __device__ inline void pipe_layout(PipeSmem& s, int R1, int NW) {
+  uint32_t o = 0;
+  for (int i = 0; i < 2; ++i) { s.set[i] = o; o += (uint32_t)R1 * 512; }
+  for (int i = 0; i < MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += 2 * 128 * 128; }
+  s.bars = o; o += (2 * MAX_NW + 4) * 8;
+  s.total = o;
+}
+
+__global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __grid_constant__ TapConvParams P1,
+                                                                      const __grid_constant__ TapConvParams P2) {
+  constexpr int BN = 128, MT = TC_ROWS;
+  extern __shared__ uint8_t smem_raw_[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
+  const int R1 = P1.R, NW = P1.tc_nw;
+  __shared__ PipeSmem S;
+  if (threadIdx.x == 0) pipe_layout(S, R1, NW);
+  __syncthreads();
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
+  uint64_t* w_empty = w_full + MAX_NW;
+  uint64_t* in_full = w_full + 2 * MAX_NW;   // [2] the set holds its tile's c1 operand (data warpgroup -> wgmma)
+  uint64_t* acc_full = in_full + 2;           // [2] the set holds its tile's c2 dump (wgmma -> data warpgroup)
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup-uniform role branches (see tcconv5_kernel)
+  int span2 = 0;
+  for (int t = 0; t < P2.ntaps; ++t) span2 = max(span2, P2.tap_off[t] - P2.lo_al);
+  const int Lv = P1.L, MTO = MT - span2, ntx = (Lv + MTO - 1) / MTO, ntiles = ntx * P1.G;
+  const int nloc = (int)blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;   // this CTA's tiles
+  const int lo = P1.lo_al, nch = P1.tc_chunks_h, total1 = nch * P1.ntaps;
+  const int RR2 = P2.R, nch2 = P2.tc_chunks_h, total2 = nch2 * P2.ntaps;
+  auto tile_of = [&](int k, int& g, int& q0) {   // local tile k -> sample g, first output row q0
+    const int T = (int)blockIdx.x + k * (int)gridDim.x;
+    g = T / ntx;
+    q0 = (T - g * ntx) * MTO;
+  };
+
+  if (tid == 0) {
+    for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], PIPE_MMA / 32); }
+    for (int i = 0; i < 2; ++i) { mbar_init(&in_full[i], PIPE_DATA); mbar_init(&acc_full[i], PIPE_MMA); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg < 2) {
+    // =========================== wgmma warpgroups: rows 64 wg .. 64 wg + 63 of each tile ===========================
+    setmaxnreg_inc<168>();
+    float acc[BN / 2];
+    int it = 0, prev = -1;   // prev: weight stage of the newest wgmma group, released once that group has completed
+    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {   // as tcpair_body
+      for (int t = 0; t < Q.ntaps; ++t, ++it) {
+        const int s = it % NW;
+        mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
+        const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
+        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
+        const uint32_t ws = smem_u32(smem + S.w[s]);
+        fence_acc<BN / 2>(acc);
+        wgmma_fence();
+        for (int k = 0; k < ksteps; ++k) {
+          const uint64_t ko = (uint64_t)((k * 32) >> 4);
+          const uint64_t dwh = make_desc(ws) + ko, dwl = make_desc(ws + BN * 128) + ko;
+          wgmma_n128(acc, dah + ko, dwh);
+          wgmma_n128(acc, dal + ko, dwh);
+          wgmma_n128(acc, dah + ko, dwl);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_acc<BN / 2>(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        prev = s;
+      }
+    };
+    auto drain = [&]() {   // all wgmmas completed, the last weight stage released
+      wgmma_wait<0>();
+      fence_acc<BN / 2>(acc);
+      if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+      prev = -1;
+    };
+    const int r0 = wg * (MT / 2) + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    for (int k = 0; k < nloc; ++k) {
+      int g, q0;
+      tile_of(k, g, q0);
+      const int qa = q0 + P2.lo_al;
+      uint8_t* set = smem + S.set[k & 1];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      mbar_wait(&in_full[k & 1], (uint32_t)((k >> 1) & 1));
+      // c1 over both resident chunks of the input
+      for (int c = 0; c < nch; ++c) {
+        const uint32_t ahi0 = smem_u32(set) + (uint32_t)c * R1 * 128 + (uint32_t)(wg * (MT / 2) - lo) * 128u;
+        mma_taps(P1, ahi0, ahi0 + (uint32_t)nch * R1 * 128, (min(H_KCH, P1.Cin - c * H_KCH) + 15) >> 4);
+      }
+      drain();
+      named_bar_sync(1, PIPE_MMA);             // both warpgroups' c1 wgmmas are done reading the set
+      // c1's epilogue -> c2's operand tile, as tcpair_body
+      const uint32_t lo_part = (uint32_t)nch2 * RR2 * 128;
+      const float dsc1 = P1.tc_descale;
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = 8 * i + c0;
+        const bool cok = col < P2.Cin;
+        float2 bv = make_float2(0.f, 0.f);
+        if (cok && P1.bias) bv = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
+        uint8_t* hi = set + (uint32_t)(col >> 6) * RR2 * 128;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + 8 * h;
+          float v0 = 0.f, v1 = 0.f;
+          if (cok && qa + r >= 0 && qa + r < Lv) {
+            v0 = lrelu(__fadd_rn(__fmul_rn(acc[4 * i + 2 * h], dsc1), bv.x), P2.slope);
+            v1 = lrelu(__fadd_rn(__fmul_rn(acc[4 * i + 2 * h + 1], dsc1), bv.y), P2.slope);
+          }
+          uint32_t l;
+          const uint32_t hw = split2(v0, v1, l);
+          const uint32_t o = sw128(r, (col & 63) >> 3) + (col & 7) * 2;
+          *reinterpret_cast<uint32_t*>(hi + o) = hw;
+          *reinterpret_cast<uint32_t*>(hi + lo_part + o) = l;
+        }
+      }
+      const int zitems = (RR2 - MT) * 8;
+      for (int idx = tid; idx < zitems * 2 * nch2; idx += PIPE_MMA) {
+        const int blk = idx / zitems, u = idx - blk * zitems;
+        *reinterpret_cast<uint4*>(set + (uint32_t)blk * RR2 * 128 + MT * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+      }
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      fence_proxy_async();
+      named_bar_sync(1, PIPE_MMA);
+      // c2 over the resident tile
+      for (int c = 0; c < nch2; ++c) {
+        const uint32_t ahi0 = smem_u32(set) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * (MT / 2) - P2.lo_al) * 128u;
+        mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, P2.Cin - c * H_KCH) + 15) >> 4);
+      }
+      drain();
+      named_bar_sync(1, PIPE_MMA);             // both warpgroups' c2 wgmmas are done reading the set
+      // accumulator x descale -> the set's dump, in tcpair_body's staging layout (one [128][32] block per 32 columns)
+      const float dsc = P2.tc_descale;
+#pragma unroll
+      for (int blk = 0; blk < BN / 32; ++blk) {
+        uint8_t* stg = set + blk * (MT * 128);
+        const float* a = &acc[4 * (blk * 32 / 8)];
+#pragma unroll
+        for (int i8 = 0; i8 < 4; ++i8) {
+          const int col = 8 * i8 + c0;
+          *reinterpret_cast<float2*>(stg + sw128(r0, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
+          *reinterpret_cast<float2*>(stg + sw128(r0 + 8, col >> 2) + (col & 3) * 4) =
+              make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+        }
+      }
+      mbar_arrive(&acc_full[k & 1]);
+    }
+  } else if (wg == 2) {
+    // =========================== data warpgroup: next tile's input, previous tile's epilogue ===========================
+    setmaxnreg_inc<152>();
+    const int dt = tid - PIPE_MMA;
+    auto transform = [&](int k) {   // fp32 rows -> leaky ReLU -> hi / lo operand chunks of set k & 1 (zeros outside)
+      int g, q0;
+      tile_of(k, g, q0);
+      const int rin = q0 + P2.lo_al + lo;   // input row of operand row 0
+      const float* __restrict__ ing = P1.in + g * P1.in_gstride;
+      uint8_t* set = smem + S.set[k & 1];
+      const int items = R1 * nch * 8;       // (row, chunk, 8-channel group)
+#pragma unroll 4
+      for (int idx = dt; idx < items; idx += PIPE_DATA) {
+        const int row = idx / (nch * 8), c = (idx >> 3) % nch, q = idx & 7;
+        const int r = rin + row, ch = c * H_KCH + 8 * q;
+        float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+        if (r >= 0 && r < Lv && ch < P1.Cin) {
+          v0 = ldg_stream(ing + (long)r * P1.in_pitch + ch);
+          v1 = ldg_stream(ing + (long)r * P1.in_pitch + ch + 4);
+        }
+        const float4 x0 = pro_apply5(P1, v0, true, nullptr), x1 = pro_apply5(P1, v1, true, nullptr);
+        uint4 h, l;
+        h.x = split2(x0.x, x0.y, l.x);
+        h.y = split2(x0.z, x0.w, l.y);
+        h.z = split2(x1.x, x1.y, l.z);
+        h.w = split2(x1.z, x1.w, l.w);
+        const uint32_t o = (uint32_t)c * R1 * 128 + sw128(row, q);
+        *reinterpret_cast<uint4*>(set + o) = h;
+        *reinterpret_cast<uint4*>(set + (uint32_t)nch * R1 * 128 + o) = l;
+      }
+      fence_proxy_async();                  // generic-proxy stores -> visible to the wgmma operand reads
+      mbar_arrive(&in_full[k & 1]);
+    };
+    auto epilogue = [&](int k) {   // the set's dump through c2's fused epilogue, as tcpair_body
+      int g, q0;
+      tile_of(k, g, q0);
+      const uint8_t* set = smem + S.set[k & 1];
+      const int jc = dt & 7;
+      for (int blk = 0; blk < BN / 32; ++blk) {
+        const int cb = blk * 32;
+        const uint8_t* stg = set + blk * (MT * 128);
+        const float4 cv = epi_colvec(P2, g, cb + 4 * jc);
+        for (int h = 0; h < 2; ++h) {   // 8 items per block, the global reads of 4 in flight at a time
+          EpiPre pre[4];
+          int pp[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int row = (dt + (4 * h + i) * PIPE_DATA) >> 3;
+            pp[i] = (row < MTO && q0 + row < Lv) ? q0 + row : -1;
+            if (pp[i] >= 0) epi_load(P2, g, pp[i], cb + 4 * jc, pre[i]);
+          }
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int row = (dt + (4 * h + i) * PIPE_DATA) >> 3;
+            if (pp[i] >= 0)
+              epi_store_cv(P2, g, pp[i], cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
+          }
+        }
+      }
+    };
+    if (nloc > 0) transform(0);
+    for (int k = 0; k < nloc; ++k) {
+      if (k + 1 < nloc) transform(k + 1);   // into the set tile k - 1 used; its epilogue is done
+      mbar_wait(&acc_full[k & 1], (uint32_t)((k >> 1) & 1));
+      epilogue(k);
+      named_bar_sync(2, PIPE_DATA);         // every data thread is done reading the dump before transform(k + 2)
+    }
+  } else {
+    setmaxnreg_dec<24>();
+    if (warp != 12 || lane != 0) return;
+    // =========================== weight producer (warp 12): per tile c1's stages, then c2's ===========================
+    const uint32_t bytes = 2u * BN * 128u;
+    int n_it = 0;
+    for (int k = 0; k < nloc; ++k)
+      for (int it = 0; it < total1 + total2; ++it, ++n_it) {
+        const int s = n_it % NW, n = n_it / NW;
+        if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
+        mbar_arrive_expect_tx(&w_full[s], bytes);
+        const uint8_t* src = it < total1 ? reinterpret_cast<const uint8_t*>(P1.w_h) + (size_t)it * bytes
+                                         : reinterpret_cast<const uint8_t*>(P2.w_h) + (size_t)(it - total1) * bytes;
+        bulk_g2s(smem + S.w[s], src, bytes, &w_full[s]);
+      }
+  }
+}
+
 // fp16 hi/lo weight image: [co-tile][chunk64][tap][hi | lo][BN rows x 128 B, SWIZZLE_128B], pre-scaled
 void build_h_image(const PackedConv& pc, const std::vector<float>& h, int BN, float wscale, DevBuf& dst) {
   const int nct = cdiv(pc.Cout, BN), nch = cdiv(pc.Cin, H_KCH), nt = pc.ntaps;
@@ -1097,6 +1352,45 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, bool dual, cu
   return true;
 }
 
+// One launch of tcpair_pipe_kernel: min(tiles, SMs) CTAs, each with two operand sets of 512 R1 bytes (R1: c1's operand
+// rows) and as many 32 KB weight stages as the rest of kMaxDyn holds, at least 2.  False -- nothing launched -- when the
+// handle does not allow it (TapConvParams::tc_pipe), the pair is not 128 -> 128 channels converted from fp32, or the
+// sets and two stages do not fit (c1 with a tap span of about 30 rows or more: k = 11 at dilation 5).
+static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
+  if (!P1.tc_pipe || P1.tc_bn != 128 || P1.Cin != 128 || P1.Cout != 128 || P2.Cout != 128 || P1.pi_hi || P2.po_hi)
+    return false;
+  tc5_rows(P1, TC_ROWS);
+  const int span2 = tc5_rows(P2, TC_ROWS);
+  if (P2.R > P1.R) return false;   // c2's tile lives in c1's operand set
+  const long wbytes = 2L * 128 * 128;
+  PipeSmem S;
+  pipe_layout(S, P1.R, 0);
+  const long spare = (long)kMaxDyn - 1024 - (long)S.total;
+  if (spare < 2 * wbytes) return false;
+  const int iters = P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps;
+  P1.tc_nw = (int)std::min<long>(std::min<long>(MAX_NW, std::max(2, iters)), spare / wbytes);
+  P2.tc_bn = 128;
+  pipe_layout(S, P1.R, P1.tc_nw);
+  const size_t smem = (size_t)S.total + 1024;
+  const long tiles = (long)cdiv(P1.L, TC_ROWS - span2) * P1.G;
+  dim3 grid((unsigned)std::min<long>(tiles, tc5_sms()));
+  int dev = 0;
+  AGPT_CUDA(cudaGetDevice(&dev));
+  static bool attr_done_dev[64] = {false};
+  if (!attr_done_dev[dev & 63]) {
+    AGPT_CUDA(cudaFuncSetAttribute(tcpair_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    attr_done_dev[dev & 63] = true;
+  }
+  void* rec = profile_begin_pair(P1, P2, st);
+  tapconv_note_launch(1, 128, TC_ROWS, 0);
+  launch_pdl(tcpair_pipe_kernel, grid, dim3(PIPE_THREADS), smem, st, P1, P2);
+  profile_count_pipe();
+  profile_end(rec, st);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+  return true;
+}
+
 // Two 128-row CTAs per SM (tcpair2_kernel) instead of one 256- or 128-row CTA: the handle allows it
 // (TapConvParams::tc_dual), the pair is narrow (BN <= 64: one 64-channel chunk) and converts its fp32 input.
 static bool tcpair_dual(const TapConvParams& P1) {
@@ -1106,8 +1400,8 @@ static bool tcpair_dual(const TapConvParams& P1) {
 // One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))) (c2's epilogue EPI_RES / EPI_ACC), as one launch of
 // tcpair_kernel: c1's output tile stays in shared memory as c2's operand tile, so the intermediate tensor never
 // reaches HBM.  A tile yields MT - span(c2) output rows (c1 is recomputed on the halo rows of neighbouring tiles);
-// two 128-row CTAs per SM where tcpair_dual allows it and the plan fits, else MT = 256 where tc5_tall allows it, else
-// 128.
+// two 128-row tiles in flight per CTA where tcpair_pipe_try takes the pair (128 -> 128 channels), else two 128-row
+// CTAs per SM where tcpair_dual allows it and the plan fits, else MT = 256 where tc5_tall allows it, else 128.
 // Returns false -- nothing launched -- when the pair needs more than one co-tile or does not fit shared memory.
 bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (!tcconv_supported(P1) || !P2.w_h) return false;
@@ -1115,6 +1409,7 @@ bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (P2.tc_bn != BN || P1.Cout > BN || P2.Cin != P1.Cout || P2.Cout > BN || P1.Wreal || P2.Wreal || P1.strips ||
       P1.G != P2.G || P1.L != P2.L || P1.pro != PRO_LRELU || P2.pro != PRO_LRELU || (P2.epi != EPI_RES && P2.epi != EPI_ACC))
     return false;
+  if (tcpair_pipe_try(P1, P2, st)) return true;
   if (tcpair_dual(P1) && tcpair_try(P1, P2, TC_ROWS, true, st)) return true;
   const int span2 = tc5_rows(P2, TC_TALL);
   if (tc5_tall(P1, BN, (long)cdiv(tc_lv(P1), TC_TALL - span2) * tc_groups(P1), tc5_sms()) &&

@@ -1,17 +1,21 @@
 """Dev probe: per-layer time table (CUDA events around every tapconv launch) for one model forward.
-usage: layer_profile.py hifigan|diffnet|unet [B]"""
+usage: layer_profile.py hifigan|diffnet|unet [B] [T] [--each]
+--each also lists every launch in issue order (a fused ResBlock pair is one line: epi >= 16, taps and spans of both
+convs summed), so pairs that share a shape but not a dilation can be told apart."""
 import ctypes as C, os, sys, collections
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from audiogpt_b200 import _lib, specs
 L = _lib.lib()
-which = sys.argv[1] if len(sys.argv) > 1 else "hifigan"
-B = int(sys.argv[2]) if len(sys.argv) > 2 else 8
+each = "--each" in sys.argv
+argv = [a for a in sys.argv if a != "--each"]
+which = argv[1] if len(argv) > 1 else "hifigan"
+B = int(argv[2]) if len(argv) > 2 else 8
 if which == "hifigan":
     from audiogpt_b200.modules.hifigan.hifigan import HifiGanGenerator
     h = specs.HIFIGAN_V1
     m = HifiGanGenerator(h); m.load_state_dict(specs.synth_hifigan(h, 1234)); m = m.eval().cuda()
-    T = int(sys.argv[3]) if len(sys.argv) > 3 else 400
+    T = int(argv[3]) if len(argv) > 3 else 400
     x = specs.synth_tensor((B, 80, T), seed=0, scale=2.0, shift=-4.0).cuda()
     run = lambda: m(x)
 elif which == "diffnet":
@@ -36,10 +40,18 @@ n = L.agpt_profile_dump(buf, 1 << 20)
 _lib.check(L.agpt_profile_enable(0))
 agg = collections.OrderedDict()
 tot = 0.0
-for line in buf.value.decode().splitlines():
+lines = buf.value.decode().splitlines()
+for line in lines:
     v, G, Ln, Cin, Cout, nt, span, epi, Wr, ms, fl = line.split()
     key = (int(G), int(Ln), int(Cin), int(Cout), int(nt), int(epi), int(Wr))
     a = agg.setdefault(key, [0, 0.0, 0.0]); a[0] += 1; a[1] += float(ms); a[2] += float(fl); tot += float(ms)
 print(f"{which} B={B}: {tot:.3f} ms in {sum(a[0] for a in agg.values())} tapconv launches")
 for k, a in sorted(agg.items(), key=lambda kv: -kv[1][1]):
     print(f"  G={k[0]:3d} L={k[1]:7d} Cin={k[2]:5d} Cout={k[3]:5d} taps={k[4]:2d} epi={k[5]:2d} W={k[6]:3d}  n={a[0]:3d}  {a[1]*1e3:9.1f} us  {a[1]/tot*100:5.1f}%  {a[2]/a[1]/1e9:7.1f} TF")
+if each:
+    print("every launch in issue order:")
+    for i, line in enumerate(lines):
+        v, G, Ln, Cin, Cout, nt, span, epi, Wr, ms, fl = line.split()
+        kind = "pair" if int(epi) >= 16 else "conv"
+        print(f"  #{i:3d} {kind} G={int(G):3d} L={int(Ln):7d} Cin={int(Cin):5d} Cout={int(Cout):5d} taps={int(nt):2d} "
+              f"span={int(span):3d} epi={int(epi):2d}  {float(ms)*1e3:9.1f} us")
