@@ -17,6 +17,7 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.modules.diffsinger_midi.fs2.FastSpeech2MIDI       (installed with install(front_end=True))
     audiogpt_b200.ldm.modules.encoders.modules.FrozenCLAPEmbedder   (installed with install(text_encoder=True))
     audiogpt_b200.wav_evaluation.models.CLAPWrapper.CLAPWrapper     (installed with install(scorer=True))
+    audiogpt_b200.modules.GenerSpeech.model.generspeech.GenerSpeech (installed with install(tts_ood=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -56,9 +57,14 @@ _SCORER_MAP = {
     "wav_evaluation.models.CLAPWrapper": ("audiogpt_b200.wav_evaluation.models.CLAPWrapper", ["CLAPWrapper"]),
 }
 
+# the out-of-domain TTS tool's acoustic model, grafted only on request (install(tts_ood=True))
+_TTS_OOD_MAP = {
+    "modules.GenerSpeech.model.generspeech": ("audiogpt_b200.modules.GenerSpeech.model.generspeech", ["GenerSpeech"]),
+}
+
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
-            text_encoder: bool = False, scorer: bool = False):
+            text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -80,13 +86,17 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     conditioning (get_learned_conditioning) runs on the engine too, from token ids to waveform.
     ``scorer=True`` also replaces ``wav_evaluation.models.CLAPWrapper.CLAPWrapper``, so the import inside
     T2A.select_best_audio resolves to the drop-in and the candidate scoring runs on the engine.
+    ``tts_ood=True`` also replaces ``modules.GenerSpeech.model.generspeech.GenerSpeech``, so the import in
+    inference/tts/GenerSpeech.py resolves to the drop-in and the TTS_OOD tool's acoustic model and post-flow run on the
+    engine (its HiFi-GAN vocoder is grafted by default).
     Returns the list of patched names."""
     import importlib
     import sys
     import types
     patched = []
     todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}), **(_FIRST_STAGE_MAP if first_stage else {}),
-                **(_TEXT_ENCODER_MAP if text_encoder else {}), **(_SCORER_MAP if scorer else {}))
+                **(_TEXT_ENCODER_MAP if text_encoder else {}), **(_SCORER_MAP if scorer else {}),
+                **(_TTS_OOD_MAP if tts_ood else {}))
     for ref_name, (our_name, attrs) in todo.items():
         ours = importlib.import_module(our_name)
         names = attrs if isinstance(attrs, dict) else {a: a for a in attrs}

@@ -68,6 +68,17 @@ class Fs2Cfg(C.Structure):
         "use_pos_embed", "rel_pos", "pitch_type", "use_energy_embed", "use_midi")]
 
 
+class GsConfig(C.Structure):
+    """agpt_gs_cfg (a tagged struct in the header, like agpt_clap_cfg; the create entry point takes a plain pointer)."""
+    _fields_ = [("fs2", Fs2Cfg)] + [(n, C.c_int) for n in (
+        "n_vq", "glow_hidden", "glow_kernel", "glow_blocks", "glow_layers", "share_wn_layers")]
+
+
+class GsTaps(C.Structure):
+    """agpt_gs_taps (a tagged struct in the header: optional stage outputs of agpt_gs_forward)."""
+    _fields_ = [("mel_pre_flow", C.c_void_p), ("prosody", C.c_void_p * 3), ("vq_idx", C.c_void_p * 3)]
+
+
 class ClapConfig(C.Structure):
     """agpt_clap_cfg: the one config struct with float fields (a tagged struct in the header; the create entry point
     takes it as a plain pointer)."""
@@ -150,6 +161,9 @@ PROTOTYPES = {
     "agpt_fs2_create": (_I, [C.POINTER(Fs2Cfg), _W, _I, _I, _OUT]),
     "agpt_fs2_encode": (_I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _P, _P, _P]),
     "agpt_fs2_decode": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _F, _F, _P, _P, _P, _P, _P, _P, _P]),
+    "agpt_gs_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_gs_encode": (_I, [_P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "agpt_gs_forward": (_I, [_P, _I, _P, _P, _P, _I, _P, _I, _P, _I, _P, _F, _F, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "agpt_clap_create": (_I, [_P, _W, _I, _I, _OUT]),
     "agpt_clap_encode": (_I, [_P, _P, _I, _I, _P, _P]),
     "agpt_clap_encode_cls": (_I, [_P, _P, _P, _P, _I, _I, _P, _P]),

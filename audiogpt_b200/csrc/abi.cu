@@ -301,6 +301,33 @@ int agpt_fs2_decode(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out
   });
 }
 
+int agpt_gs_create(const agpt_gs_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(gs_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_gs_encode(agpt_handle h, const int* txt_tokens, int B, int T_txt, const float* spk_embed, const float* emo_embed, int predict_dur,
+                   float* dur, int* dur_choice, int* mel_len_host, float* spk_out, float* emo_out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(txt_tokens && spk_embed && emo_embed && dur && (!predict_dur || mel_len_host), "null argument");
+    gs_encode(as(h, kMagicGs, "generspeech"), txt_tokens, B, T_txt, spk_embed, emo_embed, predict_dur, dur, dur_choice, mel_len_host,
+              spk_out, emo_out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_gs_forward(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out, const float* ref_mels, int T_ref, const int* ref_mel2ph,
+                    int n_seg_ph, const int* ref_mel2word, int n_seg_word, const float* z, float f0_mean, float f0_std, float* pitch_pred,
+                    float* f0_denorm, float* f0_denorm_pred, int* pitch_coarse, float* decoder_inp, float* ref_prosody, float* mel_out,
+                    const agpt_gs_taps* taps, void* stream) {
+  return guarded([&] {
+    gs_forward(as(h, kMagicGs, "generspeech"), T_mel, mel2ph, mel2ph_out, ref_mels, T_ref, ref_mel2ph, n_seg_ph, ref_mel2word, n_seg_word, z,
+               f0_mean, f0_std, pitch_pred, f0_denorm, f0_denorm_pred, pitch_coarse, decoder_inp, ref_prosody, mel_out, taps,
+               (cudaStream_t)stream);
+  });
+}
+
 int agpt_clap_create(const agpt_clap_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
   return guarded([&] {
     AGPT_CHECK(cfg && host_weights && out, "null argument");

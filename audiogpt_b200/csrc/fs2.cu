@@ -18,127 +18,6 @@ namespace agpt {
 
 namespace {
 
-constexpr int kRelMaxLen = 5000;    // RelPositionalEncoding's table length (positions run backwards from max_len - 1)
-
-// x[b][t] = escale * E[tok] (+ midi_E[pitch_midi] + midi_dur * w + b + slur_E[is_slur]), then the encoder positions:
-// pos_mode 1 = fairseq (x + table[make_positions(tokens)]), 2 = espnet rel_pos (x * sqrt(H) + pe[max(5000, T) - 1 - t]).
-// Also the source masks: nonpad[b][t] = tok != 0, kpm[b][t] = tok == 0.  Grid (T, B); out-of-range ids are clamped.
-__global__ void fs2_embed_kernel(const int* __restrict__ tok, const int* __restrict__ pmidi, const float* __restrict__ mdur,
-                                 const int* __restrict__ slur, const float* __restrict__ E, const float* __restrict__ midiE,
-                                 const float* __restrict__ mdw, const float* __restrict__ mdb, const float* __restrict__ slurE,
-                                 int ntok, float escale, int pos_mode, const float* __restrict__ rel_div, float neg_emb, float xscale,
-                                 float* __restrict__ x, float* __restrict__ nonpad, uint8_t* __restrict__ kpm, int T, int H) {
-  const int t = blockIdx.x, b = blockIdx.y;
-  const long r = (long)b * T + t;
-  const int* tb = tok + (long)b * T;
-  const int id = tb[t];
-  int pos = 0;
-  if (pos_mode == 1 && id != 0) {                        // make_positions: count of non-padding tokens in [0, t]
-    for (int i0 = 0; i0 <= t; i0 += blockDim.x) {
-      const int i = i0 + threadIdx.x;
-      pos += __syncthreads_count(i <= t && tb[i] != 0);
-    }
-  }
-  const int e = min(max(id, 0), ntok - 1);
-  const int pm = pmidi ? min(max(pmidi[r], 0), 299) : 0;
-  const int sl = slur ? min(max(slur[r], 0), 1) : 0;
-  const float md = mdur ? mdur[r] : 0.f;
-  const int half = H / 2;
-  const int relpos = max(kRelMaxLen, T) - 1 - t;
-  for (int c = threadIdx.x; c < H; c += blockDim.x) {
-    float v = __fmul_rn(escale, E[(long)e * H + c]);
-    if (pmidi) v = __fadd_rn(v, midiE[(long)pm * H + c]);
-    if (mdur) v = __fadd_rn(v, __fadd_rn(__fmul_rn(md, mdw[c]), mdb[c]));
-    if (slur) v = __fadd_rn(v, slurE[(long)sl * H + c]);
-    if (pos_mode == 1 && pos != 0 && c < 2 * half) {
-      const int k = c < half ? c : c - half;
-      const float a = (float)pos * expf((float)k * neg_emb);
-      v += c < half ? sinf(a) : cosf(a);
-    } else if (pos_mode == 2) {
-      const float a = __fmul_rn((float)relpos, rel_div[c >> 1]);
-      v = __fadd_rn(__fmul_rn(v, xscale), (c & 1) ? cosf(a) : sinf(a));
-    }
-    x[r * H + c] = v;
-  }
-  if (threadIdx.x == 0) {
-    nonpad[r] = id != 0 ? 1.f : 0.f;
-    kpm[r] = id == 0 ? 1 : 0;
-  }
-}
-
-// FFTBlocks' padding mask from the rows themselves: nonpad[r] = any(x[r] != 0), kpm[r] = !nonpad[r]  (warp per row)
-__global__ void fs2_rowmask_kernel(const float* __restrict__ x, float* __restrict__ nonpad, uint8_t* __restrict__ kpm, long rows, int C) {
-  const long r = (long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (r >= rows) return;
-  const int lane = threadIdx.x & 31;
-  float s = 0.f;
-  for (int c = lane; c < C; c += 32) s += fabsf(x[r * C + c]);
-#pragma unroll
-  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane == 0) { nonpad[r] = s == 0.f ? 0.f : 1.f; kpm[r] = s == 0.f ? 1 : 0; }
-}
-
-// DurationPredictor.inference / LengthRegulator: xs = linear * nonpad -> dur[r]; dur_choice = clamp(round(exp(xs) - 1), 0)
-// (round half to even, as torch.round), zero on padding tokens
-__global__ void fs2_dur_kernel(const float* __restrict__ pred4, const float* __restrict__ nonpad, float* __restrict__ dur,
-                               int* __restrict__ dch, long rows) {
-  for (long r = (long)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (long)gridDim.x * blockDim.x) {
-    const float xs = pred4[r * 4] * nonpad[r];
-    dur[r] = xs;
-    if (dch) dch[r] = nonpad[r] != 0.f ? (int)fmaxf(rintf(expf(xs) - 1.f), 0.f) : 0;
-  }
-}
-// per utterance: inclusive cumsum of the durations, mel_len[b] = total frames
-__global__ void fs2_lr_scan_kernel(const int* __restrict__ dch, int* __restrict__ cum, int* __restrict__ mel_len, int T) {
-  if (threadIdx.x != 0) return;
-  const int b = blockIdx.x;
-  int run = 0;
-  for (int t = 0; t < T; ++t) { run += dch[(long)b * T + t]; cum[(long)b * T + t] = run; }
-  mel_len[b] = run;
-}
-// mel2ph[b][f] = 1 + (the token whose frame range [cum[t-1], cum[t]) holds f), 0 past the utterance's last frame
-__global__ void fs2_lr_fill_kernel(const int* __restrict__ cum, const int* __restrict__ mel_len, int* __restrict__ mel2ph, int B,
-                                   int Tt, int Tm) {
-  const long total = (long)B * Tm;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int b = (int)(i / Tm), f = (int)(i - (long)b * Tm);
-    int v = 0;
-    if (f < mel_len[b]) {
-      const int* c = cum + (long)b * Tt;
-      int lo = 0, hi = Tt - 1;                             // first t with cum[t] > f
-      while (lo < hi) { const int mid = (lo + hi) >> 1; if (c[mid] > f) hi = mid; else lo = mid + 1; }
-      v = lo + 1;
-    }
-    mel2ph[i] = v;
-  }
-}
-// decoder_inp = gather(pad(encoder_out, 1 leading zero row), mel2ph); tgt_nonpad = mel2ph > 0
-__global__ void fs2_gather_kernel(const float* __restrict__ enc, const int* __restrict__ mel2ph, float* __restrict__ out,
-                                  float* __restrict__ tgt, int B, int Tt, int Tm, int H) {
-  const long total = (long)B * Tm * H;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const long r = i / H;
-    const int c = (int)(i - r * H);
-    const int b = (int)(r / Tm);
-    const int m = min(mel2ph[r], Tt);
-    out[i] = m > 0 ? enc[((long)b * Tt + m - 1) * H + c] : 0.f;
-    if (c == 0) tgt[r] = m > 0 ? 1.f : 0.f;
-  }
-}
-
-// utils/pitch_utils.py:22-32 f0_to_coarse, in the fp32 operation order torch applies (numpy constants rounded to fp32)
-__device__ __forceinline__ int f0_coarse(float f0, float mel_min, float mel_range) {
-  float m = __fmul_rn(1127.f, logf(__fadd_rn(1.f, __fdiv_rn(f0, 700.f))));
-  if (m > 0.f) m = __fadd_rn(__fdiv_rn(__fmul_rn(__fsub_rn(m, mel_min), 254.f), mel_range), 1.f);
-  if (m <= 1.f) m = 1.f;
-  if (m > 255.f) m = 255.f;
-  return (int)(m + 0.5f);
-}
-__device__ __forceinline__ float denorm(float f, int norm, float mean, float std_) {
-  if (norm == 1) f = f * std_ + mean;      // 'standard'
-  if (norm == 2) f = exp2f(f);             // 'log': 2 ** f0
-  return f;
-}
 // add_pitch, pitch_type 'frame' (fs2.py:187-220): pitch_pred (channel 0 zeroed on padding frames when it is the f0 used, as
 // the reference's in-place f0[pitch_padding] = 0 does through the view), f0_denorm (uv and padding -> 0), coarse bins
 __global__ void fs2_pitch_frame_kernel(const float* __restrict__ pred4, const int* __restrict__ mel2ph, const float* __restrict__ f0_in,
@@ -204,18 +83,6 @@ unsigned ew_grid(long total) { return (unsigned)std::min<long>(cdivl(total, 256)
 int* iptr(DevBuf& d) { return reinterpret_cast<int*>(d.p); }
 uint8_t* bptr(DevBuf& d) { return reinterpret_cast<uint8_t*>(d.p); }
 
-// EncSALayer (common_layers.py:541-587), norm 'ln', act 'gelu', padding 'SAME'
-struct FftLayer {
-  DevBuf ln1g, ln1b, ln2g, ln2b;
-  PackedConv qkv, out, ffn1, ffn2;
-  int k = 9;
-};
-
-struct FftStack {
-  std::vector<FftLayer> layers;
-  DevBuf lng, lnb;
-};
-
 }  // namespace
 
 struct Fs2Net : Handle {
@@ -224,9 +91,7 @@ struct Fs2Net : Handle {
   FftStack enc, dec;
   float dec_alpha = 1.f;
   PackedConv mel_out;
-  std::vector<PackedConv> dp_conv;
-  std::vector<DevBuf> dp_g, dp_b;
-  PackedConv dp_lin;
+  DurPredictorNet dp;
   PitchPredictorNet pitch_pp, energy_pp;
   // encode -> decode state
   int B = 0, Tt = 0, have_dur = 0;
@@ -234,26 +99,8 @@ struct Fs2Net : Handle {
   // work buffers
   DevBuf x, y, z, qkv, ffn, s[3], pred4, dnp, dkpm, tnp, pos, ebkt;
 
-  // FFTBlocks.forward after the input positions (tts_modules.py:307-332): x * nonpad, layers, last LayerNorm * nonpad.
-  // xs [rows][H] is the work tensor (overwritten), the result goes to out (which may be y); uses y, z, qkv, ffn, which
-  // ensure_work has sized (no buffer may grow once a pointer into it has been taken).
-  void fft(FftStack& S, float* xs, float* out, int B_, int T, const float* nonpad, const uint8_t* kpm, cudaStream_t st) {
-    const int H = cfg.hidden_size, heads = cfg.num_heads;
-    const long rows = (long)B_ * T;
-    fs_affine_mask(xs, nullptr, nullptr, nonpad, rows, H, st);
-    for (auto& L : S.layers) {
-      layernorm(xs, y.p, L.ln1g.p, L.ln1b.p, rows, H, 1e-5f, st);
-      fs_conv(L.qkv, y.p, H, qkv.p, 3 * H, 1, (int)rows, EPI_BIAS, st);
-      attention(qkv.p, 3 * H, qkv.p + H, 3 * H, qkv.p + 2 * H, 3 * H, y.p, H, B_, heads, H / heads, T, T, st, kpm);
-      fs_conv(L.out, y.p, H, z.p, H, 1, (int)rows, EPI_RES, st, xs);                 // residual + attention
-      fs_affine_mask(z.p, nullptr, nullptr, nonpad, rows, H, st);
-      layernorm(z.p, y.p, L.ln2g.p, L.ln2b.p, rows, H, 1e-5f, st);
-      fs_conv(L.ffn1, y.p, H, ffn.p, 4 * H, B_, T, EPI_GELU_SCALED, st, nullptr, (float)std::pow((double)L.k, -0.5));
-      fs_conv(L.ffn2, ffn.p, 4 * H, xs, H, 1, (int)rows, EPI_RES, st, z.p);          // residual + FFN
-      fs_affine_mask(xs, nullptr, nullptr, nonpad, rows, H, st);
-    }
-    layernorm(xs, out, S.lng.p, S.lnb.p, rows, H, 1e-5f, st);
-    fs_affine_mask(out, nullptr, nullptr, nonpad, rows, H, st);
+  void fft(const FftStack& S, float* xs, float* out, int B_, int T, const float* nonpad, const uint8_t* kpm, cudaStream_t st) {
+    S.forward(xs, out, B_, T, cfg.hidden_size, cfg.num_heads, nonpad, kpm, y.p, z.p, qkv.p, ffn.p, st);
   }
 
   void ensure_work(long rows) {
@@ -273,29 +120,15 @@ struct Fs2Net : Handle {
     enc_out.ensure(rows * H); snp.ensure(rows); skpm.ensure(rows / 4 + 1); dch.ensure(rows); cum.ensure(rows); mlen.ensure(B_);
     ensure_work(rows);
     const int pos_mode = cfg.use_pos_embed ? (cfg.rel_pos ? 2 : 1) : 0;
-    fs2_embed_kernel<<<dim3(T, B_), 128, 0, st>>>(tok, cfg.use_midi ? pmidi : nullptr, cfg.use_midi ? mdur : nullptr, cfg.use_midi ? slur : nullptr,
-                                                  E.p, midiE.p, mdw.p, mdb.p, slurE.p, cfg.n_tokens, (float)std::sqrt((double)H), pos_mode,
-                                                  rel_div.p, (float)(-(std::log(10000.0) / (double)(H / 2 - 1))), (float)std::sqrt((double)H),
-                                                  x.p, snp.p, bptr(skpm), T, H);
-    count_launch(1);
+    fs_embed_tokens(tok, cfg.use_midi ? pmidi : nullptr, cfg.use_midi ? mdur : nullptr, cfg.use_midi ? slur : nullptr, E.p, midiE.p, mdw.p,
+                    mdb.p, slurE.p, cfg.n_tokens, (float)std::sqrt((double)H), pos_mode, rel_div.p,
+                    (float)(-(std::log(10000.0) / (double)(H / 2 - 1))), (float)std::sqrt((double)H), x.p, snp.p, bptr(skpm), B_, T, H, st);
     fft(enc, x.p, enc_out.p, B_, T, snp.p, bptr(skpm), st);
-    // ---- DurationPredictor (tts_modules.py:98-112): n x [conv k SAME -> ReLU -> LayerNorm -> x nonpad], Linear -> 1
-    const float* cur = enc_out.p;
-    int cin = H;
-    for (size_t l = 0; l < dp_conv.size(); ++l) {
-      float* o = s[1 + (l & 1)].p;
-      fs_conv(dp_conv[l], cur, cin, s[0].p, P, B_, T, EPI_RELU, st);
-      layernorm(s[0].p, o, dp_g[l].p, dp_b[l].p, rows, P, 1e-5f, st);
-      fs_affine_mask(o, nullptr, nullptr, snp.p, rows, P, st);
-      cur = o;
-      cin = P;
-    }
-    fs_conv(dp_lin, cur, cin, pred4.p, 4, 1, (int)rows, EPI_BIAS, st);
-    fs2_dur_kernel<<<ew_grid(rows), 256, 0, st>>>(pred4.p, snp.p, dur, predict ? iptr(dch) : nullptr, rows);
-    count_launch(1);
+    // ---- DurationPredictor (tts_modules.py:98-112) on the encoder output
+    dp.forward(enc_out.p, H, B_, T, snp.p, s[0].p, s[1].p, s[2].p, pred4.p, st);
+    fs_dur(pred4.p, snp.p, dur, predict ? iptr(dch) : nullptr, rows, st);
     if (predict) {
-      fs2_lr_scan_kernel<<<B_, 32, 0, st>>>(iptr(dch), iptr(cum), iptr(mlen), T);
-      count_launch(1);
+      fs_lr_scan(iptr(dch), iptr(cum), iptr(mlen), B_, T, st);
       if (dur_choice) AGPT_CUDA(cudaMemcpyAsync(dur_choice, dch.p, sizeof(int) * rows, cudaMemcpyDeviceToDevice, st));
       // the one device -> host transfer: the frame count sizes the decoder (the reference syncs on dur.sum(-1).max())
       AGPT_CUDA(cudaMemcpyAsync(mel_len_host, mlen.p, sizeof(int) * B_, cudaMemcpyDeviceToHost, st));
@@ -321,12 +154,10 @@ struct Fs2Net : Handle {
     const int* m2p = mel2ph_in;
     if (!m2p) {
       AGPT_CHECK(mel2ph_out, "mel2ph output required when it is predicted");
-      fs2_lr_fill_kernel<<<ew_grid(rows), 256, 0, st>>>(iptr(cum), iptr(mlen), mel2ph_out, B, Tt, Tm);
-      count_launch(1);
+      fs_lr_fill(iptr(cum), iptr(mlen), mel2ph_out, B, Tt, Tm, st);
       m2p = mel2ph_out;
     }
-    fs2_gather_kernel<<<ew_grid(rows * H), 256, 0, st>>>(enc_out.p, m2p, x.p, tnp.p, B, Tt, Tm, H);
-    count_launch(1);
+    fs_gather(enc_out.p, m2p, x.p, tnp.p, B, Tt, Tm, H, st);
     // pitch_inp = decoder_inp_origin * tgt_nonpad = x (gathered rows are zero where mel2ph == 0)
     const double mmin = 1127.0 * std::log(1.0 + 50.0 / 700.0), mmax = 1127.0 * std::log(1.0 + 1100.0 / 700.0);
     const float mel_min = (float)mmin, mel_range = (float)(mmax - mmin);
@@ -355,8 +186,7 @@ struct Fs2Net : Handle {
     count_launch(1);
     if (!mel) { AGPT_CUDA(cudaGetLastError()); return; }        // skip_decoder
     // ---- FastspeechDecoder: padding mask and positions from decoder_inp itself (tts_modules.py:313-318)
-    fs2_rowmask_kernel<<<(unsigned)cdivl(rows, 8), 256, 0, st>>>(dec_inp, dnp.p, bptr(dkpm), rows, H);
-    count_launch(1);
+    fs_rowmask(dec_inp, dnp.p, bptr(dkpm), rows, H, st);
     fs_positions(dec_inp, iptr(pos), B, Tm, H, st);
     fs_posemb_add(dec_inp, x.p, iptr(pos), dec_alpha, rows, H, st);
     fft(dec, x.p, y.p, B, Tm, dnp.p, bptr(dkpm), st);
@@ -365,22 +195,6 @@ struct Fs2Net : Handle {
     AGPT_CUDA(cudaGetLastError());
   }
 };
-
-namespace {
-void load_stack(FftStack& S, WeightCursor& wc, int H, int L, int k) {
-  S.layers.resize(L);
-  for (auto& l : S.layers) {
-    l.k = k;
-    { auto g = wc.next(); auto b = wc.next(); l.ln1g.upload(g, H); l.ln1b.upload(b, H); }
-    pack_conv(l.qkv, wc.next(), nullptr, 3 * H, H, 1, false);        // in_proj_weight [3H][H], no bias
-    pack_conv(l.out, wc.next(), nullptr, H, H, 1, false);            // out_proj.weight, no bias
-    { auto g = wc.next(); auto b = wc.next(); l.ln2g.upload(g, H); l.ln2b.upload(b, H); }
-    { auto w = wc.next(); auto b = wc.next(); pack_conv(l.ffn1, w, b, 4 * H, H, k, false); }
-    { auto w = wc.next(); auto b = wc.next(); pack_conv(l.ffn2, w, b, H, 4 * H, 1, false); }
-  }
-  { auto g = wc.next(); auto b = wc.next(); S.lng.upload(g, H); S.lnb.upload(b, H); }
-}
-}  // namespace
 
 Handle* fs2_create(const agpt_fs2_cfg* cfg, const float* const* W, int nW, int device) {
   DeviceGuard dg_(device);
@@ -396,25 +210,12 @@ Handle* fs2_create(const agpt_fs2_cfg* cfg, const float* const* W, int nW, int d
   h->E.upload(wc.next(), (size_t)cfg->n_tokens * H);                // encoder_embed_tokens.weight
   wc.next();                                                      // encoder.embed_tokens.weight (the same tensor)
   if (!cfg->rel_pos) wc.next();                                   // encoder.embed_positions._float_tensor
-  load_stack(h->enc, wc, H, cfg->enc_layers, cfg->enc_ffn_kernel);
+  h->enc.load(wc, H, cfg->enc_layers, cfg->enc_ffn_kernel);
   h->dec_alpha = wc.next()[0];                                    // decoder.pos_embed_alpha
   wc.next();                                                      // decoder.embed_positions._float_tensor
-  load_stack(h->dec, wc, H, cfg->dec_layers, cfg->dec_ffn_kernel);
+  h->dec.load(wc, H, cfg->dec_layers, cfg->dec_ffn_kernel);
   { auto w = wc.next(); auto b = wc.next(); pack_conv(h->mel_out, w, b, cfg->out_dims, H, 1, false); }
-  h->dp_conv.resize(cfg->dur_predictor_layers); h->dp_g.resize(cfg->dur_predictor_layers); h->dp_b.resize(cfg->dur_predictor_layers);
-  int cin = H;
-  for (int l = 0; l < cfg->dur_predictor_layers; ++l) {
-    { auto w = wc.next(); auto b = wc.next(); pack_conv(h->dp_conv[l], w, b, P, cin, cfg->dur_predictor_kernel, false); }
-    { auto g = wc.next(); auto b = wc.next(); h->dp_g[l].upload(g, P); h->dp_b[l].upload(b, P); }
-    cin = P;
-  }
-  {  // Linear(P -> 1) padded to 4 output channels
-    auto w = wc.next(); auto b = wc.next();
-    std::vector<float> wp((size_t)4 * P, 0.f), bp(4, 0.f);
-    memcpy(wp.data(), w, sizeof(float) * P);
-    bp[0] = b[0];
-    pack_conv(h->dp_lin, wp.data(), bp.data(), 4, P, 1, false);
-  }
+  h->dp.load(wc, H, P, cfg->dur_predictor_kernel, cfg->dur_predictor_layers);
   if (cfg->pitch_type) {
     h->pitchE.upload(wc.next(), (size_t)300 * H);
     h->pitch_pp.load(wc, H, P, cfg->predictor_kernel, cfg->predictor_layers, cfg->pitch_type == 1 ? 2 : 1);

@@ -55,6 +55,13 @@ void fs2_decode(Handle* h, int Tm, const int* mel2ph_in, int* mel2ph_out, const 
                 int norm, float f0_mean, float f0_std, float* pitch_pred, float* f0d, int* coarse, float* e_pred, float* dec_inp, float* mel,
                 cudaStream_t st);
 
+Handle* gs_create(const agpt_gs_cfg* cfg, const float* const* W, int nW, int device);
+void gs_encode(Handle* h, const int* tok, int B, int T, const float* spk, const float* emo, int predict, float* dur, int* dur_choice,
+               int* mel_len_host, float* spk_out, float* emo_out, cudaStream_t st);
+void gs_forward(Handle* h, int Tm, const int* mel2ph, int* mel2ph_out, const float* ref_mels, int Tr, const int* ref_mel2ph, int nseg_ph,
+                const int* ref_mel2word, int nseg_word, const float* z, float f0_mean, float f0_std, float* pitch_pred, float* f0d,
+                float* f0d_pred, int* coarse, float* dec_inp, float* ref_prosody, float* mel, const agpt_gs_taps* taps, cudaStream_t st);
+
 Handle* clap_create(const agpt_clap_cfg* cfg, const float* const* W, int nW, int device);
 void clap_encode(Handle* h, const int* ids, int N, int L, float* z, cudaStream_t st);
 void clap_encode_cls(Handle* h, const int* ids, const int* type_ids, const int* mask, int N, int L, float* out, cudaStream_t st);

@@ -847,6 +847,187 @@ def synth_fs2_inputs(cfg, B, T, seed):
     return out
 
 
+# ---------------------------------------------------------------------------------------------- GenerSpeech
+# NeuralSeq/modules/GenerSpeech/config/generspeech.yaml over egs/egs_bases/tts/fs2.yaml: the FS2_C2 front-end plus three
+# LocalStyleAdaptors (128 VQ codes), three ProsodyAligners and an 8-block Glow post-flow (hidden 128, k 3, 3 layers,
+# in_layers / res_skip_layers shared by blocks 0-3 and 4-7)
+GS_C2 = dict(FS2_C2, n_vq=128, glow_hidden=128, glow_kernel=3, glow_blocks=8, glow_layers=3, share_wn_layers=4)
+# same topology, narrower: hidden 64 (aligner head dim 32), 16 codes, a 4-block post-flow of hidden 32
+GS_SMALL = dict(FS2_SMALL, use_energy_embed=0, n_vq=16, glow_hidden=32, glow_kernel=3, glow_blocks=4, glow_layers=2,
+                share_wn_layers=2)
+GS_LEVELS = ("utter", "ph", "word")
+GS_STYLE_C = 80          # LocalStyleAdaptor: WN / ConvBlocks width (prosody_util.py:175-178)
+GS_ALIGN_FFN = 2048      # CrossAttenLayer dim_feedforward
+
+
+def _wn_shapes(s, p, hid, k, layers, gin):
+    """modules/GenerSpeech/model/wavenet.py WN with weight norm (bias, weight_g, weight_v per conv)"""
+    for i in range(layers):
+        s[f"{p}.in_layers.{i}.bias"] = (2 * hid,)
+        s[f"{p}.in_layers.{i}.weight_g"] = (2 * hid, 1, 1)
+        s[f"{p}.in_layers.{i}.weight_v"] = (2 * hid, hid, k)
+    for i in range(layers):
+        rc = 2 * hid if i < layers - 1 else hid
+        s[f"{p}.res_skip_layers.{i}.bias"] = (rc,)
+        s[f"{p}.res_skip_layers.{i}.weight_g"] = (rc, 1, 1)
+        s[f"{p}.res_skip_layers.{i}.weight_v"] = (rc, hid, 1)
+    if gin:
+        s[f"{p}.cond_layer.bias"] = (2 * hid * layers,)
+        s[f"{p}.cond_layer.weight_g"] = (2 * hid * layers, 1, 1)
+        s[f"{p}.cond_layer.weight_v"] = (2 * hid * layers, gin, 1)
+
+
+def gs_glow_cond_channels(cfg):
+    """channels of the post-flow conditioning g = cat[mel_out, decoder_inp, spk, emo, ref_prosody] (generspeech.py:58-62)"""
+    return int(cfg["out_dims"]) + 4 * int(cfg["hidden_size"])
+
+
+def generspeech_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of NeuralSeq/modules/GenerSpeech/model/generspeech.py GenerSpeech: the FastSpeech2 keys
+    (fs2_param_shapes, with spk_embed_proj), MixStyle's affine layer (unused at inference), the three LocalStyleAdaptors
+    (ConvBlocks, VQEmbeddingEMA buffers, a weight-normed WN whose cond_layer is unused), l1_* and ProsodyAligners, the
+    pitch inpainter, and the Glow post-flow.  Tensors a coupling block shares with the block that owns them (its WN
+    in_layers / res_skip_layers) appear under every name, as in the reference's state dict."""
+    s = fs2_param_shapes(cfg)
+    H, C, k = int(cfg["hidden_size"]), GS_STYLE_C, int(cfg["predictor_kernel"])
+    s["spk_embed_proj.weight"] = (H, 256); s["spk_embed_proj.bias"] = (H,)
+    s["norm.affine_layer.linear_layer.weight"] = (2 * H, H); s["norm.affine_layer.linear_layer.bias"] = (2 * H,)
+    s["emo_embed_proj.weight"] = (H, 256); s["emo_embed_proj.bias"] = (H,)
+    for lvl in GS_LEVELS:
+        p = f"prosody_extractor_{lvl}"
+        for r in range(5):
+            for j in range(2):
+                q = f"{p}.encoder.res_blocks.{r}.blocks.{j}"
+                s[f"{q}.0.weight"] = (C,); s[f"{q}.0.bias"] = (C,)
+                s[f"{q}.1.weight"] = (2 * C, C, 5); s[f"{q}.1.bias"] = (2 * C,)
+                s[f"{q}.4.weight"] = (C, 2 * C, 1); s[f"{q}.4.bias"] = (C,)
+        s[f"{p}.encoder.last_norm.weight"] = (C,); s[f"{p}.encoder.last_norm.bias"] = (C,)
+        s[f"{p}.encoder.post_net1.weight"] = (H, C, 3); s[f"{p}.encoder.post_net1.bias"] = (H,)
+        n = int(cfg["n_vq"])
+        s[f"{p}.vqvae.data_initialized"] = (1,)
+        s[f"{p}.vqvae.embedding"] = (n, H); s[f"{p}.vqvae.ema_count"] = (n,); s[f"{p}.vqvae.ema_weight"] = (n, H)
+        _wn_shapes(s, f"{p}.wavenet", C, 3, 4, C)
+        s[f"l1_{lvl}.weight"] = (H, 2 * H); s[f"l1_{lvl}.bias"] = (H,)
+        for i in range(2):
+            q = f"align_{lvl}.layers.{i}"
+            s[f"{q}.multihead_attn.in_proj_weight"] = (3 * H, H); s[f"{q}.multihead_attn.in_proj_bias"] = (3 * H,)
+            s[f"{q}.multihead_attn.out_proj.weight"] = (H, H); s[f"{q}.multihead_attn.out_proj.bias"] = (H,)
+            s[f"{q}.linear1.weight"] = (GS_ALIGN_FFN, H); s[f"{q}.linear1.bias"] = (GS_ALIGN_FFN,)
+            s[f"{q}.norm1.weight"] = (H,); s[f"{q}.norm1.bias"] = (H,)
+            s[f"{q}.linear2.weight"] = (H, GS_ALIGN_FFN); s[f"{q}.linear2.bias"] = (H,)
+            s[f"{q}.norm2.weight"] = (H,); s[f"{q}.norm2.bias"] = (H,)
+    _predictor_shapes(s, "pitch_inpainter_predictor", H, H, k, 3, 2)
+    s["embed_positions._float_tensor"] = (1,)
+    c2, hid, L = 2 * int(cfg["out_dims"]), int(cfg["glow_hidden"]), int(cfg["glow_layers"])
+    for b in range(int(cfg["glow_blocks"])):
+        p = f"post_flow.flows.{3 * b}"
+        s[f"{p}.logs"] = (1, c2, 1); s[f"{p}.bias"] = (1, c2, 1)
+        p = f"post_flow.flows.{3 * b + 1}"
+        for n_ in ("l", "log_s", "u", "p", "sign_s", "l_mask", "eye"):
+            s[f"{p}.{n_}"] = (4,) if n_ in ("log_s", "sign_s") else (4, 4)
+        p = f"post_flow.flows.{3 * b + 2}"
+        s[f"{p}.start.bias"] = (hid,); s[f"{p}.start.weight_g"] = (hid, 1, 1); s[f"{p}.start.weight_v"] = (hid, c2 // 2, 1)
+        s[f"{p}.end.weight"] = (c2, hid, 1); s[f"{p}.end.bias"] = (c2,)
+        _wn_shapes(s, f"{p}.wn", hid, int(cfg["glow_kernel"]), L, 2 * gs_glow_cond_channels(cfg))
+    return s
+
+
+def gs_wn_owner(cfg, b):
+    """the coupling block whose WN in_layers / res_skip_layers block b uses (glow_modules.py:538-553)"""
+    share = int(cfg["share_wn_layers"])
+    return b - b % share if share > 0 else b
+
+
+def synth_generspeech(cfg, seed: int = 909):
+    """Seeded GenerSpeech weights.  The FastSpeech2 part as synth_fs2 (durations of a few frames per token); weight-norm
+    gains near the direction's norm; VQ codebooks on the scale of the style encoder's output (about 1), with the
+    VQEmbeddingEMA buffers consistent (initialised, ema_weight = embedding); InvConvNear factors of a well-conditioned
+    4x4 (a permutation, unit lower / upper triangles, log-scales about 0); ActNorm and the coupling end layers small
+    so that the reverse flow stays O(1) over every block.  Shared WN tensors hold the same tensor under every name."""
+    shapes = generspeech_param_shapes(cfg)
+    sd = synth_state_dict(shapes, seed, convtranspose_prefixes=())
+    sd.update(synth_fs2(cfg, seed))
+    g = torch.Generator().manual_seed(int(seed) + 17)
+    for key, shape in shapes.items():
+        if key.endswith(".weight_g"):
+            v = sd[key[:-1] + "v"]
+            n = v.reshape(v.shape[0], -1).norm(dim=1).reshape(shape)
+            sd[key] = n * (0.6 + 0.8 * torch.rand(shape, generator=g))
+        elif key.endswith("vqvae.embedding"):   # codes of norm sqrt(H) x 0.5..3: distances far apart between codes
+            sd[key] = torch.randn(shape, generator=g) * (0.5 + 2.5 * torch.rand((shape[0], 1), generator=g))
+        elif key.endswith("vqvae.data_initialized") or key.endswith("vqvae.ema_count"):
+            sd[key] = torch.ones(shape)
+        elif key.endswith("_float_tensor"):
+            sd[key] = torch.zeros(shape)
+        elif key.endswith(("pos_embed_alpha",)):
+            sd[key] = torch.tensor([0.7])
+    for key in shapes:
+        if key.endswith("vqvae.ema_weight"):
+            sd[key] = sd[key[:-len("ema_weight")] + "embedding"].clone()
+    for b in range(int(cfg["glow_blocks"])):
+        p = f"post_flow.flows.{3 * b}"
+        sd[p + ".logs"] = 0.1 * torch.randn(sd[p + ".logs"].shape, generator=g)
+        sd[p + ".bias"] = 0.1 * torch.randn(sd[p + ".bias"].shape, generator=g)
+        p = f"post_flow.flows.{3 * b + 1}"
+        sd[p + ".p"] = torch.eye(4)[torch.randperm(4, generator=g)]
+        sd[p + ".sign_s"] = torch.where(torch.rand(4, generator=g) > 0.5, 1.0, -1.0)
+        sd[p + ".log_s"] = 0.2 * torch.randn(4, generator=g)
+        sd[p + ".l"] = 0.3 * torch.randn(4, 4, generator=g)
+        sd[p + ".u"] = 0.3 * torch.randn(4, 4, generator=g)
+        sd[p + ".l_mask"] = torch.tril(torch.ones(4, 4), -1)
+        sd[p + ".eye"] = torch.eye(4)
+        p = f"post_flow.flows.{3 * b + 2}"
+        sd[p + ".end.weight"] = 0.3 * sd[p + ".end.weight"]
+        own = f"post_flow.flows.{3 * gs_wn_owner(cfg, b) + 2}.wn."
+        for key in shapes:
+            if key.startswith(p + ".wn.") and not key.startswith(p + ".wn.cond_layer"):
+                sd[key] = sd[own + key[len(p + ".wn."):]]
+    return sd
+
+
+def generspeech_hparams(cfg):
+    """The hparams a reference GenerSpeech of this engine config is built from: fs2_hparams plus the generspeech.yaml keys
+    (speaker embedding on, predictor_grad 1)."""
+    hp = fs2_hparams(cfg)
+    hp.update(use_spk_embed=True, predictor_grad=1.0, ffn_padding="SAME", nVQ=int(cfg["n_vq"]), vae_dropout=0.0,
+              lambda_commit=0.25, post_glow_hidden=int(cfg["glow_hidden"]), post_glow_kernel_size=int(cfg["glow_kernel"]),
+              post_glow_n_blocks=int(cfg["glow_blocks"]), post_glow_n_block_layers=int(cfg["glow_layers"]),
+              share_wn_layers=int(cfg["share_wn_layers"]), sigmoid_scale=False, post_share_cond_layers=False,
+              use_txt_cond=True, vq_start=20500, forcing=20000, noise_scale=0.8)
+    return hp
+
+
+def _segments(n_frames, n_segs, g, empty=None):
+    """segment ids 1..n_segs over n_frames frames in order (each at least one frame; `empty` is skipped), 0 after"""
+    ids = [i for i in range(1, n_segs + 1) if i != empty]
+    cuts = torch.sort(torch.randperm(n_frames - 1, generator=g)[:len(ids) - 1] + 1).values.tolist()
+    seg = torch.zeros(n_frames, dtype=torch.long)
+    for i, (a, b) in enumerate(zip([0] + cuts, cuts + [n_frames])):
+        seg[a:b] = ids[i]
+    return seg
+
+
+def synth_generspeech_inputs(cfg, B, T, T_ref, seed):
+    """A ragged TTS_OOD batch (GenerSpeechInfer.input_to_batch's tensors): txt_tokens as synth_fs2_inputs; ref_mels
+    [B, T_ref, 80] of log-mel scale with zero frames past each row's length (T_ref, T_ref - 5, 2 T_ref / 3, cycled);
+    ref_mel2ph with T_ref // 4 segments per row (row 1 skips one id: an empty phoneme segment) and ref_mel2word with
+    T_ref // 10, both 0 on the padding frames; spk_embed / emo_embed [B, 256].  Every row reaches the same largest
+    segment id, so each row's B = 1 run sees the batch's segment count.  CPU tensors."""
+    out = synth_fs2_inputs(cfg, B, T, seed)
+    g = torch.Generator().manual_seed(int(seed) + 1)
+    lens = [(T_ref, T_ref - 5, (2 * T_ref) // 3)[i % 3] for i in range(B)]
+    mels = torch.zeros(B, T_ref, 80)
+    m2p = torch.zeros(B, T_ref, dtype=torch.long)
+    m2w = torch.zeros(B, T_ref, dtype=torch.long)
+    for i, n in enumerate(lens):
+        mels[i, :n] = -4.0 + 1.5 * torch.randn(n, 80, generator=g)
+        m2p[i, :n] = _segments(n, T_ref // 4, g, empty=3 if i == 1 else None)
+        m2w[i, :n] = _segments(n, T_ref // 10, g)
+    out.update(ref_mels=mels, ref_mel2ph=m2p, ref_mel2word=m2w, spk_embed=torch.randn(B, 256, generator=g),
+               emo_embed=torch.randn(B, 256, generator=g))
+    return out
+
+
 # ---------------------------------------------------------------------------------------------- CLAP text encoder
 # FrozenCLAPEmbedder (text_to_audio/Make_An_Audio/ldm/modules/encoders/modules.py:173-212): bert-base-uncased (the
 # BertConfig() defaults) and CLAP's Projection 768 -> 1024 (CLAP/config.yml d_proj), tokens padded to max_length 77

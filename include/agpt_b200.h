@@ -362,6 +362,48 @@ int agpt_fs2_decode(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out
                     const float* energy, int use_uv, int pitch_norm, float f0_mean, float f0_std, float* pitch_pred,
                     float* f0_denorm, int* pitch_coarse, float* energy_pred, float* decoder_inp, float* mel_out, void* stream);
 
+/* ------------------------------------------------------------------ GenerSpeech
+ * Replaces GenerSpeech.forward (NeuralSeq/modules/GenerSpeech/model/generspeech.py:75-260) as GenerSpeechInfer.forward_model
+ * calls it (infer=True, global_steps past `forcing`): the FastSpeech2 encoder / durations / decoder of agpt_fs2_cfg (pitch_type
+ * 'frame', pitch_norm 'standard' with uv, fairseq positions, no energy / MIDI) with the 256 -> H speaker and emotion
+ * projections, three LocalStyleAdaptors (utterance, phoneme, word: WN, segment mean, ConvBlocks, VQ) feeding ProsodyAligners
+ * (2 heads), the pitch inpainter, and the Glow post-flow (n_sqz 2, n_split 4, post_share_cond_layers off, sigmoid_scale
+ * off, use_txt_cond on) run in reverse.  The training diagnostics (VQ losses, perplexities, guided-attention losses and
+ * maps) are not computed.                                                                                         */
+typedef struct agpt_gs_cfg {   /* tagged, as agpt_clap_cfg: it nests agpt_fs2_cfg */
+  agpt_fs2_cfg fs2;
+  int n_vq;                    /* hparams['nVQ'] */
+  int glow_hidden, glow_kernel, glow_blocks, glow_layers;   /* post_glow_hidden / _kernel_size / _n_blocks / _n_block_layers */
+  int share_wn_layers;         /* blocks b - b % share_wn_layers share their WN in_layers / res_skip_layers (0: none) */
+} agpt_gs_cfg;
+/* Optional stage outputs of agpt_gs_forward (any pointer may be NULL): the decoder's mel before the post-flow
+ * [B][T_mel][80]; per level (utterance, phoneme, word) the quantised prosody [B][T_k][H] and its code indices [B][T_k]
+ * int32, T_k = T_ref, n_seg_ph, n_seg_word.                                                                         */
+typedef struct agpt_gs_taps {
+  float* mel_pre_flow;
+  float* prosody[3];
+  int* vq_idx[3];
+} agpt_gs_taps;
+/* host_weights: fp32 HOST arrays in the order of audiogpt_b200.modules.GenerSpeech.model.generspeech.GenerSpeech
+ * .engine_weights() (weight norm folded, each InvConvNear's inverse computed, the eight cond_layers concatenated).  */
+int agpt_gs_create(const agpt_gs_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* Token side, as agpt_fs2_encode: txt_tokens [B][T_txt] int32, spk_embed / emo_embed [B][256] fp32 (device).  dur = the
+ * duration predictor's output on (encoder_out + spk + emo) * nonpadding.  predict_dur != 0: dur_choice (may be NULL) and
+ * mel_len_host [B] (HOST; the call synchronises the stream for this one copy).  spk_out / emo_out [B][H] (may be NULL):
+ * spk_embed_proj(spk_embed), emo_embed_proj(emo_embed).                                                            */
+int agpt_gs_encode(agpt_handle h, const int* txt_tokens, int B, int T_txt, const float* spk_embed, const float* emo_embed,
+                   int predict_dur, float* dur, int* dur_choice, int* mel_len_host, float* spk_out, float* emo_out, void* stream);
+/* Frame side, T_mel >= 2 frames: mel2ph [B][T_mel] int32 (teacher-forced) or NULL = the durations of the last encode,
+ * expanded into mel2ph_out.  ref_mels [B][T_ref][80] (frames whose channel 0 is exactly 0 are padding); ref_mel2ph /
+ * ref_mel2word [B][T_ref] int32 segment ids (0 = none), n_seg_* = their maximum over the batch.  z [B][80][T_mel]: the
+ * post-flow's input noise, already scaled by noise_scale.  Outputs (device): pitch_pred [B][T_mel][2], f0_denorm,
+ * f0_denorm_pred [B][T_mel], pitch_coarse [B][T_mel] int32, decoder_inp and ref_prosody [B][T_mel][H], mel_out
+ * [B][2 (T_mel / 2)][80] (the post-flow truncates an odd T_mel).                                                    */
+int agpt_gs_forward(agpt_handle h, int T_mel, const int* mel2ph, int* mel2ph_out, const float* ref_mels, int T_ref,
+                    const int* ref_mel2ph, int n_seg_ph, const int* ref_mel2word, int n_seg_word, const float* z, float f0_mean,
+                    float f0_std, float* pitch_pred, float* f0_denorm, float* f0_denorm_pred, int* pitch_coarse, float* decoder_inp,
+                    float* ref_prosody, float* mel_out, const agpt_gs_taps* taps, void* stream);
+
 /* ------------------------------------------------------------------ CLAP text encoder
  * Replaces FrozenCLAPEmbedder.encode after tokenization (text_to_audio/Make_An_Audio/ldm/modules/encoders/modules.py:
  * 205-212): BERT (HF BertModel called with input_ids only, so every position attends to every position, padding
