@@ -18,6 +18,8 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.ldm.modules.encoders.modules.FrozenCLAPEmbedder   (installed with install(text_encoder=True))
     audiogpt_b200.wav_evaluation.models.CLAPWrapper.CLAPWrapper     (installed with install(scorer=True))
     audiogpt_b200.modules.GenerSpeech.model.generspeech.GenerSpeech (installed with install(tts_ood=True))
+    audiogpt_b200.sound_extraction.model.LASSNet.LASSNet            (installed with install(extraction=True))
+    audiogpt_b200.sound_extraction.utils.stft.STFT                  (installed with install(extraction=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -62,9 +64,15 @@ _TTS_OOD_MAP = {
     "modules.GenerSpeech.model.generspeech": ("audiogpt_b200.modules.GenerSpeech.model.generspeech", ["GenerSpeech"]),
 }
 
+# the sound-extraction tool's network and STFT, grafted only on request (install(extraction=True))
+_EXTRACTION_MAP = {
+    "sound_extraction.model.LASSNet": ("audiogpt_b200.sound_extraction.model.LASSNet", ["LASSNet"]),
+    "sound_extraction.utils.stft": ("audiogpt_b200.sound_extraction.utils.stft", ["STFT"]),
+}
+
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
-            text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False):
+            text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -89,6 +97,8 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     ``tts_ood=True`` also replaces ``modules.GenerSpeech.model.generspeech.GenerSpeech``, so the import in
     inference/tts/GenerSpeech.py resolves to the drop-in and the TTS_OOD tool's acoustic model and post-flow run on the
     engine (its HiFi-GAN vocoder is grafted by default).
+    ``extraction=True`` also replaces ``sound_extraction.model.LASSNet.LASSNet`` and ``sound_extraction.utils.stft.STFT``,
+    so the SoundExtraction tool's STFT, text encoder, FiLM ResUNet and inverse STFT run on the engine.
     Returns the list of patched names."""
     import importlib
     import sys
@@ -96,7 +106,7 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     patched = []
     todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}), **(_FIRST_STAGE_MAP if first_stage else {}),
                 **(_TEXT_ENCODER_MAP if text_encoder else {}), **(_SCORER_MAP if scorer else {}),
-                **(_TTS_OOD_MAP if tts_ood else {}))
+                **(_TTS_OOD_MAP if tts_ood else {}), **(_EXTRACTION_MAP if extraction else {}))
     for ref_name, (our_name, attrs) in todo.items():
         ours = importlib.import_module(our_name)
         names = attrs if isinstance(attrs, dict) else {a: a for a in attrs}

@@ -92,6 +92,13 @@ class Cnn14Config(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("window_size", "hop_size", "mel_bins", "out_emb", "d_proj")]
 
 
+class LassConfig(C.Structure):
+    """agpt_lass_cfg (a tagged struct in the header, like agpt_clap_cfg; the create entry point takes a plain pointer)."""
+    _fields_ = [(n, C.c_int) for n in (
+        "vocab_size", "max_position_embeddings", "type_vocab_size", "hidden_size", "num_layers", "num_heads",
+        "intermediate_size")] + [("layer_norm_eps", C.c_float)]
+
+
 class TapconvProbeArgs(C.Structure):
     """agpt_tapconv_probe_args (a tagged struct in the header: it carries pointers and floats)."""
     _fields_ = [(n, C.c_int) for n in ("kind", "Cin", "Cout", "K", "dil", "Wreal", "strip_w", "u", "pad", "g")] + [
@@ -171,6 +178,12 @@ PROTOTYPES = {
     "agpt_cnn14_create": (_I, [_P, _W, _I, _I, _OUT]),
     "agpt_cnn14_set_resample": (_I, [_P, _I, _I, _I, _P, _I]),
     "agpt_cnn14_embed": (_I, [_P, _P, _L, _I, _P, _P, _P]),
+    "agpt_lass_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_lass_text": (_I, [_P, _P, _P, _I, _I, _P, _P]),
+    "agpt_lass_mask": (_I, [_P, _P, _I, _I, _I, _L, _L, _L, _P, _P, _P, _P]),
+    "agpt_stft_create": (_I, [_I, _I, _W, _I, _I, _OUT]),
+    "agpt_stft_transform": (_I, [_P, _P, _I, _L, _P, _P, _P]),
+    "agpt_stft_inverse": (_I, [_P, _P, _P, _I, _I, _P, _P]),
 }
 
 _lock = threading.Lock()

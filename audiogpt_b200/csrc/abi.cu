@@ -378,6 +378,51 @@ int agpt_cnn14_embed(agpt_handle h, const float* wav, long n_samples, int B, con
   });
 }
 
+int agpt_lass_create(const agpt_lass_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(lass_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_lass_text(agpt_handle h, const int* input_ids, const int* attention_mask, int N, int L, float* cond, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(input_ids && attention_mask && cond, "null argument");
+    lass_text(as(h, kMagicLass, "lass"), input_ids, attention_mask, N, L, cond, (cudaStream_t)stream);
+  });
+}
+
+int agpt_lass_mask(agpt_handle h, const float* mag, int B, int T, int F, long stride_b, long stride_t, long stride_f,
+                   const float* cond, float* mask, float* logits, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(mag && cond && mask, "null argument");
+    lass_mask(as(h, kMagicLass, "lass"), mag, B, T, F, stride_b, stride_t, stride_f, cond, mask, logits, (cudaStream_t)stream);
+  });
+}
+
+int agpt_stft_create(int filter_length, int hop_length, const float* const* host_weights, int n_weights, int device,
+                     agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(host_weights && out, "null argument");
+    AGPT_CHECK(n_weights == 2, "the STFT takes forward_basis and inverse_basis");
+    *out = reinterpret_cast<agpt_handle>(stft_create(filter_length, hop_length, host_weights[0], host_weights[1], device));
+  });
+}
+
+int agpt_stft_transform(agpt_handle h, const float* wav, int B, long n_samples, float* magnitude, float* phase, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(wav && magnitude && phase, "null argument");
+    stft_transform(as(h, kMagicStft, "stft"), wav, B, n_samples, magnitude, phase, (cudaStream_t)stream);
+  });
+}
+
+int agpt_stft_inverse(agpt_handle h, const float* magnitude, const float* phase, int B, int T, float* wav, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(magnitude && phase && wav, "null argument");
+    stft_inverse(as(h, kMagicStft, "stft"), magnitude, phase, B, T, wav, (cudaStream_t)stream);
+  });
+}
+
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                        double* out2, double* dbg8_or_null) {
   return guarded([&] {

@@ -71,6 +71,14 @@ Handle* cnn14_create(const agpt_cnn14_cfg* cfg, const float* const* W, int nW, i
 void cnn14_set_resample(Handle* h, int orig, int nw, int width, const float* table, int clip);
 void cnn14_embed(Handle* h, const float* wav, long n_samples, int B, const int* start_host, float* out, cudaStream_t st);
 
+Handle* lass_create(const agpt_lass_cfg* cfg, const float* const* W, int nW, int device);
+void lass_text(Handle* h, const int* ids, const int* mask, int N, int L, float* cond, cudaStream_t st);
+void lass_mask(Handle* h, const float* mag, int B, int T, int F, long sb, long st_, long sf, const float* cond, float* mask,
+               float* logits, cudaStream_t st);
+Handle* stft_create(int filter_length, int hop_length, const float* fwd_basis, const float* inv_basis, int device);
+void stft_transform(Handle* h, const float* wav, int B, long n_samples, float* mag, float* phase, cudaStream_t st);
+void stft_inverse(Handle* h, const float* mag, const float* phase, int B, int T, float* wav, cudaStream_t st);
+
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                    double* out, double* dbg_avg);
 void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);

@@ -1240,3 +1240,173 @@ def synth_scorer_clips(lens=(159744, 40000, 159744), sr: int = 16000, seed: int 
         x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.5, 3) * t)) + 0.02 * (i + 1) * rs.randn(int(n))
         clips.append(x.astype(np.float32))
     return clips
+
+
+# ---------------------------------------------------------------------------------------------- sound extraction
+# LASSNet of the SoundExtraction tool (sound_extraction/model/LASSNet.py, text_encoder.py, resunet_film.py,
+# modules.py:169-379, film.py): bert-mini (prajjwal1/bert-mini: 4 layers, hidden 256, 4 heads, FFN 1024, no pooler),
+# Linear(256, 256) + ReLU, and UNetRes_FiLM(channels=1, cond_embedding_dim=256).  The STFT is filter_length 1024, hop
+# 512, periodic Hann (sound_extraction/utils/stft.py).
+LASS = dict(vocab_size=30522, max_position_embeddings=512, type_vocab_size=2, hidden_size=256, num_layers=4, num_heads=4,
+            intermediate_size=1024, layer_norm_eps=1e-12)
+# the same network with a 1000-token vocabulary (the UNet's widths are fixed by the reference class)
+LASS_SMALL = dict(LASS, vocab_size=1000, max_position_embeddings=64)
+LASS_COND = 256
+LASS_ENC = ((1, 32), (32, 64), (64, 128), (128, 256), (256, 384), (384, 384))   # encoder_block1..6 (in, out)
+LASS_DEC = ((384, 384), (384, 384), (384, 256), (256, 128), (128, 64), (64, 32))  # decoder_block1..6 (in, out)
+LASS_FFT, LASS_HOP = 1024, 512
+
+
+def lass_blocks():
+    """The 26 ConvBlockResCond of UNetRes_FiLM in forward order: (state-dict prefix, C_in, C_out)."""
+    out = []
+    for i, (ci, co) in enumerate(LASS_ENC):
+        out += [(f"UNet.encoder_block{i + 1}.conv_block1", ci, co), (f"UNet.encoder_block{i + 1}.conv_block2", co, co)]
+    out.append(("UNet.conv_block7", 384, 384))
+    for j, (ci, co) in enumerate(LASS_DEC):
+        out += [(f"UNet.decoder_block{j + 1}.conv_block2", 2 * co, co), (f"UNet.decoder_block{j + 1}.conv_block3", co, co)]
+    out.append(("UNet.after_conv_block1", 32, 32))
+    return out
+
+
+def _film_shapes(s, p, c, d=LASS_COND):
+    s[p + ".linear.0.weight"] = (2 * c, d); s[p + ".linear.0.bias"] = (2 * c,)
+    s[p + ".linear.2.weight"] = (c, 2 * c); s[p + ".linear.2.bias"] = (c,)
+
+
+def _resblock_cond_shapes(s, p, ci, co):
+    _bn_shapes(s, p + ".bn1", ci)
+    _bn_shapes(s, p + ".bn2", co)
+    s[p + ".conv1.weight"] = (co, ci, 3, 3)
+    _film_shapes(s, p + ".film1", co)
+    s[p + ".conv2.weight"] = (co, co, 3, 3)
+    _film_shapes(s, p + ".film2", co)
+    if ci != co:
+        s[p + ".shortcut.weight"] = (co, ci, 1, 1); s[p + ".shortcut.bias"] = (co,)
+        _film_shapes(s, p + ".film_res", co)
+
+
+def lass_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of LASSNet in state-dict order, which is the order agpt_lass_create consumes (without
+    the num_batches_tracked counters): text_embedder.bert_layer (HF BertModel without pooler and without the
+    position_ids buffer current transformers no longer saves), text_embedder.linear_layer, then UNet."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    H, I = int(cfg["hidden_size"]), int(cfg["intermediate_size"])
+    b = "text_embedder.bert_layer."
+    s[b + "embeddings.word_embeddings.weight"] = (int(cfg["vocab_size"]), H)
+    s[b + "embeddings.position_embeddings.weight"] = (int(cfg["max_position_embeddings"]), H)
+    s[b + "embeddings.token_type_embeddings.weight"] = (int(cfg["type_vocab_size"]), H)
+    s[b + "embeddings.LayerNorm.weight"] = (H,); s[b + "embeddings.LayerNorm.bias"] = (H,)
+    for i in range(int(cfg["num_layers"])):
+        p = f"{b}encoder.layer.{i}."
+        for n in ("query", "key", "value"):
+            s[f"{p}attention.self.{n}.weight"] = (H, H); s[f"{p}attention.self.{n}.bias"] = (H,)
+        s[p + "attention.output.dense.weight"] = (H, H); s[p + "attention.output.dense.bias"] = (H,)
+        s[p + "attention.output.LayerNorm.weight"] = (H,); s[p + "attention.output.LayerNorm.bias"] = (H,)
+        s[p + "intermediate.dense.weight"] = (I, H); s[p + "intermediate.dense.bias"] = (I,)
+        s[p + "output.dense.weight"] = (H, I); s[p + "output.dense.bias"] = (H,)
+        s[p + "output.LayerNorm.weight"] = (H,); s[p + "output.LayerNorm.bias"] = (H,)
+    s["text_embedder.linear_layer.0.weight"] = (LASS_COND, H); s["text_embedder.linear_layer.0.bias"] = (LASS_COND,)
+    blocks = {p: (ci, co) for p, ci, co in lass_blocks()}
+    for i in range(len(LASS_ENC)):
+        for k in (1, 2):
+            p = f"UNet.encoder_block{i + 1}.conv_block{k}"
+            _resblock_cond_shapes(s, p, *blocks[p])
+    _resblock_cond_shapes(s, "UNet.conv_block7", 384, 384)
+    for j, (ci, co) in enumerate(LASS_DEC):
+        p = f"UNet.decoder_block{j + 1}"
+        s[p + ".conv1.weight"] = (ci, co, 3, 3)
+        _bn_shapes(s, p + ".bn1", ci)
+        _resblock_cond_shapes(s, p + ".conv_block2", 2 * co, co)
+        _resblock_cond_shapes(s, p + ".conv_block3", co, co)
+    _resblock_cond_shapes(s, "UNet.after_conv_block1", 32, 32)
+    s["UNet.after_conv2.weight"] = (1, 32, 1, 1); s["UNet.after_conv2.bias"] = (1,)
+    return s
+
+
+def lass_engine_keys(cfg):
+    """The keys agpt_lass_create consumes, in its order: lass_param_shapes without num_batches_tracked."""
+    return [k for k in lass_param_shapes(cfg) if not k.endswith("num_batches_tracked")]
+
+
+def synth_lass(cfg, seed: int = 6060):
+    """Seeded LASSNet weights: synth_state_dict draws (convs and Linears N(0, 1 / fan_in)), then every BatchNorm gets
+    gamma 1 + 0.2 N, beta 0.1 N, running mean 0.2 N and running variance in [0.5, 1.5) (the first block's bn1, which
+    sees raw magnitudes, mean 1 and variance in [4, 6)), and the FiLM layers' second Linear is scaled by 0.5 so the
+    62 additive vectors stay O(0.1), and after_conv2 by 0.25, so the mask logits stay O(1) and the sigmoid does not
+    saturate."""
+    shapes = lass_param_shapes(cfg)
+    sd = synth_state_dict(shapes, seed, convtranspose_prefixes=())
+    g = torch.Generator().manual_seed(int(seed) + 1)
+    first = "UNet.encoder_block1.conv_block1.bn1."
+    for k, shape in shapes.items():
+        if ".bn" not in k:
+            continue
+        if k.endswith("num_batches_tracked"):
+            sd[k] = torch.tensor(0, dtype=torch.long)
+        elif k.endswith(".weight"):
+            sd[k] = 1.0 + 0.2 * torch.randn(shape, generator=g)
+        elif k.endswith(".bias"):
+            sd[k] = 0.1 * torch.randn(shape, generator=g)
+        elif k.endswith("running_mean"):
+            sd[k] = torch.ones(shape) if k.startswith(first) else 0.2 * torch.randn(shape, generator=g)
+        elif k.endswith("running_var"):
+            sd[k] = (4.0 if k.startswith(first) else 0.5) + (2.0 if k.startswith(first) else 1.0) * torch.rand(shape, generator=g)
+    for k in shapes:
+        if ".film" in k and ".linear.2." in k:
+            sd[k] = sd[k] * 0.5
+    sd["UNet.after_conv2.weight"] = sd["UNet.after_conv2.weight"] * 0.25
+    return sd
+
+
+def stft_bases(filter_length: int = LASS_FFT, hop_length: int = LASS_HOP):
+    """sound_extraction/utils/stft.py STFT's forward_basis / inverse_basis buffers [filter_length + 2][1][filter_length]
+    (win_length = filter_length, window 'hann'): built in numpy float64 the reference's way, cast to fp32, windowed
+    with the fp32 periodic Hann window."""
+    scale = filter_length / hop_length
+    fb = np.fft.fft(np.eye(filter_length))
+    cutoff = filter_length // 2 + 1
+    fb = np.vstack([np.real(fb[:cutoff, :]), np.imag(fb[:cutoff, :])])
+    fwd = torch.FloatTensor(fb[:, None, :])
+    inv = torch.FloatTensor(np.linalg.pinv(scale * fb).T[:, None, :])
+    from scipy.signal import get_window
+    win = torch.from_numpy(get_window("hann", filter_length, fftbins=True)).float()
+    return (fwd * win).float(), (inv * win).float()
+
+
+def stft_window_sum(n_frames: int, filter_length: int = LASS_FFT, hop_length: int = LASS_HOP) -> np.ndarray:
+    """stft.py window_sumsquare('hann', n_frames, ...) with norm None: the fp32 envelope, each frame's float64 squared
+    window added in float64 and stored back to fp32, as numpy's in-place add does."""
+    n = filter_length + hop_length * (n_frames - 1)
+    x = np.zeros(n, dtype=np.float32)
+    from scipy.signal import get_window
+    win_sq = get_window("hann", filter_length, fftbins=True) ** 2
+    for i in range(n_frames):
+        s = i * hop_length
+        x[s:min(n, s + filter_length)] += win_sq[:max(0, min(filter_length, n - s))]
+    return x
+
+
+def synth_lass_ids(cfg, lens, seed: int = 61):
+    """Seeded query rows as the tool tokenizes them (add_special_tokens=False, padding=True): [N, max(lens)] ids with
+    [CLS] (101, or 1 for a vocabulary without it) first, and the attention mask."""
+    rs = np.random.RandomState(int(seed))
+    V = int(cfg["vocab_size"])
+    cls = 101 if V > 101 else 1
+    L = max(lens)
+    ids = np.zeros((len(lens), L), np.int64)
+    mask = np.zeros((len(lens), L), np.int64)
+    for i, n in enumerate(lens):
+        ids[i, 0] = cls
+        ids[i, 1:n] = rs.randint(1000 if V > 2000 else 2, V, size=n - 1)
+        mask[i, :n] = 1
+    return torch.from_numpy(ids), torch.from_numpy(mask)
+
+
+def synth_lass_wav(n_samples: int, seed: int = 62) -> torch.Tensor:
+    """A seeded mono clip at 32 kHz: a few sines under a slow envelope plus noise, [n_samples] fp32."""
+    rs = np.random.RandomState(int(seed))
+    t = np.arange(int(n_samples)) / 32000.0
+    x = sum(0.15 / (j + 1) * np.sin(2 * np.pi * rs.uniform(60, 6000) * t + rs.uniform(0, 6)) for j in range(6))
+    x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.3, 2) * t)) + 0.02 * rs.randn(int(n_samples))
+    return torch.from_numpy(x.astype(np.float32))

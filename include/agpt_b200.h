@@ -471,6 +471,42 @@ int agpt_cnn14_set_resample(agpt_handle h, int orig_freq, int new_freq, int widt
 int agpt_cnn14_embed(agpt_handle h, const float* wav, long n_samples, int B, const int* start_or_tile_host, float* out_emb,
                      void* stream);
 
+/* ------------------------------------------------------------------ Sound extraction
+ * The SoundExtraction tool (audio-chatgpt.py:675-710): sound_extraction/model/LASSNet.py -- bert-mini on the query
+ * ([CLS] row -> Linear(256, 256) -> ReLU = cond), then UNetRes_FiLM (resunet_film.py, modules.py:169-379, film.py;
+ * eval BatchNorm, eps 1e-5) conditioned on cond, then a sigmoid -- and sound_extraction/utils/stft.py's STFT.
+ * A tagged struct, as agpt_clap_cfg (it carries a float).                                                          */
+typedef struct agpt_lass_cfg {
+  int vocab_size;              /* bert-mini: 30522 */
+  int max_position_embeddings; /* 512 */
+  int type_vocab_size;         /* 2 (only type 0 is read) */
+  int hidden_size;             /* 256 (the Linear after BERT is 256 -> 256) */
+  int num_layers;              /* 4 */
+  int num_heads;               /* 4 */
+  int intermediate_size;       /* 1024 */
+  float layer_norm_eps;        /* 1e-12 */
+} agpt_lass_cfg;
+/* host_weights: fp32 HOST arrays in the key order of audiogpt_b200.specs.lass_engine_keys(cfg): LASSNet's state dict
+ * without num_batches_tracked (and without the position_ids buffer).                                              */
+int agpt_lass_create(const agpt_lass_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* input_ids / attention_mask [N][L] int32 (device; ids clamped to the table, callers reject them first) -> cond
+ * [N][256] (device): relu(Linear(BertModel(input_ids, attention_mask)[0][:, 0])), padding keys masked out.       */
+int agpt_lass_text(agpt_handle h, const int* input_ids, const int* attention_mask, int N, int L, float* cond, void* stream);
+/* mag: the magnitude [B][T][F] (device) at element strides stride_b / stride_t / stride_f (the tool passes a transposed
+ * view); cond [B][256] (device) -> mask [B][T][F] = sigmoid(UNetRes_FiLM(mag, cond, cond)) and, when logits is not
+ * NULL, the pre-sigmoid values (0 in the two top bins).  F - 2 must be 63 mod 64 and at least 127; any T >= 1.     */
+int agpt_lass_mask(agpt_handle h, const float* mag, int B, int T, int F, long stride_b, long stride_t, long stride_f,
+                   const float* cond, float* mask, float* logits, void* stream);
+/* STFT(filter_length, hop_length, win_length = filter_length, window 'hann') with filter_length = 2 hop_length:
+ * host_weights: the module's buffers forward_basis, inverse_basis [filter_length + 2][1][filter_length] (HOST).   */
+int agpt_stft_create(int filter_length, int hop_length, const float* const* host_weights, int n_weights, int device,
+                     agpt_handle* out);
+/* STFT.transform: wav [B][n_samples] (device, n_samples > filter_length / 2) -> magnitude / phase
+ * [B][filter_length / 2 + 1][n_samples / hop + 1] (device).                                                         */
+int agpt_stft_transform(agpt_handle h, const float* wav, int B, long n_samples, float* magnitude, float* phase, void* stream);
+/* STFT.inverse: magnitude / phase [B][filter_length / 2 + 1][T] (device, T >= 2) -> wav [B][(T - 1) hop] (device).   */
+int agpt_stft_inverse(agpt_handle h, const float* magnitude, const float* phase, int B, int T, float* wav, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
