@@ -20,6 +20,7 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.modules.GenerSpeech.model.generspeech.GenerSpeech (installed with install(tts_ood=True))
     audiogpt_b200.sound_extraction.model.LASSNet.LASSNet            (installed with install(extraction=True))
     audiogpt_b200.sound_extraction.utils.stft.STFT                  (installed with install(extraction=True))
+    audiogpt_b200.audio_detection.audio_infer.pytorch.models.PVT    (installed with install(detection=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -70,9 +71,16 @@ _EXTRACTION_MAP = {
     "sound_extraction.utils.stft": ("audiogpt_b200.sound_extraction.utils.stft", ["STFT"]),
 }
 
+# the sound-event-detection tool's PVT, grafted only on request (install(detection=True)) under the name the agent
+# script imports at load time (audio_detection/ is on its sys.path); the reference module imports torchlibrosa, timm,
+# mmcv and mmdet, so where those are missing this is the sys.modules alias
+_DETECTION_MAP = {
+    "audio_infer.pytorch.models": ("audiogpt_b200.audio_detection.audio_infer.pytorch.models", ["PVT"]),
+}
+
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
-            text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False):
+            text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False, detection: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -99,6 +107,10 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     engine (its HiFi-GAN vocoder is grafted by default).
     ``extraction=True`` also replaces ``sound_extraction.model.LASSNet.LASSNet`` and ``sound_extraction.utils.stft.STFT``,
     so the SoundExtraction tool's STFT, text encoder, FiLM ResUNet and inverse STFT run on the engine.
+    ``detection=True`` also replaces ``audio_infer.pytorch.models.PVT``, so the SoundDetection tool's log-mel front end,
+    pyramid transformer and framewise head run on the engine.  The agent script imports that name when it is loaded, so
+    call install first; only the ``models`` leaf is aliased, the packages ``audio_infer`` and ``audio_infer.pytorch``
+    (from which the script also imports ``audio_infer.utils.config``) stay the reference's own.
     Returns the list of patched names."""
     import importlib
     import sys
@@ -106,7 +118,7 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     patched = []
     todo = dict(_INSTALL_MAP, **(_FRONT_END_MAP if front_end else {}), **(_FIRST_STAGE_MAP if first_stage else {}),
                 **(_TEXT_ENCODER_MAP if text_encoder else {}), **(_SCORER_MAP if scorer else {}),
-                **(_TTS_OOD_MAP if tts_ood else {}), **(_EXTRACTION_MAP if extraction else {}))
+                **(_TTS_OOD_MAP if tts_ood else {}), **(_EXTRACTION_MAP if extraction else {}), **(_DETECTION_MAP if detection else {}))
     for ref_name, (our_name, attrs) in todo.items():
         ours = importlib.import_module(our_name)
         names = attrs if isinstance(attrs, dict) else {a: a for a in attrs}

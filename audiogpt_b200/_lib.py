@@ -99,6 +99,13 @@ class LassConfig(C.Structure):
         "intermediate_size")] + [("layer_norm_eps", C.c_float)]
 
 
+class PvtConfig(C.Structure):
+    """agpt_pvt_cfg (a tagged struct in the header, like agpt_clap_cfg; the create entry point takes a plain pointer)."""
+    _fields_ = [(n, C.c_int) for n in ("window_size", "hop_size", "mel_bins", "classes_num")] + [
+        (n, C.c_int * 4) for n in ("embed_dims", "depths", "num_heads", "mlp_ratios", "sr_ratios")] + [
+        ("interpolate_ratio", C.c_int), ("layer_norm_eps", C.c_float), ("embed_norm_eps", C.c_float)]
+
+
 class TapconvProbeArgs(C.Structure):
     """agpt_tapconv_probe_args (a tagged struct in the header: it carries pointers and floats)."""
     _fields_ = [(n, C.c_int) for n in ("kind", "Cin", "Cout", "K", "dil", "Wreal", "strip_w", "u", "pad", "g")] + [
@@ -184,6 +191,13 @@ PROTOTYPES = {
     "agpt_stft_create": (_I, [_I, _I, _W, _I, _I, _OUT]),
     "agpt_stft_transform": (_I, [_P, _P, _I, _L, _P, _P, _P]),
     "agpt_stft_inverse": (_I, [_P, _P, _P, _I, _I, _P, _P]),
+    "agpt_pvt_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_pvt_frames": (_I, [_P, _L, _P]),
+    "agpt_pvt_forward": (_I, [_P, _P, _I, _L, _P, _P, _P, _P]),
+    "agpt_pvt_dwconv_gelu": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    "agpt_pvt_patch7": (_I, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _I, _P, _P]),
+    "agpt_pvt_sr_gather": (_I, [_P, _I, _I, _I, _I, _I, _P, _P]),
+    "agpt_pvt_head": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
 }
 
 _lock = threading.Lock()

@@ -423,6 +423,59 @@ int agpt_stft_inverse(agpt_handle h, const float* magnitude, const float* phase,
   });
 }
 
+int agpt_pvt_create(const agpt_pvt_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(pvt_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_pvt_frames(const agpt_pvt_cfg* cfg, long n_samples, int grid_hw[4][2]) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && grid_hw, "null argument");
+    pvt_frames(cfg, n_samples, grid_hw);
+  });
+}
+
+int agpt_pvt_forward(agpt_handle h, const float* wav, int B, long n_samples, float* framewise, float* clipwise, float* logits,
+                     void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(wav && framewise && clipwise, "null argument");
+    pvt_forward(as(h, kMagicPvt, "pvt"), wav, B, n_samples, framewise, clipwise, logits, (cudaStream_t)stream);
+  });
+}
+
+int agpt_pvt_dwconv_gelu(const float* x, const float* w, const float* bias, int B, int H, int W, int C, float* out, void* plane_hi,
+                         void* plane_lo, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(x && w && bias, "null argument");
+    pvt_dwconv_gelu(x, w, bias, B, H, W, C, out, static_cast<__half*>(plane_hi), static_cast<__half*>(plane_lo), (cudaStream_t)stream);
+  });
+}
+
+int agpt_pvt_patch7(const float* img, const float* w, const float* bias, const float* gamma, const float* beta, float eps, int B,
+                    int H, int W, int C, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(img && w && bias && gamma && beta && out, "null argument");
+    pvt_patch7(img, w, bias, gamma, beta, eps, B, H, W, C, out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_pvt_sr_gather(const float* x, int B, int H, int W, int C, int sr, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(x && out, "null argument");
+    pvt_sr_gather(x, B, H, W, C, sr, out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_pvt_head(const float* x, const float* w, const float* bias, int B, int H, int W, int C, int classes, int ratio,
+                  float* framewise, float* clipwise, float* logits, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(x && w && bias && framewise && clipwise, "null argument");
+    pvt_head(x, w, bias, B, H, W, C, classes, ratio, framewise, clipwise, logits, (cudaStream_t)stream);
+  });
+}
+
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                        double* out2, double* dbg8_or_null) {
   return guarded([&] {

@@ -11,6 +11,7 @@
 #include "models.h"
 #include "fs_layers.cuh"
 #include "clap.cuh"
+#include "logmel.cuh"
 
 namespace agpt {
 
@@ -40,37 +41,6 @@ __global__ void cnn14_resample_kernel(const float* __restrict__ x, long L, const
       if (xi >= 0 && xi < L) acc = fmaf(kp[j], xb[xi], acc);
     }
     out[i] = acc;
-  }
-}
-
-// frames[b][t][j] = x_b[reflect(t * hop + j - n / 2)]  (center=True, pad_mode='reflect')
-__global__ void cnn14_frames_kernel(const float* __restrict__ x, int clip, int T, int hop, int n, float* __restrict__ fr, long total) {
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const long bt = i / n;
-    const int j = (int)(i - bt * n);
-    const long b = bt / T;
-    const int t = (int)(bt - b * T);
-    int s = t * hop + j - n / 2;
-    s = s < 0 ? -s : (s >= clip ? 2 * (clip - 1) - s : s);
-    fr[i] = x[b * clip + s];
-  }
-}
-
-// one block per frame: re^2 + im^2 -> melW projection -> 10 log10(max(., 1e-10)) -> bn0 (folded scale / shift per mel
-// bin) -> img[b][t][m][0..3] (the first conv's 4-channel padded input)
-__global__ void cnn14_logmel_kernel(const float* __restrict__ spec, int pitch, int nb, const float* __restrict__ melW,
-                                    int nm, const float* __restrict__ bn_s, const float* __restrict__ bn_t, float* __restrict__ img) {
-  extern __shared__ float pw[];
-  const long f = blockIdx.x;
-  const float* re = spec + f * pitch;
-  const float* im = re + nb;
-  for (int k = threadIdx.x; k < nb; k += blockDim.x) pw[k] = re[k] * re[k] + im[k] * im[k];
-  __syncthreads();
-  for (int m = threadIdx.x; m < nm; m += blockDim.x) {
-    float acc = 0.f;
-    for (int k = 0; k < nb; ++k) acc = fmaf(pw[k], melW[(long)k * nm + m], acc);
-    const float db = 10.f * log10f(fmaxf(acc, 1e-10f));
-    *reinterpret_cast<float4*>(img + (f * nm + m) * 4) = make_float4(db * bn_s[m] + bn_t[m], 0.f, 0.f, 0.f);
   }
 }
 
@@ -174,15 +144,14 @@ void ClapProjection::load(WeightCursor& wc, int d_in, int d_out, float eps_) {
 
 struct Cnn14Net : Handle {
   agpt_cnn14_cfg cfg;
-  PackedConv dft;
-  DevBuf melW, bn0_s, bn0_t;
+  LogmelFront front;   // framing, DFT tap-GEMM, power / mel / log / bn0 (logmel.cuh)
   PackedConv conv[kCnn14Blocks][2];
   PackedConv fc1;
   ClapProjection proj;
   // resampler (agpt_cnn14_set_resample)
   DevBuf ker;
   int orig = 0, nw = 0, width = 0, taps = 0, clip = 0;
-  DevBuf starts, wav, frames, spec, img, bufA, bufB, bufC, pooled, emb;
+  DevBuf starts, wav, img, bufA, bufB, bufC, pooled, emb;
 
   void embed(const float* x, long L, int B, const int* start_host, float* out, cudaStream_t st) {
     AGPT_CHECK(clip > 0, "agpt_cnn14_set_resample was not called");
@@ -193,7 +162,7 @@ struct Cnn14Net : Handle {
       if (R > clip) AGPT_CHECK(s >= 0 && (long)s < R - clip, "crop start outside [0, resampled length - clip)");
       else AGPT_CHECK(s == -1, "a clip no longer than the target is tiled: its start must be -1");
     }
-    const int n = cfg.window_size, hop = cfg.hop_size, nb = n / 2 + 1, nm = cfg.mel_bins;
+    const int n = cfg.window_size, hop = cfg.hop_size, nm = cfg.mel_bins;
     AGPT_CHECK(clip > n / 2, "the fitted clip must be longer than half a window (reflect padding)");
     const int T = clip / hop + 1;
     int* sd = reinterpret_cast<int*>(starts.ensure(B));
@@ -201,20 +170,9 @@ struct Cnn14Net : Handle {
     wav.ensure((size_t)B * clip);
     const long tot = (long)B * clip;
     cnn14_resample_kernel<<<ew_blocks(tot), 256, 0, st>>>(x, L, ker.p, taps, orig, nw, width, R, sd, clip, wav.p, tot);
-    frames.ensure((size_t)B * T * n);
-    cnn14_frames_kernel<<<ew_blocks((long)B * T * n), 256, 0, st>>>(wav.p, clip, T, hop, n, frames.p, (long)B * T * n);
-    count_launch(2);
-    spec.ensure((size_t)B * T * dft.cout_pad);
-    {
-      TapConvParams P = tapconv_params(dft, 1, B * T, 0, 1);
-      P.in = frames.p; P.in_pitch = n;
-      P.out = spec.p; P.out_pitch = dft.cout_pad;
-      P.epi = EPI_BIAS;
-      tapconv_launch(P, st);
-    }
-    img.ensure((size_t)B * T * nm * 4);
-    cnn14_logmel_kernel<<<(unsigned)(B * T), 64, sizeof(float) * nb, st>>>(spec.p, dft.cout_pad, nb, melW.p, nm, bn0_s.p, bn0_t.p, img.p);
     count_launch(1);
+    img.ensure((size_t)B * T * nm * 4);
+    front.run<4>(wav.p, clip, B, img.p, st);
     // conv blocks: (3x3 conv -> folded BN -> ReLU) x 2, then AvgPool2d(2) (blocks 1-5) on [B][H=T][W=F][C]
     const size_t big = (size_t)B * T * nm * kCnn14Ch[0];
     bufA.ensure(big); bufB.ensure(big); bufC.ensure(big);
@@ -269,22 +227,8 @@ Handle* cnn14_create(const agpt_cnn14_cfg* cfg, const float* const* W, int nW, i
              "bad Cnn14 config (mel_bins must be 64: Cnn14's bn0 is BatchNorm2d(64))");
   std::unique_ptr<Cnn14Net> h(new Cnn14Net());
   h->magic = kMagicCnn14; h->device = device; h->cfg = *cfg;
-  const int n = cfg->window_size, nb = n / 2 + 1, nm = cfg->mel_bins;
   WeightCursor wc{W, nW};
-  {  // conv_real / conv_imag [nb][1][n] -> one [n] -> [re | im] 1-tap GEMM
-    const float* re = wc.next(); const float* im = wc.next();
-    std::vector<float> w((size_t)2 * nb * n);
-    memcpy(w.data(), re, sizeof(float) * nb * n);
-    memcpy(w.data() + (size_t)nb * n, im, sizeof(float) * nb * n);
-    pack_conv(h->dft, w.data(), nullptr, 2 * nb, n, 1, false);
-  }
-  h->melW.upload(wc.next(), (size_t)nb * nm);
-  {
-    const float* g = wc.next(); const float* be = wc.next(); const float* rm = wc.next(); const float* rv = wc.next();
-    std::vector<float> s(nm), t(nm);
-    for (int m = 0; m < nm; ++m) { s[m] = g[m] / sqrtf(rv[m] + kBnEps); t[m] = be[m] - rm[m] * s[m]; }
-    h->bn0_s.upload(s); h->bn0_t.upload(t);
-  }
+  h->front.load(wc, cfg->window_size, cfg->hop_size, cfg->mel_bins, kBnEps);
   int cin = 1;
   for (int i = 0; i < kCnn14Blocks; ++i) {
     const int c = kCnn14Ch[i];

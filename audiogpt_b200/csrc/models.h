@@ -1,6 +1,7 @@
 // Internal C++ entry points behind the C ABI (include/agpt_b200.h).
 #pragma once
 #include "../../include/agpt_b200.h"
+#include <cuda_fp16.h>
 #include "common.cuh"
 
 namespace agpt {
@@ -78,6 +79,17 @@ void lass_mask(Handle* h, const float* mag, int B, int T, int F, long sb, long s
 Handle* stft_create(int filter_length, int hop_length, const float* fwd_basis, const float* inv_basis, int device);
 void stft_transform(Handle* h, const float* wav, int B, long n_samples, float* mag, float* phase, cudaStream_t st);
 void stft_inverse(Handle* h, const float* mag, const float* phase, int B, int T, float* wav, cudaStream_t st);
+
+Handle* pvt_create(const agpt_pvt_cfg* cfg, const float* const* W, int nW, int device);
+void pvt_frames(const agpt_pvt_cfg* cfg, long n_samples, int grid_hw[4][2]);
+void pvt_forward(Handle* h, const float* wav, int B, long n_samples, float* framewise, float* clipwise, float* logits, cudaStream_t st);
+void pvt_patch7(const float* img, const float* w, const float* bias, const float* gamma, const float* beta, float eps, int B, int H,
+                int W, int C, float* out, cudaStream_t st);
+void pvt_sr_gather(const float* x, int B, int H, int W, int C, int sr, float* out, cudaStream_t st);
+void pvt_dwconv_gelu(const float* x, const float* w, const float* bias, int B, int H, int W, int C, float* out, __half* phi, __half* plo,
+                     cudaStream_t st);
+void pvt_head(const float* x, const float* w, const float* bias, int B, int H, int W, int C, int classes, int ratio, float* framewise,
+              float* clipwise, float* logits, cudaStream_t st);
 
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                    double* out, double* dbg_avg);

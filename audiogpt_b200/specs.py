@@ -1410,3 +1410,115 @@ def synth_lass_wav(n_samples: int, seed: int = 62) -> torch.Tensor:
     x = sum(0.15 / (j + 1) * np.sin(2 * np.pi * rs.uniform(60, 6000) * t + rs.uniform(0, 6)) for j in range(6))
     x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.3, 2) * t)) + 0.02 * rs.randn(int(n_samples))
     return torch.from_numpy(x.astype(np.float32))
+
+
+# ---------------------------------------------------------------------------------------------- sound event detection
+# PVT of the SoundDetection tool (audio_detection/audio_infer/pytorch/models.py:141-237; audio-chatgpt.py:612-673 builds
+# PVT(sample_rate=32000, window_size=1024, hop_size=320, mel_bins=64, fmin=50, fmax=14000, classes_num=527)).  The
+# transformer sizes are fixed inside the reference class (PyramidVisionTransformerV2(...) at :170-188); bn0 is
+# BatchNorm2d(64), so mel_bins is 64.  Block norms and stage norms use eps 1e-6 (the norm_layer partial), the
+# patch-embedding norm and Attention.norm are plain nn.LayerNorm (1e-5).
+PVT_SHIPPED = dict(sample_rate=32000, window_size=1024, hop_size=320, mel_bins=64, fmin=50, fmax=14000, classes_num=527,
+                   embed_dims=(64, 128, 320, 512), depths=(3, 4, 6, 3), num_heads=(1, 2, 5, 8), mlp_ratios=(8, 8, 4, 4),
+                   sr_ratios=(8, 4, 2, 1), interpolate_ratio=32, layer_norm_eps=1e-6, embed_norm_eps=1e-5)
+# the same four-stage structure (sr 8 / 4 / 2 / 1, head dim 64), narrower and one block per stage, with a short window
+PVT_SMALL = dict(PVT_SHIPPED, window_size=256, hop_size=80, classes_num=23, embed_dims=(64, 64, 128, 128),
+                 depths=(1, 1, 1, 1), num_heads=(1, 1, 2, 2), mlp_ratios=(4, 4, 2, 2))
+PVT_STAGES = 4
+
+
+def pvt_grids(cfg, n_samples: int):
+    """The token grid (H = time, W = mel) of every stage for a clip of n_samples: the Python twin of agpt_pvt_frames.
+    T = n // hop + 1 frames; stage 1 is Conv2d(k 7, stride 4, padding 2), stages 2-4 Conv2d(k 3, stride 2, padding 1).
+    Raises ValueError for a clip the network cannot take: no more than window_size // 2 samples (reflect padding), or a
+    stage whose grid is smaller than its sr_ratio (Attention.sr would leave no key)."""
+    n = int(n_samples)
+    if n <= int(cfg["window_size"]) // 2:
+        raise ValueError(f"clip of {n} samples: reflect padding needs more than {int(cfg['window_size']) // 2}")
+    H, W = n // int(cfg["hop_size"]) + 1, int(cfg["mel_bins"])
+    grids = []
+    for i in range(PVT_STAGES):
+        if min(H, W) < (3 if i == 0 else 1):
+            raise ValueError(f"clip of {n} samples is too short: stage {i + 1} has no tokens")
+        H, W = ((H - 3) // 4 + 1, (W - 3) // 4 + 1) if i == 0 else ((H - 1) // 2 + 1, (W - 1) // 2 + 1)
+        sr = int(cfg["sr_ratios"][i])
+        if H < sr or W < sr:
+            raise ValueError(f"clip of {n} samples is too short: stage {i + 1}'s {H} x {W} grid is smaller than its sr_ratio {sr}")
+        grids.append((H, W))
+    return grids
+
+
+def pvt_min_samples(cfg) -> int:
+    """The shortest clip pvt_grids accepts (9600 samples, 0.3 s, for PVT_SHIPPED: stage 1 needs 8 rows, so 31 frames)."""
+    need = 1
+    for i in reversed(range(PVT_STAGES)):
+        need = max(need, int(cfg["sr_ratios"][i]))
+        need = 4 * (need - 1) + 3 if i == 0 else 2 * (need - 1) + 1      # the fewest input rows that give `need` rows
+    return max((need - 1) * int(cfg["hop_size"]), int(cfg["window_size"]) // 2 + 1)
+
+
+def pvt_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of the reference PVT in state-dict order: the frozen front-end buffers the checkpoint
+    carries, bn0, pvt_transformer.patch_embed{i} / block{i}.{j} / norm{i}, fc_audioset."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    n = int(cfg["window_size"])
+    nb = n // 2 + 1
+    s["spectrogram_extractor.stft.conv_real.weight"] = (nb, 1, n)
+    s["spectrogram_extractor.stft.conv_imag.weight"] = (nb, 1, n)
+    s["logmel_extractor.melW"] = (nb, int(cfg["mel_bins"]))
+    _bn_shapes(s, "bn0", int(cfg["mel_bins"]))
+    cin = 1
+    for i in range(PVT_STAGES):
+        C, sr, hid = int(cfg["embed_dims"][i]), int(cfg["sr_ratios"][i]), int(cfg["embed_dims"][i]) * int(cfg["mlp_ratios"][i])
+        k = 7 if i == 0 else 3
+        p = f"pvt_transformer.patch_embed{i + 1}."
+        s[p + "proj.weight"] = (C, cin, k, k); s[p + "proj.bias"] = (C,)
+        s[p + "norm.weight"] = (C,); s[p + "norm.bias"] = (C,)
+        for j in range(int(cfg["depths"][i])):
+            p = f"pvt_transformer.block{i + 1}.{j}."
+            s[p + "norm1.weight"] = (C,); s[p + "norm1.bias"] = (C,)
+            s[p + "attn.q.weight"] = (C, C); s[p + "attn.q.bias"] = (C,)
+            s[p + "attn.kv.weight"] = (2 * C, C); s[p + "attn.kv.bias"] = (2 * C,)
+            s[p + "attn.proj.weight"] = (C, C); s[p + "attn.proj.bias"] = (C,)
+            if sr > 1:
+                s[p + "attn.sr.weight"] = (C, C, sr, sr); s[p + "attn.sr.bias"] = (C,)
+                s[p + "attn.norm.weight"] = (C,); s[p + "attn.norm.bias"] = (C,)
+            s[p + "norm2.weight"] = (C,); s[p + "norm2.bias"] = (C,)
+            s[p + "mlp.fc1.weight"] = (hid, C); s[p + "mlp.fc1.bias"] = (hid,)
+            s[p + "mlp.dwconv.dwconv.weight"] = (hid, 1, 3, 3); s[p + "mlp.dwconv.dwconv.bias"] = (hid,)
+            s[p + "mlp.fc2.weight"] = (C, hid); s[p + "mlp.fc2.bias"] = (C,)
+        s[f"pvt_transformer.norm{i + 1}.weight"] = (C,); s[f"pvt_transformer.norm{i + 1}.bias"] = (C,)
+        cin = C
+    s["fc_audioset.weight"] = (int(cfg["classes_num"]), cin); s["fc_audioset.bias"] = (int(cfg["classes_num"]),)
+    return s
+
+
+def pvt_engine_keys(cfg):
+    """The keys agpt_pvt_create consumes, in its order: the state dict without bn0.num_batches_tracked."""
+    return [k for k in pvt_param_shapes(cfg) if not k.endswith("num_batches_tracked")]
+
+
+def synth_pvt(cfg, seed: int = 3030):
+    """Seeded PVT weights in the checkpoint's layout: the config's periodic-Hann DFT rows and Slaney mel matrix, and
+    random values for everything the reference initialises to a constant (LayerNorm and bn0 affine, bn0's running
+    statistics -- centred on the log-mel range of a speech-level clip --, every bias), so no term is absent."""
+    shapes = pvt_param_shapes(cfg)
+    sd = synth_state_dict(shapes, seed, convtranspose_prefixes=(), gains={"fc_audioset.weight": 3.0})
+    sd["spectrogram_extractor.stft.conv_real.weight"], sd["spectrogram_extractor.stft.conv_imag.weight"] = \
+        stft_dft_weights(int(cfg["window_size"]))
+    sd["logmel_extractor.melW"] = torch.from_numpy(np.ascontiguousarray(slaney_mel(
+        cfg["sample_rate"], cfg["window_size"], cfg["mel_bins"], cfg["fmin"], cfg["fmax"]).T))
+    g = torch.Generator().manual_seed(int(seed) + 1)
+    sd["bn0.running_mean"] = -30.0 + 5.0 * torch.randn(shapes["bn0.running_mean"], generator=g)
+    sd["bn0.running_var"] = 200.0 * (0.5 + torch.rand(shapes["bn0.running_var"], generator=g))
+    sd["bn0.num_batches_tracked"] = torch.tensor(0, dtype=torch.long)
+    return sd
+
+
+def synth_pvt_wav(n_samples: int, seed: int = 33, sr: int = 32000) -> torch.Tensor:
+    """A seeded mono test clip [n_samples] fp32: a few sines under a slow envelope plus noise."""
+    rs = np.random.RandomState(int(seed))
+    t = np.arange(int(n_samples)) / sr
+    x = sum(0.2 / (j + 1) * np.sin(2 * np.pi * rs.uniform(80, 6000) * t + rs.uniform(0, 6)) for j in range(5))
+    x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.5, 3) * t)) + 0.03 * rs.randn(int(n_samples))
+    return torch.from_numpy(x.astype(np.float32))

@@ -507,6 +507,54 @@ int agpt_stft_transform(agpt_handle h, const float* wav, int B, long n_samples, 
 /* STFT.inverse: magnitude / phase [B][filter_length / 2 + 1][T] (device, T >= 2) -> wav [B][(T - 1) hop] (device).   */
 int agpt_stft_inverse(agpt_handle h, const float* magnitude, const float* phase, int B, int T, float* wav, void* stream);
 
+/* ------------------------------------------------------------------ Sound event detection
+ * The SoundDetection tool (audio-chatgpt.py:612-673): audio_detection/audio_infer/pytorch/models.py:141-237 PVT, eval
+ * mode -- torchlibrosa Spectrogram / LogmelFilterBank / bn0 (as Cnn14's), PyramidVisionTransformerV2 (:832-927: four
+ * stages of OverlapPatchEmbed + Blocks of spatial-reduction attention and a depthwise-conv Mlp; no positional
+ * embedding, so any clip length), mean over the mel axis, fc_audioset, sigmoid.  A tagged struct, as agpt_clap_cfg.   */
+typedef struct agpt_pvt_cfg {
+  int window_size;        /* 1024 */
+  int hop_size;           /* 320 */
+  int mel_bins;           /* 64 (bn0 is BatchNorm2d(64)) */
+  int classes_num;        /* 527 */
+  int embed_dims[4];      /* 64, 128, 320, 512; embed_dims[i] = 64 * num_heads[i] */
+  int depths[4];          /* 3, 4, 6, 3 */
+  int num_heads[4];       /* 1, 2, 5, 8 */
+  int mlp_ratios[4];      /* 8, 8, 4, 4 */
+  int sr_ratios[4];       /* 8, 4, 2, 1: Attention.sr = Conv2d(C, C, sr, stride sr) when > 1 */
+  int interpolate_ratio;  /* 32: each framewise row is repeated this many times */
+  float layer_norm_eps;   /* 1e-6: Block.norm1 / norm2 and the stage norms (the norm_layer partial) */
+  float embed_norm_eps;   /* 1e-5: OverlapPatchEmbed.norm and Attention.norm (plain nn.LayerNorm) */
+} agpt_pvt_cfg;
+/* host_weights: fp32 HOST arrays in the key order of audiogpt_b200.specs.pvt_engine_keys(cfg): PVT's state dict without
+ * bn0.num_batches_tracked.  bn0 is folded (eps 1e-5).                                                             */
+int agpt_pvt_create(const agpt_pvt_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* Host only: the token grid (rows = time, columns = mel) of each stage for a clip of n_samples, from the conv
+ * arithmetic T = n / hop + 1; H1 = (T - 3) / 4 + 1, W1 = (mel_bins - 3) / 4 + 1; H(i+1) = (Hi - 1) / 2 + 1, likewise W.
+ * Fails when n_samples <= window_size / 2 (reflect padding), when a grid is empty or when a stage's grid is smaller
+ * than its sr_ratio in either direction (no key would be left).  With the shipped config the shortest clip is
+ * 30 * hop = 9600 samples (0.3 s at 32 kHz): H1 = 8 needs T >= 31.                                                 */
+int agpt_pvt_frames(const agpt_pvt_cfg* cfg, long n_samples, int grid_hw[4][2]);
+/* wav [B][n_samples] (device) -> framewise [B][interpolate_ratio * H4][classes_num] and clipwise [B][classes_num]
+ * (device; H4 from agpt_pvt_frames).  logits, when not NULL: the pre-sigmoid values [B][H4][classes_num].          */
+int agpt_pvt_forward(agpt_handle h, const float* wav, int B, long n_samples, float* framewise, float* clipwise, float* logits,
+                     void* stream);
+/* One launch of each PVT kernel on caller-owned device tensors (the unit tests' entry points).
+ * dwconv_gelu: x [B][H * W][C] -> gelu(depthwise 3 x 3 conv, padding 1, w [C][3][3] and bias [C] on the device) as fp32
+ * (out) or as fp16 hi / lo operand planes (out NULL).  C % 4 == 0.                                                  */
+int agpt_pvt_dwconv_gelu(const float* x, const float* w, const float* bias, int B, int H, int W, int C, float* out, void* plane_hi,
+                         void* plane_lo, void* stream);
+/* patch7: img [B][H][W] -> LayerNorm(Conv2d(1, C, 7, stride 4, padding 2)) as tokens [B][Ho * Wo][C]; w [C][49], bias,
+ * gamma, beta [C] on the device; C in {32, 64, 96, 128}.                                                           */
+int agpt_pvt_patch7(const float* img, const float* w, const float* bias, const float* gamma, const float* beta, float eps, int B,
+                    int H, int W, int C, float* out, void* stream);
+/* sr_gather: x [B][H * W][C] -> out [B][(H / sr) * (W / sr)][sr * sr * C], patch rows in (ky, kx, c) order.        */
+int agpt_pvt_sr_gather(const float* x, int B, int H, int W, int C, int sr, float* out, void* stream);
+/* head: x [B][H * W][C], fc weight [classes][C] and bias on the device -> framewise [B][ratio * H][classes], clipwise
+ * [B][classes], logits [B][H][classes] or NULL.                                                                    */
+int agpt_pvt_head(const float* x, const float* w, const float* bias, int B, int H, int W, int C, int classes, int ratio,
+                  float* framewise, float* clipwise, float* logits, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
