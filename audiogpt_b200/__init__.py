@@ -21,6 +21,8 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.sound_extraction.model.LASSNet.LASSNet            (installed with install(extraction=True))
     audiogpt_b200.sound_extraction.utils.stft.STFT                  (installed with install(extraction=True))
     audiogpt_b200.audio_detection.audio_infer.pytorch.models.PVT    (installed with install(detection=True))
+    audiogpt_b200.audio_detection.target_sound_detection.src.models.RaDur_fusion
+                                                                    (installed with install(target_detection=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -78,9 +80,17 @@ _DETECTION_MAP = {
     "audio_infer.pytorch.models": ("audiogpt_b200.audio_detection.audio_infer.pytorch.models", ["PVT"]),
 }
 
+# the target-sound-detection tool's RaDur_fusion, grafted only on request (install(target_detection=True)).  The tool
+# also imports the reference module's event_labels, so the module is patched in place and never aliased: when it does
+# not import, the name is reported as skipped.
+_TARGET_DETECTION_MAP = {
+    "target_sound_detection.src.models": ("audiogpt_b200.audio_detection.target_sound_detection.src.models", ["RaDur_fusion"]),
+}
+
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
-            text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False, detection: bool = False):
+            text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False, detection: bool = False,
+            target_detection: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -111,6 +121,10 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     pyramid transformer and framewise head run on the engine.  The agent script imports that name when it is loaded, so
     call install first; only the ``models`` leaf is aliased, the packages ``audio_infer`` and ``audio_infer.pytorch``
     (from which the script also imports ``audio_infer.utils.config``) stay the reference's own.
+    ``target_detection=True`` also replaces ``target_sound_detection.src.models.RaDur_fusion``, so the TargetSoundDetection
+    tool's Cnn14 reference encoder, multi-scale CNN, bidirectional GRU and enhancement pass run on the engine.  That
+    module is only patched in place: the tool also imports its ``event_labels``, so when it does not import it is
+    reported as skipped (and raises under ``strict``), never aliased.
     Returns the list of patched names."""
     import importlib
     import sys
@@ -145,6 +159,19 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
                 mine._reference_cls = theirs
             setattr(ref, a, mine)
         patched.append(ref_name)
+    if target_detection:
+        for ref_name, (our_name, attrs) in _TARGET_DETECTION_MAP.items():
+            ours = importlib.import_module(our_name)
+            try:
+                ref = importlib.import_module(ref_name)
+            except Exception:
+                if strict:
+                    raise
+                patched.append(ref_name + " (skipped: not importable)")
+                continue
+            for a in attrs:
+                setattr(ref, a, getattr(ours, a))
+            patched.append(ref_name)
     if inpaint:
         from .ldm.modules.diffusionmodules.openaimodel import AttentionUNetModel, UNetModel
         UNetModel._attention_cls = AttentionUNetModel

@@ -106,6 +106,12 @@ class PvtConfig(C.Structure):
         ("interpolate_ratio", C.c_int), ("layer_norm_eps", C.c_float), ("embed_norm_eps", C.c_float)]
 
 
+class TsdConfig(C.Structure):
+    """agpt_tsd_cfg (a tagged struct in the header, like agpt_clap_cfg; the create entry point takes a plain pointer)."""
+    _fields_ = [(n, C.c_int) for n in ("time_resolution", "att_pool", "enhancement", "top")] + [
+        ("tao", C.c_float), ("mel_bins", C.c_int), ("outputdim", C.c_int)]
+
+
 class TapconvProbeArgs(C.Structure):
     """agpt_tapconv_probe_args (a tagged struct in the header: it carries pointers and floats)."""
     _fields_ = [(n, C.c_int) for n in ("kind", "Cin", "Cout", "K", "dil", "Wreal", "strip_w", "u", "pad", "g")] + [
@@ -198,6 +204,14 @@ PROTOTYPES = {
     "agpt_pvt_patch7": (_I, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _I, _P, _P]),
     "agpt_pvt_sr_gather": (_I, [_P, _I, _I, _I, _I, _I, _P, _P]),
     "agpt_pvt_head": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
+    "agpt_tsd_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_tsd_frames": (_I, [_P, _I, _I, _P]),
+    "agpt_tsd_forward": (_I, [_P, _P, _P, _I, _I, _I, _P, _P, _P]),
+    "agpt_tsd_stage_events": (_I, [_P, _P, _I]),
+    "agpt_tsd_stem": (_I, [_P, _P, _P, _I, _I, _I, _P, _P]),
+    "agpt_tsd_avgpool": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "agpt_tsd_gru": (_I, [_P, _P, _P, _I, _I, _P, _P]),
+    "agpt_tsd_enhance": (_I, [_P, _I, _I, _I, _P, _I, _P, _I, _F, _W, _P, _P, _P, _P, _P]),
 }
 
 _lock = threading.Lock()

@@ -476,6 +476,65 @@ int agpt_pvt_head(const float* x, const float* w, const float* bias, int B, int 
   });
 }
 
+int agpt_tsd_create(const agpt_tsd_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(tsd_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_tsd_frames(const agpt_tsd_cfg* cfg, int T, int Tr, int frames[3]) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && frames, "null argument");
+    tsd_frames(cfg, T, Tr, frames);
+  });
+}
+
+int agpt_tsd_forward(agpt_handle h, const float* x, const float* ref, int B, int T, int Tr, float* decision, float* decision_up,
+                     void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(x && ref && decision && decision_up, "null argument");
+    tsd_forward(as(h, kMagicTsd, "tsd"), x, ref, B, T, Tr, decision, decision_up, (cudaStream_t)stream);
+  });
+}
+
+int agpt_tsd_stage_events(agpt_handle h, void* events, int n) {
+  return guarded([&] {
+    AGPT_CHECK(n == 0 || events, "null argument");
+    tsd_stage_events(as(h, kMagicTsd, "tsd"), static_cast<void* const*>(events), n);
+  });
+}
+
+int agpt_tsd_stem(const float* mel, const float* w, const float* b, int B, int T, int ph, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(mel && w && b && out, "null argument");
+    tsd_stem(mel, w, b, B, T, ph, out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_tsd_avgpool(const float* in, int B, int H, int W, int C, int ph, int pw, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(in && out, "null argument");
+    tsd_avgpool(in, B, H, W, C, ph, pw, out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_tsd_gru(const float* w_hh, const float* b_hh, const float* xproj, int B, int T, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(w_hh && b_hh && xproj && out, "null argument");
+    tsd_gru(w_hh, b_hh, xproj, B, T, out, (cudaStream_t)stream);
+  });
+}
+
+int agpt_tsd_enhance(const float* p1, int B, int Td, int O, const float* mix_emb, int Te, const float* emb, int top, float tao,
+                     const float* const* weights8, float* me, float* wmix, int* topk_idx, float* topk_val, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(p1 && mix_emb && emb && weights8 && me && wmix && topk_idx, "null argument");
+    for (int i = 0; i < 8; ++i) AGPT_CHECK(weights8[i], "null weight");
+    tsd_enhance(p1, B, Td, O, mix_emb, Te, emb, top, tao, weights8, me, wmix, topk_idx, topk_val, (cudaStream_t)stream);
+  });
+}
+
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                        double* out2, double* dbg8_or_null) {
   return guarded([&] {

@@ -12,6 +12,7 @@
 #include "fs_layers.cuh"
 #include "clap.cuh"
 #include "logmel.cuh"
+#include "convblock.cuh"
 
 namespace agpt {
 
@@ -179,8 +180,8 @@ struct Cnn14Net : Handle {
     const float* in = img.p;
     int H = T, W = nm;
     for (int i = 0; i < kCnn14Blocks; ++i) {
-      conv3x3(conv[i][0], in, bufB.p, B, H, W, st);
-      conv3x3(conv[i][1], bufB.p, bufC.p, B, H, W, st);
+      conv3x3_relu(conv[i][0], in, bufB.p, B, H, W, st);
+      conv3x3_relu(conv[i][1], bufB.p, bufC.p, B, H, W, st);
       if (i < kCnn14Blocks - 1) {
         avgpool2(bufC.p, bufA.p, B, H, W, kCnn14Ch[i], st);
         H /= 2; W /= 2;
@@ -197,28 +198,7 @@ struct Cnn14Net : Handle {
     proj.run(emb.p, cfg.out_emb, B, out, st);
     AGPT_CUDA(cudaGetLastError());
   }
-
-  void conv3x3(const PackedConv& pc, const float* in, float* out, int B, int H, int W, cudaStream_t st) {
-    TapConvParams P = tapconv_params(pc, B, H * W, W, 1);
-    P.in = in; P.in_gstride = (long)H * W * pc.Cin; P.in_pitch = pc.Cin;
-    P.out = out; P.out_gstride = (long)H * W * pc.Cout; P.out_pitch = pc.Cout;
-    P.epi = EPI_RELU;
-    tapconv_launch(P, st);
-  }
 };
-
-// BatchNorm2d (eval) folded into the preceding bias-free conv: w' = w * s, b' = beta - mean * s, s = gamma / sqrt(var + eps)
-static void load_conv_bn(PackedConv& pc, const float* w, WeightCursor& wc, int cout, int cin, int cin_pad) {
-  const float* g = wc.next(); const float* be = wc.next(); const float* rm = wc.next(); const float* rv = wc.next();
-  std::vector<float> wf((size_t)cout * cin_pad * 9, 0.f), bf(cout);
-  for (int co = 0; co < cout; ++co) {
-    const float s = g[co] / sqrtf(rv[co] + kBnEps);
-    bf[co] = be[co] - rm[co] * s;
-    for (int ci = 0; ci < cin; ++ci)
-      for (int k = 0; k < 9; ++k) wf[((size_t)co * cin_pad + ci) * 9 + k] = w[((size_t)co * cin + ci) * 9 + k] * s;
-  }
-  pack_conv(pc, wf.data(), bf.data(), cout, cin_pad, 9, true);
-}
 
 Handle* cnn14_create(const agpt_cnn14_cfg* cfg, const float* const* W, int nW, int device) {
   DeviceGuard dg_(device);
@@ -233,8 +213,8 @@ Handle* cnn14_create(const agpt_cnn14_cfg* cfg, const float* const* W, int nW, i
   for (int i = 0; i < kCnn14Blocks; ++i) {
     const int c = kCnn14Ch[i];
     const float* w1 = wc.next(); const float* w2 = wc.next();
-    load_conv_bn(h->conv[i][0], w1, wc, c, cin, round_up(cin, 4));
-    load_conv_bn(h->conv[i][1], w2, wc, c, c, c);
+    load_conv_bn(h->conv[i][0], w1, wc, c, cin, round_up(cin, 4), kBnEps);
+    load_conv_bn(h->conv[i][1], w2, wc, c, c, c, kBnEps);
     cin = c;
   }
   { auto w = wc.next(); auto b = wc.next(); pack_conv(h->fc1, w, b, cfg->out_emb, cin, 1, false); }

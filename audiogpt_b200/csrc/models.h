@@ -91,6 +91,17 @@ void pvt_dwconv_gelu(const float* x, const float* w, const float* bias, int B, i
 void pvt_head(const float* x, const float* w, const float* bias, int B, int H, int W, int C, int classes, int ratio, float* framewise,
               float* clipwise, float* logits, cudaStream_t st);
 
+Handle* tsd_create(const agpt_tsd_cfg* cfg, const float* const* W, int nW, int device);
+void tsd_frames(const agpt_tsd_cfg* cfg, int T, int Tr, int frames[3]);
+void tsd_forward(Handle* h, const float* x, const float* ref, int B, int T, int Tr, float* decision, float* decision_up, cudaStream_t st);
+constexpr int kTsdStages = 6;   // agpt_tsd_stage_events: the stage boundaries one forward records
+void tsd_stage_events(Handle* h, void* const* events, int n);
+void tsd_stem(const float* mel, const float* w, const float* b, int B, int T, int ph, float* out, cudaStream_t st);
+void tsd_avgpool(const float* in, int B, int H, int W, int C, int ph, int pw, float* out, cudaStream_t st);
+void tsd_gru(const float* whh, const float* bhh, const float* xp, int B, int T, float* out, cudaStream_t st);
+void tsd_enhance(const float* p1, int B, int Td, int O, const float* Emix, int Te, const float* emb, int top, float tao,
+                 const float* const wts[8], float* me, float* wmix, int* idx, float* val, cudaStream_t st);
+
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                    double* out, double* dbg_avg);
 void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);

@@ -1522,3 +1522,153 @@ def synth_pvt_wav(n_samples: int, seed: int = 33, sr: int = 32000) -> torch.Tens
     x = sum(0.2 / (j + 1) * np.sin(2 * np.pi * rs.uniform(80, 6000) * t + rs.uniform(0, 6)) for j in range(5))
     x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.5, 3) * t)) + 0.03 * rs.randn(int(n_samples))
     return torch.from_numpy(x.astype(np.float32))
+
+
+# ---------------------------------------------------------------------------------------------- target sound detection
+# RaDur_fusion of the TargetSoundDetection tool (audio_detection/target_sound_detection/src/models.py:1109-1291;
+# audio-chatgpt.py:775-806 builds it with inputdim=64, outputdim=2 and tao = 0.6).  The checkpoint's run_config.pth,
+# which holds att_pool, enhancement, top and time_resolution, is not in the reference tree: TSD_DEFAULT takes the
+# heaviest path (attention pooling and the enhancement pass) with the tool's default time_resolution and tao, and top
+# is a stand-in.  The network sizes are fixed inside the reference classes.
+TSD_DEFAULT = dict(time_resolution=125, att_pool=True, enhancement=True, top=10, tao=0.6, mel_bins=64, outputdim=2)
+TSD_DET_CHANNELS = (128, 256, 512)       # Cnn10_mul_scale.conv_block2..4
+TSD_EMB = 128                            # Cnn14.fc1 width
+TSD_GRU = 512
+# Cnn10_mul_scale's pool sizes by scale (models.py:436-455); CDur_CNN_mul_scale_fusion maps time_resolution 125 / 250 /
+# 500 / anything else to scale 8 / 4 / 2 / 0
+TSD_POOLS = {8: ((2, 2), (2, 2), (2, 4), (1, 4)), 4: ((2, 2), (2, 2), (1, 4), (1, 4)),
+             2: ((2, 2), (1, 2), (1, 4), (1, 4)), 0: ((1, 2), (1, 2), (1, 4), (1, 4))}
+TSD_ENC_POOLS = ((2, 2),) * 3 + ((1, 2),) * 3
+
+
+def tsd_scale(time_resolution) -> int:
+    return {125: 8, 250: 4, 500: 2}.get(int(time_resolution), 0)
+
+
+def tsd_stem_rows(T: int, ph: int):
+    """The stem's pooled row counts (H1, H2, H3, m) for a T-frame mel: the 1 x 1 / 3 x 3 / 5 x 5 GLU branches (all with
+    padding 1) pooled by ph rows, and m = min(min(H1, 500), H2, H3 + 1), the rows the concat keeps."""
+    if T < 3 or T - 2 < ph:
+        raise ValueError(f"clip of {T} frames is too short: the 5 x 5 stem branch has no pooled row")
+    H1, H2, H3 = (T + 2) // ph, T // ph, (T - 2) // ph
+    return H1, H2, H3, min(min(H1, 500), H2, H3 + 1)
+
+
+def tsd_frames(cfg, T: int, Tr: int):
+    """(T', Tr', Te): the detection frames of a T-frame clip, the reference encoder's frames of a Tr-frame reference and
+    the mixture encoder's frames (0 without enhancement) -- the Python twin of agpt_tsd_frames.  Raises ValueError when
+    any of them would be 0."""
+    T, Tr = int(T), int(Tr)
+    pools = TSD_POOLS[tsd_scale(cfg["time_resolution"])]
+    H = tsd_stem_rows(T, pools[0][0])[3]
+    for ph, _ in pools[1:]:
+        if H < ph:
+            raise ValueError(f"clip of {T} frames is too short: a detection pool has no output row")
+        H //= ph
+    if Tr < 8:
+        raise ValueError(f"reference of {Tr} frames is too short: Cnn14 needs 8 frames for one output frame")
+    Te = 0
+    if cfg["enhancement"]:
+        if T < 8:
+            raise ValueError(f"clip of {T} frames is too short: the enhancement's Cnn14 needs 8 frames")
+        Te = T // 8
+    return H, Tr // 8, Te
+
+
+def tsd_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of the reference RaDur_fusion in state-dict order: encoder (Cnn14 with the
+    torchlibrosa front end and fc_audioset it never runs), detection (Cnn10_mul_scale, GRU, fc, fusion, outputlayer),
+    q, k, q_ee, k_ee, bn, EE_fusion."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    e = "encoder."
+    s[e + "spectrogram_extractor.stft.conv_real.weight"] = (513, 1, 1024)     # Cnn14() defaults: window 1024, 32 kHz
+    s[e + "spectrogram_extractor.stft.conv_imag.weight"] = (513, 1, 1024)
+    s[e + "logmel_extractor.melW"] = (513, 64)
+    _bn_shapes(s, e + "bn0", 64)
+    cin = 1
+    for i, c in enumerate(CNN14_CHANNELS):
+        p = f"{e}conv_block{i + 1}."
+        s[p + "conv1.weight"] = (c, cin, 3, 3)
+        s[p + "conv2.weight"] = (c, c, 3, 3)
+        _bn_shapes(s, p + "bn1", c)
+        _bn_shapes(s, p + "bn2", c)
+        cin = c
+    s[e + "fc1.weight"] = (TSD_EMB, cin); s[e + "fc1.bias"] = (TSD_EMB,)
+    s[e + "fc_audioset.weight"] = (527, TSD_EMB); s[e + "fc_audioset.bias"] = (527,)
+    f = "detection.features."
+    for j, k in enumerate((1, 3, 5)):
+        s[f"{f}conv_block1_{j + 1}.conv1.weight"] = (64, 1, k, k)
+        _bn_shapes(s, f"{f}conv_block1_{j + 1}.bn1", 64)
+    cin = 96
+    for i, c in enumerate(TSD_DET_CHANNELS):
+        p = f"{f}conv_block{i + 2}."
+        s[p + "conv1.weight"] = (c, cin, 3, 3)
+        s[p + "conv2.weight"] = (c, c, 3, 3)
+        _bn_shapes(s, p + "bn1", c)
+        _bn_shapes(s, p + "bn2", c)
+        cin = c
+    for sfx in ("", "_reverse"):
+        s[f"detection.gru.weight_ih_l0{sfx}"] = (3 * TSD_GRU, TSD_GRU)
+        s[f"detection.gru.weight_hh_l0{sfx}"] = (3 * TSD_GRU, TSD_GRU)
+        s[f"detection.gru.bias_ih_l0{sfx}"] = (3 * TSD_GRU,)
+        s[f"detection.gru.bias_hh_l0{sfx}"] = (3 * TSD_GRU,)
+    s["detection.fc.weight"] = (256, 2 * TSD_GRU); s["detection.fc.bias"] = (256,)
+    s["detection.fusion.fuse_layer1.conv.weight"] = (1024, TSD_EMB, 1); s["detection.fusion.fuse_layer1.conv.bias"] = (1024,)
+    s["detection.fusion.fuse_layer2.conv.weight"] = (1024, 512, 1); s["detection.fusion.fuse_layer2.conv.bias"] = (1024,)
+    O = int(cfg["outputdim"])
+    s["detection.outputlayer.weight"] = (O, 256); s["detection.outputlayer.bias"] = (O,)
+    for n in ("q", "k", "q_ee", "k_ee"):
+        s[n + ".weight"] = (TSD_EMB, TSD_EMB); s[n + ".bias"] = (TSD_EMB,)
+    _bn_shapes(s, "bn", TSD_EMB)
+    for n in ("fuse_layer1", "fuse_layer2"):
+        s[f"EE_fusion.{n}.conv.weight"] = (4 * TSD_EMB, TSD_EMB, 1); s[f"EE_fusion.{n}.conv.bias"] = (4 * TSD_EMB,)
+    return s
+
+
+def tsd_engine_keys(cfg):
+    """The keys agpt_tsd_create consumes, in its order: the state dict without the encoder's front end (its forward takes
+    a mel), encoder.fc_audioset and every num_batches_tracked."""
+    skip = ("encoder.spectrogram_extractor.", "encoder.logmel_extractor.", "encoder.bn0.", "encoder.fc_audioset.")
+    return [k for k in tsd_param_shapes(cfg) if not k.startswith(skip) and not k.endswith("num_batches_tracked")]
+
+
+def synth_tsd(cfg, seed: int = 7171, out_shift: float = 0.0):
+    """Seeded RaDur_fusion weights in the checkpoint's layout: convs at He gain, BatchNorm running statistics with
+    positive variance, the encoder's front end as torchlibrosa builds it for Cnn14()'s defaults, and an outputlayer at 4x
+    gain whose class-0 bias is moved by out_shift (the fixtures use it to put the gate tao inside the top-k scores)."""
+    shapes = tsd_param_shapes(cfg)
+    sd = synth_state_dict(shapes, seed, convtranspose_prefixes=(),
+                          gains={"encoder.conv_block": math.sqrt(2.0), "detection.features.conv_block": math.sqrt(2.0),
+                                 "detection.outputlayer.weight": 4.0})
+    sd["encoder.spectrogram_extractor.stft.conv_real.weight"], sd["encoder.spectrogram_extractor.stft.conv_imag.weight"] = \
+        stft_dft_weights(1024)
+    sd["encoder.logmel_extractor.melW"] = torch.from_numpy(np.ascontiguousarray(slaney_mel(32000, 1024, 64, 50, 14000).T))
+    g = torch.Generator().manual_seed(int(seed) + 1)
+    for k, shape in shapes.items():
+        if k.endswith("num_batches_tracked"):
+            sd[k] = torch.tensor(0, dtype=torch.long)
+        elif k.endswith("running_mean"):
+            sd[k] = 0.1 * torch.randn(shape, generator=g)
+        elif k.endswith("running_var"):
+            sd[k] = 0.5 + torch.rand(shape, generator=g)
+    sd["detection.outputlayer.bias"] = sd["detection.outputlayer.bias"].clone()
+    sd["detection.outputlayer.bias"][0] += float(out_shift)
+    return sd
+
+
+def synth_tsd_mel(T: int, seed: int, B: int = 1) -> torch.Tensor:
+    """Seeded log-mel clips [B][T][64] fp32 on the scale of the tool's log(mel + eps) features: a per-band floor, a few
+    sustained events with their own spectral shape, and noise."""
+    rs = np.random.RandomState(int(seed))
+    T = int(T)
+    t = np.arange(T)[:, None]
+    x = np.empty((B, T, 64))
+    for b in range(B):
+        v = -7.0 + 1.5 * np.cos(np.arange(64) / 64 * np.pi)[None, :] + 0.8 * rs.randn(T, 64)
+        for _ in range(3):
+            on = rs.randint(0, max(T - 4, 1))
+            dur = rs.randint(4, max(T // 3, 5))
+            env = ((t >= on) & (t < on + dur)).astype(np.float64)
+            v = v + env * (3.0 + 2.0 * rs.rand(1, 64) + 0.5 * np.sin(t / rs.uniform(2, 10)))
+        x[b] = v
+    return torch.from_numpy(x.astype(np.float32))

@@ -555,6 +555,54 @@ int agpt_pvt_sr_gather(const float* x, int B, int H, int W, int C, int sr, float
 int agpt_pvt_head(const float* x, const float* w, const float* bias, int B, int H, int W, int C, int classes, int ratio,
                   float* framewise, float* clipwise, float* logits, void* stream);
 
+/* ------------------------------------------------------------------ Target sound detection
+ * The TargetSoundDetection tool (audio-chatgpt.py:775-875): audio_detection/target_sound_detection/src/models.py:1109-1291
+ * RaDur_fusion, eval mode -- Cnn14 (mel input, no front end) embeds the reference clip, Cnn10_mul_scale (a 1 x 1 /
+ * 3 x 3 / 5 x 5 GLU stem, then three ConvBlocks) and Fusion(128, 512, 2) feed a bidirectional GRU(512, 512), fc,
+ * outputlayer and a softmax; with enhancement the first decision's top-k frames select mixture embeddings that make a
+ * second fused embedding and a second GRU pass, and the two decisions are mixed.  A tagged struct, as agpt_clap_cfg.  */
+typedef struct agpt_tsd_cfg {
+  int time_resolution;    /* 125 / 250 / 500 / other: Cnn10_mul_scale(8 / 4 / 2 / 0), which sets the pool sizes */
+  int att_pool;           /* 1: attention-pool the reference embeddings (after RaDur_fusion.bn); 0: their plain mean */
+  int enhancement;        /* 1: run orcal_EE (the second, top-k enhanced pass) */
+  int top;                /* >= 1: frames in the top-k (all T' frames when T' < top) */
+  float tao;              /* the top-k score gate (the tool sets 0.6) */
+  int mel_bins;           /* 64 */
+  int outputdim;          /* 2 (1..16) */
+} agpt_tsd_cfg;
+/* host_weights: fp32 HOST arrays in the key order of audiogpt_b200.specs.tsd_engine_keys(cfg): RaDur_fusion's state dict
+ * without the encoder's unused front end (spectrogram_extractor, logmel_extractor, bn0), fc_audioset and
+ * num_batches_tracked.  BatchNorm eps 1e-5.                                                                         */
+int agpt_tsd_create(const agpt_tsd_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* Host only: frames[0] = T', the detection frames of a T-frame clip (the stem keeps min(floor((T + 2) / ph), 500,
+ * floor(T / ph), floor((T - 2) / ph) + 1) rows, then the three pools divide by their row sizes); frames[1] = Tr / 8,
+ * the reference encoder's frames; frames[2] = T / 8 with enhancement, else 0.  Fails when any of them would be 0.    */
+int agpt_tsd_frames(const agpt_tsd_cfg* cfg, int T, int Tr, int frames[3]);
+/* x [B][T][64], ref [B][Tr][64] log-mels (device) -> decision [B][T'] (the final decision's class 0) and decision_up
+ * [B][T][outputdim] (the final decision linearly interpolated to T, align_corners = False).  With enhancement and
+ * T' > T / 8 (time_resolution other than 125), a top-k frame past T / 8 is refused, as the reference's gather fails.   */
+int agpt_tsd_forward(agpt_handle h, const float* x, const float* ref, int B, int T, int Tr, float* decision, float* decision_up,
+                     void* stream);
+/* Timing: events points to n = 7 cudaEvent_t (or n = 0 to stop) that every later forward records at its stage
+ * boundaries: start, after the reference embedding, after the mixture's Cnn14 (enhancement), after the detection
+ * features, after the first GRU pass, after the enhancement and second pass, end.                                  */
+int agpt_tsd_stage_events(agpt_handle h, void* events, int n);
+/* One launch of each new RaDur_fusion kernel on caller-owned device tensors (the unit tests' entry points).
+ * stem: mel [B][T][64] -> [B][m][32][96] (m as in agpt_tsd_frames); w [3][64][25] (branch k = 1, 3, 5: the k * k
+ * taps of each output channel first) and b [3][64] are the convs with BatchNorm folded; ph (1 or 2) the row pool.    */
+int agpt_tsd_stem(const float* mel, const float* w, const float* b, int B, int T, int ph, float* out, void* stream);
+/* avgpool: F.avg_pool2d(kernel = stride = (ph, pw)) on channels-last in [B][H][W][C] -> out [B][H / ph][W / pw][C].  */
+int agpt_tsd_avgpool(const float* in, int B, int H, int W, int C, int ph, int pw, float* out, void* stream);
+/* gru: the recurrence of a bidirectional GRU(512, 512): w_hh [2][1536][512], b_hh [2][1536] (forward, reverse), xproj
+ * [B][T][3072] = the input projections W_ih x + b_ih (forward r, z, n | reverse r, z, n) -> out [B][T][1024].        */
+int agpt_tsd_gru(const float* w_hh, const float* b_hh, const float* xproj, int B, int T, float* out, void* stream);
+/* enhance: the tail of orcal_EE.  p1 [B][Td][O] the first decision (softmax), mix_emb [B][Te][128] bn(Cnn14(x)), emb
+ * [B][128]; weights (device) q_ee.weight [128][128], q_ee.bias, k_ee.weight, k_ee.bias, EE_fusion.fuse_layer1.conv
+ * weight [512][128] and bias, fuse_layer2 weight and bias -> me [B][128] (EE_fusion's output), wmix [B] (the second
+ * decision's weight), topk_idx [B][k] int32 and topk_val [B][k] (may be NULL), k = min(top, Td), Td <= 500.           */
+int agpt_tsd_enhance(const float* p1, int B, int Td, int O, const float* mix_emb, int Te, const float* emb, int top, float tao,
+                     const float* const* weights8, float* me, float* wmix, int* topk_idx, float* topk_val, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
