@@ -342,6 +342,7 @@ struct Hifigan : Handle {
   bool plane_feed = true;           // AGPT_PLANE_FEED=0: every tap-GEMM converts its fp32 input itself
   bool pair_dual = true;            // AGPT_PAIR_DUAL=0: no fused pair runs two CTAs per SM (TapConvParams::tc_dual)
   bool pair_pipe = true;            // AGPT_PAIR_PIPE=0: no C = 128 pair runs two tiles per CTA (TapConvParams::tc_pipe)
+  bool narrow_pipe = true;          // AGPT_NARROW_PIPE=0: narrow pairs keep two CTAs per SM (TapConvParams::tc_narrow_pipe)
 
   ~Hifigan() override {
     if (pin_mel) cudaFreeHost(pin_mel);
@@ -476,6 +477,7 @@ struct Hifigan : Handle {
             P1.epi = EPI_BIAS;
             P1.tc_dual = pair_dual;
             P1.tc_pipe = pair_pipe;
+            P1.tc_narrow_pipe = narrow_pipe;
             feed(P1, C);
             TapConvParams P2 = conv(rb.c2[n], rb.c2g[n], gq, 1, A, dst);
             residual_epi(P2);
@@ -547,6 +549,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   { const char* e = getenv("AGPT_PLANE_FEED"); h->plane_feed = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_PAIR_DUAL"); h->pair_dual = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_PAIR_PIPE"); h->pair_pipe = !(e && e[0] == '0'); }
+  { const char* e = getenv("AGPT_NARROW_PIPE"); h->narrow_pipe = !(e && e[0] == '0'); }
   WeightCursor wc{W, nW};
   { const float* w = wc.next(); const float* b = wc.next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
   h->ups.resize(nu);

@@ -12,8 +12,9 @@ constexpr int PROF_PAIR = 16;   // record epi code of a fused ResBlock pair: 16 
 static std::vector<ProfRec> g_recs;
 static long long g_tall = 0;    // recorded launches that ran 256-row tiles (the dump line has no field for it)
 static long long g_plane = 0;   // recorded launches that were plane-fed (likewise)
-static long long g_dual = 0;    // recorded launches of the two-CTAs-per-SM pair kernel (likewise)
+static long long g_dual = 0;    // recorded launches of narrow pairs with overlapped tiles (likewise)
 static long long g_pipe = 0;    // recorded launches of the two-tiles-per-CTA pair kernel (likewise)
+static long long g_narrow = 0;  // recorded launches of the narrow pair pipeline (likewise)
 
 bool profile_enabled() { return g_prof; }
 
@@ -26,6 +27,7 @@ void profile_enable(int on) {
     g_plane = 0;
     g_dual = 0;
     g_pipe = 0;
+    g_narrow = 0;
   }
 }
 
@@ -41,6 +43,8 @@ void profile_count_dual() { if (g_prof) ++g_dual; }
 long long profile_dual_launches() { return g_dual; }
 void profile_count_pipe() { if (g_prof) ++g_pipe; }
 long long profile_pipe_launches() { return g_pipe; }
+void profile_count_narrow_pipe() { if (g_prof) ++g_narrow; }
+long long profile_narrow_pipe_launches() { return g_narrow; }
 
 // Sums over the records since profile_enable(1): per variant (FMA BN = 128, 64, 32; 3 = wgmma)
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches) {

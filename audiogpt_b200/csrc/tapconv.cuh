@@ -86,6 +86,9 @@ struct TapConvParams {
   // 1: a C = 128 fused pair may run on tcpair_pipe_kernel (two tiles in flight per CTA); set by the HiFi-GAN driver
   // unless AGPT_PAIR_PIPE=0.
   int tc_pipe;
+  // 1: a narrow fused pair that tc_dual allows may run on tcpair_narrow_kernel (persistent, several tiles in flight
+  // per CTA) before tcpair2_kernel; set by the HiFi-GAN driver unless AGPT_NARROW_PIPE=0.
+  int tc_narrow_pipe;
 };
 
 __host__ __device__ inline int tc_wv(const TapConvParams& P) { return P.Wreal > 0 ? (P.strips > 0 ? P.strip_w + 2 : P.Wreal + 1) : 0; }
@@ -154,10 +157,12 @@ void* profile_begin_pair(const TapConvParams& c1, const TapConvParams& c2, cudaS
 void profile_end(void* rec, cudaStream_t st);
 void profile_count_tall();            // a tensor-core launch with 256-row tiles (counted while profiling)
 long long profile_tall_launches();
-void profile_count_dual();            // a fused-pair launch with two CTAs per SM (counted while profiling)
+void profile_count_dual();            // a launch of narrow pairs with overlapped tiles (counted while profiling)
 long long profile_dual_launches();
 void profile_count_pipe();            // a fused-pair launch of tcpair_pipe_kernel (counted while profiling)
 long long profile_pipe_launches();
+void profile_count_narrow_pipe();     // a fused-pair launch of tcpair_narrow_kernel (counted while profiling)
+long long profile_narrow_pipe_launches();
 void profile_count_plane();           // a plane-fed tensor-core launch (counted while profiling)
 long long profile_plane_launches();
 // The variant of the most recent tap-GEMM launch on this host thread, {1 tensor-core | 0 fp32-FMA, tile width, tile

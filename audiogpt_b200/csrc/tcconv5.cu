@@ -1042,6 +1042,331 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
   }
 }
 
+// ---- narrow fused pairs (BN = 64 / 32) on a persistent, warp-specialised tile pipeline (tcpair_narrow_kernel) ----
+// At C <= 64 a pair tile's wgmmas are a small part of its time; the rest is per-row work (input load, hi/lo transform,
+// hand-off, epilogue) and the latencies around it, and every tap's wgmmas accumulate in order into one accumulator, a
+// dependent chain.  This kernel gives each kind of work its own warps and keeps NS tiles in flight per CTA:
+//   warpgroups 0-1  each runs whole tiles (0: tiles 0, 2, ..; 1: tiles 1, 3, ..) in two 64-row accumulators, so four
+//                   chains run per SM: c1's wgmmas, the c1 -> c2 hand-off, c2's wgmmas, c2's accumulator x descale ->
+//                   fp32 dump
+//   warpgroup 2     transform: the staged fp32 input rows -> leaky ReLU -> hi / lo operand tile
+//   warpgroup 3     epilogue: the dump + bias + residual (read from the staged input rows: P2.res is P1.in) + the old
+//                   MRF sum (EPI_ACC) -> stores; it loads the old sum before the dump is ready
+//   warp 16         the input rows of each tile by TMA (32-channel fp32 boxes, zero outside the sample), NS tiles ahead
+//   warp 17         the weight stages: all of c1's and c2's loaded once where they fit (NW == iterations per tile),
+//                   else streamed through one ring, one pass per pair of tiles, read by both wgmma warpgroups
+// Set s (tiles k = s mod NS) is an operand region of 256 R1 bytes (c1's hi / lo tile, then c2's, then the dump) and a
+// staging region of R1 x 128 B per 32 input channels; its life is raw(k) -> operand(k) -> c2 operand(k) -> dump(k) ->
+// epilogue(k) -> raw(k + NS).  Tile geometry, wgmma shapes and per-row order, operand bits, hand-off and epilogue
+// arithmetic are those of tcpair_kernel<BN, 128>, so every output is bit-identical.  Launched at 96 registers per
+// thread, the warpgroups rebalance them (setmaxnreg): 2 x 112 (wgmma) + 80 (transform) + 152 (epilogue) + 24.
+constexpr int NARROW_THREADS = 640;
+constexpr int NARROW_MMA = 256, NARROW_DATA = 128, NARROW_WG = 128;
+constexpr int NARROW_MMA_REGS = 112, NARROW_XF_REGS = 80, NARROW_EPI_REGS = 152;   // + 24: 5 x 96 in all
+constexpr int NARROW_MAX_NS = 4, NARROW_MAX_NW = 22;
+struct NarrowSmem { uint32_t op[NARROW_MAX_NS], raw[NARROW_MAX_NS], w[NARROW_MAX_NW], bars, total; };
+__host__ __device__ inline void narrow_layout(NarrowSmem& s, int BN, int R1, int nbox, int NS, int NW) {
+  uint32_t o = 0;
+  for (int i = 0; i < NARROW_MAX_NS; ++i) { s.op[i] = o; if (i < NS) o += (uint32_t)R1 * 256; }
+  for (int i = 0; i < NARROW_MAX_NS; ++i) { s.raw[i] = o; if (i < NS) o += (uint32_t)R1 * 128 * nbox; }
+  for (int i = 0; i < NARROW_MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += 2u * BN * 128; }
+  s.bars = o; o += (2 * NARROW_MAX_NW + 4 * NARROW_MAX_NS) * 8;
+  s.total = o;
+}
+
+template <int BN>
+__global__ void __launch_bounds__(NARROW_THREADS, 1) tcpair_narrow_kernel(const __grid_constant__ TapConvParams P1,
+                                                                          const __grid_constant__ TapConvParams P2,
+                                                                          const __grid_constant__ CUtensorMap tmx) {
+  constexpr int NB = tc5_nb(BN), MT = TC_ROWS;
+  static_assert(NB == BN && BN <= 64, "narrow pairs: one wgmma column block");
+  extern __shared__ uint8_t smem_raw_[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
+  const int R1 = P1.R, NS = P1.tc_na, NW = P1.tc_nw, nbox = (P1.Cin + 31) >> 5;
+  __shared__ NarrowSmem S;
+  if (threadIdx.x == 0) narrow_layout(S, BN, R1, nbox, NS, NW);
+  __syncthreads();
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
+  uint64_t* w_empty = w_full + NARROW_MAX_NW;
+  uint64_t* raw_full = w_empty + NARROW_MAX_NW;   // [NS] the tile's input rows landed (TMA -> transform)
+  uint64_t* in_full = raw_full + NARROW_MAX_NS;   // [NS] the set holds the tile's c1 operand (transform -> wgmma)
+  uint64_t* acc_full = in_full + NARROW_MAX_NS;   // [NS] the set holds the tile's c2 dump (wgmma -> epilogue)
+  uint64_t* set_free = acc_full + NARROW_MAX_NS;  // [NS] the epilogue is done with the set (epilogue -> TMA)
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup-uniform role branches (see tcconv5_kernel)
+  int span2 = 0;
+  for (int t = 0; t < P2.ntaps; ++t) span2 = max(span2, P2.tap_off[t] - P2.lo_al);
+  const int Lv = P1.L, MTO = MT - span2, ntx = (Lv + MTO - 1) / MTO, ntiles = ntx * P1.G;
+  const int nloc = (int)blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  const int lo = P1.lo_al, RR2 = P2.R;
+  const int total1 = P1.ntaps, iters = total1 + P2.ntaps;   // one 64-channel chunk per conv
+  const bool wres = NW == iters;                            // resident weights: stage it of every tile is stage it
+  auto tile_of = [&](int k, int& g, int& q0) {
+    const int T = (int)blockIdx.x + k * (int)gridDim.x;
+    g = T / ntx;
+    q0 = (T - g * ntx) * MTO;
+  };
+
+  if (tid == 0) {
+    for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NARROW_MMA / 32); }
+    for (int i = 0; i < NS; ++i) {
+      mbar_init(&raw_full[i], 1);
+      mbar_init(&in_full[i], NARROW_DATA);
+      mbar_init(&acc_full[i], NARROW_WG);
+      mbar_init(&set_free[i], NARROW_DATA);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg < 2) {
+    // ====================== wgmma warpgroups: warpgroup wg runs the whole of tiles wg, wg + 2, .. ======================
+    // rows 64 b .. 64 b + 63 of the tile in accumulator b, every row block's products in tcpair_body's order
+    setmaxnreg_inc<NARROW_MMA_REGS>();
+    float acc[2][BN / 2];
+    int it = 0, prev = -1;   // prev: weight stage of the newest wgmma group, released once that group has completed
+    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {   // as tcpair_body, MB = 2
+      for (int t = 0; t < Q.ntaps; ++t, ++it) {
+        const int s = it % NW;
+        mbar_wait(&w_full[s], wres ? 0u : (uint32_t)((it / NW) & 1));
+        const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
+        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
+        const uint32_t ws = smem_u32(smem + S.w[s]);
+        fence_acc<BN / 2>(acc[0]);
+        fence_acc<BN / 2>(acc[1]);
+        wgmma_fence();
+        for (int k = 0; k < ksteps; ++k) {
+          const uint64_t ko = (uint64_t)((k * 32) >> 4);
+          const uint64_t dwh = make_desc(ws) + ko, dwl = make_desc(ws + BN * 128) + ko;
+#pragma unroll
+          for (int b = 0; b < 2; ++b) {
+            const uint64_t ab = ko + b * BLK_DESC;
+            wgmma_nb<NB>(acc[b], dah + ab, dwh);
+            wgmma_nb<NB>(acc[b], dal + ab, dwh);
+            wgmma_nb<NB>(acc[b], dah + ab, dwl);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        fence_acc<BN / 2>(acc[0]);
+        fence_acc<BN / 2>(acc[1]);
+        if (!wres && prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        prev = s;
+      }
+    };
+    auto drain = [&]() {
+      wgmma_wait<0>();
+      fence_acc<BN / 2>(acc[0]);
+      fence_acc<BN / 2>(acc[1]);
+      if (!wres && prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+      prev = -1;
+    };
+    const int bar = 1 + wg, wt = tid - wg * NARROW_WG;   // this warpgroup's named barrier and thread index
+    const int r0 = (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    const uint32_t lo_part = (uint32_t)RR2 * 128;
+    int k = wg;
+    for (; k < nloc; k += 2) {
+      int g, q0;
+      tile_of(k, g, q0);
+      const int qa = q0 + P2.lo_al, s = k % NS;
+      uint8_t* set = smem + S.op[s];
+#pragma unroll
+      for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[b][i] = 0.f;
+      mbar_wait(&in_full[s], (uint32_t)((k / NS) & 1));
+      {
+        const uint32_t ahi0 = smem_u32(set) + (uint32_t)(-lo) * 128u;
+        mma_taps(P1, ahi0, ahi0 + (uint32_t)R1 * 128, (P1.Cin + 15) >> 4);
+      }
+      drain();
+      named_bar_sync(bar, NARROW_WG);          // all of the warpgroup's c1 wgmmas are done reading the set
+      // c1's epilogue -> c2's operand tile, as tcpair_body
+      const float dsc1 = P1.tc_descale;
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = 8 * i + c0;
+        const bool cok = col < P2.Cin;
+        float2 bv = make_float2(0.f, 0.f);
+        if (cok && P1.bias) bv = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 64 * b + 8 * h;
+            float v0 = 0.f, v1 = 0.f;
+            if (cok && qa + r >= 0 && qa + r < Lv) {
+              v0 = lrelu(__fadd_rn(__fmul_rn(acc[b][4 * i + 2 * h], dsc1), bv.x), P2.slope);
+              v1 = lrelu(__fadd_rn(__fmul_rn(acc[b][4 * i + 2 * h + 1], dsc1), bv.y), P2.slope);
+            }
+            uint32_t l;
+            const uint32_t hw = split2(v0, v1, l);
+            const uint32_t o = sw128(r, col >> 3) + (col & 7) * 2;
+            *reinterpret_cast<uint32_t*>(set + o) = hw;
+            *reinterpret_cast<uint32_t*>(set + lo_part + o) = l;
+          }
+      }
+      const int zitems = (RR2 - MT) * 8;
+      for (int idx = wt; idx < zitems * 2; idx += NARROW_WG) {
+        const int blk = idx / zitems, u = idx - blk * zitems;
+        *reinterpret_cast<uint4*>(set + (uint32_t)blk * lo_part + MT * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+      }
+#pragma unroll
+      for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[b][i] = 0.f;
+      fence_proxy_async();
+      named_bar_sync(bar, NARROW_WG);
+      {
+        const uint32_t ahi0 = smem_u32(set) + (uint32_t)(-P2.lo_al) * 128u;
+        mma_taps(P2, ahi0, ahi0 + lo_part, (P2.Cin + 15) >> 4);
+      }
+      drain();
+      named_bar_sync(bar, NARROW_WG);          // all of the warpgroup's c2 wgmmas are done reading the set
+      // accumulator x descale -> the set's dump, in tcpair_body's staging layout (one [128][32] block per 32 columns)
+      const float dsc = P2.tc_descale;
+#pragma unroll
+      for (int blk = 0; blk < BN / 32; ++blk) {
+        uint8_t* stg = set + blk * (MT * 128);
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+          const float* a = &acc[b][4 * (blk * 32 / 8)];
+          const int r = r0 + 64 * b;
+#pragma unroll
+          for (int i8 = 0; i8 < 4; ++i8) {
+            const int col = 8 * i8 + c0;
+            *reinterpret_cast<float2*>(stg + sw128(r, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
+            *reinterpret_cast<float2*>(stg + sw128(r + 8, col >> 2) + (col & 3) * 4) =
+                make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+          }
+        }
+      }
+      mbar_arrive(&acc_full[s]);
+    }
+    // The weight ring is shared: the producer streams one pass per pair of tiles and a stage is refilled once both
+    // warpgroups released it.  With an odd tile count warpgroup 1 has no tile in the last pair and releases its stages
+    // unused.
+    if (!wres && k < 2 * ((nloc + 1) / 2))
+      for (int t = 0; t < iters; ++t, ++it) {
+        const int s = it % NW;
+        mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
+        if (lane == 0) mbar_arrive(&w_empty[s]);
+      }
+  } else if (wg == 2) {
+    // =========================== transform: staged fp32 rows -> c1's hi / lo operand tile ===========================
+    setmaxnreg_dec<NARROW_XF_REGS>();
+    const int dt = tid - NARROW_MMA;
+    const int lq = P1.Cin > 32 ? 3 : (P1.Cin > 16 ? 2 : 1);   // log2 of the 8-channel groups the k-steps touch
+    for (int k = 0; k < nloc; ++k) {
+      const int s = k % NS;
+      mbar_wait(&raw_full[s], (uint32_t)((k / NS) & 1));
+      const uint8_t* raw = smem + S.raw[s];
+      uint8_t* set = smem + S.op[s];
+#pragma unroll 2
+      for (int idx = dt; idx < (R1 << lq); idx += NARROW_DATA) {
+        const int row = idx >> lq, q = idx & ((1 << lq) - 1);
+        // channels 8q .. 8q + 7: 16-byte units 2q, 2q + 1 of box q / 4, in the TMA's SWIZZLE_128B order
+        const uint8_t* rr = raw + (uint32_t)(q >> 2) * R1 * 128 + row * 128;
+        const int j0 = (2 * q) & 7, sw = row & 7;
+        const float4 x0 = pro_apply5(P1, *reinterpret_cast<const float4*>(rr + ((j0 ^ sw) << 4)), true, nullptr);
+        const float4 x1 = pro_apply5(P1, *reinterpret_cast<const float4*>(rr + (((j0 + 1) ^ sw) << 4)), true, nullptr);
+        uint4 h, l;
+        h.x = split2(x0.x, x0.y, l.x);
+        h.y = split2(x0.z, x0.w, l.y);
+        h.z = split2(x1.x, x1.y, l.z);
+        h.w = split2(x1.z, x1.w, l.w);
+        const uint32_t o = sw128(row, q);
+        *reinterpret_cast<uint4*>(set + o) = h;
+        *reinterpret_cast<uint4*>(set + (uint32_t)R1 * 128 + o) = l;
+      }
+      fence_proxy_async();                    // generic-proxy stores -> visible to the wgmma operand reads
+      mbar_arrive(&in_full[s]);
+    }
+  } else if (wg == 3) {
+    // =========================== epilogue: the dump through c2's fused epilogue ===========================
+    setmaxnreg_inc<NARROW_EPI_REGS>();
+    const int dt = tid - NARROW_MMA - NARROW_DATA, jc = dt & 7;
+    const int roff = -(P1.lo_al + P2.lo_al);   // staged input row of output row 0
+    const bool old_sum = P2.epi == EPI_ACC && P2.accumulate;
+    for (int k = 0; k < nloc; ++k) {
+      int g, q0;
+      tile_of(k, g, q0);
+      const int s = k % NS;
+      const uint8_t* set = smem + S.op[s];
+      const uint8_t* raw = smem + S.raw[s];
+      // the old MRF sum of every item, read before the dump is ready
+      float4 ob[BN / 32][8];
+#pragma unroll
+      for (int b = 0; b < BN / 32; ++b)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int row = (dt >> 3) + 16 * i;
+          ob[b][i] = (old_sum && row < MTO && q0 + row < Lv) ? epi_load_b(P2, g, q0 + row, 32 * b + 4 * jc)
+                                                             : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+      mbar_wait(&acc_full[s], (uint32_t)((k / NS) & 1));
+#pragma unroll
+      for (int b = 0; b < BN / 32; ++b) {
+        const int co = 32 * b + 4 * jc;
+        const uint8_t* stg = set + b * (MT * 128);
+        const float4 cv = epi_colvec(P2, g, co);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int row = (dt >> 3) + 16 * i;
+          if (row < MTO && q0 + row < Lv) {
+            const int rr = row + roff;
+            EpiPre pre;
+            pre.a = *reinterpret_cast<const float4*>(raw + (uint32_t)b * R1 * 128 + sw128(rr, jc));
+            pre.b = ob[b][i];
+            epi_store_cv(P2, g, q0 + row, co, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre, cv);
+          }
+        }
+      }
+      mbar_arrive(&set_free[s]);
+    }
+  } else {
+    setmaxnreg_dec<24>();
+    if (lane != 0) return;
+    if (warp == 16) {
+      // =========================== input rows of each tile (TMA) ===========================
+      tma_prefetch_desc(&tmx);
+      for (int k = 0; k < nloc; ++k) {
+        int g, q0;
+        tile_of(k, g, q0);
+        const int s = k % NS;
+        if (k >= NS) mbar_wait(&set_free[s], (uint32_t)((k / NS - 1) & 1));
+        mbar_arrive_expect_tx(&raw_full[s], (uint32_t)nbox * R1 * 128);
+        for (int b = 0; b < nbox; ++b)
+          tma_load_3d(smem + S.raw[s] + (uint32_t)b * R1 * 128, &tmx, 32 * b, q0 + P2.lo_al + lo, g, &raw_full[s]);
+      }
+    } else if (warp == 17) {
+      // =========================== weight stages: c1's, then c2's ===========================
+      const uint32_t bytes = 2u * BN * 128u;
+      auto src = [&](int it) {
+        return it < total1 ? reinterpret_cast<const uint8_t*>(P1.w_h) + (size_t)it * bytes
+                           : reinterpret_cast<const uint8_t*>(P2.w_h) + (size_t)(it - total1) * bytes;
+      };
+      if (wres) {
+        for (int it = 0; it < iters && nloc > 0; ++it) {
+          mbar_arrive_expect_tx(&w_full[it], bytes);
+          bulk_g2s(smem + S.w[it], src(it), bytes, &w_full[it]);
+        }
+      } else {
+        int n_it = 0;
+        for (int j = 0; j < (nloc + 1) / 2; ++j)   // one pass per pair of tiles, read by both wgmma warpgroups
+          for (int it = 0; it < iters; ++it, ++n_it) {
+            const int s = n_it % NW, n = n_it / NW;
+            if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
+            mbar_arrive_expect_tx(&w_full[s], bytes);
+            bulk_g2s(smem + S.w[s], src(it), bytes, &w_full[s]);
+          }
+      }
+    }
+  }
+}
+
 // fp16 hi/lo weight image: [co-tile][chunk64][tap][hi | lo][BN rows x 128 B, SWIZZLE_128B], pre-scaled
 void build_h_image(const PackedConv& pc, const std::vector<float>& h, int BN, float wscale, DevBuf& dst) {
   const int nct = cdiv(pc.Cout, BN), nch = cdiv(pc.Cin, H_KCH), nt = pc.ntaps;
@@ -1397,11 +1722,72 @@ static bool tcpair_dual(const TapConvParams& P1) {
   return P1.tc_dual && P1.tc_bn <= 64 && !P1.pi_hi;
 }
 
+// One launch of tcpair_narrow_kernel for a pair that tcpair_dual allows: min(tiles, SMs) CTAs.  Shared-memory plan:
+// a set is 256 R1 bytes of operand tile and R1 x 128 B of staged input per 32 channels.  Where every weight stage of
+// c1 and c2 fits beside two sets, the stages are loaded once per CTA and the rest holds as many sets as fit (at most
+// 4); else two sets and as deep a ring as the rest holds.  At C = 64 the sets are large (68-94 KB), so a k = 11 pair
+// keeps a ring of 2-4 of its 22 stages, which both wgmma warpgroups must release before it refills; those pairs are
+// faster on tcpair2_kernel (measured on H100, DESIGN.md section 4) and are left to it: at BN = 64 the pipeline takes
+// at most 14 weight stages per tile (k <= 7).  False -- nothing launched -- when the handle does not allow it
+// (TapConvParams::tc_narrow_pipe), that limit is passed, the residual is not the pair's input, c2's tile or the
+// residual rows do not lie inside c1's operand rows, or the plan does not fit.
+static bool tcpair_narrow_try(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
+  const int BN = P1.tc_bn, iters = P1.ntaps + P2.ntaps;   // weight stages per tile: one 64-channel chunk per conv
+  if (!P1.tc_narrow_pipe || (BN != 64 && BN != 32) || (BN == 64 && iters > 14) || P1.Cin > BN || P2.po_hi ||
+      P2.res != P1.in || P2.res_pitch != P1.in_pitch || P2.res_gstride != P1.in_gstride)
+    return false;
+  const int span1 = tc5_rows(P1, TC_ROWS);
+  const int span2 = tc5_rows(P2, TC_ROWS);
+  // staged row of output row r is r - lo1 - lo2, for r < 128 - span2 it must lie in 0 .. R1 - 1
+  if (P2.R > P1.R || P1.R > 256 || P1.lo_al > 0 || P2.lo_al > 0 || (P1.lo_al + span1) + (P2.lo_al + span2) < 0)
+    return false;
+  const int nbox = cdiv(P1.Cin, 32);
+  const long wbytes = 2L * BN * 128, set = 256L * P1.R + 128L * nbox * P1.R;
+  NarrowSmem S;
+  narrow_layout(S, BN, P1.R, nbox, 0, 0);
+  const long avail = (long)kMaxDyn - 1024 - (long)S.total;
+  int NS = 2, NW;
+  if (avail - iters * wbytes >= 2 * set) {
+    NW = iters;
+    NS = (int)std::min<long>(NARROW_MAX_NS, (avail - iters * wbytes) / set);
+  } else {
+    NW = (int)std::min<long>(iters, (avail - NS * set) / wbytes);
+    if (NW < 2) return false;
+  }
+  CUtensorMap tmx;
+  if (!tma_encode_rows(&tmx, P1.in, P1.Cin, P1.L, P1.G, P1.in_pitch, P1.in_gstride, P1.R)) return false;
+  P1.tc_na = NS; P1.tc_nw = NW;
+  P2.tc_bn = BN;
+  narrow_layout(S, BN, P1.R, nbox, NS, NW);
+  const size_t smem = (size_t)S.total + 1024;
+  const long tiles = (long)cdiv(P1.L, TC_ROWS - span2) * P1.G;
+  dim3 grid((unsigned)std::min<long>(tiles, tc5_sms()));
+  int dev = 0;
+  AGPT_CUDA(cudaGetDevice(&dev));
+  static bool attr_done_dev[64] = {false};
+  if (!attr_done_dev[dev & 63]) {
+    AGPT_CUDA(cudaFuncSetAttribute(tcpair_narrow_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    AGPT_CUDA(cudaFuncSetAttribute(tcpair_narrow_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    attr_done_dev[dev & 63] = true;
+  }
+  void* rec = profile_begin_pair(P1, P2, st);
+  tapconv_note_launch(1, BN, TC_ROWS, 0);
+  if (BN == 64) launch_pdl(tcpair_narrow_kernel<64>, grid, dim3(NARROW_THREADS), smem, st, P1, P2, tmx);
+  else launch_pdl(tcpair_narrow_kernel<32>, grid, dim3(NARROW_THREADS), smem, st, P1, P2, tmx);
+  profile_count_dual();
+  profile_count_narrow_pipe();
+  profile_end(rec, st);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+  return true;
+}
+
 // One ResBlock1 pair, out = x + c2(lrelu(c1(lrelu(x)))) (c2's epilogue EPI_RES / EPI_ACC), as one launch of
 // tcpair_kernel: c1's output tile stays in shared memory as c2's operand tile, so the intermediate tensor never
 // reaches HBM.  A tile yields MT - span(c2) output rows (c1 is recomputed on the halo rows of neighbouring tiles);
-// two 128-row tiles in flight per CTA where tcpair_pipe_try takes the pair (128 -> 128 channels), else two 128-row
-// CTAs per SM where tcpair_dual allows it and the plan fits, else MT = 256 where tc5_tall allows it, else 128.
+// two 128-row tiles in flight per CTA where tcpair_pipe_try takes the pair (128 -> 128 channels); where tcpair_dual
+// allows it, the narrow pipeline (tcpair_narrow_try), else two 128-row CTAs per SM where that plan fits; else MT = 256
+// where tc5_tall allows it, else 128.
 // Returns false -- nothing launched -- when the pair needs more than one co-tile or does not fit shared memory.
 bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (!tcconv_supported(P1) || !P2.w_h) return false;
@@ -1410,7 +1796,7 @@ bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
       P1.G != P2.G || P1.L != P2.L || P1.pro != PRO_LRELU || P2.pro != PRO_LRELU || (P2.epi != EPI_RES && P2.epi != EPI_ACC))
     return false;
   if (tcpair_pipe_try(P1, P2, st)) return true;
-  if (tcpair_dual(P1) && tcpair_try(P1, P2, TC_ROWS, true, st)) return true;
+  if (tcpair_dual(P1) && (tcpair_narrow_try(P1, P2, st) || tcpair_try(P1, P2, TC_ROWS, true, st))) return true;
   const int span2 = tc5_rows(P2, TC_TALL);
   if (tc5_tall(P1, BN, (long)cdiv(tc_lv(P1), TC_TALL - span2) * tc_groups(P1), tc5_sms()) &&
       tcpair_try(P1, P2, TC_TALL, false, st))

@@ -39,10 +39,12 @@ int agpt_profile_collect(double ms[4], double flops[4], double bytes[4], long lo
 long long agpt_profile_tall_launches(void);
 /* recorded wgmma launches whose input was a pre-split fp16 operand plane (HiFi-GAN) since profiling was enabled */
 long long agpt_profile_plane_launches(void);
-/* recorded fused-pair launches that ran two 128-row CTAs per SM (narrow HiFi-GAN stages) since profiling was enabled */
+/* recorded launches of narrow pairs with overlapped tiles (HiFi-GAN's C <= 64 stages) since profiling was enabled */
 long long agpt_profile_dual_launches(void);
 /* recorded fused-pair launches that ran two tiles in flight per CTA (HiFi-GAN's C = 128 stage) since profiling was enabled */
 long long agpt_profile_pipe_launches(void);
+/* recorded narrow fused-pair launches on the persistent tile pipeline (HiFi-GAN's C <= 64 stages) since profiling was enabled */
+long long agpt_profile_narrow_pipe_launches(void);
 /* dev tooling: one text line per recorded launch ("variant G L Cin Cout ntaps span epi Wreal ms flops"); returns bytes written or -1 */
 long agpt_profile_dump(char* out, long cap);
 double agpt_fma_peak_tflops(void);
