@@ -147,6 +147,7 @@ PROTOTYPES = {
     "agpt_profile_dual_launches": (C.c_longlong, []),
     "agpt_profile_pipe_launches": (C.c_longlong, []),
     "agpt_profile_narrow_pipe_launches": (C.c_longlong, []),
+    "agpt_profile_conv_pipe_launches": (C.c_longlong, []),
     "agpt_profile_dump": (_L, [_P, _L]),
     "agpt_fma_peak_tflops": (_D, []),
     "agpt_set_tensor_cores": (_I, [_I]),

@@ -54,6 +54,7 @@ long long agpt_profile_plane_launches(void) { return profile_plane_launches(); }
 long long agpt_profile_dual_launches(void) { return profile_dual_launches(); }
 long long agpt_profile_pipe_launches(void) { return profile_pipe_launches(); }
 long long agpt_profile_narrow_pipe_launches(void) { return profile_narrow_pipe_launches(); }
+long long agpt_profile_conv_pipe_launches(void) { return profile_conv_pipe_launches(); }
 int agpt_set_tensor_cores(int on) { return guarded([&] { tc_set_enabled(on); }); }
 int agpt_set_attention_tc(int on) { return guarded([&] { attention_set_tc(on); }); }
 int agpt_attention(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch, float* o,

@@ -343,6 +343,7 @@ struct Hifigan : Handle {
   bool pair_dual = true;            // AGPT_PAIR_DUAL=0: no fused pair runs two CTAs per SM (TapConvParams::tc_dual)
   bool pair_pipe = true;            // AGPT_PAIR_PIPE=0: no C = 128 pair runs two tiles per CTA (TapConvParams::tc_pipe)
   bool narrow_pipe = true;          // AGPT_NARROW_PIPE=0: narrow pairs keep two CTAs per SM (TapConvParams::tc_narrow_pipe)
+  bool conv_pipe = true;            // AGPT_CONV_PIPE=0: plane-fed convs keep one tile per CTA (TapConvParams::tc_conv_pipe)
 
   ~Hifigan() override {
     if (pin_mel) cudaFreeHost(pin_mel);
@@ -393,6 +394,7 @@ struct Hifigan : Handle {
     auto feed = [&](TapConvParams& P, int ch) {                // P reads its input's plane
       if (!has_plane(ch)) return;
       P.pi_hi = plane_hi(P.in); P.pi_lo = P.pi_hi + mxp;
+      P.tc_conv_pipe = conv_pipe;
     };
     auto emit = [&](TapConvParams& P, int ch, bool keep_fp32) {   // P's epilogue writes its output's plane too (or only)
       if (!has_plane(ch)) return;
@@ -550,6 +552,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   { const char* e = getenv("AGPT_PAIR_DUAL"); h->pair_dual = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_PAIR_PIPE"); h->pair_pipe = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_NARROW_PIPE"); h->narrow_pipe = !(e && e[0] == '0'); }
+  { const char* e = getenv("AGPT_CONV_PIPE"); h->conv_pipe = !(e && e[0] == '0'); }
   WeightCursor wc{W, nW};
   { const float* w = wc.next(); const float* b = wc.next(); pack_conv(h->conv_pre, w, b, C0, cfg->n_mels, 7, false); }
   h->ups.resize(nu);

@@ -15,6 +15,7 @@ static long long g_plane = 0;   // recorded launches that were plane-fed (likewi
 static long long g_dual = 0;    // recorded launches of narrow pairs with overlapped tiles (likewise)
 static long long g_pipe = 0;    // recorded launches of the two-tiles-per-CTA pair kernel (likewise)
 static long long g_narrow = 0;  // recorded launches of the narrow pair pipeline (likewise)
+static long long g_cpipe = 0;   // recorded launches of the plane-fed single-conv pipeline (likewise)
 
 bool profile_enabled() { return g_prof; }
 
@@ -28,6 +29,7 @@ void profile_enable(int on) {
     g_dual = 0;
     g_pipe = 0;
     g_narrow = 0;
+    g_cpipe = 0;
   }
 }
 
@@ -45,6 +47,8 @@ void profile_count_pipe() { if (g_prof) ++g_pipe; }
 long long profile_pipe_launches() { return g_pipe; }
 void profile_count_narrow_pipe() { if (g_prof) ++g_narrow; }
 long long profile_narrow_pipe_launches() { return g_narrow; }
+void profile_count_conv_pipe() { if (g_prof) ++g_cpipe; }
+long long profile_conv_pipe_launches() { return g_cpipe; }
 
 // Sums over the records since profile_enable(1): per variant (FMA BN = 128, 64, 32; 3 = wgmma)
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches) {

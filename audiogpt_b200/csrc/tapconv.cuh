@@ -89,6 +89,9 @@ struct TapConvParams {
   // 1: a narrow fused pair that tc_dual allows may run on tcpair_narrow_kernel (persistent, several tiles in flight
   // per CTA) before tcpair2_kernel; set by the HiFi-GAN driver unless AGPT_NARROW_PIPE=0.
   int tc_narrow_pipe;
+  // 1: a plane-fed launch at BN = 128 over 1-D rows may run on tcconv_pipe_pl_kernel (persistent, one tile's epilogue
+  // beside the next tile's wgmmas); set by the HiFi-GAN driver unless AGPT_CONV_PIPE=0.
+  int tc_conv_pipe;
 };
 
 __host__ __device__ inline int tc_wv(const TapConvParams& P) { return P.Wreal > 0 ? (P.strips > 0 ? P.strip_w + 2 : P.Wreal + 1) : 0; }
@@ -163,6 +166,8 @@ void profile_count_pipe();            // a fused-pair launch of tcpair_pipe_kern
 long long profile_pipe_launches();
 void profile_count_narrow_pipe();     // a fused-pair launch of tcpair_narrow_kernel (counted while profiling)
 long long profile_narrow_pipe_launches();
+void profile_count_conv_pipe();       // a plane-fed launch of tcconv_pipe_pl_kernel (counted while profiling)
+long long profile_conv_pipe_launches();
 void profile_count_plane();           // a plane-fed tensor-core launch (counted while profiling)
 long long profile_plane_launches();
 // The variant of the most recent tap-GEMM launch on this host thread, {1 tensor-core | 0 fp32-FMA, tile width, tile

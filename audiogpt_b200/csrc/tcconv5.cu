@@ -1367,6 +1367,242 @@ __global__ void __launch_bounds__(NARROW_THREADS, 1) tcpair_narrow_kernel(const 
   }
 }
 
+// ---- plane-fed single tap-GEMMs at BN = 128 on a persistent, warp-specialised pipeline (tcconv_pipe_pl_kernel) ----
+// tcconv5_pl_kernel<128, 128> runs one tile per CTA in phases: operand load, wgmmas, epilogue; the tensor cores idle
+// while a CTA loads and stores, and all CTAs of a wave hit HBM at about the same time.  This kernel splits the roles:
+//   warpgroups 0-1  each runs whole units (0: the CTA's units 0, 2, ..; 1: units 1, 3, ..) in two 64-row
+//                   accumulators, then the unit's fused epilogue straight from its registers, while the other
+//                   warpgroup issues the next unit's wgmmas
+//   warp 8          loads each unit's 64-channel hi / lo plane chunks by TMA into a ring of NA operand buffers, and
+//                   its weight stages into a ring of NW, in unit order
+// Both warpgroups read the two rings, so they take turns: a warpgroup starts a unit's wgmmas once the other one has
+// waited for every chunk and stage of the previous unit.  A ring slot's full barrier is then never more than one phase
+// ahead of its waiter (a parity wait cannot tell phase m from m + 2), and the tensor cores pass from one unit to the
+// next without a gap.
+// A unit is one 128-row tile of one 128-wide output-channel tile.  CTA b walks units b, b + grid, .. with the
+// output-channel tile varying fastest, so the co-tiles of one row tile run on neighbouring CTAs at the same time and
+// all but the first read of those plane rows should hit L2.  When the last round has at most half as many units as CTAs,
+// it runs as 64-row half-units (one accumulator block each) on twice as many CTAs.
+// Chunk and tap order, the wgmma shapes, the hi.hi, lo.hi, hi.lo order per 64-row block, the descale and the
+// epilogue's float operations are those of tcconv5_pl_kernel<128, 128>, so every output is bit-identical.
+// Launched at 168 registers per thread, the warpgroups rebalance them (setmaxnreg): 2 x 232 (the 128-register
+// accumulator and the epilogue) + 40.
+constexpr int CPIPE_THREADS = 384;
+constexpr int CPIPE_MMA_REGS = 232, CPIPE_LOAD_REGS = 40;
+// operand buffer i: PR hi rows then PR lo rows of 128 B (PR = pl_rows(R)); weight stage i: 32 KB
+struct CpipeSmem { uint32_t a[MAX_NA], w[MAX_NW], bars, total; };
+__host__ __device__ inline void cpipe_layout(CpipeSmem& s, int PR, int NA, int NW) {
+  uint32_t o = 0;
+  for (int i = 0; i < MAX_NA; ++i) { s.a[i] = o; if (i < NA) o += (uint32_t)PR * 256; }
+  for (int i = 0; i < MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += 2 * 128 * 128; }
+  s.bars = o; o += (2 * (MAX_NW + MAX_NA) + 2) * 8;
+  s.total = o;
+}
+// CTAs of a launch of `units` units: every SM, or fewer units than SMs as half-units where twice their count fits
+inline int cpipe_grid(int units, int sms) {
+  return units >= sms ? sms : (2 * units <= sms ? 2 * units : units);
+}
+
+__global__ void __launch_bounds__(CPIPE_THREADS, 1) tcconv_pipe_pl_kernel(const __grid_constant__ TapConvParams P,
+                                                                         const __grid_constant__ CUtensorMap tmh,
+                                                                         const __grid_constant__ CUtensorMap tml) {
+  constexpr int BN = 128, MT = TC_ROWS;
+  extern __shared__ uint8_t smem_raw_[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
+  const int NA = P.tc_na, NW = P.tc_nw, PR = pl_rows(P.R);
+  __shared__ CpipeSmem S;
+  if (threadIdx.x == 0) cpipe_layout(S, PR, NA, NW);
+  __syncthreads();
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
+  uint64_t* w_empty = w_full + MAX_NW;
+  uint64_t* a_full = w_empty + MAX_NW;   // [NA] the chunk landed (TMA -> wgmma)
+  uint64_t* a_empty = a_full + MAX_NA;   // [NA] its unit's wgmmas are done with it (wgmma -> TMA)
+  uint64_t* turn = a_empty + MAX_NA;      // [2] warpgroup wg may start its next unit (the other warpgroup -> wg)
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup-uniform role branches (see tcconv5_kernel)
+  const int Lv = P.L, ntx = (Lv + MT - 1) / MT, nct = (P.Cout + BN - 1) / BN;
+  const int grid = (int)gridDim.x, cta = (int)blockIdx.x;
+  const int units = ntx * P.G * nct, nfull = units / grid, rem = units - nfull * grid;
+  const bool split = rem > 0 && 2 * rem <= grid;   // the last round as half-units
+  const int nloc = nfull + (cta < (split ? 2 * rem : rem) ? 1 : 0);
+  const int nch = P.tc_chunks_h, ntaps = P.ntaps, total = nch * ntaps, lo = P.lo_al;
+  // local item k -> sample g, first row q0, co-tile ct, half (-1: all 128 rows, else the 64-row block it runs)
+  auto item = [&](int k, int& g, int& q0, int& ct, int& half) {
+    int u;
+    if (k < nfull) { u = cta + k * grid; half = -1; }
+    else if (split) { u = nfull * grid + (cta >> 1); half = cta & 1; }
+    else { u = nfull * grid + cta; half = -1; }
+    const int rt = u / nct;
+    ct = u - rt * nct;
+    g = rt / ntx;
+    q0 = (rt - g * ntx) * MT;
+  };
+
+  if (tid == 0) {
+    for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], 4); }
+    for (int i = 0; i < NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 4); }
+    for (int i = 0; i < 2; ++i) mbar_init(&turn[i], 4);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_wait();
+
+  if (wg < 2) {
+    // =========================== wgmma warpgroups: warpgroup wg runs items wg, wg + 2, .. ===========================
+    setmaxnreg_inc<CPIPE_MMA_REGS>();
+    float acc[2][BN / 2];   // rows 64 b .. 64 b + 63 of the unit in acc[b]
+    const int wt = tid - wg * 128, rw = (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+    const float dsc = P.tc_descale;
+    const bool resacc = P.epi != EPI_BIAS, accum = P.epi == EPI_ACC && P.accumulate;
+    for (int k = wg; k < nloc; k += 2) {
+      int g, q0, ct, half;
+      item(k, g, q0, ct, half);
+      const int co0 = ct * BN;
+      const bool b0 = half != 1, b1 = half != 0;
+      {  // the epilogue's residual / old MRF sum rows into L2 while the wgmmas run
+        const float* pf0 = (resacc && P.res) ? P.res + g * P.res_gstride : nullptr;
+        const float* pf1 = accum ? P.out + g * P.out_gstride : nullptr;
+        for (int idx = wt; idx < MT * 4; idx += 128) {
+          const int row = idx >> 2, p = q0 + row, co = co0 + (idx & 3) * 32;
+          if (p < Lv && co < P.Cout && (row < 64 ? b0 : b1)) {
+            if (pf0) asm volatile("prefetch.global.L2 [%0];" ::"l"(pf0 + (long)p * P.res_pitch + co));
+            if (pf1) asm volatile("prefetch.global.L2 [%0];" ::"l"(pf1 + (long)p * P.out_pitch + co));
+          }
+        }
+      }
+#pragma unroll
+      for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[b][i] = 0.f;
+      int prev = -1;   // weight stage of the newest wgmma group, released once that group has completed
+      if (k > 0) mbar_wait(&turn[wg], (uint32_t)(((k - 1) >> 1) & 1));   // the other warpgroup's unit k - 1 is issued
+      for (int c = 0; c < nch; ++c) {
+        const int n = k * nch + c, buf = n % NA;   // n: the CTA's chunk sequence
+        mbar_wait(&a_full[buf], (uint32_t)((n / NA) & 1));
+        const uint32_t ahi0 = smem_u32(smem + S.a[buf]) - (uint32_t)lo * 128u, alo0 = ahi0 + (uint32_t)PR * 128u;
+        const int ksteps = (min(H_KCH, P.Cin - c * H_KCH) + 15) >> 4;
+        for (int t = 0; t < ntaps; ++t) {
+          const int it = k * total + c * ntaps + t, s = it % NW;   // it: the CTA's weight-stage sequence
+          mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
+          const uint32_t shift = (uint32_t)P.tap_off[t] * 128u;
+          const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
+          const uint32_t ws = smem_u32(smem + S.w[s]);
+          fence_acc<BN / 2>(acc[0]);
+          fence_acc<BN / 2>(acc[1]);
+          wgmma_fence();
+          for (int kk = 0; kk < ksteps; ++kk) {
+            const uint64_t ko = (uint64_t)((kk * 32) >> 4);
+            const uint64_t dwh = make_desc(ws) + ko, dwl = make_desc(ws + BN * 128) + ko;
+            if (b0) {
+              wgmma_n128(acc[0], dah + ko, dwh);
+              wgmma_n128(acc[0], dal + ko, dwh);
+              wgmma_n128(acc[0], dah + ko, dwl);
+            }
+            if (b1) {
+              wgmma_n128(acc[1], dah + ko + BLK_DESC, dwh);
+              wgmma_n128(acc[1], dal + ko + BLK_DESC, dwh);
+              wgmma_n128(acc[1], dah + ko + BLK_DESC, dwl);
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          fence_acc<BN / 2>(acc[0]);
+          fence_acc<BN / 2>(acc[1]);
+          if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+          // chunk n - 1's wgmmas have all completed now, so its operand buffer may be refilled
+          if (t == 0 && c > 0 && lane == 0) mbar_arrive(&a_empty[(n - 1) % NA]);
+          prev = s;
+        }
+      }
+      if (lane == 0) mbar_arrive(&turn[wg ^ 1]);
+      wgmma_wait<0>();
+      fence_acc<BN / 2>(acc[0]);
+      fence_acc<BN / 2>(acc[1]);
+      if (lane == 0) {
+        mbar_arrive(&w_empty[prev]);
+        mbar_arrive(&a_empty[(k * nch + nch - 1) % NA]);
+      }
+      // =========================== epilogue, from the accumulator fragments ===========================
+      // per element the float operations of tcconv5_body (acc x descale) and epi_store_cv<true> (+ bias,
+      // + residual, EPI_ACC: x scale + old sum), explicitly rounded so that no multiply-add is contracted
+#pragma unroll
+      for (int b = 0; b < 2; ++b) {
+        if (!(b ? b1 : b0)) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int p = q0 + 64 * b + rw + 8 * h;
+          if (p >= Lv) continue;
+          const long ro = g * P.out_gstride + (long)p * P.out_pitch, rr = g * P.res_gstride + (long)p * P.res_pitch;
+#pragma unroll
+          for (int q = 0; q < 2; ++q) {   // 64 columns at a time: their global reads in flight together
+            float2 ra[8], ob[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int co = co0 + 64 * q + 8 * i + c0;
+              ra[i] = make_float2(0.f, 0.f);
+              ob[i] = ra[i];
+              if (co < P.Cout) {
+                if (resacc && P.res) ra[i] = __ldg(reinterpret_cast<const float2*>(P.res + rr + co));
+                if (accum) ob[i] = *reinterpret_cast<const float2*>(P.out + ro + co);
+              }
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int co = co0 + 64 * q + 8 * i + c0;
+              if (co >= P.Cout) continue;
+              const float* a = &acc[b][4 * (8 * q + i) + 2 * h];
+              float2 bv = make_float2(0.f, 0.f);
+              if (P.bias) bv = __ldg(reinterpret_cast<const float2*>(P.bias + co));
+              float v0 = __fadd_rn(__fmul_rn(a[0], dsc), bv.x), v1 = __fadd_rn(__fmul_rn(a[1], dsc), bv.y);
+              if (resacc) { v0 = __fadd_rn(v0, ra[i].x); v1 = __fadd_rn(v1, ra[i].y); }
+              if (P.epi == EPI_ACC) {
+                v0 = __fadd_rn(__fmul_rn(v0, P.scale), ob[i].x);
+                v1 = __fadd_rn(__fmul_rn(v1, P.scale), ob[i].y);
+              }
+              if (P.out) *reinterpret_cast<float2*>(P.out + ro + co) = make_float2(v0, v1);
+              if (P.po_hi) {   // epi_store_plane
+                uint32_t l;
+                const uint32_t hw = split2(lrelu(v0, P.po_slope), lrelu(v1, P.po_slope), l);
+                *reinterpret_cast<uint32_t*>(P.po_hi + ro + co) = hw;
+                *reinterpret_cast<uint32_t*>(P.po_lo + ro + co) = l;
+              }
+            }
+          }
+        }
+      }
+    }
+  } else {
+    setmaxnreg_dec<CPIPE_LOAD_REGS>();
+    if (warp != 8 || lane != 0) return;
+    // =========================== warp 8: per item its plane chunks and weight stages ===========================
+    tma_prefetch_desc(&tmh);
+    tma_prefetch_desc(&tml);
+    const uint32_t bytes = 2u * BN * 128u;
+    const int nb = pl_boxes(P.R), br = pl_box_rows(P.R);
+    for (int k = 0; k < nloc; ++k) {
+      int g, q0, ct, half;
+      item(k, g, q0, ct, half);
+      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(P.w_h) + (size_t)ct * (size_t)total * bytes;
+      for (int i = 0; i < total; ++i) {
+        if (i % ntaps == 0) {   // a chunk's operand rows ahead of its first weight stage, as pl_load_chunk
+          const int c = i / ntaps, n = k * nch + c, buf = n % NA;
+          if (n >= NA) mbar_wait(&a_empty[buf], (uint32_t)((n / NA - 1) & 1));
+          mbar_arrive_expect_tx(&a_full[buf], 2u * nb * br * 128u);
+          for (int bx = 0; bx < nb; ++bx) {
+            tma_load_3d(smem + S.a[buf] + bx * br * 128, &tmh, c * H_KCH, q0 + lo + bx * br, g, &a_full[buf]);
+            tma_load_3d(smem + S.a[buf] + (PR + bx * br) * 128, &tml, c * H_KCH, q0 + lo + bx * br, g, &a_full[buf]);
+          }
+        }
+        const int it = k * total + i, s = it % NW, m = it / NW;
+        if (m >= 1) mbar_wait(&w_empty[s], (uint32_t)((m - 1) & 1));
+        mbar_arrive_expect_tx(&w_full[s], bytes);
+        bulk_g2s(smem + S.w[s], wsrc + (size_t)i * bytes, bytes, &w_full[s]);
+      }
+    }
+  }
+}
+
 // fp16 hi/lo weight image: [co-tile][chunk64][tap][hi | lo][BN rows x 128 B, SWIZZLE_128B], pre-scaled
 void build_h_image(const PackedConv& pc, const std::vector<float>& h, int BN, float wscale, DevBuf& dst) {
   const int nct = cdiv(pc.Cout, BN), nch = cdiv(pc.Cin, H_KCH), nt = pc.ntaps;
@@ -1804,10 +2040,52 @@ bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   return tcpair_try(P1, P2, TC_ROWS, false, st);
 }
 
+// One launch of tcconv_pipe_pl_kernel for tile c (pick_h_tile): cpipe_grid CTAs, each with NA operand buffers (2 to 4,
+// at most one per chunk unless there are fewer than 2 chunks) and NW weight stages: as many buffers as leave room for
+// 3 stages, then as many stages as the rest holds.  At k = 11, d = 5 (184 operand rows, 46 KB a buffer) that is 2
+// buffers and 4 stages.  False -- nothing launched -- when the handle does not allow it (TapConvParams::tc_conv_pipe),
+// the launch is not plane-fed over 1-D rows at BN = 128 with 128-row tiles and a BIAS / RES / ACC epilogue, or 2
+// buffers and 2 stages do not fit.
+static bool tcconv_pipe_try(TapConvParams P, const HTile& c, cudaStream_t st) {
+  if (!P.tc_conv_pipe || !P.pi_hi || P.Wreal || P.strips || c.bn != 128 || c.mt != TC_ROWS ||
+      (P.epi != EPI_BIAS && P.epi != EPI_RES && P.epi != EPI_ACC))
+    return false;
+  P.w_h = c.w;
+  P.tc_bn = 128;
+  tc5_rows(P, TC_ROWS);
+  const int PR = pl_rows(P.R);
+  const long abytes = 256L * PR, wbytes = 2L * 128 * 128;
+  CpipeSmem S;
+  cpipe_layout(S, PR, 0, 0);
+  const long avail = (long)kMaxDyn - 1024 - (long)S.total;
+  int NA = std::min(MAX_NA, std::max(2, P.tc_chunks_h));
+  while (NA > 2 && NA * abytes + 3 * wbytes > avail) --NA;
+  const int NW = (int)std::min<long>(MAX_NW, (avail - NA * abytes) / wbytes);
+  if (NW < 2) return false;
+  P.tc_na = NA; P.tc_nw = NW;
+  cpipe_layout(S, PR, NA, NW);
+  const size_t smem = (size_t)S.total + 1024;
+  const int units = cdiv(P.L, TC_ROWS) * P.G * cdiv(P.Cout, 128);
+  const PlMaps m = pl_tensor_maps(P);
+  int dev = 0;
+  AGPT_CUDA(cudaGetDevice(&dev));
+  static bool attr_done_dev[64] = {false};
+  if (!attr_done_dev[dev & 63]) {
+    AGPT_CUDA(cudaFuncSetAttribute(tcconv_pipe_pl_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
+    attr_done_dev[dev & 63] = true;
+  }
+  tapconv_note_launch(1, 128, TC_ROWS, 1);
+  launch_pdl(tcconv_pipe_pl_kernel, dim3(cpipe_grid(units, tc5_sms())), dim3(CPIPE_THREADS), smem, st, P, m.hi, m.lo);
+  profile_count_plane();
+  profile_count_conv_pipe();
+  return true;
+}
+
 // returns false when the layer has no fp16 image or does not fit the shared-memory budget
 bool tcconv5_launch(TapConvParams P, cudaStream_t st) {
   if (!P.w_h) return false;
   const HTile c = pick_h_tile(P, tc5_sms());
+  if (tcconv_pipe_try(P, c, st)) return true;
   if (c.bn != P.tc_bn || c.mt != TC_ROWS) {
     TapConvParams Q = P;
     Q.w_h = c.w;

@@ -45,6 +45,8 @@ long long agpt_profile_dual_launches(void);
 long long agpt_profile_pipe_launches(void);
 /* recorded narrow fused-pair launches on the persistent tile pipeline (HiFi-GAN's C <= 64 stages) since profiling was enabled */
 long long agpt_profile_narrow_pipe_launches(void);
+/* recorded plane-fed single tap-GEMM launches on the persistent tile pipeline (HiFi-GAN's C = 256 convs, ups[0] / ups[1]) since profiling was enabled */
+long long agpt_profile_conv_pipe_launches(void);
 /* dev tooling: one text line per recorded launch ("variant G L Cin Cout ntaps span epi Wreal ms flops"); returns bytes written or -1 */
 long agpt_profile_dump(char* out, long cap);
 double agpt_fma_peak_tflops(void);

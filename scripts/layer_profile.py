@@ -37,6 +37,7 @@ _lib.check(L.agpt_profile_enable(1))
 run()
 buf = C.create_string_buffer(1 << 20)
 n = L.agpt_profile_dump(buf, 1 << 20)
+conv_pipe = L.agpt_profile_conv_pipe_launches()
 _lib.check(L.agpt_profile_enable(0))
 agg = collections.OrderedDict()
 tot = 0.0
@@ -45,7 +46,8 @@ for line in lines:
     v, G, Ln, Cin, Cout, nt, span, epi, Wr, ms, fl = line.split()
     key = (int(G), int(Ln), int(Cin), int(Cout), int(nt), int(epi), int(Wr))
     a = agg.setdefault(key, [0, 0.0, 0.0]); a[0] += 1; a[1] += float(ms); a[2] += float(fl); tot += float(ms)
-print(f"{which} B={B}: {tot:.3f} ms in {sum(a[0] for a in agg.values())} tapconv launches")
+print(f"{which} B={B}: {tot:.3f} ms in {sum(a[0] for a in agg.values())} tapconv launches, "
+      f"{conv_pipe} of them plane-fed convs on the tile pipeline")
 for k, a in sorted(agg.items(), key=lambda kv: -kv[1][1]):
     print(f"  G={k[0]:3d} L={k[1]:7d} Cin={k[2]:5d} Cout={k[3]:5d} taps={k[4]:2d} epi={k[5]:2d} W={k[6]:3d}  n={a[0]:3d}  {a[1]*1e3:9.1f} us  {a[1]/tot*100:5.1f}%  {a[2]/a[1]/1e9:7.1f} TF")
 if each:
