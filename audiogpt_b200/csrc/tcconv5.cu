@@ -798,19 +798,34 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_pl_kernel(const __grid_c
 // runs the same float operations, as in tcpair_kernel<128, 128>: the results are bit-identical.
 // 4 warpgroups: 2 wgmma, 1 data, 1 whose warp 12 streams the weights.  Launched at 128 registers per thread, the
 // warpgroups then rebalance them (setmaxnreg): 2 x 168 (accumulator + hand-off) + 152 (input transform, epilogue) + 24.
+// The weights stream in half-stages of 16 KB (P.w_hk: one tap's 32 input channels, k-steps 2 h and 2 h + 1, in
+// SWIZZLE_64B rows), one wgmma group each.  A stage is released once the group after it has been issued and its own
+// group has completed, so with 32 KB stages a 2-stage ring gave each stage's load one group of wgmmas to arrive in;
+// the same 64 KB as 4 half-stages give it three half-groups (1.5 groups), and spare shared memory holds more.
 constexpr int PIPE_THREADS = 512;
+constexpr uint32_t PIPE_STAGE = 2u * 128u * 64u;   // bytes of a half-stage: hi and lo, 128 rows x 64 B
+// wgmma descriptor of a K-major SWIZZLE_64B tile (8-row groups 512 B apart)
+__device__ __forceinline__ uint64_t make_desc64(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(512 >> 4) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
 constexpr int PIPE_MMA = 256, PIPE_DATA = 128;
 template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // operand set s: [hi chunk 0][hi chunk 1][lo chunk 0][lo chunk 1] of R1 rows x 128 B (c1's input), then c2's tile in
 // the same form with R2 <= R1 rows, then the dump: 4 column blocks of [128 rows][32 fp32] (64 KB <= 512 R1 B)
-struct PipeSmem { uint32_t set[2], w[MAX_NW], bars, total; };
+constexpr int PIPE_MAX_NW = 8;
+struct PipeSmem { uint32_t set[2], w[PIPE_MAX_NW], bars, total; };
 __host__ __device__ inline void pipe_layout(PipeSmem& s, int R1, int NW) {
   uint32_t o = 0;
   for (int i = 0; i < 2; ++i) { s.set[i] = o; o += (uint32_t)R1 * 512; }
-  for (int i = 0; i < MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += 2 * 128 * 128; }
-  s.bars = o; o += (2 * MAX_NW + 4) * 8;
+  for (int i = 0; i < PIPE_MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += PIPE_STAGE; }
+  s.bars = o; o += (2 * PIPE_MAX_NW + 4) * 8;
   s.total = o;
 }
 
@@ -824,8 +839,8 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
   if (threadIdx.x == 0) pipe_layout(S, R1, NW);
   __syncthreads();
   uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
-  uint64_t* w_empty = w_full + MAX_NW;
-  uint64_t* in_full = w_full + 2 * MAX_NW;   // [2] the set holds its tile's c1 operand (data warpgroup -> wgmma)
+  uint64_t* w_empty = w_full + PIPE_MAX_NW;
+  uint64_t* in_full = w_full + 2 * PIPE_MAX_NW;   // [2] the set holds its tile's c1 operand (data warpgroup -> wgmma)
   uint64_t* acc_full = in_full + 2;           // [2] the set holds its tile's c2 dump (wgmma -> data warpgroup)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -834,8 +849,8 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
   for (int t = 0; t < P2.ntaps; ++t) span2 = max(span2, P2.tap_off[t] - P2.lo_al);
   const int Lv = P1.L, MTO = MT - span2, ntx = (Lv + MTO - 1) / MTO, ntiles = ntx * P1.G;
   const int nloc = (int)blockIdx.x < ntiles ? (ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;   // this CTA's tiles
-  const int lo = P1.lo_al, nch = P1.tc_chunks_h, total1 = nch * P1.ntaps;
-  const int RR2 = P2.R, nch2 = P2.tc_chunks_h, total2 = nch2 * P2.ntaps;
+  const int lo = P1.lo_al, nch = P1.tc_chunks_h, total1 = 2 * nch * P1.ntaps;   // half-stages per tile
+  const int RR2 = P2.R, nch2 = P2.tc_chunks_h, total2 = 2 * nch2 * P2.ntaps;
   auto tile_of = [&](int k, int& g, int& q0) {   // local tile k -> sample g, first output row q0
     const int T = (int)blockIdx.x + k * (int)gridDim.x;
     g = T / ntx;
@@ -855,28 +870,31 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
     setmaxnreg_inc<168>();
     float acc[BN / 2];
     int it = 0, prev = -1;   // prev: weight stage of the newest wgmma group, released once that group has completed
-    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {   // as tcpair_body
-      for (int t = 0; t < Q.ntaps; ++t, ++it) {
-        const int s = it % NW;
-        mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
-        const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
-        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
-        const uint32_t ws = smem_u32(smem + S.w[s]);
-        fence_acc<BN / 2>(acc);
-        wgmma_fence();
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t ko = (uint64_t)((k * 32) >> 4);
-          const uint64_t dwh = make_desc(ws) + ko, dwl = make_desc(ws + BN * 128) + ko;
-          wgmma_n128(acc, dah + ko, dwh);
-          wgmma_n128(acc, dal + ko, dwh);
-          wgmma_n128(acc, dah + ko, dwl);
+    // as tcpair_body over one 64-channel chunk (4 k-steps), the k-steps of a tap in two half-stages
+    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0) {
+      for (int t = 0; t < Q.ntaps; ++t)
+        for (int hf = 0; hf < 2; ++hf, ++it) {
+          const int s = it % NW;
+          mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
+          const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
+          const uint64_t dah = make_desc(ahi0 + shift) + 4 * hf, dal = make_desc(alo0 + shift) + 4 * hf;
+          const uint32_t ws = smem_u32(smem + S.w[s]);
+          fence_acc<BN / 2>(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            const uint64_t ko = (uint64_t)((k * 32) >> 4);
+            const uint64_t dwh = make_desc64(ws) + ko, dwl = make_desc64(ws + BN * 64) + ko;
+            wgmma_n128(acc, dah + ko, dwh);
+            wgmma_n128(acc, dal + ko, dwh);
+            wgmma_n128(acc, dah + ko, dwl);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          fence_acc<BN / 2>(acc);
+          if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+          prev = s;
         }
-        wgmma_commit();
-        wgmma_wait<1>();
-        fence_acc<BN / 2>(acc);
-        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
-        prev = s;
-      }
     };
     auto drain = [&]() {   // all wgmmas completed, the last weight stage released
       wgmma_wait<0>();
@@ -896,7 +914,7 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
       // c1 over both resident chunks of the input
       for (int c = 0; c < nch; ++c) {
         const uint32_t ahi0 = smem_u32(set) + (uint32_t)c * R1 * 128 + (uint32_t)(wg * (MT / 2) - lo) * 128u;
-        mma_taps(P1, ahi0, ahi0 + (uint32_t)nch * R1 * 128, (min(H_KCH, P1.Cin - c * H_KCH) + 15) >> 4);
+        mma_taps(P1, ahi0, ahi0 + (uint32_t)nch * R1 * 128);
       }
       drain();
       named_bar_sync(1, PIPE_MMA);             // both warpgroups' c1 wgmmas are done reading the set
@@ -937,7 +955,7 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
       // c2 over the resident tile
       for (int c = 0; c < nch2; ++c) {
         const uint32_t ahi0 = smem_u32(set) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * (MT / 2) - P2.lo_al) * 128u;
-        mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, P2.Cin - c * H_KCH) + 15) >> 4);
+        mma_taps(P2, ahi0, ahi0 + lo_part);
       }
       drain();
       named_bar_sync(1, PIPE_MMA);             // both warpgroups' c2 wgmmas are done reading the set
@@ -1027,17 +1045,16 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
   } else {
     setmaxnreg_dec<24>();
     if (warp != 12 || lane != 0) return;
-    // =========================== weight producer (warp 12): per tile c1's stages, then c2's ===========================
-    const uint32_t bytes = 2u * BN * 128u;
+    // ====================== weight producer (warp 12): per tile c1's half-stages, then c2's ======================
     int n_it = 0;
     for (int k = 0; k < nloc; ++k)
       for (int it = 0; it < total1 + total2; ++it, ++n_it) {
         const int s = n_it % NW, n = n_it / NW;
         if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
-        mbar_arrive_expect_tx(&w_full[s], bytes);
-        const uint8_t* src = it < total1 ? reinterpret_cast<const uint8_t*>(P1.w_h) + (size_t)it * bytes
-                                         : reinterpret_cast<const uint8_t*>(P2.w_h) + (size_t)(it - total1) * bytes;
-        bulk_g2s(smem + S.w[s], src, bytes, &w_full[s]);
+        mbar_arrive_expect_tx(&w_full[s], PIPE_STAGE);
+        const uint8_t* src = it < total1 ? reinterpret_cast<const uint8_t*>(P1.w_hk) + (size_t)it * PIPE_STAGE
+                                         : reinterpret_cast<const uint8_t*>(P2.w_hk) + (size_t)(it - total1) * PIPE_STAGE;
+        bulk_g2s(smem + S.w[s], src, PIPE_STAGE, &w_full[s]);
       }
   }
 }
@@ -1660,6 +1677,34 @@ void plane_split(const float* x, __half* hi, __half* lo, long n, float slope, cu
   AGPT_CUDA(cudaGetLastError());
 }
 
+// The BN = 128 image of a 128 -> 128 conv in half-stages for tcpair_pipe_kernel: [chunk64][tap][half][hi | lo][128 rows
+// x 64 B, SWIZZLE_64B], half h holding input channels 32 h .. 32 h + 31 of the chunk (the k-steps 2 h, 2 h + 1).  The
+// same fp16 values as build_h_image's, in 16 KB stages.
+static void build_hk_image(const PackedConv& pc, const std::vector<float>& h, float wscale, DevBuf& dst) {
+  const int nch = cdiv(pc.Cin, H_KCH), nt = pc.ntaps;
+  const size_t blk = (size_t)128 * 32;   // halves per hi (or lo) block
+  std::vector<uint16_t> img((size_t)nch * nt * 2 * 2 * blk, 0);
+  for (int c = 0; c < nch; ++c)
+    for (int t = 0; t < nt; ++t)
+      for (int hf = 0; hf < 2; ++hf) {
+        uint16_t* hi = &img[((((size_t)c * nt + t) * 2 + hf) * 2) * blk];
+        uint16_t* lo = hi + blk;
+        for (int j = 0; j < 128; ++j)
+          for (int k = 0; k < 32; ++k) {
+            const int ci = c * H_KCH + hf * 32 + k;
+            const float w = h[((size_t)t * pc.cin_pad + ci) * pc.cout_pad + j] * wscale;
+            const __half wh = __float2half_rn(w);
+            const __half wl = __float2half_rn(w - __half2float(wh));
+            const size_t off = (size_t)j * 32 + (size_t)(((k >> 3) ^ ((j >> 1) & 3)) << 3) + (k & 7);
+            memcpy(&hi[off], &wh, 2);
+            memcpy(&lo[off], &wl, 2);
+          }
+      }
+  std::vector<float> packed((img.size() + 1) / 2, 0.f);
+  memcpy(packed.data(), img.data(), img.size() * 2);
+  dst.upload(packed);
+}
+
 void pack_h_weights(PackedConv& pc, const std::vector<float>& h) {
   float mx = 0.f;
   for (float v : h) mx = std::max(mx, std::fabs(v));
@@ -1674,6 +1719,7 @@ void pack_h_weights(PackedConv& pc, const std::vector<float>& h) {
   build_h_image(pc, h, pc.tc_bn, wscale, pc.w_h);
   if (pc.tc_bn == 128) build_h_image(pc, h, 64, wscale, pc.w_h64);   // narrower tiles for launches that would not fill the SMs
   if (pc.tc_bn == 128 && pc.Cout > 128) build_h_image(pc, h, 96, wscale, pc.w_h96);
+  if (pc.tc_bn == 128 && pc.Cin == 128 && pc.Cout == 128 && !pc.is2d) build_hk_image(pc, h, wscale, pc.w_hk);
 }
 
 // lo_al = the lowest tap offset, R = operand-tile rows (MT + tap span, rounded to the 8-row swizzle atom); returns the span
@@ -1914,22 +1960,24 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, bool dual, cu
 }
 
 // One launch of tcpair_pipe_kernel: min(tiles, SMs) CTAs, each with two operand sets of 512 R1 bytes (R1: c1's operand
-// rows) and as many 32 KB weight stages as the rest of kMaxDyn holds, at least 2.  False -- nothing launched -- when the
-// handle does not allow it (TapConvParams::tc_pipe), the pair is not 128 -> 128 channels converted from fp32, or the
-// sets and two stages do not fit (c1 with a tap span of about 30 rows or more: k = 11 at dilation 5).
+// rows) and as many 16 KB weight half-stages as the rest of kMaxDyn holds, at least 4.  False -- nothing launched --
+// when the handle does not allow it (TapConvParams::tc_pipe), the pair is not 128 -> 128 channels converted from fp32
+// with half-stage images, or the sets and four half-stages do not fit (c1 with a tap span of about 30 rows or more:
+// k = 11 at dilation 5).
 static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
-  if (!P1.tc_pipe || P1.tc_bn != 128 || P1.Cin != 128 || P1.Cout != 128 || P2.Cout != 128 || P1.pi_hi || P2.po_hi)
+  if (!P1.tc_pipe || P1.tc_bn != 128 || P1.Cin != 128 || P1.Cout != 128 || P2.Cout != 128 || P1.pi_hi || P2.po_hi ||
+      !P1.w_hk || !P2.w_hk)
     return false;
   tc5_rows(P1, TC_ROWS);
   const int span2 = tc5_rows(P2, TC_ROWS);
   if (P2.R > P1.R) return false;   // c2's tile lives in c1's operand set
-  const long wbytes = 2L * 128 * 128;
+  const long wbytes = PIPE_STAGE;
   PipeSmem S;
   pipe_layout(S, P1.R, 0);
   const long spare = (long)kMaxDyn - 1024 - (long)S.total;
-  if (spare < 2 * wbytes) return false;
-  const int iters = P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps;
-  P1.tc_nw = (int)std::min<long>(std::min<long>(MAX_NW, std::max(2, iters)), spare / wbytes);
+  if (spare < 4 * wbytes) return false;
+  const int iters = 2 * (P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps);
+  P1.tc_nw = (int)std::min<long>(std::min<long>(PIPE_MAX_NW, iters), spare / wbytes);
   P2.tc_bn = 128;
   pipe_layout(S, P1.R, P1.tc_nw);
   const size_t smem = (size_t)S.total + 1024;
