@@ -23,6 +23,7 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.audio_detection.audio_infer.pytorch.models.PVT    (installed with install(detection=True))
     audiogpt_b200.audio_detection.target_sound_detection.src.models.RaDur_fusion
                                                                     (installed with install(target_detection=True))
+    audiogpt_b200.mono2binaural.src.models.BinauralNetwork          (installed with install(binaural=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -87,10 +88,17 @@ _TARGET_DETECTION_MAP = {
     "target_sound_detection.src.models": ("audiogpt_b200.audio_detection.target_sound_detection.src.models", ["RaDur_fusion"]),
 }
 
+# the Binaural tool's BinauralNetwork, grafted only on request (install(binaural=True)).  The tool imports it as
+# ``src.models`` (mono2binaural/ on its sys.path), a generic name: the module is patched in place only when it is the
+# reference's (it defines Warpnet and BinauralNetwork), and never aliased.
+_BINAURAL_MAP = {
+    "src.models": ("audiogpt_b200.mono2binaural.src.models", ["BinauralNetwork"]),
+}
+
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
             text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False, detection: bool = False,
-            target_detection: bool = False):
+            target_detection: bool = False, binaural: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -125,6 +133,10 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     tool's Cnn14 reference encoder, multi-scale CNN, bidirectional GRU and enhancement pass run on the engine.  That
     module is only patched in place: the tool also imports its ``event_labels``, so when it does not import it is
     reported as skipped (and raises under ``strict``), never aliased.
+    ``binaural=True`` also replaces ``src.models.BinauralNetwork`` (mono2binaural/src/models.py), so the Binaural tool's
+    geometric and neural time warp run on the engine.  ``src`` is a generic name, so the module is patched in place only
+    when it is the reference's (it defines ``Warpnet`` and ``BinauralNetwork``); when it does not import or is some other
+    ``src``, it is reported as skipped (and raises under ``strict``), never aliased.
     Returns the list of patched names."""
     import importlib
     import sys
@@ -168,6 +180,25 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
                 if strict:
                     raise
                 patched.append(ref_name + " (skipped: not importable)")
+                continue
+            for a in attrs:
+                setattr(ref, a, getattr(ours, a))
+            patched.append(ref_name)
+    if binaural:
+        for ref_name, (our_name, attrs) in _BINAURAL_MAP.items():
+            ours = importlib.import_module(our_name)
+            try:
+                ref = importlib.import_module(ref_name)
+            except Exception:
+                if strict:
+                    raise
+                patched.append(ref_name + " (skipped: not importable)")
+                continue
+            if not all(isinstance(getattr(ref, n, None), type) for n in ("Warpnet", "BinauralNetwork")):
+                if strict:
+                    raise ImportError(f"{ref_name} ({getattr(ref, '__file__', None)}) is not mono2binaural's: it lacks "
+                                      "Warpnet / BinauralNetwork")
+                patched.append(ref_name + " (skipped: not mono2binaural's)")
                 continue
             for a in attrs:
                 setattr(ref, a, getattr(ours, a))

@@ -112,6 +112,16 @@ class TsdConfig(C.Structure):
         ("tao", C.c_float), ("mel_bins", C.c_int), ("outputdim", C.c_int)]
 
 
+class BinauralConfig(C.Structure):
+    """agpt_binaural_cfg (the create entry point takes a plain pointer)."""
+    _fields_ = [("layers", C.c_int), ("channels", C.c_int)]
+
+
+class BinauralRow(C.Structure):
+    """agpt_binaural_row: one BinauralNetwork forward (a batch item or a chunk of the tool's loop)."""
+    _fields_ = [(n, C.c_int64) for n in ("mono_off", "T", "view_off", "view_stride", "K", "keep", "out_off", "out_stride")]
+
+
 class TapconvProbeArgs(C.Structure):
     """agpt_tapconv_probe_args (a tagged struct in the header: it carries pointers and floats)."""
     _fields_ = [(n, C.c_int) for n in ("kind", "Cin", "Cout", "K", "dil", "Wreal", "strip_w", "u", "pad", "g")] + [
@@ -214,6 +224,10 @@ PROTOTYPES = {
     "agpt_tsd_avgpool": (_I, [_P, _I, _I, _I, _I, _I, _I, _P, _P]),
     "agpt_tsd_gru": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "agpt_tsd_enhance": (_I, [_P, _I, _I, _I, _P, _I, _P, _I, _F, _W, _P, _P, _P, _P, _P]),
+    "agpt_binaural_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_binaural_forward": (_I, [_P, _P, _P, _P, _I, _P, _I, _P]),
+    "agpt_binaural_frames": (_I, [_P, _P, _P, _I, _P, _P]),
+    "agpt_binaural_warp": (_I, [_P, _P, _P, _P, _I, _P, _I, _P]),
 }
 
 _lock = threading.Lock()

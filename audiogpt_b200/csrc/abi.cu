@@ -537,6 +537,37 @@ int agpt_tsd_enhance(const float* p1, int B, int Td, int O, const float* mix_emb
   });
 }
 
+int agpt_binaural_create(const agpt_binaural_cfg* cfg, const float* const* host_weights, int n_weights, int device,
+                         agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(binaural_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_binaural_forward(agpt_handle h, const float* mono, const float* view, const agpt_binaural_row* rows, int n_rows,
+                          float* out, int clamp, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(mono && view && out, "null argument");
+    binaural_forward(as(h, kMagicBinaural, "binaural"), mono, view, rows, n_rows, out, clamp, (cudaStream_t)stream);
+  });
+}
+
+int agpt_binaural_frames(agpt_handle h, const float* view, const agpt_binaural_row* rows, int n_rows, float* field, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(view && field, "null argument");
+    binaural_frames(as(h, kMagicBinaural, "binaural"), view, rows, n_rows, field, (cudaStream_t)stream);
+  });
+}
+
+int agpt_binaural_warp(agpt_handle h, const float* field, const float* mono, const agpt_binaural_row* rows, int n_rows,
+                       float* out, int clamp, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(field && mono && out, "null argument");
+    binaural_warp(as(h, kMagicBinaural, "binaural"), field, mono, rows, n_rows, out, clamp, (cudaStream_t)stream);
+  });
+}
+
 int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                        double* out2, double* dbg8_or_null) {
   return guarded([&] {

@@ -102,6 +102,13 @@ void tsd_gru(const float* whh, const float* bhh, const float* xp, int B, int T, 
 void tsd_enhance(const float* p1, int B, int Td, int O, const float* Emix, int Te, const float* emb, int top, float tao,
                  const float* const wts[8], float* me, float* wmix, int* idx, float* val, cudaStream_t st);
 
+Handle* binaural_create(const agpt_binaural_cfg* cfg, const float* const* W, int nW, int device);
+void binaural_forward(Handle* h, const float* mono, const float* view, const agpt_binaural_row* rows, int n, float* out, int clamp,
+                      cudaStream_t st);
+void binaural_frames(Handle* h, const float* view, const agpt_binaural_row* rows, int n, float* field, cudaStream_t st);
+void binaural_warp(Handle* h, const float* field, const float* mono, const agpt_binaural_row* rows, int n, float* out, int clamp,
+                   cudaStream_t st);
+
 void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
                    double* out, double* dbg_avg);
 void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);

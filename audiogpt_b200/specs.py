@@ -1672,3 +1672,106 @@ def synth_tsd_mel(T: int, seed: int, B: int = 1) -> torch.Tensor:
             v = v + env * (3.0 + 2.0 * rs.rand(1, 64) + 0.5 * np.sin(t / rs.uniform(2, 10)))
         x[b] = v
     return torch.from_numpy(x.astype(np.float32))
+
+
+# ---------------------------------------------------------------------------------------------------------- Binaural
+# mono2binaural/src/models.py BinauralNetwork(view_dim=7, warpnet_layers=4, warpnet_channels=64): the Binaural tool's
+# network (audio-chatgpt.py:713-773).  The view is 7 x K: a position (metres) and a scalar-last quaternion per frame,
+# one frame per 400 samples at 48 kHz.
+BINAURAL = dict(layers=4, channels=64)
+BINAURAL_SMALL = dict(layers=2, channels=16)
+BINAURAL_VIEW_DIM = 7
+BINAURAL_HOP = 400
+
+
+def binaural_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """The state-dict keys and shapes of BinauralNetwork (Warpnet's convs; its warpers hold no parameters), in the order
+    agpt_binaural_create consumes them."""
+    C = int(cfg["channels"])
+    out: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    for l in range(int(cfg["layers"])):
+        out[f"warper.layers.{l}.weight"] = (C, BINAURAL_VIEW_DIM if l == 0 else C, 2)
+        out[f"warper.layers.{l}.bias"] = (C,)
+    out["warper.linear.weight"] = (2, C, 1)
+    out["warper.linear.bias"] = (2,)
+    return out
+
+
+def synth_binaural(cfg, seed: int = 4242, warp_gain: float = 250.0):
+    """Seeded BinauralNetwork weights: He-gain convs and a linear head at warp_gain, so the neural warp spans about a
+    few hundred samples either side of zero -- enough to push some frames' total warp above 0, where the reference clips
+    it."""
+    return synth_state_dict(binaural_param_shapes(cfg), seed, convtranspose_prefixes=(),
+                            gains={"warper.layers.": math.sqrt(2.0), "warper.linear.": warp_gain})
+
+
+def synth_binaural_view(K: int, seed: int, B: int = 1) -> torch.Tensor:
+    """A seeded trajectory [B][7][K] fp32: the transmitter wanders 0.5-3 m from the listener (a smooth random walk in
+    direction and distance) and turns through random unit quaternions (x, y, z, w), a new one every few frames."""
+    rs = np.random.RandomState(int(seed))
+    out = np.empty((B, BINAURAL_VIEW_DIM, int(K)), dtype=np.float64)
+    for b in range(B):
+        d = np.cumsum(rs.randn(int(K), 3) * 0.05, axis=0) + rs.randn(3)
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+        r = 1.75 + 1.25 * np.sin(np.cumsum(rs.uniform(0.0, 0.2, int(K))) + rs.uniform(0, 2 * np.pi))
+        out[b, 0:3] = (d * r[:, None]).T
+        q = rs.randn(int(K), 4)
+        hold = rs.randint(1, 6)
+        q = np.repeat(q[::hold], hold, axis=0)[: int(K)]
+        out[b, 3:7] = (q / np.linalg.norm(q, axis=1, keepdims=True)).T
+    return torch.from_numpy(out.astype(np.float32))
+
+
+def synth_binaural_mono(L: int, seed: int, B: int = 1) -> torch.Tensor:
+    """Seeded mono clips [B][L] as a loaded 16-bit wav is: int16 PCM / 32768.  A few sines up to 2 kHz under a slow
+    envelope, plus a little noise."""
+    rs = np.random.RandomState(int(seed))
+    t = np.arange(int(L)) / 48000.0
+    out = np.empty((B, int(L)))
+    for b in range(B):
+        x = sum(rs.uniform(0.05, 0.25) * np.sin(2 * np.pi * rs.uniform(50, 2000) * t + rs.uniform(0, 2 * np.pi)) for _ in range(4))
+        x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.2, 2.0) * t)) + 0.01 * rs.randn(int(L))
+        out[b] = x
+    pcm = np.clip(np.round(out * 32768.0), -32768, 32767).astype(np.int16)
+    return torch.from_numpy(pcm.astype(np.float32) / 32768.0)
+
+
+def binaural_nearest(T: int, K: int) -> np.ndarray:
+    """F.interpolate(mode='nearest', size=T) source frame of each of T samples from K frames (UpSample.h nearest_idx:
+    the identity when K == T, i >> 1 when T == 2K, else min(floor(float(i) * (float(K) / float(T))), K - 1) in fp32)."""
+    i = np.arange(int(T), dtype=np.int64)
+    if K == T:
+        return i
+    if T == 2 * K:
+        return i >> 1
+    scale = np.float32(K) / np.float32(T)
+    return np.minimum(np.floor(i.astype(np.float32) * scale).astype(np.int64), int(K) - 1)
+
+
+def binaural_chunks(L: int, Kv: int, chunk_size: int = 48000, rec_field: int = 800):
+    """The Binaural tool's chunk plan (audio-chatgpt.py:729-766) for a mono clip of L samples and a view of Kv frames.
+
+    When Kv * 400 != L the clip is trimmed to a multiple of 400 and a longer view keeps its last L' / 400 frames (the
+    tool slices from m_a; its random start is never used); a shorter view is left as it is.  Chunk i (a multiple of
+    chunk_size) reads mono[max(0, i - rec_field) : i + chunk_size] and view[max(0, i - rec_field) // 400 : (i +
+    chunk_size) // 400]; every chunk after the first keeps binaural[:, -(T - rec_field):].
+
+    Returns (L_out, rows): rows are dicts of mono_off, T, view_off (a frame of the untrimmed view), K, keep (the first
+    kept sample) and out_off, in the output's order.  A chunk whose view slice is empty has K = 0: the reference's
+    F.interpolate raises there."""
+    L, Kv, cs, rf = int(L), int(Kv), int(chunk_size), int(rec_field)
+    vs, kv = 0, Kv
+    if Kv * BINAURAL_HOP != L:
+        L = (L // BINAURAL_HOP) * BINAURAL_HOP
+        if Kv * BINAURAL_HOP > L:
+            vs = Kv - L // BINAURAL_HOP
+            kv = L // BINAURAL_HOP
+    rows, out = [], 0
+    for n, i in enumerate(range(0, L, cs)):
+        m0, m1 = max(0, i - rf), min(L, i + cs)
+        v0, v1 = max(0, i - rf) // BINAURAL_HOP, min(kv, (i + cs) // BINAURAL_HOP)
+        T = m1 - m0
+        keep = 0 if n == 0 else slice(-(T - rf), None).indices(T)[0]
+        rows.append(dict(mono_off=m0, T=T, view_off=vs + min(v0, kv), K=max(0, v1 - v0), keep=keep, out_off=out))
+        out += T - keep
+    return out, rows

@@ -607,6 +607,39 @@ int agpt_tsd_gru(const float* w_hh, const float* b_hh, const float* xproj, int B
 int agpt_tsd_enhance(const float* p1, int B, int Td, int O, const float* mix_emb, int Te, const float* emb, int top, float tao,
                      const float* const* weights8, float* me, float* wmix, int* topk_idx, float* topk_val, void* stream);
 
+/* ------------------------------------------------------------------ Binaural
+ * The Binaural tool (audio-chatgpt.py:713-773): mono2binaural/src/models.py BinauralNetwork -> Warpnet, eval mode.  A
+ * warpnet of `layers` causal convs (F.pad([1, 0]), Conv1d(k = 2), ReLU; 7 -> C, then C -> C) and a 1 x 1 Conv1d C -> 2
+ * plus a geometric warp from the mouth-to-ear distance give each view frame a warp per ear; it is selected per sample
+ * as F.interpolate(mode = 'nearest') does, clipped to <= 0, added to the sample index, clamped to [0, T - 1], made
+ * monotone by a running max, and the mono signal is read there by linear interpolation, for each ear.          */
+typedef struct agpt_binaural_cfg {
+  int layers;             /* warpnet_layers: 1..4 (the tool ships 4) */
+  int channels;           /* warpnet_channels: a multiple of 8 in [8, 64] (the tool ships 64) */
+} agpt_binaural_cfg;
+/* One row: one BinauralNetwork forward of T samples and K view frames.  mono[mono_off + t], t < T; view channel c of
+ * frame k at view[view_off + c * view_stride + k]; samples t >= keep of ear e go to out[out_off + e * out_stride + t -
+ * keep].  A batch is B rows of one shape; the tool's chunk loop is one row per chunk, each writing its kept tail.   */
+typedef struct agpt_binaural_row {
+  int64_t mono_off, T, view_off, view_stride, K, keep, out_off, out_stride;
+} agpt_binaural_row;
+/* host_weights: fp32 HOST arrays in the order of audiogpt_b200.specs.binaural_param_shapes(cfg): warper.layers.{l}
+ * .weight [C][cin][2] and .bias [C] for each layer, then warper.linear.weight [2][C][1] and .bias [2].             */
+int agpt_binaural_create(const agpt_binaural_cfg* cfg, const float* const* host_weights, int n_weights, int device,
+                         agpt_handle* out);
+/* mono and view (device) -> out (device) for n_rows rows (a HOST array): three launches whatever the rows, no host
+ * synchronisation.  clamp = 1 clamps every output sample to [-1, 1] (the tool's final clamp).  Every row needs
+ * 1 <= T <= 2^24, K >= 1 and 0 <= keep < T.  The frame field, tile maxima and row table are workspaces of the handle:
+ * calls on one handle must be ordered on one stream (calls from two streams at once race on them).               */
+int agpt_binaural_forward(agpt_handle h, const float* mono, const float* view, const agpt_binaural_row* rows, int n_rows,
+                          float* out, int clamp, void* stream);
+/* The two stages apart (the unit tests' entry points).  frames: view -> the frame field, rows packed one after the
+ * other, each [2][K]: f[e][k] = ((-d_e) / 343) * 48000 + n_e[k], d_e the mouth-to-ear distance, n the warpnet output.
+ * warp: a frame field in that layout and mono -> out, as agpt_binaural_forward does after its frame stage.          */
+int agpt_binaural_frames(agpt_handle h, const float* view, const agpt_binaural_row* rows, int n_rows, float* field, void* stream);
+int agpt_binaural_warp(agpt_handle h, const float* field, const float* mono, const agpt_binaural_row* rows, int n_rows,
+                       float* out, int clamp, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
