@@ -89,6 +89,7 @@ void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st
   AGPT_CHECK(!a.plane_in || (a.pro == PRO_LRELU && !a.fma), "tapconv probe: plane input needs PRO_LRELU on the tensor cores");
   AGPT_CHECK(!a.pair || (a.kind == 0 && a.w2 && a.res && a.Cin == a.Cout && !a.fma),
              "tapconv probe: a pair is two Conv1d C -> C with a residual, on the tensor cores");
+  AGPT_CHECK(!a.pair || (!a.plane_in && !a.po_hi), "tapconv probe: a pair reads and writes fp32 only, no operand planes");
   const int dil = a.dil > 0 ? a.dil : 1;
   int gk = 1;   // time steps per row of the grouped view (kind 3)
   PackedConv pc, pc2;

@@ -13,14 +13,19 @@
 // a conv tap = a row-shifted descriptor start address.  Two worker warpgroups convert fp32 activations into the fp16
 // hi/lo tiles, then each issues wgmma for its MT / 2 rows (MT / 128 blocks of 64) with the accumulators in registers
 // (one wgmma group in flight while the next chunk is converted), then runs the fused epilogue; warp 8 streams the
-// weights (cp.async.bulk, mbarrier full/empty ring).  The plane-fed variants (tcconv5_pl_kernel, tcpair_pl_kernel)
-// take the input as pre-split fp16 hi/lo planes: warp 8 also loads them by TMA, and the workers skip the transform.
+// weights (cp.async.bulk, mbarrier full/empty ring).  The plane-fed variant (tcconv5_pl_kernel) takes the input as
+// pre-split fp16 hi/lo planes: warp 8 also loads them by TMA, and the workers skip the transform.
+// The fused-pair kernels and the warp-specialised pipelines further down reuse the phases defined once here (hi/lo
+// split, raw staging, one wgmma group, the c1 -> c2 hand-off, accumulator staging, the fused epilogue, a weight-ring
+// step), so that every kernel that must match another bit for bit runs the same code for them.
 #include "tapconv.cuh"
 #include "tapconv_epi.cuh"
 #include "tc_common.cuh"
 #include "tc_h16.cuh"
 #include "tc_tma.cuh"
 #include "models.h"
+
+#include <set>
 
 namespace agpt {
 
@@ -87,6 +92,225 @@ __device__ __forceinline__ int item_row(int xt, int i) { return (xt >> 3) + i * 
 constexpr int TC_TALL = 256;                 // rows of a tall tile (BN <= 64 only: the doubled accumulator still fits)
 constexpr uint64_t BLK_DESC = (64 * 128) >> 4;   // descriptor start-address step from one 64-row block to the next
 
+// A worker warpgroup's accumulator acc[MB][NJ][NH]: row block b = 64 rows, column block j = NB = 2 NH columns (wgmma
+// fragment layout), BN = NJ NB columns in all.
+template <int MB, int NJ, int NH>
+__device__ __forceinline__ void fence_tile(float (&acc)[MB][NJ][NH]) {
+#pragma unroll
+  for (int b = 0; b < MB; ++b)
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) fence_acc<NH>(acc[b][j]);
+}
+template <int MB, int NJ, int NH>
+__device__ __forceinline__ void zero_tile(float (&acc)[MB][NJ][NH]) {
+#pragma unroll
+  for (int b = 0; b < MB; ++b)
+#pragma unroll
+    for (int j = 0; j < NJ; ++j)
+#pragma unroll
+      for (int i = 0; i < NH; ++i) acc[b][j][i] = 0.f;
+}
+
+// hi / lo fp16 parts of 8 channels (x0: channels 0..3, x1: 4..7): one 16-byte unit of the hi and of the lo operand tile
+__device__ __forceinline__ void split8(const float4 x0, const float4 x1, uint4& h, uint4& l) {
+  h.x = split2(x0.x, x0.y, l.x);
+  h.y = split2(x0.z, x0.w, l.y);
+  h.z = split2(x1.x, x1.y, l.z);
+  h.w = split2(x1.z, x1.w, l.w);
+}
+
+// Raw fp32 staging of chunk c (channels 64 c ..) of the RRA operand rows into dst, by the NWK worker threads (xt);
+// rowinfo[r]: row r's offset in ing, or -1 outside the sample.  Row r = 256 bytes; 16-byte unit u (4 channels) sits at
+// slot (u >> 1) + 8 * (u & 1), so that the two units of one 8-channel item are read conflict-free by the transform.
+__device__ __forceinline__ void issue_raw(uint8_t* dst, const TapConvParams& P, const float* __restrict__ ing,
+                                          const int* rowinfo, int RRA, int c, int xt) {
+  const int kv = min(H_KCH, P.Cin - c * H_KCH);          // valid channels of this chunk
+  const int nu = ((kv + 15) >> 4) << 2;                  // 16-byte units the MMA k-steps will touch
+  for (int idx = xt; idx < RRA * 16; idx += NWK) {
+    const int row = idx >> 4, u = idx & 15;
+    if (u >= nu) continue;
+    const int ch = c * H_KCH + 4 * u;
+    const int a = rowinfo[row];
+    const bool ok = (a >= 0) && (ch < P.Cin);
+    cp_async16_zfill(dst + row * 256 + (((u >> 1) + ((u & 1) << 3)) << 4), ok ? (ing + a + ch) : P.in, ok ? 16u : 0u);
+  }
+  cp_async_commit_();
+}
+
+// One wgmma group of one tap over a resident K-major SWIZZLE_128B operand tile: per k-step, row block b (the operand
+// descriptors dah / dal shifted by 64 b rows) and column block j, the products x_hi w_hi + x_lo w_hi + x_hi w_lo into
+// acc[b][j]; ws: the weight stage, [hi | lo][BN rows x 128 B].  At most this group stays in flight; the older one has
+// then completed, so its weight stage, ring slot rel (-1: none), is released on w_empty[rel].
+template <int MB, int NJ, int NH>
+__device__ __forceinline__ void mma_group(float (&acc)[MB][NJ][NH], uint64_t dah, uint64_t dal, uint32_t ws, int ksteps,
+                                          uint64_t* w_empty, int rel) {
+  constexpr int NB = 2 * NH, BN = NJ * NB;
+  fence_tile(acc);
+  wgmma_fence();
+  for (int k = 0; k < ksteps; ++k) {
+    const uint64_t ko = (uint64_t)((k * 32) >> 4);
+#pragma unroll
+    for (int b = 0; b < MB; ++b)
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
+        const uint64_t ab = ko + b * BLK_DESC;
+        wgmma_nb<NB>(acc[b][j], dah + ab, dwh);
+        wgmma_nb<NB>(acc[b][j], dal + ab, dwh);
+        wgmma_nb<NB>(acc[b][j], dah + ab, dwl);
+      }
+  }
+  wgmma_commit();
+  wgmma_wait<1>();
+  fence_tile(acc);
+  if (rel >= 0 && (threadIdx.x & 31) == 0) mbar_arrive(&w_empty[rel]);
+}
+// the end of a conv's wgmmas: all completed, the last weight stage, ring slot rel (-1: none), released on w_empty[rel]
+template <int MB, int NJ, int NH>
+__device__ __forceinline__ void mma_drain(float (&acc)[MB][NJ][NH], uint64_t* w_empty, int rel) {
+  wgmma_wait<0>();
+  fence_tile(acc);
+  if (rel >= 0 && (threadIdx.x & 31) == 0) mbar_arrive(&w_empty[rel]);
+}
+
+// Columns cb .. cb + 31 of the accumulator x descale -> the swizzled staging block stg [rows][32 fp32]; r0 / c0: this
+// thread's first fragment row (of row block 0) and column.
+template <int MB, int NJ, int NH>
+__device__ __forceinline__ void stage_block(const float (&acc)[MB][NJ][NH], uint8_t* stg, int cb, int r0, int c0, float dsc) {
+  constexpr int NB = 2 * NH;
+#pragma unroll
+  for (int b = 0; b < MB; ++b) {
+    const float* a = &acc[b][cb / NB][4 * ((cb % NB) / 8)];
+    const int r = r0 + 64 * b;
+#pragma unroll
+    for (int i8 = 0; i8 < 4; ++i8) {
+      const int col = 8 * i8 + c0;
+      *reinterpret_cast<float2*>(stg + sw128(r, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
+      *reinterpret_cast<float2*>(stg + sw128(r + 8, col >> 2) + (col & 3) * 4) =
+          make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
+    }
+  }
+}
+
+// The fused epilogue of a worker-warpgroup tile [MT rows x BN] of P at output columns co0 .. (rowp: a tile row's output
+// row, or -1): registers (x inverse weight scale) -> swizzled staging block [MT rows][32 cols] in shared memory (two of
+// them, 2 x MT x 128 B inside the first operand buffers, which are free by then: tc5_plan) -> coalesced (row, 16-byte
+// chunk) items through the fused epilogue.  wg: the worker warpgroup (rows MT/2 wg .. of the tile).  The
+// global READS of the first LA items of a block (residual / old accumulator) are issued one block ahead -- on a 128-row
+// tile with LA = 4 for block 0 before the accumulator is complete.  A tall tile, and LA < 4 (tcpair2_kernel, within
+// the registers of two CTAs per SM), read block 0 once that block is staged, not next to the whole accumulator, and
+// item i + LA once item i is stored.  dbg: the timed thread's debug record (tcconv5_body), else null.
+template <int BN, int MT, int LA, bool PL, int MB, int NJ, int NH>
+__device__ __forceinline__ void tile_epilogue(float (&acc)[MB][NJ][NH], const TapConvParams& P, int g, int co0,
+                                              const int* rowp, uint8_t* smem, const Tc5Smem& S, int wg, int xt,
+                                              long long* dbg) {
+  constexpr bool early = MT == TC_ROWS && LA == 4;
+  EpiPre pre[8];
+  int pp[8];
+  constexpr int nitem = (MT * 8) / NWK;   // 4 items per worker and block (8 on a tall tile)
+  const float dsc = P.tc_descale;
+  auto load_block = [&](int cb) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int idx = xt + i * NWK;
+      pp[i] = (i < LA && i < nitem) ? rowp[early ? idx >> 3 : item_row(xt, i)] : -1;
+      if (pp[i] >= 0) epi_load(P, g, pp[i], co0 + cb + 4 * (idx & 7), pre[i]);
+    }
+  };
+  if (early) load_block(0);
+  if (dbg) { dbg[2] = dbg[1]; dbg[3] = clock64(); dbg[6] = 0; dbg[7] = 0; }   // the workers issue the wgmmas: no waits of a separate issuer
+  mma_drain(acc, nullptr, -1);
+  named_bar_sync(1, NWK);                      // both warpgroups' wgmmas are done reading the operand buffers
+  if (dbg) dbg[4] = clock64();
+  uint8_t* stg0 = smem + S.a_hi[0];
+  const int lane = xt & 31, r0 = wg * (MT / 2) + ((xt >> 5) & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int blk = 0; blk < BN / 32; ++blk) {
+    const int cb = blk * 32;
+    uint8_t* stg = stg0 + (blk & 1) * (MT * 128);
+    stage_block(acc, stg, cb, r0, c0, dsc);
+    if (!early && blk == 0) load_block(0);
+    named_bar_sync(1, NWK);
+    const int jc = xt & 7;                       // all items of this thread share the 4-channel group
+    const float4 cv = epi_colvec(P, g, co0 + cb + 4 * jc);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int idx = xt + i * NWK;
+      const int row = (idx >> 3) & (MT - 1);   // pp[i] < 0 for i >= LA until read below
+      if (pp[i] >= 0)
+        epi_store_cv<PL>(P, g, pp[i], co0 + cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
+      if (i + LA < nitem) {
+        const int idxa = idx + LA * NWK;
+        pp[i + LA] = rowp[item_row(xt, i + LA)];
+        if (pp[i + LA] >= 0) epi_load(P, g, pp[i + LA], co0 + cb + 4 * (idxa & 7), pre[i + LA]);
+      }
+    }
+    if (cb + 32 < BN) load_block(cb + 32);
+    // staging halves alternate; a half is rewritten two blocks later, after the next named
+    // barrier, so no extra barrier is needed here
+  }
+  if (dbg) dbg[5] = clock64();
+}
+
+// c1 -> c2 hand-off of a fused pair: c1's accumulator becomes c2's operand tile a2 with the arithmetic of c1's EPI_BIAS
+// store followed by c2's PRO_LRELU transform (acc * descale + bias, leaky ReLU, hi/lo split), so c2 multiplies the
+// operands a separate launch would.  The tile [P2.R rows][C channels] (K-major SWIZZLE_128B: nch2 hi blocks of 64
+// channels, then nch2 lo blocks) replaces c1's operand buffers: rows outside the sample are c2's zero padding, channels
+// >= C are zero, rows MT .. RR2 - 1 (RR2 = P2.R) feed only the discarded outputs and are zero (written by the nthr
+// threads xt).  Lv = P1.L; r0 / c0: this thread's first fragment row and column; qa: the sample row of tile row 0.
+// Clears acc for c2.
+template <int MT, int MB, int NJ, int NH>
+__device__ __forceinline__ void pair_handoff(float (&acc)[MB][NJ][NH], const TapConvParams& P1, const TapConvParams& P2,
+                                             uint8_t* a2, int nch2, int RR2, int Lv, int r0, int c0, int qa, int xt, int nthr) {
+  constexpr int NB = 2 * NH;
+  const int C2 = P2.Cin;
+  const uint32_t lo_part = (uint32_t)nch2 * RR2 * 128;   // the hi blocks, then the lo blocks
+  const float dsc1 = P1.tc_descale;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j)
+#pragma unroll
+    for (int i = 0; i < NB / 8; ++i) {
+      const int col = j * NB + 8 * i + c0;   // accumulator fragment layout: see wgmma_n16
+      const bool cok = col < C2;
+      float2 bv = make_float2(0.f, 0.f);
+      if (cok && P1.bias) bv = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
+      uint8_t* hi = a2 + (uint32_t)(col >> 6) * RR2 * 128;
+#pragma unroll
+      for (int b = 0; b < MB; ++b)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = r0 + 64 * b + 8 * h;
+          float v0 = 0.f, v1 = 0.f;
+          if (cok && qa + r >= 0 && qa + r < Lv) {
+            v0 = lrelu(__fadd_rn(__fmul_rn(acc[b][j][4 * i + 2 * h], dsc1), bv.x), P2.slope);
+            v1 = lrelu(__fadd_rn(__fmul_rn(acc[b][j][4 * i + 2 * h + 1], dsc1), bv.y), P2.slope);
+          }
+          uint32_t l;
+          const uint32_t hw = split2(v0, v1, l);
+          const uint32_t o = sw128(r, (col & 63) >> 3) + (col & 7) * 2;
+          *reinterpret_cast<uint32_t*>(hi + o) = hw;
+          *reinterpret_cast<uint32_t*>(hi + lo_part + o) = l;
+        }
+    }
+  const int zitems = (RR2 - MT) * 8;         // 16-byte units of rows MT .. RR2 - 1 per block
+  for (int idx = xt; idx < zitems * 2 * nch2; idx += nthr) {
+    const int blk = idx / zitems, u = idx - blk * zitems;
+    *reinterpret_cast<uint4*>(a2 + (uint32_t)blk * RR2 * 128 + MT * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
+  }
+  zero_tile(acc);
+  fence_proxy_async();                       // generic-proxy stores -> visible to c2's wgmma operand reads
+}
+
+// Weight stage `it` of a ring of NW slots (smem + w[s]): once the wgmma warps released the slot's previous stage, copy
+// `bytes` from src into it, completing on w_full[s].
+__device__ __forceinline__ void ring_put(uint8_t* smem, const uint32_t* w, uint64_t* w_full, uint64_t* w_empty, int NW,
+                                         int it, const uint8_t* src, uint32_t bytes) {
+  const int s = it % NW, n = it / NW;
+  if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
+  mbar_arrive_expect_tx(&w_full[s], bytes);
+  bulk_g2s(smem + w[s], src, bytes, &w_full[s]);
+}
+
 // Plane-fed operand chunk c (channels 64 c ..) of rows r0 .. r0 + R - 1 of sample g into operand buffer c % NA, hi
 // and lo planes, completing on a_full; the buffer's previous chunk must have been released on a_empty first.  Rows
 // outside the sample and channels past C load as zeros, which is the conv's zero padding: split(lrelu(0)) = 0.
@@ -125,7 +349,7 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
   int* rowinfo = reinterpret_cast<int*>(smem + S.rowinfo);
   int* rowp = reinterpret_cast<int*>(smem + S.rowp);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
   // warpgroup index broadcast from lane 0: ptxas then sees the role branches as warpgroup-uniform, which keeps the
   // wgmmas of the worker warpgroups asynchronous instead of serialized
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // workers: output rows MT/2 wg .. MT/2 (wg + 1) - 1 of the tile
@@ -162,25 +386,9 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
     // =========================== worker warps: transform ===========================
     const float* __restrict__ ing = P.in + g * P.in_gstride;
     const float* pvg = (P.pro == PRO_ADDVEC) ? (P.pvec + (long)g * P.pvec_gstride) : nullptr;
-    // raw fp32 staging: row r = 256 bytes; 16-byte unit u (4 channels) sits at slot (u >> 1) + 8 * (u & 1),
-    // so that the two units of one 8-channel item are read conflict-free (see the transform loop)
-    auto issue_raw = [&](int c, int rb) {
-      uint8_t* dst = smem + S.raw[rb];
-      const int kv = min(H_KCH, P.Cin - c * H_KCH);          // valid channels of this chunk
-      const int nu = ((kv + 15) >> 4) << 2;                  // 16-byte units the MMA k-steps will touch
-      for (int idx = xt; idx < RRA * 16; idx += NWK) {
-        const int row = idx >> 4, u = idx & 15;
-        if (u >= nu) continue;
-        const int ch = c * H_KCH + 4 * u;
-        const int a = rowinfo[row];
-        const bool ok = (a >= 0) && (ch < P.Cin);
-        cp_async16_zfill(dst + row * 256 + (((u >> 1) + ((u & 1) << 3)) << 4), ok ? (ing + a + ch) : P.in, ok ? 16u : 0u);
-      }
-      cp_async_commit_();
-    };
     if constexpr (!PL) {
-      issue_raw(0, 0);
-      if (NR == 2 && nchunks > 1) issue_raw(1, 1);
+      issue_raw(smem + S.raw[0], P, ing, rowinfo, RRA, 0, xt);
+      if (NR == 2 && nchunks > 1) issue_raw(smem + S.raw[1], P, ing, rowinfo, RRA, 1, xt);
     }
     {  // pull the epilogue's global operands (residual / old accumulator) into L2 while the main loop runs
       const float* pf0 = nullptr; long gs0 = 0; int pitch0 = 0;
@@ -203,12 +411,7 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
     // this warpgroup's accumulator: row block b = rows MT/2 wg + 64 b .. + 63, BN columns in NJ blocks of NB (wgmma
     // fragment layout)
     float acc[MB][NJ][NB / 2];
-#pragma unroll
-    for (int b = 0; b < MB; ++b)
-#pragma unroll
-      for (int j = 0; j < NJ; ++j)
-#pragma unroll
-        for (int i = 0; i < NB / 2; ++i) acc[b][j][i] = 0.f;
+    zero_tile(acc);
     const int items = RRA * 8;
     int it = 0, prev = -1;     // prev: weight stage of the newest wgmma group, released once that group has completed
     for (int c = 0; c < nchunks; ++c) {
@@ -243,10 +446,7 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
         const float4 x0 = pro_apply5(P, v0, rowok && ch < P.Cin, pvg ? (pvg + ch) : nullptr);
         const float4 x1 = pro_apply5(P, v1, rowok && ch + 4 < P.Cin, pvg ? (pvg + ch + 4) : nullptr);
         uint4 h, l;
-        h.x = split2(x0.x, x0.y, l.x);
-        h.y = split2(x0.z, x0.w, l.y);
-        h.z = split2(x1.x, x1.y, l.z);
-        h.w = split2(x1.z, x1.w, l.w);
+        split8(x0, x1, h, l);
         const uint32_t o = sw128(row, q);
         *reinterpret_cast<uint4*>(ahi + o) = h;
         *reinterpret_cast<uint4*>(alo + o) = l;
@@ -254,121 +454,29 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
       fence_proxy_async();               // generic-proxy stores -> visible to wgmma operand reads
       named_bar_sync(1, NWK);            // a_*[buf] complete; everyone finished reading raw[rb]
       const int cn = c + NR;
-      if (cn < nchunks) issue_raw(cn, rb);
+      if (cn < nchunks) issue_raw(smem + S.raw[rb], P, ing, rowinfo, RRA, cn, xt);
       }
       // =========================== worker warps: wgmma over the taps of chunk c ===========================
-      // products x_hi w_hi + x_lo w_hi + x_hi w_lo into one fp32 accumulator; a tap is a start address shifted by rows,
-      // a row block one shifted by 64 rows more: every block reuses the weight stage, which is released (one group
-      // later) when the group holding all blocks' wgmmas has completed
+      // a tap is a start address shifted by rows, a row block one shifted by 64 rows more: every block reuses the
+      // weight stage, which is released (one group later) when the group holding all blocks' wgmmas has completed
       const uint32_t ahi0 = smem_u32(ahi) + (uint32_t)(wg * (MT / 2) - lo) * 128u, alo0 = smem_u32(alo) + (uint32_t)(wg * (MT / 2) - lo) * 128u;
       for (int t = 0; t < ntaps; ++t, ++it) {
         const int s = it % NW;
         mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
         const uint32_t shift = (uint32_t)P.tap_off[t] * 128u;
-        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
-        const uint32_t ws = smem_u32(smem + S.w[s]);
-#pragma unroll
-        for (int b = 0; b < MB; ++b)
-#pragma unroll
-          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
-        wgmma_fence();
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t ko = (uint64_t)((k * 32) >> 4);
-#pragma unroll
-          for (int b = 0; b < MB; ++b)
-#pragma unroll
-            for (int j = 0; j < NJ; ++j) {
-              const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
-              const uint64_t ab = ko + b * BLK_DESC;
-              wgmma_nb<NB>(acc[b][j], dah + ab, dwh);
-              wgmma_nb<NB>(acc[b][j], dal + ab, dwh);
-              wgmma_nb<NB>(acc[b][j], dah + ab, dwl);
-            }
-        }
-        wgmma_commit();
-        wgmma_wait<1>();
-#pragma unroll
-        for (int b = 0; b < MB; ++b)
-#pragma unroll
-          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
-        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        mma_group(acc, make_desc(ahi0 + shift), make_desc(alo0 + shift), smem_u32(smem + S.w[s]), ksteps, w_empty, prev);
         // plane-fed: chunk c - 1's wgmmas have all completed now, so its operand buffer may be refilled
         if (PL && NA > 1 && t == 0 && c > 0 && lane == 0) mbar_arrive(&a_empty[(c - 1) % NA]);
         prev = s;
       }
       if (NA == 1) {
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(&w_empty[prev]);
+        mma_drain(acc, w_empty, prev);
         if (PL && lane == 0) mbar_arrive(&a_empty[0]);
         prev = -1;
       }
     }
     // =========================== worker warps: epilogue ===========================
-    // registers (x inverse weight scale) -> swizzled staging block [MT rows][32 cols] in shared memory (the operand
-    // buffers are free now) -> coalesced (row, 16-byte chunk) items through the fused epilogue.  The global READS of
-    // items 0..3 (rows 0..127) of a block (residual / old accumulator) are issued one block ahead -- for block 0 before
-    // the accumulator is complete.  A tall tile holds the reads of 4 items too, next to an accumulator as large as a
-    // 128-wide one: it reads block 0 once that block is staged, and item i + 4 (rows 128..255) once item i is stored.
-    EpiPre pre[8];
-    int pp[8];
-    constexpr int nitem = (MT * 8) / NWK;   // 4 items per worker and block (8 on a tall tile)
-    const float dsc = P.tc_descale;
-    auto load_block = [&](int cb) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int idx = xt + i * NWK;
-        pp[i] = (i < 4 && i < nitem) ? rowp[MT == TC_ROWS ? idx >> 3 : item_row(xt, i)] : -1;
-        if (pp[i] >= 0) epi_load(P, g, pp[i], co0 + cb + 4 * (idx & 7), pre[i]);
-      }
-    };
-    if (MT == TC_ROWS) load_block(0);
-    if (dbg_on && tid == 0) { dbg[2] = dbg[1]; dbg[3] = clock64(); dbg[6] = 0; dbg[7] = 0; }   // the workers issue the wgmmas: no waits of a separate issuer
-    wgmma_wait<0>();
-#pragma unroll
-    for (int b = 0; b < MB; ++b)
-#pragma unroll
-      for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
-    named_bar_sync(1, NWK);                      // both warpgroups' wgmmas are done reading the operand buffers
-    if (dbg_on && tid == 0) dbg[4] = clock64();
-    uint8_t* stg0 = smem + S.a_hi[0];            // 2 x MT x 128 B inside the first operand buffers (tc5_plan)
-    const int r0 = wg * (MT / 2) + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-    for (int blk = 0; blk < BN / 32; ++blk) {
-      const int cb = blk * 32;
-      uint8_t* stg = stg0 + (blk & 1) * (MT * 128);
-#pragma unroll
-      for (int b = 0; b < MB; ++b) {
-        const float* a = &acc[b][cb / NB][4 * ((cb % NB) / 8)];
-        const int r = r0 + 64 * b;
-#pragma unroll
-        for (int i8 = 0; i8 < 4; ++i8) {
-          const int col = 8 * i8 + c0;
-          *reinterpret_cast<float2*>(stg + sw128(r, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
-          *reinterpret_cast<float2*>(stg + sw128(r + 8, col >> 2) + (col & 3) * 4) =
-              make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
-        }
-      }
-      if (MT == TC_TALL && blk == 0) load_block(0);
-      named_bar_sync(1, NWK);
-      const int jc = xt & 7;                       // all items of this thread share the 4-channel group
-      const float4 cv = epi_colvec(P, g, co0 + cb + 4 * jc);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int idx = xt + i * NWK;
-        const int row = (idx >> 3) & (MT - 1);   // pp[i] < 0 for i >= nitem (items 4..7 of a tall tile: read below)
-        if (pp[i] >= 0)
-          epi_store_cv<PL>(P, g, pp[i], co0 + cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
-        if (i + 4 < nitem) {
-          const int idx4 = idx + 4 * NWK;
-          pp[i + 4] = rowp[item_row(xt, i + 4)];
-          if (pp[i + 4] >= 0) epi_load(P, g, pp[i + 4], co0 + cb + 4 * (idx4 & 7), pre[i + 4]);
-        }
-      }
-      if (cb + 32 < BN) load_block(cb + 32);
-      // staging halves alternate; a half is rewritten two blocks later, after the next named
-      // barrier, so no extra barrier is needed here
-    }
-    if (dbg_on && tid == 0) dbg[5] = clock64();
+    tile_epilogue<BN, MT, 4, PL>(acc, P, g, co0, rowp, smem, S, wg, xt, dbg_on && tid == 0 ? dbg : nullptr);
   } else if (lane == 0) {
     // =========================== weight producer (warp 8) ===========================
     const uint32_t bytes = 2u * BN * 128u;
@@ -376,10 +484,7 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
     for (int it = 0; it < total; ++it) {
       if constexpr (PL)   // a chunk's operand tile ahead of its first weight stage
         if (it % ntaps == 0) pl_load_chunk(smem, S, tmh, tml, a_full, a_empty, NA, it / ntaps, q0 + lo, gz, RRA);
-      const int s = it % NW, n = it / NW;
-      if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
-      mbar_arrive_expect_tx(&w_full[s], bytes);
-      bulk_g2s(smem + S.w[s], wsrc + (size_t)it * bytes, bytes, &w_full[s]);
+      ring_put(smem, S.w, w_full, w_empty, NW, it, wsrc + (size_t)it * bytes, bytes);
     }
   }
 }
@@ -400,30 +505,25 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcconv5_pl_kernel(const __grid_
 // runs c1 over the MT intermediate rows qa .. qa + MT - 1 (qa = q0 + lowest tap of c2), c1's accumulator becomes c2's
 // operand tile in shared memory, and the tcconv5 pipeline runs c2 over it; a tile keeps the MT - span(c2) outputs
 // that read only those rows.  P1 / P2: the two convs' launch parameters (leaky-ReLU prologue, 1-D rows, one co-tile,
-// BN >= C); P2's epilogue (EPI_RES / EPI_ACC) writes the output.  The weight producer streams c1's stages, then c2's,
-// through one mbarrier ring.
-// PL: c1's input is plane-fed (as tcconv5_body), and c2's epilogue may write the output's plane.
+// BN >= C, fp32 input and output); P2's epilogue (EPI_RES / EPI_ACC) writes the output.  The weight producer streams
+// c1's stages, then c2's, through one mbarrier ring.
 // HALF: c1's input (Cin <= 64: one chunk) is staged in 32-channel halves of 128-byte rows, P1.tc_nr of them in flight
 // (tcpair2_kernel: two CTAs per SM, where 256-byte staging rows would not fit).
-template <int BN, int MT, bool PL, bool HALF = false>
-__device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapConvParams& P2, const CUtensorMap* tmh,
-                                            const CUtensorMap* tml) {
+// c1's chunk loop stays apart from tcconv5_body's: sharing it would make the pair's transform evaluate the PRO_ADDVEC
+// row and channel guards of a general prologue, work the pair does not do today.
+template <int BN, int MT, bool HALF = false>
+__device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapConvParams& P2) {
   constexpr int NB = tc5_nb(BN), NJ = BN / NB, MB = MT / 128;
   static_assert(MT == TC_ROWS || (MT == TC_TALL && BN <= 64), "tall tiles are for narrow BN");
-  static_assert(!HALF || (MT == TC_ROWS && BN <= 64 && !PL), "half staging is for the 128-row transform path");
+  static_assert(!HALF || (MT == TC_ROWS && BN <= 64), "half staging is for 128-row tiles");
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
-  const int RRA = P1.R, NA = P1.tc_na, NW = P1.tc_nw, NR = PL ? 0 : P1.tc_nr;
+  const int RRA = P1.R, NA = P1.tc_na, NW = P1.tc_nw, NR = P1.tc_nr;
   __shared__ Tc5Smem S;
-  if (threadIdx.x == 0) {
-    if constexpr (PL) tc5_layout(S, BN, MT, pl_rows(RRA), NA, NW, 0, true);
-    else tc5_layout(S, BN, MT, RRA, NA, NW, NR, false, HALF ? 128 : 256);
-  }
+  if (threadIdx.x == 0) tc5_layout(S, BN, MT, RRA, NA, NW, NR, false, HALF ? 128 : 256);
   __syncthreads();
   uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
   uint64_t* w_empty = w_full + MAX_NW;
-  uint64_t* a_full = w_full + 2 * MAX_NW;   // [MAX_NA] plane-fed only
-  uint64_t* a_empty = a_full + MAX_NA;
   int* rowinfo = reinterpret_cast<int*>(smem + S.rowinfo);
   int* rowp = reinterpret_cast<int*>(smem + S.rowp);
 
@@ -439,16 +539,13 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
 
   if (tid == 0) {
     for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NWK / 32); }
-    if constexpr (PL)
-      for (int i = 0; i < NA; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], NWK / 32); }
     fence_barrier_init();
   }
   if (is_worker) {
-    if constexpr (!PL)
-      for (int i = xt; i < RRA; i += NWK) {
-        const int r = qa + lo + i;
-        rowinfo[i] = (r >= 0 && r < Lv) ? r * P1.in_pitch : -1;
-      }
+    for (int i = xt; i < RRA; i += NWK) {
+      const int r = qa + lo + i;
+      rowinfo[i] = (r >= 0 && r < Lv) ? r * P1.in_pitch : -1;
+    }
     if (xt < MT) rowp[xt] = (xt < MT - span2 && q0 + xt < Lv) ? q0 + xt : -1;
   }
   __syncthreads();
@@ -456,7 +553,9 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
 
   if (is_worker) {
     const float* __restrict__ ing = P1.in + g * P1.in_gstride;
-    auto issue_raw = [&](int c, int rb) {   // as tcconv5_kernel
+    // issue_raw for c1's input, kept as a copy: with issue_raw called here tcpair_kernel<128, 128> compiles to 8 more
+    // SASS instructions than with this lambda (ptxas, sm_90a)
+    auto issue_raw1 = [&](int c, int rb) {
       uint8_t* dst = smem + S.raw[rb];
       const int kv = min(H_KCH, P1.Cin - c * H_KCH);
       const int nu = ((kv + 15) >> 4) << 2;
@@ -490,9 +589,9 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
     if constexpr (HALF) {
       issue_half(0, 0);
       if (NR == 2) issue_half(1, 1);
-    } else if constexpr (!PL) {
-      issue_raw(0, 0);
-      if (NR == 2 && nchunks > 1) issue_raw(1, 1);
+    } else {
+      issue_raw1(0, 0);
+      if (NR == 2 && nchunks > 1) issue_raw1(1, 1);
     }
     {  // the epilogue's residual / old accumulator rows into L2 while the main loop runs
       const int lines = (BN * 4) / 128 > 0 ? (BN * 4) / 128 : 1;
@@ -507,60 +606,25 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
       }
     }
     float acc[MB][NJ][NB / 2];   // row block b: rows MT/2 wg + 64 b .. + 63 of the tile
-#pragma unroll
-    for (int b = 0; b < MB; ++b)
-#pragma unroll
-      for (int j = 0; j < NJ; ++j)
-#pragma unroll
-        for (int i = 0; i < NB / 2; ++i) acc[b][j][i] = 0.f;
+    zero_tile(acc);
     int it = 0, prev = -1;     // prev: weight stage of the newest wgmma group, released once that group has completed
-    // wgmma over the taps of one conv and one 64-channel chunk of its operand tile (ahi0 / alo0: this warpgroup's rows);
-    // rel >= 0 (plane-fed c1): release that operand buffer once the first tap's group is issued (all older completed)
-    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps, int rel) {
+    // wgmma over the taps of one conv and one 64-channel chunk of its operand tile (ahi0 / alo0: this warpgroup's rows)
+    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {
       for (int t = 0; t < Q.ntaps; ++t, ++it) {
         const int s = it % NW;
         mbar_wait(&w_full[s], (uint32_t)((it / NW) & 1));
         const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
-        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
-        const uint32_t ws = smem_u32(smem + S.w[s]);
-#pragma unroll
-        for (int b = 0; b < MB; ++b)
-#pragma unroll
-          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
-        wgmma_fence();
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t ko = (uint64_t)((k * 32) >> 4);
-#pragma unroll
-          for (int b = 0; b < MB; ++b)
-#pragma unroll
-            for (int j = 0; j < NJ; ++j) {
-              const uint64_t dwh = make_desc(ws + j * NB * 128) + ko, dwl = make_desc(ws + (BN + j * NB) * 128) + ko;
-              const uint64_t ab = ko + b * BLK_DESC;
-              wgmma_nb<NB>(acc[b][j], dah + ab, dwh);
-              wgmma_nb<NB>(acc[b][j], dal + ab, dwh);
-              wgmma_nb<NB>(acc[b][j], dah + ab, dwl);
-            }
-        }
-        wgmma_commit();
-        wgmma_wait<1>();
-#pragma unroll
-        for (int b = 0; b < MB; ++b)
-#pragma unroll
-          for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
-        if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
-        if (PL && t == 0 && rel >= 0 && lane == 0) mbar_arrive(&a_empty[rel]);
+        mma_group(acc, make_desc(ahi0 + shift), make_desc(alo0 + shift), smem_u32(smem + S.w[s]), ksteps, w_empty, prev);
         prev = s;
       }
     };
-    // =========================== c1: transform + wgmma, chunk by chunk (as tcconv5_kernel) ===========================
+    // =========================== c1: transform + wgmma, chunk by chunk ===========================
     for (int c = 0; c < nchunks; ++c) {
       const int buf = c % NA;
       const int rb = (NR == 2) ? (c & 1) : 0;
       const int kv = min(H_KCH, P1.Cin - c * H_KCH);
       const int nq = ((kv + 15) >> 4) << 1;
-      if constexpr (PL) {
-        mbar_wait(&a_full[buf], (uint32_t)((c / NA) & 1));
-      } else if constexpr (!HALF) {
+      if constexpr (!HALF) {
         if (NR == 2 && c + 1 < nchunks) asm volatile("cp.async.wait_group 1;" ::: "memory");
         else cp_async_wait_all_();
         named_bar_sync(1, NWK);
@@ -584,10 +648,7 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
           const float4 x0 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 128 + ((q * 16) ^ sw)), true, nullptr);
           const float4 x1 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 128 + ((64 + q * 16) ^ sw)), true, nullptr);
           uint4 hv, lv;
-          hv.x = split2(x0.x, x0.y, lv.x);
-          hv.y = split2(x0.z, x0.w, lv.y);
-          hv.z = split2(x1.x, x1.y, lv.z);
-          hv.w = split2(x1.z, x1.w, lv.w);
+          split8(x0, x1, hv, lv);
           const uint32_t o = sw128(row, qg);
           *reinterpret_cast<uint4*>(ahi + o) = hv;
           *reinterpret_cast<uint4*>(alo + o) = lv;
@@ -599,7 +660,7 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
       }
       fence_proxy_async();
       named_bar_sync(1, NWK);
-      } else if constexpr (!PL) {
+      } else {
       const uint8_t* rawb = smem + S.raw[rb];
 #pragma unroll 2
       for (int idx = xt; idx < RRA * 8; idx += NWK) {
@@ -608,160 +669,47 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
         const float4 x0 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 256 + q * 16), true, nullptr);
         const float4 x1 = pro_apply5(P1, *reinterpret_cast<const float4*>(rawb + row * 256 + 128 + q * 16), true, nullptr);
         uint4 h, l;
-        h.x = split2(x0.x, x0.y, l.x);
-        h.y = split2(x0.z, x0.w, l.y);
-        h.z = split2(x1.x, x1.y, l.z);
-        h.w = split2(x1.z, x1.w, l.w);
+        split8(x0, x1, h, l);
         const uint32_t o = sw128(row, q);
         *reinterpret_cast<uint4*>(ahi + o) = h;
         *reinterpret_cast<uint4*>(alo + o) = l;
       }
       fence_proxy_async();
       named_bar_sync(1, NWK);
-      if (c + NR < nchunks) issue_raw(c + NR, rb);
+      if (c + NR < nchunks) issue_raw1(c + NR, rb);
       }
       mma_taps(P1, smem_u32(ahi) + (uint32_t)(wg * (MT / 2) - lo) * 128u, smem_u32(alo) + (uint32_t)(wg * (MT / 2) - lo) * 128u,
-               (kv + 15) >> 4, (PL && NA > 1 && c > 0) ? (c - 1) % NA : -1);
+               (kv + 15) >> 4);
       if (NA == 1) {
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(&w_empty[prev]);
-        if (PL && lane == 0) mbar_arrive(&a_empty[0]);
+        mma_drain(acc, w_empty, prev);
         prev = -1;
       }
     }
     // =========================== c1's epilogue -> c2's operand tile ===========================
-    // The arithmetic of c1's EPI_BIAS store followed by c2's PRO_LRELU transform (acc * descale + bias, leaky ReLU,
-    // hi/lo split), so c2 multiplies the operands a separate launch would.  The tile [RR2 rows][C channels] (K-major
-    // SWIZZLE_128B, per 64-channel chunk a hi and a lo block) replaces c1's operand buffers: rows outside the sample are
-    // c2's zero padding, channels >= C are zero, rows >= MT feed only the discarded outputs and are zero.
-    wgmma_wait<0>();
-#pragma unroll
-    for (int b = 0; b < MB; ++b)
-#pragma unroll
-      for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
-    if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+    mma_drain(acc, w_empty, prev);
     prev = -1;
     named_bar_sync(1, NWK);                    // both warpgroups' c1 wgmmas are done reading the operand buffers
-    const int RR2 = P2.R, nch2 = P2.tc_chunks_h, C2 = P2.Cin;
+    const int nch2 = P2.tc_chunks_h;
     uint8_t* a2 = smem + S.a_hi[0];
-    const uint32_t lo_part = (uint32_t)nch2 * RR2 * 128;   // the hi blocks, then the lo blocks
-    const float dsc1 = P1.tc_descale;
+    const uint32_t lo_part = (uint32_t)nch2 * P2.R * 128;
     const int r0 = wg * (MT / 2) + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
-#pragma unroll
-    for (int j = 0; j < NJ; ++j)
-#pragma unroll
-      for (int i = 0; i < NB / 8; ++i) {
-        const int col = j * NB + 8 * i + c0;   // accumulator fragment layout: see wgmma_n16
-        const bool cok = col < C2;
-        float2 bv = make_float2(0.f, 0.f);
-        if (cok && P1.bias) bv = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
-        uint8_t* hi = a2 + (uint32_t)(col >> 6) * RR2 * 128;
-#pragma unroll
-        for (int b = 0; b < MB; ++b)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = r0 + 64 * b + 8 * h;
-            float v0 = 0.f, v1 = 0.f;
-            if (cok && qa + r >= 0 && qa + r < Lv) {
-              v0 = lrelu(__fadd_rn(__fmul_rn(acc[b][j][4 * i + 2 * h], dsc1), bv.x), P2.slope);
-              v1 = lrelu(__fadd_rn(__fmul_rn(acc[b][j][4 * i + 2 * h + 1], dsc1), bv.y), P2.slope);
-            }
-            uint32_t l;
-            const uint32_t hw = split2(v0, v1, l);
-            const uint32_t o = sw128(r, (col & 63) >> 3) + (col & 7) * 2;
-            *reinterpret_cast<uint32_t*>(hi + o) = hw;
-            *reinterpret_cast<uint32_t*>(hi + lo_part + o) = l;
-          }
-      }
-    const int zitems = (RR2 - MT) * 8;         // 16-byte units of rows MT .. RR2 - 1 per block
-    for (int idx = xt; idx < zitems * 2 * nch2; idx += NWK) {
-      const int blk = idx / zitems, u = idx - blk * zitems;
-      *reinterpret_cast<uint4*>(a2 + (uint32_t)blk * RR2 * 128 + MT * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
-    }
-#pragma unroll
-    for (int b = 0; b < MB; ++b)
-#pragma unroll
-      for (int j = 0; j < NJ; ++j)
-#pragma unroll
-        for (int i = 0; i < NB / 2; ++i) acc[b][j][i] = 0.f;
-    fence_proxy_async();
+    pair_handoff<MT>(acc, P1, P2, a2, nch2, P2.R, Lv, r0, c0, qa, xt, NWK);
     named_bar_sync(1, NWK);
     // =========================== c2: wgmma over the resident tile ===========================
     for (int c = 0; c < nch2; ++c) {
-      const uint32_t ahi0 = smem_u32(a2) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * (MT / 2) - P2.lo_al) * 128u;
-      mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, C2 - c * H_KCH) + 15) >> 4, -1);
+      const uint32_t ahi0 = smem_u32(a2) + (uint32_t)c * P2.R * 128 + (uint32_t)(wg * (MT / 2) - P2.lo_al) * 128u;
+      mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, P2.Cin - c * H_KCH) + 15) >> 4);
     }
-    // =========================== c2's epilogue (as tcconv5_kernel) ===========================
-    EpiPre pre[8];
-    int pp[8];
-    constexpr int nitem = (MT * 8) / NWK;
-    // items whose global reads are issued one block ahead; item i + LA is read once item i is stored.  HALF keeps 1 to
-    // stay within the registers of two CTAs per SM.
-    constexpr int LA = HALF ? 1 : 4;
-    const float dsc = P2.tc_descale;
-    auto load_block = [&](int cb) {   // as tcconv5_kernel: items 0..LA-1 one block ahead, the rest during the stores
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int idx = xt + i * NWK;
-        pp[i] = (i < LA && i < nitem) ? rowp[MT == TC_ROWS && !HALF ? idx >> 3 : item_row(xt, i)] : -1;
-        if (pp[i] >= 0) epi_load(P2, g, pp[i], cb + 4 * (idx & 7), pre[i]);
-      }
-    };
-    if (MT == TC_ROWS && !HALF) load_block(0);
-    wgmma_wait<0>();
-#pragma unroll
-    for (int b = 0; b < MB; ++b)
-#pragma unroll
-      for (int j = 0; j < NJ; ++j) fence_acc<NB / 2>(acc[b][j]);
-    named_bar_sync(1, NWK);
-    uint8_t* stg0 = smem + S.a_hi[0];
-#pragma unroll
-    for (int blk = 0; blk < BN / 32; ++blk) {
-      const int cb = blk * 32;
-      uint8_t* stg = stg0 + (blk & 1) * (MT * 128);
-#pragma unroll
-      for (int b = 0; b < MB; ++b) {
-        const float* a = &acc[b][cb / NB][4 * ((cb % NB) / 8)];
-        const int r = r0 + 64 * b;
-#pragma unroll
-        for (int i8 = 0; i8 < 4; ++i8) {
-          const int col = 8 * i8 + c0;
-          *reinterpret_cast<float2*>(stg + sw128(r, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
-          *reinterpret_cast<float2*>(stg + sw128(r + 8, col >> 2) + (col & 3) * 4) =
-              make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
-        }
-      }
-      if ((MT == TC_TALL || HALF) && blk == 0) load_block(0);   // not next to the whole accumulator
-      named_bar_sync(1, NWK);
-      const int jc = xt & 7;
-      const float4 cv = epi_colvec(P2, g, cb + 4 * jc);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int idx = xt + i * NWK;
-        const int row = (idx >> 3) & (MT - 1);
-        if (pp[i] >= 0)
-          epi_store_cv<PL>(P2, g, pp[i], cb + 4 * jc, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre[i], cv);
-        if (i + LA < nitem) {
-          const int idxa = idx + LA * NWK;
-          pp[i + LA] = rowp[item_row(xt, i + LA)];
-          if (pp[i + LA] >= 0) epi_load(P2, g, pp[i + LA], cb + 4 * (idxa & 7), pre[i + LA]);
-        }
-      }
-      if (cb + 32 < BN) load_block(cb + 32);
-    }
+    // =========================== c2's epilogue ===========================
+    tile_epilogue<BN, MT, HALF ? 1 : 4, false>(acc, P2, g, 0, rowp, smem, S, wg, xt, nullptr);
   } else if (lane == 0) {
     // =========================== weight producer (warp 8): c1's stages, then c2's ===========================
     const uint32_t bytes = 2u * BN * 128u;
     const int total2 = P2.tc_chunks_h * P2.ntaps;
     for (int it = 0; it < total + total2; ++it) {
-      if constexpr (PL)   // c1's operand chunks ahead of their first weight stage
-        if (it < total && it % P1.ntaps == 0) pl_load_chunk(smem, S, tmh, tml, a_full, a_empty, NA, it / P1.ntaps, qa + lo, g, RRA);
-      const int s = it % NW, n = it / NW;
-      if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
-      mbar_arrive_expect_tx(&w_full[s], bytes);
       const uint8_t* src = it < total ? reinterpret_cast<const uint8_t*>(P1.w_h) + (size_t)it * bytes
                                       : reinterpret_cast<const uint8_t*>(P2.w_h) + (size_t)(it - total) * bytes;
-      bulk_g2s(smem + S.w[s], src, bytes, &w_full[s]);
+      ring_put(smem, S.w, w_full, w_empty, NW, it, src, bytes);
     }
   }
 }
@@ -769,7 +717,7 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
 template <int BN, int MT>
 __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_constant__ TapConvParams P1,
                                                                const __grid_constant__ TapConvParams P2) {
-  tcpair_body<BN, MT, false>(P1, P2, nullptr, nullptr);
+  tcpair_body<BN, MT>(P1, P2);
 }
 // The same 128-row pair tile with two CTAs per SM (tcpair_plan_dual): one tile's input load, transform, c1 -> c2
 // hand-off and epilogue run beside the other tile's wgmmas.  Needs <= 112 registers per thread and <= kDualDyn bytes
@@ -777,14 +725,7 @@ __global__ void __launch_bounds__(V5_THREADS, 1) tcpair_kernel(const __grid_cons
 template <int BN>
 __global__ void __launch_bounds__(V5_THREADS, 2) tcpair2_kernel(const __grid_constant__ TapConvParams P1,
                                                                 const __grid_constant__ TapConvParams P2) {
-  tcpair_body<BN, TC_ROWS, false, true>(P1, P2, nullptr, nullptr);
-}
-template <int BN, int MT>
-__global__ void __launch_bounds__(V5_THREADS, 1) tcpair_pl_kernel(const __grid_constant__ TapConvParams P1,
-                                                                 const __grid_constant__ TapConvParams P2,
-                                                                 const __grid_constant__ CUtensorMap tmh,
-                                                                 const __grid_constant__ CUtensorMap tml) {
-  tcpair_body<BN, MT, true>(P1, P2, &tmh, &tml);
+  tcpair_body<BN, TC_ROWS, true>(P1, P2);
 }
 
 // ---- C = 128 fused pairs with two tiles in flight per CTA (tcpair_pipe_kernel) ----
@@ -868,9 +809,10 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
   if (wg < 2) {
     // =========================== wgmma warpgroups: rows 64 wg .. 64 wg + 63 of each tile ===========================
     setmaxnreg_inc<168>();
-    float acc[BN / 2];
+    float acc[1][1][BN / 2];
     int it = 0, prev = -1;   // prev: weight stage of the newest wgmma group, released once that group has completed
-    // as tcpair_body over one 64-channel chunk (4 k-steps), the k-steps of a tap in two half-stages
+    // one 64-channel chunk (4 k-steps) in tcpair_body's product order, the k-steps of a tap in two SWIZZLE_64B
+    // half-stages: a copy of mma_group's loop for that weight layout
     auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0) {
       for (int t = 0; t < Q.ntaps; ++t)
         for (int hf = 0; hf < 2; ++hf, ++it) {
@@ -879,28 +821,22 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
           const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
           const uint64_t dah = make_desc(ahi0 + shift) + 4 * hf, dal = make_desc(alo0 + shift) + 4 * hf;
           const uint32_t ws = smem_u32(smem + S.w[s]);
-          fence_acc<BN / 2>(acc);
+          fence_tile(acc);
           wgmma_fence();
 #pragma unroll
           for (int k = 0; k < 2; ++k) {
             const uint64_t ko = (uint64_t)((k * 32) >> 4);
             const uint64_t dwh = make_desc64(ws) + ko, dwl = make_desc64(ws + BN * 64) + ko;
-            wgmma_n128(acc, dah + ko, dwh);
-            wgmma_n128(acc, dal + ko, dwh);
-            wgmma_n128(acc, dah + ko, dwl);
+            wgmma_n128(acc[0][0], dah + ko, dwh);
+            wgmma_n128(acc[0][0], dal + ko, dwh);
+            wgmma_n128(acc[0][0], dah + ko, dwl);
           }
           wgmma_commit();
           wgmma_wait<1>();
-          fence_acc<BN / 2>(acc);
+          fence_tile(acc);
           if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
           prev = s;
         }
-    };
-    auto drain = [&]() {   // all wgmmas completed, the last weight stage released
-      wgmma_wait<0>();
-      fence_acc<BN / 2>(acc);
-      if (prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
-      prev = -1;
     };
     const int r0 = wg * (MT / 2) + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
     for (int k = 0; k < nloc; ++k) {
@@ -908,71 +844,30 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
       tile_of(k, g, q0);
       const int qa = q0 + P2.lo_al;
       uint8_t* set = smem + S.set[k & 1];
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      zero_tile(acc);
       mbar_wait(&in_full[k & 1], (uint32_t)((k >> 1) & 1));
       // c1 over both resident chunks of the input
       for (int c = 0; c < nch; ++c) {
         const uint32_t ahi0 = smem_u32(set) + (uint32_t)c * R1 * 128 + (uint32_t)(wg * (MT / 2) - lo) * 128u;
         mma_taps(P1, ahi0, ahi0 + (uint32_t)nch * R1 * 128);
       }
-      drain();
+      mma_drain(acc, w_empty, prev);
+      prev = -1;
       named_bar_sync(1, PIPE_MMA);             // both warpgroups' c1 wgmmas are done reading the set
-      // c1's epilogue -> c2's operand tile, as tcpair_body
-      const uint32_t lo_part = (uint32_t)nch2 * RR2 * 128;
-      const float dsc1 = P1.tc_descale;
-#pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int col = 8 * i + c0;
-        const bool cok = col < P2.Cin;
-        float2 bv = make_float2(0.f, 0.f);
-        if (cok && P1.bias) bv = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
-        uint8_t* hi = set + (uint32_t)(col >> 6) * RR2 * 128;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = r0 + 8 * h;
-          float v0 = 0.f, v1 = 0.f;
-          if (cok && qa + r >= 0 && qa + r < Lv) {
-            v0 = lrelu(__fadd_rn(__fmul_rn(acc[4 * i + 2 * h], dsc1), bv.x), P2.slope);
-            v1 = lrelu(__fadd_rn(__fmul_rn(acc[4 * i + 2 * h + 1], dsc1), bv.y), P2.slope);
-          }
-          uint32_t l;
-          const uint32_t hw = split2(v0, v1, l);
-          const uint32_t o = sw128(r, (col & 63) >> 3) + (col & 7) * 2;
-          *reinterpret_cast<uint32_t*>(hi + o) = hw;
-          *reinterpret_cast<uint32_t*>(hi + lo_part + o) = l;
-        }
-      }
-      const int zitems = (RR2 - MT) * 8;
-      for (int idx = tid; idx < zitems * 2 * nch2; idx += PIPE_MMA) {
-        const int blk = idx / zitems, u = idx - blk * zitems;
-        *reinterpret_cast<uint4*>(set + (uint32_t)blk * RR2 * 128 + MT * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
-      }
-#pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      fence_proxy_async();
+      pair_handoff<MT>(acc, P1, P2, set, nch2, RR2, Lv, r0, c0, qa, tid, PIPE_MMA);
       named_bar_sync(1, PIPE_MMA);
       // c2 over the resident tile
+      const uint32_t lo_part = (uint32_t)nch2 * RR2 * 128;
       for (int c = 0; c < nch2; ++c) {
         const uint32_t ahi0 = smem_u32(set) + (uint32_t)c * RR2 * 128 + (uint32_t)(wg * (MT / 2) - P2.lo_al) * 128u;
         mma_taps(P2, ahi0, ahi0 + lo_part);
       }
-      drain();
+      mma_drain(acc, w_empty, prev);
+      prev = -1;
       named_bar_sync(1, PIPE_MMA);             // both warpgroups' c2 wgmmas are done reading the set
-      // accumulator x descale -> the set's dump, in tcpair_body's staging layout (one [128][32] block per 32 columns)
-      const float dsc = P2.tc_descale;
+      // accumulator x descale -> the set's dump: one [128][32] staging block per 32 columns
 #pragma unroll
-      for (int blk = 0; blk < BN / 32; ++blk) {
-        uint8_t* stg = set + blk * (MT * 128);
-        const float* a = &acc[4 * (blk * 32 / 8)];
-#pragma unroll
-        for (int i8 = 0; i8 < 4; ++i8) {
-          const int col = 8 * i8 + c0;
-          *reinterpret_cast<float2*>(stg + sw128(r0, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
-          *reinterpret_cast<float2*>(stg + sw128(r0 + 8, col >> 2) + (col & 3) * 4) =
-              make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
-        }
-      }
+      for (int blk = 0; blk < BN / 32; ++blk) stage_block(acc, set + blk * (MT * 128), blk * 32, r0, c0, P2.tc_descale);
       mbar_arrive(&acc_full[k & 1]);
     }
   } else if (wg == 2) {
@@ -997,10 +892,7 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
         }
         const float4 x0 = pro_apply5(P1, v0, true, nullptr), x1 = pro_apply5(P1, v1, true, nullptr);
         uint4 h, l;
-        h.x = split2(x0.x, x0.y, l.x);
-        h.y = split2(x0.z, x0.w, l.y);
-        h.z = split2(x1.x, x1.y, l.z);
-        h.w = split2(x1.z, x1.w, l.w);
+        split8(x0, x1, h, l);
         const uint32_t o = (uint32_t)c * R1 * 128 + sw128(row, q);
         *reinterpret_cast<uint4*>(set + o) = h;
         *reinterpret_cast<uint4*>(set + (uint32_t)nch * R1 * 128 + o) = l;
@@ -1008,7 +900,7 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
       fence_proxy_async();                  // generic-proxy stores -> visible to the wgmma operand reads
       mbar_arrive(&in_full[k & 1]);
     };
-    auto epilogue = [&](int k) {   // the set's dump through c2's fused epilogue, as tcpair_body
+    auto epilogue = [&](int k) {   // the set's dump through c2's fused epilogue (epi_store_cv)
       int g, q0;
       tile_of(k, g, q0);
       const uint8_t* set = smem + S.set[k & 1];
@@ -1049,12 +941,9 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
     int n_it = 0;
     for (int k = 0; k < nloc; ++k)
       for (int it = 0; it < total1 + total2; ++it, ++n_it) {
-        const int s = n_it % NW, n = n_it / NW;
-        if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
-        mbar_arrive_expect_tx(&w_full[s], PIPE_STAGE);
         const uint8_t* src = it < total1 ? reinterpret_cast<const uint8_t*>(P1.w_hk) + (size_t)it * PIPE_STAGE
                                          : reinterpret_cast<const uint8_t*>(P2.w_hk) + (size_t)(it - total1) * PIPE_STAGE;
-        bulk_g2s(smem + S.w[s], src, PIPE_STAGE, &w_full[s]);
+        ring_put(smem, S.w, w_full, w_empty, NW, n_it, src, PIPE_STAGE);
       }
   }
 }
@@ -1140,45 +1029,19 @@ __global__ void __launch_bounds__(NARROW_THREADS, 1) tcpair_narrow_kernel(const 
 
   if (wg < 2) {
     // ====================== wgmma warpgroups: warpgroup wg runs the whole of tiles wg, wg + 2, .. ======================
-    // rows 64 b .. 64 b + 63 of the tile in accumulator b, every row block's products in tcpair_body's order
+    // rows 64 b .. 64 b + 63 of the tile in accumulator b
     setmaxnreg_inc<NARROW_MMA_REGS>();
-    float acc[2][BN / 2];
+    float acc[2][1][BN / 2];
     int it = 0, prev = -1;   // prev: weight stage of the newest wgmma group, released once that group has completed
-    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {   // as tcpair_body, MB = 2
+    auto mma_taps = [&](const TapConvParams& Q, uint32_t ahi0, uint32_t alo0, int ksteps) {
       for (int t = 0; t < Q.ntaps; ++t, ++it) {
         const int s = it % NW;
         mbar_wait(&w_full[s], wres ? 0u : (uint32_t)((it / NW) & 1));
         const uint32_t shift = (uint32_t)Q.tap_off[t] * 128u;
-        const uint64_t dah = make_desc(ahi0 + shift), dal = make_desc(alo0 + shift);
-        const uint32_t ws = smem_u32(smem + S.w[s]);
-        fence_acc<BN / 2>(acc[0]);
-        fence_acc<BN / 2>(acc[1]);
-        wgmma_fence();
-        for (int k = 0; k < ksteps; ++k) {
-          const uint64_t ko = (uint64_t)((k * 32) >> 4);
-          const uint64_t dwh = make_desc(ws) + ko, dwl = make_desc(ws + BN * 128) + ko;
-#pragma unroll
-          for (int b = 0; b < 2; ++b) {
-            const uint64_t ab = ko + b * BLK_DESC;
-            wgmma_nb<NB>(acc[b], dah + ab, dwh);
-            wgmma_nb<NB>(acc[b], dal + ab, dwh);
-            wgmma_nb<NB>(acc[b], dah + ab, dwl);
-          }
-        }
-        wgmma_commit();
-        wgmma_wait<1>();
-        fence_acc<BN / 2>(acc[0]);
-        fence_acc<BN / 2>(acc[1]);
-        if (!wres && prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
+        mma_group(acc, make_desc(ahi0 + shift), make_desc(alo0 + shift), smem_u32(smem + S.w[s]), ksteps,
+                  w_empty, wres ? -1 : prev);
         prev = s;
       }
-    };
-    auto drain = [&]() {
-      wgmma_wait<0>();
-      fence_acc<BN / 2>(acc[0]);
-      fence_acc<BN / 2>(acc[1]);
-      if (!wres && prev >= 0 && lane == 0) mbar_arrive(&w_empty[prev]);
-      prev = -1;
     };
     const int bar = 1 + wg, wt = tid - wg * NARROW_WG;   // this warpgroup's named barrier and thread index
     const int r0 = (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
@@ -1189,77 +1052,27 @@ __global__ void __launch_bounds__(NARROW_THREADS, 1) tcpair_narrow_kernel(const 
       tile_of(k, g, q0);
       const int qa = q0 + P2.lo_al, s = k % NS;
       uint8_t* set = smem + S.op[s];
-#pragma unroll
-      for (int b = 0; b < 2; ++b)
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[b][i] = 0.f;
+      zero_tile(acc);
       mbar_wait(&in_full[s], (uint32_t)((k / NS) & 1));
       {
         const uint32_t ahi0 = smem_u32(set) + (uint32_t)(-lo) * 128u;
         mma_taps(P1, ahi0, ahi0 + (uint32_t)R1 * 128, (P1.Cin + 15) >> 4);
       }
-      drain();
+      mma_drain(acc, w_empty, wres ? -1 : prev);
+      prev = -1;
       named_bar_sync(bar, NARROW_WG);          // all of the warpgroup's c1 wgmmas are done reading the set
-      // c1's epilogue -> c2's operand tile, as tcpair_body
-      const float dsc1 = P1.tc_descale;
-#pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int col = 8 * i + c0;
-        const bool cok = col < P2.Cin;
-        float2 bv = make_float2(0.f, 0.f);
-        if (cok && P1.bias) bv = __ldg(reinterpret_cast<const float2*>(P1.bias + col));
-#pragma unroll
-        for (int b = 0; b < 2; ++b)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = r0 + 64 * b + 8 * h;
-            float v0 = 0.f, v1 = 0.f;
-            if (cok && qa + r >= 0 && qa + r < Lv) {
-              v0 = lrelu(__fadd_rn(__fmul_rn(acc[b][4 * i + 2 * h], dsc1), bv.x), P2.slope);
-              v1 = lrelu(__fadd_rn(__fmul_rn(acc[b][4 * i + 2 * h + 1], dsc1), bv.y), P2.slope);
-            }
-            uint32_t l;
-            const uint32_t hw = split2(v0, v1, l);
-            const uint32_t o = sw128(r, col >> 3) + (col & 7) * 2;
-            *reinterpret_cast<uint32_t*>(set + o) = hw;
-            *reinterpret_cast<uint32_t*>(set + lo_part + o) = l;
-          }
-      }
-      const int zitems = (RR2 - MT) * 8;
-      for (int idx = wt; idx < zitems * 2; idx += NARROW_WG) {
-        const int blk = idx / zitems, u = idx - blk * zitems;
-        *reinterpret_cast<uint4*>(set + (uint32_t)blk * lo_part + MT * 128 + u * 16) = make_uint4(0u, 0u, 0u, 0u);
-      }
-#pragma unroll
-      for (int b = 0; b < 2; ++b)
-#pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[b][i] = 0.f;
-      fence_proxy_async();
+      pair_handoff<MT>(acc, P1, P2, set, 1, RR2, Lv, r0, c0, qa, wt, NARROW_WG);
       named_bar_sync(bar, NARROW_WG);
       {
         const uint32_t ahi0 = smem_u32(set) + (uint32_t)(-P2.lo_al) * 128u;
         mma_taps(P2, ahi0, ahi0 + lo_part, (P2.Cin + 15) >> 4);
       }
-      drain();
+      mma_drain(acc, w_empty, wres ? -1 : prev);
+      prev = -1;
       named_bar_sync(bar, NARROW_WG);          // all of the warpgroup's c2 wgmmas are done reading the set
-      // accumulator x descale -> the set's dump, in tcpair_body's staging layout (one [128][32] block per 32 columns)
-      const float dsc = P2.tc_descale;
+      // accumulator x descale -> the set's dump: one [128][32] staging block per 32 columns
 #pragma unroll
-      for (int blk = 0; blk < BN / 32; ++blk) {
-        uint8_t* stg = set + blk * (MT * 128);
-#pragma unroll
-        for (int b = 0; b < 2; ++b) {
-          const float* a = &acc[b][4 * (blk * 32 / 8)];
-          const int r = r0 + 64 * b;
-#pragma unroll
-          for (int i8 = 0; i8 < 4; ++i8) {
-            const int col = 8 * i8 + c0;
-            *reinterpret_cast<float2*>(stg + sw128(r, col >> 2) + (col & 3) * 4) = make_float2(a[4 * i8] * dsc, a[4 * i8 + 1] * dsc);
-            *reinterpret_cast<float2*>(stg + sw128(r + 8, col >> 2) + (col & 3) * 4) =
-                make_float2(a[4 * i8 + 2] * dsc, a[4 * i8 + 3] * dsc);
-          }
-        }
-      }
+      for (int blk = 0; blk < BN / 32; ++blk) stage_block(acc, set + blk * (MT * 128), blk * 32, r0, c0, P2.tc_descale);
       mbar_arrive(&acc_full[s]);
     }
     // The weight ring is shared: the producer streams one pass per pair of tiles and a stage is refilled once both
@@ -1290,10 +1103,7 @@ __global__ void __launch_bounds__(NARROW_THREADS, 1) tcpair_narrow_kernel(const 
         const float4 x0 = pro_apply5(P1, *reinterpret_cast<const float4*>(rr + ((j0 ^ sw) << 4)), true, nullptr);
         const float4 x1 = pro_apply5(P1, *reinterpret_cast<const float4*>(rr + (((j0 + 1) ^ sw) << 4)), true, nullptr);
         uint4 h, l;
-        h.x = split2(x0.x, x0.y, l.x);
-        h.y = split2(x0.z, x0.w, l.y);
-        h.z = split2(x1.x, x1.y, l.z);
-        h.w = split2(x1.z, x1.w, l.w);
+        split8(x0, x1, h, l);
         const uint32_t o = sw128(row, q);
         *reinterpret_cast<uint4*>(set + o) = h;
         *reinterpret_cast<uint4*>(set + (uint32_t)R1 * 128 + o) = l;
@@ -1373,12 +1183,7 @@ __global__ void __launch_bounds__(NARROW_THREADS, 1) tcpair_narrow_kernel(const 
       } else {
         int n_it = 0;
         for (int j = 0; j < (nloc + 1) / 2; ++j)   // one pass per pair of tiles, read by both wgmma warpgroups
-          for (int it = 0; it < iters; ++it, ++n_it) {
-            const int s = n_it % NW, n = n_it / NW;
-            if (n >= 1) mbar_wait(&w_empty[s], (uint32_t)((n - 1) & 1));
-            mbar_arrive_expect_tx(&w_full[s], bytes);
-            bulk_g2s(smem + S.w[s], src(it), bytes, &w_full[s]);
-          }
+          for (int it = 0; it < iters; ++it, ++n_it) ring_put(smem, S.w, w_full, w_empty, NW, n_it, src(it), bytes);
       }
     }
   }
@@ -1611,10 +1416,7 @@ __global__ void __launch_bounds__(CPIPE_THREADS, 1) tcconv_pipe_pl_kernel(const 
             tma_load_3d(smem + S.a[buf] + (PR + bx * br) * 128, &tml, c * H_KCH, q0 + lo + bx * br, g, &a_full[buf]);
           }
         }
-        const int it = k * total + i, s = it % NW, m = it / NW;
-        if (m >= 1) mbar_wait(&w_empty[s], (uint32_t)((m - 1) & 1));
-        mbar_arrive_expect_tx(&w_full[s], bytes);
-        bulk_g2s(smem + S.w[s], wsrc + (size_t)i * bytes, bytes, &w_full[s]);
+        ring_put(smem, S.w, w_full, w_empty, NW, k * total + i, wsrc + (size_t)i * bytes, bytes);
       }
     }
   }
@@ -1791,38 +1593,38 @@ static bool tcpair_plan_dual(TapConvParams& P, int BN, long a_min, int iters, si
   return false;
 }
 
-static void tc5_set_smem_limits() {
+// Dynamic shared-memory limit of a tap-GEMM kernel, set once per kernel and device: kMaxDyn, or for tcpair2_kernel
+// (dual) kDualDyn with the max-shared carveout, so that two CTAs fit an SM.  Occupancy queries depend on it too.
+static void tc_func_attrs(const void* kern, bool dual) {
   int dev = 0;
   AGPT_CUDA(cudaGetDevice(&dev));
-  static bool attr_done_dev[64] = {false};
-  if (attr_done_dev[dev & 63]) return;
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<96, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<96, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcconv5_pl_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<128, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<64, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<32, TC_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<64, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair_pl_kernel<32, TC_TALL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDualDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDualDyn));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<64>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  AGPT_CUDA(cudaFuncSetAttribute(tcpair2_kernel<32>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  attr_done_dev[dev & 63] = true;
+  static std::set<std::pair<const void*, int>> done;
+  if (done.count({kern, dev})) return;
+  AGPT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, dual ? kDualDyn : kMaxDyn));
+  if (dual) AGPT_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  done.insert({kern, dev});
+}
+template <typename... KArgs, typename... Args>
+static void tc_launch(void (*kern)(KArgs...), bool dual, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  tc_func_attrs(reinterpret_cast<const void*>(kern), dual);
+  launch_pdl(kern, grid, block, smem, st, std::forward<Args>(args)...);
+}
+
+// the instantiation of each tile-kernel family for a BN-column, MT-row tile (BN <= 64 for MT = TC_TALL)
+static auto tcconv5_kern(int BN, int MT) {
+  if (MT == TC_TALL) return BN == 64 ? tcconv5_kernel<64, TC_TALL> : tcconv5_kernel<32, TC_TALL>;
+  return BN == 128 ? tcconv5_kernel<128, TC_ROWS>
+                   : BN == 96 ? tcconv5_kernel<96, TC_ROWS> : BN == 64 ? tcconv5_kernel<64, TC_ROWS> : tcconv5_kernel<32, TC_ROWS>;
+}
+static auto tcconv5_pl_kern(int BN, int MT) {
+  if (MT == TC_TALL) return BN == 64 ? tcconv5_pl_kernel<64, TC_TALL> : tcconv5_pl_kernel<32, TC_TALL>;
+  return BN == 128 ? tcconv5_pl_kernel<128, TC_ROWS>
+                   : BN == 96 ? tcconv5_pl_kernel<96, TC_ROWS>
+                              : BN == 64 ? tcconv5_pl_kernel<64, TC_ROWS> : tcconv5_pl_kernel<32, TC_ROWS>;
+}
+static auto tcpair_kern(int BN, int MT) {
+  if (MT == TC_TALL) return BN == 64 ? tcpair_kernel<64, TC_TALL> : tcpair_kernel<32, TC_TALL>;
+  return BN == 128 ? tcpair_kernel<128, TC_ROWS> : BN == 64 ? tcpair_kernel<64, TC_ROWS> : tcpair_kernel<32, TC_ROWS>;
 }
 
 static int tc5_sms() {
@@ -1860,29 +1662,15 @@ static bool tcconv5_try(TapConvParams P, int BN, int MT, cudaStream_t st) {
   if (!tc5_plan(P, BN, MT, 0, P.tc_chunks_h * P.ntaps, smem)) return false;
   const int Lv = tc_lv(P);
   dim3 grid(cdiv(Lv, MT), cdiv(P.Cout, BN), tc_groups(P));
-  tc5_set_smem_limits();
   tapconv_note_launch(1, BN, MT, P.pi_hi ? 1 : 0);
   if (P.pi_hi) {
     const PlMaps m = pl_tensor_maps(P);
-    if (MT == TC_TALL) {
-      if (BN == 64) launch_pdl(tcconv5_pl_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
-      else launch_pdl(tcconv5_pl_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
-      profile_count_tall();
-    } else if (BN == 128) launch_pdl(tcconv5_pl_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
-    else if (BN == 96) launch_pdl(tcconv5_pl_kernel<96, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
-    else if (BN == 64) launch_pdl(tcconv5_pl_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
-    else launch_pdl(tcconv5_pl_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
-    profile_count_plane();
-    return true;
+    tc_launch(tcconv5_pl_kern(BN, MT), false, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
+  } else {
+    tc_launch(tcconv5_kern(BN, MT), false, grid, dim3(V5_THREADS), smem, st, P);
   }
-  if (MT == TC_TALL) {
-    if (BN == 64) launch_pdl(tcconv5_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P);
-    else launch_pdl(tcconv5_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P);
-    profile_count_tall();
-  } else if (BN == 128) launch_pdl(tcconv5_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
-  else if (BN == 96) launch_pdl(tcconv5_kernel<96, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
-  else if (BN == 64) launch_pdl(tcconv5_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
-  else launch_pdl(tcconv5_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P);
+  if (MT == TC_TALL) profile_count_tall();
+  if (P.pi_hi) profile_count_plane();
   return true;
 }
 
@@ -1923,36 +1711,22 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, bool dual, cu
   const int iters = P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps;
   if (dual ? !tcpair_plan_dual(P1, BN, a2bytes, iters, smem) : !tc5_plan(P1, BN, MT, a2bytes, iters, smem)) return false;
   dim3 grid(cdiv(tc_lv(P1), MT - span2), 1, tc_groups(P1));
-  tc5_set_smem_limits();
+  const auto dual_kern = BN == 64 ? tcpair2_kernel<64> : tcpair2_kernel<32>;
   if (dual) {
+    tc_func_attrs(reinterpret_cast<const void*>(dual_kern), true);
     int per_sm = 0;
-    AGPT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(
-        &per_sm, BN == 64 ? tcpair2_kernel<64> : tcpair2_kernel<32>, V5_THREADS, smem));
+    AGPT_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dual_kern, V5_THREADS, smem));
     if (per_sm != 2) return false;
   }
   void* rec = profile_begin_pair(P1, P2, st);
-  tapconv_note_launch(1, BN, MT, P1.pi_hi ? 1 : 0);
+  tapconv_note_launch(1, BN, MT, 0);
   if (dual) {
-    if (BN == 64) launch_pdl(tcpair2_kernel<64>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-    else launch_pdl(tcpair2_kernel<32>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+    tc_launch(dual_kern, true, grid, dim3(V5_THREADS), smem, st, P1, P2);
     profile_count_dual();
-  } else if (P1.pi_hi) {
-    const PlMaps m = pl_tensor_maps(P1);
-    if (MT == TC_TALL) {
-      if (BN == 64) launch_pdl(tcpair_pl_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
-      else launch_pdl(tcpair_pl_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
-      profile_count_tall();
-    } else if (BN == 128) launch_pdl(tcpair_pl_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
-    else if (BN == 64) launch_pdl(tcpair_pl_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
-    else launch_pdl(tcpair_pl_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2, m.hi, m.lo);
-    profile_count_plane();
-  } else if (MT == TC_TALL) {
-    if (BN == 64) launch_pdl(tcpair_kernel<64, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-    else launch_pdl(tcpair_kernel<32, TC_TALL>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-    profile_count_tall();
-  } else if (BN == 128) launch_pdl(tcpair_kernel<128, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-  else if (BN == 64) launch_pdl(tcpair_kernel<64, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2);
-  else launch_pdl(tcpair_kernel<32, TC_ROWS>, grid, dim3(V5_THREADS), smem, st, P1, P2);
+  } else {
+    tc_launch(tcpair_kern(BN, MT), false, grid, dim3(V5_THREADS), smem, st, P1, P2);
+    if (MT == TC_TALL) profile_count_tall();
+  }
   profile_end(rec, st);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
@@ -1965,8 +1739,7 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, bool dual, cu
 // with half-stage images, or the sets and four half-stages do not fit (c1 with a tap span of about 30 rows or more:
 // k = 11 at dilation 5).
 static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
-  if (!P1.tc_pipe || P1.tc_bn != 128 || P1.Cin != 128 || P1.Cout != 128 || P2.Cout != 128 || P1.pi_hi || P2.po_hi ||
-      !P1.w_hk || !P2.w_hk)
+  if (!P1.tc_pipe || P1.tc_bn != 128 || P1.Cin != 128 || P1.Cout != 128 || P2.Cout != 128 || !P1.w_hk || !P2.w_hk)
     return false;
   tc5_rows(P1, TC_ROWS);
   const int span2 = tc5_rows(P2, TC_ROWS);
@@ -1983,16 +1756,9 @@ static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st)
   const size_t smem = (size_t)S.total + 1024;
   const long tiles = (long)cdiv(P1.L, TC_ROWS - span2) * P1.G;
   dim3 grid((unsigned)std::min<long>(tiles, tc5_sms()));
-  int dev = 0;
-  AGPT_CUDA(cudaGetDevice(&dev));
-  static bool attr_done_dev[64] = {false};
-  if (!attr_done_dev[dev & 63]) {
-    AGPT_CUDA(cudaFuncSetAttribute(tcpair_pipe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    attr_done_dev[dev & 63] = true;
-  }
   void* rec = profile_begin_pair(P1, P2, st);
   tapconv_note_launch(1, 128, TC_ROWS, 0);
-  launch_pdl(tcpair_pipe_kernel, grid, dim3(PIPE_THREADS), smem, st, P1, P2);
+  tc_launch(tcpair_pipe_kernel, false, grid, dim3(PIPE_THREADS), smem, st, P1, P2);
   profile_count_pipe();
   profile_end(rec, st);
   count_launch(1);
@@ -2001,9 +1767,9 @@ static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st)
 }
 
 // Two 128-row CTAs per SM (tcpair2_kernel) instead of one 256- or 128-row CTA: the handle allows it
-// (TapConvParams::tc_dual), the pair is narrow (BN <= 64: one 64-channel chunk) and converts its fp32 input.
+// (TapConvParams::tc_dual) and the pair is narrow (BN <= 64: one 64-channel chunk).
 static bool tcpair_dual(const TapConvParams& P1) {
-  return P1.tc_dual && P1.tc_bn <= 64 && !P1.pi_hi;
+  return P1.tc_dual && P1.tc_bn <= 64;
 }
 
 // One launch of tcpair_narrow_kernel for a pair that tcpair_dual allows: min(tiles, SMs) CTAs.  Shared-memory plan:
@@ -2017,7 +1783,7 @@ static bool tcpair_dual(const TapConvParams& P1) {
 // residual rows do not lie inside c1's operand rows, or the plan does not fit.
 static bool tcpair_narrow_try(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   const int BN = P1.tc_bn, iters = P1.ntaps + P2.ntaps;   // weight stages per tile: one 64-channel chunk per conv
-  if (!P1.tc_narrow_pipe || (BN != 64 && BN != 32) || (BN == 64 && iters > 14) || P1.Cin > BN || P2.po_hi ||
+  if (!P1.tc_narrow_pipe || (BN != 64 && BN != 32) || (BN == 64 && iters > 14) || P1.Cin > BN ||
       P2.res != P1.in || P2.res_pitch != P1.in_pitch || P2.res_gstride != P1.in_gstride)
     return false;
   const int span1 = tc5_rows(P1, TC_ROWS);
@@ -2046,18 +1812,10 @@ static bool tcpair_narrow_try(TapConvParams P1, TapConvParams P2, cudaStream_t s
   const size_t smem = (size_t)S.total + 1024;
   const long tiles = (long)cdiv(P1.L, TC_ROWS - span2) * P1.G;
   dim3 grid((unsigned)std::min<long>(tiles, tc5_sms()));
-  int dev = 0;
-  AGPT_CUDA(cudaGetDevice(&dev));
-  static bool attr_done_dev[64] = {false};
-  if (!attr_done_dev[dev & 63]) {
-    AGPT_CUDA(cudaFuncSetAttribute(tcpair_narrow_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    AGPT_CUDA(cudaFuncSetAttribute(tcpair_narrow_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    attr_done_dev[dev & 63] = true;
-  }
   void* rec = profile_begin_pair(P1, P2, st);
   tapconv_note_launch(1, BN, TC_ROWS, 0);
-  if (BN == 64) launch_pdl(tcpair_narrow_kernel<64>, grid, dim3(NARROW_THREADS), smem, st, P1, P2, tmx);
-  else launch_pdl(tcpair_narrow_kernel<32>, grid, dim3(NARROW_THREADS), smem, st, P1, P2, tmx);
+  tc_launch(BN == 64 ? tcpair_narrow_kernel<64> : tcpair_narrow_kernel<32>, false, grid, dim3(NARROW_THREADS), smem, st, P1,
+            P2, tmx);
   profile_count_dual();
   profile_count_narrow_pipe();
   profile_end(rec, st);
@@ -2072,10 +1830,12 @@ static bool tcpair_narrow_try(TapConvParams P1, TapConvParams P2, cudaStream_t s
 // two 128-row tiles in flight per CTA where tcpair_pipe_try takes the pair (128 -> 128 channels); where tcpair_dual
 // allows it, the narrow pipeline (tcpair_narrow_try), else two 128-row CTAs per SM where that plan fits; else MT = 256
 // where tc5_tall allows it, else 128.
-// Returns false -- nothing launched -- when the pair needs more than one co-tile or does not fit shared memory.
+// Returns false -- nothing launched -- when the pair needs more than one co-tile, reads or writes an operand plane
+// (TapConvParams::pi_hi / po_hi: the fused kernels convert fp32 and store fp32 only), or does not fit shared memory.
 bool tcpair_launch(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (!tcconv_supported(P1) || !P2.w_h) return false;
   const int BN = P1.tc_bn;
+  if (P1.pi_hi || P2.po_hi) return false;
   if (P2.tc_bn != BN || P1.Cout > BN || P2.Cin != P1.Cout || P2.Cout > BN || P1.Wreal || P2.Wreal || P1.strips ||
       P1.G != P2.G || P1.L != P2.L || P1.pro != PRO_LRELU || P2.pro != PRO_LRELU || (P2.epi != EPI_RES && P2.epi != EPI_ACC))
     return false;
@@ -2115,15 +1875,8 @@ static bool tcconv_pipe_try(TapConvParams P, const HTile& c, cudaStream_t st) {
   const size_t smem = (size_t)S.total + 1024;
   const int units = cdiv(P.L, TC_ROWS) * P.G * cdiv(P.Cout, 128);
   const PlMaps m = pl_tensor_maps(P);
-  int dev = 0;
-  AGPT_CUDA(cudaGetDevice(&dev));
-  static bool attr_done_dev[64] = {false};
-  if (!attr_done_dev[dev & 63]) {
-    AGPT_CUDA(cudaFuncSetAttribute(tcconv_pipe_pl_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDyn));
-    attr_done_dev[dev & 63] = true;
-  }
   tapconv_note_launch(1, 128, TC_ROWS, 1);
-  launch_pdl(tcconv_pipe_pl_kernel, dim3(cpipe_grid(units, tc5_sms())), dim3(CPIPE_THREADS), smem, st, P, m.hi, m.lo);
+  tc_launch(tcconv_pipe_pl_kernel, false, dim3(cpipe_grid(units, tc5_sms())), dim3(CPIPE_THREADS), smem, st, P, m.hi, m.lo);
   profile_count_plane();
   profile_count_conv_pipe();
   return true;

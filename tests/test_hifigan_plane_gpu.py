@@ -1,4 +1,4 @@
-"""Plane-fed HiFi-GAN tap-GEMMs (tcconv5_pl_kernel / tcpair_pl_kernel): the leaky-ReLU convs whose input has more
+"""Plane-fed HiFi-GAN tap-GEMMs (tcconv5_pl_kernel / tcconv_pipe_pl_kernel): the leaky-ReLU convs whose input has more
 than 128 channels read it as a pre-split fp16 hi / lo operand plane that the producing epilogue wrote, instead of
 converting the fp32 tensor themselves.  The plane holds exactly the operands the fp32 transform makes, so an engine
 created with AGPT_PLANE_FEED=0 must give the same waveform bit for bit, with the same tap-GEMM launches."""

@@ -607,7 +607,7 @@ def test_plane_output(mode):
 
 # ================================================================================================ fused pairs
 PAIRS = [  # (C, K, dil, tall, plane)
-    (128, 3, 1, 0, 0), (128, 11, 5, 0, 1), (64, 7, 3, 0, 0), (64, 3, 3, 1, 1), (32, 11, 5, 1, 0), (32, 7, 1, 0, 1),
+    (128, 3, 1, 0, 0), (128, 11, 5, 0, 0), (64, 7, 3, 0, 0), (64, 3, 3, 1, 0), (32, 11, 5, 1, 0), (32, 7, 1, 0, 0),
 ]
 
 
@@ -644,3 +644,8 @@ def test_probe_rejects_what_it_cannot_run():
         probe(**dict(base, pro=PRO_SILU, plane_in=1))
     with pytest.raises(RuntimeError, match="pair"):
         probe(**dict(base, pro=PRO_LRELU, pair=1, w2=w.data_ptr(), K2=3, fma=1, res=x, res_gstride=64 * 32, res_pitch=32))
+    pair = dict(base, pro=PRO_LRELU, pair=1, w2=w.data_ptr(), K2=3, res=x, res_gstride=64 * 32, res_pitch=32)
+    with pytest.raises(RuntimeError, match="pair"):
+        probe(**dict(pair, plane_in=1))
+    with pytest.raises(RuntimeError, match="pair"):
+        probe(**dict(pair, po_hi=y, po_lo=y))
