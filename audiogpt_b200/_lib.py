@@ -164,7 +164,6 @@ PROTOTYPES = {
     "agpt_attention": (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _P]),
     "agpt_set_attention_tc": (_I, [_I]),
     "agpt_attention_masked": (_I, [_P, _I, _P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
-    "agpt_bench_tapconv": (_I, [_I] * 10 + [_P, _P]),
     "agpt_tapconv_probe": (_I, [_P, _P, _P]),
     "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
     "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),

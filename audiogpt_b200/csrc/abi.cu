@@ -568,14 +568,6 @@ int agpt_binaural_warp(agpt_handle h, const float* field, const float* mono, con
   });
 }
 
-int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
-                       double* out2, double* dbg8_or_null) {
-  return guarded([&] {
-    AGPT_CHECK(out2, "null argument");
-    bench_tapconv(G, L, Cin, Cout, K, dil, Wreal, epi_res, use_tc, reps, out2, dbg8_or_null);
-  });
-}
-
 int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream) {
   return guarded([&] {
     AGPT_CHECK(args && ran, "null argument");

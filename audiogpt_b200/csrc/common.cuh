@@ -34,40 +34,6 @@ struct Error : public std::runtime_error {
     if (!(cond)) throw ::agpt::Error(std::string("check failed: ") + #cond + ": " + (msg)); \
   } while (0)
 
-// ---- programmatic dependent launch ---------------------------------------------
-// The denoising steps are chains of 50-240 short dependent kernels.  A kernel launched through launch_pdl() may
-// start (block scheduling, shared-memory carve-up, barrier init, tensor-map prefetch) while its
-// predecessor in the stream is still draining; it calls pdl_wait() before its first access to global memory, which
-// returns once the predecessor has completed and flushed.  ONLY kernels that call pdl_wait() may go through
-// launch_pdl(); everything else keeps the ordinary stream order.  The replayed graphs leave little launch gap
-// to hide and the early CTAs compete with the predecessor's last wave, so it is opt-in: AGPT_PDL=1.
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("AGPT_PDL"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
-}
-template <typename... KArgs, typename... Args>
-inline void launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  memset(at, 0, sizeof(at));
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
-  if (e != cudaSuccess) throw Error(std::string("kernel launch: ") + cudaGetErrorString(e));
-}
-#ifdef __CUDACC__
-// wait for the preceding kernel (no-op when this kernel was launched without the attribute), then let the next one in
-__device__ __forceinline__ void pdl_wait() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-#endif
-
 inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 inline long cdivl(long a, long b) { return (a + b - 1) / b; }
 inline int round_up(int a, int b) { return cdiv(a, b) * b; }

@@ -56,7 +56,6 @@ __global__ void diff_step_embed_dev_kernel(float* __restrict__ out, const int* _
 __global__ void p_sample_tab_kernel(float* __restrict__ x, const float* __restrict__ eps, const float* const* __restrict__ noises_pp,
                                     long noise_stride, const float* __restrict__ coef_tab, const int* __restrict__ ctr,
                                     int nsteps, int clip, long n) {
-  pdl_wait();
   const int k = *ctr;
   const float* coef = coef_tab + 5 * (long)k;
   const float A = coef[0], Bc = coef[1], c1 = coef[2], c2 = coef[3], s = coef[4];
@@ -343,18 +342,16 @@ void gd_sample_loop(Handle* hh, float* x_io, int t_hi, int t_lo, const float* co
     select_row(h->dproj_table.p, ctr, h->dproj_cur.p, L * C, s);
     h->eps_core(xl, h->dproj_cur.p, 0, h->loop_eps.p, s);
     dim3 grid((unsigned)std::min<long>(cdivl(n, 256), 1184), B);
-    launch_pdl(p_sample_tab_kernel, grid, dim3(256), 0, s, xl, h->loop_eps.p, noise_pp, noise_stride, h->coef_table.p, ctr, nsteps, clip, n);
+    p_sample_tab_kernel<<<grid, dim3(256), 0, s>>>(xl, h->loop_eps.p, noise_pp, noise_stride, h->coef_table.p, ctr, nsteps, clip, n);
     count_launch(1);
     AGPT_CUDA(cudaGetLastError());
     step_inc(ctr, s);
   };
-  static int allow_graph = -1;
-  if (allow_graph < 0) { const char* e = getenv("AGPT_GRAPH"); allow_graph = (e && e[0] == '0') ? 0 : 1; }
   const long long l0 = launch_count_now();
   step(st);
   h->launches_per_step = (long)(launch_count_now() - l0);
   int done = 1;
-  if (allow_graph && nsteps > 1 && !profile_enabled()) {
+  if (nsteps > 1 && !profile_enabled()) {
     Diffnet::GraphKey k;
     k.B = B; k.T = h->T; k.nsteps = nsteps; k.clip = clip; k.x = xl; k.condp = h->condp.p; k.xcur = h->xcur.p; k.z = h->z.p; k.stride = noise_stride;
     const Diffnet::GraphKey& o = h->gkey;

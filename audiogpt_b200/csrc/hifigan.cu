@@ -587,10 +587,8 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
       const int nd = cfg->resblock_num_dilations[j];
       rb.dil.assign(cfg->resblock_dilations[j], cfg->resblock_dilations[j] + nd);
       // narrow stages: dilation-1 convs with k >= 7 also get a time-grouped image (N = 128 per MMA instead of C)
-      static int allow_group = -1;
-      if (allow_group < 0) { const char* e = getenv("AGPT_TIME_GROUP"); allow_group = (e && e[0] == '0') ? 0 : 1; }
       auto group_of = [&](int dil) {
-        if (!allow_group || cfg->activation != 0 || dil != 1 || rb.ks < 7) return 0;
+        if (cfg->activation != 0 || dil != 1 || rb.ks < 7) return 0;
         if (C == 32) return 4;
         if (C == 64 && rb.ks >= 11) return 2;
         return 0;
@@ -652,34 +650,10 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   return h.release();
 }
 
-// Optional (AGPT_HIFI_L2_MB=<per-tensor MB>): run the generator over sub-batches whose per-stage tensors
-// fit the 50 MB L2 together.  Utterances are independent, so this changes nothing numerically.
-// OFF by default: the smaller grids of a sub-batch fill fewer SMs (not measured on H100).
-static void hifigan_forward_l2(Hifigan* h, const float* mel, const float* har, int B, int T, float* wav, cudaStream_t st) {
-  static long target = -1;
-  if (target < 0) {
-    const char* e = getenv("AGPT_HIFI_L2_MB");          // per-tensor budget in MB; 0 disables sub-batching
-    target = e ? atol(e) * (1L << 20) : 0;
-  }
-  size_t per = (size_t)T * h->cfg.upsample_initial_channel;
-  {
-    long L = T; int C = h->cfg.upsample_initial_channel;
-    for (int i = 0; i < h->cfg.num_upsamples; ++i) { L *= h->cfg.upsample_rates[i]; C /= 2; per = std::max(per, (size_t)L * C); }
-  }
-  per *= sizeof(float);
-  int sb = B;
-  if (target > 0) sb = (int)std::max<long>(1, std::min<long>(B, target / (long)std::max<size_t>(per, 1)));
-  const long wav_per = (long)h->cfg.c_out * T * h->hop, mel_per = (long)h->cfg.n_mels * T, har_per = (long)T * h->hop;
-  for (int b0 = 0; b0 < B; b0 += sb) {
-    const int nb = std::min(sb, B - b0);
-    h->forward(mel + b0 * mel_per, har ? har + b0 * har_per : nullptr, nb, T, wav + b0 * wav_per, st);
-  }
-}
-
 void hifigan_forward(Handle* hh, const float* mel, const float* har, int B, int T, float* wav, cudaStream_t st) {
   auto* h = static_cast<Hifigan*>(hh);
   DeviceGuard dg_(h->device);
-  hifigan_forward_l2(h, mel, har, B, T, wav, st);
+  h->forward(mel, har, B, T, wav, st);
 }
 
 void hifigan_vocode_host(Handle* hh, const float* mel_host, const float* har_host, int B, int T, float* wav_host) {
@@ -700,7 +674,7 @@ void hifigan_vocode_host(Handle* hh, const float* mel_host, const float* har_hos
     AGPT_CUDA(cudaMemcpyAsync(h->io_har.p, har_host, nhar * 4, cudaMemcpyHostToDevice, st));
     har_dev = h->io_har.p;
   }
-  hifigan_forward_l2(h, h->io_mel.p, har_dev, B, T, h->io_wav.p, st);
+  h->forward(h->io_mel.p, har_dev, B, T, h->io_wav.p, st);
   AGPT_CUDA(cudaMemcpyAsync(h->pin_wav, h->io_wav.p, nwav * 4, cudaMemcpyDeviceToHost, st));
   AGPT_CUDA(cudaStreamSynchronize(st));
   memcpy(wav_host, h->pin_wav, nwav * 4);

@@ -109,8 +109,6 @@ void binaural_frames(Handle* h, const float* view, const agpt_binaural_row* rows
 void binaural_warp(Handle* h, const float* field, const float* mono, const agpt_binaural_row* rows, int n, float* out, int clamp,
                    cudaStream_t st);
 
-void bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc, int reps,
-                   double* out, double* dbg_avg);
 void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);
 
 }  // namespace agpt

@@ -45,12 +45,13 @@ __global__ void __launch_bounds__(GN_THREADS) gn_fused_kernel(const float* __res
                                                                int HW, int C, int cpg, float eps, int silu /* 0 none, 1 SiLU, 2 ReLU */, int cached,
                                                                __half* __restrict__ phi, __half* __restrict__ plo,
                                                                const float* __restrict__ res /* added after the activation, or null */) {
-  pdl_wait();
   extern __shared__ __align__(16) float gn_cache[];
   __shared__ double red[GN_THREADS / 32];
   const int n = blockIdx.y, g = blockIdx.x;
-  const float* xb = x + (long)n * HW * C + g * cpg;
-  float* yb = y + (long)n * HW * C + g * cpg;
+  const long slab0 = (long)n * HW * C + g * cpg;   // this CTA's slab: element 0 of its rows in x, y, res and the planes
+  const float* xb = x + slab0;
+  float* yb = y + slab0;
+  const float* rb = res ? res + slab0 : nullptr;
   const int vpr = cpg / V;                 // vectors per row
   const int nvec = HW * vpr;
   // pass 1: sum (and fill the cache)
@@ -87,11 +88,11 @@ __global__ void __launch_bounds__(GN_THREADS) gn_fused_kernel(const float* __res
       float t = (xv - mean) * rstd * __ldg(gamma + g * cpg + c + k) + __ldg(beta + g * cpg + c + k);
       if (silu == 1) t = siluf_(t);
       else if (silu == 2) t = fmaxf(t, 0.f);
-      if (res) t += __ldg(res + ((long)n * HW + r) * C + g * cpg + c + k);
+      if (rb) t += __ldg(rb + (long)r * C + c + k);
       o[k] = t;
     }
     if (phi) {     // operand planes instead of the fp32 tensor (the consumer is a plane-fed GEMM)
-      const long base = ((long)n * HW + r) * C + g * cpg + c;
+      const long base = slab0 + (long)r * C + c;
 #pragma unroll
       for (int k = 0; k < V; ++k) plane_split(o[k], phi[base + k], plo[base + k]);
       continue;
@@ -127,9 +128,9 @@ void groupnorm_ex(const float* x, float* y, const float* gamma, const float* bet
   }
   const dim3 grid(G, N);
   const int si = act;
-  if (cpg % 4 == 0) launch_pdl(gn_fused_kernel<4>, grid, dim3(GN_THREADS), smem, st, x, y, gamma, beta, HW, C, cpg, eps, si, cached, phi, plo, res);
-  else if (cpg % 2 == 0) launch_pdl(gn_fused_kernel<2>, grid, dim3(GN_THREADS), smem, st, x, y, gamma, beta, HW, C, cpg, eps, si, cached, phi, plo, res);
-  else launch_pdl(gn_fused_kernel<1>, grid, dim3(GN_THREADS), smem, st, x, y, gamma, beta, HW, C, cpg, eps, si, cached, phi, plo, res);
+  if (cpg % 4 == 0) gn_fused_kernel<4><<<grid, dim3(GN_THREADS), smem, st>>>(x, y, gamma, beta, HW, C, cpg, eps, si, cached, phi, plo, res);
+  else if (cpg % 2 == 0) gn_fused_kernel<2><<<grid, dim3(GN_THREADS), smem, st>>>(x, y, gamma, beta, HW, C, cpg, eps, si, cached, phi, plo, res);
+  else gn_fused_kernel<1><<<grid, dim3(GN_THREADS), smem, st>>>(x, y, gamma, beta, HW, C, cpg, eps, si, cached, phi, plo, res);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
@@ -139,7 +140,6 @@ size_t groupnorm_scratch_doubles(int N, int C) { (void)N; (void)C; return 16; }
 __global__ void layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                                  const float* __restrict__ beta, float* __restrict__ y, long rows, int C, float eps,
                                  __half* __restrict__ phi, __half* __restrict__ plo) {
-  pdl_wait();
   const long row = (long)blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
@@ -165,7 +165,7 @@ __global__ void layernorm_kernel(const float* __restrict__ x, const float* __res
 void layernorm(const float* x, float* y, const float* gamma, const float* beta, long rows, int C, float eps,
                cudaStream_t st, __half* phi, __half* plo) {
   const int wpb = 8;
-  launch_pdl(layernorm_kernel, dim3((unsigned)cdivl(rows, wpb)), dim3(wpb * 32), 0, st, x, gamma, beta, y, rows, C, eps, phi, plo);
+  layernorm_kernel<<<dim3((unsigned)cdivl(rows, wpb)), dim3(wpb * 32), 0, st>>>(x, gamma, beta, y, rows, C, eps, phi, plo);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
@@ -418,19 +418,17 @@ void timestep_embedding_dev(float* out, const int* t_dev, int rows, int dim, cud
 // A denoising loop replays ONE captured step; everything that changes from step to step is read from device
 // tables indexed by a device counter: out[c] = table[*step][c]; the counter is bumped by the last node of the step.
 __global__ void select_row_kernel(const float* __restrict__ table, const int* __restrict__ step, float* __restrict__ out, int ncols) {
-  pdl_wait();
   const long k = *step;
   for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < ncols; c += gridDim.x * blockDim.x) out[c] = table[k * ncols + c];
 }
 void select_row(const float* table, const int* step_dev, float* out, int ncols, cudaStream_t st) {
-  launch_pdl(select_row_kernel, dim3(std::min(64, cdiv(ncols, 256))), dim3(256), 0, st, table, step_dev, out, ncols);
+  select_row_kernel<<<dim3(std::min(64, cdiv(ncols, 256))), dim3(256), 0, st>>>(table, step_dev, out, ncols);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
-__global__ void step_inc_kernel(int* step) {
-  pdl_wait(); *step += 1; }
+__global__ void step_inc_kernel(int* step) { *step += 1; }
 void step_inc(int* step_dev, cudaStream_t st) {
-  launch_pdl(step_inc_kernel, dim3(1), dim3(1), 0, st, step_dev);
+  step_inc_kernel<<<dim3(1), dim3(1), 0, st>>>(step_dev);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
@@ -438,7 +436,6 @@ void step_inc(int* step_dev, cudaStream_t st) {
 // ------------------------------------------------------------------ gathers
 __global__ void concat_kernel(const float* __restrict__ a, int Ca, const float* __restrict__ b, int Cb,
                               float* __restrict__ out, long rows) {
-  pdl_wait();
   const int C = Ca + Cb;
   const long total = rows * (C / 4);
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -452,14 +449,13 @@ __global__ void concat_kernel(const float* __restrict__ a, int Ca, const float* 
 void concat_channels(const float* a, int Ca, const float* b, int Cb, float* out, long rows, cudaStream_t st) {
   AGPT_CHECK(Ca % 4 == 0 && Cb % 4 == 0, "concat channels must be multiples of 4");
   const long total = rows * ((Ca + Cb) / 4);
-  launch_pdl(concat_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, a, Ca, b, Cb, out, rows);
+  concat_kernel<<<dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st>>>(a, Ca, b, Cb, out, rows);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
 
 // nearest x2: out[n][2H][2W][C] = in[n][h/2][w/2][C]   (F.interpolate(scale_factor=2, mode='nearest'))
 __global__ void upsample2_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int H, int W, int C) {
-  pdl_wait();
   const long total = (long)N * 4 * H * W * (C / 4);
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int c = (int)(i % (C / 4)) * 4;
@@ -473,7 +469,7 @@ __global__ void upsample2_kernel(const float* __restrict__ in, float* __restrict
 }
 void upsample_nearest2(const float* in, float* out, int N, int H, int W, int C, cudaStream_t st) {
   const long total = (long)N * 4 * H * W * (C / 4);
-  launch_pdl(upsample2_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, in, out, N, H, W, C);
+  upsample2_kernel<<<dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st>>>(in, out, N, H, W, C);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
@@ -481,7 +477,6 @@ void upsample_nearest2(const float* in, float* out, int N, int H, int W, int C, 
 // 2x2 average pool with stride 2 and floor (the ResBlock down path's AvgPool2d(2, 2), openaimodel.py:134-160):
 // out[n][ho][wo][C] = (x[2ho][2wo] + x[2ho][2wo+1] + x[2ho+1][2wo] + x[2ho+1][2wo+1]) / 4, summed in that order
 __global__ void avgpool2_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int H, int W, int C) {
-  pdl_wait();
   const int Ho = H / 2, Wo = W / 2;
   const long total = (long)N * Ho * Wo * (C / 4);
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -501,7 +496,7 @@ __global__ void avgpool2_kernel(const float* __restrict__ in, float* __restrict_
 void avgpool2(const float* in, float* out, int N, int H, int W, int C, cudaStream_t st) {
   AGPT_CHECK(C % 4 == 0 && H >= 2 && W >= 2, "avgpool2: channels must be a multiple of 4 and the map at least 2x2");
   const long total = (long)N * (H / 2) * (W / 2) * (C / 4);
-  launch_pdl(avgpool2_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, in, out, N, H, W, C);
+  avgpool2_kernel<<<dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st>>>(in, out, N, H, W, C);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
@@ -511,7 +506,6 @@ void avgpool2(const float* in, float* out, int N, int H, int W, int C, cudaStrea
 // conv without padding -- the one zero row / column past the end is the same out-of-range read
 __global__ void im2col_s2_kernel(const float* __restrict__ in, float* __restrict__ col, int N, int H, int W, int C,
                                  int Ho, int Wo, int pad) {
-  pdl_wait();
   const long total = (long)N * Ho * Wo * 9 * (C / 4);
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int c = (int)(i % (C / 4)) * 4;
@@ -528,8 +522,7 @@ __global__ void im2col_s2_kernel(const float* __restrict__ in, float* __restrict
 }
 void im2col_stride2(const float* in, float* col, int N, int H, int W, int C, int Ho, int Wo, int pad, cudaStream_t st) {
   const long total = (long)N * Ho * Wo * 9 * (C / 4);
-  launch_pdl(im2col_s2_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, in, col, N, H, W, C, Ho, Wo,
-             pad);
+  im2col_s2_kernel<<<dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st>>>(in, col, N, H, W, C, Ho, Wo, pad);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
@@ -538,7 +531,6 @@ void im2col_stride2(const float* in, float* col, int N, int H, int W, int C, int
 // sample n reads source sample n % Nsrc: the doubled batch of classifier-free guidance (x_in = cat([x] * 2),
 // ddim.py:178) is produced here instead of by two device-to-device copies
 __global__ void cf_to_cl_pad_kernel(const float* __restrict__ in, float* __restrict__ out, int C, int Cpad, int HW, long total, int Nsrc) {
-  pdl_wait();
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int c = (int)(i % Cpad);
     const long r = i / Cpad;
@@ -548,7 +540,7 @@ __global__ void cf_to_cl_pad_kernel(const float* __restrict__ in, float* __restr
 }
 void cf_to_cl_pad(const float* in, float* out, int N, int C, int Cpad, int HW, cudaStream_t st, int Nsrc) {
   const long total = (long)N * HW * Cpad;
-  launch_pdl(cf_to_cl_pad_kernel, dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st, in, out, C, Cpad, HW, total, Nsrc > 0 ? Nsrc : N);
+  cf_to_cl_pad_kernel<<<dim3((unsigned)std::min<long>(cdivl(total, 256), 4096)), dim3(256), 0, st>>>(in, out, C, Cpad, HW, total, Nsrc > 0 ? Nsrc : N);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }
@@ -605,7 +597,6 @@ __global__ void __launch_bounds__(256) conv_out_ddim_kernel(const float* __restr
                                                              const float* __restrict__ bias, float* __restrict__ x /*[B][4][HW] in place*/,
                                                              float* __restrict__ pred_x0, const float* __restrict__ coef,
                                                              const int* __restrict__ step, int B, int H, int W, int C, int single) {
-  pdl_wait();
   const int HW = H * W;
   const int lane = threadIdx.x & 31;
   const int p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -658,7 +649,7 @@ __global__ void __launch_bounds__(256) conv_out_ddim_kernel(const float* __restr
 void conv_out_ddim(const float* hn, const float* w9c4, const float* bias4, float* x_io, float* pred_x0, const float* coef_dev,
                    const int* step_dev, int B, int H, int W, int C, int single, cudaStream_t st) {
   dim3 grid(cdiv(H * W, 8), B);
-  launch_pdl(conv_out_ddim_kernel, grid, dim3(256), 0, st, hn, w9c4, bias4, x_io, pred_x0, coef_dev, step_dev, B, H, W, C, single);
+  conv_out_ddim_kernel<<<grid, dim3(256), 0, st>>>(hn, w9c4, bias4, x_io, pred_x0, coef_dev, step_dev, B, H, W, C, single);
   count_launch(1);
   AGPT_CUDA(cudaGetLastError());
 }

@@ -56,10 +56,9 @@ struct TapConvParams {
   int epi; const float* res; long res_gstride; int res_pitch; float scale; int accumulate;
   const float* evec; int evec_gstride;
   float* out2; long out2_gstride; int out2_pitch; int csplit;
-  const float* w_h; const float* w_h256; const float* w_h64; const float* w_h96; int tc_chunks_h; float tc_descale;   // fp16 hi/lo image (tcconv5.cu): 64-channel chunks, weights pre-scaled by 1/tc_descale
+  const float* w_h; const float* w_h64; const float* w_h96; int tc_chunks_h; float tc_descale;   // fp16 hi/lo image (tcconv5.cu): 64-channel chunks, weights pre-scaled by 1/tc_descale
   const float* w_hk;   // 128 -> 128 channels: the same weights in 32-channel half-stages (tcpair_pipe_kernel's ring)
-  int tc_bn, tc_na, tc_nw, tc_nr, tc_nwk, tc_nb, tc_tps, tc_flags, tc_flags_user;   // tc_bn == 0 => FMA only
-  long long* dbg;      // optional per-CTA phase timestamps (tc_flags & 2)
+  int tc_bn, tc_na, tc_nw, tc_nr;   // tc_bn == 0 => FMA only
   float flops_scale;   // useful fraction of the MACs (zero-padded polyphase taps); 0 => 1
   // 2-D convs on WIDE images (the VAE decoder's 80x624 maps): the image is cut into `strips` vertical strips of
   // `strip_w` columns; grid slice gz = g * strips + s works on the virtual grid [H][strip_w + 2] of strip s
@@ -71,9 +70,9 @@ struct TapConvParams {
   // consumer (UNet ff2, a 4C-deep 1-tap GEMM) is then plane-fed; with out == nullptr the fp32 tensor is not written
   __half* pl_hi; __half* pl_lo; int pl_pitch;
   // 1: the tensor-core kernels may run 256-row tiles (tc5_tall in tcconv5.cu decides per launch); set by the HiFi-GAN
-  // driver.  Kept last: the kernels read the fields above at fixed parameter-bank offsets, which stay as they were.
+  // driver.
   int tc_tall;
-  // Operand planes of the leaky-ReLU tap-GEMMs (HiFi-GAN driver; tensor-core kernels only, appended as tc_tall was).
+  // Operand planes of the leaky-ReLU tap-GEMMs (HiFi-GAN driver; tensor-core kernels only).
   // A plane is two fp16 tensors laid out like the fp32 one (same pitch and sample stride, in elements):
   //   hi = fp16(lrelu(x, slope)),  lo = fp16(lrelu(x, slope) - hi)
   // bit for bit the operands the kernels' own fp32 transform makes.  pi_*: the input is read from this plane (TMA)
@@ -125,7 +124,7 @@ __host__ __device__ inline int tc_row_out(const TapConvParams& P, int gz, int q,
 
 // ---------------------------------------------------------------- host side
 struct PackedConv {
-  DevBuf w, b, w_h, w_h256, w_h64, w_h96, w_hk;
+  DevBuf w, b, w_h, w_h64, w_h96, w_hk;
   int tc_bn = 0, h_chunks = 0;
   float h_descale = 1.f;
   int Cin = 0, cin_pad = 0, Cout = 0, cout_pad = 0, ntaps = 0;
@@ -201,7 +200,7 @@ inline TapConvParams tapconv_params(const PackedConv& pc, int G, int L, int Wrea
   P.scale = 1.f;
   P.flops_scale = pc.useful;
   P.tc_bn = pc.tc_bn;
-  P.w_h = pc.w_h.p; P.w_h256 = pc.w_h256.p; P.w_h64 = pc.w_h64.p; P.w_h96 = pc.w_h96.p; P.w_hk = pc.w_hk.p; P.tc_chunks_h = pc.h_chunks; P.tc_descale = pc.h_descale;
+  P.w_h = pc.w_h.p; P.w_h64 = pc.w_h64.p; P.w_h96 = pc.w_h96.p; P.w_hk = pc.w_hk.p; P.tc_chunks_h = pc.h_chunks; P.tc_descale = pc.h_descale;
   return P;
 }
 

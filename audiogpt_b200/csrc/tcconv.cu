@@ -1,10 +1,12 @@
-// Dispatcher of the fp16 hi/lo tensor-core tap-GEMM (the kernel lives in tcconv5.cu):
+// Host entry of the fp16 hi/lo tensor-core tap-GEMM (the kernels, their tile choice and their launches live in
+// tcconv5.cu):
 //
 //   out[g, p, co] = epi( bias[co] + sum_tap sum_ci pro(in[g, p + off_tap, ci]) * W[tap][ci][co] )
 //
 // Same TapConvParams contract (and the same fused prologue / epilogue table) as the fp32-FMA kernel in tapconv.cu;
 // the inner product runs as wgmma on error-compensated fp16 hi/lo operand parts with fp32 accumulation in registers
-// (header of tcconv5.cu): one [128 x BN] tile per CTA.
+// (header of tcconv5.cu).  This file packs the weights, holds the AGPT_TENSOR_CORES switch, decides whether a layer
+// can run on the tensor cores, and fails the launch of a layer that fits no tile.
 #include "tapconv.cuh"
 #include "models.h"
 
@@ -33,7 +35,6 @@ bool tcconv_supported(const TapConvParams& P) {
 }
 
 void tcconv_launch(TapConvParams P, cudaStream_t st) {
-  P.tc_flags = P.tc_flags_user;
   if (tcconv5_launch(P, st)) return;
   throw Error("tcconv: layer does not fit the shared-memory budget of the tensor-core kernel (image too wide for the halo tile?)");
 }

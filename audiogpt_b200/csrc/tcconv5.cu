@@ -199,11 +199,10 @@ __device__ __forceinline__ void stage_block(const float (&acc)[MB][NJ][NH], uint
 // global READS of the first LA items of a block (residual / old accumulator) are issued one block ahead -- on a 128-row
 // tile with LA = 4 for block 0 before the accumulator is complete.  A tall tile, and LA < 4 (tcpair2_kernel, within
 // the registers of two CTAs per SM), read block 0 once that block is staged, not next to the whole accumulator, and
-// item i + LA once item i is stored.  dbg: the timed thread's debug record (tcconv5_body), else null.
+// item i + LA once item i is stored.
 template <int BN, int MT, int LA, bool PL, int MB, int NJ, int NH>
 __device__ __forceinline__ void tile_epilogue(float (&acc)[MB][NJ][NH], const TapConvParams& P, int g, int co0,
-                                              const int* rowp, uint8_t* smem, const Tc5Smem& S, int wg, int xt,
-                                              long long* dbg) {
+                                              const int* rowp, uint8_t* smem, const Tc5Smem& S, int wg, int xt) {
   constexpr bool early = MT == TC_ROWS && LA == 4;
   EpiPre pre[8];
   int pp[8];
@@ -218,10 +217,8 @@ __device__ __forceinline__ void tile_epilogue(float (&acc)[MB][NJ][NH], const Ta
     }
   };
   if (early) load_block(0);
-  if (dbg) { dbg[2] = dbg[1]; dbg[3] = clock64(); dbg[6] = 0; dbg[7] = 0; }   // the workers issue the wgmmas: no waits of a separate issuer
   mma_drain(acc, nullptr, -1);
   named_bar_sync(1, NWK);                      // both warpgroups' wgmmas are done reading the operand buffers
-  if (dbg) dbg[4] = clock64();
   uint8_t* stg0 = smem + S.a_hi[0];
   const int lane = xt & 31, r0 = wg * (MT / 2) + ((xt >> 5) & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
@@ -249,7 +246,6 @@ __device__ __forceinline__ void tile_epilogue(float (&acc)[MB][NJ][NH], const Ta
     // staging halves alternate; a half is rewritten two blocks later, after the next named
     // barrier, so no extra barrier is needed here
   }
-  if (dbg) dbg[5] = clock64();
 }
 
 // c1 -> c2 hand-off of a fused pair: c1's accumulator becomes c2's operand tile a2 with the arithmetic of c1's EPI_BIAS
@@ -360,9 +356,6 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
   const int Lv = tc_lv(P);
   const int nchunks = P.tc_chunks_h, ntaps = P.ntaps, total = nchunks * ntaps;
   const int lo = P.lo_al;
-  const bool dbg_on = (P.tc_flags & 2) && P.dbg;
-  long long* dbg = dbg_on ? P.dbg + 8 * ((long)(blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) : nullptr;
-  if (dbg_on && tid == 0) dbg[0] = clock64();
 
   if (tid == 0) {
     for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], NWK / 32); }
@@ -379,8 +372,6 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
     if (xt < MT) rowp[xt] = tc_row_out(P, gz, q0 + xt, Wv, Lv);   // output row -> real position (or -1)
   }
   __syncthreads();
-  pdl_wait();          // everything above overlaps the previous kernel's tail
-  if (dbg_on && tid == 0) dbg[1] = clock64();
 
   if (is_worker) {
     // =========================== worker warps: transform ===========================
@@ -476,7 +467,7 @@ __device__ __forceinline__ void tcconv5_body(const TapConvParams& P, const CUten
       }
     }
     // =========================== worker warps: epilogue ===========================
-    tile_epilogue<BN, MT, 4, PL>(acc, P, g, co0, rowp, smem, S, wg, xt, dbg_on && tid == 0 ? dbg : nullptr);
+    tile_epilogue<BN, MT, 4, PL>(acc, P, g, co0, rowp, smem, S, wg, xt);
   } else if (lane == 0) {
     // =========================== weight producer (warp 8) ===========================
     const uint32_t bytes = 2u * BN * 128u;
@@ -549,7 +540,6 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
     if (xt < MT) rowp[xt] = (xt < MT - span2 && q0 + xt < Lv) ? q0 + xt : -1;
   }
   __syncthreads();
-  pdl_wait();
 
   if (is_worker) {
     const float* __restrict__ ing = P1.in + g * P1.in_gstride;
@@ -701,7 +691,7 @@ __device__ __forceinline__ void tcpair_body(const TapConvParams& P1, const TapCo
       mma_taps(P2, ahi0, ahi0 + lo_part, (min(H_KCH, P2.Cin - c * H_KCH) + 15) >> 4);
     }
     // =========================== c2's epilogue ===========================
-    tile_epilogue<BN, MT, HALF ? 1 : 4, false>(acc, P2, g, 0, rowp, smem, S, wg, xt, nullptr);
+    tile_epilogue<BN, MT, HALF ? 1 : 4, false>(acc, P2, g, 0, rowp, smem, S, wg, xt);
   } else if (lane == 0) {
     // =========================== weight producer (warp 8): c1's stages, then c2's ===========================
     const uint32_t bytes = 2u * BN * 128u;
@@ -804,7 +794,6 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
 
   if (wg < 2) {
     // =========================== wgmma warpgroups: rows 64 wg .. 64 wg + 63 of each tile ===========================
@@ -1025,7 +1014,6 @@ __global__ void __launch_bounds__(NARROW_THREADS, 1) tcpair_narrow_kernel(const 
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
 
   if (wg < 2) {
     // ====================== wgmma warpgroups: warpgroup wg runs the whole of tiles wg, wg + 2, .. ======================
@@ -1268,7 +1256,6 @@ __global__ void __launch_bounds__(CPIPE_THREADS, 1) tcconv_pipe_pl_kernel(const 
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();
 
   if (wg < 2) {
     // =========================== wgmma warpgroups: warpgroup wg runs items wg, wg + 2, .. ===========================
@@ -1607,7 +1594,8 @@ static void tc_func_attrs(const void* kern, bool dual) {
 template <typename... KArgs, typename... Args>
 static void tc_launch(void (*kern)(KArgs...), bool dual, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   tc_func_attrs(reinterpret_cast<const void*>(kern), dual);
-  launch_pdl(kern, grid, block, smem, st, std::forward<Args>(args)...);
+  kern<<<grid, block, smem, st>>>(std::forward<Args>(args)...);
+  AGPT_CUDA(cudaGetLastError());
 }
 
 // the instantiation of each tile-kernel family for a BN-column, MT-row tile (BN <= 64 for MT = TC_TALL)
@@ -1681,8 +1669,6 @@ static bool tcconv5_try(TapConvParams P, int BN, int MT, cudaStream_t st) {
 HTile pick_h_tile(const TapConvParams& P, int sms) {
   const int Lv = tc_lv(P);
   const long rt = (long)cdiv(Lv, TC_ROWS) * tc_groups(P);
-  static int allow96 = -1;
-  if (allow96 < 0) { const char* e = getenv("AGPT_TC_BN96"); allow96 = (e && e[0] == '0') ? 0 : 1; }
   auto cost = [](int bn) { return bn == 128 ? 1.0 : (bn == 96 ? 0.82 : (bn == 64 ? 0.62 : 0.45)); };
   HTile best{P.tc_bn, P.w_h, rt * cdiv(P.Cout, P.tc_bn), TC_ROWS};
   double bs = (double)cdiv(best.ntiles, (long)sms) * cost(P.tc_bn);
@@ -1693,7 +1679,7 @@ HTile pick_h_tile(const TapConvParams& P, int sms) {
     if (sc < bs - 1e-9) { bs = sc; best = HTile{bn, w, nt, TC_ROWS}; }
   };
   if (P.tc_bn == 128) consider(64, P.w_h64);
-  if (P.tc_bn == 128 && allow96) consider(96, P.w_h96);   // e.g. 640 channels on 16 row tiles: 112 tiles in one wave
+  if (P.tc_bn == 128) consider(96, P.w_h96);     // e.g. 640 channels on 16 row tiles: 112 tiles in one wave
   const long tall = (long)cdiv(Lv, TC_TALL) * tc_groups(P) * cdiv(P.Cout, best.bn);
   if (tc5_tall(P, best.bn, tall, sms)) { best.mt = TC_TALL; best.ntiles = tall; }
   return best;

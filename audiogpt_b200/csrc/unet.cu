@@ -356,9 +356,7 @@ struct Unet : Handle {
     int* ctr = reinterpret_cast<int*>(step_ctr.p);
     select_row(emb_table.p, ctr, emb_cur.p, emb_total, s);
     emb_gstride = 0;
-    static int fuse_tail = -1;
-    if (fuse_tail < 0) { const char* e = getenv("AGPT_FUSE_DDIM"); fuse_tail = (e && e[0] == '0') ? 0 : 1; }
-    if (fuse_tail && out_w9c4.p) {
+    if (out_w9c4.p) {
       forward_core(ddim_x.p, B, emb_cur.p, N, H, W, nullptr, s, cat);      // ... -> GN -> [out conv + CFG + x_prev update]
     } else {
       forward_core(ddim_x.p, B, emb_cur.p, N, H, W, ddim_eps.p, s, cat);
@@ -584,7 +582,7 @@ void unet_forward(Handle* hh, const float* x, const int* t_host, int N, int H, i
 // Whole DDIM loop (ddim.py:143-164 + p_sample_ddim): the context holds [uncond ; cond] (2B rows) when
 // cfg_scale != 1, else B rows.  Step-invariant work is hoisted: the time-embedding MLP and the 12 ResBlock
 // embedding projections run ONCE for all S timesteps (one GEMM with S rows); step 0 runs eagerly (sizes every
-// buffer), then one step is captured into a CUDA graph and replayed S - 1 times (AGPT_GRAPH=0: plain launches).
+// buffer), then one step is captured into a CUDA graph and replayed S - 1 times (plain launches while profiling).
 void unet_ddim_sample(Handle* hh, const float* x_T, int B, int H, int W, int S, const int* t_steps,
                       const float* a_t, const float* a_prev, const float* sigma, const float* sqrt_om,
                       float cfg_scale, float* x_out, float* pred_x0_out, cudaStream_t st) {
@@ -633,13 +631,11 @@ void unet_ddim_sample(Handle* hh, const float* x_T, int B, int H, int W, int S, 
   }
   AGPT_CUDA(cudaMemcpyAsync(u->ddim_x.p, x_T, (size_t)B * n * sizeof(float), cudaMemcpyDeviceToDevice, st));
 
-  static int allow_graph = -1;
-  if (allow_graph < 0) { const char* e = getenv("AGPT_GRAPH"); allow_graph = (e && e[0] == '0') ? 0 : 1; }
   const long l0 = launch_count_now();
   u->ddim_step(B, N, H, W, n, cat, st);                              // step 0, eager
   u->launches_per_step = launch_count_now() - l0;
   int done = 1;
-  if (allow_graph && S > 1 && !profile_enabled()) {
+  if (S > 1 && !profile_enabled()) {
     Unet::GraphKey k;
     k.N = N; k.H = H; k.W = W; k.single = cfg_on ? 0 : 1; k.arena = u->arena.p; k.ctx = u->ctx_kv.p; k.x = u->ddim_x.p; k.ctxS = u->ctxS;
     k.cat = cat;

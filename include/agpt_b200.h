@@ -68,13 +68,6 @@ int agpt_set_attention_tc(int on);
 int agpt_attention_masked(const float* q, int q_pitch, const float* k, int k_pitch, const float* v, int v_pitch,
                           const uint8_t* key_padding_mask, float* o, int o_pitch, int N, int heads, int d, int Lq, int Lk,
                           void* stream);
-/* Micro-benchmark of one tapconv layer (random data): out2 = {ms per launch, algorithmic TFLOP/s}; dbg8
- * (tensor-core kernel only) = average per-CTA phase cycles {setup, first activation tile, MMA issue loop, drain,
- * epilogue, total, wait-on-activations, wait-on-weights}.  Wreal > 0 selects a 3x3 conv on an (L/Wreal) x Wreal
- * image.                                                                                                       */
-int agpt_bench_tapconv(int G, int L, int Cin, int Cout, int K, int dil, int Wreal, int epi_res, int use_tc,
-                       int reps, double* out2, double* dbg8_or_null);
-
 /* Conformance entry of the tap-GEMM primitive (tests/test_tapconv_gpu.py): ONE launch of the production path --
  * the production weight packer, tapconv_launch (or the fused pair launch) -- on caller-owned device tensors.
  * Weights and bias are fp32 HOST arrays in the torch layouts; everything else passes through to the launch
@@ -202,7 +195,8 @@ int agpt_gd_p_sample(agpt_handle h_or_null, const float* x, const float* eps_or_
  * agpt_gd_p_sample in SAMPLING order (row k belongs to t = t_hi-1-k).  noises_or_null: device
  * [t_hi-t_lo][noise_step_stride] floats, pre-drawn by the caller in the reference's RNG call order.  The
  * step-embedding MLP and the per-layer diffusion projections run once for all steps; step 0 runs as plain
- * launches, then ONE captured step (CUDA graph + device-side step counter) is replayed.  AGPT_GRAPH=0 disables. */
+ * launches, then ONE captured step (CUDA graph + device-side step counter) is replayed; while agpt_profile_enable
+ * is on, every step runs as plain launches.                                                                 */
 int agpt_gd_sample_loop(agpt_handle h, float* x_io, int t_hi, int t_lo, const float* coef_host,
                         const float* noises_or_null, long noise_step_stride, int clip_denoised, void* stream);
 long agpt_diffnet_launches_per_step(agpt_handle h);
@@ -265,7 +259,7 @@ int agpt_ddim_update(const float* x, const float* eps2, int eps2_is_single, floa
  * launches, then ONE captured step (CUDA graph, device-side step counter and coefficient tables)
  * is replayed S-1 times; the step's x_prev update reads its scalars from the table (no host sync,
  * no per-step H2D).  pred_x0_or_null receives the last step's pred_x0 (ddim.py:216).
- * AGPT_GRAPH=0 in the environment replaces the replays by plain launches.                     */
+ * While agpt_profile_enable is on, every step runs as plain launches.                          */
 int agpt_unet_ddim_sample(agpt_handle h, const float* x_T, int B, int H, int W, int S,
                           const int* t_steps_host, const float* a_t, const float* a_prev,
                           const float* sigma, const float* sqrt_om, float cfg_scale,
