@@ -24,6 +24,7 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
     audiogpt_b200.audio_detection.target_sound_detection.src.models.RaDur_fusion
                                                                     (installed with install(target_detection=True))
     audiogpt_b200.mono2binaural.src.models.BinauralNetwork          (installed with install(binaural=True))
+    audiogpt_b200.inference.tts.base_tts_infer.Wav2Vec2ForCTC       (installed with install(asr=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -88,6 +89,12 @@ _TARGET_DETECTION_MAP = {
     "target_sound_detection.src.models": ("audiogpt_b200.audio_detection.target_sound_detection.src.models", ["RaDur_fusion"]),
 }
 
+# the TTS_OOD tool's reference-audio ASR, grafted only on request (install(asr=True)).  The module also holds
+# BaseTTSInfer, which the TTS inferers import, so it is patched in place as _TARGET_DETECTION_MAP is, never aliased.
+_ASR_MAP = {
+    "inference.tts.base_tts_infer": ("audiogpt_b200.inference.tts.base_tts_infer", ["Wav2Vec2ForCTC"]),
+}
+
 # the Binaural tool's BinauralNetwork, grafted only on request (install(binaural=True)).  The tool imports it as
 # ``src.models`` (mono2binaural/ on its sys.path), a generic name: the module is patched in place only when it is the
 # reference's (it defines Warpnet and BinauralNetwork), and never aliased.
@@ -98,7 +105,7 @@ _BINAURAL_MAP = {
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
             text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False, detection: bool = False,
-            target_detection: bool = False, binaural: bool = False):
+            target_detection: bool = False, binaural: bool = False, asr: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -133,6 +140,10 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     tool's Cnn14 reference encoder, multi-scale CNN, bidirectional GRU and enhancement pass run on the engine.  That
     module is only patched in place: the tool also imports its ``event_labels``, so when it does not import it is
     reported as skipped (and raises under ``strict``), never aliased.
+    ``asr=True`` also replaces ``inference.tts.base_tts_infer.Wav2Vec2ForCTC``, so build_asr's
+    ``Wav2Vec2ForCTC.from_pretrained`` builds the drop-in and the TTS_OOD tool's reference-audio transcription runs on the
+    engine.  Like ``target_detection``, the module is only patched in place (it also holds BaseTTSInfer): when it does not
+    import it is reported as skipped (and raises under ``strict``), never aliased.
     ``binaural=True`` also replaces ``src.models.BinauralNetwork`` (mono2binaural/src/models.py), so the Binaural tool's
     geometric and neural time warp run on the engine.  ``src`` is a generic name, so the module is patched in place only
     when it is the reference's (it defines ``Warpnet`` and ``BinauralNetwork``); when it does not import or is some other
@@ -171,8 +182,9 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
                 mine._reference_cls = theirs
             setattr(ref, a, mine)
         patched.append(ref_name)
-    if target_detection:
-        for ref_name, (our_name, attrs) in _TARGET_DETECTION_MAP.items():
+    in_place = dict(**(_TARGET_DETECTION_MAP if target_detection else {}), **(_ASR_MAP if asr else {}))
+    if in_place:
+        for ref_name, (our_name, attrs) in in_place.items():
             ours = importlib.import_module(our_name)
             try:
                 ref = importlib.import_module(ref_name)

@@ -19,6 +19,7 @@ AGPT_MAX_UPS = 8
 AGPT_MAX_RBK = 8
 AGPT_MAX_DIL = 8
 AGPT_MAX_LEVELS = 8
+AGPT_W2V_MAX_CONV = 8
 
 
 class HifiganCfg(C.Structure):
@@ -120,6 +121,14 @@ class BinauralConfig(C.Structure):
 class BinauralRow(C.Structure):
     """agpt_binaural_row: one BinauralNetwork forward (a batch item or a chunk of the tool's loop)."""
     _fields_ = [(n, C.c_int64) for n in ("mono_off", "T", "view_off", "view_stride", "K", "keep", "out_off", "out_stride")]
+
+
+class W2vConfig(C.Structure):
+    """agpt_w2v_cfg (a tagged struct in the header, like agpt_clap_cfg; the create entry point takes a plain pointer)."""
+    _fields_ = [("conv_layers", C.c_int), ("conv_dim", C.c_int), ("conv_kernel", C.c_int * AGPT_W2V_MAX_CONV),
+                ("conv_stride", C.c_int * AGPT_W2V_MAX_CONV)] + [(n, C.c_int) for n in (
+        "hidden_size", "num_layers", "num_heads", "intermediate_size", "num_conv_pos_embeddings",
+        "num_conv_pos_embedding_groups", "vocab_size")] + [("layer_norm_eps", C.c_float)]
 
 
 class TapconvProbeArgs(C.Structure):
@@ -227,6 +236,11 @@ PROTOTYPES = {
     "agpt_binaural_forward": (_I, [_P, _P, _P, _P, _I, _P, _I, _P]),
     "agpt_binaural_frames": (_I, [_P, _P, _P, _I, _P, _P]),
     "agpt_binaural_warp": (_I, [_P, _P, _P, _P, _I, _P, _I, _P]),
+    "agpt_w2v_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_w2v_frames": (_I, [_P, _L, _P]),
+    "agpt_w2v_logits": (_I, [_P, _P, _I, _L, _P, _P]),
+    "agpt_w2v_features": (_I, [_P, _P, _I, _L, _P, _P]),
+    "agpt_w2v_pos_conv": (_I, [_P, _P, _I, _I, _P, _P]),
 }
 
 _lock = threading.Lock()

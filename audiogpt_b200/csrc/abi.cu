@@ -568,6 +568,43 @@ int agpt_binaural_warp(agpt_handle h, const float* field, const float* mono, con
   });
 }
 
+int agpt_w2v_create(const agpt_w2v_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(w2v_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_w2v_frames(const agpt_w2v_cfg* cfg, long n_samples, int* frames) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && frames, "null argument");
+    AGPT_CHECK(cfg->conv_layers >= 1 && cfg->conv_layers <= AGPT_W2V_MAX_CONV, "conv_layers must be 1..8");
+    for (int i = 0; i < cfg->conv_layers; ++i) AGPT_CHECK(cfg->conv_kernel[i] >= 1 && cfg->conv_stride[i] >= 1, "bad conv geometry");
+    w2v_lengths(cfg, n_samples, frames);
+  });
+}
+
+int agpt_w2v_logits(agpt_handle h, const float* input_values, int B, long n_samples, float* logits, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(input_values && logits, "null argument");
+    w2v_logits(as(h, kMagicW2v, "w2v"), input_values, B, n_samples, logits, (cudaStream_t)stream);
+  });
+}
+
+int agpt_w2v_features(agpt_handle h, const float* input_values, int B, long n_samples, float* features, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(input_values && features, "null argument");
+    w2v_features(as(h, kMagicW2v, "w2v"), input_values, B, n_samples, features, (cudaStream_t)stream);
+  });
+}
+
+int agpt_w2v_pos_conv(agpt_handle h, const float* hidden, int B, int T, float* out, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(hidden && out, "null argument");
+    w2v_pos_conv(as(h, kMagicW2v, "w2v"), hidden, B, T, out, (cudaStream_t)stream);
+  });
+}
+
 int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream) {
   return guarded([&] {
     AGPT_CHECK(args && ran, "null argument");

@@ -114,10 +114,15 @@ void ClapNet::trunk(int N, int L, const uint8_t* kpm_, cudaStream_t st) {
 }
 
 void ClapNet::load_bert(WeightCursor& wc) {
-  const int H = cfg.hidden_size, I = cfg.intermediate_size;
+  const int H = cfg.hidden_size;
   word.upload(wc.next(), (size_t)cfg.vocab_size * H);
   pos.upload(wc.next(), (size_t)cfg.max_position_embeddings * H);
   types.upload(wc.next(), (size_t)cfg.type_vocab_size * H);
+  load_trunk(wc);
+}
+
+void ClapNet::load_trunk(WeightCursor& wc) {
+  const int H = cfg.hidden_size, I = cfg.intermediate_size;
   { auto g = wc.next(); auto b = wc.next(); elng.upload(g, H); elnb.upload(b, H); }
   layers.resize(cfg.num_layers);
   for (auto& Ly : layers) {

@@ -1,5 +1,5 @@
 // Pieces shared by the two CLAP towers of the candidate scorer (clap.cu: the masked BERT text tower, clap_score.cu:
-// the Cnn14 audio tower), and the BERT trunk LASSNet's text encoder (lass.cu) runs.
+// the Cnn14 audio tower), and the BERT trunk LASSNet's text encoder (lass.cu) and wav2vec2's encoder (w2v.cu) run.
 #pragma once
 #include "common.cuh"
 #include "tapconv.cuh"
@@ -35,6 +35,8 @@ struct ClapNet : Handle {
 
   // consumes the BertModel keys of embeddings.* and encoder.layer.* (the clap_param_shapes order) for cfg
   void load_bert(WeightCursor& wc);
+  // consumes the embeddings LayerNorm and the encoder layers only (load_bert's tail; wav2vec2's encoder in w2v.cu)
+  void load_trunk(WeightCursor& wc);
   void ensure_work(long rows);
   void encode(const int* ids, int N, int L, float* z, cudaStream_t st);
   // TextEncoder.forward of the scorer: BertModel(input_ids, token_type_ids, attention_mask)[0][:, 0] -> Projection,

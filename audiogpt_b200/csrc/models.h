@@ -109,6 +109,12 @@ void binaural_frames(Handle* h, const float* view, const agpt_binaural_row* rows
 void binaural_warp(Handle* h, const float* field, const float* mono, const agpt_binaural_row* rows, int n, float* out, int clamp,
                    cudaStream_t st);
 
+Handle* w2v_create(const agpt_w2v_cfg* cfg, const float* const* W, int nW, int device);
+void w2v_lengths(const agpt_w2v_cfg* cfg, long S, int* frames);
+void w2v_logits(Handle* h, const float* x, int B, long S, float* logits, cudaStream_t st);
+void w2v_features(Handle* h, const float* x, int B, long S, float* feats, cudaStream_t st);
+void w2v_pos_conv(Handle* h, const float* x, int B, int T, float* y, cudaStream_t st);
+
 void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);
 
 }  // namespace agpt

@@ -1775,3 +1775,175 @@ def binaural_chunks(L: int, Kv: int, chunk_size: int = 48000, rec_field: int = 8
         rows.append(dict(mono_off=m0, T=T, view_off=vs + min(v0, kv), K=max(0, v1 - v0), keep=keep, out_off=out))
         out += T - keep
     return out, rows
+
+
+# --------------------------------------------------------------------------------------------------- wav2vec2 ASR
+# transformers' Wav2Vec2ForCTC with facebook/wav2vec2-base-960h's config (the Wav2Vec2Config() defaults): the model
+# GenerSpeechInfer.preprocess_input transcribes the reference clip with (NeuralSeq/inference/tts/base_tts_infer.py:38-42,
+# 83-101).  Keys are Wav2Vec2Config's attribute names.
+W2V_BASE = dict(conv_dim=(512,) * 7, conv_kernel=(10, 3, 3, 3, 3, 2, 2), conv_stride=(5, 2, 2, 2, 2, 2, 2),
+                hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072,
+                num_conv_pos_embeddings=128, num_conv_pos_embedding_groups=16, vocab_size=32, layer_norm_eps=1e-5,
+                feat_extract_norm="group", do_stable_layer_norm=False, hidden_act="gelu", feat_extract_activation="gelu",
+                conv_bias=False)
+W2V_SMALL = dict(W2V_BASE, num_hidden_layers=2)     # base widths (the positional conv's 48-channel groups), 2 layers
+W2V_SR = 16000                                      # the processor's (and GenerSpeech's) sampling rate
+W2V_POS_GROUP = 48                                  # channels per positional-conv group the engine runs
+W2V_HEAD_DIMS = (8, 16, 32, 40, 64, 80, 128)        # head dims of the attention kernel
+
+
+def _w2v(cfg, key):
+    return cfg[key] if isinstance(cfg, dict) else getattr(cfg, key)
+
+
+def w2v_check(cfg):
+    """Raise ValueError unless the engine covers cfg (a W2V_* dict or a Wav2Vec2Config): the "group" feature-extractor
+    norm, post-LN layers, GELU everywhere, bias-free convs of one width, 48-channel positional-conv groups and a head dim
+    the attention kernel takes.  wav2vec2-large-960h-lv60-self (stable layer norm, LayerNorm conv encoder) is refused."""
+    def need(ok, what):
+        if not ok:
+            raise ValueError(f"audiogpt_b200.Wav2Vec2ForCTC does not cover this config: {what}")
+    need(_w2v(cfg, "feat_extract_norm") == "group", f"feat_extract_norm={_w2v(cfg, 'feat_extract_norm')!r} (needs 'group')")
+    need(not _w2v(cfg, "do_stable_layer_norm"), "do_stable_layer_norm=True (the large / lv60 layout)")
+    need(_w2v(cfg, "hidden_act") == "gelu" and _w2v(cfg, "feat_extract_activation") == "gelu", "activations other than gelu")
+    need(not _w2v(cfg, "conv_bias"), "conv_bias=True")
+    dims, ks, ss = list(_w2v(cfg, "conv_dim")), list(_w2v(cfg, "conv_kernel")), list(_w2v(cfg, "conv_stride"))
+    need(len(dims) == len(ks) == len(ss) and 1 <= len(dims) <= 8, "1..8 conv layers of matching conv_dim / kernel / stride")
+    need(len(set(dims)) == 1 and dims[0] % 32 == 0 and 32 <= dims[0] <= 1024, "conv widths must be equal (a multiple of 32, <= 1024)")
+    need(1 <= ks[0] <= 16 and 1 <= ss[0] <= 64, "conv_kernel[0] must be <= 16")
+    need(all(1 <= s <= 8 and -(-k // s) <= 12 for k, s in zip(ks[1:], ss[1:])), "conv_kernel / conv_stride past layer 0 "
+         "must give at most 12 super-row taps")
+    H, nh = int(_w2v(cfg, "hidden_size")), int(_w2v(cfg, "num_attention_heads"))
+    need(H % nh == 0 and H // nh in W2V_HEAD_DIMS, f"head dim {H / nh:g} (needs one of {W2V_HEAD_DIMS})")
+    need(H == W2V_POS_GROUP * int(_w2v(cfg, "num_conv_pos_embedding_groups")),
+         "hidden_size must be 48 * num_conv_pos_embedding_groups")
+    need(1 <= int(_w2v(cfg, "num_conv_pos_embeddings")) <= 128, "num_conv_pos_embeddings must be <= 128")
+    if not isinstance(cfg, dict):
+        need(not getattr(cfg, "add_adapter", False), "add_adapter=True")
+
+
+def w2v_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """State-dict keys and shapes of Wav2Vec2ForCTC (group-norm, post-LN layout) in state-dict order."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    dims, ks = [int(v) for v in _w2v(cfg, "conv_dim")], [int(v) for v in _w2v(cfg, "conv_kernel")]
+    H, I, K = int(_w2v(cfg, "hidden_size")), int(_w2v(cfg, "intermediate_size")), int(_w2v(cfg, "num_conv_pos_embeddings"))
+    G = int(_w2v(cfg, "num_conv_pos_embedding_groups"))
+    w = "wav2vec2."
+    s[w + "masked_spec_embed"] = (H,)
+    for i, (c, k) in enumerate(zip(dims, ks)):
+        p = f"{w}feature_extractor.conv_layers.{i}."
+        s[p + "conv.weight"] = (c, 1 if i == 0 else dims[i - 1], k)
+        if i == 0:
+            s[p + "layer_norm.weight"] = (c,); s[p + "layer_norm.bias"] = (c,)
+    C = dims[-1]
+    s[w + "feature_projection.layer_norm.weight"] = (C,); s[w + "feature_projection.layer_norm.bias"] = (C,)
+    s[w + "feature_projection.projection.weight"] = (H, C); s[w + "feature_projection.projection.bias"] = (H,)
+    p = w + "encoder.pos_conv_embed.conv."
+    s[p + "bias"] = (H,)
+    s[p + "parametrizations.weight.original0"] = (1, 1, K)
+    s[p + "parametrizations.weight.original1"] = (H, H // G, K)
+    s[w + "encoder.layer_norm.weight"] = (H,); s[w + "encoder.layer_norm.bias"] = (H,)
+    for i in range(int(_w2v(cfg, "num_hidden_layers"))):
+        p = f"{w}encoder.layers.{i}."
+        for n in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            s[f"{p}attention.{n}.weight"] = (H, H); s[f"{p}attention.{n}.bias"] = (H,)
+        s[p + "layer_norm.weight"] = (H,); s[p + "layer_norm.bias"] = (H,)
+        s[p + "feed_forward.intermediate_dense.weight"] = (I, H); s[p + "feed_forward.intermediate_dense.bias"] = (I,)
+        s[p + "feed_forward.output_dense.weight"] = (H, I); s[p + "feed_forward.output_dense.bias"] = (H,)
+        s[p + "final_layer_norm.weight"] = (H,); s[p + "final_layer_norm.bias"] = (H,)
+    s["lm_head.weight"] = (int(_w2v(cfg, "vocab_size")), H); s["lm_head.bias"] = (int(_w2v(cfg, "vocab_size")),)
+    return s
+
+
+def w2v_lengths(cfg, n_samples: int) -> List[int]:
+    """Output length of each conv of the feature encoder for n_samples of input ((T - k) // s + 1 in turn; 0 from the
+    first layer without a frame on) -- the twin of agpt_w2v_frames, whose answer is the last entry."""
+    out, t = [], int(n_samples)
+    for k, s in zip(_w2v(cfg, "conv_kernel"), _w2v(cfg, "conv_stride")):
+        t = (t - int(k)) // int(s) + 1 if t >= int(k) else 0
+        out.append(t)
+    return out
+
+
+def w2v_superrow_weight(w: torch.Tensor, stride: int) -> torch.Tensor:
+    """A stride-s Conv1d weight [Co][Ci][k] as the stride-1 conv over super-rows (s consecutive rows of [T][Ci] read as
+    one row of s Ci channels): [Co][s Ci][ceil(k / s)], tap t's channel block j holding w[:, :, t s + j] (zero past k).
+    Output row p then reads super-rows p .. p + ceil(k / s) - 1.  The engine's only copy of this packing."""
+    Co, Ci, k = w.shape
+    s = int(stride)
+    nt = -(-k // s)
+    out = w.new_zeros((Co, s, Ci, nt))
+    for t in range(nt):
+        for j in range(s):
+            if t * s + j < k:
+                out[:, j, :, t] = w[:, :, t * s + j]
+    return out.reshape(Co, s * Ci, nt)
+
+
+def w2v_fold_pos_weight(g: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+    """The positional conv's weight_norm(dim=2) folded: g v / |v|, the norm over dims (0, 1) per tap (what the module's
+    parametrization computes)."""
+    return torch._weight_norm(v, g, 2)
+
+
+def w2v_engine_cfg(cfg) -> dict:
+    """The fields of agpt_w2v_cfg for cfg (after w2v_check)."""
+    w2v_check(cfg)
+    return dict(conv_layers=len(_w2v(cfg, "conv_dim")), conv_dim=int(_w2v(cfg, "conv_dim")[0]),
+                conv_kernel=[int(v) for v in _w2v(cfg, "conv_kernel")], conv_stride=[int(v) for v in _w2v(cfg, "conv_stride")],
+                hidden_size=int(_w2v(cfg, "hidden_size")), num_layers=int(_w2v(cfg, "num_hidden_layers")),
+                num_heads=int(_w2v(cfg, "num_attention_heads")), intermediate_size=int(_w2v(cfg, "intermediate_size")),
+                num_conv_pos_embeddings=int(_w2v(cfg, "num_conv_pos_embeddings")),
+                num_conv_pos_embedding_groups=int(_w2v(cfg, "num_conv_pos_embedding_groups")),
+                vocab_size=int(_w2v(cfg, "vocab_size")), layer_norm_eps=float(_w2v(cfg, "layer_norm_eps")))
+
+
+def w2v_engine_weights(cfg, sd) -> List[torch.Tensor]:
+    """The arrays agpt_w2v_create consumes, in its order, from a Wav2Vec2ForCTC state dict: conv0 and its GroupNorm;
+    conv 1.. packed by w2v_superrow_weight; the feature projection; the positional conv's folded weight, then its bias;
+    encoder.layer_norm; per layer q, k, v (reordered from the state dict's k, v, q into the [Q | K | V] GEMM), out_proj,
+    layer_norm, intermediate_dense, output_dense, final_layer_norm; lm_head.  masked_spec_embed (training only) is
+    left out."""
+    w = "wav2vec2."
+    out = []
+    fe = w + "feature_extractor.conv_layers."
+    out += [sd[fe + "0.conv.weight"], sd[fe + "0.layer_norm.weight"], sd[fe + "0.layer_norm.bias"]]
+    for i, s in enumerate(_w2v(cfg, "conv_stride")):
+        if i:
+            out.append(w2v_superrow_weight(sd[f"{fe}{i}.conv.weight"], int(s)))
+    fp = w + "feature_projection."
+    out += [sd[fp + "layer_norm.weight"], sd[fp + "layer_norm.bias"], sd[fp + "projection.weight"], sd[fp + "projection.bias"]]
+    pc = w + "encoder.pos_conv_embed.conv."
+    out += [w2v_fold_pos_weight(sd[pc + "parametrizations.weight.original0"], sd[pc + "parametrizations.weight.original1"]),
+            sd[pc + "bias"]]
+    out += [sd[w + "encoder.layer_norm.weight"], sd[w + "encoder.layer_norm.bias"]]
+    for i in range(int(_w2v(cfg, "num_hidden_layers"))):
+        p = f"{w}encoder.layers.{i}."
+        for n in ("attention.q_proj", "attention.k_proj", "attention.v_proj", "attention.out_proj", "layer_norm",
+                  "feed_forward.intermediate_dense", "feed_forward.output_dense", "final_layer_norm"):
+            out += [sd[f"{p}{n}.weight"], sd[f"{p}{n}.bias"]]
+    out += [sd["lm_head.weight"], sd["lm_head.bias"]]
+    return out
+
+
+def synth_w2v(cfg, seed: int = 2626):
+    """Seeded Wav2Vec2ForCTC weights (synth_state_dict) with He-gain feature-encoder convs, so the GELU stack keeps its
+    scale, and positional weight-norm gains g in [1.5, 2.5], so that conv is O(1) next to the projection it is added to."""
+    sd = synth_state_dict(w2v_param_shapes(cfg), seed, convtranspose_prefixes=(),
+                          gains={"wav2vec2.feature_extractor.conv_layers.": math.sqrt(2.0)})
+    k = "wav2vec2.encoder.pos_conv_embed.conv.parametrizations.weight.original0"
+    sd[k] = 1.5 + torch.rand(sd[k].shape, generator=torch.Generator().manual_seed(int(seed) + 1))
+    return sd
+
+
+def synth_w2v_wav(n_samples: int, seed: int, B: int = 1, offset: float = 0.0) -> torch.Tensor:
+    """Seeded input_values [B][n_samples] as the base-960h processor returns them (zero mean, unit variance per clip): a
+    few sines under a slow envelope plus noise, then offset added (a DC offset the GroupNorm statistics must survive)."""
+    rs = np.random.RandomState(int(seed))
+    t = np.arange(int(n_samples)) / float(W2V_SR)
+    out = np.empty((B, int(n_samples)))
+    for b in range(B):
+        x = sum(rs.uniform(0.2, 1.0) * np.sin(2 * np.pi * rs.uniform(80, 3000) * t + rs.uniform(0, 2 * np.pi)) for _ in range(5))
+        x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.5, 4.0) * t)) + 0.1 * rs.randn(int(n_samples))
+        out[b] = (x - x.mean()) / np.sqrt(x.var() + 1e-7)
+    return torch.from_numpy((out + offset).astype(np.float32))

@@ -634,6 +634,44 @@ int agpt_binaural_frames(agpt_handle h, const float* view, const agpt_binaural_r
 int agpt_binaural_warp(agpt_handle h, const float* field, const float* mono, const agpt_binaural_row* rows, int n_rows,
                        float* out, int clamp, void* stream);
 
+/* ------------------------------------------------------------------ Reference-audio ASR (wav2vec2 CTC)
+ * GenerSpeechInfer.preprocess_input transcribes the reference clip with transformers' Wav2Vec2ForCTC
+ * (facebook/wav2vec2-base-960h; NeuralSeq/inference/tts/base_tts_infer.py:38-42, 83-101), eval mode, no attention mask:
+ * the conv feature encoder (conv0 + GroupNorm(C groups) + GELU, then stride-s convs + GELU, no conv bias), the feature
+ * projection (LayerNorm + Linear), the weight-normed grouped positional conv (padding K / 2, SamePad, GELU) added to it,
+ * LayerNorm, post-LN encoder layers (exact GELU) and lm_head.  Only that layout is covered ("group" feature-extractor
+ * norm, no stable layer norm); the drop-in rejects the others.  A tagged struct, as agpt_clap_cfg.                 */
+#define AGPT_W2V_MAX_CONV 8
+typedef struct agpt_w2v_cfg {
+  int conv_layers;                    /* 7 */
+  int conv_dim;                       /* 512: the width of every conv (a multiple of 32, at most 1024) */
+  int conv_kernel[AGPT_W2V_MAX_CONV]; /* 10, 3, 3, 3, 3, 2, 2 (conv_kernel[0] <= 16) */
+  int conv_stride[AGPT_W2V_MAX_CONV]; /* 5, 2, 2, 2, 2, 2, 2 */
+  int hidden_size;                    /* 768 */
+  int num_layers;                     /* 12 */
+  int num_heads;                      /* 12: head dim 64 */
+  int intermediate_size;              /* 3072 */
+  int num_conv_pos_embeddings;        /* 128: the positional conv's taps (<= 128) */
+  int num_conv_pos_embedding_groups;  /* 16: hidden_size = 48 * groups */
+  int vocab_size;                     /* 32: lm_head's width */
+  float layer_norm_eps;               /* 1e-5 (the GroupNorm's eps is nn.GroupNorm's 1e-5) */
+} agpt_w2v_cfg;
+/* host_weights: fp32 HOST arrays in the order of audiogpt_b200.specs.w2v_engine_weights(cfg, state_dict): conv0 weight,
+ * GroupNorm weight / bias, conv 1.. as super-row weights [C][s C][ceil(k / s)], the projection's LayerNorm and Linear,
+ * the positional conv's folded weight g v / |v| [H][48][K] and bias, encoder.layer_norm, each layer's q, k, v, out_proj,
+ * layer_norm, intermediate_dense, output_dense, final_layer_norm (weight, bias each), lm_head weight / bias.           */
+int agpt_w2v_create(const agpt_w2v_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* Host only: the frames an input of n_samples yields (the conv lengths (T - k) / s + 1 in turn; 0 when a layer has none). */
+int agpt_w2v_frames(const agpt_w2v_cfg* cfg, long n_samples, int* frames);
+/* input_values [B][n_samples] (device) -> logits [B][frames][vocab_size] (device).  frames >= 1.  Work buffers belong
+ * to the handle: calls on one handle must be ordered on one stream.                                                 */
+int agpt_w2v_logits(agpt_handle h, const float* input_values, int B, long n_samples, float* logits, void* stream);
+/* The stages apart (the unit tests' entry points).  features: the conv feature encoder's output, channels last
+ * [B][frames][conv_dim].  pos_conv: hidden [B][T][H] -> out = hidden + gelu(pos_conv(hidden)) [B][T][H] (not aliased;
+ * hidden 16-byte and out 8-byte aligned).                                                                            */
+int agpt_w2v_features(agpt_handle h, const float* input_values, int B, long n_samples, float* features, void* stream);
+int agpt_w2v_pos_conv(agpt_handle h, const float* hidden, int B, int T, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
