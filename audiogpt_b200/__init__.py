@@ -25,6 +25,9 @@ Drop-in classes (same names / signatures / state-dict layouts as the reference):
                                                                     (installed with install(target_detection=True))
     audiogpt_b200.mono2binaural.src.models.BinauralNetwork          (installed with install(binaural=True))
     audiogpt_b200.inference.tts.base_tts_infer.Wav2Vec2ForCTC       (installed with install(asr=True))
+    audiogpt_b200.data_gen.tts.emotion.model.EmotionEncoder         (installed with install(emotion=True))
+    audiogpt_b200.data_gen.tts.emotion.inference.embed_utterance / embed_frames_batch
+                                                                    (installed with install(emotion=True))
 
 All arithmetic lives in libagpt_b200.so (audiogpt_b200/csrc, C ABI in include/agpt_b200.h).
 There is no CPU fallback.
@@ -95,6 +98,14 @@ _ASR_MAP = {
     "inference.tts.base_tts_infer": ("audiogpt_b200.inference.tts.base_tts_infer", ["Wav2Vec2ForCTC"]),
 }
 
+# the TTS_OOD tool's emotion encoder, grafted only on request (install(emotion=True)).  The inference module also holds
+# preprocess_wav and load_model, which stay the reference's, so both modules are patched in place, never aliased.
+_EMOTION_MAP = {
+    "data_gen.tts.emotion.model": ("audiogpt_b200.data_gen.tts.emotion.model", ["EmotionEncoder"]),
+    "data_gen.tts.emotion.inference": ("audiogpt_b200.data_gen.tts.emotion.inference",
+                                       ["EmotionEncoder", "embed_frames_batch", "embed_utterance"]),
+}
+
 # the Binaural tool's BinauralNetwork, grafted only on request (install(binaural=True)).  The tool imports it as
 # ``src.models`` (mono2binaural/ on its sys.path), a generic name: the module is patched in place only when it is the
 # reference's (it defines Warpnet and BinauralNetwork), and never aliased.
@@ -105,7 +116,7 @@ _BINAURAL_MAP = {
 
 def install(strict: bool = False, front_end: bool = False, first_stage: bool = False, inpaint: bool = False,
             text_encoder: bool = False, scorer: bool = False, tts_ood: bool = False, extraction: bool = False, detection: bool = False,
-            target_detection: bool = False, binaural: bool = False, asr: bool = False):
+            target_detection: bool = False, binaural: bool = False, asr: bool = False, emotion: bool = False):
     """Make AudioGPT's tool classes pick up this back-end.
 
     Call once, after the reference's packages are importable (``sys.path`` contains
@@ -144,6 +155,12 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
     ``Wav2Vec2ForCTC.from_pretrained`` builds the drop-in and the TTS_OOD tool's reference-audio transcription runs on the
     engine.  Like ``target_detection``, the module is only patched in place (it also holds BaseTTSInfer): when it does not
     import it is reported as skipped (and raises under ``strict``), never aliased.
+    ``emotion=True`` also replaces ``data_gen.tts.emotion.model.EmotionEncoder`` and, in
+    ``data_gen.tts.emotion.inference``, ``EmotionEncoder``, ``embed_frames_batch`` and ``embed_utterance``: the reference's
+    load_model then builds the drop-in, and the TTS_OOD tool's emo_embed runs on the engine.  inference/tts/GenerSpeech.py
+    binds ``embed_utterance`` by name when it is imported, so call install before that module is loaded (when it already
+    is, its ``Embed_utterance`` is rebound too).  Like ``asr``, the modules are only patched in place: when one does not
+    import (it needs webrtcvad, librosa and matplotlib) it is reported as skipped (and raises under ``strict``).
     ``binaural=True`` also replaces ``src.models.BinauralNetwork`` (mono2binaural/src/models.py), so the Binaural tool's
     geometric and neural time warp run on the engine.  ``src`` is a generic name, so the module is patched in place only
     when it is the reference's (it defines ``Warpnet`` and ``BinauralNetwork``); when it does not import or is some other
@@ -182,7 +199,8 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
                 mine._reference_cls = theirs
             setattr(ref, a, mine)
         patched.append(ref_name)
-    in_place = dict(**(_TARGET_DETECTION_MAP if target_detection else {}), **(_ASR_MAP if asr else {}))
+    in_place = dict(**(_TARGET_DETECTION_MAP if target_detection else {}), **(_ASR_MAP if asr else {}),
+                    **(_EMOTION_MAP if emotion else {}))
     if in_place:
         for ref_name, (our_name, attrs) in in_place.items():
             ours = importlib.import_module(our_name)
@@ -195,6 +213,11 @@ def install(strict: bool = False, front_end: bool = False, first_stage: bool = F
                 continue
             for a in attrs:
                 setattr(ref, a, getattr(ours, a))
+            if ref_name == "data_gen.tts.emotion.inference":
+                ours._state = ref    # the reference's load_model stores the model there
+                tool = sys.modules.get("inference.tts.GenerSpeech")
+                if tool is not None:
+                    tool.Embed_utterance = ours.embed_utterance
             patched.append(ref_name)
     if binaural:
         for ref_name, (our_name, attrs) in _BINAURAL_MAP.items():

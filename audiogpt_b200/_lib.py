@@ -131,6 +131,11 @@ class W2vConfig(C.Structure):
         "num_conv_pos_embedding_groups", "vocab_size")] + [("layer_norm_eps", C.c_float)]
 
 
+class EmoConfig(C.Structure):
+    """agpt_emo_cfg (a tagged struct in the header, like agpt_clap_cfg; the create entry point takes a plain pointer)."""
+    _fields_ = [(n, C.c_int) for n in ("input_size", "hidden_size", "num_layers", "embedding_size")]
+
+
 class TapconvProbeArgs(C.Structure):
     """agpt_tapconv_probe_args (a tagged struct in the header: it carries pointers and floats)."""
     _fields_ = [(n, C.c_int) for n in ("kind", "Cin", "Cout", "K", "dil", "Wreal", "strip_w", "u", "pad", "g")] + [
@@ -241,6 +246,13 @@ PROTOTYPES = {
     "agpt_w2v_logits": (_I, [_P, _P, _I, _L, _P, _P]),
     "agpt_w2v_features": (_I, [_P, _P, _I, _L, _P, _P]),
     "agpt_w2v_pos_conv": (_I, [_P, _P, _I, _I, _P, _P]),
+    "agpt_emo_create": (_I, [_P, _W, _I, _I, _OUT]),
+    "agpt_emo_partials": (_I, [_L, _I, _D, _D, _P, _P, _P]),
+    "agpt_emo_embed": (_I, [_P, _P, _L, _I, _D, _D, _P, _P, _P]),
+    "agpt_emo_hidden": (_I, [_P, _P, _I, _I, _P, _P]),
+    "agpt_emo_forward": (_I, [_P, _P, _I, _I, _P, _P]),
+    "agpt_emo_mel": (_I, [_P, _P, _L, _P, _P]),
+    "agpt_emo_lstm": (_I, [_P, _P, _I, _I, _L, _P, _P, _P]),
 }
 
 _lock = threading.Lock()

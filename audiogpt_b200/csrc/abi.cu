@@ -605,6 +605,58 @@ int agpt_w2v_pos_conv(agpt_handle h, const float* hidden, int B, int T, float* o
   });
 }
 
+int agpt_emo_create(const agpt_emo_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out) {
+  return guarded([&] {
+    AGPT_CHECK(cfg && host_weights && out, "null argument");
+    *out = reinterpret_cast<agpt_handle>(emo_create(cfg, host_weights, n_weights, device));
+  });
+}
+
+int agpt_emo_partials(long n_samples, int partial_frames, double min_pad_coverage, double overlap, int* n_partials, int* frame_step,
+                      long* padded) {
+  return guarded([&] {
+    AGPT_CHECK(n_partials && frame_step && padded, "null argument");
+    emo_partials(n_samples, partial_frames, min_pad_coverage, overlap, n_partials, frame_step, padded);
+  });
+}
+
+int agpt_emo_embed(agpt_handle h, const float* wav, long n_samples, int partial_frames, double min_pad_coverage, double overlap,
+                   float* embed, float* partials, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(wav && embed, "null argument");
+    emo_embed(as(h, kMagicEmo, "emotion"), wav, n_samples, partial_frames, min_pad_coverage, overlap, embed, partials,
+              (cudaStream_t)stream);
+  });
+}
+
+int agpt_emo_hidden(agpt_handle h, const float* frames, int N, int T, float* hidden, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(frames && hidden, "null argument");
+    emo_hidden(as(h, kMagicEmo, "emotion"), frames, N, T, hidden, (cudaStream_t)stream);
+  });
+}
+
+int agpt_emo_forward(agpt_handle h, const float* frames, int N, int T, float* embeds, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(frames && embeds, "null argument");
+    emo_forward(as(h, kMagicEmo, "emotion"), frames, N, T, embeds, (cudaStream_t)stream);
+  });
+}
+
+int agpt_emo_mel(agpt_handle h, const float* wav, long n_samples, float* mel, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(wav && mel, "null argument");
+    emo_mel(as(h, kMagicEmo, "emotion"), wav, n_samples, mel, (cudaStream_t)stream);
+  });
+}
+
+int agpt_emo_lstm(const float* w_hh, const float* xproj, int N, int T, long seq_stride, float* h_seq, float* h_last, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(w_hh && xproj, "null argument");
+    emo_lstm(w_hh, xproj, N, T, seq_stride, h_seq, h_last, (cudaStream_t)stream);
+  });
+}
+
 int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream) {
   return guarded([&] {
     AGPT_CHECK(args && ran, "null argument");

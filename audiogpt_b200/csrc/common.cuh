@@ -112,6 +112,7 @@ constexpr uint32_t kMagicPvt = 0x50565432;      // 'PVT2'
 constexpr uint32_t kMagicTsd = 0x54534430;      // 'TSD0'
 constexpr uint32_t kMagicBinaural = 0x42494e30; // 'BIN0'
 constexpr uint32_t kMagicW2v = 0x57325643;      // 'W2VC'
+constexpr uint32_t kMagicEmo = 0x454d4f30;      // 'EMO0'
 
 // ---- small device functions --------------------------------------------------
 __device__ __forceinline__ float lrelu(float x, float a) { return x > 0.f ? x : a * x; }

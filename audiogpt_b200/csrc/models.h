@@ -115,6 +115,16 @@ void w2v_logits(Handle* h, const float* x, int B, long S, float* logits, cudaStr
 void w2v_features(Handle* h, const float* x, int B, long S, float* feats, cudaStream_t st);
 void w2v_pos_conv(Handle* h, const float* x, int B, int T, float* y, cudaStream_t st);
 
+Handle* emo_create(const agpt_emo_cfg* cfg, const float* const* W, int nW, int device);
+void emo_partials(long n_samples, int partial_frames, double min_pad_coverage, double overlap, int* n_partials, int* frame_step,
+                  long* padded);
+void emo_mel(Handle* h, const float* wav, long n, float* mel, cudaStream_t st);
+void emo_lstm(const float* whh, const float* xp, int N, int T, long seq_stride, float* h_seq, float* h_last, cudaStream_t st);
+void emo_hidden(Handle* h, const float* frames, int N, int T, float* hidden, cudaStream_t st);
+void emo_forward(Handle* h, const float* frames, int N, int T, float* embeds, cudaStream_t st);
+void emo_embed(Handle* h, const float* wav, long n, int partial_frames, double min_pad_coverage, double overlap, float* embed,
+               float* partials, cudaStream_t st);
+
 void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);
 
 }  // namespace agpt

@@ -1947,3 +1947,132 @@ def synth_w2v_wav(n_samples: int, seed: int, B: int = 1, offset: float = 0.0) ->
         x = x * (0.6 + 0.4 * np.sin(2 * np.pi * rs.uniform(0.5, 4.0) * t)) + 0.1 * rs.randn(int(n_samples))
         out[b] = (x - x.mean()) / np.sqrt(x.var() + 1e-7)
     return torch.from_numpy((out + offset).astype(np.float32))
+
+
+# ------------------------------------------------------------------------------------------------ emotion encoder
+# The TTS_OOD tool's emotion encoder (NeuralSeq/data_gen/tts/emotion/: params_data.py, params_model.py, model.py,
+# inference.py, audio.py): embed_utterance's partial slices, librosa's power mel and EmotionEncoder's nn.LSTM(40, 256, 3).
+# Keys are the engine config's (agpt_emo_cfg).
+EMO = dict(input_size=40, hidden_size=256, num_layers=3, embedding_size=256)
+EMO_SR = 16000                # sampling_rate
+EMO_N_FFT = 400               # mel_window_length 25 ms (win_length = n_fft)
+EMO_HOP = 160                 # mel_window_step 10 ms
+EMO_MELS = 40                 # mel_n_channels
+EMO_PARTIAL_FRAMES = 160      # partials_n_frames
+EMO_DBFS = -30                # audio_norm_target_dBFS: the level preprocess_wav normalises to
+# librosa.feature.melspectrogram's stft padding.  audio.py passes wav and sr positionally, which only runs on librosa
+# < 0.10 (numpy is pinned to 1.23.1), and those versions pad 'reflect' (0.10 changed the default to 'constant').
+EMO_PAD_MODE = "reflect"
+
+
+def emo_check(cfg):
+    """Raise ValueError unless the engine covers cfg (an EMO-style dict): 40 mel inputs, hidden size 256, at least one
+    layer, and a linear width in [1, 4096]."""
+    if int(cfg["input_size"]) != EMO_MELS:
+        raise ValueError(f"EmotionEncoder: input_size must be {EMO_MELS} (mel_n_channels), got {cfg['input_size']}")
+    if int(cfg["hidden_size"]) != 256:
+        raise ValueError(f"EmotionEncoder: the engine's LSTM has hidden_size 256, got {cfg['hidden_size']}")
+    if not 1 <= int(cfg["num_layers"]) <= 16:
+        raise ValueError(f"EmotionEncoder: num_layers must be in [1, 16], got {cfg['num_layers']}")
+    if not 1 <= int(cfg["embedding_size"]) <= 4096:
+        raise ValueError(f"EmotionEncoder: embedding_size must be in [1, 4096], got {cfg['embedding_size']}")
+
+
+def emo_param_shapes(cfg) -> "OrderedDict[str, Tuple[int, ...]]":
+    """EmotionEncoder's state-dict keys and shapes in state-dict order: its own parameters (the similarity scaling)
+    first, then lstm (gate order i, f, g, o in every [1024] axis) and linear."""
+    s: "OrderedDict[str, Tuple[int, ...]]" = OrderedDict()
+    s["similarity_weight"] = (1,)
+    s["similarity_bias"] = (1,)
+    H, G = int(cfg["hidden_size"]), 4 * int(cfg["hidden_size"])
+    for k in range(int(cfg["num_layers"])):
+        s[f"lstm.weight_ih_l{k}"] = (G, int(cfg["input_size"]) if k == 0 else H)
+        s[f"lstm.weight_hh_l{k}"] = (G, H)
+        s[f"lstm.bias_ih_l{k}"] = (G,)
+        s[f"lstm.bias_hh_l{k}"] = (G,)
+    s["linear.weight"] = (int(cfg["embedding_size"]), H)
+    s["linear.bias"] = (int(cfg["embedding_size"]),)
+    return s
+
+
+def emo_partials(n_samples: int, partial_utterance_n_frames: int = EMO_PARTIAL_FRAMES, min_pad_coverage: float = 0.75,
+                 overlap: float = 0.5):
+    """compute_partial_slices (inference.py:59-108): (wav_slices, mel_slices), lists of slices in samples and in mel
+    frames of 160 samples -- the twin of agpt_emo_partials."""
+    assert 0 <= overlap < 1
+    assert 0 < min_pad_coverage <= 1
+    n_frames = int(np.ceil((n_samples + 1) / EMO_HOP))
+    frame_step = max(int(np.round(partial_utterance_n_frames * (1 - overlap))), 1)
+    wav_slices, mel_slices = [], []
+    steps = max(1, n_frames - partial_utterance_n_frames + frame_step + 1)
+    for i in range(0, steps, frame_step):
+        mel_slices.append(slice(i, i + partial_utterance_n_frames))
+        wav_slices.append(slice(i * EMO_HOP, (i + partial_utterance_n_frames) * EMO_HOP))
+    last = wav_slices[-1]
+    coverage = (n_samples - last.start) / (last.stop - last.start)
+    if coverage < min_pad_coverage and len(mel_slices) > 1:
+        mel_slices, wav_slices = mel_slices[:-1], wav_slices[:-1]
+    return wav_slices, mel_slices
+
+
+def emo_padded_length(n_samples: int, wav_slices) -> int:
+    """The length embed_utterance zero-pads the wav to: wav_slices[-1].stop when that is at least n_samples."""
+    return max(int(n_samples), int(wav_slices[-1].stop))
+
+
+def emo_fold_bias(b_ih: torch.Tensor, b_hh: torch.Tensor) -> torch.Tensor:
+    """The one bias of a layer's input projection: b_ih + b_hh (both are added to every gate pre-activation)."""
+    return b_ih + b_hh
+
+
+def emo_front_weights():
+    """The front end's constant arrays: the periodic-Hann DFT rows for n_fft 400, real and imaginary [201][400], and
+    librosa's Slaney mel matrix (0 .. 8 kHz, area-normalised) transposed, [201][40]."""
+    re, im = stft_dft_weights(EMO_N_FFT)
+    mel = torch.from_numpy(np.ascontiguousarray(slaney_mel(EMO_SR, EMO_N_FFT, EMO_MELS, 0.0, EMO_SR / 2.0).T))
+    return re[:, 0], im[:, 0], mel
+
+
+def emo_engine_weights(cfg, sd) -> List[torch.Tensor]:
+    """The arrays agpt_emo_create consumes, in its order: per layer weight_ih, weight_hh and the folded bias; linear's
+    weight and bias; then emo_front_weights().  The similarity scaling (training only) is left out."""
+    out = []
+    for k in range(int(cfg["num_layers"])):
+        p = "lstm."
+        out += [sd[f"{p}weight_ih_l{k}"], sd[f"{p}weight_hh_l{k}"], emo_fold_bias(sd[f"{p}bias_ih_l{k}"], sd[f"{p}bias_hh_l{k}"])]
+    out += [sd["linear.weight"], sd["linear.bias"]]
+    out += list(emo_front_weights())
+    return out
+
+
+# weight_ih_l0's gain over N(0, 1 / 40): a -30 dBFS power mel is O(1e-2), where PyTorch's own U(-1/16, 1/16) init
+# leaves every gate almost linear; this puts a real fraction of the pre-activations past |z| > 1 for synth_emotion_wav
+EMO_INPUT_GAIN = 60.0
+
+
+def synth_emotion(cfg=EMO, seed: int = 5353):
+    """Seeded EmotionEncoder weights (synth_state_dict): weight_ih_l0 at EMO_INPUT_GAIN, the deeper layers' weight_ih
+    and every weight_hh at gain 2 (so layers 1.. see O(1) pre-activations from |h| < 1), and the similarity scaling at
+    its initial values (10, -5)."""
+    # synth_state_dict applies the last matching prefix: weight_ih_l0 takes EMO_INPUT_GAIN
+    sd = synth_state_dict(emo_param_shapes(cfg), seed, convtranspose_prefixes=(),
+                          gains={"lstm.weight_ih_l": 2.0, "lstm.weight_hh_l": 2.0, "lstm.weight_ih_l0": EMO_INPUT_GAIN})
+    sd["similarity_weight"] = torch.tensor([10.0])
+    sd["similarity_bias"] = torch.tensor([-5.0])
+    return sd
+
+
+def synth_emotion_wav(n_samples: int, seed: int) -> np.ndarray:
+    """A seeded speech-like clip, float32 numpy at 16 kHz, as preprocess_wav returns one: voiced harmonics of a gliding
+    f0 (80-250 Hz) with a 1/k spectral tilt, a little noise, and a syllable-rate (3-6 Hz) envelope with short pauses,
+    normalised to -30 dBFS."""
+    rs = np.random.RandomState(int(seed))
+    n = int(n_samples)
+    t = np.arange(n) / float(EMO_SR)
+    f0 = rs.uniform(90, 200) * (1.0 + 0.15 * np.sin(2 * np.pi * rs.uniform(0.2, 0.8) * t + rs.uniform(0, 6)))
+    ph = 2 * np.pi * np.cumsum(f0) / EMO_SR
+    x = sum(np.sin(k * ph + rs.uniform(0, 6)) / k for k in range(1, 30) if k * f0.max() < 0.45 * EMO_SR)
+    env = np.maximum(0.0, np.sin(2 * np.pi * rs.uniform(3, 6) * t + rs.uniform(0, 6))) ** 0.7
+    x = x * (0.1 + env) + 0.05 * rs.randn(n)
+    x = x * 10 ** ((EMO_DBFS - 10 * np.log10(np.mean(x ** 2) + 1e-20)) / 20)
+    return x.astype(np.float32)

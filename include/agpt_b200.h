@@ -672,6 +672,47 @@ int agpt_w2v_logits(agpt_handle h, const float* input_values, int B, long n_samp
 int agpt_w2v_features(agpt_handle h, const float* input_values, int B, long n_samples, float* features, void* stream);
 int agpt_w2v_pos_conv(agpt_handle h, const float* hidden, int B, int T, float* out, void* stream);
 
+/* ------------------------------------------------------------------ Emotion encoder
+ * The TTS_OOD tool's emo_embed (NeuralSeq/inference/tts/GenerSpeech.py:37,58): data_gen/tts/emotion/inference.py
+ * embed_utterance -- the partial-utterance slices of compute_partial_slices, librosa's power mel of the zero-padded wav
+ * (n_fft 400 = win, hop 160, periodic Hann, center with reflect padding, power 2, 40 Slaney bands 0..8 kHz, no log),
+ * EmotionEncoder.inference (model.py: nn.LSTM(40, 256, num_layers, batch_first) from h0 = c0 = 0, the last layer's
+ * final h) per partial, their mean and its L2 norm.  A tagged struct, as agpt_clap_cfg.                              */
+typedef struct agpt_emo_cfg {
+  int input_size;      /* 40: mel_n_channels */
+  int hidden_size;     /* 256 */
+  int num_layers;      /* 3 (1..16) */
+  int embedding_size;  /* 256: EmotionEncoder.linear's width (forward only; 1..4096) */
+} agpt_emo_cfg;
+/* host_weights: fp32 HOST arrays in the order of audiogpt_b200.specs.emo_engine_weights(cfg, state_dict): per layer
+ * lstm.weight_ih_l{k} [1024][in], lstm.weight_hh_l{k} [1024][256], bias_ih_l{k} + bias_hh_l{k} [1024]; linear.weight
+ * [E][256] and bias [E]; the DFT rows of the periodic-Hann window, real and imaginary [201][400] each; the Slaney mel
+ * matrix transposed, [201][40].                                                                                     */
+int agpt_emo_create(const agpt_emo_cfg* cfg, const float* const* host_weights, int n_weights, int device, agpt_handle* out);
+/* Host only: compute_partial_slices(n_samples, partial_frames, min_pad_coverage, overlap) in frames of 160 samples ->
+ * the partial count, the frame step between partials (partial p is mel frames step p .. step p + partial_frames - 1)
+ * and the length embed_utterance zero-pads the wav to (wav_slices[-1].stop when that is at least n_samples, else
+ * n_samples).                                                                                                        */
+int agpt_emo_partials(long n_samples, int partial_frames, double min_pad_coverage, double overlap, int* n_partials, int* frame_step,
+                      long* padded);
+/* wav [n_samples] (device, not padded) -> embed [256] (device): embed_utterance.  partial_frames >= 1: the slices of
+ * agpt_emo_partials, and partials [n_partials][256] (device, may be NULL) receives each partial's hidden[-1];
+ * partial_frames = 0: using_partials=False, the whole mel as one sequence (then the embedding is hidden[-1] itself,
+ * not normalised, as the reference returns it).  The mel needs at least 201 samples after padding.  Work buffers
+ * belong to the handle: calls on one handle must be ordered on one stream.                                           */
+int agpt_emo_embed(agpt_handle h, const float* wav, long n_samples, int partial_frames, double min_pad_coverage, double overlap,
+                   float* embed, float* partials, void* stream);
+/* frames [N][T][40] (device) -> hidden [N][256]: EmotionEncoder.inference (the last layer's final h).              */
+int agpt_emo_hidden(agpt_handle h, const float* frames, int N, int T, float* hidden, void* stream);
+/* frames [N][T][40] (device) -> embeds [N][E]: EmotionEncoder.forward, relu(linear(hidden[-1])) / its L2 norm.      */
+int agpt_emo_forward(agpt_handle h, const float* frames, int N, int T, float* embeds, void* stream);
+/* The stages apart (the unit tests' entry points).  mel: wav [n_samples] (device, n_samples >= 201) -> mel
+ * [n_samples / 160 + 1][40], wav_to_mel_spectrogram.  lstm: one layer's recurrence, no handle: w_hh [1024][256], xproj
+ * [.][1024] the input projections W_ih x + b_ih + b_hh, sequence n's step t at row n * seq_stride + t -> h_seq
+ * [N][T][256] every step's h and h_last [N][256] the final h (either may be NULL, not both).                          */
+int agpt_emo_mel(agpt_handle h, const float* wav, long n_samples, float* mel, void* stream);
+int agpt_emo_lstm(const float* w_hh, const float* xproj, int N, int T, long seq_stride, float* h_seq, float* h_last, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
