@@ -154,6 +154,21 @@ class TapconvProbeArgs(C.Structure):
         ("w2", C.c_void_p), ("b2", C.c_void_p), ("K2", C.c_int), ("dil2", C.c_int)]
 
 
+# agpt_nn_probe_args.op, in the header's enum order (AGPT_NN_<name>)
+NN_OPS = ("GROUPNORM", "LAYERNORM", "SOFTMAX_ROWS", "TRANSPOSE_PAD", "COPY_PAD_ROWS", "CONCAT", "UPSAMPLE2", "AVGPOOL2",
+          "IM2COL_S2", "CF_TO_CL_PAD", "TIMESTEP", "TIMESTEP_DEV", "DDIM_TAB", "CONV_OUT_DDIM")
+
+
+class NnProbeArgs(C.Structure):
+    """agpt_nn_probe_args (a tagged struct in the header: it carries pointers and floats)."""
+    _fields_ = [("op", C.c_int)] + [(n, C.c_void_p) for n in (
+        "x", "x2", "y", "y2", "gamma", "beta", "w", "b", "table", "step", "sel_table", "sel_out")] + [
+        ("sel_cols", C.c_int), ("t", C.c_void_p)] + [(n, C.c_int) for n in (
+        "N", "H", "W", "C", "C2", "G", "act", "pad", "Nsrc", "single")] + [
+        ("rows", C.c_long), ("cols", C.c_int), ("pitch", C.c_int), ("rows_pad", C.c_int),
+        ("eps", C.c_float), ("scale", C.c_float)]
+
+
 # (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
 # takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
 _I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
@@ -179,6 +194,7 @@ PROTOTYPES = {
     "agpt_set_attention_tc": (_I, [_I]),
     "agpt_attention_masked": (_I, [_P, _I, _P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "agpt_tapconv_probe": (_I, [_P, _P, _P]),
+    "agpt_nn_probe": (_I, [_P, _P]),
     "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
     "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "agpt_hifigan_vocode_host": (_I, [_P, _P, _P, _I, _I, _P]),

@@ -664,4 +664,11 @@ int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* st
   });
 }
 
+int agpt_nn_probe(const agpt_nn_probe_args* args, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(args, "null argument");
+    nn_probe(*args, (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

@@ -1,6 +1,8 @@
-// Conformance entry: one production launch of the tap-GEMM primitive on caller-owned tensors (tapconv_probe).
+// Conformance entries: one production launch of the tap-GEMM primitive (tapconv_probe) or of a non-contraction
+// kernel (nn_probe) on caller-owned tensors.
 #include "tapconv.cuh"
 #include "models.h"
+#include "nn_kernels.h"
 
 namespace agpt {
 
@@ -78,6 +80,39 @@ void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st
   }
   tc_set_enabled(tc_prev ? 1 : 0);
   tapconv_last_launch(ran);
+}
+
+// One call of a production nn_kernels.cu launcher on caller-owned tensors (agpt_nn_probe, include/agpt_b200.h).
+void nn_probe(const agpt_nn_probe_args& a, cudaStream_t st) {
+  const int HW = a.H * a.W;
+  switch (a.op) {
+    case AGPT_NN_GROUPNORM:
+      groupnorm_ex(a.x, a.y, a.gamma, a.beta, a.N, (int)a.rows, a.C, a.G, a.eps, a.act, a.x2, st); break;
+    case AGPT_NN_LAYERNORM: layernorm(a.x, a.y, a.gamma, a.beta, a.rows, a.C, a.eps, st); break;
+    case AGPT_NN_SOFTMAX_ROWS: softmax_rows(a.y, a.pitch, a.rows, a.cols, a.scale, st); break;
+    case AGPT_NN_TRANSPOSE_PAD: transpose_pad(a.x, a.pitch, (int)a.rows, a.cols, a.y, a.rows_pad, st); break;
+    case AGPT_NN_COPY_PAD_ROWS: copy_pad_rows(a.x, a.pitch, (int)a.rows, a.cols, a.y, a.rows_pad, st); break;
+    case AGPT_NN_CONCAT: concat_channels(a.x, a.C, a.x2, a.C2, a.y, a.rows, st); break;
+    case AGPT_NN_UPSAMPLE2: upsample_nearest2(a.x, a.y, a.N, a.H, a.W, a.C, st); break;
+    case AGPT_NN_AVGPOOL2: avgpool2(a.x, a.y, a.N, a.H, a.W, a.C, st); break;
+    case AGPT_NN_IM2COL_S2: {
+      const int Ho = a.pad ? (a.H - 1) / 2 + 1 : a.H / 2, Wo = a.pad ? (a.W - 1) / 2 + 1 : a.W / 2;
+      im2col_stride2(a.x, a.y, a.N, a.H, a.W, a.C, Ho, Wo, a.pad, st);
+      break;
+    }
+    case AGPT_NN_CF_TO_CL_PAD: cf_to_cl_pad(a.x, a.y, a.N, a.C, a.pitch, HW, st, a.Nsrc); break;
+    case AGPT_NN_TIMESTEP: timestep_embedding(a.y, a.t, a.N, a.C, st); break;
+    case AGPT_NN_TIMESTEP_DEV: timestep_embedding_dev(a.y, a.t, a.N, a.C, st); break;
+    case AGPT_NN_DDIM_TAB:
+      select_row(a.sel_table, a.step, a.sel_out, a.sel_cols, st);
+      ddim_update_tab(a.x, a.x2, a.single, a.table, a.step, a.N, a.rows, a.y, a.y2, st);
+      step_inc(a.step, st);
+      break;
+    case AGPT_NN_CONV_OUT_DDIM:
+      conv_out_ddim(a.x, a.w, a.b, a.y, a.y2, a.table, a.step, a.N, a.H, a.W, a.C, a.single, st); break;
+    default: throw Error("nn probe: unknown op " + std::to_string(a.op));
+  }
+  AGPT_CUDA(cudaStreamSynchronize(st));
 }
 
 }  // namespace agpt

@@ -104,6 +104,48 @@ typedef struct agpt_tapconv_probe_args {
 /* ran = what actually launched: {1 tensor-core | 0 fp32-FMA, tile width BN, tile height MT, 1 plane-fed}.
  * Synchronises `stream` before returning.                                                                   */
 int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream);
+/* Conformance entry of the non-contraction kernels (nn_kernels.cu, tests/test_nn_kernels_gpu.py): ONE call of the
+ * production launcher selected by `op` on caller-owned device tensors, with the arguments as given.  All tensors are
+ * fp32 device arrays unless marked host; the fields each op reads:
+ *   GROUPNORM      groupnorm_ex: x [N][rows][C] -> y, gamma / beta [C], G, eps, act (0 none, 1 SiLU, 2 ReLU),
+ *                  x2 = residual added after the activation (NULL = none)
+ *   LAYERNORM      layernorm: x [rows][C] -> y, gamma / beta [C], eps
+ *   SOFTMAX_ROWS   softmax_rows: y [rows][pitch] in place, softmax over the first cols after scaling by scale
+ *   TRANSPOSE_PAD  transpose_pad: x [rows][pitch] (cols used) -> y [cols][rows_pad]
+ *   COPY_PAD_ROWS  copy_pad_rows: x [rows][pitch] (cols used) -> y [rows_pad][cols]
+ *   CONCAT         concat_channels: x [rows][C], x2 [rows][C2] -> y [rows][C + C2]
+ *   UPSAMPLE2      upsample_nearest2: x [N][H][W][C] -> y [N][2H][2W][C]
+ *   AVGPOOL2       avgpool2: x [N][H][W][C] -> y [N][H/2][W/2][C]
+ *   IM2COL_S2      im2col_stride2: x [N][H][W][C] -> y [N][Ho][Wo][9][C]; pad 1: Ho = (H - 1) / 2 + 1 (Conv2d k3 s2
+ *                  p1), pad 0: Ho = H / 2 (the VAE encoder's pad-after Downsample); likewise Wo
+ *   CF_TO_CL_PAD   cf_to_cl_pad: x [Nsrc][C][H*W] -> y [N][H*W][pitch], sample n reads source n % Nsrc (0 = N)
+ *   TIMESTEP       timestep_embedding: t HOST [N] -> y [N][C]
+ *   TIMESTEP_DEV   timestep_embedding_dev: t device [N] -> y [N][C]
+ *   DDIM_TAB       select_row(sel_table [..][sel_cols] -> sel_out), ddim_update_tab(x [N][rows], x2 = eps [N or 2N][rows],
+ *                  single, table = coefficients [steps][6] at *step) -> y = x_prev (may be x), y2 = pred_x0 (NULL = none),
+ *                  then step_inc(step)
+ *   CONV_OUT_DDIM  conv_out_ddim: x = normalised activation [N or 2N][H*W][C], w [9][C][4], b [4], y = the latent
+ *                  [N][4][H*W] updated in place, y2 = pred_x0 (NULL = none), single, table / step as DDIM_TAB
+ * Synchronises `stream` before returning.                                                                      */
+enum {
+  AGPT_NN_GROUPNORM = 0, AGPT_NN_LAYERNORM, AGPT_NN_SOFTMAX_ROWS, AGPT_NN_TRANSPOSE_PAD, AGPT_NN_COPY_PAD_ROWS,
+  AGPT_NN_CONCAT, AGPT_NN_UPSAMPLE2, AGPT_NN_AVGPOOL2, AGPT_NN_IM2COL_S2, AGPT_NN_CF_TO_CL_PAD, AGPT_NN_TIMESTEP,
+  AGPT_NN_TIMESTEP_DEV, AGPT_NN_DDIM_TAB, AGPT_NN_CONV_OUT_DDIM
+};
+typedef struct agpt_nn_probe_args {
+  int op;
+  const float* x; const float* x2;
+  float* y; float* y2;
+  const float* gamma; const float* beta;
+  const float* w; const float* b;
+  const float* table; int* step;
+  const float* sel_table; float* sel_out; int sel_cols;
+  const int* t;
+  int N, H, W, C, C2, G, act, pad, Nsrc, single;
+  long rows; int cols, pitch, rows_pad;
+  float eps, scale;
+} agpt_nn_probe_args;
+int agpt_nn_probe(const agpt_nn_probe_args* args, void* stream);
 
 /* ------------------------------------------------------------------ HiFi-GAN
  * Replaces HifiGanGenerator.__init__/forward/remove_weight_norm

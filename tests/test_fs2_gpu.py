@@ -109,44 +109,54 @@ def test_cpu_tensor_raises():
         m(torch.ones(1, 4, dtype=torch.long))
 
 
-def _masked_attention(q, kv, mask, N, heads, d, Lq, Lk):
+def _masked_attention(ptrs, mask, N, heads, d, Lq, Lk):
+    qp, q_pitch, kp, vp, kv_pitch = ptrs
     L = _lib.lib()
     C_ = heads * d
     o = torch.full((N, Lq, C_), float("nan"), device="cuda")
-    _lib.check(L.agpt_attention_masked(_lib.fptr(q), C_, _lib.fptr(kv), 2 * C_, C.c_void_p(kv.data_ptr() + 4 * C_), 2 * C_,
-                                       _lib.fptr(mask), _lib.fptr(o), C_, N, heads, d, Lq, Lk, _lib.cur_stream()))
+    _lib.check(L.agpt_attention_masked(qp, q_pitch, kp, kv_pitch, vp, kv_pitch, _lib.fptr(mask), _lib.fptr(o), C_, N, heads,
+                                       d, Lq, Lk, _lib.cur_stream()))
     torch.cuda.synchronize()
     return o.cpu()
 
 
+# kind -> (Lq, Lk, operand layout of test_ldm_gpu.attention_operands)
+MASK_KINDS = {"suffix": (150, 150, "kv"), "scattered": (150, 150, "kv"), "prefix": (150, 150, "kv"),
+              "packed": (150, 150, "packed"), "peaky": (150, 150, "peaky"), "lq1": (1, 150, "kv"), "lk1": (70, 1, "kv"),
+              "lk65": (65, 65, "packed")}
+
+
 @pytest.mark.parametrize("d", [40, 128])
-@pytest.mark.parametrize("kind", ["suffix", "scattered"])
+@pytest.mark.parametrize("kind", list(MASK_KINDS))
 def test_masked_attention_vs_fp64(d, kind):
     """agpt_attention_masked against the fp64 masked softmax, on the wgmma kernel and on the fp32 kernel
-    (AGPT_ATTN_TC=0); sample 2 has every key masked and must come out as zeros.  rel-RMSE <= 1e-5."""
-    N, heads, Lq, Lk = 3, 2, 150, 150
+    (AGPT_ATTN_TC=0); sample 2 has every key masked and must come out as zeros.  Suffix, scattered and prefix masks
+    (the whole first 64-key block, then live keys), packed q | k | v rows, peaky scores, Lq = 1, Lk = 1, Lk = 65.
+    rel-RMSE <= 1e-5."""
+    from test_ldm_gpu import attention_operands
+    N, heads = 3, 2
+    Lq, Lk, layout = MASK_KINDS[kind]
     C_ = heads * d
-    q = specs.synth_tensor((N, Lq, C_), seed=11).cuda()
-    kv = specs.synth_tensor((N, Lk, 2 * C_), seed=12).cuda()
+    ptrs, (qh, kh, vh), _keep = attention_operands(N, heads, d, Lq, Lk, layout, 11)
     mask = torch.zeros(N, Lk, dtype=torch.uint8)
-    if kind == "suffix":
-        mask[0, 100:] = 1
-        mask[1, 7:] = 1
-    else:
+    if kind == "scattered":
         g = torch.Generator().manual_seed(5)
         mask[:2] = (torch.rand(2, Lk, generator=g) < 0.4).to(torch.uint8)
         mask[0, 64:128] = 1                                   # a whole 64-key block masked
+    elif kind == "prefix":
+        mask[:2, :64] = 1
+        mask[1, 64:70] = 1
+    elif Lk > 1:
+        mask[0, Lk * 2 // 3:] = 1
+        mask[1, 7:] = 1
     mask[2] = 1
-    qh = q.double().cpu().reshape(N, Lq, heads, d).permute(0, 2, 1, 3)
-    kh = kv[:, :, :C_].double().cpu().reshape(N, Lk, heads, d).permute(0, 2, 1, 3)
-    vh = kv[:, :, C_:].double().cpu().reshape(N, Lk, heads, d).permute(0, 2, 1, 3)
     s = (qh @ kh.transpose(-1, -2) * d ** -0.5).masked_fill(mask.bool()[:, None, None, :], float("-inf"))
     ref = (torch.softmax(s, dim=-1) @ vh).permute(0, 2, 1, 3).reshape(N, Lq, C_)
     L = _lib.lib()
     for tc in (1, 0):
         _lib.check(L.agpt_set_attention_tc(tc))
         try:
-            o = _masked_attention(q, kv, mask.cuda(), N, heads, d, Lq, Lk)
+            o = _masked_attention(ptrs, mask.cuda(), N, heads, d, Lq, Lk)
         finally:
             _lib.check(L.agpt_set_attention_tc(-1))
         assert torch.equal(o[2], torch.zeros_like(o[2])), tc

@@ -379,20 +379,41 @@ def test_bench_reference_arm_contract():
     assert r1.returncode == 0 and r1.stdout.strip() == ""
 
 
-def test_tapconv_probe_args_mirror_the_header():
-    """_lib.TapconvProbeArgs has the fields of agpt_tapconv_probe_args in the header's order and C types (a mismatch
-    would hand the probe shifted launch parameters)."""
-    from audiogpt_b200 import _lib
-    hdr = re.sub(r"/\*.*?\*/", " ", open(os.path.join(ROOT, "include", "agpt_b200.h")).read(), flags=re.S)
-    body = re.search(r"typedef struct agpt_tapconv_probe_args \{(.*?)\}\s*agpt_tapconv_probe_args;", hdr, re.S).group(1)
+def _header():
+    return re.sub(r"/\*.*?\*/", " ", open(os.path.join(ROOT, "include", "agpt_b200.h")).read(), flags=re.S)
+
+
+def _header_struct_fields(name):
+    """(field name, ctypes type) of the tagged struct `name` of the header, in declaration order"""
+    body = re.search(r"typedef struct %s \{(.*?)\}\s*%s;" % (name, name), _header(), re.S).group(1)
     want = []
     for decl in filter(str.strip, body.split(";")):
         decl = decl.replace("const", " ").strip()
         ptr = "*" in decl
         t = decl.split()[0]
-        for name in decl.split(None, 1)[1].replace("*", " ").split(","):
+        for field in decl.split(None, 1)[1].replace("*", " ").split(","):
             ct = ctypes.c_void_p if ptr else {"int": ctypes.c_int, "long": ctypes.c_long, "float": ctypes.c_float}[t]
-            want.append((name.strip(), ct))
+            want.append((field.strip(), ct))
+    return want
+
+
+def test_tapconv_probe_args_mirror_the_header():
+    """_lib.TapconvProbeArgs has the fields of agpt_tapconv_probe_args in the header's order and C types (a mismatch
+    would hand the probe shifted launch parameters)."""
+    from audiogpt_b200 import _lib
+    want = _header_struct_fields("agpt_tapconv_probe_args")
     got = [(n, t) for n, t in _lib.TapconvProbeArgs._fields_]
     assert [t for _, t in got] == [t for _, t in want]
     assert [n for n, _ in got] == [("inp" if n == "in" else n) for n, _ in want]   # `in` is a Python keyword
+
+
+def test_nn_probe_args_mirror_the_header():
+    """_lib.NnProbeArgs has the fields of agpt_nn_probe_args in the header's order and C types, and _lib.NN_OPS lists
+    the AGPT_NN_* selectors in the enum's order (a mismatch would run another kernel or shift its arguments)."""
+    from audiogpt_b200 import _lib
+    want = _header_struct_fields("agpt_nn_probe_args")
+    assert [(n, t) for n, t in _lib.NnProbeArgs._fields_] == want
+    enum = re.search(r"enum \{([^}]*AGPT_NN_GROUPNORM[^}]*)\}", _header(), re.S).group(1)
+    names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
+    assert names == ["AGPT_NN_" + n for n in _lib.NN_OPS]
+    assert "AGPT_NN_GROUPNORM = 0" in enum and enum.count("=") == 1

@@ -211,32 +211,56 @@ def test_c4_full_size_properties():
     assert torch.allclose(e1[0], e[2], atol=2e-5, rtol=1e-4)
 
 
-@pytest.mark.parametrize("N,heads,d,Lq,Lk", [(2, 8, 40, 780, 780), (2, 8, 40, 780, 77), (2, 8, 80, 195, 195), (1, 8, 80, 195, 77),
-                                             (1, 2, 8, 5, 3), (2, 3, 16, 130, 70), (1, 4, 32, 64, 129), (1, 2, 64, 200, 64)])
-def test_tensor_core_attention_vs_fp64(N, heads, d, Lq, Lk):
-    """agpt_attention (QK^T and PV on wgmma, online softmax) against softmax(q k^T d^-0.5) v evaluated in fp64, for the
-    UNet's shapes (8 heads of 40 / 80 channels; 780 / 195 queries; 780 / 195 / 77 keys) and ragged small ones; the
-    fp32-FMA kernel is held to the same gate.  Stated tolerance: rel-RMSE <= 1e-5 (3 x fp16-part products, 2^-22)."""
+def attention_operands(N, heads, d, Lq, Lk, layout, seed):
+    """device (q, q_pitch, k, v, kv_pitch) pointers and their fp64 CPU heads [N][h][L][d].  layout "kv": q [N][Lq][C]
+    and K | V interleaved rows [N][Lk][2C] (the hoisted context projection); "packed": q | k | v rows [N][L][3C] (the
+    UNet self-attention, FS2, CLAP, GenerSpeech); "peaky": "kv" with q scaled so that the scores have sigma ~ 8 (the
+    running max jumps between key blocks and most p underflow)."""
     import ctypes as C
+    C_ = heads * d
+    heads_of = lambda t, L: t.double().cpu().reshape(N, L, heads, d).permute(0, 2, 1, 3)
+    if layout == "packed":
+        assert Lq == Lk
+        qkv = specs.synth_tensor((N, Lq, 3 * C_), seed=seed).cuda()
+        base = qkv.data_ptr()
+        ptrs = (C.c_void_p(base), 3 * C_, C.c_void_p(base + 4 * C_), C.c_void_p(base + 8 * C_), 3 * C_)
+        return ptrs, (heads_of(qkv[..., :C_], Lq), heads_of(qkv[..., C_:2 * C_], Lk), heads_of(qkv[..., 2 * C_:], Lk)), qkv
+    q = specs.synth_tensor((N, Lq, C_), seed=seed, scale=8.0 if layout == "peaky" else 1.0).cuda()
+    kv = specs.synth_tensor((N, Lk, 2 * C_), seed=seed + 1).cuda()
+    ptrs = (C.c_void_p(q.data_ptr()), C_, C.c_void_p(kv.data_ptr()), C.c_void_p(kv.data_ptr() + 4 * C_), 2 * C_)
+    return ptrs, (heads_of(q, Lq), heads_of(kv[..., :C_], Lk), heads_of(kv[..., C_:], Lk)), (q, kv)
+
+
+ATTN_KV = [(2, 8, 40, 780, 780), (2, 8, 40, 780, 77), (2, 8, 80, 195, 195), (1, 8, 80, 195, 77), (1, 2, 8, 5, 3),
+           (2, 3, 16, 130, 70), (1, 4, 32, 64, 129), (1, 2, 64, 200, 64)]
+ATTN_MORE = [(2, 8, 40, 780, 780, "packed"), (2, 12, 64, 77, 77, "packed"), (3, 2, 128, 150, 150, "packed"),
+             (2, 8, 40, 780, 780, "peaky"), (1, 2, 64, 200, 300, "peaky"), (2, 2, 128, 150, 150, "kv"),
+             (1, 2, 128, 65, 200, "peaky"), (2, 8, 40, 1, 77, "kv"), (2, 4, 80, 70, 1, "kv"), (1, 8, 40, 1, 1, "packed"),
+             (2, 4, 64, 100, 65, "kv"), (1, 2, 40, 65, 65, "peaky")]
+
+
+@pytest.mark.parametrize("N,heads,d,Lq,Lk,layout", [c + ("kv",) for c in ATTN_KV] + ATTN_MORE,
+                         ids=["-".join(map(str, c)) for c in ATTN_KV + ATTN_MORE])
+def test_tensor_core_attention_vs_fp64(N, heads, d, Lq, Lk, layout):
+    """agpt_attention (QK^T and PV on wgmma, online softmax) against softmax(q k^T d^-0.5) v evaluated in fp64, for the
+    UNet's shapes (8 heads of 40 / 80 channels; 780 / 195 queries; 780 / 195 / 77 keys), ragged small ones, packed
+    q | k | v rows, peaky scores, d = 128, and Lq = 1, Lk = 1, Lk = 65; the fp32-FMA kernel is held to the same gate.
+    Stated tolerance: rel-RMSE <= 1e-5 (3 x fp16-part products, 2^-22)."""
     from audiogpt_b200 import _lib
     L = _lib.lib()
     C_ = heads * d
-    q = specs.synth_tensor((N, Lq, C_), seed=1).cuda()
-    kv = specs.synth_tensor((N, Lk, 2 * C_), seed=2).cuda()            # K | V interleaved rows, like the hoisted context projection
-    qh = q.double().cpu().reshape(N, Lq, heads, d).permute(0, 2, 1, 3)
-    kh = kv[:, :, :C_].double().cpu().reshape(N, Lk, heads, d).permute(0, 2, 1, 3)
-    vh = kv[:, :, C_:].double().cpu().reshape(N, Lk, heads, d).permute(0, 2, 1, 3)
+    (qp, q_pitch, kp, vp, kv_pitch), (qh, kh, vh), _keep = attention_operands(N, heads, d, Lq, Lk, layout, 1)
     ref = (torch.softmax(qh @ kh.transpose(-1, -2) * d ** -0.5, dim=-1) @ vh).permute(0, 2, 1, 3).reshape(N, Lq, C_)
     errs = []
     for tc in (1, 0):     # 1: wgmma kernel, 0: fp32-FMA kernel
         _lib.check(L.agpt_set_attention_tc(tc))
         try:
             o = torch.full((N, Lq, C_), float("nan"), device="cuda")
-            _lib.check(L.agpt_attention(_lib.fptr(q), C_, _lib.fptr(kv), 2 * C_, C.c_void_p(kv.data_ptr() + 4 * C_), 2 * C_,
-                                        _lib.fptr(o), C_, N, heads, d, Lq, Lk, _lib.cur_stream()))
+            _lib.check(L.agpt_attention(qp, q_pitch, kp, kv_pitch, vp, kv_pitch, _lib.fptr(o), C_, N, heads, d, Lq, Lk,
+                                        _lib.cur_stream()))
             torch.cuda.synchronize()
         finally:
             _lib.check(L.agpt_set_attention_tc(-1))
         errs.append(rel_rmse(o.cpu(), ref))
-    print(f"attention N={N} h={heads} d={d} {Lq}x{Lk}: rel-RMSE wgmma {errs[0]:.2e}  fp32 kernel {errs[1]:.2e}")
+    print(f"attention N={N} h={heads} d={d} {Lq}x{Lk} {layout}: rel-RMSE wgmma {errs[0]:.2e}  fp32 kernel {errs[1]:.2e}")
     assert errs[0] < 1e-5 and errs[1] < 1e-5
