@@ -169,6 +169,21 @@ class NnProbeArgs(C.Structure):
         ("eps", C.c_float), ("scale", C.c_float)]
 
 
+# agpt_fs_probe_args.op, in the header's enum order (AGPT_FS_<name>)
+FS_OPS = ("EMBED_TOKENS", "ROWMASK", "DUR", "LR_SCAN", "LR_FILL", "GATHER", "AFFINE_MASK", "POSITIONS", "POSEMB_ADD",
+          "PITCH_FRAME", "PITCH_PH", "ENERGY", "EMBED_ADD", "GS_SUM", "GS_ACCUM", "GS_REFMASK", "GS_WN_GATE", "GS_SEGMEAN",
+          "GS_VQ", "GS_CATPOS", "GS_KPM", "GS_PITCH", "GS_COND_CAT", "GS_SQUEEZE", "GS_FLOW_STEP", "PE_MASK", "PE_DENORM")
+
+
+class FsProbeArgs(C.Structure):
+    """agpt_fs_probe_args (a tagged struct in the header: it carries pointers, ints and floats)."""
+    _fields_ = [("op", C.c_int)] + [(n, C.c_void_p) for n in (
+        "tok", "midi", "slur", "idx", "idx2", "idx3", "mel2ph", "x", "x2", "x3", "x4", "x5", "E", "E2", "E3", "w", "b",
+        "y", "y2", "y3", "iy", "iy2", "kpm")] + [(n, C.c_int) for n in (
+        "B", "T", "T2", "H", "C", "M", "nseg", "ntok", "pos_mode", "use_uv", "norm", "first")] + [
+        ("rows", C.c_long)] + [(n, C.c_float) for n in ("escale", "neg_emb", "xscale", "alpha", "mean", "std_")]
+
+
 # (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
 # takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
 _I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
@@ -195,6 +210,7 @@ PROTOTYPES = {
     "agpt_attention_masked": (_I, [_P, _I, _P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "agpt_tapconv_probe": (_I, [_P, _P, _P]),
     "agpt_nn_probe": (_I, [_P, _P]),
+    "agpt_fs_probe": (_I, [_P, _P]),
     "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
     "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "agpt_hifigan_vocode_host": (_I, [_P, _P, _P, _I, _I, _P]),

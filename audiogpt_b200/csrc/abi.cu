@@ -671,4 +671,11 @@ int agpt_nn_probe(const agpt_nn_probe_args* args, void* stream) {
   });
 }
 
+int agpt_fs_probe(const agpt_fs_probe_args* args, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(args, "null argument");
+    fs_probe(*args, (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

@@ -85,6 +85,31 @@ uint8_t* bptr(DevBuf& d) { return reinterpret_cast<uint8_t*>(d.p); }
 
 }  // namespace
 
+void fs2_pitch_frame(const float* pred4, const int* mel2ph, const float* f0_in, const float* uv_in, int use_uv, int norm, float mean,
+                     float std_, float* pitch_pred, float* f0d, int* coarse, long rows, cudaStream_t st) {
+  fs2_pitch_frame_kernel<<<ew_grid(rows), 256, 0, st>>>(pred4, mel2ph, f0_in, uv_in, use_uv, norm, mean, std_, f0_mel_min(),
+                                                        f0_mel_range(), pitch_pred, f0d, coarse, rows);
+  count_launch(1);
+}
+
+void fs2_pitch_ph(const float* pred4, const float* f0_in, int norm, float mean, float std_, float* pitch_pred, float* f0d, int* coarse,
+                  long rows, cudaStream_t st) {
+  fs2_pitch_ph_kernel<<<ew_grid(rows), 256, 0, st>>>(pred4, f0_in, norm, mean, std_, f0_mel_min(), f0_mel_range(), pitch_pred, f0d,
+                                                     coarse, rows);
+  count_launch(1);
+}
+
+void fs2_energy(const float* pred4, const float* e_in, float* e_pred, int* bucket, long rows, cudaStream_t st) {
+  fs2_energy_kernel<<<ew_grid(rows), 256, 0, st>>>(pred4, e_in, e_pred, bucket, rows);
+  count_launch(1);
+}
+
+void fs2_embed_add(const float* x, const float* tgt, const float* pE, const int* pframe, const int* ptok, const int* mel2ph,
+                   const float* eE, const int* ebucket, float* out, int Tt, int Tm, long rows, int H, cudaStream_t st) {
+  fs2_embed_add_kernel<<<ew_grid(rows * H), 256, 0, st>>>(x, tgt, pE, pframe, ptok, mel2ph, eE, ebucket, out, Tt, Tm, rows * H, H);
+  count_launch(1);
+}
+
 struct Fs2Net : Handle {
   agpt_fs2_cfg cfg;
   DevBuf E, midiE, mdw, mdb, slurE, rel_div, pitchE, energyE;
@@ -159,31 +184,23 @@ struct Fs2Net : Handle {
     }
     fs_gather(enc_out.p, m2p, x.p, tnp.p, B, Tt, Tm, H, st);
     // pitch_inp = decoder_inp_origin * tgt_nonpad = x (gathered rows are zero where mel2ph == 0)
-    const double mmin = 1127.0 * std::log(1.0 + 50.0 / 700.0), mmax = 1127.0 * std::log(1.0 + 1100.0 / 700.0);
-    const float mel_min = (float)mmin, mel_range = (float)(mmax - mmin);
     const int* ptok = nullptr;
     const int* pframe = nullptr;
     if (cfg.pitch_type == 1) {
       pitch_pp.forward(x.p, H, B, Tm, s[0].p, s[1].p, s[2].p, pred4.p, st);
-      fs2_pitch_frame_kernel<<<ew_grid(rows), 256, 0, st>>>(pred4.p, m2p, f0_in, uv_in, use_uv, norm, f0_mean, f0_std, mel_min, mel_range,
-                                                            pitch_pred, f0d, coarse, rows);
-      count_launch(1);
+      fs2_pitch_frame(pred4.p, m2p, f0_in, uv_in, use_uv, norm, f0_mean, f0_std, pitch_pred, f0d, coarse, rows, st);
       pframe = coarse;
     } else if (cfg.pitch_type == 2) {
       pitch_pp.forward(enc_out.p, H, B, Tt, s[0].p, s[1].p, s[2].p, pred4.p, st);
-      fs2_pitch_ph_kernel<<<ew_grid(trow), 256, 0, st>>>(pred4.p, f0_in, norm, f0_mean, f0_std, mel_min, mel_range, pitch_pred, f0d, coarse,
-                                                         trow);
-      count_launch(1);
+      fs2_pitch_ph(pred4.p, f0_in, norm, f0_mean, f0_std, pitch_pred, f0d, coarse, trow, st);
       ptok = coarse;
     }
     if (cfg.use_energy_embed) {
       energy_pp.forward(x.p, H, B, Tm, s[0].p, s[1].p, s[2].p, pred4.p, st);
-      fs2_energy_kernel<<<ew_grid(rows), 256, 0, st>>>(pred4.p, e_in, e_pred, iptr(ebkt), rows);
-      count_launch(1);
+      fs2_energy(pred4.p, e_in, e_pred, iptr(ebkt), rows, st);
     }
-    fs2_embed_add_kernel<<<ew_grid(rows * H), 256, 0, st>>>(x.p, tnp.p, cfg.pitch_type ? pitchE.p : nullptr, pframe, ptok, m2p,
-                                                            cfg.use_energy_embed ? energyE.p : nullptr, iptr(ebkt), dec_inp, Tt, Tm, rows * H, H);
-    count_launch(1);
+    fs2_embed_add(x.p, tnp.p, cfg.pitch_type ? pitchE.p : nullptr, pframe, ptok, m2p, cfg.use_energy_embed ? energyE.p : nullptr,
+                  iptr(ebkt), dec_inp, Tt, Tm, rows, H, st);
     if (!mel) { AGPT_CUDA(cudaGetLastError()); return; }        // skip_decoder
     // ---- FastspeechDecoder: padding mask and positions from decoder_inp itself (tts_modules.py:313-318)
     fs_rowmask(dec_inp, dnp.p, bptr(dkpm), rows, H, st);

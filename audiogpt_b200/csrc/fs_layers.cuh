@@ -16,11 +16,15 @@ __device__ __forceinline__ int f0_coarse(float f0, float mel_min, float mel_rang
   if (m > 255.f) m = 255.f;
   return (int)(m + 0.5f);
 }
+// utils/pitch_utils.py denorm_f0: 'standard' rounds the product and the sum separately, as torch does (no FMA)
 __device__ __forceinline__ float denorm(float f, int norm, float mean, float std_) {
-  if (norm == 1) f = f * std_ + mean;      // 'standard'
-  if (norm == 2) f = exp2f(f);             // 'log': 2 ** f0
+  if (norm == 1) f = __fadd_rn(__fmul_rn(f, std_), mean);   // 'standard'
+  if (norm == 2) f = exp2f(f);                              // 'log': 2 ** f0
   return f;
 }
+// f0_to_coarse's f0_mel_min and f0_mel_max - f0_mel_min (f0 in [50, 1100] Hz), computed in double and rounded to fp32
+inline float f0_mel_min() { return (float)(1127.0 * std::log(1.0 + 50.0 / 700.0)); }
+inline float f0_mel_range() { return (float)(1127.0 * std::log(1.0 + 1100.0 / 700.0) - 1127.0 * std::log(1.0 + 50.0 / 700.0)); }
 
 constexpr int kRelMaxLen = 5000;    // RelPositionalEncoding's table length (positions run backwards from max_len - 1)
 
@@ -94,5 +98,53 @@ struct PitchPredictorNet {
   // x [B][T][H] (read only) -> pred4 [B][T][4] (channels >= odim are zero); s0 / s1 / s2: scratch of B*T*max(H, P) floats
   void forward(const float* x, int H, int B, int T, float* s0, float* s1, float* s2, float* pred4, cudaStream_t st);
 };
+
+// ---- the element-wise kernels of fs2.cu, generspeech.cu and pe.cu, one launch each (the drivers and agpt_fs_probe
+// call these).  norm: 0 none, 1 'standard', 2 'log'.
+// add_pitch 'frame': pitch_pred [rows][2], f0d (uv and mel2ph == 0 -> 0), coarse; f0_in / uv_in may be null (predicted)
+void fs2_pitch_frame(const float* pred4, const int* mel2ph, const float* f0_in, const float* uv_in, int use_uv, int norm, float mean,
+                     float std_, float* pitch_pred, float* f0d, int* coarse, long rows, cudaStream_t st);
+// add_pitch 'ph': per token, no uv; pitch_pred [rows]
+void fs2_pitch_ph(const float* pred4, const float* f0_in, int norm, float mean, float std_, float* pitch_pred, float* f0d, int* coarse,
+                  long rows, cudaStream_t st);
+// add_energy: e_pred = pred4[..., 0]; bucket = clamp(floor(e * 256 / 4), 0, 255) of e_in (or e_pred when null)
+void fs2_energy(const float* pred4, const float* e_in, float* e_pred, int* bucket, long rows, cudaStream_t st);
+// out = (x + pE[pitch bin] + eE[bucket]) * tgt; pitch bin from pframe [B*Tm] or (ptok [B*Tt] through mel2ph); pE / eE may be null
+void fs2_embed_add(const float* x, const float* tgt, const float* pE, const int* pframe, const int* ptok, const int* mel2ph,
+                   const float* eE, const int* ebucket, float* out, int Tt, int Tm, long rows, int H, cudaStream_t st);
+// out[r] = (x[r] + a[b] + e[b] (+ tab[idx[r]]) (+ s[r])) * mask[r], b = r / T
+void gs_sum(const float* x, const float* a, const float* e, const float* tab, const int* idx, const float* s, const float* mask, float* out,
+            int T, long rows, int H, cudaStream_t st);
+// dst (+)= src over n floats (first: dst = src)
+void gs_accum(float* dst, const float* src, long n, int first, cudaStream_t st);
+// mask[r] = mel[r][0] != 0 (mel rows of 80 bins)
+void gs_refmask(const float* mel, float* mask, long rows, cudaStream_t st);
+// acts [rows][C] = tanh(a[:, :C]) * sigmoid(a[:, C:]), a [rows][2C]
+void gs_wn_gate(const float* a, float* acts, long rows, int C, cudaStream_t st);
+// out [B][nseg][C] = mean of h [B][T][C] over the frames with seg == s + 1 (0 for an empty segment)
+void gs_segmean(const float* h, const int* seg, float* out, int B, int T, int nseg, int C, cudaStream_t st);
+// VQ argmin over M codes from dots [rows][M] = x . e_m, enorm [M] = |e_m|^2; idx (may be null), q = x + (e - x) (may alias x)
+void gs_vq(const float* x, const float* dots, const float* emb, const float* enorm, int* idx, float* q, long rows, int H, int M,
+           cudaStream_t st);
+// out [rows][2H] = cat[p, SinusoidalPositionalEmbedding(pos)]
+void gs_catpos(const float* p, const int* pos, float* out, long rows, int H, cudaStream_t st);
+// kpm[r] = x[r][0] == 0
+void gs_kpm(const float* x, uint8_t* kpm, long rows, int H, cudaStream_t st);
+// inpaint_pitch: pitch_pred = p1 + p2 (channels 0, 1 of [rows][4]); f0d = f0d_pred = denorm 'standard' (uv, mel2ph == 0 -> 0)
+void gs_pitch(const float* p1, const float* p2, const int* mel2ph, float mean, float std_, float* pitch_pred, float* f0d, float* f0d_pred,
+              int* coarse, long rows, cudaStream_t st);
+// g [rows][M + 4H] = cat[mel [rows][M], dec [rows][H], spk [b][H], emo [b][H], pros [rows][H]], b = r / T
+void gs_cond_cat(const float* mel, const float* dec, const float* spk, const float* emo, const float* pros, float* g, int T, long rows,
+                 int M, int H, cudaStream_t st);
+// x [B][T2][2M] = squeeze(z [B][M][Tz], 2) channels-last (Tz >= 2 T2)
+void gs_squeeze(const float* z, float* x, int B, int Tz, int T2, int M, cudaStream_t st);
+// one reverse post-flow step (coupling, InvConvNear, ActNorm) on x [rows][C2] in place; e = the end layer's [rows][C2];
+// blk = winv[16], bias[C2], logs[C2]
+void gs_flow_step(float* x, const float* e, const float* blk, long rows, int C2, cudaStream_t st);
+// PitchExtractor: mask[r] = any(mel[r] != 0) over M bins (warp per row)
+void pe_mask(const float* mel, float* mask, long rows, int M, cudaStream_t st);
+// PitchExtractor: pitch_pred [rows][2] = pred4[..., :2]; f0 = denorm_f0(pred4[..., 0]) (uv, mask == 0 -> 0)
+void pe_denorm(const float* pred4, const float* mask, float* pitch_pred, float* f0, long rows, int use_uv, int norm, float mean,
+               float std_, cudaStream_t st);
 
 }  // namespace agpt

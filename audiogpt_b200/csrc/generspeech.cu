@@ -214,6 +214,77 @@ __global__ void gs_flow_step_kernel(float* __restrict__ x, const float* __restri
   }
 }
 
+}  // namespace
+
+void gs_sum(const float* x, const float* a, const float* e, const float* tab, const int* idx, const float* s, const float* mask, float* out,
+            int T, long rows, int H, cudaStream_t st) {
+  gs_sum_kernel<<<ew_grid(rows * H), 256, 0, st>>>(x, a, e, tab, idx, s, mask, out, T, rows * H, H);
+  count_launch(1);
+}
+
+void gs_accum(float* dst, const float* src, long n, int first, cudaStream_t st) {
+  gs_accum_kernel<<<ew_grid(n), 256, 0, st>>>(dst, src, n, first);
+  count_launch(1);
+}
+
+void gs_refmask(const float* mel, float* mask, long rows, cudaStream_t st) {
+  gs_refmask_kernel<<<ew_grid(rows), 256, 0, st>>>(mel, mask, rows);
+  count_launch(1);
+}
+
+void gs_wn_gate(const float* a, float* acts, long rows, int C, cudaStream_t st) {
+  gs_wn_gate_kernel<<<ew_grid(rows * C), 256, 0, st>>>(a, acts, rows * C, C);
+  count_launch(1);
+}
+
+void gs_segmean(const float* h, const int* seg, float* out, int B, int T, int nseg, int C, cudaStream_t st) {
+  gs_segmean_kernel<<<dim3(nseg, B), 128, 0, st>>>(h, seg, out, T, nseg, C);
+  count_launch(1);
+}
+
+void gs_vq(const float* x, const float* dots, const float* emb, const float* enorm, int* idx, float* q, long rows, int H, int M,
+           cudaStream_t st) {
+  gs_vq_kernel<<<(unsigned)cdivl(rows, 8), 256, 0, st>>>(x, dots, emb, enorm, idx, q, rows, H, M);
+  count_launch(1);
+}
+
+void gs_catpos(const float* p, const int* pos, float* out, long rows, int H, cudaStream_t st) {
+  const float neg_emb = (float)(-(std::log(10000.0) / (double)(H / 2 - 1)));
+  gs_catpos_kernel<<<ew_grid(rows * 2 * H), 256, 0, st>>>(p, pos, out, rows * 2 * H, H, neg_emb);
+  count_launch(1);
+}
+
+void gs_kpm(const float* x, uint8_t* kpm, long rows, int H, cudaStream_t st) {
+  gs_kpm_kernel<<<ew_grid(rows), 256, 0, st>>>(x, kpm, rows, H);
+  count_launch(1);
+}
+
+void gs_pitch(const float* p1, const float* p2, const int* mel2ph, float mean, float std_, float* pitch_pred, float* f0d, float* f0d_pred,
+              int* coarse, long rows, cudaStream_t st) {
+  gs_pitch_kernel<<<ew_grid(rows), 256, 0, st>>>(p1, p2, mel2ph, mean, std_, f0_mel_min(), f0_mel_range(), pitch_pred, f0d, f0d_pred,
+                                                 coarse, rows);
+  count_launch(1);
+}
+
+void gs_cond_cat(const float* mel, const float* dec, const float* spk, const float* emo, const float* pros, float* g, int T, long rows,
+                 int M, int H, cudaStream_t st) {
+  gs_cond_cat_kernel<<<ew_grid(rows * (M + 4 * H)), 256, 0, st>>>(mel, dec, spk, emo, pros, g, T, rows * (M + 4 * H), M, H);
+  count_launch(1);
+}
+
+void gs_squeeze(const float* z, float* x, int B, int Tz, int T2, int M, cudaStream_t st) {
+  const long total = (long)B * T2 * 2 * M;
+  gs_squeeze_kernel<<<ew_grid(total), 256, 0, st>>>(z, x, Tz, T2, M, total);
+  count_launch(1);
+}
+
+void gs_flow_step(float* x, const float* e, const float* blk, long rows, int C2, cudaStream_t st) {
+  gs_flow_step_kernel<<<ew_grid(rows * (C2 / 4)), 256, 0, st>>>(x, e, blk, rows * (C2 / 4), C2);
+  count_launch(1);
+}
+
+namespace {
+
 // A tap-GEMM on explicitly strided channels-last operands (squeezed views, column slices); epi as TapConvParams
 void gs_conv(const PackedConv& pc, const float* in, int in_pitch, long in_gs, float* out, int out_pitch, long out_gs, int G, int L,
              int epi, cudaStream_t st, const float* res = nullptr, int res_pitch = 0, long res_gs = 0, int accumulate = 0,
@@ -304,8 +375,7 @@ struct GsNet : Handle {
     if (spk_out) AGPT_CUDA(cudaMemcpyAsync(spk_out, spk.p, sizeof(float) * B_ * H, cudaMemcpyDeviceToDevice, st));
     if (emo_out) AGPT_CUDA(cudaMemcpyAsync(emo_out, emo.p, sizeof(float) * B_ * H, cudaMemcpyDeviceToDevice, st));
     // dur_inp = (encoder_out + spk + emo) * src_nonpadding (generspeech.py:87)
-    gs_sum_kernel<<<ew_grid(rows * H), 256, 0, st>>>(enc_out.p, spk.p, emo.p, nullptr, nullptr, nullptr, snp.p, x.p, T, rows * H, H);
-    count_launch(1);
+    gs_sum(enc_out.p, spk.p, emo.p, nullptr, nullptr, nullptr, snp.p, x.p, T, rows, H, st);
     dp.forward(x.p, H, B_, T, snp.p, s[0].p, s[1].p, s[2].p, p4a.p, st);
     fs_dur(p4a.p, snp.p, dur, predict ? iptr(dch) : nullptr, rows, st);
     if (predict) {
@@ -327,8 +397,7 @@ struct GsNet : Handle {
       if (cond) gs_conv(in[i], h, C, (long)L * C, a, 2 * C, (long)L * 2 * C, G, L, EPI_RES, st, cond + (size_t)i * 2 * C, cond_pitch,
                         (long)L * cond_pitch);
       else gs_conv(in[i], h, C, (long)L * C, a, 2 * C, (long)L * 2 * C, G, L, EPI_BIAS, st);
-      gs_wn_gate_kernel<<<ew_grid(rows * C), 256, 0, st>>>(a, acts, rows * C, C);
-      count_launch(1);
+      gs_wn_gate(a, acts, rows, C, st);
       if (i < layers - 1) {
         gs_conv(res[i], acts, C, (long)L * C, h, C, (long)L * C, G, L, EPI_ACC, st, nullptr, 0, 0, 1);
         if (mask) fs_affine_mask(h, nullptr, nullptr, mask, rows, C, st);
@@ -351,8 +420,7 @@ struct GsNet : Handle {
     float* cb_in = so.p;
     if (seg) {
       Tk = nseg;
-      gs_segmean_kernel<<<dim3(nseg, B), 128, 0, st>>>(so.p, seg, sseg.p, Tr, nseg, C);
-      count_launch(1);
+      gs_segmean(so.p, seg, sseg.p, B, Tr, nseg, C, st);
       cb_in = sseg.p;
     }
     const long rk = (long)B * Tk;
@@ -375,16 +443,12 @@ struct GsNet : Handle {
     fs_affine_mask(q, nullptr, nullptr, cnp.p, rk, H, st);
     // VQ: x . e^T on the tap-GEMM, then argmin + gather
     fs_conv(S.vq_dot, q, H, dots.p, M, 1, (int)rk, EPI_BIAS, st);
-    gs_vq_kernel<<<(unsigned)cdivl(rk, 8), 256, 0, st>>>(q, dots.p, S.emb.p, S.enorm.p, idx_out, q, rk, H, M);
-    count_launch(1);
+    gs_vq(q, dots.p, S.emb.p, S.enorm.p, idx_out, q, rk, H, M, st);
     // positions of prosody[..., 0], l1(cat[prosody, positions]), key padding of its output
     fs_positions(q, iptr(pos), B, Tk, H, st);
-    gs_catpos_kernel<<<ew_grid(rk * 2 * H), 256, 0, st>>>(q, iptr(pos), cat.p, rk * 2 * H, H,
-                                                          (float)(-(std::log(10000.0) / (double)(H / 2 - 1))));
-    count_launch(1);
+    gs_catpos(q, iptr(pos), cat.p, rk, H, st);
     fs_conv(S.l1, cat.p, 2 * H, kv.p, H, 1, (int)rk, EPI_BIAS, st);
-    gs_kpm_kernel<<<ew_grid(rk), 256, 0, st>>>(kv.p, bptr(kkpm), rk, H);
-    count_launch(1);
+    gs_kpm(kv.p, bptr(kkpm), rk, H, st);
     // ProsodyAligner: 2 post-norm cross-attention layers, queries = the frame-level decoder input
     const long rq = (long)B * Tm;
     const float* sq = dec0;
@@ -402,8 +466,7 @@ struct GsNet : Handle {
       sq = outp;
     }
     if (!first) {
-      gs_accum_kernel<<<ew_grid(rq * H), 256, 0, st>>>(psum, src.p, rq * H, 0);
-      count_launch(1);
+      gs_accum(psum, src.p, rq * H, 0, st);
     }
   }
 
@@ -441,8 +504,7 @@ struct GsNet : Handle {
     }
     fs_gather(enc_out.p, m2p, x.p, tnp.p, B, Tt, Tm, H, st);      // decoder_inp after expand_states (MixStyle: identity)
     // ---- the three prosody levels (generspeech.py:96-98)
-    gs_refmask_kernel<<<ew_grid(rr), 256, 0, st>>>(ref, rmask.p, rr);
-    count_launch(1);
+    gs_refmask(ref, rmask.p, rr, st);
     const int* segs[3] = {nullptr, ref_mel2ph, ref_mel2word};
     const int nsegs[3] = {Tr, nseg_ph, nseg_word};
     for (int l = 0; l < 3; ++l)
@@ -450,16 +512,11 @@ struct GsNet : Handle {
                   taps ? taps->vq_idx[l] : nullptr, st);
     // ---- pitch (inpaint_pitch): pitch_predictor(decoder_inp * tgt) + pitch_inpainter((decoder_inp + spk + emo + prosody) * tgt)
     pp.forward(x.p, H, B, Tm, s[0].p, s[1].p, s[2].p, p4a.p, st);
-    gs_sum_kernel<<<ew_grid(rows * H), 256, 0, st>>>(x.p, spk.p, emo.p, nullptr, nullptr, ref_prosody, tnp.p, y.p, Tm, rows * H, H);
-    count_launch(1);
+    gs_sum(x.p, spk.p, emo.p, nullptr, nullptr, ref_prosody, tnp.p, y.p, Tm, rows, H, st);
     ppi.forward(y.p, H, B, Tm, s[0].p, s[1].p, s[2].p, p4b.p, st);
-    const double mmin = 1127.0 * std::log(1.0 + 50.0 / 700.0), mmax = 1127.0 * std::log(1.0 + 1100.0 / 700.0);
-    gs_pitch_kernel<<<ew_grid(rows), 256, 0, st>>>(p4a.p, p4b.p, m2p, f0_mean, f0_std, (float)mmin, (float)(mmax - mmin), pitch_pred, f0d,
-                                                   f0d_pred, coarse, rows);
-    count_launch(1);
+    gs_pitch(p4a.p, p4b.p, m2p, f0_mean, f0_std, pitch_pred, f0d, f0d_pred, coarse, rows, st);
     // ---- decoder_inp = (decoder_inp + spk + emo + pitch_embed + prosody) * tgt, FFT decoder, mel_out
-    gs_sum_kernel<<<ew_grid(rows * H), 256, 0, st>>>(x.p, spk.p, emo.p, pitchE.p, coarse, ref_prosody, tnp.p, dec_inp, Tm, rows * H, H);
-    count_launch(1);
+    gs_sum(x.p, spk.p, emo.p, pitchE.p, coarse, ref_prosody, tnp.p, dec_inp, Tm, rows, H, st);
     fs_rowmask(dec_inp, dnp.p, bptr(dkpm), rows, H, st);
     fs_positions(dec_inp, iptr(pos), B, Tm, H, st);
     fs_posemb_add(dec_inp, x.p, iptr(pos), dec_alpha, rows, H, st);
@@ -467,11 +524,9 @@ struct GsNet : Handle {
     fs_conv(mel_out, y.p, H, melpre, Mo, 1, (int)rows, EPI_BIAS, st);
     fs_affine_mask(melpre, nullptr, nullptr, tnp.p, rows, Mo, st);
     // ---- Glow post-flow, reverse (generspeech.py:233-260): the squeezed views are strided reads of [B][Tm][*]
-    gs_cond_cat_kernel<<<ew_grid(rows * Gc), 256, 0, st>>>(melpre, dec_inp, spk.p, emo.p, ref_prosody, gcond.p, Tm, rows * Gc, Mo, H);
-    count_launch(1);
+    gs_cond_cat(melpre, dec_inp, spk.p, emo.p, ref_prosody, gcond.p, Tm, rows, Mo, H, st);
     gs_conv(cond_all, gcond.p, 2 * Gc, (long)Tm * Gc, cond.p, CC, (long)T2 * CC, B, T2, EPI_BIAS, st);
-    gs_squeeze_kernel<<<ew_grid(r2 * 2 * Mo), 256, 0, st>>>(znoise, mel, Tm, T2, Mo, r2 * 2 * Mo);
-    count_launch(1);
+    gs_squeeze(znoise, mel, B, Tm, T2, Mo, st);
     const int C2 = 2 * Mo;
     for (int b = NB - 1; b >= 0; --b) {
       GlowBlock& G = glow[b];
@@ -480,8 +535,7 @@ struct GsNet : Handle {
       wn(W.in.data(), W.res.data(), W.skip.data(), L, gh.p, hid, gskip.p, cond.p + (size_t)b * 2 * hid * L, CC, nullptr, B, T2, ga.p,
          gacts.p, st);
       gs_conv(G.end, gskip.p, hid, (long)T2 * hid, gend.p, C2, (long)T2 * C2, B, T2, EPI_BIAS, st);
-      gs_flow_step_kernel<<<ew_grid(r2 * (C2 / 4)), 256, 0, st>>>(mel, gend.p, G.prm.p, r2 * (C2 / 4), C2);
-      count_launch(1);
+      gs_flow_step(mel, gend.p, G.prm.p, r2, C2, st);
     }
     AGPT_CUDA(cudaGetLastError());
   }

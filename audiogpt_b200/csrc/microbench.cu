@@ -1,8 +1,9 @@
-// Conformance entries: one production launch of the tap-GEMM primitive (tapconv_probe) or of a non-contraction
-// kernel (nn_probe) on caller-owned tensors.
+// Conformance entries: one production launch of the tap-GEMM primitive (tapconv_probe), of a non-contraction
+// kernel (nn_probe) or of a FastSpeech-family element-wise kernel (fs_probe) on caller-owned tensors.
 #include "tapconv.cuh"
 #include "models.h"
 #include "nn_kernels.h"
+#include "fs_layers.cuh"
 
 namespace agpt {
 
@@ -111,6 +112,46 @@ void nn_probe(const agpt_nn_probe_args& a, cudaStream_t st) {
     case AGPT_NN_CONV_OUT_DDIM:
       conv_out_ddim(a.x, a.w, a.b, a.y, a.y2, a.table, a.step, a.N, a.H, a.W, a.C, a.single, st); break;
     default: throw Error("nn probe: unknown op " + std::to_string(a.op));
+  }
+  AGPT_CUDA(cudaStreamSynchronize(st));
+}
+
+// One call of a production FastSpeech-family launcher on caller-owned tensors (agpt_fs_probe, include/agpt_b200.h).
+void fs_probe(const agpt_fs_probe_args& a, cudaStream_t st) {
+  switch (a.op) {
+    case AGPT_FS_EMBED_TOKENS:
+      fs_embed_tokens(a.tok, a.midi, a.x, a.slur, a.E, a.E2, a.w, a.b, a.E3, a.ntok, a.escale, a.pos_mode, a.x2, a.neg_emb, a.xscale, a.y,
+                      a.y2, a.kpm, a.B, a.T, a.H, st);
+      break;
+    case AGPT_FS_ROWMASK: fs_rowmask(a.x, a.y, a.kpm, a.rows, a.C, st); break;
+    case AGPT_FS_DUR: fs_dur(a.x, a.x2, a.y, a.iy, a.rows, st); break;
+    case AGPT_FS_LR_SCAN: fs_lr_scan(a.idx, a.iy, a.iy2, a.B, a.T, st); break;
+    case AGPT_FS_LR_FILL: fs_lr_fill(a.idx, a.idx2, a.iy, a.B, a.T, a.T2, st); break;
+    case AGPT_FS_GATHER: fs_gather(a.x, a.mel2ph, a.y, a.y2, a.B, a.T, a.T2, a.H, st); break;
+    case AGPT_FS_AFFINE_MASK: fs_affine_mask(a.y, a.w, a.b, a.x, a.rows, a.C, st); break;
+    case AGPT_FS_POSITIONS: fs_positions(a.x, a.iy, a.B, a.T, a.C, st); break;
+    case AGPT_FS_POSEMB_ADD: fs_posemb_add(a.x, a.y, a.idx, a.alpha, a.rows, a.C, st); break;
+    case AGPT_FS_PITCH_FRAME:
+      fs2_pitch_frame(a.x, a.mel2ph, a.x2, a.x3, a.use_uv, a.norm, a.mean, a.std_, a.y, a.y2, a.iy, a.rows, st); break;
+    case AGPT_FS_PITCH_PH: fs2_pitch_ph(a.x, a.x2, a.norm, a.mean, a.std_, a.y, a.y2, a.iy, a.rows, st); break;
+    case AGPT_FS_ENERGY: fs2_energy(a.x, a.x2, a.y, a.iy, a.rows, st); break;
+    case AGPT_FS_EMBED_ADD:
+      fs2_embed_add(a.x, a.x2, a.E, a.idx, a.idx2, a.mel2ph, a.E2, a.idx3, a.y, a.T, a.T2, a.rows, a.H, st); break;
+    case AGPT_FS_GS_SUM: gs_sum(a.x, a.x2, a.x3, a.E, a.idx, a.x4, a.x5, a.y, a.T, a.rows, a.H, st); break;
+    case AGPT_FS_GS_ACCUM: gs_accum(a.y, a.x, a.rows, a.first, st); break;
+    case AGPT_FS_GS_REFMASK: gs_refmask(a.x, a.y, a.rows, st); break;
+    case AGPT_FS_GS_WN_GATE: gs_wn_gate(a.x, a.y, a.rows, a.C, st); break;
+    case AGPT_FS_GS_SEGMEAN: gs_segmean(a.x, a.idx, a.y, a.B, a.T, a.nseg, a.C, st); break;
+    case AGPT_FS_GS_VQ: gs_vq(a.x, a.x2, a.E, a.x3, a.iy, a.y, a.rows, a.H, a.M, st); break;
+    case AGPT_FS_GS_CATPOS: gs_catpos(a.x, a.idx, a.y, a.rows, a.H, st); break;
+    case AGPT_FS_GS_KPM: gs_kpm(a.x, a.kpm, a.rows, a.H, st); break;
+    case AGPT_FS_GS_PITCH: gs_pitch(a.x, a.x2, a.mel2ph, a.mean, a.std_, a.y, a.y2, a.y3, a.iy, a.rows, st); break;
+    case AGPT_FS_GS_COND_CAT: gs_cond_cat(a.x, a.x2, a.x3, a.x4, a.x5, a.y, a.T, a.rows, a.M, a.H, st); break;
+    case AGPT_FS_GS_SQUEEZE: gs_squeeze(a.x, a.y, a.B, a.T, a.T2, a.M, st); break;
+    case AGPT_FS_GS_FLOW_STEP: gs_flow_step(a.y, a.x, a.w, a.rows, a.C, st); break;
+    case AGPT_FS_PE_MASK: pe_mask(a.x, a.y, a.rows, a.M, st); break;
+    case AGPT_FS_PE_DENORM: pe_denorm(a.x, a.x2, a.y, a.y2, a.rows, a.use_uv, a.norm, a.mean, a.std_, st); break;
+    default: throw Error("fs probe: unknown op " + std::to_string(a.op));
   }
   AGPT_CUDA(cudaStreamSynchronize(st));
 }

@@ -32,12 +32,23 @@ __global__ void pe_denorm_kernel(const float* __restrict__ pred4, const float* _
     const float p0 = pred4[r * 4], p1 = pred4[r * 4 + 1];
     pitch_pred[r * 2] = p0; pitch_pred[r * 2 + 1] = p1;
     float v = p0;
-    if (norm_mode == 1) v = v * f0_std + f0_mean;       // 'standard'
-    if (norm_mode == 2) v = exp2f(v);                    // 'log': 2 ** f0
+    v = denorm(v, norm_mode, f0_mean, f0_std);
     if (use_uv && p1 > 0.f) v = 0.f;
     if (mask[r] == 0.f) v = 0.f;
     f0[r] = v;
   }
+}
+
+void pe_mask(const float* mel, float* mask, long rows, int M, cudaStream_t st) {
+  pe_mask_kernel<<<(unsigned)cdivl(rows, 8), 256, 0, st>>>(mel, mask, rows, M);
+  count_launch(1);
+}
+
+void pe_denorm(const float* pred4, const float* mask, float* pitch_pred, float* f0, long rows, int use_uv, int norm, float mean,
+               float std_, cudaStream_t st) {
+  pe_denorm_kernel<<<(unsigned)std::min<long>(cdivl(rows, 256), 1184), 256, 0, st>>>(pred4, mask, pitch_pred, f0, rows, use_uv, norm, mean,
+                                                                                  std_);
+  count_launch(1);
 }
 
 struct PeNet : Handle {
@@ -58,8 +69,7 @@ struct PeNet : Handle {
     mask.ensure(rows); pred4.ensure(rows * 4);
     for (auto& b : buf) b.ensure((size_t)rows * Cmax);
     float *x = buf[0].p, *y = buf[1].p, *z = buf[2].p;
-    pe_mask_kernel<<<(unsigned)cdivl(rows, 8), 256, 0, st>>>(mel, mask.p, rows, M);
-    count_launch(1);
+    pe_mask(mel, mask.p, rows, M, st);
     // ---- Prenet (pe.py:23-42): 3 x [Conv1d k5 -> ReLU -> BatchNorm1d(eval) -> x mask], out_proj, x mask
     const float* in = mel;
     int cin = M;
@@ -85,9 +95,7 @@ struct PeNet : Handle {
     }
     // ---- PitchPredictor (tts_modules.py:247-260)
     pp.forward(x, H, B, T, y, z, buf[3].p, pred4.p, st);
-    pe_denorm_kernel<<<(unsigned)std::min<long>(cdivl(rows, 256), 1184), 256, 0, st>>>(pred4.p, mask.p, pitch_pred, f0, rows, use_uv,
-                                                                                   norm_mode, f0_mean, f0_std);
-    count_launch(1);
+    pe_denorm(pred4.p, mask.p, pitch_pred, f0, rows, use_uv, norm_mode, f0_mean, f0_std, st);
     AGPT_CUDA(cudaGetLastError());
   }
 };

@@ -146,6 +146,65 @@ typedef struct agpt_nn_probe_args {
   float eps, scale;
 } agpt_nn_probe_args;
 int agpt_nn_probe(const agpt_nn_probe_args* args, void* stream);
+/* Conformance entry of the FastSpeech-family element-wise kernels (fs_layers.cu, fs2.cu, generspeech.cu, pe.cu;
+ * tests/test_fs_kernels_gpu.py): ONE call of the production launcher selected by `op` on caller-owned device tensors,
+ * with the arguments as given.  Tensors are fp32 (x*, E*, w, b, y*), int32 (tok, midi, slur, idx*, mel2ph, iy*) or
+ * uint8 (kpm) device arrays; null where an op allows it.  norm: 0 none, 1 'standard', 2 'log'.  The fields each op reads:
+ *   EMBED_TOKENS  fs_embed_tokens: tok [B][T] -> y = x [B][T][H], y2 = nonpad, kpm; E [ntok][H] * escale (+ midi [B][T] rows
+ *                 of E2 [300][H], + x = midi_dur * w + b, + slur rows of E3 [2][H]: each of the three null = off); pos_mode
+ *                 0 none, 1 fairseq (neg_emb), 2 rel_pos (x2 = div_term [H/2], xscale)
+ *   ROWMASK       fs_rowmask: x [rows][C] -> y = nonpad [rows], kpm
+ *   DUR           fs_dur: x = pred4 [rows][4], x2 = nonpad -> y = dur, iy = dur_choice (null = none)
+ *   LR_SCAN       fs_lr_scan: idx = dur_choice [B][T] -> iy = cum [B][T], iy2 = mel_len [B]
+ *   LR_FILL       fs_lr_fill: idx = cum [B][T], idx2 = mel_len [B] -> iy = mel2ph [B][T2]
+ *   GATHER        fs_gather: x = enc [B][T][H], mel2ph [B][T2] -> y [B][T2][H], y2 = tgt [B][T2]
+ *   AFFINE_MASK   fs_affine_mask: y [rows][C] in place, w = a [C], b [C] (both null: mask only), x = mask [rows]
+ *   POSITIONS     fs_positions: x [B][T][C] -> iy = pos [B][T]
+ *   POSEMB_ADD    fs_posemb_add: x [rows][C], idx = pos [rows], alpha -> y (may be x)
+ *   PITCH_FRAME   fs2_pitch_frame: x = pred4 [rows][4], mel2ph, x2 = f0 / x3 = uv (null = predicted), use_uv, norm, mean,
+ *                 std_ -> y = pitch_pred [rows][2], y2 = f0_denorm, iy = coarse
+ *   PITCH_PH      fs2_pitch_ph: x = pred4, x2 = f0 (null = predicted), norm, mean, std_ -> y = pitch_pred [rows], y2, iy
+ *   ENERGY        fs2_energy: x = pred4, x2 = energy (null = predicted) -> y = energy_pred, iy = bucket
+ *   EMBED_ADD     fs2_embed_add: x [B*T2][H], x2 = tgt, E = pitch table (null = none) with idx = bins [B*T2] or idx2 = bins
+ *                 [B][T] through mel2ph [B][T2], E2 = energy table (null = none) with idx3 = buckets -> y; rows = B*T2
+ *   GS_SUM        gs_sum: x [rows][H], x2 = spk / x3 = emo [rows / T][H], E (null = none) with idx, x4 (null = none),
+ *                 x5 = mask [rows] -> y
+ *   GS_ACCUM      gs_accum: y (+)= x over rows floats (first: y = x)
+ *   GS_REFMASK    gs_refmask: x = ref mel [rows][80] -> y [rows]
+ *   GS_WN_GATE    gs_wn_gate: x [rows][2C] -> y [rows][C]
+ *   GS_SEGMEAN    gs_segmean: x [B][T][C], idx = seg [B][T] -> y [B][nseg][C]
+ *   GS_VQ         gs_vq: x [rows][H], x2 = dots [rows][M], E = codebook [M][H], x3 = |e|^2 [M] -> iy (null = none),
+ *                 y = quantised (may be x)
+ *   GS_CATPOS     gs_catpos: x [rows][H], idx = pos [rows] -> y [rows][2H]
+ *   GS_KPM        gs_kpm: x [rows][H] -> kpm
+ *   GS_PITCH      gs_pitch: x / x2 = the two predictors' [rows][4], mel2ph, mean, std_ -> y = pitch_pred [rows][2],
+ *                 y2 = f0_denorm, y3 = f0_denorm_pred, iy = coarse
+ *   GS_COND_CAT   gs_cond_cat: x = mel [rows][M], x2 = dec [rows][H], x3 / x4 = spk / emo [rows / T][H], x5 = prosody
+ *                 [rows][H] -> y [rows][M + 4H]
+ *   GS_SQUEEZE    gs_squeeze: x = z [B][M][T] -> y [B][T2][2M] (T >= 2 T2)
+ *   GS_FLOW_STEP  gs_flow_step: y [rows][C] in place, x = the end layer's output [rows][C], w = winv[16] bias[C] logs[C]
+ *   PE_MASK       pe_mask: x = mel [rows][M] -> y [rows]
+ *   PE_DENORM     pe_denorm: x = pred4 [rows][4], x2 = mask, use_uv, norm, mean, std_ -> y = pitch_pred [rows][2], y2 = f0
+ * Synchronises `stream` before returning.                                                                          */
+enum {
+  AGPT_FS_EMBED_TOKENS = 0, AGPT_FS_ROWMASK, AGPT_FS_DUR, AGPT_FS_LR_SCAN, AGPT_FS_LR_FILL, AGPT_FS_GATHER, AGPT_FS_AFFINE_MASK,
+  AGPT_FS_POSITIONS, AGPT_FS_POSEMB_ADD, AGPT_FS_PITCH_FRAME, AGPT_FS_PITCH_PH, AGPT_FS_ENERGY, AGPT_FS_EMBED_ADD, AGPT_FS_GS_SUM,
+  AGPT_FS_GS_ACCUM, AGPT_FS_GS_REFMASK, AGPT_FS_GS_WN_GATE, AGPT_FS_GS_SEGMEAN, AGPT_FS_GS_VQ, AGPT_FS_GS_CATPOS, AGPT_FS_GS_KPM,
+  AGPT_FS_GS_PITCH, AGPT_FS_GS_COND_CAT, AGPT_FS_GS_SQUEEZE, AGPT_FS_GS_FLOW_STEP, AGPT_FS_PE_MASK, AGPT_FS_PE_DENORM
+};
+typedef struct agpt_fs_probe_args {
+  int op;
+  const int* tok; const int* midi; const int* slur; const int* idx; const int* idx2; const int* idx3; const int* mel2ph;
+  const float* x; const float* x2; const float* x3; const float* x4; const float* x5;
+  const float* E; const float* E2; const float* E3; const float* w; const float* b;
+  float* y; float* y2; float* y3;
+  int* iy; int* iy2;
+  uint8_t* kpm;
+  int B, T, T2, H, C, M, nseg, ntok, pos_mode, use_uv, norm, first;
+  long rows;
+  float escale, neg_emb, xscale, alpha, mean, std_;
+} agpt_fs_probe_args;
+int agpt_fs_probe(const agpt_fs_probe_args* args, void* stream);
 
 /* ------------------------------------------------------------------ HiFi-GAN
  * Replaces HifiGanGenerator.__init__/forward/remove_weight_norm

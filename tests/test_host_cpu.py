@@ -417,3 +417,15 @@ def test_nn_probe_args_mirror_the_header():
     names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
     assert names == ["AGPT_NN_" + n for n in _lib.NN_OPS]
     assert "AGPT_NN_GROUPNORM = 0" in enum and enum.count("=") == 1
+
+
+def test_fs_probe_args_mirror_the_header():
+    """_lib.FsProbeArgs has the fields of agpt_fs_probe_args in the header's order and C types, and _lib.FS_OPS lists
+    the AGPT_FS_* selectors in the enum's order (a mismatch would run another kernel or shift its arguments)."""
+    from audiogpt_b200 import _lib
+    want = _header_struct_fields("agpt_fs_probe_args")
+    assert [(n, t) for n, t in _lib.FsProbeArgs._fields_] == want
+    enum = re.search(r"enum \{([^}]*AGPT_FS_EMBED_TOKENS[^}]*)\}", _header(), re.S).group(1)
+    names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
+    assert names == ["AGPT_FS_" + n for n in _lib.FS_OPS]
+    assert "AGPT_FS_EMBED_TOKENS = 0" in enum and enum.count("=") == 1
