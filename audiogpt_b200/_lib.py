@@ -184,6 +184,20 @@ class FsProbeArgs(C.Structure):
         ("rows", C.c_long)] + [(n, C.c_float) for n in ("escale", "neg_emb", "xscale", "alpha", "mean", "std_")]
 
 
+# agpt_audio_probe_args.op, in the header's enum order (AGPT_AU_<name>)
+AU_OPS = ("FRAMES", "LOGMEL", "POWMEL", "STFT_ROWS", "MAGPHASE", "ISTFT_FRAMES", "ISTFT_FINISH", "RESAMPLE", "CNN14_HEAD",
+          "L2NORM2", "SIMILARITY", "LASS_INPUT", "LASS_HEAD", "W2V_STEM")
+
+
+class AudioProbeArgs(C.Structure):
+    """agpt_audio_probe_args (a tagged struct in the header: it carries pointers, ints, longs and floats)."""
+    _fields_ = [("op", C.c_int)] + [(n, C.c_void_p) for n in (
+        "x", "x2", "w", "g", "b", "starts", "y", "y2", "part", "stat", "cnt")] + [(n, C.c_int) for n in (
+        "B", "T", "F", "C", "D", "W", "n", "hop", "nb", "nm", "ch", "pitch", "Na", "Nt", "k0", "s0", "s1", "orig", "nw",
+        "width", "clip")] + [(n, C.c_long) for n in ("rows", "N", "R", "sb", "stt", "sf")] + [
+        (n, C.c_float) for n in ("scale", "shift", "eps")]
+
+
 # (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
 # takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
 _I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
@@ -211,6 +225,7 @@ PROTOTYPES = {
     "agpt_tapconv_probe": (_I, [_P, _P, _P]),
     "agpt_nn_probe": (_I, [_P, _P]),
     "agpt_fs_probe": (_I, [_P, _P]),
+    "agpt_audio_probe": (_I, [_P, _P]),
     "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
     "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "agpt_hifigan_vocode_host": (_I, [_P, _P, _P, _I, _I, _P]),

@@ -678,4 +678,11 @@ int agpt_fs_probe(const agpt_fs_probe_args* args, void* stream) {
   });
 }
 
+int agpt_audio_probe(const agpt_audio_probe_args* args, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(args, "null argument");
+    audio_probe(*args, (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

@@ -22,6 +22,40 @@ constexpr int kCnn14Blocks = 6;
 constexpr int kCnn14Ch[kCnn14Blocks] = {64, 128, 256, 512, 1024, 2048};
 constexpr float kBnEps = 1e-5f;
 
+// frames[b][t][j] = x_b[reflect(t * hop + j - n / 2)]  (center=True, pad_mode='reflect')
+__global__ void cnn14_frames_kernel(const float* __restrict__ x, int clip, int T, int hop, int n, float* __restrict__ fr, long total) {
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const long bt = i / n;
+    const int j = (int)(i - bt * n);
+    const long b = bt / T;
+    const int t = (int)(bt - b * T);
+    int s = t * hop + j - n / 2;
+    s = s < 0 ? -s : (s >= clip ? 2 * (clip - 1) - s : s);
+    fr[i] = x[b * clip + s];
+  }
+}
+
+// one block per frame: re^2 + im^2 -> melW projection -> 10 log10(max(., 1e-10)) -> bn0 (folded scale / shift per mel
+// bin) -> CH == 4: img[b][t][m][0..3] (Cnn14's first conv reads a 4-channel padded input); CH == 1: img[b][t][m]
+template <int CH>
+__global__ void cnn14_logmel_kernel(const float* __restrict__ spec, int pitch, int nb, const float* __restrict__ melW,
+                                    int nm,const float* __restrict__ bn_s, const float* __restrict__ bn_t, float* __restrict__ img) {
+  extern __shared__ float pw[];
+  const long f = blockIdx.x;
+  const float* re = spec + f * pitch;
+  const float* im = re + nb;
+  for (int k = threadIdx.x; k < nb; k += blockDim.x) pw[k] = re[k] * re[k] + im[k] * im[k];
+  __syncthreads();
+  for (int m = threadIdx.x; m < nm; m += blockDim.x) {
+    float acc = 0.f;
+    for (int k = 0; k < nb; ++k) acc = fmaf(pw[k], melW[(long)k * nm + m], acc);
+    const float db = 10.f * log10f(fmaxf(acc, 1e-10f));
+    const float v = db * bn_s[m] + bn_t[m];
+    if constexpr (CH == 4) *reinterpret_cast<float4*>(img + (f * nm + m) * 4) = make_float4(v, 0.f, 0.f, 0.f);
+    else img[f * nm + m] = v;
+  }
+}
+
 // out[b][i] = y_b[(start_b + i) mod R] for i < clip, y_b the resampled clip b: one rule for the crop (start_b >= 0,
 // start_b + clip <= R) and the tiling (start_b = 0, R <= clip) of resample_and_duration.
 // y[k * nw + p] = sum_j ker[p][j] * x[k * orig + j - width]  (torchaudio's conv1d over the zero-padded clip)
@@ -119,6 +153,48 @@ void clap_similarity(const float* a, int Na, const float* t, int Nt, int D, floa
   AGPT_CUDA(cudaGetLastError());
 }
 
+void cnn14_frames(const float* x, int clip, int B, int hop, int n, float* fr, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && hop >= 1 && n >= 2, "framing: bad sizes");
+  if (clip <= n / 2)
+    throw Error("framing: " + std::to_string(clip) + " samples are too few for the reflect padding of " + std::to_string(n / 2));
+  const int T = clip / hop + 1;
+  const long tot = (long)B * T * n;
+  cnn14_frames_kernel<<<ew_blocks(tot), 256, 0, st>>>(x, clip, T, hop, n, fr, tot);
+  count_launch(1);
+}
+
+void cnn14_logmel(const float* spec, int pitch, int nb, const float* melW, int nm, const float* bn_s, const float* bn_t, float* img,
+                  long frames, int ch, cudaStream_t st) {
+  AGPT_CHECK(frames >= 1 && nb >= 1 && nm >= 1 && pitch >= 2 * nb, "log-mel: bad sizes");
+  AGPT_CHECK(nb <= 12 * 1024, "log-mel: at most 12288 bins (the power row lives in 48 KB of shared memory)");
+  if (ch == 4) cnn14_logmel_kernel<4><<<(unsigned)frames, 64, sizeof(float) * nb, st>>>(spec, pitch, nb, melW, nm, bn_s, bn_t, img);
+  else if (ch == 1) cnn14_logmel_kernel<1><<<(unsigned)frames, 64, sizeof(float) * nb, st>>>(spec, pitch, nb, melW, nm, bn_s, bn_t, img);
+  else throw Error("log-mel: 1 or 4 output channels");
+  count_launch(1);
+}
+
+void cnn14_resample(const float* x, long L, int B, const float* ker, int orig, int nw, int width, const int* start_host,
+                    DevBuf& start_dev, int clip, float* out, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && L >= 1 && orig >= 1 && nw >= 1 && width >= 0 && clip >= 1, "resampler: bad sizes");
+  const long R = cdivl((long)nw * L, orig);   // ceil(new * L / orig): the resampled length
+  for (int b = 0; b < B; ++b) {
+    const int s = start_host[b];
+    if (R > clip) AGPT_CHECK(s >= 0 && (long)s < R - clip, "crop start outside [0, resampled length - clip)");
+    else AGPT_CHECK(s == -1, "a clip no longer than the target is tiled: its start must be -1");
+  }
+  int* sd = reinterpret_cast<int*>(start_dev.ensure(B));
+  AGPT_CUDA(cudaMemcpyAsync(sd, start_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
+  const long tot = (long)B * clip;
+  cnn14_resample_kernel<<<ew_blocks(tot), 256, 0, st>>>(x, L, ker, 2 * width + orig, orig, nw, width, R, sd, clip, out, tot);
+  count_launch(1);
+}
+
+void cnn14_head(const float* x, int B, int T, int F, int C, float* out, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && T >= 1 && F >= 1 && C >= 1, "pooling head: bad sizes");
+  cnn14_head_kernel<<<(unsigned)cdivl((long)B * C, 256), 256, 0, st>>>(x, T, F, C, out, B);
+  count_launch(1);
+}
+
 // CLAP's Projection (clap.py:8-20, dropout off) on [rows][d_in] rows of pitch in_pitch, then the two L2 norms:
 // out = l2(l2(LayerNorm(e1 + linear2(gelu(e1))))), e1 = linear1(x)
 void ClapProjection::run(const float* x, int in_pitch, int rows, float* out, cudaStream_t st) {
@@ -157,21 +233,11 @@ struct Cnn14Net : Handle {
   void embed(const float* x, long L, int B, const int* start_host, float* out, cudaStream_t st) {
     AGPT_CHECK(clip > 0, "agpt_cnn14_set_resample was not called");
     AGPT_CHECK(B >= 1 && L >= 1, "empty batch");
-    const long R = cdivl((long)nw * L, orig);   // ceil(new * L / orig): the resampled length
-    for (int b = 0; b < B; ++b) {
-      const int s = start_host[b];
-      if (R > clip) AGPT_CHECK(s >= 0 && (long)s < R - clip, "crop start outside [0, resampled length - clip)");
-      else AGPT_CHECK(s == -1, "a clip no longer than the target is tiled: its start must be -1");
-    }
     const int n = cfg.window_size, hop = cfg.hop_size, nm = cfg.mel_bins;
     AGPT_CHECK(clip > n / 2, "the fitted clip must be longer than half a window (reflect padding)");
     const int T = clip / hop + 1;
-    int* sd = reinterpret_cast<int*>(starts.ensure(B));
-    AGPT_CUDA(cudaMemcpyAsync(sd, start_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
     wav.ensure((size_t)B * clip);
-    const long tot = (long)B * clip;
-    cnn14_resample_kernel<<<ew_blocks(tot), 256, 0, st>>>(x, L, ker.p, taps, orig, nw, width, R, sd, clip, wav.p, tot);
-    count_launch(1);
+    cnn14_resample(x, L, B, ker.p, orig, nw, width, start_host, starts, clip, wav.p, st);
     img.ensure((size_t)B * T * nm * 4);
     front.run<4>(wav.p, clip, B, img.p, st);
     // conv blocks: (3x3 conv -> folded BN -> ReLU) x 2, then AvgPool2d(2) (blocks 1-5) on [B][H=T][W=F][C]
@@ -192,8 +258,7 @@ struct Cnn14Net : Handle {
     }
     const int C = kCnn14Ch[kCnn14Blocks - 1];
     pooled.ensure((size_t)B * C); emb.ensure((size_t)B * cfg.out_emb);
-    cnn14_head_kernel<<<(unsigned)cdivl((long)B * C, 256), 256, 0, st>>>(in, H, W, C, pooled.p, B);
-    count_launch(1);
+    cnn14_head(in, B, H, W, C, pooled.p, st);
     fs_conv(fc1, pooled.p, C, emb.p, cfg.out_emb, 1, B, EPI_RELU, st);
     proj.run(emb.p, cfg.out_emb, B, out, st);
     AGPT_CUDA(cudaGetLastError());

@@ -4,7 +4,7 @@
 // audio.py:43-55 (wav_to_mel_spectrogram: librosa's power mel, n_fft 400, hop 160, 40 Slaney bands, no log) and
 // model.py:41-77 (EmotionEncoder: nn.LSTM(40, 256, 3, batch_first) from h0 = c0 = 0; forward adds Linear, ReLU and an
 // L2 norm).
-// Front end: reflect-padded framing (cnn14_frames_kernel), one 1-tap tap-GEMM against the periodic-Hann DFT rows, then
+// Front end: reflect-padded framing (cnn14_frames), one 1-tap tap-GEMM against the periodic-Hann DFT rows, then
 // emo_powmel_kernel (re^2 + im^2 projected on the mel matrix).  Each layer's input projection W_ih x + b_ih + b_hh is
 // one tap-GEMM; layer 0 runs it once over the mel frames the partials cover, and partial p reads rows step p ..
 // step p + T - 1 of it (the partials overlap by half, so this halves layer 0's projection).  The recurrence is
@@ -14,7 +14,7 @@
 #include "common.cuh"
 #include "tapconv.cuh"
 #include "models.h"
-#include "logmel.cuh"
+#include "audio_front.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -172,8 +172,6 @@ __global__ void __launch_bounds__(kTailThreads) emo_linear_norm_kernel(const flo
   for (int o = threadIdx.x; o < E; o += blockDim.x) out[n * E + o] = e[o] / nrm;
 }
 
-unsigned ew_blocks(long n) { return (unsigned)std::max<long>(1, std::min<long>(cdivl(n, 256), 4096)); }
-
 // sequences per cluster: spread N over the clusters the device can hold at once, at most kLstmMaxB each
 int lstm_group(int N) {
   static int max_clusters[64] = {};
@@ -202,6 +200,12 @@ int lstm_group(int N) {
 }  // namespace
 
 // ---------------------------------------------------------------- launchers (also the unit tests' entry points)
+void emo_powmel(const float* spec, int pitch, const float* melW, float* mel, long frames, cudaStream_t st) {
+  AGPT_CHECK(frames >= 1 && pitch >= 2 * kBins, "power mel: bad sizes");
+  emo_powmel_kernel<<<(unsigned)frames, kMelThreads, 0, st>>>(spec, pitch, melW, mel);
+  count_launch(1);
+}
+
 void emo_lstm(const float* whh, const float* xp, int N, int T, long seq_stride, float* h_seq, float* h_last, cudaStream_t st) {
   AGPT_CHECK(N >= 1 && T >= 1, "lstm: empty input");
   AGPT_CHECK(seq_stride >= 0, "lstm: negative sequence stride");
@@ -266,10 +270,8 @@ struct EmoNet : Handle {
     AGPT_CHECK(clip > kNfft / 2, "the wav must have at least n_fft / 2 + 1 = 201 samples (reflect padding)");
     AGPT_CHECK(clip < (1L << 31), "the wav is too long");
     const int F = (int)(clip / kHop) + 1;
-    const long tot = (long)F * kNfft;
-    frames.ensure((size_t)tot);
-    cnn14_frames_kernel<<<ew_blocks(tot), 256, 0, st>>>(x, (int)clip, F, kHop, kNfft, frames.p, tot);
-    count_launch(1);
+    frames.ensure((size_t)F * kNfft);
+    cnn14_frames(x, (int)clip, 1, kHop, kNfft, frames.p, st);
     AGPT_CUDA(cudaGetLastError());
     spec.ensure((size_t)F * dft.cout_pad);
     TapConvParams P = tapconv_params(dft, 1, F, 0, 1);
@@ -277,8 +279,7 @@ struct EmoNet : Handle {
     P.out = spec.p; P.out_pitch = dft.cout_pad;
     P.epi = EPI_BIAS;
     tapconv_launch(P, st);
-    emo_powmel_kernel<<<(unsigned)F, kMelThreads, 0, st>>>(spec.p, dft.cout_pad, melW.p, out);
-    count_launch(1);
+    emo_powmel(spec.p, dft.cout_pad, melW.p, out, F, st);
     AGPT_CUDA(cudaGetLastError());
   }
 

@@ -30,6 +30,7 @@
 #include "nn_kernels.h"
 #include "models.h"
 #include "clap.cuh"
+#include "audio_front.cuh"
 
 namespace agpt {
 
@@ -220,6 +221,59 @@ __global__ void istft_finish_kernel(const float* __restrict__ y, long ylen, cons
     out[i] = __fmul_rn(v, scale);
   }
 }
+
+}  // namespace
+
+void lass_input(const float* mag, long sb, long stt, long sf, int B, int T, int Tp, int W, float s, float sh, float* img,
+                cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && T >= 1 && Tp >= T && W >= 1, "LASS input: bad sizes");
+  const long tot = (long)B * Tp * W;
+  lass_input_kernel<<<ew_blocks(tot), 256, 0, st>>>(mag, sb, stt, sf, T, Tp, W, s, sh, reinterpret_cast<float4*>(img), tot);
+  count_launch(1);
+}
+
+void lass_head(const float* x, const float* wb, int B, int T, int Tp, int W, float* mask, float* logits, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && T >= 1 && Tp >= T && W >= 1, "LASS head: bad sizes");
+  const int F = W + 2;
+  const long tot = (long)B * T * F;
+  lass_head_kernel<<<ew_blocks(tot), 256, 0, st>>>(x, wb, T, Tp, W, F, mask, logits, tot);
+  count_launch(1);
+}
+
+void stft_rows(const float* wav, int B, long N, int n, int hop, float* rows, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && n >= 2 && hop >= 1, "STFT rows: bad sizes");
+  if (N <= n / 2)
+    throw Error("STFT: " + std::to_string(N) + " samples are too few for the reflect padding of " + std::to_string(n / 2));
+  const long R = cdivl(N + n, hop);
+  stft_rows_kernel<<<ew_blocks((long)B * R * hop), 256, 0, st>>>(wav, N, n / 2, hop, R, rows, (long)B * R * hop);
+  count_launch(1);
+}
+
+void stft_magphase(const float* spec, int B, long R, int pitch, int nb, int T, float* mag, float* phase, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && T >= 1 && T <= R && nb >= 1 && pitch >= 2 * nb, "STFT magnitude / phase: bad sizes");
+  const long tot = (long)B * nb * T;
+  stft_magphase_kernel<<<ew_blocks(tot), 256, 0, st>>>(spec, R, pitch, nb, T, mag, phase, tot);
+  count_launch(1);
+}
+
+void istft_frames(const float* mag, const float* phase, int B, int nb, int T, int pitch, float* X, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && T >= 2, "the inverse STFT needs at least two frames");
+  AGPT_CHECK(nb >= 1 && pitch >= 2 * nb, "inverse STFT frames: bad sizes");
+  const long tot = (long)B * (T + 1) * pitch;
+  istft_frames_kernel<<<ew_blocks(tot), 256, 0, st>>>(mag, phase, nb, T, pitch, X, tot);
+  count_launch(1);
+}
+
+void istft_finish(const float* y, const float* ws, int B, int T, int n, int hop, float* out, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && T >= 2, "the inverse STFT needs at least two frames");
+  AGPT_CHECK(hop >= 1 && n == 2 * hop, "inverse STFT: filter_length = 2 hop_length");
+  const long n_out = (long)(T - 1) * hop;
+  istft_finish_kernel<<<ew_blocks((long)B * n_out), 256, 0, st>>>(y, (long)(T + 1) * hop, ws, n / 2, (float)n / (float)hop, n_out,
+                                                                  out, (long)B * n_out);
+  count_launch(1);
+}
+
+namespace {
 
 // Every ConvBlockResCond of the UNet; vector offsets index the per-sample FiLM vector buffer
 struct LBlock {
@@ -457,11 +511,7 @@ struct LassNet : Handle {
       lass_film_kernel<<<(unsigned)cdivl(warps * 32, 256), 256, 0, st>>>(hid.p, hid_len, w2.p, jobs(), njobs, B, vec.p, vec_len);
       count_launch(1);
     }
-    {
-      const long tot = (long)B * Tp * W0;
-      lass_input_kernel<<<ew_blocks(tot), 256, 0, st>>>(mag, sb, stt, sf, T, Tp, W0, in_s, in_t, reinterpret_cast<float4*>(bx.p), tot);
-      count_launch(1);
-    }
+    lass_input(mag, sb, stt, sf, B, T, Tp, W0, in_s, in_t, bx.p, st);
     // encoder: two blocks per level, the second one's output is the skip; then 2x2 average pool (floor)
     int bi = 0;
     for (int k = 0; k < kLevels; ++k) {
@@ -500,11 +550,7 @@ struct LassNet : Handle {
       y = bo.p;
     }
     run_block(blocks[bi++], bo.p, bx.p, B, Tp, W0, st);                       // after_conv_block1
-    {
-      const long tot = (long)B * T * F;
-      lass_head_kernel<<<ew_blocks(tot), 256, 0, st>>>(bx.p, head.p, T, Tp, W0, F, out_mask, out_logits, tot);
-      count_launch(1);
-    }
+    lass_head(bx.p, head.p, B, T, Tp, W0, out_mask, out_logits, st);
     AGPT_CUDA(cudaGetLastError());
   }
 };
@@ -576,17 +622,14 @@ struct StftNet : Handle {
     const int T = (int)(N / hop + 1);
     const long R = cdivl(N + n, hop);
     rows.ensure((size_t)B * R * hop);
-    stft_rows_kernel<<<ew_blocks((long)B * R * hop), 256, 0, st>>>(wav, N, n / 2, hop, R, rows.p, (long)B * R * hop);
-    count_launch(1);
+    stft_rows(wav, B, N, n, hop, rows.p, st);
     spec.ensure((size_t)B * R * fwd.cout_pad);
     TapConvParams P = tapconv_params(fwd, B, (int)R, 0, 1);
     P.in = rows.p; P.in_gstride = R * hop; P.in_pitch = hop;
     P.out = spec.p; P.out_gstride = R * fwd.cout_pad; P.out_pitch = fwd.cout_pad;
     P.epi = EPI_BIAS;
     tapconv_launch(P, st);
-    const long tot = (long)B * nb * T;
-    stft_magphase_kernel<<<ew_blocks(tot), 256, 0, st>>>(spec.p, R, fwd.cout_pad, nb, T, mag, phase, tot);
-    count_launch(1);
+    stft_magphase(spec.p, B, R, fwd.cout_pad, nb, T, mag, phase, st);
     AGPT_CUDA(cudaGetLastError());
   }
 
@@ -612,9 +655,7 @@ struct StftNet : Handle {
     AGPT_CHECK(B >= 1 && T >= 2, "the inverse STFT needs at least two frames");
     const int pitch = inv.cin_pad;
     X.ensure((size_t)B * (T + 1) * pitch);
-    const long tot = (long)B * (T + 1) * pitch;
-    istft_frames_kernel<<<ew_blocks(tot), 256, 0, st>>>(mag, phase, nb, T, pitch, X.p, tot);
-    count_launch(1);
+    istft_frames(mag, phase, B, nb, T, pitch, X.p, st);
     Y.ensure((size_t)B * (T + 1) * hop);
     TapConvParams P = tapconv_params(inv, B, T + 1, 0, 1);
     P.in = X.p; P.in_gstride = (long)(T + 1) * pitch; P.in_pitch = pitch;
@@ -622,10 +663,7 @@ struct StftNet : Handle {
     P.epi = EPI_BIAS;
     tapconv_launch(P, st);
     window_sum(T);
-    const long n_out = (long)(T - 1) * hop;
-    istft_finish_kernel<<<ew_blocks((long)B * n_out), 256, 0, st>>>(Y.p, (long)(T + 1) * hop, ws.p, n / 2, (float)n / (float)hop,
-                                                                    n_out, out, (long)B * n_out);
-    count_launch(1);
+    istft_finish(Y.p, ws.p, B, T, n, hop, out, st);
     AGPT_CUDA(cudaGetLastError());
   }
 };

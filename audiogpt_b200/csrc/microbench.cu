@@ -1,9 +1,12 @@
 // Conformance entries: one production launch of the tap-GEMM primitive (tapconv_probe), of a non-contraction
-// kernel (nn_probe) or of a FastSpeech-family element-wise kernel (fs_probe) on caller-owned tensors.
+// kernel (nn_probe), of a FastSpeech-family element-wise kernel (fs_probe) or of an audio / spectrogram kernel
+// (audio_probe) on caller-owned tensors.
 #include "tapconv.cuh"
 #include "models.h"
 #include "nn_kernels.h"
 #include "fs_layers.cuh"
+#include "audio_front.cuh"
+#include "clap.cuh"
 
 namespace agpt {
 
@@ -152,6 +155,53 @@ void fs_probe(const agpt_fs_probe_args& a, cudaStream_t st) {
     case AGPT_FS_PE_MASK: pe_mask(a.x, a.y, a.rows, a.M, st); break;
     case AGPT_FS_PE_DENORM: pe_denorm(a.x, a.x2, a.y, a.y2, a.rows, a.use_uv, a.norm, a.mean, a.std_, st); break;
     default: throw Error("fs probe: unknown op " + std::to_string(a.op));
+  }
+  AGPT_CUDA(cudaStreamSynchronize(st));
+}
+
+// One call of a production audio / spectrogram launcher on caller-owned tensors (agpt_audio_probe, include/agpt_b200.h).
+void audio_probe(const agpt_audio_probe_args& a, cudaStream_t st) {
+  switch (a.op) {
+    case AGPT_AU_FRAMES:
+      AGPT_CHECK(a.N < (1L << 31), "framing: the clip is too long");
+      cnn14_frames(a.x, (int)a.N, a.B, a.hop, a.n, a.y, st);
+      break;
+    case AGPT_AU_LOGMEL: cnn14_logmel(a.x, a.pitch, a.nb, a.w, a.nm, a.g, a.b, a.y, a.rows, a.ch, st); break;
+    case AGPT_AU_POWMEL: emo_powmel(a.x, a.pitch, a.w, a.y, a.rows, st); break;
+    case AGPT_AU_STFT_ROWS: stft_rows(a.x, a.B, a.N, a.n, a.hop, a.y, st); break;
+    case AGPT_AU_MAGPHASE: stft_magphase(a.x, a.B, a.R, a.pitch, a.nb, a.T, a.y, a.y2, st); break;
+    case AGPT_AU_ISTFT_FRAMES: istft_frames(a.x, a.x2, a.B, a.nb, a.T, a.pitch, a.y, st); break;
+    case AGPT_AU_ISTFT_FINISH: istft_finish(a.x, a.x2, a.B, a.T, a.n, a.hop, a.y, st); break;
+    case AGPT_AU_RESAMPLE: {
+      AGPT_CHECK(a.starts && a.B >= 1, "resampler: starts [B] (host) is required");
+      DevBuf sd;
+      cnn14_resample(a.x, a.N, a.B, a.w, a.orig, a.nw, a.width, a.starts, sd, a.clip, a.y, st);
+      AGPT_CUDA(cudaStreamSynchronize(st));   // sd is freed on return
+      break;
+    }
+    case AGPT_AU_CNN14_HEAD: cnn14_head(a.x, a.B, a.T, a.F, a.C, a.y, st); break;
+    case AGPT_AU_L2NORM2:
+      AGPT_CHECK(a.rows >= 1 && a.D >= 1, "l2norm2: bad sizes");
+      clap_l2norm2(a.x, a.y, (int)a.rows, a.D, st);
+      break;
+    case AGPT_AU_SIMILARITY: clap_similarity(a.x, a.Na, a.x2, a.Nt, a.D, a.scale, a.y, st); break;
+    case AGPT_AU_LASS_INPUT:
+      AGPT_CHECK(a.T >= 1, "LASS input: T >= 1");
+      lass_input(a.x, a.sb, a.stt, a.sf, a.B, a.T, round_up(a.T, 64), a.W, a.scale, a.shift, a.y, st);
+      break;
+    case AGPT_AU_LASS_HEAD:
+      AGPT_CHECK(a.T >= 1, "LASS head: T >= 1");
+      lass_head(a.x, a.w, a.B, a.T, round_up(a.T, 64), a.W, a.y, a.y2, st);
+      break;
+    case AGPT_AU_W2V_STEM: {
+      AGPT_CHECK(a.k0 >= 1 && a.s0 >= 1 && a.N >= a.k0 && a.s1 >= 0, "conv0: bad sizes");
+      const long T0 = (a.N - a.k0) / a.s0 + 1;
+      AGPT_CHECK(T0 <= (1 << 24), "conv0: input too long");
+      const int zpad = a.s1 > 0 ? round_up((int)T0, a.s1) - (int)T0 : 0;
+      w2v_stem(a.x, a.N, a.B, (int)T0, zpad, a.C, a.w, a.k0, a.s0, a.g, a.b, a.eps, a.part, a.stat, a.cnt, a.y, a.R, st);
+      break;
+    }
+    default: throw Error("audio probe: unknown op " + std::to_string(a.op));
   }
   AGPT_CUDA(cudaStreamSynchronize(st));
 }

@@ -20,6 +20,7 @@
 #include "nn_kernels.h"
 #include "models.h"
 #include "clap.cuh"
+#include "audio_front.cuh"
 
 namespace agpt {
 
@@ -253,6 +254,20 @@ __global__ void __launch_bounds__(192) pos_conv_fma_kernel(const float* __restri
 
 }  // namespace
 
+void w2v_stem(const float* x, long S, int B, int T0, int zpad, int C, const float* w0, int k0, int s0, const float* gamma,
+              const float* beta, float eps, void* part, void* stat, int* cnt, float* out, long R, cudaStream_t st) {
+  AGPT_CHECK(k0 >= 1 && k0 <= kStemMaxK && s0 >= 1 && s0 <= 64, "conv0: k0 must be 1..16 and s0 1..64");
+  AGPT_CHECK(C >= 1 && C <= 1024, "conv0: at most 1024 channels (one thread each)");
+  AGPT_CHECK(B >= 1 && T0 >= 1 && zpad >= 0 && R >= (long)T0 + zpad && (long)(T0 - 1) * s0 + k0 <= S, "conv0: bad sizes");
+  const int nch = cdiv(T0, kStemRows);
+  const size_t xs_bytes = sizeof(float) * ((kStemRows - 1) * s0 + k0);
+  w2v_stem_stats_kernel<<<dim3(nch, B), C, xs_bytes, st>>>(x, S, T0, C, w0, k0, s0, static_cast<double2*>(part),
+                                                         static_cast<float2*>(stat), cnt, eps);
+  w2v_stem_apply_kernel<<<dim3(cdiv(T0 + zpad, kStemRows), B), C, xs_bytes, st>>>(
+      x, S, T0, zpad, C, w0, k0, s0, static_cast<const float2*>(stat), gamma, beta, out, R);
+  count_launch(2);
+}
+
 // conv output lengths T_0 .. T_{n-1} of an S-sample input (0 from the first layer without a frame on)
 static void w2v_conv_lengths(const agpt_w2v_cfg& c, long S, std::vector<int>& T) {
   T.assign(c.conv_layers, 0);
@@ -300,14 +315,9 @@ void W2vNet::features(const float* x, int B, long S, cudaStream_t st) {
     cnt.ensure(B);
     AGPT_CUDA(cudaMemsetAsync(cnt.p, 0, sizeof(int) * B, st));
   }
-  const size_t xs_bytes = sizeof(float) * ((kStemRows - 1) * s0 + k0);
   const float gn_eps = 1e-5f;                                 // nn.GroupNorm's default (Wav2Vec2GroupNormConvLayer)
-  w2v_stem_stats_kernel<<<dim3(nch, B), C, xs_bytes, st>>>(x, S, T[0], C, w0.p, k0, s0, reinterpret_cast<double2*>(part.p),
-                                                         reinterpret_cast<float2*>(stat.p), reinterpret_cast<int*>(cnt.p), gn_eps);
   const int zpad = n > 1 ? round_up(T[0], cfg.conv_stride[1]) - T[0] : 0;
-  w2v_stem_apply_kernel<<<dim3(cdiv(T[0] + zpad, kStemRows), B), C, xs_bytes, st>>>(
-      x, S, T[0], zpad, C, w0.p, k0, s0, reinterpret_cast<const float2*>(stat.p), gng.p, gnb.p, fa.p, R);
-  count_launch(2);
+  w2v_stem(x, S, B, T[0], zpad, C, w0.p, k0, s0, gng.p, gnb.p, gn_eps, part.p, stat.p, reinterpret_cast<int*>(cnt.p), fa.p, R, st);
   AGPT_CUDA(cudaGetLastError());
   float* cur = fa.p;
   float* nxt = fb.p;

@@ -205,6 +205,48 @@ typedef struct agpt_fs_probe_args {
   float escale, neg_emb, xscale, alpha, mean, std_;
 } agpt_fs_probe_args;
 int agpt_fs_probe(const agpt_fs_probe_args* args, void* stream);
+/* Conformance entry of the kernels that touch audio samples and spectrogram bins (logmel front end, emotion power mel,
+ * STFT / inverse STFT, LASS's mask input and output stores, Cnn14's resampler and pooling head, the CLAP scorer's L2
+ * norms and similarity, wav2vec2's conv stem; tests/test_audio_kernels_gpu.py): ONE call of the production launcher
+ * selected by `op` on caller-owned device tensors, with the arguments as given.  Tensors are fp32 device arrays except
+ * `starts` (int32, HOST), `cnt` (int32) and the stem workspaces `part` (double2) / `stat` (float2).  The launcher's
+ * preconditions are checked first; a violation returns an error with nothing launched.  The fields each op reads:
+ *   FRAMES        x [B][N] -> y [B][N / hop + 1][n]; N > n / 2
+ *   LOGMEL        x = spec [rows][pitch] ([re | im], nb bins each), w = melW [nb][nm], g = bn0 scale [nm], b = bn0
+ *                 shift [nm], ch (1 or 4) -> y [rows][nm][ch]
+ *   POWMEL        x = spec [rows][pitch] (201 bins each), w = melW [201][40] -> y [rows][40]
+ *   STFT_ROWS     x = wav [B][N], n, hop -> y [B][ceil((N + n) / hop)][hop]; N > n / 2
+ *   MAGPHASE      x = spec [B][R][pitch], nb, T -> y = mag, y2 = phase [B][nb][T]
+ *   ISTFT_FRAMES  x = mag, x2 = phase [B][nb][T], pitch -> y [B][T + 1][pitch]; T >= 2
+ *   ISTFT_FINISH  x = overlap-added y [B][(T + 1) hop], x2 = window sum [(T + 1) hop], n = 2 hop -> y [B][(T - 1) hop];
+ *                 T >= 2
+ *   RESAMPLE      x [B][N], w = kernel [nw][2 width + orig], orig, nw, width, starts [B] (host), clip -> y [B][clip]
+ *   CNN14_HEAD    x [B][T][F][C] -> y [B][C]
+ *   L2NORM2       x [rows][D] -> y [rows][D]
+ *   SIMILARITY    x = a [Na][D], x2 = t [Nt][D], scale -> y [Na][Nt]
+ *   LASS_INPUT    x = mag at element strides sb / stt / sf, B, T, W, scale, shift -> y [B][64 ceil(T / 64)][W][4]
+ *   LASS_HEAD     x [B][64 ceil(T / 64)][W][32], w = after_conv2 [33] (32 weights, bias) -> y = mask, y2 = logits (null =
+ *                 none) [B][T][W + 2]
+ *   W2V_STEM      x [B][N], w = conv0 [C][k0], s0, g = gamma [C], b = beta [C], eps, s1 (the next conv's stride; 0 = no
+ *                 zero rows), part, stat, cnt (zero) -> y [B][R][C]; T0 = (N - k0) / s0 + 1 rows plus
+ *                 round_up(T0, s1) - T0 zero rows; k0 <= 16, C <= 1024
+ * Synchronises `stream` before returning.                                                                          */
+enum {
+  AGPT_AU_FRAMES = 0, AGPT_AU_LOGMEL, AGPT_AU_POWMEL, AGPT_AU_STFT_ROWS, AGPT_AU_MAGPHASE, AGPT_AU_ISTFT_FRAMES,
+  AGPT_AU_ISTFT_FINISH, AGPT_AU_RESAMPLE, AGPT_AU_CNN14_HEAD, AGPT_AU_L2NORM2, AGPT_AU_SIMILARITY, AGPT_AU_LASS_INPUT,
+  AGPT_AU_LASS_HEAD, AGPT_AU_W2V_STEM
+};
+typedef struct agpt_audio_probe_args {
+  int op;
+  const float* x; const float* x2; const float* w; const float* g; const float* b;
+  const int* starts;
+  float* y; float* y2;
+  void* part; void* stat; int* cnt;
+  int B, T, F, C, D, W, n, hop, nb, nm, ch, pitch, Na, Nt, k0, s0, s1, orig, nw, width, clip;
+  long rows, N, R, sb, stt, sf;
+  float scale, shift, eps;
+} agpt_audio_probe_args;
+int agpt_audio_probe(const agpt_audio_probe_args* args, void* stream);
 
 /* ------------------------------------------------------------------ HiFi-GAN
  * Replaces HifiGanGenerator.__init__/forward/remove_weight_norm

@@ -429,3 +429,15 @@ def test_fs_probe_args_mirror_the_header():
     names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
     assert names == ["AGPT_FS_" + n for n in _lib.FS_OPS]
     assert "AGPT_FS_EMBED_TOKENS = 0" in enum and enum.count("=") == 1
+
+
+def test_audio_probe_args_mirror_the_header():
+    """_lib.AudioProbeArgs has the fields of agpt_audio_probe_args in the header's order and C types, and _lib.AU_OPS
+    lists the AGPT_AU_* selectors in the enum's order (a mismatch would run another kernel or shift its arguments)."""
+    from audiogpt_b200 import _lib
+    want = _header_struct_fields("agpt_audio_probe_args")
+    assert [(n, t) for n, t in _lib.AudioProbeArgs._fields_] == want
+    enum = re.search(r"enum \{([^}]*AGPT_AU_FRAMES[^}]*)\}", _header(), re.S).group(1)
+    names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
+    assert names == ["AGPT_AU_" + n for n in _lib.AU_OPS]
+    assert "AGPT_AU_FRAMES = 0" in enum and enum.count("=") == 1
