@@ -198,6 +198,18 @@ class AudioProbeArgs(C.Structure):
         (n, C.c_float) for n in ("scale", "shift", "eps")]
 
 
+# agpt_voc_probe_args.op, in the header's enum order (AGPT_VC_<name>)
+VC_OPS = ("CF_TO_CL", "CONV_POST", "AA_SNAKE", "NSF_ADD", "STEP_EMBED", "STEP_EMBED_DEV", "P_SAMPLE_TAB")
+
+
+class VocProbeArgs(C.Structure):
+    """agpt_voc_probe_args (a tagged struct in the header: it carries pointers, ints, longs and a float)."""
+    _fields_ = [("op", C.c_int)] + [(n, C.c_void_p) for n in (
+        "x", "w", "b", "a", "inv_b", "taps", "t", "ctr", "noises_pp", "y", "ran")] + [(n, C.c_int) for n in (
+        "B", "L", "C", "c_out", "Lh", "K", "st", "pad", "nsteps", "clip")] + [
+        (n, C.c_long) for n in ("n", "noise_stride")] + [("slope", C.c_float)]
+
+
 # (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
 # takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
 _I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
@@ -226,6 +238,7 @@ PROTOTYPES = {
     "agpt_nn_probe": (_I, [_P, _P]),
     "agpt_fs_probe": (_I, [_P, _P]),
     "agpt_audio_probe": (_I, [_P, _P]),
+    "agpt_voc_probe": (_I, [_P, _P]),
     "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
     "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "agpt_hifigan_vocode_host": (_I, [_P, _P, _P, _I, _I, _P]),

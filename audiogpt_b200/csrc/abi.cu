@@ -685,4 +685,11 @@ int agpt_audio_probe(const agpt_audio_probe_args* args, void* stream) {
   });
 }
 
+int agpt_voc_probe(const agpt_voc_probe_args* args, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(args, "null argument");
+    voc_probe(*args, (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

@@ -6,6 +6,7 @@
 #include "tapconv.cuh"
 #include "models.h"
 #include "nn_kernels.h"
+#include "voc_kernels.cuh"
 
 namespace agpt {
 
@@ -70,6 +71,39 @@ __global__ void p_sample_tab_kernel(float* __restrict__ x, const float* __restri
     if (noise) o += s * noise[base + i];
     x[base + i] = o;
   }
+}
+
+// net.py:41: emb = log(10000) / (half_dim - 1), rounded to fp32 once on the host
+static float step_embed_neg_emb(int C) {
+  AGPT_CHECK(C % 2 == 0 && C / 2 > 1, "step embedding: needs an even C with C / 2 > 1 (the exponent divides by C / 2 - 1)");
+  return (float)(-(std::log(10000.0) / (double)(C / 2 - 1)));
+}
+
+void diff_step_embed(const int* t_host, float* out, int B, int C, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && B <= kMaxBatchParam && t_host, "step embedding: needs 1 <= B <= 256 host timesteps");
+  const float neg_emb = step_embed_neg_emb(C);
+  StepT stp;
+  for (int b = 0; b < B; ++b) stp.t[b] = t_host[b];
+  diff_step_embed_kernel<<<B, 128, 0, st>>>(out, stp, B, C, neg_emb);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+}
+
+void diff_step_embed_dev(const int* t_dev, float* out, int N, int C, cudaStream_t st) {
+  AGPT_CHECK(N >= 1, "step embedding: needs N >= 1");
+  const float neg_emb = step_embed_neg_emb(C);
+  diff_step_embed_dev_kernel<<<N, 128, 0, st>>>(out, t_dev, C, neg_emb);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+}
+
+void p_sample_tab(float* x, const float* eps, const float* const* noises_pp, long noise_stride, const float* coef_tab,
+                  const int* ctr, int nsteps, int clip, int B, long n, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && n >= 1 && nsteps >= 1, "p_sample_tab: needs B >= 1, n >= 1 and nsteps >= 1");
+  dim3 grid((unsigned)std::min<long>(cdivl(n, 256), 1184), B);
+  p_sample_tab_kernel<<<grid, dim3(256), 0, st>>>(x, eps, noises_pp, noise_stride, coef_tab, ctr, nsteps, clip, n);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
 }
 
 __global__ void axpby5_kernel(const float* __restrict__ x, const float* __restrict__ e0, const float* __restrict__ e1,
@@ -172,12 +206,7 @@ struct Diffnet : Handle {
     AGPT_CHECK(B > 0, "agpt_diffnet_set_cond must be called first");
     const int C = cfg.residual_channels, L = cfg.residual_layers;
     ensure_bufs();
-    StepT stp;
-    for (int b = 0; b < B; ++b) stp.t[b] = t_host[b];
-    const float neg_emb = (float)(-(std::log(10000.0) / (double)(C / 2 - 1)));
-    diff_step_embed_kernel<<<B, 128, 0, st>>>(emb.p, stp, B, C, neg_emb);
-    count_launch(1);
-    AGPT_CUDA(cudaGetLastError());
+    diff_step_embed(t_host, emb.p, B, C, st);
     step_mlp(emb.p, B, e1.p, e2.p, dproj.p, st);
     eps_core(x, dproj.p, L * C, out, st);
   }
@@ -328,10 +357,7 @@ void gd_sample_loop(Handle* hh, float* x_io, int t_hi, int t_lo, const float* co
   {
     DevBuf &te = h->z, &t1 = h->skip, &t2 = h->hbuf;      // scratch: free before the first step
     te.ensure((size_t)nsteps * C); t1.ensure((size_t)nsteps * 4 * C); t2.ensure((size_t)nsteps * C);
-    const float neg_emb = (float)(-(std::log(10000.0) / (double)(C / 2 - 1)));
-    diff_step_embed_dev_kernel<<<nsteps, 128, 0, st>>>(te.p, reinterpret_cast<const int*>(h->t_dev.p), C, neg_emb);
-    count_launch(1);
-    AGPT_CUDA(cudaGetLastError());
+    diff_step_embed_dev(reinterpret_cast<const int*>(h->t_dev.p), te.p, nsteps, C, st);
     h->step_mlp(te.p, nsteps, t1.p, t2.p, h->dproj_table.p, st);
     h->ensure_bufs();                                        // (scratch may have grown the buffers: keep sizes valid)
   }
@@ -341,10 +367,7 @@ void gd_sample_loop(Handle* hh, float* x_io, int t_hi, int t_lo, const float* co
   auto step = [&](cudaStream_t s) {
     select_row(h->dproj_table.p, ctr, h->dproj_cur.p, L * C, s);
     h->eps_core(xl, h->dproj_cur.p, 0, h->loop_eps.p, s);
-    dim3 grid((unsigned)std::min<long>(cdivl(n, 256), 1184), B);
-    p_sample_tab_kernel<<<grid, dim3(256), 0, s>>>(xl, h->loop_eps.p, noise_pp, noise_stride, h->coef_table.p, ctr, nsteps, clip, n);
-    count_launch(1);
-    AGPT_CUDA(cudaGetLastError());
+    p_sample_tab(xl, h->loop_eps.p, noise_pp, noise_stride, h->coef_table.p, ctr, nsteps, clip, B, n, s);
     step_inc(ctr, s);
   };
   const long long l0 = launch_count_now();

@@ -4,6 +4,7 @@
 #include "common.cuh"
 #include "tapconv.cuh"
 #include "models.h"
+#include "voc_kernels.cuh"
 
 namespace agpt {
 
@@ -112,6 +113,23 @@ __global__ void __launch_bounds__(CP_ROWS) conv_post32_kernel(const float* __res
   }
 }
 
+bool launch_conv_post(const float* in, const float* w, const float* b, float* out, int B, int L, int C, int c_out,
+                      float slope, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && L >= 1 && c_out >= 1 && C >= 4 && C % 4 == 0, "conv_post: needs C % 4 == 0 (float4 rows)");
+  const size_t smem = (size_t)c_out * 7 * C * sizeof(float);
+  AGPT_CHECK(smem <= 48 * 1024, "conv_post: c_out * 7 * C weights exceed 48 KB of shared memory");
+  const int threads = 256;
+  dim3 grid(cdiv(L, threads), B);
+  const bool c32 = C == 32 && smem <= 8 * 1024;
+  if (c32)
+    conv_post32_kernel<<<grid, CP_ROWS, smem, st>>>(in, w, b, out, L, c_out, slope);
+  else
+    conv_post_kernel<<<grid, threads, smem, st>>>(in, w, b, out, L, C, c_out, slope);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+  return c32;
+}
+
 // Anti-aliased periodic activation of BigVGAN (Activation1d(Snake | SnakeBeta),
 // vocoder/bigvgan/alias_free_torch/act.py:22-27, resample.py:22-31, filter.py:80-90, activations.py:46-57,104-117):
 //   u = 2 * upfir2(replicate_pad(x, 5))[15:-15]          (12-tap Kaiser sinc, zero-stuffing stride 2: 6 taps per sample)
@@ -167,6 +185,17 @@ __global__ void __launch_bounds__(256) aa_snake_kernel(const float* __restrict__
   }
 }
 
+void aa_snake(const float* x, float* y, const float* a, const float* inv_b, const float* taps, int B, int L, int C,
+              cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && L >= 1 && C >= 1 && taps, "aa_snake: needs L >= 1 and the 12 filter taps");
+  AaFilter F;
+  for (int k = 0; k < 12; ++k) F.f[k] = taps[k];
+  dim3 block(32, 8), grid(cdiv(L, AA_TT), cdiv(C, 32), B);
+  aa_snake_kernel<<<grid, block, 0, st>>>(x, y, a, inv_b, L, C, F);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
+}
+
 // NSF excitation add: x[b][p][c] += bias[c] + sum_k w[c][k] * har[b][p*st - pad + k]   (hifigan.py:155-157)
 __global__ void nsf_add_kernel(float* __restrict__ x, const float* __restrict__ har, const float* __restrict__ w,
                                const float* __restrict__ bias, int L, int C, int Lh, int K, int st, int pad) {
@@ -182,6 +211,15 @@ __global__ void nsf_add_kernel(float* __restrict__ x, const float* __restrict__ 
     if (q >= 0 && q < Lh) acc = fmaf(w[c * K + k], hb[q], acc);
   }
   x[((long)b * L + p) * C + c] += acc;
+}
+
+void nsf_add(float* x, const float* har, const float* w, const float* bias, int B, int L, int C, int Lh, int K, int stride,
+             int pad, cudaStream_t st) {
+  AGPT_CHECK(B >= 1 && L >= 1 && C >= 1 && K >= 1 && stride >= 1, "nsf_add: needs K >= 1 and stride >= 1");
+  dim3 block(32, 8), grid(cdiv(L, 8), cdiv(C, 32), B);
+  nsf_add_kernel<<<grid, block, 0, st>>>(x, har, w, bias, L, C, Lh, K, stride, pad);
+  count_launch(1);
+  AGPT_CUDA(cudaGetLastError());
 }
 
 // ------------------------------------------------------------------ NSF harmonic source (SourceModuleHnNSF)
@@ -405,10 +443,7 @@ struct Hifigan : Handle {
       if (has_plane(ch)) plane_split(t, plane_hi(t), plane_hi(t) + mxp, rows * ch, 0.1f, st);
     };
     auto snake = [&](const float* src, float* dst, long Lr, int Cr, const SnakeW& w) {
-      dim3 block(32, 8), grid(cdiv((int)Lr, AA_TT), cdiv(Cr, 32), B);
-      aa_snake_kernel<<<grid, block, 0, st>>>(src, dst, w.a.p, w.inv_b.p, (int)Lr, Cr, aaf);
-      count_launch(1);
-      AGPT_CUDA(cudaGetLastError());
+      aa_snake(src, dst, w.a.p, w.inv_b.p, aaf.f, B, (int)Lr, Cr, st);
     };
     launch_cf_to_cl(mel, melT.p, B, cfg.n_mels, T, st);
     {
@@ -439,10 +474,7 @@ struct Hifigan : Handle {
       if (har) {
         AGPT_CHECK(cfg.use_nsf, "har_source given but the generator has no noise_convs");
         const NoiseConvW& nc = noise[i];
-        dim3 block(32, 8), grid(cdiv((int)L, 8), cdiv(C, 32), B);
-        nsf_add_kernel<<<grid, block, 0, st>>>(X, har, nc.w.p, nc.b.p, (int)L, C, T * hop, nc.K, nc.st, nc.pad);
-        count_launch(1);
-        AGPT_CUDA(cudaGetLastError());
+        nsf_add(X, har, nc.w.p, nc.b.p, B, (int)L, C, T * hop, nc.K, nc.st, nc.pad, st);
         split(X, (long)B * L, C);   // the plane of X after the excitation add
       }
       const long gs = L * C;
@@ -512,18 +544,10 @@ struct Hifigan : Handle {
       std::swap(cur, acc);
     }
     {
-      const int threads = 256;
-      dim3 grid(cdiv((int)L, threads), B);
-      const size_t smem = (size_t)cfg.c_out * 7 * C * sizeof(float);
       const float* pin = cur;
       float slope = 0.01f;                      // HiFi-GAN: F.leaky_relu default slope (hifigan.py:165)
       if (big) { snake(cur, S, L, C, act_post); pin = S; slope = 1.f; }   // BigVGAN: activation_post, no leaky-relu
-      if (C == 32 && smem <= 8 * 1024)
-        conv_post32_kernel<<<grid, CP_ROWS, smem, st>>>(pin, post_w.p, post_b.p, wav, (int)L, cfg.c_out, slope);
-      else
-        conv_post_kernel<<<grid, threads, smem, st>>>(pin, post_w.p, post_b.p, wav, (int)L, C, cfg.c_out, slope);
-      count_launch(1);
-      AGPT_CUDA(cudaGetLastError());
+      launch_conv_post(pin, post_w.p, post_b.p, wav, B, (int)L, C, cfg.c_out, slope, st);
     }
   }
 };

@@ -1,12 +1,13 @@
 // Conformance entries: one production launch of the tap-GEMM primitive (tapconv_probe), of a non-contraction
-// kernel (nn_probe), of a FastSpeech-family element-wise kernel (fs_probe) or of an audio / spectrogram kernel
-// (audio_probe) on caller-owned tensors.
+// kernel (nn_probe), of a FastSpeech-family element-wise kernel (fs_probe), of an audio / spectrogram kernel
+// (audio_probe) or of a vocoder / diffusion-step kernel (voc_probe) on caller-owned tensors.
 #include "tapconv.cuh"
 #include "models.h"
 #include "nn_kernels.h"
 #include "fs_layers.cuh"
 #include "audio_front.cuh"
 #include "clap.cuh"
+#include "voc_kernels.cuh"
 
 namespace agpt {
 
@@ -202,6 +203,30 @@ void audio_probe(const agpt_audio_probe_args& a, cudaStream_t st) {
       break;
     }
     default: throw Error("audio probe: unknown op " + std::to_string(a.op));
+  }
+  AGPT_CUDA(cudaStreamSynchronize(st));
+}
+
+// One call of a production vocoder / diffusion-step launcher on caller-owned tensors (agpt_voc_probe, include/agpt_b200.h).
+void voc_probe(const agpt_voc_probe_args& a, cudaStream_t st) {
+  switch (a.op) {
+    case AGPT_VC_CF_TO_CL:
+      AGPT_CHECK(a.B >= 1 && a.C >= 1 && a.L >= 1, "cf_to_cl: bad sizes");
+      launch_cf_to_cl(a.x, a.y, a.B, a.C, a.L, st);
+      break;
+    case AGPT_VC_CONV_POST: {
+      const bool c32 = launch_conv_post(a.x, a.w, a.b, a.y, a.B, a.L, a.C, a.c_out, a.slope, st);
+      if (a.ran) *a.ran = c32 ? 1 : 0;
+      break;
+    }
+    case AGPT_VC_AA_SNAKE: aa_snake(a.x, a.y, a.a, a.inv_b, a.taps, a.B, a.L, a.C, st); break;
+    case AGPT_VC_NSF_ADD: nsf_add(a.y, a.x, a.w, a.b, a.B, a.L, a.C, a.Lh, a.K, a.st, a.pad, st); break;
+    case AGPT_VC_STEP_EMBED: diff_step_embed(a.t, a.y, a.B, a.C, st); break;
+    case AGPT_VC_STEP_EMBED_DEV: diff_step_embed_dev(a.t, a.y, a.B, a.C, st); break;
+    case AGPT_VC_P_SAMPLE_TAB:
+      p_sample_tab(a.y, a.x, a.noises_pp, a.noise_stride, a.w, a.ctr, a.nsteps, a.clip, a.B, a.n, st);
+      break;
+    default: throw Error("voc probe: unknown op " + std::to_string(a.op));
   }
   AGPT_CUDA(cudaStreamSynchronize(st));
 }

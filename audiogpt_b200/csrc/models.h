@@ -129,5 +129,6 @@ void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st
 void nn_probe(const agpt_nn_probe_args& a, cudaStream_t st);
 void fs_probe(const agpt_fs_probe_args& a, cudaStream_t st);
 void audio_probe(const agpt_audio_probe_args& a, cudaStream_t st);
+void voc_probe(const agpt_voc_probe_args& a, cudaStream_t st);
 
 }  // namespace agpt

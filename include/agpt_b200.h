@@ -247,6 +247,39 @@ typedef struct agpt_audio_probe_args {
   float scale, shift, eps;
 } agpt_audio_probe_args;
 int agpt_audio_probe(const agpt_audio_probe_args* args, void* stream);
+/* Conformance entry of the vocoder and diffusion-step kernels that no other entry reaches on their own (HiFi-GAN /
+ * BigVGAN layout, conv_post, BigVGAN's anti-aliased Snake, the NSF excitation add, DiffNet's step embedding and the
+ * graph-replayed p_sample step; tests/test_vocoder_kernels_gpu.py): ONE call of the production launcher selected by
+ * `op` on caller-owned device tensors, with the arguments as given.  Tensors are fp32 device arrays except `taps`
+ * (fp32, HOST), `t` (int32: HOST for STEP_EMBED, device for STEP_EMBED_DEV), `ctr` (int32, device), `noises_pp` (a
+ * device slot holding a device pointer) and `ran` (int32, HOST).  The launcher's preconditions are checked first; a
+ * violation returns an error with nothing launched.  The fields each op reads:
+ *   CF_TO_CL        x [B][C][L] -> y [B][L][C]
+ *   CONV_POST       x [B][L][C], w [c_out][7][C], b [c_out], slope -> y [B][c_out][L]; ran (null = not reported) <- 1
+ *                   when conv_post32_kernel ran, 0 for the generic kernel; C % 4 == 0, c_out 7 C 4 bytes <= 48 KB
+ *   AA_SNAKE        x [B][L][C], a [C], inv_b [C], taps [12] -> y [B][L][C]; L >= 1
+ *   NSF_ADD         y [B][L][C] in place, x = har [B][Lh], w [C][K], b [C], K, st, pad; K >= 1, st >= 1
+ *   STEP_EMBED      t [B] (host) -> y [B][C]; B <= 256, C even, C / 2 > 1
+ *   STEP_EMBED_DEV  t [B] (device) -> y [B][C]; C even, C / 2 > 1
+ *   P_SAMPLE_TAB    y = x [B][n] in place, x = eps [B][n], w = coefficient table [nsteps][5], ctr [1], nsteps,
+ *                   noises_pp, noise_stride, clip; nsteps >= 1
+ * Synchronises `stream` before returning.                                                                          */
+enum {
+  AGPT_VC_CF_TO_CL = 0, AGPT_VC_CONV_POST, AGPT_VC_AA_SNAKE, AGPT_VC_NSF_ADD, AGPT_VC_STEP_EMBED, AGPT_VC_STEP_EMBED_DEV,
+  AGPT_VC_P_SAMPLE_TAB
+};
+typedef struct agpt_voc_probe_args {
+  int op;
+  const float* x; const float* w; const float* b; const float* a; const float* inv_b; const float* taps;
+  const int* t; const int* ctr;
+  const float* const* noises_pp;
+  float* y;
+  int* ran;
+  int B, L, C, c_out, Lh, K, st, pad, nsteps, clip;
+  long n, noise_stride;
+  float slope;
+} agpt_voc_probe_args;
+int agpt_voc_probe(const agpt_voc_probe_args* args, void* stream);
 
 /* ------------------------------------------------------------------ HiFi-GAN
  * Replaces HifiGanGenerator.__init__/forward/remove_weight_norm

@@ -441,3 +441,15 @@ def test_audio_probe_args_mirror_the_header():
     names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
     assert names == ["AGPT_AU_" + n for n in _lib.AU_OPS]
     assert "AGPT_AU_FRAMES = 0" in enum and enum.count("=") == 1
+
+
+def test_voc_probe_args_mirror_the_header():
+    """_lib.VocProbeArgs has the fields of agpt_voc_probe_args in the header's order and C types, and _lib.VC_OPS lists
+    the AGPT_VC_* selectors in the enum's order (a mismatch would run another kernel or shift its arguments)."""
+    from audiogpt_b200 import _lib
+    want = _header_struct_fields("agpt_voc_probe_args")
+    assert [(n, t) for n, t in _lib.VocProbeArgs._fields_] == want
+    enum = re.search(r"enum \{([^}]*AGPT_VC_CF_TO_CL[^}]*)\}", _header(), re.S).group(1)
+    names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
+    assert names == ["AGPT_VC_" + n for n in _lib.VC_OPS]
+    assert "AGPT_VC_CF_TO_CL = 0" in enum and enum.count("=") == 1
