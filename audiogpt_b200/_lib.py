@@ -210,6 +210,21 @@ class VocProbeArgs(C.Structure):
         (n, C.c_long) for n in ("n", "noise_stride")] + [("slope", C.c_float)]
 
 
+# agpt_an_probe_args.op, in the header's enum order (AGPT_AN_<name>)
+AN_OPS = ("LASS_AFFINE", "LASS_UPCOL", "LASS_SHUFFLE", "LASS_FILM", "LASS_FILM_VEC", "LASS_UP", "TSD_PAD4", "TSD_FUSE",
+          "TSD_REFEMB", "TSD_HEAD", "TSD_MIX_INTERP", "CLAP_EMBED", "CLAP_EMBED_TYPED", "CLAP_GELU", "EMO_MEAN_NORM",
+          "EMO_LINEAR_NORM")
+
+
+class AnProbeArgs(C.Structure):
+    """agpt_an_probe_args (a tagged struct in the header: it carries a handle, pointers, ints and longs)."""
+    _fields_ = [("op", C.c_int)] + [(n, C.c_void_p) for n in (
+        "h", "x", "x2", "s", "t", "w", "b", "w2", "b2", "vec", "alpha", "beta", "ids", "type_ids", "mask", "woff", "hoff",
+        "nin", "dst", "ja", "jb", "y", "y2", "scratch", "kpm", "info")] + [(n, C.c_int) for n in (
+        "B", "C", "hh", "ww", "level", "nj", "hid_len", "vec_len", "vec_off", "Td", "T", "O", "n", "att_pool", "N", "L", "H",
+        "E", "vocab", "ntypes", "max_blocks")] + [(n, C.c_long) for n in ("rows", "rows_per_sample")]
+
+
 # (restype, argtypes) of every entry point of include/agpt_b200.h.  Every data pointer and stream is a c_void_p, which
 # takes fptr(t), ndarray.ctypes.data_as(...), ctypes arrays, string buffers, byref(...) and None alike.
 _I, _L, _F, _D, _P = C.c_int, C.c_long, C.c_float, C.c_double, C.c_void_p
@@ -239,6 +254,7 @@ PROTOTYPES = {
     "agpt_fs_probe": (_I, [_P, _P]),
     "agpt_audio_probe": (_I, [_P, _P]),
     "agpt_voc_probe": (_I, [_P, _P]),
+    "agpt_an_probe": (_I, [_P, _P]),
     "agpt_hifigan_create": (_I, [C.POINTER(HifiganCfg), _W, _I, _I, _OUT]),
     "agpt_hifigan_forward": (_I, [_P, _P, _P, _I, _I, _P, _P]),
     "agpt_hifigan_vocode_host": (_I, [_P, _P, _P, _I, _I, _P]),

@@ -692,4 +692,13 @@ int agpt_voc_probe(const agpt_voc_probe_args* args, void* stream) {
   });
 }
 
+int agpt_an_probe(const agpt_an_probe_args* args, void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(args, "null argument");
+    const bool handle_op = args->op == AGPT_AN_LASS_FILM_VEC || args->op == AGPT_AN_LASS_UP;
+    an_probe(*args, handle_op ? as(reinterpret_cast<agpt_handle>(args->h), kMagicLass, "lass") : nullptr,
+             (cudaStream_t)stream);
+  });
+}
+
 }  // extern "C"

@@ -14,6 +14,7 @@
 #include "models.h"
 #include "fs_layers.cuh"
 #include "clap.cuh"
+#include "an_kernels.cuh"
 
 namespace agpt {
 
@@ -54,6 +55,27 @@ __global__ void clap_gelu_kernel(const float* __restrict__ in, float* __restrict
 
 }  // namespace
 
+void clap_embed(const int* ids, const float* word, const float* pos, const float* type0, float* x, int N, int L, int H, int vocab,
+                cudaStream_t st) {
+  AGPT_CHECK(vocab >= 1 && H >= 1 && L >= 1 && N >= 1, "embeddings: vocab, H, L, N >= 1");
+  clap_embed_kernel<<<(unsigned)((long)N * L), 128, 0, st>>>(ids, word, pos, type0, x, L, H, vocab);
+  count_launch(1);
+}
+
+void clap_embed_typed(const int* ids, const int* type_ids, const int* mask, const float* word, const float* pos,
+                      const float* types, float* x, uint8_t* kpm, int N, int L, int H, int vocab, int ntypes, cudaStream_t st) {
+  AGPT_CHECK(vocab >= 1 && ntypes >= 1 && H >= 1 && L >= 1 && N >= 1, "embeddings: vocab, ntypes, H, L, N >= 1");
+  clap_embed_typed_kernel<<<(unsigned)((long)N * L), 128, 0, st>>>(ids, type_ids, mask, word, pos, types, x, kpm, L, H, vocab,
+                                                                   ntypes);
+  count_launch(1);
+}
+
+void clap_gelu(const float* in, float* out, long n, int max_blocks, cudaStream_t st) {
+  AGPT_CHECK(n >= 1 && max_blocks >= 1, "gelu: n >= 1 and max_blocks >= 1");
+  clap_gelu_kernel<<<(unsigned)std::min<long>(cdivl(n, 256), max_blocks), 256, 0, st>>>(in, out, n);
+  count_launch(1);
+}
+
 void ClapNet::ensure_work(long rows) {
   const int H = cfg.hidden_size, I = cfg.intermediate_size;
   x.ensure(rows * H); y.ensure(rows * H); qkv.ensure(rows * 3 * H); ctx.ensure(rows * H); ffn.ensure(rows * I);
@@ -66,13 +88,11 @@ void ClapNet::encode(const int* ids, int N, int L, float* z, cudaStream_t st) {
   const long rows = (long)N * L;
   ensure_work(rows);
   e1.ensure(rows * D); g1.ensure(rows * D); e12.ensure(rows * D);
-  clap_embed_kernel<<<(unsigned)rows, 128, 0, st>>>(ids, word.p, pos.p, types.p, y.p, L, H, cfg.vocab_size);
-  count_launch(1);
+  clap_embed(ids, word.p, pos.p, types.p, y.p, N, L, H, cfg.vocab_size, st);
   trunk(N, L, nullptr, st);
   // Projection: LayerNorm(e1 + linear2(gelu(e1))), both Linears without bias
   fs_conv(proj.lin1, x.p, H, e1.p, D, 1, (int)rows, EPI_BIAS, st);
-  clap_gelu_kernel<<<(unsigned)std::min<long>(cdivl(rows * D, 256), 2368), 256, 0, st>>>(e1.p, g1.p, rows * D);
-  count_launch(1);
+  clap_gelu(e1.p, g1.p, rows * D, 2368, st);
   fs_conv(proj.lin2, g1.p, D, e12.p, D, 1, (int)rows, EPI_RES, st, e1.p);
   layernorm(e12.p, z, proj.lng.p, proj.lnb.p, rows, D, cfg.proj_layer_norm_eps, st);
   AGPT_CUDA(cudaGetLastError());
@@ -91,9 +111,7 @@ void ClapNet::encode_hidden(const int* ids, const int* type_ids, const int* mask
   const long rows = (long)N * L;
   ensure_work(rows);
   uint8_t* m = reinterpret_cast<uint8_t*>(kpm.ensure(cdivl(rows, 4)));
-  clap_embed_typed_kernel<<<(unsigned)rows, 128, 0, st>>>(ids, type_ids, mask, word.p, pos.p, types.p, y.p, m, L, H,
-                                                          cfg.vocab_size, cfg.type_vocab_size);
-  count_launch(1);
+  clap_embed_typed(ids, type_ids, mask, word.p, pos.p, types.p, y.p, m, N, L, H, cfg.vocab_size, cfg.type_vocab_size, st);
   trunk(N, L, m, st);
 }
 

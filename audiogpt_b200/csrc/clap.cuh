@@ -48,6 +48,10 @@ struct ClapNet : Handle {
   void trunk(int N, int L, const uint8_t* kpm_, cudaStream_t st);
 };
 
+// the Projection's exact GELU, out [n] = gelu_erf(in [n]), on a grid-stride grid of at most max_blocks blocks of 256
+// (clap.cu).  n >= 1, max_blocks >= 1.
+void clap_gelu(const float* in, float* out, long n, int max_blocks, cudaStream_t st);
+
 // out[r] = in[r] / |in[r]|, applied twice (in may equal out)
 void clap_l2norm2(const float* in, float* out, int rows, int D, cudaStream_t st);
 

@@ -133,10 +133,6 @@ __global__ void clap_similarity_kernel(const float* __restrict__ a, const float*
   if (threadIdx.x == 0) out[blockIdx.x] = scale * s;
 }
 
-__global__ void clap_gelu2_kernel(const float* __restrict__ in, float* __restrict__ out, long n) {
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) out[i] = gelu_erf(in[i]);
-}
-
 unsigned ew_blocks(long n) { return (unsigned)std::min<long>(cdivl(n, 256), 4096); }
 
 }  // namespace
@@ -205,8 +201,7 @@ void ClapProjection::run(const float* x, int in_pitch, int rows, float* out, cud
   P.out = e1.p; P.out_pitch = D;
   P.epi = EPI_BIAS;
   tapconv_launch(P, st);
-  clap_gelu2_kernel<<<ew_blocks((long)rows * D), 256, 0, st>>>(e1.p, g1.p, (long)rows * D);
-  count_launch(1);
+  clap_gelu(e1.p, g1.p, (long)rows * D, 4096, st);
   fs_conv(lin2, g1.p, D, e12.p, D, 1, rows, EPI_RES, st, e1.p);
   layernorm(e12.p, z.p, lng.p, lnb.p, rows, D, eps, st);
   clap_l2norm2(z.p, out, rows, D, st);

@@ -15,6 +15,7 @@
 #include "tapconv.cuh"
 #include "models.h"
 #include "audio_front.cuh"
+#include "an_kernels.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -200,6 +201,20 @@ int lstm_group(int N) {
 }  // namespace
 
 // ---------------------------------------------------------------- launchers (also the unit tests' entry points)
+void emo_mean_norm(const float* h, int N, float* embed, cudaStream_t st) {
+  AGPT_CHECK(N >= 1, "mean_norm: N >= 1");
+  emo_mean_norm_kernel<<<1, kEmoH, 0, st>>>(h, N, embed);
+  count_launch(1);
+}
+
+void emo_linear_norm(const float* h, const float* W, const float* bias, int N, int E, float* out, cudaStream_t st) {
+  AGPT_CHECK(E >= 1 && N >= 1, "linear_norm: E >= 1 and N >= 1");
+  AGPT_CHECK(sizeof(float) * ((size_t)E + kEmoH + 32) <= 48 * 1024,
+             "linear_norm: E floats of dynamic shared memory exceed the 48 KB a launch allows");
+  emo_linear_norm_kernel<<<(unsigned)N, kTailThreads, sizeof(float) * E, st>>>(h, W, bias, E, out);
+  count_launch(1);
+}
+
 void emo_powmel(const float* spec, int pitch, const float* melW, float* mel, long frames, cudaStream_t st) {
   AGPT_CHECK(frames >= 1 && pitch >= 2 * kBins, "power mel: bad sizes");
   emo_powmel_kernel<<<(unsigned)frames, kMelThreads, 0, st>>>(spec, pitch, melW, mel);
@@ -310,8 +325,7 @@ struct EmoNet : Handle {
     last.ensure((size_t)N * kEmoH);
     hidden(x, N, T, last.p, st);
     const int E = cfg.embedding_size;
-    emo_linear_norm_kernel<<<(unsigned)N, kTailThreads, sizeof(float) * E, st>>>(last.p, linw.p, linb.p, E, out);
-    count_launch(1);
+    emo_linear_norm(last.p, linw.p, linb.p, N, E, out, st);
     AGPT_CUDA(cudaGetLastError());
   }
 
@@ -340,8 +354,7 @@ struct EmoNet : Handle {
     float* h = partials;
     if (!h) { last.ensure((size_t)N * kEmoH); h = last.p; }
     stack(mel.p, used, step, N, partial_frames, h, st);
-    emo_mean_norm_kernel<<<1, kEmoH, 0, st>>>(h, N, out);
-    count_launch(1);
+    emo_mean_norm(h, N, out, st);
     AGPT_CUDA(cudaGetLastError());
   }
 };

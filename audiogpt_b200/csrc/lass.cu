@@ -31,6 +31,7 @@
 #include "models.h"
 #include "clap.cuh"
 #include "audio_front.cuh"
+#include "an_kernels.cuh"
 
 namespace agpt {
 
@@ -117,7 +118,6 @@ __global__ void lass_shuffle_kernel(const float4* __restrict__ up, const float4*
 
 // The FiLM second Linears, one warp per (sample, job): film(o) = relu(w2[o] . hid[o's slice] + b2[o]);
 // vec[b][dst] = alpha film(A) + beta (+ film(B))
-struct FilmJobs { const int *woff, *hoff, *nin, *dst, *ja, *jb; const float *b2, *alpha, *beta; };
 __global__ void lass_film_kernel(const float* __restrict__ hid, int hid_len, const float* __restrict__ w2, FilmJobs J, int nj,
                                  int B, float* __restrict__ vec, int vec_len) {
   const int warp = (int)(((long)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
@@ -223,6 +223,47 @@ __global__ void istft_finish_kernel(const float* __restrict__ y, long ylen, cons
 }
 
 }  // namespace
+
+void lass_affine(const float* x, const float* s, const float* t, float* a, float* r, const float* vec, int vec_len, int vec_off,
+                 long rows, long rows_per_sample, int C, cudaStream_t st) {
+  AGPT_CHECK(C >= 4 && C % 4 == 0, "LASS affine: C % 4 == 0 (float4 rows)");
+  AGPT_CHECK(rows >= 1 && rows_per_sample >= 1, "LASS affine: rows >= 1 and rows_per_sample >= 1");
+  AGPT_CHECK(!r || (vec_off >= 0 && (long)vec_off + C <= vec_len), "LASS affine: the vector slice must fit in vec_len");
+  AGPT_CHECK(!r || (vec_off % 4 == 0 && vec_len % 4 == 0), "LASS affine: vec_off and vec_len must be multiples of 4 (float4 reads)");
+  const long tot = rows * (C / 4);
+  lass_affine_kernel<<<ew_blocks(tot), 256, 0, st>>>(
+      reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(s), reinterpret_cast<const float4*>(t),
+      reinterpret_cast<float4*>(a), reinterpret_cast<float4*>(r), vec ? vec + vec_off : nullptr, vec_len, rows_per_sample, C / 4,
+      tot);
+  count_launch(1);
+}
+
+void lass_upcol(const float* y, const float* s, const float* t, int B, int h, int w, int C, float* col, cudaStream_t st) {
+  AGPT_CHECK(C >= 4 && C % 4 == 0, "LASS upcol: C % 4 == 0 (float4 rows)");
+  AGPT_CHECK(B >= 1 && h >= 1 && w >= 1, "LASS upcol: B, h, w >= 1");
+  const long tot = (long)B * h * (w + 1) * 4 * (C / 4);
+  lass_upcol_kernel<<<ew_blocks(tot), 256, 0, st>>>(reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(s),
+                                                   reinterpret_cast<const float4*>(t), h, w, C / 4, reinterpret_cast<float4*>(col),
+                                                   tot);
+  count_launch(1);
+}
+
+void lass_shuffle(const float* up, const float* skip, int B, int h, int w, int C, float* cat, cudaStream_t st) {
+  AGPT_CHECK(C >= 4 && C % 4 == 0, "LASS shuffle: C % 4 == 0 (float4 rows)");
+  AGPT_CHECK(B >= 1 && h >= 1 && w >= 1, "LASS shuffle: B, h, w >= 1");
+  const long tot = (long)B * (2 * h) * (2 * w + 1) * 2 * (C / 4);
+  lass_shuffle_kernel<<<ew_blocks(tot), 256, 0, st>>>(reinterpret_cast<const float4*>(up), reinterpret_cast<const float4*>(skip),
+                                                     h, w, C / 4, reinterpret_cast<float4*>(cat), tot);
+  count_launch(1);
+}
+
+void lass_film(const float* hid, int hid_len, const float* w2, const FilmJobs& J, int nj, int B, float* vec, int vec_len,
+               cudaStream_t st) {
+  AGPT_CHECK(nj >= 1 && B >= 1 && hid_len >= 1 && vec_len >= 1, "LASS FiLM: nj, B, hid_len, vec_len >= 1");
+  const long warps = (long)nj * B;
+  lass_film_kernel<<<(unsigned)cdivl(warps * 32, 256), 256, 0, st>>>(hid, hid_len, w2, J, nj, B, vec, vec_len);
+  count_launch(1);
+}
 
 void lass_input(const float* mag, long sb, long stt, long sf, int B, int T, int Tp, int W, float s, float sh, float* img,
                 cudaStream_t st) {
@@ -455,12 +496,7 @@ struct LassNet : Handle {
     const long rows = (long)B * H * W;
     const float* a = x;
     if (b.s1.p) {
-      const long tot = rows * (b.cin / 4);
-      lass_affine_kernel<<<ew_blocks(tot), 256, 0, st>>>(
-          reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(b.s1.p), reinterpret_cast<const float4*>(b.t1.p),
-          reinterpret_cast<float4*>(ba.p), b.sc ? nullptr : reinterpret_cast<float4*>(br.p), vec.p + b.r2, vec_len,
-          (long)H * W, b.cin / 4, tot);
-      count_launch(1);
+      lass_affine(x, b.s1.p, b.t1.p, ba.p, b.sc ? nullptr : br.p, vec.p, vec_len, b.r2, rows, (long)H * W, b.cin, st);
       a = ba.p;
     }
     if (b.sc) {   // shortcut(x) + bias + film_res + film2
@@ -472,6 +508,31 @@ struct LassNet : Handle {
     }
     conv3x3(b.conv1, a, bh.p, B, H, W, EPI_ADDVEC, vec.p + b.e1, nullptr, st);
     conv3x3(b.conv2, bh.p, out, B, H, W, EPI_RES, nullptr, br.p, st);
+  }
+
+  // the FiLM vectors of a request: cond [B][256] -> film1 (EPI_RELU) into hid, lass_film -> v [B][vec_len]
+  void film_vec(const float* cond, int B, float* v, cudaStream_t st) {
+    hid.ensure((size_t)B * hid_len);
+    TapConvParams P = tapconv_params(film1, 1, B, 0, 1);
+    P.in = cond; P.in_pitch = kCond;
+    P.out = hid.p; P.out_pitch = hid_len;
+    P.epi = EPI_RELU;
+    tapconv_launch(P, st);
+    lass_film(hid.p, hid_len, w2.p, jobs(), njobs, B, v, vec_len, st);
+  }
+
+  // decoder d's bn1, ReLU and ConvTranspose2d(k3, s2) + prune on y [B][h][w][d.cin], next to the skip [B][2h][2w + 1]
+  // [d.cout] -> cat [B][2h][2w + 1][2 d.cout]: lass_upcol, the packed 4 C_in -> 4 C_out GEMM, lass_shuffle
+  void up(const LDec& d, const float* y, const float* skp, int B, int h, int w, float* out, cudaStream_t st) {
+    col.ensure((size_t)B * h * (w + 1) * 4 * d.cin);
+    upb.ensure((size_t)B * h * (w + 1) * 4 * d.cout);
+    lass_upcol(y, d.s.p, d.t.p, B, h, w, d.cin, col.p, st);
+    TapConvParams P = tapconv_params(d.up, 1, B * h * (w + 1), 0, 1);
+    P.in = col.p; P.in_pitch = 4 * d.cin;
+    P.out = upb.p; P.out_pitch = 4 * d.cout;
+    P.epi = EPI_BIAS;
+    tapconv_launch(P, st);
+    lass_shuffle(upb.p, skp, B, h, w, d.cout, out, st);
   }
 
   void mask(const float* mag, int B, int T, int F, long sb, long stt, long sf, const float* cond, float* out_mask,
@@ -499,18 +560,8 @@ struct LassNet : Handle {
     mx = std::max(mx, (size_t)Hs[kLevels] * Ws[kLevels] * 384);
     for (DevBuf* d : {&bx, &bo, &ba, &bh, &br}) d->ensure(mx * B);
     cat.ensure(mcat * B); col.ensure(mcol * B); upb.ensure(mup * B);
-    hid.ensure((size_t)B * hid_len); vec.ensure((size_t)B * vec_len);
-    // FiLM vectors of the whole request
-    {
-      TapConvParams P = tapconv_params(film1, 1, B, 0, 1);
-      P.in = cond; P.in_pitch = kCond;
-      P.out = hid.p; P.out_pitch = hid_len;
-      P.epi = EPI_RELU;
-      tapconv_launch(P, st);
-      const long warps = (long)njobs * B;
-      lass_film_kernel<<<(unsigned)cdivl(warps * 32, 256), 256, 0, st>>>(hid.p, hid_len, w2.p, jobs(), njobs, B, vec.p, vec_len);
-      count_launch(1);
-    }
+    vec.ensure((size_t)B * vec_len);
+    film_vec(cond, B, vec.p, st);     // FiLM vectors of the whole request
     lass_input(mag, sb, stt, sf, B, T, Tp, W0, in_s, in_t, bx.p, st);
     // encoder: two blocks per level, the second one's output is the skip; then 2x2 average pool (floor)
     int bi = 0;
@@ -525,26 +576,7 @@ struct LassNet : Handle {
       const LDec& d = dec[k];
       const int h = Hs[k + 1], w = Ws[k + 1];
       AGPT_CHECK(Hs[k] == 2 * h && Ws[k] == 2 * w + 1, "decoder shape");
-      {
-        const long tot = (long)B * h * (w + 1) * 4 * (d.cin / 4);
-        lass_upcol_kernel<<<ew_blocks(tot), 256, 0, st>>>(reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(d.s.p),
-                                                         reinterpret_cast<const float4*>(d.t.p), h, w, d.cin / 4,
-                                                         reinterpret_cast<float4*>(col.p), tot);
-        count_launch(1);
-      }
-      {
-        TapConvParams P = tapconv_params(d.up, 1, B * h * (w + 1), 0, 1);
-        P.in = col.p; P.in_pitch = 4 * d.cin;
-        P.out = upb.p; P.out_pitch = 4 * d.cout;
-        P.epi = EPI_BIAS;
-        tapconv_launch(P, st);
-      }
-      {
-        const long tot = (long)B * Hs[k] * Ws[k] * 2 * (d.cout / 4);
-        lass_shuffle_kernel<<<ew_blocks(tot), 256, 0, st>>>(reinterpret_cast<const float4*>(upb.p), reinterpret_cast<const float4*>(skip[k].p),
-                                                           h, w, d.cout / 4, reinterpret_cast<float4*>(cat.p), tot);
-        count_launch(1);
-      }
+      up(d, y, skip[k].p, B, h, w, cat.p, st);
       run_block(blocks[bi++], cat.p, bx.p, B, Hs[k], Ws[k], st);
       run_block(blocks[bi++], bx.p, bo.p, B, Hs[k], Ws[k], st);
       y = bo.p;
@@ -607,6 +639,23 @@ void lass_mask(Handle* hh, const float* mag, int B, int T, int F, long sb, long 
   auto* h = static_cast<LassNet*>(hh);
   DeviceGuard dg_(h->device);
   h->mask(mag, B, T, F, sb, stt, sf, cond, mask, logits, st);
+}
+
+int lass_film_vec(Handle* hh, const float* cond, int B, float* vec, cudaStream_t st) {
+  auto* h = static_cast<LassNet*>(hh);
+  DeviceGuard dg_(h->device);
+  if (vec) {
+    AGPT_CHECK(B >= 1 && cond, "LASS FiLM vectors: B >= 1 and a condition");
+    h->film_vec(cond, B, vec, st);
+  }
+  return h->vec_len;
+}
+
+void lass_up(Handle* hh, int level, const float* y, const float* skip, int B, int h, int w, float* cat, cudaStream_t st) {
+  auto* net = static_cast<LassNet*>(hh);
+  DeviceGuard dg_(net->device);
+  AGPT_CHECK(level >= 0 && level < kLevels, "LASS up: the decoder level must be in [0, 6)");
+  net->up(net->dec[level], y, skip, B, h, w, cat, st);
 }
 
 struct StftNet : Handle {

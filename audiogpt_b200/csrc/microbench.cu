@@ -1,6 +1,7 @@
 // Conformance entries: one production launch of the tap-GEMM primitive (tapconv_probe), of a non-contraction
 // kernel (nn_probe), of a FastSpeech-family element-wise kernel (fs_probe), of an audio / spectrogram kernel
-// (audio_probe) or of a vocoder / diffusion-step kernel (voc_probe) on caller-owned tensors.
+// (audio_probe), of a vocoder / diffusion-step kernel (voc_probe) or of an analysis-model kernel (an_probe) on
+// caller-owned tensors.
 #include "tapconv.cuh"
 #include "models.h"
 #include "nn_kernels.h"
@@ -8,6 +9,7 @@
 #include "audio_front.cuh"
 #include "clap.cuh"
 #include "voc_kernels.cuh"
+#include "an_kernels.cuh"
 
 namespace agpt {
 
@@ -227,6 +229,46 @@ void voc_probe(const agpt_voc_probe_args& a, cudaStream_t st) {
       p_sample_tab(a.y, a.x, a.noises_pp, a.noise_stride, a.w, a.ctr, a.nsteps, a.clip, a.B, a.n, st);
       break;
     default: throw Error("voc probe: unknown op " + std::to_string(a.op));
+  }
+  AGPT_CUDA(cudaStreamSynchronize(st));
+}
+
+// One call of a production analysis-model launcher on caller-owned tensors (agpt_an_probe, include/agpt_b200.h); lass is
+// the checked LASSNet handle of the two handle ops, else null.
+void an_probe(const agpt_an_probe_args& a, Handle* lass, cudaStream_t st) {
+  switch (a.op) {
+    case AGPT_AN_LASS_AFFINE:
+      lass_affine(a.x, a.s, a.t, a.y, a.y2, a.vec, a.vec_len, a.vec_off, a.rows, a.rows_per_sample, a.C, st);
+      break;
+    case AGPT_AN_LASS_UPCOL: lass_upcol(a.x, a.s, a.t, a.B, a.hh, a.ww, a.C, a.y, st); break;
+    case AGPT_AN_LASS_SHUFFLE: lass_shuffle(a.x, a.x2, a.B, a.hh, a.ww, a.C, a.y, st); break;
+    case AGPT_AN_LASS_FILM: {
+      const FilmJobs J{a.woff, a.hoff, a.nin, a.dst, a.ja, a.jb, a.b2, a.alpha, a.beta};
+      lass_film(a.x, a.hid_len, a.w2, J, a.nj, a.B, a.y, a.vec_len, st);
+      break;
+    }
+    case AGPT_AN_LASS_FILM_VEC: {
+      const int vl = lass_film_vec(lass, a.x, a.B, a.y, st);
+      if (a.info) a.info[0] = vl;
+      break;
+    }
+    case AGPT_AN_LASS_UP:
+      lass_up(lass, a.level, a.x, a.x2, a.B, a.hh, a.ww, a.y, st);
+      if (a.info) a.info[0] = lass_film_vec(lass, nullptr, 0, nullptr, st);
+      break;
+    case AGPT_AN_TSD_PAD4: tsd_pad4(a.x, a.y, a.rows, st); break;
+    case AGPT_AN_TSD_FUSE: tsd_fuse(a.x, a.x2, a.B, a.Td, a.C, a.n, a.y, st); break;
+    case AGPT_AN_TSD_REFEMB: tsd_refemb(a.x, a.B, a.T, a.att_pool, a.w, a.b, a.w2, a.b2, a.scratch, a.y, st); break;
+    case AGPT_AN_TSD_HEAD: tsd_head(a.x, a.w, a.b, a.O, a.rows, a.y, st); break;
+    case AGPT_AN_TSD_MIX_INTERP: tsd_mix_interp(a.x, a.x2, a.vec, a.B, a.Td, a.T, a.O, a.y, a.y2, st); break;
+    case AGPT_AN_CLAP_EMBED: clap_embed(a.ids, a.w, a.x, a.x2, a.y, a.N, a.L, a.H, a.vocab, st); break;
+    case AGPT_AN_CLAP_EMBED_TYPED:
+      clap_embed_typed(a.ids, a.type_ids, a.mask, a.w, a.x, a.x2, a.y, a.kpm, a.N, a.L, a.H, a.vocab, a.ntypes, st);
+      break;
+    case AGPT_AN_CLAP_GELU: clap_gelu(a.x, a.y, a.rows, a.max_blocks, st); break;
+    case AGPT_AN_EMO_MEAN_NORM: emo_mean_norm(a.x, a.N, a.y, st); break;
+    case AGPT_AN_EMO_LINEAR_NORM: emo_linear_norm(a.x, a.w, a.b, a.N, a.E, a.y, st); break;
+    default: throw Error("an probe: unknown op " + std::to_string(a.op));
   }
   AGPT_CUDA(cudaStreamSynchronize(st));
 }

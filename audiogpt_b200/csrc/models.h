@@ -76,6 +76,10 @@ Handle* lass_create(const agpt_lass_cfg* cfg, const float* const* W, int nW, int
 void lass_text(Handle* h, const int* ids, const int* mask, int N, int L, float* cond, cudaStream_t st);
 void lass_mask(Handle* h, const float* mag, int B, int T, int F, long sb, long st_, long sf, const float* cond, float* mask,
                float* logits, cudaStream_t st);
+// the probe's view of a LASSNet handle: its FiLM vectors for cond [B][256] into vec [B][vec_len] (vec null: nothing
+// runs), returning vec_len; and decoder level `level`'s up path (LassNet::up) on caller-owned maps
+int lass_film_vec(Handle* h, const float* cond, int B, float* vec, cudaStream_t st);
+void lass_up(Handle* h, int level, const float* y, const float* skip, int B, int hh, int w, float* cat, cudaStream_t st);
 Handle* stft_create(int filter_length, int hop_length, const float* fwd_basis, const float* inv_basis, int device);
 void stft_transform(Handle* h, const float* wav, int B, long n_samples, float* mag, float* phase, cudaStream_t st);
 void stft_inverse(Handle* h, const float* mag, const float* phase, int B, int T, float* wav, cudaStream_t st);
@@ -130,5 +134,6 @@ void nn_probe(const agpt_nn_probe_args& a, cudaStream_t st);
 void fs_probe(const agpt_fs_probe_args& a, cudaStream_t st);
 void audio_probe(const agpt_audio_probe_args& a, cudaStream_t st);
 void voc_probe(const agpt_voc_probe_args& a, cudaStream_t st);
+void an_probe(const agpt_an_probe_args& a, Handle* lass, cudaStream_t st);
 
 }  // namespace agpt

@@ -17,6 +17,7 @@
 #include "tapconv.cuh"
 #include "models.h"
 #include "convblock.cuh"
+#include "an_kernels.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -210,12 +211,12 @@ __device__ void attend(const float* __restrict__ Wk, const float* __restrict__ b
 
 // ---- the reference embedding (RaDur_fusion.forward before the detection): E [B][Tr][128] -> emb [B][128].
 // att_pool: E holds bn(fc1(.)) rows; emb = sum_t softmax_t(get_w(mean_t E, E)) E_t.  Otherwise emb = mean_t E.
+// The scores live in global scratch [B][Tr] (a long reference clip's Tr floats would not fit in shared memory).
 constexpr int kTailThreads = 256;
 __global__ void __launch_bounds__(kTailThreads) tsd_refemb_kernel(const float* __restrict__ E, int Tr, int att_pool,
                                                                   const float* __restrict__ qw, const float* __restrict__ qb,
                                                                   const float* __restrict__ kw, const float* __restrict__ kb,
-                                                                  float* __restrict__ emb) {
-  extern __shared__ float sc[];                   // [Tr]
+                                                                  float* __restrict__ scores, float* __restrict__ emb) {
   __shared__ float m[kEmb], q[kEmb], u[kEmb], red[32];
   const long b = blockIdx.x;
   const float* Eb = E + b * Tr * kEmb;
@@ -229,6 +230,7 @@ __global__ void __launch_bounds__(kTailThreads) tsd_refemb_kernel(const float* _
     for (int c = threadIdx.x; c < kEmb; c += blockDim.x) emb[b * kEmb + c] = m[c];
     return;
   }
+  float* sc = scores + b * Tr;
   linear128(qw, qb, m, q, kEmb, false);
   __syncthreads();
   attend(kw, kb, q, Eb, Tr, [](int i) { return i; }, u, sc, red);
@@ -425,6 +427,45 @@ unsigned ew_blocks(long n) { return (unsigned)std::max<long>(1, std::min<long>(c
 }  // namespace
 
 // ---------------------------------------------------------------- launchers (also the unit tests' entry points)
+void tsd_pad4(const float* mel, float* img, long n, cudaStream_t st) {
+  AGPT_CHECK(n >= 1, "pad4: n >= 1");
+  tsd_pad4_kernel<<<ew_blocks(n), 256, 0, st>>>(mel, reinterpret_cast<float4*>(img), n);
+  count_launch(1);
+}
+
+void tsd_fuse(const float* f2, const float* e1, int B, int Td, int C, int n, float* out, cudaStream_t st) {
+  AGPT_CHECK(n >= 1, "fuse: n >= 1");
+  AGPT_CHECK(B >= 1 && Td >= 1 && C >= 1, "fuse: B, Td, C >= 1");
+  const long total = (long)B * Td * C;
+  tsd_fuse_kernel<<<ew_blocks(total), 256, 0, st>>>(f2, e1, Td, C, n, out, total);
+  count_launch(1);
+}
+
+void tsd_refemb(const float* E, int B, int Trr, int att_pool, const float* qw, const float* qb, const float* kw, const float* kb,
+                float* scratch, float* emb, cudaStream_t st) {
+  AGPT_CHECK(Trr >= 1, "refemb: Trr >= 1");
+  AGPT_CHECK(B >= 1, "refemb: B >= 1");
+  AGPT_CHECK(!att_pool || scratch, "refemb: attention pooling needs a [B][Trr] score scratch");
+  tsd_refemb_kernel<<<B, kTailThreads, 0, st>>>(E, Trr, att_pool, qw, qb, kw, kb, scratch, emb);
+  count_launch(1);
+}
+
+void tsd_head(const float* h, const float* w, const float* bias, int O, long rows, float* p, cudaStream_t st) {
+  AGPT_CHECK(O >= 1 && O <= kMaxOut, "head: 1 <= O <= 16");
+  AGPT_CHECK(rows >= 1, "head: rows >= 1");
+  tsd_head_kernel<<<(unsigned)cdivl(rows, kHeadWarps), kHeadWarps * 32, 0, st>>>(h, w, bias, O, rows, p);
+  count_launch(1);
+}
+
+void tsd_mix_interp(const float* p1, const float* p2, const float* wmix, int B, int Td, int T, int O, float* decision, float* up,
+                    cudaStream_t st) {
+  AGPT_CHECK(O >= 1 && O <= kMaxOut, "mix_interp: 1 <= O <= 16");
+  AGPT_CHECK(B >= 1 && Td >= 1 && T >= 1, "mix_interp: B, Td, T >= 1");
+  const long n = (long)B * T * O + (long)B * Td;
+  tsd_mix_interp_kernel<<<ew_blocks(n), 256, 0, st>>>(p1, p2, wmix, B, Td, T, O, decision, up);
+  count_launch(1);
+}
+
 void tsd_avgpool(const float* in, int B, int H, int W, int C, int ph, int pw, float* out, cudaStream_t st) {
   AGPT_CHECK(B >= 1 && ph >= 1 && pw >= 1 && C >= 4 && C % 4 == 0, "avgpool: C must be a multiple of 4");
   AGPT_CHECK(H >= ph && W >= pw, "avgpool: the map is smaller than the pool window");
@@ -534,7 +575,7 @@ struct TsdNet : Handle {
   PackedConv wih, fuse1, fuse2;
   DevBuf whh, bhh, headw, headb;
   DevBuf qw, qb, kw, kb, qew, qeb, kew, keb, ee1w, ee1b, ee2w, ee2b;
-  DevBuf img, bA, bB, bC, eref, emix, emb, me, e1, stem, f2, fused, xp, hs, p1, p2, wmix, idx;
+  DevBuf img, bA, bB, bC, eref, emix, emb, me, e1, stem, f2, fused, xp, hs, p1, p2, wmix, idx, scores;
   cudaEvent_t ev[kTsdStages + 1] = {};
   bool timed = false;
 
@@ -550,9 +591,7 @@ struct TsdNet : Handle {
 
   // Cnn14.forward on mel [B][T][64] -> [B][T / 8][128] through fc (fc1, or fc1 with bn folded)
   void encode(const float* mel, int B, int T, const PackedConv& fc, float* out, cudaStream_t st) {
-    const long n = (long)B * T * kMel;
-    tsd_pad4_kernel<<<ew_blocks(n), 256, 0, st>>>(mel, reinterpret_cast<float4*>(img.p), n);
-    count_launch(1);
+    tsd_pad4(mel, img.p, (long)B * T * kMel, st);
     const float* in = img.p;
     int H = T, W = kMel;
     for (int i = 0; i < kEnc; ++i) {
@@ -569,12 +608,10 @@ struct TsdNet : Handle {
   // one detection pass from the fused-in embedding's fuse_layer1 output e1 [B][1024]: Fusion product, GRU, head -> p
   void pass(int B, int Td, const float* e1v, float* p, cudaStream_t st) {
     const long rows = (long)B * Td;
-    tsd_fuse_kernel<<<ew_blocks(rows * kFeat), 256, 0, st>>>(f2.p, e1v, Td, kFeat, 2, fused.p, rows * kFeat);
-    count_launch(1);
+    tsd_fuse(f2.p, e1v, B, Td, kFeat, 2, fused.p, st);
     linear(wih, fused.p, xp.p, rows, EPI_BIAS, st);
     tsd_gru(whh.p, bhh.p, xp.p, B, Td, hs.p, st);
-    tsd_head_kernel<<<(unsigned)cdivl(rows, kHeadWarps), kHeadWarps * 32, 0, st>>>(hs.p, headw.p, headb.p, cfg.outputdim, rows, p);
-    count_launch(1);
+    tsd_head(hs.p, headw.p, headb.p, cfg.outputdim, rows, p, st);
     AGPT_CUDA(cudaGetLastError());
   }
 
@@ -597,8 +634,8 @@ struct TsdNet : Handle {
     mark(0, st);
     // the reference embedding
     encode(ref, B, Tr, cfg.att_pool ? fc1_bn : fc1, eref.p, st);
-    tsd_refemb_kernel<<<B, kTailThreads, sizeof(float) * Trr, st>>>(eref.p, Trr, cfg.att_pool, qw.p, qb.p, kw.p, kb.p, emb.p);
-    count_launch(1);
+    if (cfg.att_pool) scores.ensure((size_t)B * Trr);
+    tsd_refemb(eref.p, B, Trr, cfg.att_pool, qw.p, qb.p, kw.p, kb.p, scores.p, emb.p, st);
     AGPT_CUDA(cudaGetLastError());
     mark(1, st);
     if (cfg.enhancement) encode(x, B, T, fc1_bn, emix.p, st);   // the mixture's embeddings, bn applied
@@ -629,10 +666,7 @@ struct TsdNet : Handle {
       pass(B, Td, e1.p, p2.p, st);
     }
     mark(5, st);
-    const long n = (long)B * T * cfg.outputdim + (long)B * Td;
-    tsd_mix_interp_kernel<<<ew_blocks(n), 256, 0, st>>>(p1.p, cfg.enhancement ? p2.p : nullptr, wmix.p, B, Td, T, cfg.outputdim,
-                                                        decision, decision_up);
-    count_launch(1);
+    tsd_mix_interp(p1.p, cfg.enhancement ? p2.p : nullptr, wmix.p, B, Td, T, cfg.outputdim, decision, decision_up, st);
     AGPT_CUDA(cudaGetLastError());
     mark(6, st);
   }

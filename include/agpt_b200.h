@@ -280,6 +280,56 @@ typedef struct agpt_voc_probe_args {
   float slope;
 } agpt_voc_probe_args;
 int agpt_voc_probe(const agpt_voc_probe_args* args, void* stream);
+/* Conformance entry of the analysis models' kernels outside the GEMMs (LASSNet's FiLM ResUNet, RaDur's detection tail,
+ * the BERT embeddings, the emotion encoder's tail; tests/test_an_kernels_gpu.py): ONE call of the production launcher
+ * selected by `op` on caller-owned device tensors, with the arguments as given.  Tensors are fp32 device arrays except
+ * the int32 device arrays ids, type_ids, mask and the FiLM tables (woff .. jb), kpm (uint8_t, device) and info (int32,
+ * HOST); h is an agpt_handle.  The launcher's preconditions are checked first; a violation returns an error with nothing
+ * launched.  Rows are channels-last; the map sizes h, w below are the fields hh, ww.  The fields each op reads:
+ *   LASS_AFFINE      x [rows][C], s [C], t [C], vec [B][vec_len], vec_off, rows, rows_per_sample -> y = fmaf(x, s, t)
+ *                    [rows][C], y2 (null = none) = x + vec[row / rows_per_sample][vec_off + c]; C % 4 == 0,
+ *                    rows, rows_per_sample >= 1; with y2: vec_off + C <= vec_len, vec_off and vec_len multiples of 4
+ *   LASS_UPCOL       x [B][h][w][C], s [C], t [C] -> y [B][h][w + 1][4][C]; C % 4 == 0, h, w >= 1
+ *   LASS_SHUFFLE     x = up [B][h][w + 1][4][C], x2 = skip [B][2h][2w + 1][C] -> y [B][2h][2w + 1][2C]; C % 4 == 0
+ *   LASS_FILM        x = hid [B][hid_len], w2 [..], woff / hoff / nin [outputs], b2 [outputs], dst / ja / jb / alpha /
+ *                    beta [nj] -> y = vec [B][vec_len] (only the dst entries are written)
+ *   LASS_FILM_VEC    h (LASSNet), x = cond [B][256] -> y = the FiLM vectors [B][vec_len] (y null: nothing runs);
+ *                    info[0] <- vec_len
+ *   LASS_UP          h (LASSNet), level in [0, 6), x [B][h][w][cin], x2 = skip [B][2h][2w + 1][cout] -> y = the
+ *                    decoder's concat [B][2h][2w + 1][2 cout] (bn1, ReLU, ConvTranspose2d(3, 2) pruned, skip);
+ *                    info[0] <- vec_len
+ *   TSD_PAD4         x [rows] -> y [rows][4]
+ *   TSD_FUSE         x = f2 [B][Td][C n], x2 = e1 [B][C n], n -> y [B][Td][C]; n >= 1
+ *   TSD_REFEMB       x = E [B][T][128], att_pool, w = q weight [128][128], b = q bias, w2 = k weight, b2 = k bias,
+ *                    scratch [B][T] -> y [B][128]; T >= 1, scratch required when att_pool
+ *   TSD_HEAD         x [rows][1024], w [O][1024], b [O] -> y [rows][O]; 1 <= O <= 16
+ *   TSD_MIX_INTERP   x = p1 [B][Td][O], x2 = p2 (null = one pass), vec = wmix [B] -> y = decision [B][Td], y2 = the
+ *                    interpolated [B][T][O]; 1 <= O <= 16
+ *   CLAP_EMBED       ids [N][L], w = word [vocab][H], x = pos [L][H], x2 = type row [H] -> y [N][L][H]
+ *   CLAP_EMBED_TYPED ids, type_ids, mask [N][L], w = word, x = pos, x2 = types [ntypes][H] -> y [N][L][H], kpm [N][L]
+ *   CLAP_GELU        x [rows], max_blocks -> y [rows]
+ *   EMO_MEAN_NORM    x [N][256] -> y [256]; N >= 1
+ *   EMO_LINEAR_NORM  x [N][256], w [E][256], b [E] -> y [N][E]; E >= 1, (E + 288) floats <= 48 KB
+ * Synchronises `stream` before returning.                                                                          */
+enum {
+  AGPT_AN_LASS_AFFINE = 0, AGPT_AN_LASS_UPCOL, AGPT_AN_LASS_SHUFFLE, AGPT_AN_LASS_FILM, AGPT_AN_LASS_FILM_VEC, AGPT_AN_LASS_UP,
+  AGPT_AN_TSD_PAD4, AGPT_AN_TSD_FUSE, AGPT_AN_TSD_REFEMB, AGPT_AN_TSD_HEAD, AGPT_AN_TSD_MIX_INTERP, AGPT_AN_CLAP_EMBED,
+  AGPT_AN_CLAP_EMBED_TYPED, AGPT_AN_CLAP_GELU, AGPT_AN_EMO_MEAN_NORM, AGPT_AN_EMO_LINEAR_NORM
+};
+typedef struct agpt_an_probe_args {
+  int op;
+  void* h;
+  const float* x; const float* x2; const float* s; const float* t; const float* w; const float* b; const float* w2;
+  const float* b2; const float* vec; const float* alpha; const float* beta;
+  const int* ids; const int* type_ids; const int* mask;
+  const int* woff; const int* hoff; const int* nin; const int* dst; const int* ja; const int* jb;
+  float* y; float* y2; float* scratch;
+  uint8_t* kpm;
+  int* info;
+  int B, C, hh, ww, level, nj, hid_len, vec_len, vec_off, Td, T, O, n, att_pool, N, L, H, E, vocab, ntypes, max_blocks;
+  long rows, rows_per_sample;
+} agpt_an_probe_args;
+int agpt_an_probe(const agpt_an_probe_args* args, void* stream);
 
 /* ------------------------------------------------------------------ HiFi-GAN
  * Replaces HifiGanGenerator.__init__/forward/remove_weight_norm

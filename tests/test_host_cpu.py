@@ -453,3 +453,15 @@ def test_voc_probe_args_mirror_the_header():
     names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
     assert names == ["AGPT_VC_" + n for n in _lib.VC_OPS]
     assert "AGPT_VC_CF_TO_CL = 0" in enum and enum.count("=") == 1
+
+
+def test_an_probe_args_mirror_the_header():
+    """_lib.AnProbeArgs has the fields of agpt_an_probe_args in the header's order and C types, and _lib.AN_OPS lists
+    the AGPT_AN_* selectors in the enum's order (a mismatch would run another kernel or shift its arguments)."""
+    from audiogpt_b200 import _lib
+    want = _header_struct_fields("agpt_an_probe_args")
+    assert [(n, t) for n, t in _lib.AnProbeArgs._fields_] == want
+    enum = re.search(r"enum \{([^}]*AGPT_AN_LASS_AFFINE[^}]*)\}", _header(), re.S).group(1)
+    names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
+    assert names == ["AGPT_AN_" + n for n in _lib.AN_OPS]
+    assert "AGPT_AN_LASS_AFFINE = 0" in enum and enum.count("=") == 1

@@ -208,7 +208,7 @@ def test_installed_tool_call():
 
 
 # ---------------------------------------------------------------- kernels through their unit entry points
-@pytest.mark.parametrize("B", [1, 3])
+@pytest.mark.parametrize("B", [1, 3, 4, 5, 9])     # 5 and 9: a second and third group of kGruMaxB = 4 over blockIdx.z
 @pytest.mark.parametrize("T", [1, 2, 63, 125, 500])
 def test_gru_kernel(T, B):
     g = torch.Generator().manual_seed(T * 10 + B)
