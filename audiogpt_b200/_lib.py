@@ -154,6 +154,15 @@ class TapconvProbeArgs(C.Structure):
         ("w2", C.c_void_p), ("b2", C.c_void_p), ("K2", C.c_int), ("dil2", C.c_int)]
 
 
+class TapconvPipes(C.Structure):
+    """agpt_tapconv_pipes: the pipeline switches of agpt_tapconv_probe_pipes."""
+    _fields_ = [(n, C.c_int) for n in ("tc_dual", "tc_pipe", "tc_narrow_pipe", "tc_conv_pipe")]
+
+
+# ran[4] of agpt_tapconv_probe_pipes, in the header's enum order (AGPT_TC_KERN_<name>)
+TC_KERNS = ("TILE", "DUAL", "PAIR_PIPE", "NARROW_PIPE", "CONV_PIPE")
+
+
 # agpt_nn_probe_args.op, in the header's enum order (AGPT_NN_<name>)
 NN_OPS = ("GROUPNORM", "LAYERNORM", "SOFTMAX_ROWS", "TRANSPOSE_PAD", "COPY_PAD_ROWS", "CONCAT", "UPSAMPLE2", "AVGPOOL2",
           "IM2COL_S2", "CF_TO_CL_PAD", "TIMESTEP", "TIMESTEP_DEV", "DDIM_TAB", "CONV_OUT_DDIM")
@@ -250,6 +259,7 @@ PROTOTYPES = {
     "agpt_set_attention_tc": (_I, [_I]),
     "agpt_attention_masked": (_I, [_P, _I, _P, _I, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "agpt_tapconv_probe": (_I, [_P, _P, _P]),
+    "agpt_tapconv_probe_pipes": (_I, [_P, _P, _P, _P]),
     "agpt_nn_probe": (_I, [_P, _P]),
     "agpt_fs_probe": (_I, [_P, _P]),
     "agpt_audio_probe": (_I, [_P, _P]),

@@ -660,7 +660,18 @@ int agpt_emo_lstm(const float* w_hh, const float* xproj, int N, int T, long seq_
 int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream) {
   return guarded([&] {
     AGPT_CHECK(args && ran, "null argument");
-    tapconv_probe(*args, ran, (cudaStream_t)stream);
+    int r[5];
+    for (int i = 0; i < 4; ++i) ran[i] = -1;
+    tapconv_probe(*args, agpt_tapconv_pipes{}, r, (cudaStream_t)stream);
+    for (int i = 0; i < 4; ++i) ran[i] = r[i];
+  });
+}
+
+int agpt_tapconv_probe_pipes(const agpt_tapconv_probe_args* args, const agpt_tapconv_pipes* pipes, int ran[5],
+                             void* stream) {
+  return guarded([&] {
+    AGPT_CHECK(args && pipes && ran, "null argument");
+    tapconv_probe(*args, *pipes, ran, (cudaStream_t)stream);
   });
 }
 

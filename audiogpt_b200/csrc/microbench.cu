@@ -13,12 +13,16 @@
 
 namespace agpt {
 
-// One launch of the production tap-GEMM path on caller-owned tensors (agpt_tapconv_probe, include/agpt_b200.h).
-void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st) {
+// One launch of the production tap-GEMM path on caller-owned tensors, with the pipeline switches sw
+// (agpt_tapconv_probe / agpt_tapconv_probe_pipes, include/agpt_b200.h).
+void tapconv_probe(const agpt_tapconv_probe_args& a, const agpt_tapconv_pipes& sw, int ran[5], cudaStream_t st) {
   AGPT_CHECK(a.w && a.G >= 1 && a.L >= 1 && a.Cin >= 1 && a.Cout >= 1, "tapconv probe: bad arguments");
   AGPT_CHECK(!a.plane_in || (a.pro == PRO_LRELU && !a.fma), "tapconv probe: plane input needs PRO_LRELU on the tensor cores");
-  AGPT_CHECK(!a.pair || (a.kind == 0 && a.w2 && a.res && a.Cin == a.Cout && !a.fma),
+  AGPT_CHECK(!a.pair || ((a.kind == 0 || a.kind == 3) && a.w2 && a.res && a.Cin == a.Cout && !a.fma),
              "tapconv probe: a pair is two Conv1d C -> C with a residual, on the tensor cores");
+  AGPT_CHECK(!a.pair || a.kind == 0 || a.dil2 <= 1, "tapconv probe: a grouped pair has dilation 1 in both convs");
+  AGPT_CHECK(!a.fma || !(sw.tc_dual || sw.tc_pipe || sw.tc_narrow_pipe || sw.tc_conv_pipe),
+             "tapconv probe: the pipeline switches select tensor-core kernels");
   AGPT_CHECK(!a.pair || (!a.plane_in && !a.po_hi), "tapconv probe: a pair reads and writes fp32 only, no operand planes");
   const int dil = a.dil > 0 ? a.dil : 1;
   int gk = 1;   // time steps per row of the grouped view (kind 3)
@@ -47,6 +51,7 @@ void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st
   P.epi = a.epi; P.scale = a.scale; P.accumulate = a.accumulate; P.csplit = a.csplit;
   P.evec = a.evec; P.evec_gstride = a.evec_gstride;
   P.tc_tall = a.tc_tall;
+  P.tc_dual = sw.tc_dual; P.tc_pipe = sw.tc_pipe; P.tc_narrow_pipe = sw.tc_narrow_pipe; P.tc_conv_pipe = sw.tc_conv_pipe;
   P.po_hi = static_cast<__half*>(a.po_hi); P.po_lo = static_cast<__half*>(a.po_lo); P.po_slope = a.po_slope;
   P.pl_hi = static_cast<__half*>(a.pl_hi); P.pl_lo = static_cast<__half*>(a.pl_lo); P.pl_pitch = a.pl_pitch;
   DevBuf planes;
@@ -57,18 +62,20 @@ void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st
     plane_split(a.in, hi, hi + n, n, a.slope, st);
     P.pi_hi = hi; P.pi_lo = hi + n;
   }
-  for (int i = 0; i < 4; ++i) ran[i] = -1;
-  tapconv_note_launch(-1, -1, -1, -1);
+  for (int i = 0; i < 5; ++i) ran[i] = -1;
+  tapconv_note_launch(-1, -1, -1, -1, -1);
   const bool tc_prev = tc_enabled();
   if (a.fma) tc_set_enabled(0);
   try {
     if (a.pair) {
-      pack_conv(pc2, a.w2, a.b2, a.Cout, a.Cout, a.K2, false);
+      // c2 over the same view as c1: plain rows, or (kind 3) the time-grouped view, as the HiFi-GAN driver packs it
+      if (gk > 1) pack_conv_grouped(pc2, a.w2, a.b2, a.Cout, a.K2, gk);
+      else pack_conv(pc2, a.w2, a.b2, a.Cout, a.Cout, a.K2, false);
       TapConvParams P1 = P;                       // c1: leaky ReLU, bias; its output stays in shared memory
       P1.out = nullptr; P1.res = nullptr; P1.out2 = nullptr; P1.epi = EPI_BIAS; P1.scale = 1.f; P1.accumulate = 0;
       P1.po_hi = P1.po_lo = nullptr; P1.pl_hi = P1.pl_lo = nullptr;
-      TapConvParams P2 = tapconv_params(pc2, a.G, a.L, 0, a.dil2 > 0 ? a.dil2 : 1);
-      P2.in = nullptr; P2.in_pitch = a.Cout;      // c2 reads c1's tile, never global memory
+      TapConvParams P2 = tapconv_params(pc2, a.G, a.L / gk, 0, a.dil2 > 0 ? a.dil2 : 1);
+      P2.in = nullptr; P2.in_pitch = a.Cout * gk; // c2 reads c1's tile, never global memory
       P2.out = P.out; P2.out_gstride = P.out_gstride; P2.out_pitch = P.out_pitch;
       P2.res = P.res; P2.res_gstride = P.res_gstride; P2.res_pitch = P.res_pitch;
       P2.pro = PRO_LRELU; P2.slope = a.slope;

@@ -129,7 +129,7 @@ void emo_forward(Handle* h, const float* frames, int N, int T, float* embeds, cu
 void emo_embed(Handle* h, const float* wav, long n, int partial_frames, double min_pad_coverage, double overlap, float* embed,
                float* partials, cudaStream_t st);
 
-void tapconv_probe(const agpt_tapconv_probe_args& a, int ran[4], cudaStream_t st);
+void tapconv_probe(const agpt_tapconv_probe_args& a, const agpt_tapconv_pipes& sw, int ran[5], cudaStream_t st);
 void nn_probe(const agpt_nn_probe_args& a, cudaStream_t st);
 void fs_probe(const agpt_fs_probe_args& a, cudaStream_t st);
 void audio_probe(const agpt_audio_probe_args& a, cudaStream_t st);

@@ -33,9 +33,11 @@ void profile_enable(int on) {
   }
 }
 
-static thread_local int g_ran[4] = {-1, -1, -1, -1};
-void tapconv_note_launch(int tc, int bn, int mt, int plane) { g_ran[0] = tc; g_ran[1] = bn; g_ran[2] = mt; g_ran[3] = plane; }
-void tapconv_last_launch(int ran[4]) { for (int i = 0; i < 4; ++i) ran[i] = g_ran[i]; }
+static thread_local int g_ran[5] = {-1, -1, -1, -1, -1};
+void tapconv_note_launch(int tc, int bn, int mt, int plane, int kern) {
+  g_ran[0] = tc; g_ran[1] = bn; g_ran[2] = mt; g_ran[3] = plane; g_ran[4] = kern;
+}
+void tapconv_last_launch(int ran[5]) { for (int i = 0; i < 5; ++i) ran[i] = g_ran[i]; }
 
 void profile_count_tall() { if (g_prof) ++g_tall; }
 long long profile_tall_launches() { return g_tall; }
@@ -256,7 +258,7 @@ static void fma_launch(TapConvParams P, cudaStream_t st) {
     attr_done = true;
   }
   AGPT_CHECK(smem <= 100 * 1024, "tapconv smem too large (image too wide?)");
-  tapconv_note_launch(0, bn, TC_BM, 0);
+  tapconv_note_launch(0, bn, TC_BM, 0, AGPT_TC_KERN_TILE);
   if (bn == 128) tapconv_kernel<128><<<grid, 256, smem, st>>>(P);
   else if (bn == 64) tapconv_kernel<64><<<grid, 128, smem, st>>>(P);
   else tapconv_kernel<32><<<grid, 64, smem, st>>>(P);

@@ -20,6 +20,7 @@
 #pragma once
 #include <cuda_fp16.h>
 #include "common.cuh"
+#include "../../include/agpt_b200.h"   // AGPT_TC_KERN_*, the kernel family a launch records
 
 namespace agpt {
 
@@ -171,9 +172,10 @@ long long profile_conv_pipe_launches();
 void profile_count_plane();           // a plane-fed tensor-core launch (counted while profiling)
 long long profile_plane_launches();
 // The variant of the most recent tap-GEMM launch on this host thread, {1 tensor-core | 0 fp32-FMA, tile width, tile
-// height, 1 plane-fed}, recorded where a kernel is actually launched (agpt_tapconv_probe reports it); -1s before any.
-void tapconv_note_launch(int tc, int bn, int mt, int plane);
-void tapconv_last_launch(int ran[4]);
+// height, 1 plane-fed, kernel family AGPT_TC_KERN_*}, recorded where a kernel is actually launched
+// (agpt_tapconv_probe reports it); -1s before any.
+void tapconv_note_launch(int tc, int bn, int mt, int plane, int kern);
+void tapconv_last_launch(int ran[5]);
 // fp32 [n] -> operand plane hi / lo of lrelu(x, slope) (TapConvParams::pi_hi), n a multiple of 4 (tcconv5.cu)
 void plane_split(const float* x, __half* hi, __half* lo, long n, float slope, cudaStream_t st);
 void profile_collect(double* ms, double* flops, double* bytes, long long* launches);

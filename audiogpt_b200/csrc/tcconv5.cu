@@ -1650,7 +1650,7 @@ static bool tcconv5_try(TapConvParams P, int BN, int MT, cudaStream_t st) {
   if (!tc5_plan(P, BN, MT, 0, P.tc_chunks_h * P.ntaps, smem)) return false;
   const int Lv = tc_lv(P);
   dim3 grid(cdiv(Lv, MT), cdiv(P.Cout, BN), tc_groups(P));
-  tapconv_note_launch(1, BN, MT, P.pi_hi ? 1 : 0);
+  tapconv_note_launch(1, BN, MT, P.pi_hi ? 1 : 0, AGPT_TC_KERN_TILE);
   if (P.pi_hi) {
     const PlMaps m = pl_tensor_maps(P);
     tc_launch(tcconv5_pl_kern(BN, MT), false, grid, dim3(V5_THREADS), smem, st, P, m.hi, m.lo);
@@ -1705,7 +1705,7 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, bool dual, cu
     if (per_sm != 2) return false;
   }
   void* rec = profile_begin_pair(P1, P2, st);
-  tapconv_note_launch(1, BN, MT, 0);
+  tapconv_note_launch(1, BN, MT, 0, dual ? AGPT_TC_KERN_DUAL : AGPT_TC_KERN_TILE);
   if (dual) {
     tc_launch(dual_kern, true, grid, dim3(V5_THREADS), smem, st, P1, P2);
     profile_count_dual();
@@ -1743,7 +1743,7 @@ static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st)
   const long tiles = (long)cdiv(P1.L, TC_ROWS - span2) * P1.G;
   dim3 grid((unsigned)std::min<long>(tiles, tc5_sms()));
   void* rec = profile_begin_pair(P1, P2, st);
-  tapconv_note_launch(1, 128, TC_ROWS, 0);
+  tapconv_note_launch(1, 128, TC_ROWS, 0, AGPT_TC_KERN_PAIR_PIPE);
   tc_launch(tcpair_pipe_kernel, false, grid, dim3(PIPE_THREADS), smem, st, P1, P2);
   profile_count_pipe();
   profile_end(rec, st);
@@ -1799,7 +1799,7 @@ static bool tcpair_narrow_try(TapConvParams P1, TapConvParams P2, cudaStream_t s
   const long tiles = (long)cdiv(P1.L, TC_ROWS - span2) * P1.G;
   dim3 grid((unsigned)std::min<long>(tiles, tc5_sms()));
   void* rec = profile_begin_pair(P1, P2, st);
-  tapconv_note_launch(1, BN, TC_ROWS, 0);
+  tapconv_note_launch(1, BN, TC_ROWS, 0, AGPT_TC_KERN_NARROW_PIPE);
   tc_launch(BN == 64 ? tcpair_narrow_kernel<64> : tcpair_narrow_kernel<32>, false, grid, dim3(NARROW_THREADS), smem, st, P1,
             P2, tmx);
   profile_count_dual();
@@ -1861,7 +1861,7 @@ static bool tcconv_pipe_try(TapConvParams P, const HTile& c, cudaStream_t st) {
   const size_t smem = (size_t)S.total + 1024;
   const int units = cdiv(P.L, TC_ROWS) * P.G * cdiv(P.Cout, 128);
   const PlMaps m = pl_tensor_maps(P);
-  tapconv_note_launch(1, 128, TC_ROWS, 1);
+  tapconv_note_launch(1, 128, TC_ROWS, 1, AGPT_TC_KERN_CONV_PIPE);
   tc_launch(tcconv_pipe_pl_kernel, false, dim3(cpipe_grid(units, tc5_sms())), dim3(CPIPE_THREADS), smem, st, P, m.hi, m.lo);
   profile_count_plane();
   profile_count_conv_pipe();

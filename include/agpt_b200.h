@@ -98,12 +98,25 @@ typedef struct agpt_tapconv_probe_args {
   int fma;         /* 1: force the fp32-FMA kernel (the tensor-core setting is restored afterwards) */
   int pair;        /* 1: fused ResBlock pair out = epi(c2(lrelu(c1(lrelu(in))))) in one launch: c1 = (w, b, K, dil),
                       Cin == Cout; c2 = (w2, b2, K2, dil2) Conv1d [Cout][Cout][K2]; the epilogue fields are c2's.
+                      kind 0, or kind 3 (both convs time-grouped by g, dil = dil2 = 1).
                       An error when the pair launch is not taken.                                                */
   const float* w2; const float* b2; int K2, dil2;
 } agpt_tapconv_probe_args;
 /* ran = what actually launched: {1 tensor-core | 0 fp32-FMA, tile width BN, tile height MT, 1 plane-fed}.
  * Synchronises `stream` before returning.                                                                   */
 int agpt_tapconv_probe(const agpt_tapconv_probe_args* args, int ran[4], void* stream);
+/* The HiFi-GAN driver's pipeline switches (TapConvParams::tc_*): set on the launch and, for a pair, on c1; 0 keeps
+ * the launch off that pipeline.  Tensor cores only (an error with fma = 1).                                    */
+typedef struct agpt_tapconv_pipes {
+  int tc_dual, tc_pipe, tc_narrow_pipe, tc_conv_pipe;
+} agpt_tapconv_pipes;
+/* ran[4] of agpt_tapconv_probe_pipes: the kernel family of the launch.  TILE covers the FMA kernel, tcconv5[_pl]
+ * and tcpair, which ran[0..3] tell apart; the others are the persistent / two-CTA pipelines the switches allow.   */
+enum { AGPT_TC_KERN_TILE = 0, AGPT_TC_KERN_DUAL, AGPT_TC_KERN_PAIR_PIPE, AGPT_TC_KERN_NARROW_PIPE, AGPT_TC_KERN_CONV_PIPE };
+/* agpt_tapconv_probe with the pipeline switches `pipes`; ran = {the four fields of agpt_tapconv_probe, kernel
+ * family AGPT_TC_KERN_*}.  Synchronises `stream` before returning.                                           */
+int agpt_tapconv_probe_pipes(const agpt_tapconv_probe_args* args, const agpt_tapconv_pipes* pipes, int ran[5],
+                             void* stream);
 /* Conformance entry of the non-contraction kernels (nn_kernels.cu, tests/test_nn_kernels_gpu.py): ONE call of the
  * production launcher selected by `op` on caller-owned device tensors, with the arguments as given.  All tensors are
  * fp32 device arrays unless marked host; the fields each op reads:

@@ -407,6 +407,18 @@ def test_tapconv_probe_args_mirror_the_header():
     assert [n for n, _ in got] == [("inp" if n == "in" else n) for n, _ in want]   # `in` is a Python keyword
 
 
+def test_tapconv_pipes_and_kernel_ids_mirror_the_header():
+    """_lib.TapconvPipes has the fields of agpt_tapconv_pipes, and _lib.TC_KERNS lists the AGPT_TC_KERN_* kernel
+    families of agpt_tapconv_probe_pipes's ran[4] in the enum's order (a mismatch would set the wrong pipeline or let
+    a case assert the wrong kernel)."""
+    from audiogpt_b200 import _lib
+    assert [(n, t) for n, t in _lib.TapconvPipes._fields_] == _header_struct_fields("agpt_tapconv_pipes")
+    enum = re.search(r"enum \{([^}]*AGPT_TC_KERN_TILE[^}]*)\}", _header(), re.S).group(1)
+    names = [e.split("=")[0].strip() for e in enum.split(",") if e.strip()]
+    assert names == ["AGPT_TC_KERN_" + n for n in _lib.TC_KERNS]
+    assert "AGPT_TC_KERN_TILE = 0" in enum and enum.count("=") == 1
+
+
 def test_nn_probe_args_mirror_the_header():
     """_lib.NnProbeArgs has the fields of agpt_nn_probe_args in the header's order and C types, and _lib.NN_OPS lists
     the AGPT_NN_* selectors in the enum's order (a mismatch would run another kernel or shift its arguments)."""
