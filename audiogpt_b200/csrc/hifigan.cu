@@ -380,6 +380,7 @@ struct Hifigan : Handle {
   bool plane_feed = true;           // AGPT_PLANE_FEED=0: every tap-GEMM converts its fp32 input itself
   bool pair_dual = true;            // AGPT_PAIR_DUAL=0: no fused pair runs two CTAs per SM (TapConvParams::tc_dual)
   bool pair_pipe = true;            // AGPT_PAIR_PIPE=0: no C = 128 pair runs two tiles per CTA (TapConvParams::tc_pipe)
+  bool pair_pipe_stage = true;      // AGPT_PAIR_PIPE_STAGE=0: those pairs load their input and residual per thread
   bool narrow_pipe = true;          // AGPT_NARROW_PIPE=0: narrow pairs keep two CTAs per SM (TapConvParams::tc_narrow_pipe)
   bool conv_pipe = true;            // AGPT_CONV_PIPE=0: plane-fed convs keep one tile per CTA (TapConvParams::tc_conv_pipe)
 
@@ -510,7 +511,7 @@ struct Hifigan : Handle {
             TapConvParams P1 = conv(rb.c1[n], rb.c1g[n], gq, rb.dil[n], x, A);
             P1.epi = EPI_BIAS;
             P1.tc_dual = pair_dual;
-            P1.tc_pipe = pair_pipe;
+            P1.tc_pipe = pair_pipe ? (pair_pipe_stage ? 1 : 2) : 0;
             P1.tc_narrow_pipe = narrow_pipe;
             feed(P1, C);
             TapConvParams P2 = conv(rb.c2[n], rb.c2g[n], gq, 1, A, dst);
@@ -575,6 +576,7 @@ Handle* hifigan_create(const agpt_hifigan_cfg* cfg, const float* const* W, int n
   { const char* e = getenv("AGPT_PLANE_FEED"); h->plane_feed = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_PAIR_DUAL"); h->pair_dual = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_PAIR_PIPE"); h->pair_pipe = !(e && e[0] == '0'); }
+  { const char* e = getenv("AGPT_PAIR_PIPE_STAGE"); h->pair_pipe_stage = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_NARROW_PIPE"); h->narrow_pipe = !(e && e[0] == '0'); }
   { const char* e = getenv("AGPT_CONV_PIPE"); h->conv_pipe = !(e && e[0] == '0'); }
   WeightCursor wc{W, nW};

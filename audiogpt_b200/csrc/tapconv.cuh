@@ -84,8 +84,9 @@ struct TapConvParams {
   // 1: a fused ResBlock pair (tcpair_launch) may run as two 128-row CTAs per SM (tcpair2_kernel); set by the HiFi-GAN
   // driver unless AGPT_PAIR_DUAL=0.
   int tc_dual;
-  // 1: a C = 128 fused pair may run on tcpair_pipe_kernel (two tiles in flight per CTA); set by the HiFi-GAN driver
-  // unless AGPT_PAIR_PIPE=0.
+  // 1: a C = 128 fused pair may run on tcpair_pipe_kernel (two tiles in flight per CTA), its input and residual
+  // staged by TMA; 2: the same pipeline with one data warpgroup loading them per thread.  Set by the HiFi-GAN driver
+  // unless AGPT_PAIR_PIPE=0 (2 with AGPT_PAIR_PIPE_STAGE=0).
   int tc_pipe;
   // 1: a narrow fused pair that tc_dual allows may run on tcpair_narrow_kernel (persistent, several tiles in flight
   // per CTA) before tcpair2_kernel; set by the HiFi-GAN driver unless AGPT_NARROW_PIPE=0.

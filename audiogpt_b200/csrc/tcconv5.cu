@@ -733,6 +733,12 @@ __global__ void __launch_bounds__(V5_THREADS, 2) tcpair2_kernel(const __grid_con
 // SWIZZLE_64B rows), one wgmma group each.  A stage is released once the group after it has been issued and its own
 // group has completed, so with 32 KB stages a 2-stage ring gave each stage's load one group of wgmmas to arrive in;
 // the same 64 KB as 4 half-stages give it three half-groups (1.5 groups), and spare shared memory holds more.
+// tcpair_pipe_kernel<true> (the staged form) splits the data warpgroup's work, which bounded the k = 3 pairs: 640
+// threads, warpgroup 2 converts each tile's input in place from shared memory, warpgroup 3 runs the epilogue, and of
+// the last warpgroup warp 16 streams the weights, warp 17 loads each tile's fp32 input rows by TMA straight into its
+// operand set (32-channel boxes, zero outside the sample; box b of row r fills the bytes of row r of operand quarter
+// b) and warp 18 loads the residual (the pair's input) by TMA in 32 x 32 boxes through a small ring.  A set's life
+// gains one step: ... -> epilogue(t) -> set_free -> TMA input(t + 2).
 constexpr int PIPE_THREADS = 512;
 constexpr uint32_t PIPE_STAGE = 2u * 128u * 64u;   // bytes of a half-stage: hi and lo, 128 rows x 64 B
 // wgmma descriptor of a K-major SWIZZLE_64B tile (8-row groups 512 B apart)
@@ -750,29 +756,41 @@ template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile
 
 // operand set s: [hi chunk 0][hi chunk 1][lo chunk 0][lo chunk 1] of R1 rows x 128 B (c1's input), then c2's tile in
 // the same form with R2 <= R1 rows, then the dump: 4 column blocks of [128 rows][32 fp32] (64 KB <= 512 R1 B)
-constexpr int PIPE_MAX_NW = 8;
-struct PipeSmem { uint32_t set[2], w[PIPE_MAX_NW], bars, total; };
-__host__ __device__ inline void pipe_layout(PipeSmem& s, int R1, int NW) {
+// STAGED (tc_pipe == 1): the residual arrives in boxes of 32 rows x 32 fp32 channels (4 KB) through a ring of
+// NSP slots after the weight stages and (R1 - 128) / 8 slots in each set past its dump (free once c2 is done).
+constexpr int PIPE_MAX_NW = 8, PIPE_MAX_RES = 8;
+constexpr uint32_t PIPE_RES_BOX = 32u * 128u, PIPE_DUMP = 128u * 512u;
+struct PipeSmem { uint32_t set[2], w[PIPE_MAX_NW], res[PIPE_MAX_RES], bars, total; };
+__host__ __device__ inline void pipe_layout(PipeSmem& s, int R1, int NW, int NSP) {
   uint32_t o = 0;
   for (int i = 0; i < 2; ++i) { s.set[i] = o; o += (uint32_t)R1 * 512; }
   for (int i = 0; i < PIPE_MAX_NW; ++i) { s.w[i] = o; if (i < NW) o += PIPE_STAGE; }
-  s.bars = o; o += (2 * PIPE_MAX_NW + 4) * 8;
+  for (int i = 0; i < PIPE_MAX_RES; ++i) { s.res[i] = o; if (i < NSP) o += PIPE_RES_BOX; }
+  s.bars = o; o += (2 * PIPE_MAX_NW + 8 + 2 * PIPE_MAX_RES) * 8;
   s.total = o;
 }
+// STAGED: 5 warpgroups, launched at 96 registers per thread: 2 x 168 (wgmma) + 48 (transform) + 72 (epilogue) + 24
+constexpr int PIPE_STAGED_THREADS = 640, PIPE_XF_REGS = 48, PIPE_EPI_REGS = 72;
 
-__global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __grid_constant__ TapConvParams P1,
-                                                                      const __grid_constant__ TapConvParams P2) {
+template <bool STAGED>
+__global__ void __launch_bounds__(STAGED ? PIPE_STAGED_THREADS : PIPE_THREADS, 1)
+    tcpair_pipe_kernel(const __grid_constant__ TapConvParams P1, const __grid_constant__ TapConvParams P2,
+                       const __grid_constant__ CUtensorMap tmx, const __grid_constant__ CUtensorMap tmr) {
   constexpr int BN = 128, MT = TC_ROWS;
   extern __shared__ uint8_t smem_raw_[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw_) + 1023) & ~(uintptr_t)1023);
-  const int R1 = P1.R, NW = P1.tc_nw;
+  const int R1 = P1.R, NW = P1.tc_nw, NSP = P1.tc_na;
   __shared__ PipeSmem S;
-  if (threadIdx.x == 0) pipe_layout(S, R1, NW);
+  if (threadIdx.x == 0) pipe_layout(S, R1, NW, NSP);
   __syncthreads();
   uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + S.bars);
   uint64_t* w_empty = w_full + PIPE_MAX_NW;
   uint64_t* in_full = w_full + 2 * PIPE_MAX_NW;   // [2] the set holds its tile's c1 operand (data warpgroup -> wgmma)
   uint64_t* acc_full = in_full + 2;           // [2] the set holds its tile's c2 dump (wgmma -> data warpgroup)
+  uint64_t* raw_full = acc_full + 2;          // [2] STAGED: the tile's fp32 input rows landed in the set (TMA -> transform)
+  uint64_t* set_free = raw_full + 2;          // [2] STAGED: the epilogue is done with the set (epilogue -> TMA)
+  uint64_t* res_full = set_free + 2;          // [PIPE_MAX_RES] STAGED: a residual box landed (TMA -> epilogue)
+  uint64_t* res_empty = res_full + PIPE_MAX_RES;   // [PIPE_MAX_RES] STAGED: the epilogue is done with it
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);   // warpgroup-uniform role branches (see tcconv5_kernel)
@@ -788,9 +806,19 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
     q0 = (T - g * ntx) * MTO;
   };
 
+  // STAGED: residual ring of NRS slots; a tile's 4 column blocks x nj row boxes pass through it in order
+  const int NSL = (R1 - 128) / 8, NRS = NSP + NSL, nj = (MTO + 31) / 32, NU = 4 * nj;
+  auto res_slot = [&](int j, int s) -> uint8_t* {
+    return j < NSP ? smem + S.res[j] : smem + S.set[s] + PIPE_DUMP + (uint32_t)(j - NSP) * PIPE_RES_BOX;
+  };
+
   if (tid == 0) {
     for (int i = 0; i < NW; ++i) { mbar_init(&w_full[i], 1); mbar_init(&w_empty[i], PIPE_MMA / 32); }
     for (int i = 0; i < 2; ++i) { mbar_init(&in_full[i], PIPE_DATA); mbar_init(&acc_full[i], PIPE_MMA); }
+    if constexpr (STAGED) {
+      for (int i = 0; i < 2; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&set_free[i], PIPE_DATA); }
+      for (int i = 0; i < NRS; ++i) { mbar_init(&res_full[i], 1); mbar_init(&res_empty[i], PIPE_DATA); }
+    }
     fence_barrier_init();
   }
   __syncthreads();
@@ -859,7 +887,77 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
       for (int blk = 0; blk < BN / 32; ++blk) stage_block(acc, set + blk * (MT * 128), blk * 32, r0, c0, P2.tc_descale);
       mbar_arrive(&acc_full[k & 1]);
     }
-  } else if (wg == 2) {
+  } else if (STAGED && wg == 2) {
+    // ================ transform: the set's fp32 input rows -> c1's hi / lo operand, in place ================
+    // Box b (channels 32 b ..) of row r sits in the 128 B of row r of the set's quarter b, the same bytes that hold
+    // row r of operand quarter b afterwards, so a half-warp reads all 16 items of its row before any is written.
+    setmaxnreg_dec<PIPE_XF_REGS>();
+    const int dt = tid - PIPE_MMA, i16 = dt & 15, c = i16 >> 3, q = i16 & 7, odd = q >> 2;
+    const uint32_t qsz = (uint32_t)R1 * 128, src = (uint32_t)(2 * c + odd) * qsz;
+    for (int k = 0; k < nloc; ++k) {
+      const int s = k & 1;
+      mbar_wait(&raw_full[s], (uint32_t)((k >> 1) & 1));
+      uint8_t* set = smem + S.set[s];
+      for (int row = dt >> 4; row < R1; row += PIPE_DATA / 16) {
+        // channels 8 q' .. 8 q' + 7 (q' = 8 c + q): 16-byte units 2 (q & 3) and + 1 of box 2 c + q / 4 (TMA
+        // SWIZZLE_128B); the upper half-quarter reads its pair odd unit first, off the lower one's banks
+        const uint8_t* rr = set + src + row * 128;
+        const int u0 = 2 * (q & 3), sw = row & 7;
+        const float4 a = *reinterpret_cast<const float4*>(rr + (((u0 + odd) ^ sw) << 4));
+        const float4 b = *reinterpret_cast<const float4*>(rr + (((u0 + 1 - odd) ^ sw) << 4));
+        __syncwarp();
+        const float4 x0 = pro_apply5(P1, odd ? b : a, true, nullptr), x1 = pro_apply5(P1, odd ? a : b, true, nullptr);
+        uint4 h, l;
+        split8(x0, x1, h, l);
+        const uint32_t o = (uint32_t)c * qsz + sw128(row, q);
+        *reinterpret_cast<uint4*>(set + o) = h;
+        *reinterpret_cast<uint4*>(set + 2 * qsz + o) = l;
+      }
+      fence_proxy_async();                  // generic-proxy stores -> visible to the wgmma operand reads
+      mbar_arrive(&in_full[s]);
+    }
+  } else if (STAGED && wg == 3) {
+    // ================ epilogue: the dump + the residual boxes through c2's fused epilogue (epi_store_cv) ================
+    setmaxnreg_dec<PIPE_EPI_REGS>();
+    const int dt = tid - PIPE_MMA - PIPE_DATA, jc = dt & 7;
+    int n = 0;   // residual boxes consumed so far
+    for (int k = 0; k < nloc; ++k) {
+      int g, q0;
+      tile_of(k, g, q0);
+      const int s = k & 1;
+      const uint8_t* set = smem + S.set[s];
+      mbar_wait(&acc_full[s], (uint32_t)((k >> 1) & 1));
+      for (int b = 0; b < 4; ++b) {
+        const int co = 32 * b + 4 * jc;
+        const uint8_t* stg = set + b * (MT * 128);
+        const float4 cv = epi_colvec(P2, g, co);
+        for (int j = 0; j < nj; ++j, ++n) {
+          float4 ob[2];   // the old MRF sum (EPI_ACC with accumulate), read before the residual box is waited for
+          int pp[2];
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int row = 32 * j + (dt >> 3) + 16 * i;
+            pp[i] = (row < MTO && q0 + row < Lv) ? q0 + row : -1;
+            ob[i] = pp[i] >= 0 ? epi_load_b(P2, g, pp[i], co) : make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+          const int slot = n % NRS;
+          mbar_wait(&res_full[slot], (uint32_t)((n / NRS) & 1));
+          const uint8_t* rb = res_slot(slot, s);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int rl = (dt >> 3) + 16 * i, row = 32 * j + rl;
+            EpiPre pre;
+            pre.a = *reinterpret_cast<const float4*>(rb + sw128(rl, jc));
+            pre.b = ob[i];
+            if (pp[i] >= 0) epi_store_cv(P2, g, pp[i], co, *reinterpret_cast<const float4*>(stg + sw128(row, jc)), pre, cv);
+          }
+          mbar_arrive(&res_empty[slot]);
+        }
+      }
+      fence_proxy_async();                  // the dump's generic stores before the next TMA into the set
+      mbar_arrive(&set_free[s]);
+    }
+  } else if (!STAGED && wg == 2) {
     // =========================== data warpgroup: next tile's input, previous tile's epilogue ===========================
     setmaxnreg_inc<152>();
     const int dt = tid - PIPE_MMA;
@@ -925,8 +1023,46 @@ __global__ void __launch_bounds__(PIPE_THREADS, 1) tcpair_pipe_kernel(const __gr
     }
   } else {
     setmaxnreg_dec<24>();
-    if (warp != 12 || lane != 0) return;
-    // ====================== weight producer (warp 12): per tile c1's half-stages, then c2's ======================
+    constexpr int wwarp = STAGED ? 16 : 12;   // the first warp of the last warpgroup
+    if (lane != 0) return;
+    if (STAGED && warp == wwarp + 1) {
+      // ================ input rows of each tile (TMA, 4 boxes of 32 channels, zero outside the sample) ================
+      tma_prefetch_desc(&tmx);
+      for (int k = 0; k < nloc; ++k) {
+        int g, q0;
+        tile_of(k, g, q0);
+        const int s = k & 1;
+        if (k >= 2) mbar_wait(&set_free[s], (uint32_t)(((k >> 1) - 1) & 1));
+        mbar_arrive_expect_tx(&raw_full[s], 4u * R1 * 128u);
+        for (int b = 0; b < 4; ++b)
+          tma_load_3d(smem + S.set[s] + (uint32_t)b * R1 * 128, &tmx, 32 * b, q0 + P2.lo_al + lo, g, &raw_full[s]);
+      }
+      return;
+    }
+    if (STAGED && warp == wwarp + 2) {
+      // ================ residual boxes of each tile's output rows (TMA), in the epilogue's order ================
+      tma_prefetch_desc(&tmr);
+      int n = 0;
+      for (int k = 0; k < nloc; ++k) {
+        int g, q0;
+        tile_of(k, g, q0);
+        const int s = k & 1;
+        bool c2_done = false;
+        for (int u = 0; u < NU; ++u, ++n) {
+          const int slot = n % NRS;
+          if (n >= NRS) mbar_wait(&res_empty[slot], (uint32_t)((n / NRS - 1) & 1));
+          if (slot >= NSP && !c2_done) {   // a slot past the dump: c2's wgmmas are done with the set
+            mbar_wait(&acc_full[s], (uint32_t)((k >> 1) & 1));
+            c2_done = true;
+          }
+          mbar_arrive_expect_tx(&res_full[slot], PIPE_RES_BOX);
+          tma_load_3d(res_slot(slot, s), &tmr, 32 * (u / nj), q0 + 32 * (u % nj), g, &res_full[slot]);
+        }
+      }
+      return;
+    }
+    if (warp != wwarp) return;
+    // ====================== weight producer: per tile c1's half-stages, then c2's ======================
     int n_it = 0;
     for (int k = 0; k < nloc; ++k)
       for (int it = 0; it < total1 + total2; ++it, ++n_it) {
@@ -1724,6 +1860,13 @@ static bool tcpair_try(TapConvParams P1, TapConvParams P2, int MT, bool dual, cu
 // when the handle does not allow it (TapConvParams::tc_pipe), the pair is not 128 -> 128 channels converted from fp32
 // with half-stage images, or the sets and four half-stages do not fit (c1 with a tap span of about 30 rows or more:
 // k = 11 at dilation 5).
+//
+// tc_pipe == 1 runs the staged form (STAGED): the input rows arrive by TMA, a transform warpgroup and an epilogue
+// warpgroup split the data work, and the residual (the pair's own input) arrives by TMA in 32 x 32 boxes through the
+// shared memory left beside the weight ring plus each set's bytes past its dump: R1 = 136 / 144 / 152 / 160 get
+// 2 + 1 / 0 + 2 / 2 + 3 / 0 + 4 slots at 5 / 5 / 4 / 4 half-stages, the same rings as without it.  tc_pipe == 2, a
+// residual that is not the pair's input, or an input the tensor maps cannot describe keep one data warpgroup with
+// plain global loads.
 static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st) {
   if (!P1.tc_pipe || P1.tc_bn != 128 || P1.Cin != 128 || P1.Cout != 128 || P2.Cout != 128 || !P1.w_hk || !P2.w_hk)
     return false;
@@ -1732,19 +1875,30 @@ static bool tcpair_pipe_try(TapConvParams P1, TapConvParams P2, cudaStream_t st)
   if (P2.R > P1.R) return false;   // c2's tile lives in c1's operand set
   const long wbytes = PIPE_STAGE;
   PipeSmem S;
-  pipe_layout(S, P1.R, 0);
+  pipe_layout(S, P1.R, 0, 0);
   const long spare = (long)kMaxDyn - 1024 - (long)S.total;
   if (spare < 4 * wbytes) return false;
   const int iters = 2 * (P1.tc_chunks_h * P1.ntaps + P2.tc_chunks_h * P2.ntaps);
   P1.tc_nw = (int)std::min<long>(std::min<long>(PIPE_MAX_NW, iters), spare / wbytes);
+  const int nsl = (P1.R - 128) / 8;
+  const int nsp = (int)std::min<long>(PIPE_MAX_RES - nsl, (spare - P1.tc_nw * wbytes) / PIPE_RES_BOX);
+  CUtensorMap tmx{}, tmr{};
+  const bool staged = P1.tc_pipe == 1 && P2.res == P1.in && P2.res_pitch == P1.in_pitch &&
+                      P2.res_gstride == P1.in_gstride && nsl + nsp >= 1 &&
+                      tma_encode_rows(&tmx, P1.in, 128, P1.L, P1.G, P1.in_pitch, P1.in_gstride, P1.R) &&
+                      tma_encode_rows(&tmr, P1.in, 128, P1.L, P1.G, P1.in_pitch, P1.in_gstride, 32);
+  P1.tc_na = staged ? nsp : 0;
   P2.tc_bn = 128;
-  pipe_layout(S, P1.R, P1.tc_nw);
+  pipe_layout(S, P1.R, P1.tc_nw, P1.tc_na);
   const size_t smem = (size_t)S.total + 1024;
   const long tiles = (long)cdiv(P1.L, TC_ROWS - span2) * P1.G;
   dim3 grid((unsigned)std::min<long>(tiles, tc5_sms()));
   void* rec = profile_begin_pair(P1, P2, st);
   tapconv_note_launch(1, 128, TC_ROWS, 0, AGPT_TC_KERN_PAIR_PIPE);
-  tc_launch(tcpair_pipe_kernel, false, grid, dim3(PIPE_THREADS), smem, st, P1, P2);
+  if (staged)
+    tc_launch(tcpair_pipe_kernel<true>, false, grid, dim3(PIPE_STAGED_THREADS), smem, st, P1, P2, tmx, tmr);
+  else
+    tc_launch(tcpair_pipe_kernel<false>, false, grid, dim3(PIPE_THREADS), smem, st, P1, P2, tmx, tmr);
   profile_count_pipe();
   profile_end(rec, st);
   count_launch(1);
